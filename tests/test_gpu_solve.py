@@ -342,39 +342,3 @@ def test_light_check_matches_the_spmv_check(engine_lib, oracle, monkeypatch, war
     to = orc["trace"]
     assert len(to) == len(tb) and np.array_equal(to[:, 0], tb[:, 0])
     assert (np.abs(to[:11, 1:9] - tb[:11, 1:9]) <= 1e-7 * scale).all()
-
-
-@pytest.mark.parametrize("mode", ["1", "2"], ids=["bulk_copy", "cooperative_loads"])
-def test_tiled_spmv_shape_matches_the_default(engine_lib, monkeypatch, mode):
-    """DevSell::tiled (spmv_sell_tile_kernel): one 1024-thread CTA per 8192-row window, the window of the input vector staged in
-    shared memory (mode 1: one cp.async.bulk by the TMA unit + mbarrier; mode 2: cooperative loads), gathers from there.  Same
-    per-row arithmetic in the same order as the default shapes: A x and A'y agree exactly (up to the sign of an exact zero), the
-    fused pass kernels give the same trajectory up to the grouping of the block partial sums."""
-    from highs_b200 import engine
-    from highs_b200.lp import synthetic_lp
-    lp = synthetic_lp(60000, 50000, 7, seed=5, band=1500)       # banded: every tile's window fits the staging buffer
-    rng = np.random.default_rng(1)
-    monkeypatch.setenv("B200PDLP_TILE", "0")
-    base = engine.Problem(lp, ordered_max=-1)
-    x, y = rng.standard_normal(base.n), rng.standard_normal(base.m)
-    ax0, aty0 = base.spmv_ax(x), base.spmv_aty(y)
-    r0 = base.solve(iter_limit=80, trace_cap=64)
-    base.close()
-    monkeypatch.setenv("B200PDLP_TILE", mode)
-    monkeypatch.setenv("B200PDLP_TILE_FORCE", "1")     # (this LP has only 8 tiles: fewer than half the SMs)
-    monkeypatch.setenv("B200PDLP_TIMING", "1")
-    til = engine.Problem(lp, ordered_max=-1)
-    ax1, aty1 = til.spmv_ax(x), til.spmv_aty(y)
-    r1 = til.solve(iter_limit=80, trace_cap=64)
-    til.close()
-    # rows of ordinary length: the same sum in the same order (bit for bit, up to the sign of an exact zero); the band's clipping
-    # piles entries onto the first and last row -- long rows, whose segment sums run on 1024 instead of 256 threads
-    for u, v in ((ax0, ax1), (aty0, aty1)):
-        assert np.abs(u - v).max() <= 1e-12 * (1 + np.abs(u).max())
-        assert (u != v).sum() <= 8
-    assert r0["iters"] == r1["iters"] and len(r0["trace"]) == len(r1["trace"])
-    scale = 1.0 + np.abs(r0["trace"][:, 1:9]).max(axis=0)
-    # (80 iterations: rounding differences of the regrouped partial sums grow along a PDHG trajectory -- 8e-6 after 200)
-    assert (np.abs(r0["trace"][:, 1:9] - r1["trace"][:, 1:9]) <= 1e-6 * scale).all()
-    for k in ("col_value", "row_dual"):
-        assert np.abs(r0[k] - r1[k]).max() <= 1e-5 * (1 + np.abs(r0[k]).max())
