@@ -143,52 +143,59 @@ inline int grid_for(long long work) {
 inline int warp_grid(long long rows) { return (int)std::max<long long>(1, (rows * 32 + kTpb - 1) / kTpb); }
 
 // ---- formulateLP_highs, CupdlpWrapper.cpp:280-448 (host twin: host_prep.cpp::formulate)
-// row classes with the +-1e20 thresholds (:316-317); eq-like = EQ or BOUND (they come first in the new order)
+// row classes with the +-1e20 thresholds (:316-317); eq-like = EQ or BOUND (they come first in the new order).
+// hip (HiPDLP mode, pdhg.cc:175-198; host twin formulate_hipdlp): thresholds +-infinity, so a bound of 1e25 is finite, and
+// free rows are a class of their own (kFreeRow = 4, eq-like, with a slack column like BOUND rows)
 __global__ void __launch_bounds__(kTpb)
-classify_rows_kernel(int m, const double* __restrict__ rl, const double* __restrict__ ru, int* __restrict__ cls,
+classify_rows_kernel(int m, int hip, const double* __restrict__ rl, const double* __restrict__ ru, int* __restrict__ cls,
                      int* __restrict__ eqlike, int* __restrict__ isbound) {
   const int stride = gridDim.x * kTpb;
+  const double thr = hip ? INFINITY : 1e20;
   for (int i = blockIdx.x * kTpb + threadIdx.x; i < m; i += stride) {
-    const bool lo = rl[i] > -1e20, up = ru[i] < 1e20;
+    const bool lo = rl[i] > -thr, up = ru[i] < thr;
     int c;
     if (lo && up && rl[i] == ru[i]) c = 0;      // kEq
     else if (lo && !up) c = 2;                   // kGeq
     else if (!lo && up) c = 1;                   // kLeq
-    else c = 3;                                  // kBound (ranged and free rows)
+    else if (hip && !lo && !up) c = 4;           // kFreeRow
+    else c = 3;                                  // kBound (ranged rows; free rows too outside HiPDLP mode)
     cls[i] = c;
-    eqlike[i] = (c == 0 || c == 3) ? 1 : 0;
-    isbound[i] = c == 3 ? 1 : 0;
+    eqlike[i] = (c == 0 || c >= 3) ? 1 : 0;
+    isbound[i] = c >= 3 ? 1 : 0;
   }
 }
 
 // new row order: EQ/BOUND rows first (original order), then LEQ/GEQ (:380-404); rhs; slack column of a BOUND row
 // (:328-331,367-373,439-445): A x - z = 0, lo <= z <= up
+// hip: rup != nullptr receives the row upper bounds (EQ [b, b], GEQ / LEQ [b, inf], BOUND / FREE [0, 0], pdhg.cc:247-270) and
+// the slack columns keep the row's bounds unclamped (:235-244)
 __global__ void __launch_bounds__(kTpb)
 row_maps_kernel(int m, int n0, int nnz0, int neq, const double* __restrict__ rl, const double* __restrict__ ru,
                 const int* __restrict__ cls, const int* __restrict__ eq_ex, const int* __restrict__ bd_ex,
                 int* __restrict__ new_idx, int* __restrict__ row_old, int* __restrict__ slack_row, double* __restrict__ rhs,
                 double* __restrict__ cost, double* __restrict__ lower, double* __restrict__ upper, int* __restrict__ cbeg,
-                int* __restrict__ cidx, double* __restrict__ cval, int* __restrict__ colof) {
+                int* __restrict__ cidx, double* __restrict__ cval, int* __restrict__ colof, double* __restrict__ rup) {
   const int stride = gridDim.x * kTpb;
   for (int i = blockIdx.x * kTpb + threadIdx.x; i < m; i += stride) {
     const int c = cls[i];
-    const bool eql = c == 0 || c == 3;
+    const bool eql = c == 0 || c >= 3;
     const int ni = eql ? eq_ex[i] : neq + (i - eq_ex[i]);
     new_idx[i] = ni;
     row_old[ni] = i;
     double b;
     if (c == 0) b = rl[i];
-    else if (c == 3) b = 0.0;
+    else if (c >= 3) b = 0.0;
     else if (c == 1) b = -ru[i];
     else b = rl[i];
     rhs[ni] = b;
-    if (c == 3) {
+    if (rup) rup[ni] = c == 0 ? ru[i] : (c >= 3 ? 0.0 : INFINITY);
+    if (c >= 3) {
       const int k = bd_ex[i], j = n0 + k;
       slack_row[k] = i;
       cost[j] = 0.0;
       double l = rl[i], u = ru[i];
-      if (l < -1e20) l = -INFINITY;     // :375-378
-      if (u > 1e20) u = INFINITY;
+      if (!rup && l < -1e20) l = -INFINITY;     // :375-378
+      if (!rup && u > 1e20) u = INFINITY;
       lower[j] = l;
       upper[j] = u;
       cbeg[j] = nnz0 + k;
@@ -203,10 +210,15 @@ __global__ void __launch_bounds__(kTpb)
 col_vectors_kernel(int n0, int n, int nnz, double sense, const int* __restrict__ a_start, const double* __restrict__ cc,
                    const double* __restrict__ cl, const double* __restrict__ cu, double* __restrict__ cost,
                    double* __restrict__ lower, double* __restrict__ upper, int* __restrict__ cbeg, int what) {
-  // what & 1: the column starts (structure);  what & 2: cost and bounds (values, which arrive on the second copy stream)
+  // what & 1: the column starts (structure);  what & 2: cost and bounds (values, which arrive on the second copy stream);
+  // what & 4: HiPDLP mode -- the cost is not multiplied by the sense and the bounds are not clamped (pdhg.cc:280-297)
   const int stride = gridDim.x * kTpb;
   for (int j = blockIdx.x * kTpb + threadIdx.x; j < n0; j += stride) {
-    if (what & 2) {
+    if (what & 4) {
+      cost[j] = cc[j];
+      lower[j] = cl[j];
+      upper[j] = cu[j];
+    } else if (what & 2) {
       cost[j] = cc[j] * sense;
       double l = cl[j], u = cu[j];
       if (l < -1e20) l = -INFINITY;
@@ -230,10 +242,10 @@ nnz_flags_kernel(int nnz0, int m, const int* __restrict__ a_index, const int* __
     const int r = a_index[p];
     if ((unsigned)r >= (unsigned)m) { bad = 1; fl[p] = 0; continue; }
     fl[p] = eqlike[r];
-    if (p > 0 && colof[p - 1] == colof[p] && a_index[p - 1] > r) desc = 1;
+    if (p > 0 && colof[p - 1] == colof[p] && a_index[p - 1] >= r) desc |= a_index[p - 1] > r ? 1 : 2;   // 2: a repeated row
   }
   if (bad) atomicOr(&flags[0], 1);
-  if (desc) atomicOr(&flags[1], 1);
+  if (desc) atomicOr(&flags[1], desc);
 }
 
 // structural columns: within a column EQ/BOUND entries first, then LEQ (negated) / GEQ, each group in storage order
@@ -253,7 +265,7 @@ scatter_entries_kernel(int nnz0, const int* __restrict__ a_start, const int* __r
     const int k = fl_ex[p] - fl_ex[s];           // eq-like entries before p
     const int r = a_index[p];
     const int c = cls[r];
-    const bool eql = c == 0 || c == 3;
+    const bool eql = c == 0 || c >= 3;
     const int q = eql ? s + k : s + ne + (p - s - k);
     cidx[q] = new_idx[r];
     dest[p] = (unsigned)q | (c == 1 ? 0x80000000u : 0u);
@@ -472,9 +484,64 @@ __global__ void long_plan_kernel(int nlong, const int* __restrict__ list, const 
   totals[1] = lpos + 8;
 }
 
-// the second index of a matrix whose columns are not stored with ascending rows: positions ordered by (column, row,
-// storage order) = the order in which the reference's row scatter adds into a column (cupdlp_linalg.c:73-109).
-// keys for the second (stable) pass of an LSD sort: the column of the row-sorted positions
+// ---- HiPDLP mode: entries of a column ordered by (new row, value), as std::sort of (row, value) pairs (pdhg.cc:300-333).
+// Columns stored with strictly ascending rows need nothing beyond the stable eq-like partition (the renumbering is
+// monotone inside each group); otherwise an LSD radix sort: first by value, then (stably) by (column, new row).
+// Doubles as radix keys: flip all bits of a negative value, the sign bit of a non-negative one (ascending numeric order;
+// -0.0 sorts before +0.0, which std::sort leaves in either order -- both orders give the same sums)
+__global__ void __launch_bounds__(kTpb) value_key_kernel(int len, const double* __restrict__ v, unsigned long long* __restrict__ key) {
+  const int stride = gridDim.x * kTpb;
+  for (int i = blockIdx.x * kTpb + threadIdx.x; i < len; i += stride) {
+    const unsigned long long u = (unsigned long long)__double_as_longlong(v[i]);
+    key[i] = (u >> 63) ? ~u : (u | 0x8000000000000000ull);
+  }
+}
+__global__ void __launch_bounds__(kTpb)
+colrow_key_kernel(int len, const int* __restrict__ perm, const int* __restrict__ colof, const int* __restrict__ cidx,
+                  unsigned long long* __restrict__ key) {
+  const int stride = gridDim.x * kTpb;
+  for (int i = blockIdx.x * kTpb + threadIdx.x; i < len; i += stride) {
+    const int q = perm[i];
+    key[i] = ((unsigned long long)colof[q] << 32) | (unsigned)cidx[q];
+  }
+}
+// |c|_2^2 and |b|_2^2 of the UNSCALED HiPDLP data, added in index order like the host's loops (pdhg.cc:353-354): warp 0
+// sums the cost, warp 1 the rhs; every lane adds all terms in index order (shuffle broadcast).  The terms come in batches of
+// kNormBatch x 32, the next batch's loads in flight while the current one is added, so that the chain of dependent
+// additions, not the load latency, sets the time.
+constexpr int kNormBatch = 8;
+__global__ void __launch_bounds__(64)
+ordered_norms_kernel(int n, const double* __restrict__ cost, int m, const double* __restrict__ rhs, double* __restrict__ out) {
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int len = w == 0 ? n : m;
+  const double* v = w == 0 ? cost : rhs;
+  auto load = [&](int base, double* t) {
+#pragma unroll
+    for (int u = 0; u < kNormBatch; u++) {
+      const int i = base + 32 * u + lane;
+      t[u] = i < len ? v[i] * v[i] : 0.0;
+    }
+  };
+  double cur[kNormBatch], nxt[kNormBatch];
+  load(0, cur);
+  double sum = 0.0;
+  for (int base = 0; base < len; base += 32 * kNormBatch) {
+    load(base + 32 * kNormBatch, nxt);
+#pragma unroll
+    for (int u = 0; u < kNormBatch; u++) {
+      const int cb = base + 32 * u;
+      if (cb + 32 <= len) {
+#pragma unroll
+        for (int k = 0; k < 32; k++) sum = sum + __shfl_sync(0xffffffffu, cur[u], k);
+      } else if (cb < len) {
+        for (int k = 0; k < len - cb; k++) sum = sum + __shfl_sync(0xffffffffu, cur[u], k);
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < kNormBatch; u++) cur[u] = nxt[u];
+  }
+  if (lane == 0) out[w] = sum;
+}
 }  // namespace
 
 // ===================================================================================== the prologue
@@ -545,6 +612,7 @@ void make_perm_device(cudaStream_t s, Tmp& tmp, int len, int boundary, const int
 void DevicePrologue::run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, int long_threshold) {
   NvtxRange nvtx("b200pdlp: device prologue");
   nvtxRangePushA("H2D of the HighsLp arrays + formulate");
+  const bool hip = hipdlp;
   Tmp tmp;
   tmp.stream = s;
   const int n0 = lp.num_col, m = lp.num_row, nnz0 = lp.a_start[n0];
@@ -563,15 +631,18 @@ void DevicePrologue::run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, i
   // (radix sort), both length orderings, the slice plans and the three size read-backs -- runs underneath that copy.
   struct Side {
     cudaStream_t st = nullptr; cudaEvent_t structure_up = nullptr, values_up = nullptr;
+    cudaEvent_t norms_in = nullptr, norms_t0 = nullptr, norms_t1 = nullptr;   // HiPDLP: the ordered norms on this stream
     Side() {
       PREP_OK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
       PREP_OK(cudaEventCreateWithFlags(&structure_up, cudaEventDisableTiming));
       PREP_OK(cudaEventCreateWithFlags(&values_up, cudaEventDisableTiming));
+      PREP_OK(cudaEventCreateWithFlags(&norms_in, cudaEventDisableTiming));
+      PREP_OK(cudaEventCreate(&norms_t0));
+      PREP_OK(cudaEventCreate(&norms_t1));
     }
     ~Side() {   // before `tmp` hands the staging buffers back: no copy may still be writing them (exception paths)
       if (st) { cudaStreamSynchronize(st); cudaStreamDestroy(st); }
-      if (structure_up) cudaEventDestroy(structure_up);
-      if (values_up) cudaEventDestroy(values_up);
+      for (cudaEvent_t e : {structure_up, values_up, norms_in, norms_t0, norms_t1}) if (e) cudaEventDestroy(e);
     }
   } side;
   auto up = [&](cudaStream_t q, void* d, const void* h, size_t bytes) { if (bytes) PREP_OK(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, q)); };
@@ -595,7 +666,7 @@ void DevicePrologue::run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, i
   PREP_OK(cudaMemsetAsync(flags, 0, 4 * sizeof(int), s));
   PREP_OK(cudaMemsetAsync(eqlike + m, 0, sizeof(int), s));
   PREP_OK(cudaMemsetAsync(isbound + m, 0, sizeof(int), s));
-  if (m > 0) classify_rows_kernel<<<grid_for(m), kTpb, 0, s>>>(m, rl, ru, cls, eqlike, isbound);
+  if (m > 0) classify_rows_kernel<<<grid_for(m), kTpb, 0, s>>>(m, hip ? 1 : 0, rl, ru, cls, eqlike, isbound);
   exclusive_scan_i(s, tmp, eqlike, eq_ex, m + 1);     // eq_ex[m] = number of eq-like rows
   exclusive_scan_i(s, tmp, isbound, bd_ex, m + 1);    // bd_ex[m] = number of BOUND rows
   int* colof0 = tmp.get<int>(nnz0);
@@ -611,7 +682,8 @@ void DevicePrologue::run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, i
   PREP_OK(cudaMemcpyAsync(&h4[1], bd_ex + m, sizeof(int), cudaMemcpyDeviceToHost, s));
   PREP_OK(cudaMemcpyAsync(hflags, flags, 4 * sizeof(int), cudaMemcpyDeviceToHost, s));
   PREP_OK(cudaStreamSynchronize(s));
-  sc.neq = h4[0]; sc.nbound = h4[1]; sc.bad_index = hflags[0]; sc.cols_sorted = hflags[1] ? 0 : 1;
+  sc.neq = h4[0]; sc.nbound = h4[1]; sc.bad_index = hflags[0]; sc.cols_sorted = (hflags[1] & 1) ? 0 : 1;
+  const bool hip_sort = hip && hflags[1] != 0;   // a descent or a repeated row inside a column: sort by (new row, value)
   if (hflags[3]) throw std::invalid_argument("b200pdlp: a_start must be non-decreasing and within [0, nnz]");
   if (sc.bad_index) throw std::invalid_argument("b200pdlp: a_index entry outside [0, num_row)");
   const int neq = sc.neq, nbound = sc.nbound;
@@ -632,14 +704,67 @@ void DevicePrologue::run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, i
   double* colscale = tmp.get<double>(n);
   double* rhs = tmp.get<double>(m);
   double* rowscale = tmp.get<double>(m);
+  double* rup = hip ? tmp.get<double>(m) : nullptr;   // HiPDLP: row upper bounds, standard-form order
   col_vectors_kernel<<<grid_for(std::max(n0, 1)), kTpb, 0, s>>>(n0, n, nnz, lp.sense, a_start, cc, cl, cu, cost, lower, upper, cbeg, 1);
   if (m > 0)
     row_maps_kernel<<<grid_for(m), kTpb, 0, s>>>(m, n0, nnz0, neq, rl, ru, cls, eq_ex, bd_ex, arr.row_new_idx, arr.row_old,
-                                                 arr.slack_row, rhs, cost, lower, upper, cbeg, cidx, cval, colof);
+                                                 arr.slack_row, rhs, cost, lower, upper, cbeg, cidx, cval, colof, rup);
   unsigned* dest = tmp.get<unsigned>(nnz0);
   if (nnz0 > 0) {
     scatter_entries_kernel<<<grid_for(nnz0), kTpb, 0, s>>>(nnz0, a_start, a_index, colof0, fl_ex, cls, arr.row_new_idx, cidx, dest);
     PREP_OK(cudaMemcpyAsync(colof, colof0, (size_t)nnz0 * sizeof(int), cudaMemcpyDeviceToDevice, s));
+  }
+  if (hip_sort && nnz0 > 0) {
+    // the values are needed for the order: wait for them here (only inputs whose columns are not strictly ascending)
+    PREP_OK(cudaStreamWaitEvent(s, side.values_up, 0));
+    scatter_values_kernel<<<grid_for(nnz0), kTpb, 0, s>>>(nnz0, a_value, dest, cval);
+    unsigned long long* k_in = tmp.get<unsigned long long>(nnz0);
+    unsigned long long* k_out = tmp.get<unsigned long long>(nnz0);
+    int* v_in = tmp.get<int>(nnz0);
+    int* perm1 = tmp.get<int>(nnz0);
+    int* perm2 = tmp.get<int>(nnz0);
+    value_key_kernel<<<grid_for(nnz0), kTpb, 0, s>>>(nnz0, cval, k_in);
+    iota_kernel<<<grid_for(nnz0), kTpb, 0, s>>>(nnz0, v_in);
+    size_t bytes = 0;
+    PREP_OK(cub::DeviceRadixSort::SortPairs(nullptr, bytes, k_in, k_out, v_in, perm1, nnz0, 0, 64, s));
+    void* w = tmp.get<char>(bytes);
+    PREP_OK(cub::DeviceRadixSort::SortPairs(w, bytes, k_in, k_out, v_in, perm1, nnz0, 0, 64, s));
+    colrow_key_kernel<<<grid_for(nnz0), kTpb, 0, s>>>(nnz0, perm1, colof0, cidx, k_in);
+    const int end_bit = 32 + bits_for(std::max(n0 - 1, 1));
+    bytes = 0;
+    PREP_OK(cub::DeviceRadixSort::SortPairs(nullptr, bytes, k_in, k_out, perm1, perm2, nnz0, 0, end_bit, s));
+    w = tmp.get<char>(bytes);
+    PREP_OK(cub::DeviceRadixSort::SortPairs(w, bytes, k_in, k_out, perm1, perm2, nnz0, 0, end_bit, s));
+    int* ci = tmp.get<int>(nnz0);
+    double* cv = tmp.get<double>(nnz0);
+    gather_i_kernel<<<grid_for(nnz0), kTpb, 0, s>>>(nnz0, cidx, perm2, ci);
+    gather_d_kernel<<<grid_for(nnz0), kTpb, 0, s>>>(nnz0, cval, perm2, cv);
+    PREP_OK(cudaMemcpyAsync(cidx, ci, (size_t)nnz0 * sizeof(int), cudaMemcpyDeviceToDevice, s));
+    PREP_OK(cudaMemcpyAsync(cval, cv, (size_t)nnz0 * sizeof(double), cudaMemcpyDeviceToDevice, s));
+  }
+  // HiPDLP: row-major index of the CALLER's matrix for the postsolve's row_value = A x (stable sort of the original
+  // positions by row: a row's entries in column order, the order of the host's column loop)
+  int* orpos = nullptr;
+  if (hip) {
+    arr.orow_ptr = keep<int>(m + 1);
+    arr.orow_col = keep<int>(nnz0);
+    arr.orow_val = keep<double>(nnz0);
+    int* cnt = tmp.get<int>(m + 1);
+    PREP_OK(cudaMemsetAsync(cnt, 0, (size_t)(m + 1) * sizeof(int), s));
+    if (nnz0 > 0) hist_kernel<<<grid_for(nnz0), kTpb, 0, s>>>(nnz0, a_index, cnt);
+    exclusive_scan_i(s, tmp, cnt, arr.orow_ptr, m + 1);
+    if (nnz0 > 0) {
+      orpos = tmp.get<int>(nnz0);
+      int* k_out = tmp.get<int>(nnz0);
+      int* v_in = tmp.get<int>(nnz0);
+      iota_kernel<<<grid_for(nnz0), kTpb, 0, s>>>(nnz0, v_in);
+      size_t bytes = 0;
+      const int end_bit = bits_for(std::max(m - 1, 1));
+      PREP_OK(cub::DeviceRadixSort::SortPairs(nullptr, bytes, a_index, k_out, v_in, orpos, nnz0, 0, end_bit, s));
+      void* w = tmp.get<char>(bytes);
+      PREP_OK(cub::DeviceRadixSort::SortPairs(w, bytes, a_index, k_out, v_in, orpos, nnz0, 0, end_bit, s));
+      gather_i_kernel<<<grid_for(nnz0), kTpb, 0, s>>>(nnz0, colof0, orpos, arr.orow_col);
+    }
   }
   double* part = tmp.get<double>(4 * 4736);
   double* dsc = tmp.get<double>(16);
@@ -674,7 +799,7 @@ void DevicePrologue::run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, i
   }
   // columns not stored with ascending rows: positions ordered by (column, row) for A' (second, stable LSD pass)
   int* cpos = nullptr;
-  if (!sc.cols_sorted && nnz > 0) {
+  if (!hip && !sc.cols_sorted && nnz > 0) {
     int* k_in = tmp.get<int>(nnz);
     int* k_out = tmp.get<int>(nnz);
     cpos = tmp.get<int>(nnz);
@@ -717,6 +842,31 @@ void DevicePrologue::run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, i
     sumsq(rhs, m, dsc + 3, 3);
 
   };
+  // HiPDLP mode (PDLPSolver::preprocessLp + Scaling::scaleProblem; host twin host_prep_hipdlp.cpp)
+  double* unscaled = hip ? tmp.get<double>((size_t)n + m) : nullptr;
+  auto values_and_scaling_hip = [&]() {
+    NvtxRange r2("values: HiPDLP formulate + scaling");
+    PREP_OK(cudaStreamWaitEvent(s, side.values_up, 0));
+    col_vectors_kernel<<<grid_for(std::max(n0, 1)), kTpb, 0, s>>>(n0, n, nnz, 1.0, a_start, cc, cl, cu, cost, lower, upper, cbeg, 4);
+    if (nnz0 > 0 && !hip_sort) scatter_values_kernel<<<grid_for(nnz0), kTpb, 0, s>>>(nnz0, a_value, dest, cval);
+    if (nnz0 > 0) gather_d_kernel<<<grid_for(nnz0), kTpb, 0, s>>>(nnz0, a_value, orpos, arr.orow_val);
+    if (n > 0) fill_d_kernel<<<grid_for(n), kTpb, 0, s>>>(n, colscale, 1.0);
+    if (m > 0) fill_d_kernel<<<grid_for(m), kTpb, 0, s>>>(m, rowscale, 1.0);
+    // |c|^2 and |b|^2 of the unscaled data in index order: one warp each, on the side stream under the scaling and the layouts
+    if (n > 0) PREP_OK(cudaMemcpyAsync(unscaled, cost, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, s));
+    if (m > 0) PREP_OK(cudaMemcpyAsync(unscaled + n, rhs, (size_t)m * sizeof(double), cudaMemcpyDeviceToDevice, s));
+    PREP_OK(cudaEventRecord(side.norms_in, s));
+    PREP_OK(cudaStreamWaitEvent(side.st, side.norms_in, 0));
+    PREP_OK(cudaEventRecord(side.norms_t0, side.st));
+    ordered_norms_kernel<<<1, 64, 0, side.st>>>(n, unscaled, m, unscaled + n, dsc);
+    PREP_OK(cudaEventRecord(side.norms_t1, side.st));
+    double* cs = tmp.get<double>(n);
+    double* rs = tmp.get<double>(m);
+    DevForm F{n, m, nnz, cbeg, cidx, colof, cval, cost, lower, upper, colscale, rhs, rowscale};
+    DevScaleScratch w{cs, nullptr, rs, nullptr, dsc + 4};
+    sc.scaled = device_scale_hipdlp(s, F, w, rptr, rpos, rup, scaling_mode, ruiz_iterations) ? 1 : 0;
+    PREP_OK(cudaGetLastError());
+  };
   auto keep_the_form = [&]() {
     // the standard form in standard-form order survives the prologue (tests: b200pdlp_problem_get_*; several GPUs: the host
     // builds every rank's layouts from it)
@@ -726,6 +876,7 @@ void DevicePrologue::run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, i
     form.cost = dup_d(cost, n); form.lower = dup_d(lower, n); form.upper = dup_d(upper, n); form.colscale = dup_d(colscale, n);
     form.rhs = dup_d(rhs, m); form.rowscale = dup_d(rowscale, m);
     form.rptr = dup_i(rptr, m + 1); form.rpos = dup_i(rpos, nnz);
+    if (hip) form.row_upper = dup_d(rup, m);
     form.rcol = keep<int>(nnz);
     if (nnz > 0) gather_i_kernel<<<grid_for(nnz), kTpb, 0, s>>>(nnz, colof, rpos, form.rcol);
   };
@@ -803,7 +954,8 @@ void DevicePrologue::run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, i
   if (sc.a_lcount > 2000000000LL || sc.at_lcount > 2000000000LL)
     throw std::runtime_error("b200pdlp: long rows too large for 32-bit offsets");
 
-  values_and_scaling();
+  if (hip) values_and_scaling_hip();
+  else values_and_scaling();
 
   // ---- allocate and fill the layouts
   auto build = [&](DevSellOwned& M, Plan& P, int nrows, int ncols, long long padded, int nlong, int nsegs, long long lcount,
@@ -871,11 +1023,16 @@ void DevicePrologue::run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, i
     gather_d_kernel<<<grid_for(m), kTpb, 0, s>>>(m, rhs, arr.rperm, arr.rhs);
     gather_d_kernel<<<grid_for(m), kTpb, 0, s>>>(m, rowscale, arr.rperm, arr.rowscale);
   }
+  if (hip) {
+    arr.rup = keep<double>(m);
+    if (m > 0) gather_d_kernel<<<grid_for(m), kTpb, 0, s>>>(m, rup, arr.rperm, arr.rup);
+  }
   PREP_OK(cudaGetLastError());
   if (keep_form) keep_the_form();
   nvtxRangePop();
   struct { double d[5]; int tb; int sect[4]; int fit[2]; } hfin;
   memset(&hfin, 0, sizeof(hfin));
+  if (hip) PREP_OK(cudaStreamWaitEvent(s, side.norms_t1, 0));   // the ordered norms (side stream)
   PREP_OK(cudaMemcpyAsync(hfin.d, dsc, 5 * sizeof(double), cudaMemcpyDeviceToHost, s));
   PREP_OK(cudaMemcpyAsync(hfin.sect, sect, 4 * sizeof(int), cudaMemcpyDeviceToHost, s));
   PREP_OK(cudaMemcpyAsync(hfin.fit, fit, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -884,6 +1041,11 @@ void DevicePrologue::run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, i
   sc.norm_cost_sq = hfin.d[0]; sc.norm_rhs_sq = hfin.d[1]; sc.beta_cost_sq = hfin.d[2]; sc.beta_rhs_sq = hfin.d[3]; sc.amax = hfin.d[4];
   sc.a_sectors = hfin.sect[0]; sc.a_lanes = hfin.sect[1]; sc.at_sectors = hfin.sect[2]; sc.at_lanes = hfin.sect[3];
   A.tiles_staged = hfin.fit[0]; AT.tiles_staged = hfin.fit[1];
+  if (hip) {
+    float ms = 0.f;
+    PREP_OK(cudaEventElapsedTime(&ms, side.norms_t0, side.norms_t1));
+    sc.norms_ms = ms;
+  }
   if (hfin.tb) throw std::runtime_error("b200pdlp: matrix too large for 32-bit slice offsets");
 }
 
@@ -1002,6 +1164,69 @@ void launch_postsolve(cudaStream_t s, const DevProblemArrays& a, double sense, i
                                                     colscale, rowscale, row_value, row_dual);
 }
 
+namespace {
+__global__ void __launch_bounds__(kTpb)
+hip_init_kernel(int n, const double* __restrict__ lower, const double* __restrict__ upper, double* __restrict__ x,
+                double* __restrict__ xa) {
+  const int stride = gridDim.x * kTpb;
+  for (int i = blockIdx.x * kTpb + threadIdx.x; i < n; i += stride) {
+    double v = 0.0;
+    if (v > upper[i]) v = upper[i];
+    if (v < lower[i]) v = lower[i];
+    x[i] = v;
+    xa[i] = v;
+  }
+}
+__global__ void __launch_bounds__(kTpb)
+hip_post_cols_kernel(int n0, int converged, int scaled, double sense, const int* __restrict__ cinv, const double* __restrict__ x,
+                     const double* __restrict__ sp, const double* __restrict__ sn, const double* __restrict__ colscale,
+                     double* __restrict__ col_value, double* __restrict__ col_dual) {
+  const int stride = gridDim.x * kTpb;
+  for (int j = blockIdx.x * kTpb + threadIdx.x; j < n0; j += stride) {
+    const int jd = cinv[j];
+    const double cs = colscale[jd];
+    double xv = converged ? x[jd] : 0.0;
+    if (scaled) xv = xv / cs;
+    col_value[j] = xv;
+    const double a = sp[jd] * cs, b = sn[jd] * cs;
+    double v = a - b;
+    v = v * sense;
+    col_dual[j] = v;
+  }
+}
+// one thread per row (the postsolve runs once per solve; a long row is a few thousand dependent adds)
+__global__ void __launch_bounds__(kTpb)
+hip_post_rows_kernel(int m, int converged, int scaled, const int* __restrict__ new_idx, const int* __restrict__ cls,
+                     const int* __restrict__ rinv, const double* __restrict__ y, const double* __restrict__ rowscale,
+                     const int* __restrict__ optr, const int* __restrict__ ocol, const double* __restrict__ oval,
+                     const double* __restrict__ col_value, double* __restrict__ row_value, double* __restrict__ row_dual) {
+  const int stride = gridDim.x * kTpb;
+  for (int i = blockIdx.x * kTpb + threadIdx.x; i < m; i += stride) {
+    const int id = rinv[new_idx[i]];
+    double d = converged ? y[id] : 0.0;
+    if (scaled) d = d / rowscale[id];
+    row_dual[i] = cls[i] == 1 ? -d : d;
+    double v = 0.0;
+    for (int q = optr[i]; q < optr[i + 1]; q++) v = v + oval[q] * col_value[ocol[q]];
+    row_value[i] = v;
+  }
+}
+}  // namespace
+
+void launch_hip_init_point(cudaStream_t s, int n, const double* lower, const double* upper, double* x, double* xa) {
+  if (n > 0) hip_init_kernel<<<grid_for(n), kTpb, 0, s>>>(n, lower, upper, x, xa);
+}
+
+void launch_hip_postsolve(cudaStream_t s, const DevProblemArrays& a, double sense, int converged, int scaled, const double* x,
+                          const double* y, const double* sp, const double* sn, const double* colscale, const double* rowscale,
+                          double* col_value, double* col_dual, double* row_value, double* row_dual) {
+  if (a.n0 > 0)
+    hip_post_cols_kernel<<<grid_for(a.n0), kTpb, 0, s>>>(a.n0, converged, scaled, sense, a.cinv, x, sp, sn, colscale, col_value, col_dual);
+  if (a.m > 0)
+    hip_post_rows_kernel<<<grid_for(a.m), kTpb, 0, s>>>(a.m, converged, scaled, a.row_new_idx, a.row_class, a.rinv, y, rowscale,
+                                                        a.orow_ptr, a.orow_col, a.orow_val, col_value, row_value, row_dual);
+}
+
 void DevSellOwned::release() {
   dev_cache_free(slices); dev_cache_free(col); dev_cache_free(val); dev_cache_free(segs); dev_cache_free(long_rows);
   dev_cache_free(lcol); dev_cache_free(lval); dev_cache_free(long_partial); dev_cache_free(long_counter);
@@ -1013,6 +1238,7 @@ void DevicePrologue::release_form() {
   dev_cache_free(form.cbeg); dev_cache_free(form.cidx); dev_cache_free(form.cval); dev_cache_free(form.cost);
   dev_cache_free(form.lower); dev_cache_free(form.upper); dev_cache_free(form.colscale); dev_cache_free(form.rhs);
   dev_cache_free(form.rowscale); dev_cache_free(form.rptr); dev_cache_free(form.rpos); dev_cache_free(form.rcol);
+  dev_cache_free(form.row_upper);
   form = DevStdForm();
 }
 
@@ -1021,6 +1247,7 @@ void DevicePrologue::release_arrays() {
   dev_cache_free(arr.bound_ord); dev_cache_free(arr.rperm); dev_cache_free(arr.rinv); dev_cache_free(arr.cperm);
   dev_cache_free(arr.cinv); dev_cache_free(arr.cost); dev_cache_free(arr.lower); dev_cache_free(arr.upper);
   dev_cache_free(arr.colscale); dev_cache_free(arr.rhs); dev_cache_free(arr.rowscale);
+  dev_cache_free(arr.rup); dev_cache_free(arr.orow_ptr); dev_cache_free(arr.orow_col); dev_cache_free(arr.orow_val);
   arr = DevProblemArrays();
 }
 

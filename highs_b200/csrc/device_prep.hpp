@@ -35,6 +35,9 @@ struct PrepScalars {
   int a_nlong = 0, a_nsegs = 0, at_nlong = 0, at_nsegs = 0;
   long long a_lcount = 8, at_lcount = 8;
   double norm_cost_sq = 0, norm_rhs_sq = 0;                  // unscaled cost (x sense) and rhs: sums of squares
+                                                             // (HiPDLP mode: cost not x sense, added in index order)
+  int scaled = 0;                                            // HiPDLP mode: some scaling pass ran (StdForm::scaled)
+  float norms_ms = 0.f;                                      // HiPDLP mode: device time of the ordered norm sums
   double beta_cost_sq = 0, beta_rhs_sq = 0;                  // the same sums over the SCALED data (PDHG_Init_Step_Sizes)
   double amax = 0;                                           // max |a_ij| after scaling
   // sector sharing of the SpMV gathers, sampled over <= 4096 slices of each layout: distinct 32-byte sectors among the first
@@ -47,14 +50,20 @@ struct DevProblemArrays {
   int n = 0, m = 0, nnz = 0, neq = 0, n0 = 0, nbound = 0;
   // by ORIGINAL row
   int* row_new_idx = nullptr;   // [m] standard-form row
-  int* row_class = nullptr;     // [m] EQ 0, LEQ 1, GEQ 2, BOUND 3
+  int* row_class = nullptr;     // [m] EQ 0, LEQ 1, GEQ 2, BOUND 3 (HiPDLP mode: FREE 4)
   int* bound_ord = nullptr;     // [m + 1] exclusive count of BOUND rows: slack column of BOUND row i = n0 + bound_ord[i]
+                                // (HiPDLP mode: BOUND and FREE rows)
   int* row_old = nullptr;       // [m] original row of a standard-form row
   int* slack_row = nullptr;     // [nbound] original row of slack column n0 + k
   // device orderings (length-sorted in windows): perm[new] = old, inv[old] = new
   int *rperm = nullptr, *rinv = nullptr, *cperm = nullptr, *cinv = nullptr;
   // vectors in device order
   double *cost = nullptr, *lower = nullptr, *upper = nullptr, *colscale = nullptr, *rhs = nullptr, *rowscale = nullptr;
+  // HiPDLP mode only
+  double* rup = nullptr;        // [m] row upper bounds, device order
+  int* orow_ptr = nullptr;      // [m + 1] the caller's matrix, row-major (a row's entries in column order): row pointer,
+  int* orow_col = nullptr;      // [nnz0]  column ids,
+  double* orow_val = nullptr;   // [nnz0]  values (for the postsolve's row_value = A x)
 };
 
 struct DevSellOwned {   // one sliced-ELL matrix, blocks owned through the cache
@@ -80,6 +89,7 @@ struct DevStdForm {     // tests only (keep_form): the scaled standard form, sta
   int *cbeg = nullptr, *cidx = nullptr, *rptr = nullptr, *rpos = nullptr, *rcol = nullptr;   // rcol[q] = column of position rpos[q]
   double *cval = nullptr, *cost = nullptr, *lower = nullptr, *upper = nullptr, *colscale = nullptr, *rhs = nullptr,
          *rowscale = nullptr;
+  double* row_upper = nullptr;   // HiPDLP mode
 };
 
 struct DevicePrologue {
@@ -89,6 +99,10 @@ struct DevicePrologue {
   DevStdForm form;
   bool keep_form = false;
   bool stop_after_scaling = false;   // formulate + row index + scaling only (several GPUs: the layouts are built per rank by the host)
+  // HiPDLP mode (solver=hipdlp): its own formulate and scaling (host twin host_prep_hipdlp.cpp), the same orderings and
+  // layouts; `do_scale` is then ignored in favour of scaling_mode (bits 1 Ruiz, 4 Pock-Chambolle, 2 L2) / ruiz_iterations
+  bool hipdlp = false;
+  int scaling_mode = 0, ruiz_iterations = 0;
   size_t h2d_bytes = 0;
   // formulate + scale + row index + orderings + sliced-ELL layouts, all on stream `s`; returns with the stream idle.
   // Throws std::exception on bad input / CUDA errors (the caller releases what was produced so far).
@@ -106,5 +120,14 @@ void launch_postsolve(cudaStream_t s, const DevProblemArrays& a, double sense, i
                       const double* y, const double* ax, const double* cost, const double* lower, const double* upper,
                       const double* colscale, const double* rowscale, double* col_value, double* col_dual, double* row_value,
                       double* row_dual);
+// HiPDLP mode (host twins: engine.cu solve_hipdlp_on_device).  Initial point x = xa = proj_[l,u](0) (upper bound first,
+// then lower, pdhg.cc:512-552), device order.
+void launch_hip_init_point(cudaStream_t s, int n, const double* lower, const double* upper, double* x, double* xa);
+// unscaleSolution + postprocess (pdhg.cc:1883-1897, :359-492) into original-order arrays on the device: x, y only when
+// `converged` (else 0), divided by their scales only when `scaled`; s+ and s- always times col_scale; LEQ row duals negated;
+// col_dual = (s+ - s-) sense; row_value = A x over the caller's matrix, each row from 0.0 with the columns ascending
+void launch_hip_postsolve(cudaStream_t s, const DevProblemArrays& a, double sense, int converged, int scaled, const double* x,
+                          const double* y, const double* sp, const double* sn, const double* colscale, const double* rowscale,
+                          double* col_value, double* col_dual, double* row_value, double* row_dual);
 
 }  // namespace b200

@@ -447,9 +447,10 @@ struct DeviceSetup {
 
 // experiment (B200PDLP_SPMV_CTAS_PER_SM=k, one GPU, tree mode): the SpMV bodies run on a persistent grid of k CTAs per SM and
 // walk their slices in a software pipeline (spmv_sell_kernel<Epi, true>) instead of one CTA per 8 slices
-static void apply_spmv_grid(b200pdlp_problem* p) {
+// hipdlp: the HiPDLP mode's SpMVs (the fused step rule B200PDLP_FUSE_K4 is a pdlp-mode kernel: it stays off)
+static void apply_spmv_grid(b200pdlp_problem* p, bool hipdlp = false) {
   if (p->world != 1 || p->ordered) return;
-  if (const char* e = getenv("B200PDLP_FUSE_K4")) p->fuse_k4 = atoi(e) != 0 && p->AT.grid() > 0;
+  if (const char* e = getenv("B200PDLP_FUSE_K4"); e && !hipdlp) p->fuse_k4 = atoi(e) != 0 && p->AT.grid() > 0;
   auto val = [](const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; };
   const int both = val("B200PDLP_SPMV_CTAS_PER_SM", -1);
   // measured on one H100 (S3, DESIGN.md section 6): the pipelined walk at 3 CTAs per SM helps A'y a little (K3 87.3 -> 85.8
@@ -684,6 +685,25 @@ static bool use_device_prep(const b200pdlp_lp& lp, const b200pdlp_params& prm, i
   return true;
 }
 
+// the engine takes over one sliced-ELL matrix the device prologue built
+static void adopt_matrix(DeviceMatrix& M, DevSellOwned& O) {
+  M.slices.adopt(O.slices, O.nslices); M.col.adopt(O.col, (size_t)O.padded + 32); M.val.adopt(O.val, (size_t)O.padded + 32);
+  M.segs.adopt(O.segs, O.nsegs); M.long_rows.adopt(O.long_rows, O.nlong); M.lcol.adopt(O.lcol, (size_t)O.lcount);
+  M.lval.adopt(O.lval, (size_t)O.lcount); M.long_partial.adopt(O.long_partial, O.nsegs);
+  M.long_counter.adopt(O.long_counter, O.nlong);
+  if (O.ntiles > 0) { M.tile_lo.adopt(O.tile_lo, O.ntiles); M.tile_w.adopt(O.tile_w, O.ntiles); }
+  M.ntiles = O.ntiles; M.tiles_staged = O.tiles_staged;
+  M.host.nrows = O.nrows; M.host.ncols = O.ncols; M.host.padded = O.padded; M.host.lcount = O.lcount; M.host.n_partials = O.nsegs;
+  M.dev.nrows = O.nrows; M.dev.nslices = O.nslices;
+  M.dev.nblocks_body = (O.nslices + kThreads / 32 - 1) / (kThreads / 32);
+  M.dev.nblocks_full = M.dev.nblocks_body;
+  M.dev.nsegs = O.nsegs;
+  M.dev.slices = M.slices.p; M.dev.col = M.col.p; M.dev.val = M.val.p; M.dev.segs = M.segs.p; M.dev.long_rows = M.long_rows.p;
+  M.dev.lcol = M.lcol.p; M.dev.lval = M.lval.p; M.dev.long_partial = M.long_partial.p; M.dev.long_counter = M.long_counter.p;
+  M.dev.padded_total = (int)O.padded; M.dev.prefetch_dist = 0;
+  O = DevSellOwned();   // ownership moved
+}
+
 static void create_problem_device(const b200pdlp_lp& lp, const b200pdlp_params& prm, b200pdlp_problem* p) {
   NvtxRange nvtx("b200pdlp: prologue (device)");
   int ndev = 0;
@@ -724,23 +744,6 @@ static void create_problem_device(const b200pdlp_lp& lp, const b200pdlp_params& 
   p->nl = p->nl_real = n; p->c0 = 0; p->shard_len = n; p->seg_len = n;
   p->device_filled = true;
   p->csr_local.nrows = m; p->csr_local.ncols = n; p->csr_local.nnz = f.nnz;   // dimensions only (built on demand)
-  auto adopt_matrix = [&](DeviceMatrix& M, DevSellOwned& O) {
-    M.slices.adopt(O.slices, O.nslices); M.col.adopt(O.col, (size_t)O.padded + 32); M.val.adopt(O.val, (size_t)O.padded + 32);
-    M.segs.adopt(O.segs, O.nsegs); M.long_rows.adopt(O.long_rows, O.nlong); M.lcol.adopt(O.lcol, (size_t)O.lcount);
-    M.lval.adopt(O.lval, (size_t)O.lcount); M.long_partial.adopt(O.long_partial, O.nsegs);
-    M.long_counter.adopt(O.long_counter, O.nlong);
-    if (O.ntiles > 0) { M.tile_lo.adopt(O.tile_lo, O.ntiles); M.tile_w.adopt(O.tile_w, O.ntiles); }
-    M.ntiles = O.ntiles; M.tiles_staged = O.tiles_staged;
-    M.host.nrows = O.nrows; M.host.ncols = O.ncols; M.host.padded = O.padded; M.host.lcount = O.lcount; M.host.n_partials = O.nsegs;
-    M.dev.nrows = O.nrows; M.dev.nslices = O.nslices;
-    M.dev.nblocks_body = (O.nslices + kThreads / 32 - 1) / (kThreads / 32);
-    M.dev.nblocks_full = M.dev.nblocks_body;
-    M.dev.nsegs = O.nsegs;
-    M.dev.slices = M.slices.p; M.dev.col = M.col.p; M.dev.val = M.val.p; M.dev.segs = M.segs.p; M.dev.long_rows = M.long_rows.p;
-    M.dev.lcol = M.lcol.p; M.dev.lval = M.lval.p; M.dev.long_partial = M.long_partial.p; M.dev.long_counter = M.long_counter.p;
-    M.dev.padded_total = (int)O.padded; M.dev.prefetch_dist = 0;
-    O = DevSellOwned();   // ownership moved
-  };
   adopt_matrix(p->A, P.A);
   adopt_matrix(p->AT, P.AT);
   p->cost.adopt(P.arr.cost, n); p->lower.adopt(P.arr.lower, n); p->upper.adopt(P.arr.upper, n); p->colscale.adopt(P.arr.colscale, n);
@@ -2014,8 +2017,96 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
 
 // =================================================================================================== HiPDLP mode
 // solveLpHiPdlp -> PDLPSolver::solve (/root/reference/highs/pdlp/hipdlp/pdhg.cc:494-707) on the device, single GPU.
-// STATUS (round 2): runs on hardware (tests/test_gpu_hipdlp.py, tests/test_gpu_dropin.py, bench.py --solver hipdlp); the
-// prologue of this mode is still the host's (host_prep_hipdlp.cpp).
+// STATUS: runs on hardware (tests/test_gpu_hipdlp.py, tests/test_gpu_dropin.py, tests/test_gpu_hipdlp_device_prep.py,
+// bench.py --solver hipdlp).  Tree mode on one GPU takes the device-resident prologue, initial point and postsolve by default;
+// ordered mode keeps the host prologue (host_prep_hipdlp.cpp, the device prologue's tested twin).
+
+// The device prologue (DevicePrologue::hipdlp) unless: B200PDLP_DEVICE_PREP=0 or params.device_prep = -1 (the host prologue on
+// request), ordered mode (the standard form's max(n, m) <= ordered_max, decided with HiPDLP's classification: +-infinity
+// thresholds, a slack column for every ranged and free row), or an empty matrix.
+static bool use_device_prep_hipdlp(const b200pdlp_lp& lp, const b200pdlp_hipdlp_params& prm) {
+  if (const char* e = getenv("B200PDLP_DEVICE_PREP")) { if (atoi(e) == 0) return false; }
+  if (prm.device_prep == -1) return false;
+  const int omax = prm.ordered_max == 0 ? 4096 : prm.ordered_max;
+  if (omax > 0 && lp.num_col <= omax && lp.num_row <= omax) {
+    const double inf = std::numeric_limits<double>::infinity();
+    int nslack = 0;
+    for (int i = 0; i < lp.num_row; i++) {
+      const bool lo = lp.row_lower[i] > -inf, up = lp.row_upper[i] < inf;
+      nslack += (lo && up && lp.row_lower[i] != lp.row_upper[i]) || (!lo && !up);
+    }
+    if (lp.num_col + nslack <= omax) return false;
+  }
+  if (lp.num_col <= 0 || lp.num_row <= 0 || lp.a_start[lp.num_col] <= 0) return false;
+  return true;
+}
+
+static void hipdlp_buffers(b200pdlp_problem* p) {
+  const int n = p->n, m = p->m;
+  auto& h = p->hip;
+  for (DevBuf<double>* b : {&h.x, &h.xn, &h.rx, &h.xa, &h.aty, &h.atyp, &h.atdy, &h.hslack, &h.sp, &h.sn}) b->alloc(n);
+  for (DevBuf<double>* b : {&h.y, &h.yn, &h.ry, &h.ya, &h.axp, &h.dy}) b->alloc(m);
+  h.state.alloc(1);
+  h.hstate = static_cast<HipState*>(pinned_cache_alloc(sizeof(HipState), false));
+  size_t maxgrid = std::max<size_t>(kMaxEwBlocks, std::max(p->A.grid_full(), p->AT.grid_full()));
+  p->scratch_stride = 24 * maxgrid;
+  p->partials.alloc(p->scratch_stride * kNumSlots);
+  p->counters.alloc(kNumSlots);
+  p->terms.alloc(1);
+  p->ordered_cap = 0;
+  p->outs.alloc(kOutsCount);
+  p->houts = static_cast<double*>(pinned_cache_alloc(kOutsCount * sizeof(double), false));
+}
+
+// the whole HiPDLP prologue on the device: formulate, scale, unscaled norms, row index, orderings, both layouts, the
+// row-major copy of the caller's matrix for the postsolve (device_prep.cu); the host learns sizes and scalars only
+static void create_problem_hipdlp_device(const b200pdlp_lp& lp, const b200pdlp_hipdlp_params& prm, b200pdlp_problem* p) {
+  NvtxRange nvtx("b200pdlp: HiPDLP prologue (device)");
+  Laps lap;
+  CUDA_OK(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
+  cudaStream_t s = p->stream;
+  p->dev_form = true;
+  DevicePrologue& P = p->prep;
+  P.hipdlp = true;
+  P.scaling_mode = prm.scaling_mode;
+  P.ruiz_iterations = prm.ruiz_iterations;
+  try {
+    P.run(s, lp, true, /*long_threshold=*/512);
+  } catch (const std::invalid_argument& ex) {
+    throw Error(B200PDLP_ERR_ARG, ex.what());
+  } catch (const std::runtime_error& ex) {
+    throw Error(B200PDLP_ERR_CUDA, ex.what());
+  }
+  lap("setup", "device prologue (HiPDLP)");
+  if (lap.on) fprintf(stderr, "[b200pdlp setup] ordered |c|^2, |b|^2 (side stream, under the layouts) %8.3f ms\n", P.sc.norms_ms);
+  StdForm& f = p->form;
+  f = StdForm();
+  f.hipdlp = true;
+  f.n = P.arr.n; f.m = P.arr.m; f.nnz = P.arr.nnz; f.neq = P.arr.neq; f.n_orig = P.arr.n0;
+  f.sense = lp.sense; f.offset = lp.offset;
+  f.norm_cost = std::sqrt(P.sc.norm_cost_sq); f.norm_rhs = std::sqrt(P.sc.norm_rhs_sq);
+  f.amax = P.sc.amax;
+  f.scaled = P.sc.scaled != 0;
+  const int n = f.n, m = f.m;
+  p->n = n; p->m = m; p->ml = m; p->r0 = 0; p->r1 = m; p->neq_local = f.neq; p->ordered = false;
+  p->row_bounds = {0, m};
+  p->nl = p->nl_real = n; p->c0 = 0; p->shard_len = n; p->seg_len = n;
+  p->device_filled = true;
+  p->csr_local.nrows = m; p->csr_local.ncols = n; p->csr_local.nnz = f.nnz;
+  adopt_matrix(p->A, P.A);
+  adopt_matrix(p->AT, P.AT);
+  p->cost.adopt(P.arr.cost, n); p->lower.adopt(P.arr.lower, n); p->upper.adopt(P.arr.upper, n); p->colscale.adopt(P.arr.colscale, n);
+  p->rhs.adopt(P.arr.rhs, m); p->rowscale.adopt(P.arr.rowscale, m); p->hip.rup.adopt(P.arr.rup, m);
+  P.arr.cost = P.arr.lower = P.arr.upper = P.arr.colscale = P.arr.rhs = P.arr.rowscale = P.arr.rup = nullptr;
+  if (const char* ev = getenv("B200PDLP_PREFETCH")) { p->A.dev.prefetch_dist = atoi(ev); p->AT.dev.prefetch_dist = atoi(ev); }
+  apply_spmv_grid(p, /*hipdlp=*/true);
+  hipdlp_buffers(p);
+  p->io_col.alloc((size_t)2 * std::max(f.n_orig, 1), false);
+  p->io_row.alloc((size_t)2 * std::max(m, 1), false);
+  CUDA_OK(cudaStreamSynchronize(s));
+  lap("setup", "vectors + scratch");
+}
+
 static void create_problem_hipdlp(const b200pdlp_lp& lp, const b200pdlp_hipdlp_params& prm, b200pdlp_problem* p) {
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
@@ -2024,11 +2115,15 @@ static void create_problem_hipdlp(const b200pdlp_lp& lp, const b200pdlp_hipdlp_p
   if (prm.device >= 0) p->device = prm.device; else CUDA_OK(cudaGetDevice(&p->device));
   set_device(p);
   p->rank = 0; p->world = 1;
+  if (use_device_prep_hipdlp(lp, prm)) { create_problem_hipdlp_device(lp, prm, p); return; }
+  Laps lap;
   formulate_hipdlp(lp, p->form);
   scale_hipdlp(p->form, prm.scaling_mode, prm.ruiz_iterations);
+  lap("setup", "formulate + scale (host)");
   StdForm& f = p->form;
   HostLayout L;
   build_layout(f, 0, 1, prm.ordered_max, L);
+  lap("setup", "layouts (host)");
   p->r0 = L.r0; p->r1 = L.r1; p->ml = L.ml; p->neq_local = L.neq_local; p->ordered = L.ordered;
   p->n = f.n; p->m = f.m;
   p->nl = L.nl; p->nl_real = L.nl_real; p->c0 = 0; p->shard_len = L.shard_len; p->seg_len = L.seg_len;
@@ -2051,20 +2146,9 @@ static void create_problem_hipdlp(const b200pdlp_lp& lp, const b200pdlp_hipdlp_p
   };
   up_col(p->cost, f.cost); up_col(p->lower, f.lower); up_col(p->upper, f.upper); up_col(p->colscale, f.col_scale);
   up_row(p->rhs, f.rhs); up_row(p->hip.rup, f.row_upper); up_row(p->rowscale, f.row_scale);
-  auto& h = p->hip;
-  for (DevBuf<double>* b : {&h.x, &h.xn, &h.rx, &h.xa, &h.aty, &h.atyp, &h.atdy, &h.hslack, &h.sp, &h.sn}) b->alloc(n);
-  for (DevBuf<double>* b : {&h.y, &h.yn, &h.ry, &h.ya, &h.axp, &h.dy}) b->alloc(m);
-  h.state.alloc(1);
-  h.hstate = static_cast<HipState*>(pinned_cache_alloc(sizeof(HipState), false));
-  size_t maxgrid = std::max<size_t>(kMaxEwBlocks, std::max(p->A.grid_full(), p->AT.grid_full()));
-  p->scratch_stride = 24 * maxgrid;
-  p->partials.alloc(p->scratch_stride * kNumSlots);
-  p->counters.alloc(kNumSlots);
-  p->terms.alloc(1);
-  p->ordered_cap = 0;
-  p->outs.alloc(kOutsCount);
-  p->houts = static_cast<double*>(pinned_cache_alloc(kOutsCount * sizeof(double), false));
+  hipdlp_buffers(p);
   CUDA_OK(cudaDeviceSynchronize());
+  lap("setup", "upload + scratch");
 }
 
 static void hip_step(b200pdlp_problem* p, int k_offset, int is_major) {
@@ -2136,19 +2220,10 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
   }
   HipController ctl;   // step sizes, fixed-point error, convergence test, restart criteria, PID weight (host_prep_hipdlp.cpp)
   ctl.init(f.norm_cost, f.norm_rhs, op_norm_sq, prm.tolerance, prm.step_size_strategy);
-  // x = proj_[l,u](0), y = 0; anchors = iterates; A'y (:512-552)
+  // x = xa = proj_[l,u](0) (a kernel on the device-order bounds, upper first, then lower), y = ya = 0; A'y (:512-552)
   {
-    std::vector<double> x0(std::max(n, 1), 0.0);
-    for (int i = 0; i < n; i++) {
-      const int j = p->cperm[i];
-      double v = 0.0;
-      if (v > f.upper[j]) v = f.upper[j];
-      if (v < f.lower[j]) v = f.lower[j];
-      x0[i] = v;
-    }
-    CUDA_OK(cudaMemcpyAsync(h.x.p, x0.data(), (size_t)n * sizeof(double), cudaMemcpyHostToDevice, s));
+    launch_hip_init_point(s, n, p->lower.p, p->upper.p, h.x.p, h.xa.p);
     CUDA_OK(cudaMemsetAsync(h.y.p, 0, (size_t)std::max(m, 1) * sizeof(double), s));
-    CUDA_OK(cudaMemcpyAsync(h.xa.p, h.x.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, s));
     CUDA_OK(cudaMemsetAsync(h.ya.p, 0, (size_t)std::max(m, 1) * sizeof(double), s));
     for (DevBuf<double>* b : {&h.xn, &h.rx, &h.hslack, &h.sp, &h.sn, &h.atdy}) CUDA_OK(cudaMemsetAsync(b->p, 0, (size_t)std::max(n, 1) * sizeof(double), s));
     for (DevBuf<double>* b : {&h.yn, &h.ry, &h.dy}) CUDA_OK(cudaMemsetAsync(b->p, 0, (size_t)std::max(m, 1) * sizeof(double), s));
@@ -2220,40 +2295,62 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
   const double solve_seconds = std::chrono::duration<double>(clk::now() - t_loop).count();
   // unscaleSolution + postprocess (pdhg.cc:1883-1897, :359-492): the iterate is copied out ONLY on convergence --
   // an iteration-limited run returns x = y = 0, like the reference
-  std::vector<double> hx(std::max(n, 1), 0.0), hy(std::max(m, 1), 0.0), hsp(std::max(n, 1)), hsn(std::max(n, 1));
-  {
-    std::vector<double> t(std::max(std::max(n, m), 1));
-    auto down_col = [&](const double* d, std::vector<double>& v) {
-      CUDA_OK(cudaMemcpyAsync(t.data(), d, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, s));
-      CUDA_OK(cudaStreamSynchronize(s));
-      for (int i = 0; i < n; i++) v[p->cperm[i]] = t[i];
-    };
-    if (converged) {
-      down_col(sol_x, hx);
-      if (m) CUDA_OK(cudaMemcpyAsync(t.data(), sol_y, (size_t)m * sizeof(double), cudaMemcpyDeviceToHost, s));
-      CUDA_OK(cudaStreamSynchronize(s));
-      for (int i = 0; i < m; i++) hy[p->rperm[i]] = t[i];
+  if (p->dev_form) {
+    // on the device (launch_hip_postsolve), one download of the four original-order vectors
+    const int n0 = f.n_orig;
+    double* cv = p->io_col.p;
+    double* cd = cv + std::max(n0, 1);
+    double* rv = p->io_row.p;
+    double* rd = rv + std::max(m, 1);
+    launch_hip_postsolve(s, p->prep.arr, f.sense, converged ? 1 : 0, f.scaled ? 1 : 0, sol_x, sol_y, h.sp.p, h.sn.p, p->colscale.p,
+                         p->rowscale.p, cv, cd, rv, rd);
+    CUDA_OK(cudaGetLastError());
+    if (out->col_value && out->col_dual && out->row_value && out->row_dual) {
+      auto dn = [&](double* dst, const double* src, int len) {
+        if (len > 0) CUDA_OK(cudaMemcpyAsync(dst, src, (size_t)len * sizeof(double), cudaMemcpyDeviceToHost, s));
+      };
+      dn(out->col_value, cv, n0); dn(out->col_dual, cd, n0); dn(out->row_value, rv, m); dn(out->row_dual, rd, m);
     }
-    down_col(h.sp.p, hsp); down_col(h.sn.p, hsn);
-  }
-  if (f.scaled) {
-    for (int i = 0; i < n; i++) hx[i] /= f.col_scale[i];
-    for (int i = 0; i < m; i++) hy[i] /= f.row_scale[i];
-  }
-  for (int i = 0; i < n; i++) { hsp[i] *= f.col_scale[i]; hsn[i] *= f.col_scale[i]; }
-  if (out->col_value && out->col_dual && out->row_value && out->row_dual) {
-    for (int j = 0; j < f.n_orig; j++) out->col_value[j] = hx[j];
-    for (int i = 0; i < m; i++) {
-      const double d = hy[f.row_new_idx[i]];
-      out->row_dual[i] = f.row_class[i] == kLeq ? -d : d;
+    CUDA_OK(cudaStreamSynchronize(s));
+  } else {
+    std::vector<double> hx(std::max(n, 1), 0.0), hy(std::max(m, 1), 0.0), hsp(std::max(n, 1)), hsn(std::max(n, 1));
+    {
+      std::vector<double> t(std::max(std::max(n, m), 1));
+      auto down_col = [&](const double* d, std::vector<double>& v) {
+        CUDA_OK(cudaMemcpyAsync(t.data(), d, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, s));
+        CUDA_OK(cudaStreamSynchronize(s));
+        for (int i = 0; i < n; i++) v[p->cperm[i]] = t[i];
+      };
+      if (converged) {
+        down_col(sol_x, hx);
+        if (m) CUDA_OK(cudaMemcpyAsync(t.data(), sol_y, (size_t)m * sizeof(double), cudaMemcpyDeviceToHost, s));
+        CUDA_OK(cudaStreamSynchronize(s));
+        for (int i = 0; i < m; i++) hy[p->rperm[i]] = t[i];
+      }
+      down_col(h.sp.p, hsp); down_col(h.sn.p, hsn);
     }
-    for (int i = 0; i < m; i++) out->row_value[i] = 0.0;
-    for (int c = 0; c < lp.num_col; c++) {
-      const double xv = hx[c];
-      for (int q = lp.a_start[c]; q < lp.a_start[c + 1]; q++) out->row_value[lp.a_index[q]] += lp.a_value[q] * xv;
+    if (f.scaled) {
+      for (int i = 0; i < n; i++) hx[i] /= f.col_scale[i];
+      for (int i = 0; i < m; i++) hy[i] /= f.row_scale[i];
     }
-    for (int j = 0; j < f.n_orig; j++) { double v = hsp[j] - hsn[j]; v *= f.sense; out->col_dual[j] = v; }
+    for (int i = 0; i < n; i++) { hsp[i] *= f.col_scale[i]; hsn[i] *= f.col_scale[i]; }
+    if (out->col_value && out->col_dual && out->row_value && out->row_dual) {
+      for (int j = 0; j < f.n_orig; j++) out->col_value[j] = hx[j];
+      for (int i = 0; i < m; i++) {
+        const double d = hy[f.row_new_idx[i]];
+        out->row_dual[i] = f.row_class[i] == kLeq ? -d : d;
+      }
+      for (int i = 0; i < m; i++) out->row_value[i] = 0.0;
+      for (int c = 0; c < lp.num_col; c++) {
+        const double xv = hx[c];
+        for (int q = lp.a_start[c]; q < lp.a_start[c + 1]; q++) out->row_value[lp.a_index[q]] += lp.a_value[q] * xv;
+      }
+      for (int j = 0; j < f.n_orig; j++) { double v = hsp[j] - hsn[j]; v *= f.sense; out->col_dual[j] = v; }
+    }
   }
+  if (getenv("B200PDLP_TIMING"))
+    fprintf(stderr, "[b200pdlp solve] postsolve (%s) %8.3f ms\n", p->dev_form ? "device" : "host",
+            std::chrono::duration<double, std::milli>(clk::now() - t_loop).count() - 1e3 * solve_seconds);
   out->value_valid = 1; out->dual_valid = 1;
   out->term_code = term;
   out->term_iterate = timed_out ? 2 : 0;   // 2: the time limit, not the iteration limit, ended the run
@@ -3092,6 +3189,74 @@ int b200pdlp_form_layout_eval(b200pdlp_form* fh, int32_t rank, int32_t world, in
   });
 }
 
+// the device prologue against its host twin, array by array, bit for bit (report[0..31], see include/b200pdlp.h); false if
+// the sizes differ (nothing else is compared then)
+static double cmp_dev_i(const int* dev, const int* host, size_t cnt) {
+  std::vector<int> t(cnt);
+  if (cnt) CUDA_OK(cudaMemcpy(t.data(), dev, cnt * sizeof(int), cudaMemcpyDeviceToHost));
+  double bad = 0;
+  for (size_t i = 0; i < cnt; i++) bad += t[i] != host[i];
+  return bad;
+}
+static double cmp_dev_d(const double* dev, const double* host, size_t cnt) {
+  std::vector<double> t(cnt);
+  if (cnt) CUDA_OK(cudaMemcpy(t.data(), dev, cnt * sizeof(double), cudaMemcpyDeviceToHost));
+  double bad = 0;
+  for (size_t i = 0; i < cnt; i++) bad += memcmp(&t[i], &host[i], sizeof(double)) != 0;
+  return bad;
+}
+static bool prep_compare_arrays(const DevicePrologue& P, const StdForm& f, const HostLayout& L, double* report) {
+  const auto cmp_i = cmp_dev_i;
+  const auto cmp_d = cmp_dev_d;
+  const DevProblemArrays& a = P.arr;
+  const int n = f.n, m = f.m, nnz = f.nnz;
+  report[0] = a.n != n; report[1] = a.m != m; report[2] = a.nnz != nnz; report[3] = a.neq != f.neq;
+  if (report[0] + report[1] + report[2] + report[3] > 0) return false;
+  report[4] = cmp_i(P.form.cbeg, f.cbeg.data(), n + 1);
+  report[5] = cmp_i(P.form.cidx, f.cidx.data(), nnz);
+  report[6] = cmp_d(P.form.cval, f.cval.data(), nnz);
+  report[7] = cmp_d(P.form.cost, f.cost.data(), n);
+  report[8] = cmp_d(P.form.lower, f.lower.data(), n);
+  report[9] = cmp_d(P.form.upper, f.upper.data(), n);
+  report[10] = cmp_d(P.form.colscale, f.col_scale.data(), n);
+  report[11] = cmp_d(P.form.rhs, f.rhs.data(), m);
+  report[12] = cmp_d(P.form.rowscale, f.row_scale.data(), m);
+  report[13] = cmp_i(P.form.rptr, f.rptr.data(), m + 1);
+  report[14] = cmp_i(P.form.rpos, f.rpos.data(), nnz);
+  report[15] = cmp_i(a.row_new_idx, f.row_new_idx.data(), m);
+  report[16] = cmp_i(a.row_class, f.row_class.data(), m);
+  report[17] = cmp_i(a.rperm, L.rperm.data(), m);
+  report[18] = cmp_i(a.cperm, L.cperm.data(), n);
+  auto cmp_sell = [&](const DevSellOwned& D, const SellMatrix& H, double* r_slices, double* r_col, double* r_val, double* r_long) {
+    if ((size_t)D.nslices != H.slices.size() || D.padded != H.padded || (size_t)D.nlong != H.long_rows.size() ||
+        (size_t)D.nsegs != H.segs.size() || D.lcount != H.lcount) { *r_slices = -1; return; }
+    *r_slices = cmp_i(reinterpret_cast<const int*>(D.slices), reinterpret_cast<const int*>(H.slices.data()), 4 * H.slices.size());
+    *r_col = cmp_i(D.col, H.col.data(), (size_t)H.padded);
+    *r_val = cmp_d(D.val, H.val.data(), (size_t)H.padded);
+    *r_long = cmp_i(reinterpret_cast<const int*>(D.long_rows), reinterpret_cast<const int*>(H.long_rows.data()), 4 * H.long_rows.size()) +
+              cmp_i(reinterpret_cast<const int*>(D.segs), reinterpret_cast<const int*>(H.segs.data()), 4 * H.segs.size()) +
+              cmp_i(D.lcol, H.lcol.data(), H.lcol.size()) + cmp_d(D.lval, H.lval.data(), H.lval.size());
+  };
+  cmp_sell(P.A, L.A, report + 19, report + 20, report + 21, report + 25);
+  cmp_sell(P.AT, L.AT, report + 22, report + 23, report + 24, report + 26);
+  report[27] = P.sc.amax != f.amax;
+  report[28] = std::fabs(std::sqrt(P.sc.norm_cost_sq) - f.norm_cost) / (1.0 + f.norm_cost);
+  report[29] = std::fabs(std::sqrt(P.sc.norm_rhs_sq) - f.norm_rhs) / (1.0 + f.norm_rhs);
+  {
+    std::vector<double> t(std::max(n, m));
+    double bad = 0;
+    auto cmp_perm = [&](const double* dev, const std::vector<double>& v, const std::vector<int>& perm, int len) {
+      for (int i = 0; i < len; i++) t[i] = v[perm[i]];
+      bad += cmp_d(dev, t.data(), len);
+    };
+    cmp_perm(a.cost, f.cost, L.cperm, n); cmp_perm(a.lower, f.lower, L.cperm, n); cmp_perm(a.upper, f.upper, L.cperm, n);
+    cmp_perm(a.colscale, f.col_scale, L.cperm, n); cmp_perm(a.rhs, f.rhs, L.rperm, m); cmp_perm(a.rowscale, f.row_scale, L.rperm, m);
+    report[30] = bad;
+  }
+  report[31] = P.sc.cols_sorted;
+  return true;
+}
+
 // Test entry point: the device prologue (device_prep.cu) against its host twin (host_prep.cpp), array by array, bit for
 // bit.  report[k] = number of mismatching entries of item k (0 everywhere = identical), see include/b200pdlp.h.
 int b200pdlp_debug_prep_compare(const b200pdlp_lp* lp, int32_t scaling, double report[32]) {
@@ -3113,66 +3278,59 @@ int b200pdlp_debug_prep_compare(const b200pdlp_lp* lp, int32_t scaling, double r
     struct Cleanup { DevicePrologue& P; cudaStream_t s; ~Cleanup() { P.A.release(); P.AT.release(); P.release_arrays(); P.release_form(); cudaStreamDestroy(s); } } cleanup{P, s};
     try { P.run(s, *lp, scaling != 0, 512); }
     catch (const std::exception& ex) { throw Error(B200PDLP_ERR_CUDA, ex.what()); }
-    auto cmp_i = [&](const int* dev, const int* host, size_t cnt) {
-      std::vector<int> t(cnt);
-      if (cnt) CUDA_OK(cudaMemcpy(t.data(), dev, cnt * sizeof(int), cudaMemcpyDeviceToHost));
-      double bad = 0;
-      for (size_t i = 0; i < cnt; i++) bad += t[i] != host[i];
-      return bad;
-    };
-    auto cmp_d = [&](const double* dev, const double* host, size_t cnt) {
-      std::vector<double> t(cnt);
-      if (cnt) CUDA_OK(cudaMemcpy(t.data(), dev, cnt * sizeof(double), cudaMemcpyDeviceToHost));
-      double bad = 0;
-      for (size_t i = 0; i < cnt; i++) bad += memcmp(&t[i], &host[i], sizeof(double)) != 0;
-      return bad;
-    };
-    const DevProblemArrays& a = P.arr;
-    const int n = f.n, m = f.m, nnz = f.nnz;
-    report[0] = a.n != n; report[1] = a.m != m; report[2] = a.nnz != nnz; report[3] = a.neq != f.neq;
-    if (report[0] + report[1] + report[2] + report[3] > 0) return;
-    report[4] = cmp_i(P.form.cbeg, f.cbeg.data(), n + 1);
-    report[5] = cmp_i(P.form.cidx, f.cidx.data(), nnz);
-    report[6] = cmp_d(P.form.cval, f.cval.data(), nnz);
-    report[7] = cmp_d(P.form.cost, f.cost.data(), n);
-    report[8] = cmp_d(P.form.lower, f.lower.data(), n);
-    report[9] = cmp_d(P.form.upper, f.upper.data(), n);
-    report[10] = cmp_d(P.form.colscale, f.col_scale.data(), n);
-    report[11] = cmp_d(P.form.rhs, f.rhs.data(), m);
-    report[12] = cmp_d(P.form.rowscale, f.row_scale.data(), m);
-    report[13] = cmp_i(P.form.rptr, f.rptr.data(), m + 1);
-    report[14] = cmp_i(P.form.rpos, f.rpos.data(), nnz);
-    report[15] = cmp_i(a.row_new_idx, f.row_new_idx.data(), m);
-    report[16] = cmp_i(a.row_class, f.row_class.data(), m);
-    report[17] = cmp_i(a.rperm, L.rperm.data(), m);
-    report[18] = cmp_i(a.cperm, L.cperm.data(), n);
-    auto cmp_sell = [&](const DevSellOwned& D, const SellMatrix& H, double* r_slices, double* r_col, double* r_val, double* r_long) {
-      if ((size_t)D.nslices != H.slices.size() || D.padded != H.padded || (size_t)D.nlong != H.long_rows.size() ||
-          (size_t)D.nsegs != H.segs.size() || D.lcount != H.lcount) { *r_slices = -1; return; }
-      *r_slices = cmp_i(reinterpret_cast<const int*>(D.slices), reinterpret_cast<const int*>(H.slices.data()), 4 * H.slices.size());
-      *r_col = cmp_i(D.col, H.col.data(), (size_t)H.padded);
-      *r_val = cmp_d(D.val, H.val.data(), (size_t)H.padded);
-      *r_long = cmp_i(reinterpret_cast<const int*>(D.long_rows), reinterpret_cast<const int*>(H.long_rows.data()), 4 * H.long_rows.size()) +
-                cmp_i(reinterpret_cast<const int*>(D.segs), reinterpret_cast<const int*>(H.segs.data()), 4 * H.segs.size()) +
-                cmp_i(D.lcol, H.lcol.data(), H.lcol.size()) + cmp_d(D.lval, H.lval.data(), H.lval.size());
-    };
-    cmp_sell(P.A, L.A, report + 19, report + 20, report + 21, report + 25);
-    cmp_sell(P.AT, L.AT, report + 22, report + 23, report + 24, report + 26);
-    report[27] = P.sc.amax != f.amax;
-    report[28] = std::fabs(std::sqrt(P.sc.norm_cost_sq) - f.norm_cost) / (1.0 + f.norm_cost);
-    report[29] = std::fabs(std::sqrt(P.sc.norm_rhs_sq) - f.norm_rhs) / (1.0 + f.norm_rhs);
+    prep_compare_arrays(P, f, L, report);
+  });
+}
+
+// The same for the HiPDLP mode's prologue (DevicePrologue::hipdlp against host_prep_hipdlp.cpp); report[32..39] adds the
+// HiPDLP items, see include/b200pdlp.h.
+int b200pdlp_debug_prep_compare_hipdlp(const b200pdlp_lp* lp, int32_t scaling_mode, int32_t ruiz_iterations, double report[40]) {
+  DeviceGuard dg;
+  return guarded([&] {
+    check_lp(lp);
+    if (!report) throw Error(B200PDLP_ERR_ARG, "null argument");
+    for (int k = 0; k < 40; k++) report[k] = 0.0;
+    StdForm f;
+    formulate_hipdlp(*lp, f);
+    scale_hipdlp(f, scaling_mode, ruiz_iterations);
+    if (f.rptr.empty()) build_row_index(f);
+    HostLayout L;
+    build_layout(f, 0, 1, /*ordered_max=*/-1, L);
+    cudaStream_t s = nullptr;
+    CUDA_OK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+    DevicePrologue P;
+    P.keep_form = true;
+    P.hipdlp = true;
+    P.scaling_mode = scaling_mode;
+    P.ruiz_iterations = ruiz_iterations;
+    struct Cleanup { DevicePrologue& P; cudaStream_t s; ~Cleanup() { P.A.release(); P.AT.release(); P.release_arrays(); P.release_form(); cudaStreamDestroy(s); } } cleanup{P, s};
+    try { P.run(s, *lp, true, 512); }
+    catch (const std::exception& ex) { throw Error(B200PDLP_ERR_CUDA, ex.what()); }
+    if (!prep_compare_arrays(P, f, L, report)) return;
+    const int m = f.m, n0 = lp->num_col, nnz0 = lp->a_start[n0];
+    // the norms set omega and both step sizes: bitwise
+    const double nc = std::sqrt(P.sc.norm_cost_sq), nr = std::sqrt(P.sc.norm_rhs_sq);
+    report[28] = memcmp(&nc, &f.norm_cost, sizeof(double)) != 0;
+    report[29] = memcmp(&nr, &f.norm_rhs, sizeof(double)) != 0;
+    report[32] = cmp_dev_d(P.form.row_upper, f.row_upper.data(), m);
     {
-      std::vector<double> t(std::max(n, m));
-      double bad = 0;
-      auto cmp_perm = [&](const double* dev, const std::vector<double>& v, const std::vector<int>& perm, int len) {
-        for (int i = 0; i < len; i++) t[i] = v[perm[i]];
-        bad += cmp_d(dev, t.data(), len);
-      };
-      cmp_perm(a.cost, f.cost, L.cperm, n); cmp_perm(a.lower, f.lower, L.cperm, n); cmp_perm(a.upper, f.upper, L.cperm, n);
-      cmp_perm(a.colscale, f.col_scale, L.cperm, n); cmp_perm(a.rhs, f.rhs, L.rperm, m); cmp_perm(a.rowscale, f.row_scale, L.rperm, m);
-      report[30] = bad;
+      std::vector<double> t(m);
+      for (int i = 0; i < m; i++) t[i] = f.row_upper[L.rperm[i]];
+      report[33] = cmp_dev_d(P.arr.rup, t.data(), m);
     }
-    report[31] = P.sc.cols_sorted;
+    {
+      // row-major copy of the caller's matrix: counting sort of the positions by row (a row's entries in column order)
+      std::vector<int> ptr(m + 1, 0), col(nnz0), fill;
+      std::vector<double> val(nnz0);
+      for (int q = 0; q < nnz0; q++) ptr[lp->a_index[q] + 1]++;
+      for (int i = 0; i < m; i++) ptr[i + 1] += ptr[i];
+      fill.assign(ptr.begin(), ptr.end() - 1);
+      for (int j = 0; j < n0; j++)
+        for (int q = lp->a_start[j]; q < lp->a_start[j + 1]; q++) { const int k = fill[lp->a_index[q]]++; col[k] = j; val[k] = lp->a_value[q]; }
+      report[34] = cmp_dev_i(P.arr.orow_ptr, ptr.data(), m + 1);
+      report[35] = cmp_dev_i(P.arr.orow_col, col.data(), nnz0) + cmp_dev_d(P.arr.orow_val, val.data(), nnz0);
+    }
+    report[36] = (P.sc.scaled != 0) != f.scaled;
   });
 }
 

@@ -2445,7 +2445,12 @@ void launch_hip_dual(cudaStream_t s, const DevSell& A, const HipState* st, int k
   HipDualEpilogue e{};
   e.st = st; e.k_offset = k_offset; e.is_major = is_major; e.in = rx; e.y = y; e.ya = ya; e.rlo = rlo; e.rup = rup;
   e.yn = yn; e.ry = ry;
-  spmv_sell_kernel<HipDualEpilogue><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, ReduceScratch{nullptr, nullptr, nullptr, 0, 0});
+  // the launch shape the engine chose for A (apply_spmv_grid): a persistent grid must take the pipelined walk, which visits
+  // every slice; the one-slice-per-warp kernel on that capped grid would skip slices
+  const ReduceScratch none{nullptr, nullptr, nullptr, 0, 0};
+  if (A.tiled) { launch_tile(s, A, e, none); return; }
+  if (A.pipelined) spmv_sell_kernel<HipDualEpilogue, true><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, none);
+  else spmv_sell_kernel<HipDualEpilogue, false><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, none);
 }
 
 // ------------------------------------------------------------------------------------------------ checks

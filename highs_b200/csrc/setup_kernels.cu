@@ -177,13 +177,123 @@ __global__ void __launch_bounds__(kTpb) abs_max_kernel(int nnz, const double* __
   if ((threadIdx.x & 31) == 0) atomic_max_nonneg(amax, am);
 }
 
+// ---- HiPDLP mode (Scaling::scaleProblem, hipdlp/scaling.cc; host twin host_prep_hipdlp.cpp::scale_hipdlp)
+// OP 0: max |v| (Ruiz), 1: sum |v| (Pock-Chambolle, alpha = 1), 2: sum v^2 (L2).  The host evaluates the Pock-Chambolle terms as
+// std::pow(|v|, 2 - alpha) and std::pow(|v|, alpha) with alpha = 1; glibc's pow returns its argument exactly for an exponent of
+// 1.0, so |v| IS that term.  CUDA's pow is only guaranteed to 2 ulp, so it is not called here.
+template <int OP> __device__ __forceinline__ double hip_term(double v) { return OP == 2 ? v * v : fabs(v); }
+template <int OP> __device__ __forceinline__ double hip_op(double a, double t) {
+  return OP == 0 ? (a < t ? t : a) : a + t;   // std::max(a, t) / a + t, the host's folds
+}
+// out[r] = fold of the terms of entries [ptr[r], ptr[r+1]) (through pos when given) in index order; same scheme as
+// ordered_abs_sums_kernel: one thread per short row, one warp (loads in parallel, additions in order) per long row
+template <int OP>
+__global__ void __launch_bounds__(kTpb)
+hip_ordered_reduce_kernel(int nrows, const int* __restrict__ ptr, const int* __restrict__ pos, const double* __restrict__ val,
+                          double* __restrict__ out) {
+  const int r = blockIdx.x * kTpb + threadIdx.x, lane = threadIdx.x & 31;
+  int b = 0, e = 0;
+  if (r < nrows) { b = ptr[r]; e = ptr[r + 1]; }
+  const bool is_long = e - b > kShortRow;
+  if (r < nrows && !is_long) {
+    double a = 0.0;
+    for (int q = b; q < e; q++) a = hip_op<OP>(a, hip_term<OP>(val[pos ? pos[q] : q]));
+    out[r] = a;
+  }
+  unsigned todo = __ballot_sync(0xffffffffu, is_long);
+  while (todo) {
+    const int src = __ffs(todo) - 1;
+    todo &= todo - 1;
+    const int lb = __shfl_sync(0xffffffffu, b, src), le = __shfl_sync(0xffffffffu, e, src);
+    double a = 0.0;
+    for (int base = lb; base < le; base += 32) {
+      const int q = base + lane;
+      const double t = q < le ? hip_term<OP>(val[pos ? pos[q] : q]) : 0.0;
+      const int cnt = (le - base) < 32 ? (le - base) : 32;
+      for (int k = 0; k < cnt; k++) a = hip_op<OP>(a, __shfl_sync(0xffffffffu, t, k));
+    }
+    if (lane == 0) out[(r - lane) + src] = a;
+  }
+}
+// fold -> factor in place (scaling.cc: Ruiz sqrt with 0 -> 1; Pock-Chambolle sqrt(pow(sum, 1 / alpha)) = sqrt(sum); L2
+// sqrt(sqrt(sum)); empty / zero -> 1)
+__global__ void __launch_bounds__(kTpb) hip_factors_kernel(int len, int op, double* __restrict__ v) {
+  const int stride = gridDim.x * kTpb;
+  for (int i = blockIdx.x * kTpb + threadIdx.x; i < len; i += stride) {
+    const double q = v[i];
+    double f;
+    if (op == 0) { f = sqrt(q); if (f == 0.0) f = 1.0; }
+    else if (op == 1) f = q > 0.0 ? sqrt(q) : 1.0;
+    else f = q > 0.0 ? sqrt(sqrt(q)) : 1.0;
+    v[i] = f;
+  }
+}
+// Scaling::applyScaling (scaling.cc:232-263)
+__global__ void __launch_bounds__(kTpb)
+hip_apply_cols_kernel(int n, const double* __restrict__ cs, double* __restrict__ cost, double* __restrict__ lower,
+                      double* __restrict__ upper, double* __restrict__ colscale) {
+  const int stride = gridDim.x * kTpb;
+  for (int j = blockIdx.x * kTpb + threadIdx.x; j < n; j += stride) {
+    const double c = cs[j];
+    cost[j] = cost[j] / c;
+    if (lower[j] > -INFINITY) lower[j] = lower[j] * c;
+    if (upper[j] < INFINITY) upper[j] = upper[j] * c;
+    colscale[j] = colscale[j] * c;
+  }
+}
+__global__ void __launch_bounds__(kTpb)
+hip_apply_rows_kernel(int m, const double* __restrict__ rs, double* __restrict__ rhs, double* __restrict__ rup,
+                      double* __restrict__ rowscale) {
+  const int stride = gridDim.x * kTpb;
+  for (int i = blockIdx.x * kTpb + threadIdx.x; i < m; i += stride) {
+    const double r = rs[i];
+    if (rhs[i] > -INFINITY) rhs[i] = rhs[i] / r;
+    if (rup[i] < INFINITY) rup[i] = rup[i] / r;
+    rowscale[i] = rowscale[i] * r;
+  }
+}
+__global__ void __launch_bounds__(kTpb)
+hip_apply_nnz_kernel(int nnz, const int* __restrict__ cidx, const int* __restrict__ colof, const double* __restrict__ rs,
+                     const double* __restrict__ cs, double* __restrict__ cval) {
+  const int stride = gridDim.x * kTpb;
+  for (int p = blockIdx.x * kTpb + threadIdx.x; p < nnz; p += stride) cval[p] = cval[p] / (rs[cidx[p]] * cs[colof[p]]);   // ONE division by the product
+}
+
 inline int grid_for(long long work) {
   long long g = (work + kTpb - 1) / kTpb;
   if (g < 1) g = 1;
   return (int)(g > kGridUnit * 32LL ? kGridUnit * 32LL : g);
 }
 inline int warp_grid(int rows) { return (int)(((long long)rows * 32 + kTpb - 1) / kTpb); }
+
+template <int OP>
+void hip_pass(cudaStream_t s, const DevForm& F, DevScaleScratch& w, const int* rptr, const int* rpos, double* row_upper) {
+  if (F.n > 0) {
+    hip_ordered_reduce_kernel<OP><<<(F.n + kTpb - 1) / kTpb, kTpb, 0, s>>>(F.n, F.cbeg, nullptr, F.cval, w.cs);
+    hip_factors_kernel<<<grid_for(F.n), kTpb, 0, s>>>(F.n, OP, w.cs);
+  }
+  if (F.m > 0) {
+    hip_ordered_reduce_kernel<OP><<<(F.m + kTpb - 1) / kTpb, kTpb, 0, s>>>(F.m, rptr, rpos, F.cval, w.rs);
+    hip_factors_kernel<<<grid_for(F.m), kTpb, 0, s>>>(F.m, OP, w.rs);
+  }
+  if (F.n > 0) hip_apply_cols_kernel<<<grid_for(F.n), kTpb, 0, s>>>(F.n, w.cs, F.cost, F.lower, F.upper, F.colscale);
+  if (F.nnz > 0) hip_apply_nnz_kernel<<<grid_for(F.nnz), kTpb, 0, s>>>(F.nnz, F.cidx, F.colof, w.rs, w.cs, F.cval);
+  if (F.m > 0) hip_apply_rows_kernel<<<grid_for(F.m), kTpb, 0, s>>>(F.m, w.rs, F.rhs, row_upper, F.rowscale);
+}
 }  // namespace
+
+bool device_scale_hipdlp(cudaStream_t s, const DevForm& F, DevScaleScratch& w, const int* rptr, const int* rpos,
+                         double* row_upper, int scaling_mode, int ruiz_iterations) {
+  bool scaled = false;
+  if (scaling_mode & 1) {
+    for (int it = 0; it < ruiz_iterations; it++) hip_pass<0>(s, F, w, rptr, rpos, row_upper);
+    scaled = true;
+  }
+  if (scaling_mode & 4) { hip_pass<1>(s, F, w, rptr, rpos, row_upper); scaled = true; }
+  if (scaling_mode & 2) { hip_pass<2>(s, F, w, rptr, rpos, row_upper); scaled = true; }
+  device_abs_max(s, F.nnz, F.cval, w.amax);
+  return scaled;
+}
 
 void device_abs_max(cudaStream_t s, int nnz, const double* val, double* amax) {
   cudaMemsetAsync(amax, 0, sizeof(double), s);

@@ -28,6 +28,14 @@ void device_abs_max(cudaStream_t s, int nnz, const double* val, double* amax);
 // the Pock-Chambolle pass (:174-231); rptr[m+1] / rpos[nnz] = device copy of the row-major index of the nonzeros
 void device_scale_pock_chambolle(cudaStream_t s, const DevForm& F, DevScaleScratch& w, const int* rptr, const int* rpos);
 
+// HiPDLP mode: Scaling::scaleProblem (hipdlp/scaling.cc:23-263), bit-identical to host_prep_hipdlp.cpp::scale_hipdlp.
+// scaling_mode bits: 1 Ruiz (inf-norm) x ruiz_iterations, then 4 Pock-Chambolle (alpha = 1), then 2 L2.  Every pass divides
+// a_ij by (r_i * c_j), scales only finite bounds and rhs / row_upper entries, and accumulates the scales.  Column sums run in
+// a column's storage order, row sums in the order of the row-major index (rptr / rpos).  w.amax = max |a_ij| at the end.
+// Returns true if any pass ran (the host's StdForm::scaled).
+bool device_scale_hipdlp(cudaStream_t s, const DevForm& F, DevScaleScratch& w, const int* rptr, const int* rpos,
+                         double* row_upper, int scaling_mode, int ruiz_iterations);
+
 // where a sliced-ELL fill reads a row's entries from: entries [beg[r], end[r]) of the OLD row r, optionally through an
 // index (pos), column id = colmap[idx[.] - idx_offset], value = val[.]
 struct SellSource {

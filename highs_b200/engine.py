@@ -44,7 +44,8 @@ class CParams(C.Structure):
 class CHipdlpParams(C.Structure):
     _fields_ = [("tolerance", C.c_double), ("iter_limit", C.c_int32), ("scaling_mode", C.c_int32),
                 ("ruiz_iterations", C.c_int32), ("step_size_strategy", C.c_int32), ("time_limit", C.c_double),
-                ("ordered_max", C.c_int32), ("device", C.c_int32), ("log_level", C.c_int32), ("reserved", C.c_int32 * 3)]
+                ("ordered_max", C.c_int32), ("device", C.c_int32), ("log_level", C.c_int32), ("device_prep", C.c_int32),
+                ("reserved", C.c_int32 * 2)]
 
 
 class CWarm(C.Structure):
@@ -73,7 +74,8 @@ ABI_SYMBOLS = [
     "b200pdlp_form_get_vector", "b200pdlp_form_get_csc", "b200pdlp_form_get_csr", "b200pdlp_form_get_row_map",
     "b200pdlp_form_layout_eval", "b200pdlp_p2p_link_local", "b200pdlp_solve_multi",
     "b200pdlp_hipdlp_form_create", "b200pdlp_hipdlp_power_method", "b200pdlp_hipdlp_default_params",
-    "b200pdlp_solve_hipdlp", "b200pdlp_hipdlp_controller_replay", "b200pdlp_debug_prep_compare", "b200pdlp_release_cache",
+    "b200pdlp_solve_hipdlp", "b200pdlp_hipdlp_controller_replay", "b200pdlp_debug_prep_compare",
+    "b200pdlp_debug_prep_compare_hipdlp", "b200pdlp_release_cache",
     "b200pdlp_host_register", "b200pdlp_host_unregister", "b200pdlp_primal_step", "b200pdlp_dual_step", "b200pdlp_residuals",
     "b200pdlp_kkt_check", "b200pdlp_kkt_check_host", "b200pdlp_kkt_default_tolerances",
 ]
@@ -238,6 +240,21 @@ def prep_compare(lp: HighsLp, scaling: int = 1) -> dict:
     return dict(zip(PREP_ITEMS, rep.tolist()))
 
 
+PREP_ITEMS_HIPDLP = PREP_ITEMS[:28] + ["norm_cost_bits", "norm_rhs_bits"] + PREP_ITEMS[30:] + [
+    "row_upper", "row_upper_device_order", "orig_row_ptr", "orig_row_entries", "scaled", "unused37", "unused38", "unused39"]
+
+
+def prep_compare_hipdlp(lp: HighsLp, scaling_mode: int = 5, ruiz_iterations: int = 10) -> dict:
+    """b200pdlp_debug_prep_compare_hipdlp: the HiPDLP mode's device prologue against its host twin, mismatches per array."""
+    L = lib()
+    L.b200pdlp_debug_prep_compare_hipdlp.argtypes = [C.POINTER(CLp), C.c_int32, C.c_int32, _dp]
+    clp, keep = make_clp(lp)
+    rep = np.zeros(40)
+    _check(L.b200pdlp_debug_prep_compare_hipdlp(C.byref(clp), scaling_mode, ruiz_iterations, _p(rep, _dp)),
+           "b200pdlp_debug_prep_compare_hipdlp")
+    return dict(zip(PREP_ITEMS_HIPDLP, rep.tolist()))
+
+
 def lp_arrays(lp: HighsLp):
     a = lp.a_matrix_
     return [a.start_, a.index_, a.value_, lp.col_cost_, lp.col_lower_, lp.col_upper_, lp.row_lower_, lp.row_upper_]
@@ -311,7 +328,8 @@ def hipdlp_controller_replay(norm_cost, norm_rhs, op_norm_sq, tolerance, strateg
 
 def solve_hipdlp(lp: HighsLp, **params) -> dict:
     """b200pdlp_solve_hipdlp: the HiPDLP mode (reflected Halpern PDHG, solver=hipdlp) on one GPU; parameters are the
-    HighsOptions of the same meaning (tolerance, iter_limit, scaling_mode, ruiz_iterations, step_size_strategy ...)."""
+    HighsOptions of the same meaning (tolerance, iter_limit, scaling_mode, ruiz_iterations, step_size_strategy ...), and
+    device_prep=-1 for the host prologue instead of the device-resident one."""
     L = lib()
     L.b200pdlp_hipdlp_default_params.argtypes = [C.POINTER(CHipdlpParams)]
     L.b200pdlp_hipdlp_default_params.restype = None

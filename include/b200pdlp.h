@@ -223,7 +223,7 @@ int b200pdlp_form_get_csr(b200pdlp_form* f, int32_t* rowptr, int32_t* col, doubl
 /* row_new_idx[m], row_class[m] by ORIGINAL row (EQ=0, LEQ=1, GEQ=2, BOUND=3) */
 int b200pdlp_form_get_row_map(const b200pdlp_form* f, int32_t* row_new_idx, int32_t* row_class);
 
-/* HiPDLP mode (solver=hipdlp; SURVEY.md 8(a) a20 / 8(f) rank 2), host prologue only so far: PDLPSolver::preprocessLp
+/* HiPDLP mode (solver=hipdlp; SURVEY.md 8(a) a20 / 8(f) rank 2), the host prologue (the device prologue's twin): PDLPSolver::preprocessLp
  * (hipdlp/pdhg.cc:152-358) + Scaling::scaleProblem (hipdlp/scaling.cc; scaling_mode bits 1 Ruiz, 4 Pock-Chambolle, 2 L2 =
  * HighsOptions::pdlp_scaling_mode, ruiz_iterations = pdlp_ruiz_iterations).  The form answers the b200pdlp_form_* getters;
  * rows carry an upper bound too: b200pdlp_form_get_vector(which = 6).  row_class uses 4 for FREE rows. */
@@ -232,7 +232,10 @@ int b200pdlp_hipdlp_form_create(const b200pdlp_lp* lp, int32_t scaling_mode, int
  * Parameters are the HighsOptions the reference's setup() reads (hipdlp/pdhg.cc:1783-1874).  term_code is B200PDLP_OPTIMAL or
  * B200PDLP_TIMELIMIT_OR_ITERLIMIT (term_iterate = 2 when it was the time limit); like the reference, a run that does not
  * converge returns x = y = 0 (the iterate is copied out only on convergence, pdhg.cc:784-899).
- * STATUS (round 2): runs on hardware; tests/test_gpu_hipdlp.py (bit-exact against the oracle), tests/test_gpu_dropin.py (through
+ * Tree mode on one GPU (the standard form's max(n, m) > ordered_max) runs the prologue, the initial point and the postsolve
+ * on the device by default (device_prep.cu; the same bits as the host prologue, tests/test_gpu_hipdlp_device_prep.py); ordered
+ * mode, device_prep = -1 or B200PDLP_DEVICE_PREP=0 take the host prologue (host_prep_hipdlp.cpp).
+ * STATUS: runs on hardware; tests/test_gpu_hipdlp.py (bit-exact against the oracle), tests/test_gpu_dropin.py (through
  * the shim), bench.py --solver hipdlp. */
 typedef struct {
   double tolerance;           /* pdlp_optimality_tolerance, or kkt_tolerance when set */
@@ -244,7 +247,8 @@ typedef struct {
   int32_t ordered_max;        /* as in b200pdlp_params: checks add in the reference's order up to this size */
   int32_t device;             /* CUDA device ordinal; -1 = current */
   int32_t log_level;
-  int32_t reserved[3];
+  int32_t device_prep;        /* 0 = device prologue where it applies (one GPU, tree mode), -1 = always the host prologue */
+  int32_t reserved[2];
 } b200pdlp_hipdlp_params;
 void b200pdlp_hipdlp_default_params(b200pdlp_hipdlp_params* p);
 int b200pdlp_solve_hipdlp(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params* params, b200pdlp_result* out);
@@ -282,6 +286,12 @@ int b200pdlp_partition_rows(const b200pdlp_lp* lp, int32_t world, int32_t* bound
  *  27 max|a_ij|  28, 29 relative error of |c|_2, |b|_2 (tree sums vs sequential)  30 vectors in device order
  *  31 (info) 1 if every column is stored with ascending rows */
 int b200pdlp_debug_prep_compare(const b200pdlp_lp* lp, int32_t scaling, double report[32]);
+/* The same for the HiPDLP mode: its device prologue against formulate_hipdlp + scale_hipdlp + build_layout (ordered_max = -1).
+ * report[0..31] as above, except 28, 29: 1 if |c|_2, |b|_2 differ in any bit (both are sums in index order here), and
+ *  32 row_upper (standard-form order)  33 row_upper in device order
+ *  34 row pointer of the row-major copy of the caller's matrix  35 its column ids + values (a row's entries in column order)
+ *  36 1 if the device and the host disagree on whether any scaling pass ran   37-39 unused (0) */
+int b200pdlp_debug_prep_compare_hipdlp(const b200pdlp_lp* lp, int32_t scaling_mode, int32_t ruiz_iterations, double report[40]);
 
 /* The engine keeps the device blocks of finished solves in a process-wide cache (a solve allocates ~60 buffers; cudaMalloc /
  * cudaFree would cost more than the prologue).  This returns them to the driver.  B200PDLP_CACHE_MB caps the cache. */
