@@ -197,14 +197,20 @@ struct LocalGroup {
   std::condition_variable cv;
   int world = 0, count = 0;
   unsigned long long gen = 0;
-  void arrive_and_wait() {
+  bool shared[2] = {false, false};
+  // returns rank 0's `v` to every rank (rank < 0: a plain rendezvous).  The value sits in the slot of the generation's
+  // parity: rank 0 writes that slot again two generations later, which it cannot reach before every rank has passed the
+  // generation in between, i.e. has read this one.
+  bool arrive_and_wait(int rank = -1, bool v = false) {
     std::unique_lock<std::mutex> lk(m);
     const unsigned long long g = gen;
-    if (++count == world) { count = 0; gen++; cv.notify_all(); return; }
+    if (rank == 0) shared[g & 1] = v;
+    if (++count == world) { count = 0; gen++; cv.notify_all(); return shared[g & 1]; }
     if (!cv.wait_for(lk, std::chrono::seconds(120), [&] { return gen != g; })) {
       count--;
       throw std::runtime_error("logical shards: a peer rank's solve thread did not arrive");
     }
+    return shared[g & 1];
   }
 };
 
@@ -243,8 +249,13 @@ struct b200pdlp_problem {
     DevBuf<HipState> state;
     HipState* hstate = nullptr;    // pinned
     cudaGraphExec_t graph = nullptr;
+    long long graph_launches = 0;  // kernels in `graph`
     ~HipBuffers() { if (graph) cudaGraphExecDestroy(graph); if (hstate) pinned_cache_free(hstate); }
   } hip;
+  // HiPDLP on several GPUs (b200pdlp_solve_hipdlp_multi): every rank's problem, by rank (empty on one GPU).  This rank owns
+  // device rows [hip_r0, hip_r1) and device columns [hip_c0, hip_c1) of the one-GPU orders; its vectors are full length.
+  std::vector<b200pdlp_problem*> hip_peers;
+  int hip_r0 = 0, hip_r1 = 0, hip_c0 = 0, hip_c1 = 0;
   bool local_link = false;         // peers are problems of this process (logical shards, b200pdlp_p2p_link_local)
   std::shared_ptr<b200::LocalGroup> group;   // their host-side rendezvous
   bool no_graph = false;           // B200PDLP_NO_GRAPH: every pass and check as direct launches (debugging aid)
@@ -2151,9 +2162,91 @@ static void create_problem_hipdlp(const b200pdlp_lp& lp, const b200pdlp_hipdlp_p
   lap("setup", "upload + scratch");
 }
 
+// ---- HiPDLP on several GPUs.  Rank g computes whole rows of A (device rows [hip_r0, hip_r1)) and whole rows of A'
+// (device columns [hip_c0, hip_c1)) in the one-GPU entry order, and every check sum runs over full vectors with the
+// one-GPU kernels, so a G-rank solve returns the one-GPU bits (DESIGN section 5, "HiPDLP on several GPUs").
+using HipBufs = b200pdlp_problem::HipBuffers;
+using HipVec = DevBuf<double> HipBufs::*;
+static bool hip_sharded(const b200pdlp_problem* p) { return !p->hip_peers.empty(); }
+
+// what the solve loop reads of the standard form on every rank (rank 0 takes the whole form for the postsolve)
+static StdForm hip_form_scalars(const StdForm& f) {
+  StdForm s;
+  s.hipdlp = true; s.scaled = f.scaled;
+  s.n = f.n; s.m = f.m; s.nnz = f.nnz; s.neq = f.neq; s.n_orig = f.n_orig;
+  s.sense = f.sense; s.offset = f.offset; s.norm_cost = f.norm_cost; s.norm_rhs = f.norm_rhs; s.amax = f.amax;
+  return s;
+}
+
+// rank g's problem on `device`: A_g, A_g' (build_hipdlp_shard) and every vector full length in the one-GPU device order
+static void create_problem_hipdlp_shard(const StdForm& f, const HipShards& S, int rank, int device, b200pdlp_problem* p) {
+  p->device = device;
+  set_device(p);
+  p->rank = rank; p->world = S.world;
+  p->form = hip_form_scalars(f);
+  p->n = f.n; p->m = f.m; p->ml = f.m; p->r0 = 0; p->r1 = f.m; p->neq_local = f.neq; p->ordered = S.ordered;
+  p->nl = p->nl_real = f.n; p->c0 = 0; p->shard_len = f.n; p->seg_len = f.n;
+  p->hip_r0 = S.rb[rank]; p->hip_r1 = S.rb[rank + 1]; p->hip_c0 = S.cb[rank]; p->hip_c1 = S.cb[rank + 1];
+  if (rank == 0) { p->rperm = S.rperm; p->cperm = S.cperm; }   // the postsolve's un-permutation
+  build_hipdlp_shard(S, rank, p->A.host, p->AT.host);
+  CUDA_OK(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
+  p->A.upload();
+  p->AT.upload();
+  const int n = f.n, m = f.m;
+  std::vector<double> t(std::max(std::max(n, m), 1));
+  auto up = [&](DevBuf<double>& d, const std::vector<double>& v, const std::vector<int>& perm) {
+    for (size_t i = 0; i < perm.size(); i++) t[i] = v[perm[i]];
+    d.alloc(perm.size(), false); d.upload(t.data(), perm.size());
+  };
+  up(p->cost, f.cost, S.cperm); up(p->lower, f.lower, S.cperm); up(p->upper, f.upper, S.cperm); up(p->colscale, f.col_scale, S.cperm);
+  up(p->rhs, f.rhs, S.rperm); up(p->hip.rup, f.row_upper, S.rperm); up(p->rowscale, f.row_scale, S.rperm);
+  hipdlp_buffers(p);
+  p->flags.alloc(kMaxPeers);   // arrival words, one per peer (hip_barrier_kernel)
+  p->epochs.alloc(1);
+  p->fault.alloc(1);
+  CUDA_OK(cudaDeviceSynchronize());
+}
+
+static void hip_barrier(b200pdlp_problem* p) {
+  PeerFlags pf{};
+  for (size_t g = 0; g < p->hip_peers.size(); g++) pf.f[g] = p->hip_peers[g]->flags.p;
+  launch_hip_barrier(p->stream, pf, p->world, p->rank, p->epochs.p, p->fault.p);
+  p->launches++;
+}
+static PeerVec hip_peer_vec(const b200pdlp_problem* p, HipVec v, int offset = 0) {
+  PeerVec r{};
+  for (size_t g = 0; g < p->hip_peers.size(); g++) r.v[g] = (p->hip_peers[g]->hip.*v).p + offset;
+  return r;
+}
+// this rank's columns (cols) or rows of the given vectors into every peer's copies
+static void hip_gather(b200pdlp_problem* p, bool cols, std::initializer_list<HipVec> vs) {
+  HipGather g{};
+  g.lo = cols ? p->hip_c0 : p->hip_r0;
+  g.hi = cols ? p->hip_c1 : p->hip_r1;
+  for (HipVec v : vs) { g.src[g.nv] = (p->hip.*v).p; g.dst[g.nv] = hip_peer_vec(p, v); g.nv++; }
+  launch_hip_gather(p->stream, g, p->world, p->rank);
+  p->launches++;
+}
+
 static void hip_step(b200pdlp_problem* p, int k_offset, int is_major) {
   auto& h = p->hip;
   cudaStream_t s = p->stream;
+  if (hip_sharded(p)) {
+    // The reflected x and the blended y go straight into the peers' copies, and two barriers per step suffice.  A rank
+    // stores into a peer's rx only after it has left the previous step's second barrier, which every rank reaches after
+    // its A_g rx, the only reader of rx in a block.  It stores into a peer's y only after this step's first barrier, which
+    // every rank reaches after the previous step's A_g' y, the only reader of other ranks' rows of y in a block.
+    const int r0 = p->hip_r0, c0 = p->hip_c0;
+    launch_hip_primal_shard(s, c0, p->hip_c1, h.state.p, k_offset, is_major, h.x.p, h.xa.p, p->cost.p, h.aty.p, p->lower.p,
+                            p->upper.p, h.rx.p, h.xn.p, h.hslack.p, hip_peer_vec(p, &HipBufs::rx), p->world, p->rank);
+    hip_barrier(p);
+    launch_hip_dual_shard(s, p->A.dev, h.state.p, k_offset, is_major, h.rx.p, h.y.p + r0, h.ya.p + r0, p->rhs.p + r0,
+                          h.rup.p + r0, h.yn.p + r0, h.ry.p + r0, hip_peer_vec(p, &HipBufs::y, r0), p->world, p->rank);
+    hip_barrier(p);
+    launch_spmv_plain(s, p->AT.dev, h.y.p, h.aty.p + c0);
+    p->launches += 3;
+    return;
+  }
   launch_hip_primal(s, p->n, h.state.p, k_offset, is_major, h.x.p, h.xa.p, p->cost.p, h.aty.p, p->lower.p, p->upper.p,
                     h.rx.p, h.xn.p, h.hslack.p);
   launch_hip_dual(s, p->A.dev, h.state.p, k_offset, is_major, h.rx.p, h.y.p, h.ya.p, p->rhs.p, h.rup.p, h.yn.p, h.ry.p);
@@ -2161,18 +2254,38 @@ static void hip_step(b200pdlp_problem* p, int k_offset, int is_major) {
   p->launches += 3;
 }
 
-// the scalars of one check (launch_hip_check) for the iterate (x, y); with_fpe: also the fixed-point error of the major
-// step that produced it.  Leaves them in p->houts[0..8] after ONE synchronisation.
-static void hip_check(b200pdlp_problem* p, const double* x, const double* y, int with_fpe, int use_cached_slack) {
+// the scalars of one check (launch_hip_check) for the iterate (x, y), or with `major` for (xn, yn) together with the
+// fixed-point error and the cached slacks of the major step that produced it.  Leaves them in p->houts[0..8] after ONE
+// synchronisation.  Several GPUs: the iterate is gathered to every rank, each rank forms its rows of A x and its
+// columns of A'y (and A'dy), those are gathered too, and every rank then sums full vectors with the one-GPU kernels,
+// so all ranks see the one-GPU sums and take the same decisions.
+static void hip_check(b200pdlp_problem* p, int major) {
   auto& h = p->hip;
   cudaStream_t s = p->stream;
-  if (with_fpe) {
+  const HipVec xv = major ? &HipBufs::xn : &HipBufs::x, yv = major ? &HipBufs::yn : &HipBufs::y;
+  const double* x = (h.*xv).p;
+  const double* y = (h.*yv).p;
+  const bool shard = hip_sharded(p);
+  const int r0 = p->hip_r0, c0 = p->hip_c0;
+  if (shard) {
+    if (major) { hip_gather(p, true, {xv, &HipBufs::hslack}); hip_gather(p, false, {yv, &HipBufs::ry}); }
+    else { hip_gather(p, true, {xv}); hip_gather(p, false, {yv}); }
+    hip_barrier(p);
+  }
+  if (major) {
     launch_hip_diff(s, p->m, y, h.ry.p, h.dy.p);
-    launch_spmv_plain(s, p->AT.dev, h.dy.p, h.atdy.p);
+    launch_spmv_plain(s, p->AT.dev, h.dy.p, h.atdy.p + c0);
     p->launches += 2;
   }
-  launch_spmv_plain(s, p->A.dev, x, h.axp.p);
-  launch_spmv_plain(s, p->AT.dev, y, h.atyp.p);
+  launch_spmv_plain(s, p->A.dev, x, h.axp.p + r0);
+  launch_spmv_plain(s, p->AT.dev, y, h.atyp.p + c0);
+  if (shard) {
+    if (major) hip_gather(p, true, {&HipBufs::atyp, &HipBufs::atdy});
+    else hip_gather(p, true, {&HipBufs::atyp});
+    hip_gather(p, false, {&HipBufs::axp});
+    hip_barrier(p);
+  }
+  const int with_fpe = major, use_cached_slack = major;
   launch_hip_slack(s, p->n, use_cached_slack, h.hslack.p, p->cost.p, h.atyp.p, p->lower.p, p->upper.p, h.sp.p, h.sn.p);
   HipCheckArgs a{};
   a.n = p->n; a.m = p->m; a.neq = p->neq_local; a.scaled = p->form.scaled ? 1 : 0; a.offset = p->form.offset;
@@ -2182,7 +2295,14 @@ static void hip_check(b200pdlp_problem* p, const double* x, const double* y, int
   launch_hip_check(s, a, with_fpe, p->ordered ? 1 : 0, p->rs(kSlotChk, std::max(p->n, p->m)), p->outs.p);
   p->launches += 4;
   CUDA_OK(cudaMemcpyAsync(p->houts, p->outs.p, 9 * sizeof(double), cudaMemcpyDeviceToHost, s));
+  int* hfault = reinterpret_cast<int*>(p->houts + 32);
+  if (shard) CUDA_OK(cudaMemcpyAsync(hfault, p->fault.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   CUDA_OK(cudaStreamSynchronize(s));
+  if (shard) {
+    if (*hfault) throw Error(B200PDLP_ERR_STATE, "HiPDLP shards: a barrier timed out (a peer rank did not arrive)");
+    // no rank starts the next step (which stores into its peers' rx) before every rank has finished reading rx here
+    p->group->arrive_and_wait();
+  }
 }
 
 static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, const b200pdlp_hipdlp_params& prm, b200pdlp_result* out) {
@@ -2195,22 +2315,58 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
   cudaStream_t s = p->stream;
   const int n = p->n, m = p->m;
   const long long launches0 = p->launches;
+  const bool shard = hip_sharded(p);
+  const int r0 = p->hip_r0, c0 = p->hip_c0;
+  CudaEvent evl0, evl1;
+  if (!h.graph) {   // steps 2 .. 40 of a block: 38 minor steps and the closing major step (:629-632)
+    const long long l0 = p->launches;
+    cudaGraph_t g = nullptr;
+    CUDA_OK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+    for (int i = 2; i <= 39; i++) hip_step(p, i, 0);
+    hip_step(p, 40, 1);
+    CUDA_OK(cudaStreamEndCapture(s, &g));
+    CUDA_OK(cudaGraphInstantiate(&h.graph, g, 0));
+    CUDA_OK(cudaGraphDestroy(g));
+    h.graph_launches = p->launches - l0;   // counted when replayed
+    p->launches = l0;
+  }
+  if (shard) {
+    // On one device a graph upload, a lazy kernel load or an allocation waits for every running kernel, a peer's spinning
+    // barrier included (DESIGN section 5): all of them happen before any rank launches its first barrier.  The kernels
+    // were loaded when the ranks were linked; the initial-point kernel and the copy / fill operations are loaded here by
+    // running them once.
+    CUDA_OK(cudaGraphUpload(h.graph, s));
+    launch_hip_init_point(s, n, p->lower.p, p->upper.p, h.x.p, h.xa.p);
+    CUDA_OK(cudaMemsetAsync(h.dy.p, 0, (size_t)std::max(m, 1) * sizeof(double), s));
+    CUDA_OK(cudaMemcpyAsync(h.dy.p, h.ry.p, (size_t)std::max(m, 1) * sizeof(double), cudaMemcpyDeviceToDevice, s));
+    CUDA_OK(cudaStreamSynchronize(s));
+    p->group->arrive_and_wait();
+  }
   // PDLPSolver::powerMethod (pdhg.cc:1529-1671) on the device: 20 iterations of q <- A A'q / |A A'q| from the ones vector,
-  // lambda = |A'q|^2; no host round trip inside (the norm stays on the device), one read-back at the end
+  // lambda = |A'q|^2; no host round trip inside (the norm stays on the device), one read-back at the end.  Several GPUs:
+  // every rank holds q and z whole, forms its columns of w and its rows of z, and gathers them; the norms are then the
+  // one-GPU sums over full vectors.
   double op_norm_sq = 1.0;
   if (n > 0 && m > 0) {
     double* xq = h.dy.p;      // m-vectors: q (dy), z (axp); n-vector: w = A'q (atdy)
     double* zq = h.axp.p;
     double* wq = h.atdy.p;
+    // several GPUs: A'z goes to a second buffer, so that a rank's next A'q cannot overwrite a peer's A'z while that peer
+    // still sums it (no barrier lies between the two)
+    const HipVec wzv = shard ? &HipBufs::atyp : &HipBufs::atdy;
+    double* wz = (h.*wzv).p;
     double* sc = p->outs.p + 16;
     launch_fill(s, m, xq, 1.0);
     for (int it = 0; it < 20; it++) {
-      launch_spmv_plain(s, p->AT.dev, xq, wq);
-      launch_spmv_plain(s, p->A.dev, wq, zq);
+      launch_spmv_plain(s, p->AT.dev, xq, wq + c0);
+      if (shard) { hip_gather(p, true, {&HipBufs::atdy}); hip_barrier(p); }
+      launch_spmv_plain(s, p->A.dev, wq, zq + r0);
+      if (shard) { hip_gather(p, false, {&HipBufs::axp}); hip_barrier(p); }
       launch_hip_dot(s, m, zq, zq, p->ordered ? 1 : 0, p->rs(kSlotChk, m), sc);
       launch_hip_div_norm(s, m, zq, sc);
-      launch_spmv_plain(s, p->AT.dev, zq, wq);
-      launch_hip_dot(s, n, wq, wq, p->ordered ? 1 : 0, p->rs(kSlotChk, n), sc + 1);
+      launch_spmv_plain(s, p->AT.dev, zq, wz + c0);
+      if (shard) { hip_gather(p, true, {wzv}); hip_barrier(p); }
+      launch_hip_dot(s, n, wz, wz, p->ordered ? 1 : 0, p->rs(kSlotChk, n), sc + 1);
       CUDA_OK(cudaMemcpyAsync(xq, zq, (size_t)m * sizeof(double), cudaMemcpyDeviceToDevice, s));
       p->launches += 6;
     }
@@ -2227,45 +2383,37 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
     CUDA_OK(cudaMemsetAsync(h.ya.p, 0, (size_t)std::max(m, 1) * sizeof(double), s));
     for (DevBuf<double>* b : {&h.xn, &h.rx, &h.hslack, &h.sp, &h.sn, &h.atdy}) CUDA_OK(cudaMemsetAsync(b->p, 0, (size_t)std::max(n, 1) * sizeof(double), s));
     for (DevBuf<double>* b : {&h.yn, &h.ry, &h.dy}) CUDA_OK(cudaMemsetAsync(b->p, 0, (size_t)std::max(m, 1) * sizeof(double), s));
-    launch_spmv_plain(s, p->AT.dev, h.y.p, h.aty.p);
+    launch_spmv_plain(s, p->AT.dev, h.y.p, h.aty.p + c0);
     CUDA_OK(cudaStreamSynchronize(s));
+    if (shard) p->group->arrive_and_wait();   // nobody gathers into a peer's vectors before that peer has set them
   }
   auto push_state = [&]() {
     h.hstate->primal_step = ctl.primal_step; h.hstate->dual_step = ctl.dual_step; h.hstate->halpern_iteration = ctl.halpern_iteration;
     CUDA_OK(cudaMemcpyAsync(h.state.p, h.hstate, sizeof(HipState), cudaMemcpyHostToDevice, s));
   };
-  if (!h.graph) {   // steps 2 .. 40 of a block: 38 minor steps and the closing major step (:629-632)
-    cudaGraph_t g = nullptr;
-    CUDA_OK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-    for (int i = 2; i <= 39; i++) hip_step(p, i, 0);
-    hip_step(p, 40, 1);
-    CUDA_OK(cudaStreamEndCapture(s, &g));
-    CUDA_OK(cudaGraphInstantiate(&h.graph, g, 0));
-    CUDA_OK(cudaGraphDestroy(g));
-    p->launches -= 39 * 3;   // counted when replayed
-  }
   const double t_lim = (prm.time_limit >= 0 && std::isfinite(prm.time_limit)) ? prm.time_limit : -1.0;   // < 0: none
   int term = B200PDLP_TIMELIMIT_OR_ITERLIMIT;
   bool converged = false, timed_out = false;
   const auto t_loop = clk::now();
-  CudaEvent evl0, evl1;
   CUDA_OK(cudaEventRecord(evl0, s));
-  hip_check(p, h.x.p, h.y.p, 0, 0);   // iteration 0 (:566-572)
+  hip_check(p, 0);   // iteration 0 (:566-572)
   const double* sol_x = h.x.p;
   const double* sol_y = h.y.p;
   if (ctl.converged(p->houts)) { converged = true; }
   else {
     while (ctl.iters < prm.iter_limit) {
-      if (t_lim >= 0 && std::chrono::duration<double>(clk::now() - t_loop).count() > t_lim) { timed_out = true; break; }
+      bool over = t_lim >= 0 && std::chrono::duration<double>(clk::now() - t_loop).count() > t_lim;
+      if (shard) over = p->group->arrive_and_wait(p->rank, over);   // rank 0's clock decides for every rank
+      if (over) { timed_out = true; break; }
       push_state();
       hip_step(p, 1, 1);
       if (ctl.pending_restart_fpe) {   // the restart's reference fixed-point error is that of the first step after it (:600-608)
-        hip_check(p, h.xn.p, h.yn.p, 1, 1);
+        hip_check(p, 1);
         ctl.restart_reference(p->houts);
       }
       CUDA_OK(cudaGraphLaunch(h.graph, s));
-      p->launches += 39 * 3;
-      hip_check(p, h.xn.p, h.yn.p, 1, 1);
+      p->launches += h.graph_launches;
+      hip_check(p, 1);
       const bool restart = ctl.after_block(p->houts);
       if (prm.log_level >= 2)
         printf("[b200pdlp hipdlp] it %8d  pobj %+.8e dobj %+.8e  pfeas %.2e dfeas %.2e  fpe %.3e  weight %.3e\n", ctl.iters,
@@ -2274,11 +2422,12 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
         converged = true; sol_x = h.xn.p; sol_y = h.yn.p; break;
       }
       if (restart) {   // anchors and iterates <- the PDHG iterate of the last major step (:664-688)
+        // (several GPUs: xn and yn were gathered by the check, so every rank copies them whole and holds full anchors)
         CUDA_OK(cudaMemcpyAsync(h.xa.p, h.xn.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, s));
         CUDA_OK(cudaMemcpyAsync(h.ya.p, h.yn.p, (size_t)std::max(m, 1) * sizeof(double), cudaMemcpyDeviceToDevice, s));
         CUDA_OK(cudaMemcpyAsync(h.x.p, h.xn.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, s));
         CUDA_OK(cudaMemcpyAsync(h.y.p, h.yn.p, (size_t)std::max(m, 1) * sizeof(double), cudaMemcpyDeviceToDevice, s));
-        launch_spmv_plain(s, p->AT.dev, h.y.p, h.aty.p);
+        launch_spmv_plain(s, p->AT.dev, h.y.p, h.aty.p + c0);
         p->launches++;
       }
     }
@@ -2288,6 +2437,8 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
   if (converged) term = B200PDLP_OPTIMAL;
   CUDA_OK(cudaEventRecord(evl1, s));
   CUDA_OK(cudaEventSynchronize(evl1));
+  // the postsolve's pageable copies wait for every kernel of the context: no barrier kernel may still be in flight
+  if (shard) p->group->arrive_and_wait();
   float loop_ms = 0.f;
   CUDA_OK(cudaEventElapsedTime(&loop_ms, evl0, evl1));
   out->loop_device_ms = loop_ms;
@@ -2312,7 +2463,7 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
       dn(out->col_value, cv, n0); dn(out->col_dual, cd, n0); dn(out->row_value, rv, m); dn(out->row_dual, rd, m);
     }
     CUDA_OK(cudaStreamSynchronize(s));
-  } else {
+  } else if (p->rank == 0) {   // (several GPUs: rank 0 holds the whole iterate and slacks after the final check)
     std::vector<double> hx(std::max(n, 1), 0.0), hy(std::max(m, 1), 0.0), hsp(std::max(n, 1)), hsn(std::max(n, 1));
     {
       std::vector<double> t(std::max(std::max(n, m), 1));
@@ -2915,6 +3066,111 @@ int b200pdlp_solve_hipdlp(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params* p
     }
     cudaSetDevice(p->device);
     delete p;
+  });
+}
+
+// The HiPDLP mode on several devices of this process: the host prologue once, then one problem per rank (its blocks of
+// the one-GPU device orders, build_hipdlp_shard), wired by peer pointers, one host thread per rank, no NCCL.
+int b200pdlp_solve_hipdlp_multi(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params* params, b200pdlp_result* out,
+                                int32_t ngpus, const int32_t* devices) {
+  if (ngpus <= 1) return b200pdlp_solve_hipdlp(lp, params, out);
+  DeviceGuard dg;
+  std::vector<b200pdlp_problem*> probs;
+  const int rc = guarded([&] {
+    check_lp(lp);
+    if (!params || !out || ngpus > kMaxPeers) throw Error(B200PDLP_ERR_ARG, "b200pdlp_solve_hipdlp_multi: bad arguments");
+    int ndev = 0;
+    const cudaError_t e = cudaGetDeviceCount(&ndev);
+    if (e != cudaSuccess || ndev == 0)
+      throw Error(B200PDLP_ERR_CUDA, std::string("no CUDA device: the engine has no CPU fallback (") + cudaGetErrorString(e) + ")");
+    std::vector<int> dev(ngpus);
+    for (int g = 0; g < ngpus; g++) {
+      dev[g] = devices ? devices[g] : g;
+      if (dev[g] < 0 || dev[g] >= ndev) throw Error(B200PDLP_ERR_ARG, "b200pdlp_solve_hipdlp_multi: no such device");
+    }
+    for (int a : dev)   // every rank stores into every other rank's memory
+      for (int b : dev)
+        if (a != b) {
+          int ok = 0;
+          CUDA_OK(cudaDeviceCanAccessPeer(&ok, a, b));
+          if (!ok) throw Error(B200PDLP_ERR_ARG, "b200pdlp_solve_hipdlp_multi: devices cannot access each other");
+        }
+    const auto t0 = std::chrono::steady_clock::now();
+    StdForm f;
+    formulate_hipdlp(*lp, f);
+    scale_hipdlp(f, params->scaling_mode, params->ruiz_iterations);
+    HipShards S;
+    plan_hipdlp_shards(f, ngpus, params->ordered_max, S);
+    probs.assign(ngpus, nullptr);
+    for (int g = 0; g < ngpus; g++) {
+      probs[g] = new b200pdlp_problem();
+      create_problem_hipdlp_shard(f, S, g, dev[g], probs[g]);
+    }
+    probs[0]->form = std::move(f);
+    auto group = std::make_shared<LocalGroup>();
+    group->world = ngpus;
+    for (b200pdlp_problem* p : probs) {
+      set_device(p);
+      preload_hipdlp_shard_kernels();
+      for (b200pdlp_problem* q : probs)
+        if (q->device != p->device) {
+          const cudaError_t pe = cudaDeviceEnablePeerAccess(q->device, 0);
+          if (pe != cudaSuccess && pe != cudaErrorPeerAccessAlreadyEnabled) CUDA_OK(pe);
+          cudaGetLastError();
+        }
+      p->hip_peers = probs;
+      p->group = group;
+      p->local_link = true;
+    }
+    const double setup = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    // rank 0 writes the caller's arrays; the other ranks' results carry no vectors
+    std::vector<b200pdlp_result> res((size_t)ngpus, *out);
+    std::vector<int> codes((size_t)ngpus, B200PDLP_OK);
+    std::vector<std::string> msgs((size_t)ngpus);
+    for (int g = 0; g < ngpus; g++) {
+      res[g].setup_seconds = 0.0;
+      if (g > 0) { res[g].col_value = res[g].col_dual = res[g].row_value = res[g].row_dual = nullptr; res[g].trace = nullptr; res[g].trace_cap = 0; }
+    }
+    std::vector<std::thread> th;
+    for (int g = 0; g < ngpus; g++)
+      th.emplace_back([&, g] {
+        codes[g] = guarded([&] { solve_hipdlp_on_device(probs[g], *lp, *params, &res[g]); CUDA_OK(cudaGetLastError()); });
+        if (codes[g] != B200PDLP_OK) msgs[g] = g_last_error;   // thread-local: hand it to the caller's thread
+      });
+    for (auto& t : th) t.join();
+    for (int g = 0; g < ngpus; g++)
+      if (codes[g] != B200PDLP_OK) throw Error(codes[g], "rank " + std::to_string(g) + ": " + msgs[g]);
+    *out = res[0];
+    out->setup_seconds += setup;
+  });
+  for (b200pdlp_problem* p : probs)
+    if (p) { cudaSetDevice(p->device); delete p; }
+  return rc;
+}
+
+int b200pdlp_hipdlp_shard_layout_eval(b200pdlp_form* fh, int32_t rank, int32_t world, int32_t ordered_max, const double* x,
+                                      const double* y, double* ax, double* aty, double stats[7]) {
+  return guarded([&] {
+    if (!fh || !x || !y || !ax || !aty || !stats) throw Error(B200PDLP_ERR_ARG, "null argument");
+    if (world < 1 || world > kMaxPeers || rank < 0 || rank >= world) throw Error(B200PDLP_ERR_ARG, "bad rank/world");
+    StdForm& f = fh->f;
+    if (!f.hipdlp) throw Error(B200PDLP_ERR_ARG, "b200pdlp_hipdlp_shard_layout_eval needs a HiPDLP form");
+    HipShards S;
+    plan_hipdlp_shards(f, world, ordered_max, S);
+    SellMatrix A, AT;
+    build_hipdlp_shard(S, rank, A, AT);
+    const int n = f.n, m = f.m;
+    const int r0 = S.rb[rank], r1 = S.rb[rank + 1], c0 = S.cb[rank], c1 = S.cb[rank + 1];
+    std::vector<double> xin((size_t)std::max(n, 1), 0.0), yin((size_t)std::max(m, 1), 0.0);
+    std::vector<double> rows((size_t)std::max(r1 - r0, 1)), cols((size_t)std::max(c1 - c0, 1));
+    for (int j = 0; j < n; j++) xin[j] = x[S.cperm[j]];
+    for (int i = 0; i < m; i++) yin[i] = y[S.rperm[i]];
+    sell_apply_host(A, xin.data(), rows.data());
+    sell_apply_host(AT, yin.data(), cols.data());
+    for (int i = r0; i < r1; i++) ax[S.rperm[i]] = rows[i - r0];
+    for (int j = c0; j < c1; j++) aty[S.cperm[j]] = cols[j - c0];
+    stats[0] = r0; stats[1] = r1; stats[2] = c0; stats[3] = c1; stats[4] = S.ordered ? 1 : 0;
+    stats[5] = (double)A.long_rows.size(); stats[6] = (double)AT.long_rows.size();
   });
 }
 

@@ -10,6 +10,7 @@
 // drop-in (libhighs_b200.so).
 #include <algorithm>
 #include <cmath>
+#include <cstdlib>
 
 #include "lp_data/HighsLpSolverObject.h"
 #include "lp_data/HighsSolution.h"
@@ -58,7 +59,11 @@ HighsStatus solveLpHiPdlp(const HighsOptions& options, HighsTimer& timer, const 
   res.col_dual = highs_solution.col_dual.data();
   res.row_value = highs_solution.row_value.data();
   res.row_dual = highs_solution.row_dual.data();
-  const int rc = b200pdlp_solve_hipdlp(&clp, &prm, &res);
+  // B200PDLP_GPUS=N: N devices of this process (blocks of the device rows and columns, peer memory; the same bits as one GPU
+  // with the host prologue)
+  int ngpus = 1;
+  if (const char* e = getenv("B200PDLP_GPUS")) ngpus = std::max(1, std::min(atoi(e), b200pdlp_device_count()));
+  const int rc = ngpus > 1 ? b200pdlp_solve_hipdlp_multi(&clp, &prm, &res, ngpus, nullptr) : b200pdlp_solve_hipdlp(&clp, &prm, &res);
   model_status = HighsModelStatus::kUnknown;
   highs_basis.valid = false;
   if (rc != B200PDLP_OK) {

@@ -710,6 +710,48 @@ void build_layout(StdForm& f, int rank, int world, int ordered_max, HostLayout& 
   mark("sliced-ELL build");
 }
 
+// offsets of `world` contiguous blocks of perm[0..count) balancing entries + a per-row cost (as partition_rows does)
+static std::vector<int> balanced_blocks(const std::vector<int>& ptr, const std::vector<int>& perm, int world) {
+  const int count = (int)perm.size();
+  std::vector<long long> pre(count + 1, 0);
+  for (int i = 0; i < count; i++) pre[i + 1] = pre[i] + (ptr[perm[i] + 1] - ptr[perm[i]]) + 5;
+  std::vector<int> b(world + 1, 0);
+  b[world] = count;
+  for (int g = 1; g < world; g++) {
+    const long long target = pre[count] * g / world;
+    b[g] = (int)(std::lower_bound(pre.begin() + b[g - 1], pre.end(), target) - pre.begin());
+    b[g] = std::min(b[g], count);
+  }
+  return b;
+}
+
+void plan_hipdlp_shards(StdForm& f, int world, int ordered_max, HipShards& S) {
+  S = HipShards();
+  S.world = world;
+  HostLayout L;   // the one-GPU orders (the plan-only build computes exactly the full build's orderings)
+  build_layout(f, 0, 1, ordered_max, L, nullptr, /*plan_only=*/true);
+  S.ordered = L.ordered;
+  S.long_threshold = L.ordered ? std::numeric_limits<int>::max() : 512;
+  S.rperm = std::move(L.rperm); S.rinv = std::move(L.rinv);
+  S.cperm = std::move(L.cperm); S.cinv = std::move(L.cinv);
+  build_row_major(f, 0, f.m, S.a);
+  build_col_major(f, 0, f.m, S.at);
+  S.rb = balanced_blocks(S.a.rowptr, S.rperm, world);
+  S.cb = balanced_blocks(S.at.rowptr, S.cperm, world);
+}
+
+void build_hipdlp_shard(const HipShards& S, int rank, SellMatrix& A, SellMatrix& AT) {
+  auto build = [&](const Csr& a, const std::vector<int>& order, int b0, int b1, const std::vector<int>& colmap, SellMatrix& out) {
+    const std::vector<int> perm(order.begin() + b0, order.begin() + b1);
+    long long nnz = 0;
+    for (int r : perm) nnz += a.rowptr[r + 1] - a.rowptr[r];
+    plan_sell(b1 - b0, a.ncols, nnz, perm, [&](int r) { return a.rowptr[r + 1] - a.rowptr[r]; }, S.long_threshold, out);
+    fill_sell_host(a, perm, colmap, out);
+  };
+  build(S.a, S.rperm, S.rb[rank], S.rb[rank + 1], S.cinv, A);
+  build(S.at, S.cperm, S.cb[rank], S.cb[rank + 1], S.rinv, AT);
+}
+
 void sell_apply_host(const SellMatrix& a, const double* xin, double* out) {
   // exactly what spmv_sell_kernel does: EVERY lane of a slice runs over the slice's full length (padding included),
   // so padding must be (col 0, val 0) and every column id must be a valid position of the input vector

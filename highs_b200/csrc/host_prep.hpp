@@ -169,6 +169,22 @@ struct HostLayout {
 // arrays are then filled on the device from the scaled matrix resident there
 void build_layout(StdForm& f, int rank, int world, int ordered_max, HostLayout& L,
                   const std::function<void(const char*)>& lap = nullptr, bool plan_only = false);
+// HiPDLP on several GPUs: the ONE-GPU device orders (build_layout(f, 0, 1, ...): rperm / cperm, ordered or tree mode
+// decided on the whole problem) cut into `world` contiguous, nnz-balanced blocks.  Rank g computes whole rows: device
+// rows [rb[g], rb[g+1]) of A and device columns [cb[g], cb[g+1]) of A (rows of A'), each in the one-GPU entry order, so
+// every value it produces has the one-GPU bits.  A rank may own no rows or no columns.
+struct HipShards {
+  int world = 1;
+  bool ordered = false;
+  int long_threshold = 512;
+  Csr a, at;                                  // the whole matrix, row-major and column-major (standard-form order)
+  std::vector<int> rperm, rinv, cperm, cinv;  // the one-GPU device orders
+  std::vector<int> rb, cb;                    // world + 1 block offsets in device row / column order
+};
+void plan_hipdlp_shards(StdForm& f, int world, int ordered_max, HipShards& S);
+// rank g's matrices: A_g (rows = device rows [rb[g], rb[g+1]); column ids = device column positions 0..n-1) and
+// A_g' (rows = device columns [cb[g], cb[g+1]); column ids = device row positions 0..m-1)
+void build_hipdlp_shard(const HipShards& S, int rank, SellMatrix& A, SellMatrix& AT);
 // host evaluation of a sliced-ELL matrix exactly as the kernels traverse it (body: lane = row, k ascending;
 // long rows: per-segment partial sums, added in segment order): out[row] for row < nrows
 void sell_apply_host(const SellMatrix& a, const double* xin, double* out);

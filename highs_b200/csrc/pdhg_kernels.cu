@@ -2381,26 +2381,34 @@ namespace b200 {
 __device__ __forceinline__ double std_max(double a, double b) { return a < b ? b : a; }   // std::max / std::min semantics
 __device__ __forceinline__ double std_min(double a, double b) { return b < a ? b : a; }
 
-// x-side of performHalpernPdhgStep (:974-986, :1006-1009)
+// x-side of performHalpernPdhgStep (:974-986, :1006-1009) for column i; returns the reflected x
+__device__ __forceinline__ double hip_primal_col(int i, double ps, double w, int is_major, double* __restrict__ x,
+                                                 const double* __restrict__ xa, const double* __restrict__ c,
+                                                 const double* __restrict__ aty, const double* __restrict__ lo,
+                                                 const double* __restrict__ up, double* __restrict__ rx,
+                                                 double* __restrict__ xn, double* __restrict__ hslack) {
+  const double rho = 1.0;
+  const double xc = x[i];
+  const double temp = xc - ps * (c[i] - aty[i]);
+  const double proj = std_max(lo[i], std_min(temp, up[i]));
+  if (is_major) { xn[i] = proj; hslack[i] = (proj - temp) / ps; }
+  const double r = 2.0 * proj - xc;
+  rx[i] = r;
+  const double blended = rho * r + (1.0 - rho) * xc;
+  x[i] = w * blended + (1.0 - w) * xa[i];
+  return r;
+}
 __global__ void __launch_bounds__(kThreads)
 hip_primal_kernel(int n, const HipState* __restrict__ st, int k_offset, int is_major, double* __restrict__ x,
                   const double* __restrict__ xa, const double* __restrict__ c, const double* __restrict__ aty,
                   const double* __restrict__ lo, const double* __restrict__ up, double* __restrict__ rx,
                   double* __restrict__ xn, double* __restrict__ hslack) {
-  const double ps = st->primal_step, rho = 1.0;
+  const double ps = st->primal_step;
   const int k = st->halpern_iteration + k_offset;
   const double w = (double)k / (k + 1.0);
   const int stride = gridDim.x * kThreads;
-  for (int i = blockIdx.x * kThreads + threadIdx.x; i < n; i += stride) {
-    const double xc = x[i];
-    const double temp = xc - ps * (c[i] - aty[i]);
-    const double proj = std_max(lo[i], std_min(temp, up[i]));
-    if (is_major) { xn[i] = proj; hslack[i] = (proj - temp) / ps; }
-    const double r = 2.0 * proj - xc;
-    rx[i] = r;
-    const double blended = rho * r + (1.0 - rho) * xc;
-    x[i] = w * blended + (1.0 - w) * xa[i];
-  }
+  for (int i = blockIdx.x * kThreads + threadIdx.x; i < n; i += stride)
+    hip_primal_col(i, ps, w, is_major, x, xa, c, aty, lo, up, rx, xn, hslack);
 }
 
 // y-side (:992-1003, :1010-1013) as the epilogue of ax = A * reflected x
@@ -2422,7 +2430,8 @@ struct HipDualEpilogue {
   __device__ const double* input() const { return in; }
   double p_y, p_ya, p_lo, p_up;
   __device__ void prefetch(int r) { p_y = y[r]; p_ya = ya[r]; p_lo = rlo[r]; p_up = rup[r]; }
-  __device__ void row(int r, double s, double*) const {
+  // the blended y of row r, given s = (A * reflected x)[r]
+  __device__ double blend(int r, double s) const {
     const double rho = 1.0;
     const double temp = p_y / ds - s;
     const double proj = std_max(-p_up, std_min(temp, -p_lo));
@@ -2430,8 +2439,9 @@ struct HipDualEpilogue {
     const double refl = 2.0 * pd - p_y;
     if (is_major) { yn[r] = pd; ry[r] = refl; }
     const double blended = rho * refl + (1.0 - rho) * p_y;
-    y[r] = w * blended + (1.0 - w) * p_ya;
+    return w * blended + (1.0 - w) * p_ya;
   }
+  __device__ void row(int r, double s, double*) const { y[r] = blend(r, s); }
 };
 
 void launch_hip_primal(cudaStream_t s, int n, const HipState* st, int k_offset, int is_major, double* x, const double* xa,
@@ -2607,5 +2617,118 @@ void launch_hip_dot(cudaStream_t s, int len, const double* a, const double* b, i
 }
 void launch_hip_div_norm(cudaStream_t s, int len, double* v, const double* norm_sq) {
   if (len > 0) hip_div_norm_kernel<<<ew_grid(len), kThreads, 0, s>>>(len, v, norm_sq);
+}
+}  // namespace b200
+
+// ---- HiPDLP shards: the Halpern step on several GPUs (engine.cu, "HiPDLP on several GPUs").  Rank g owns device columns
+// [c0, c1) and device rows [r0, r1); every vector is held full length in the one-GPU device order.  The step's two
+// exchanged vectors are stored straight into the peers' copies: the reflected x by the primal kernel, the blended y by the
+// dual epilogue.  The flag barrier carries no data: a Halpern step has no reduction, so nothing but arrival is exchanged.
+namespace b200 {
+
+__global__ void __launch_bounds__(kThreads)
+hip_primal_shard_kernel(int c0, int c1, const HipState* __restrict__ st, int k_offset, int is_major, double* __restrict__ x,
+                        const double* __restrict__ xa, const double* __restrict__ c, const double* __restrict__ aty,
+                        const double* __restrict__ lo, const double* __restrict__ up, double* __restrict__ rx,
+                        double* __restrict__ xn, double* __restrict__ hslack, PeerVec rx_peers, int world, int rank) {
+  const double ps = st->primal_step;
+  const int k = st->halpern_iteration + k_offset;
+  const double w = (double)k / (k + 1.0);
+  const int stride = gridDim.x * kThreads;
+  for (int i = c0 + blockIdx.x * kThreads + threadIdx.x; i < c1; i += stride) {
+    const double r = hip_primal_col(i, ps, w, is_major, x, xa, c, aty, lo, up, rx, xn, hslack);
+#pragma unroll
+    for (int h = 0; h < kMaxPeers; h++)   // (constant indices: the peer table stays in parameter space)
+      if (h < world && h != rank) rx_peers.v[h][i] = r;
+  }
+}
+
+// HipDualEpilogue over rank g's rows (the pointers are offset to the rank's first row) + the blended y into every peer
+struct HipDualShardEpilogue : HipDualEpilogue {
+  PeerVec y_peers;
+  int world, rank;
+  __device__ void row(int r, double s, double*) const {
+    const double v = blend(r, s);
+    y[r] = v;
+#pragma unroll
+    for (int h = 0; h < kMaxPeers; h++)
+      if (h < world && h != rank) y_peers.v[h][r] = v;
+  }
+};
+
+__global__ void __launch_bounds__(kThreads) hip_gather_kernel(HipGather g, int world, int rank) {
+  const int stride = gridDim.x * kThreads;
+  for (int q = 0; q < g.nv; q++)
+    for (int i = g.lo + blockIdx.x * kThreads + threadIdx.x; i < g.hi; i += stride) {
+      const double v = g.src[q][i];
+#pragma unroll
+      for (int h = 0; h < kMaxPeers; h++)
+        if (h < world && h != rank) g.dst[q].v[h][i] = v;
+    }
+}
+
+// Flag barrier: lane h stores the new epoch into peer h's arrival word for this rank (release, system scope: it publishes
+// every store this rank made into peer h's memory before it, by this or an earlier kernel of the stream) and waits for
+// peer h's word here (acquire).  Epochs only grow and no rank can pass barrier e + 1 before every rank has arrived at
+// it, so a word is never more than one epoch ahead: "seen >= e" needs no double buffering.  The wait is bounded like
+// p2p_barrier_kernel's: a peer that never arrives raises the fault word, and later barriers return at once.
+__global__ void hip_barrier_kernel(PeerFlags pf, int world, int rank, unsigned long long* epoch, int* fault) {
+  if (*reinterpret_cast<volatile int*>(fault)) return;
+  const int lane = threadIdx.x;
+  unsigned long long e = 0;
+  if (lane == 0) { e = *epoch + 1; *epoch = e; }
+  e = __shfl_sync(0xffffffffu, e, 0);
+  __threadfence_system();
+  if (lane < world) {
+    unsigned long long* theirs = pf.f[lane] + rank;
+    const unsigned long long* mine = pf.f[rank] + lane;
+    asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(theirs), "l"(e) : "memory");
+    long long spins = 0;
+    const unsigned long long t0 = global_ns();
+    unsigned long long seen = 0;
+    do {
+      asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(seen) : "l"(mine) : "memory");
+      if (seen < e && barrier_expired(spins, t0)) { *fault = 1; break; }
+    } while (seen < e);
+  }
+}
+
+void launch_hip_primal_shard(cudaStream_t s, int c0, int c1, const HipState* st, int k_offset, int is_major, double* x,
+                             const double* xa, const double* c, const double* aty, const double* lo, const double* up,
+                             double* rx, double* xn, double* hslack, const PeerVec& rx_peers, int world, int rank) {
+  if (c1 <= c0) return;
+  hip_primal_shard_kernel<<<ew_grid(c1 - c0), kThreads, 0, s>>>(c0, c1, st, k_offset, is_major, x, xa, c, aty, lo, up, rx,
+                                                                 xn, hslack, rx_peers, world, rank);
+}
+// one slice per warp only: the shape the sharded solve uses (the tiled and persistent shapes stay one-GPU)
+void launch_hip_dual_shard(cudaStream_t s, const DevSell& A, const HipState* st, int k_offset, int is_major, const double* rx,
+                           double* y, const double* ya, const double* rlo, const double* rup, double* yn, double* ry,
+                           const PeerVec& y_peers, int world, int rank) {
+  if (A.nblocks_body + A.nsegs == 0) return;
+  HipDualShardEpilogue e{};
+  e.st = st; e.k_offset = k_offset; e.is_major = is_major; e.in = rx; e.y = y; e.ya = ya; e.rlo = rlo; e.rup = rup;
+  e.yn = yn; e.ry = ry; e.y_peers = y_peers; e.world = world; e.rank = rank;
+  const ReduceScratch none{nullptr, nullptr, nullptr, 0, 0};
+  spmv_sell_kernel<HipDualShardEpilogue, false><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, none);
+}
+void launch_hip_gather(cudaStream_t s, const HipGather& g, int world, int rank) {
+  if (g.hi <= g.lo || g.nv == 0) return;
+  hip_gather_kernel<<<ew_grid(g.hi - g.lo), kThreads, 0, s>>>(g, world, rank);
+}
+void launch_hip_barrier(cudaStream_t s, const PeerFlags& flags, int world, int rank, unsigned long long* epoch, int* fault) {
+  hip_barrier_kernel<<<1, 32, 0, s>>>(flags, world, rank, epoch, fault);
+}
+
+// every kernel a sharded HiPDLP solve launches, loaded before the first barrier can spin (see preload_multi_gpu_kernels)
+void preload_hipdlp_shard_kernels() {
+  const void* fns[] = {
+      (const void*)hip_primal_shard_kernel, (const void*)spmv_sell_kernel<HipDualShardEpilogue, false>,
+      (const void*)hip_gather_kernel, (const void*)hip_barrier_kernel, (const void*)spmv_sell_kernel<PlainEpilogue, false>,
+      (const void*)hip_diff_kernel, (const void*)hip_slack_kernel, (const void*)hip_check_ordered_kernel,
+      (const void*)hip_check_tree_kernel, (const void*)hip_dot_ordered_kernel, (const void*)hip_dot_tree_kernel,
+      (const void*)hip_div_norm_kernel, (const void*)fill_kernel,
+  };
+  cudaFuncAttributes at;
+  for (const void* f : fns) cudaFuncGetAttributes(&at, f);
 }
 }  // namespace b200

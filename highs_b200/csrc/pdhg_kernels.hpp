@@ -139,4 +139,24 @@ void launch_hip_check(cudaStream_t s, const HipCheckArgs& a, int with_fpe, int o
 void launch_hip_dot(cudaStream_t s, int len, const double* a, const double* b, int ordered, ReduceScratch rs, double* out);
 void launch_hip_div_norm(cudaStream_t s, int len, double* v, const double* norm_sq);
 
+// ---- HiPDLP on several GPUs (pdhg_kernels.cu, "HiPDLP shards"): every rank holds full-length vectors in the one-GPU
+// device order; peers' copies of one vector, by rank (this rank's own entry included)
+struct PeerVec { double* v[kMaxPeers]; };
+struct PeerFlags { unsigned long long* f[kMaxPeers]; };   // every rank's kMaxPeers arrival words
+constexpr int kMaxGather = 4;
+struct HipGather {   // entries [lo, hi) of up to kMaxGather vectors, copied from this rank into every peer
+  const double* src[kMaxGather];
+  PeerVec dst[kMaxGather];
+  int nv, lo, hi;
+};
+void launch_hip_primal_shard(cudaStream_t s, int c0, int c1, const HipState* st, int k_offset, int is_major, double* x,
+                             const double* xa, const double* c, const double* aty, const double* lo, const double* up,
+                             double* rx, double* xn, double* hslack, const PeerVec& rx_peers, int world, int rank);
+void launch_hip_dual_shard(cudaStream_t s, const DevSell& A, const HipState* st, int k_offset, int is_major, const double* rx,
+                           double* y, const double* ya, const double* rlo, const double* rup, double* yn, double* ry,
+                           const PeerVec& y_peers, int world, int rank);
+void launch_hip_gather(cudaStream_t s, const HipGather& g, int world, int rank);
+void launch_hip_barrier(cudaStream_t s, const PeerFlags& flags, int world, int rank, unsigned long long* epoch, int* fault);
+void preload_hipdlp_shard_kernels();
+
 }  // namespace b200

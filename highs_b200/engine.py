@@ -74,7 +74,8 @@ ABI_SYMBOLS = [
     "b200pdlp_form_get_vector", "b200pdlp_form_get_csc", "b200pdlp_form_get_csr", "b200pdlp_form_get_row_map",
     "b200pdlp_form_layout_eval", "b200pdlp_p2p_link_local", "b200pdlp_solve_multi",
     "b200pdlp_hipdlp_form_create", "b200pdlp_hipdlp_power_method", "b200pdlp_hipdlp_default_params",
-    "b200pdlp_solve_hipdlp", "b200pdlp_hipdlp_controller_replay", "b200pdlp_debug_prep_compare",
+    "b200pdlp_solve_hipdlp", "b200pdlp_solve_hipdlp_multi", "b200pdlp_hipdlp_shard_layout_eval",
+    "b200pdlp_hipdlp_controller_replay", "b200pdlp_debug_prep_compare",
     "b200pdlp_debug_prep_compare_hipdlp", "b200pdlp_release_cache",
     "b200pdlp_host_register", "b200pdlp_host_unregister", "b200pdlp_primal_step", "b200pdlp_dual_step", "b200pdlp_residuals",
     "b200pdlp_kkt_check", "b200pdlp_kkt_check_host", "b200pdlp_kkt_default_tolerances",
@@ -326,24 +327,84 @@ def hipdlp_controller_replay(norm_cost, norm_rhs, op_norm_sq, tolerance, strateg
     return out[:nb]
 
 
-def solve_hipdlp(lp: HighsLp, **params) -> dict:
-    """b200pdlp_solve_hipdlp: the HiPDLP mode (reflected Halpern PDHG, solver=hipdlp) on one GPU; parameters are the
-    HighsOptions of the same meaning (tolerance, iter_limit, scaling_mode, ruiz_iterations, step_size_strategy ...), and
-    device_prep=-1 for the host prologue instead of the device-resident one."""
+def _hipdlp_params(params) -> CHipdlpParams:
     L = lib()
     L.b200pdlp_hipdlp_default_params.argtypes = [C.POINTER(CHipdlpParams)]
     L.b200pdlp_hipdlp_default_params.restype = None
-    L.b200pdlp_solve_hipdlp.argtypes = [C.POINTER(CLp), C.POINTER(CHipdlpParams), C.POINTER(CResult)]
-    clp, keep = make_clp(lp)
     prm = CHipdlpParams()
     L.b200pdlp_hipdlp_default_params(C.byref(prm))
     for k, v in params.items():
         if not hasattr(prm, k):
             raise TypeError(f"unknown parameter {k}")
         setattr(prm, k, v)
+    return prm
+
+
+def solve_hipdlp(lp: HighsLp, **params) -> dict:
+    """b200pdlp_solve_hipdlp: the HiPDLP mode (reflected Halpern PDHG, solver=hipdlp) on one GPU; parameters are the
+    HighsOptions of the same meaning (tolerance, iter_limit, scaling_mode, ruiz_iterations, step_size_strategy ...), and
+    device_prep=-1 for the host prologue instead of the device-resident one."""
+    L = lib()
+    L.b200pdlp_solve_hipdlp.argtypes = [C.POINTER(CLp), C.POINTER(CHipdlpParams), C.POINTER(CResult)]
+    clp, keep = make_clp(lp)
+    prm = _hipdlp_params(params)
     res, arrays = _mk_result(lp, 0)
     _check(L.b200pdlp_solve_hipdlp(C.byref(clp), C.byref(prm), C.byref(res)), "b200pdlp_solve_hipdlp")
     return _result_dict(res, arrays)
+
+
+def solve_hipdlp_multi(lp: HighsLp, ngpus: int, devices=None, out_arrays=None, **params) -> dict:
+    """b200pdlp_solve_hipdlp_multi: the HiPDLP mode on `ngpus` ranks of this process (devices may repeat: logical shards
+    on one device); the same bits as solve_hipdlp(lp, device_prep=-1, **params).
+    out_arrays = (col_value, col_dual, row_value, row_dual): caller-owned (e.g. page-locked) result storage."""
+    L = lib()
+    L.b200pdlp_solve_hipdlp_multi.argtypes = [C.POINTER(CLp), C.POINTER(CHipdlpParams), C.POINTER(CResult), C.c_int32, _ip]
+    clp, keep = make_clp(lp)
+    prm = _hipdlp_params(params)
+    res, arrays = _mk_result(lp, 0)
+    if out_arrays is not None:
+        arrays = tuple(out_arrays)
+        res.col_value, res.col_dual, res.row_value, res.row_dual = (_p(a, _dp) for a in arrays)
+    dev = None if devices is None else np.ascontiguousarray(devices, dtype=np.int32)
+    _check(L.b200pdlp_solve_hipdlp_multi(C.byref(clp), C.byref(prm), C.byref(res), ngpus,
+                                         _p(dev, _ip) if dev is not None else None), "b200pdlp_solve_hipdlp_multi")
+    return _result_dict(res, arrays)
+
+
+def hipdlp_shard_layout_eval(lp: HighsLp, world: int, ordered_max: int = 0, x=None, y=None, scaling_mode: int = 5,
+                             ruiz_iterations: int = 10, seed: int = 0) -> dict:
+    """Host-only: every rank's A_g and A_g' of solve_hipdlp_multi evaluated on the host (b200pdlp_hipdlp_shard_layout_eval).
+    Returns x, y, the per-rank ax / aty (NaN outside the rank's rows / columns, standard-form order), stats, and the
+    one-GPU layout's A x and A'y of the same form (b200pdlp_form_layout_eval, world = 1) as ref_ax / ref_aty."""
+    L = lib()
+    L.b200pdlp_hipdlp_form_create.argtypes = [C.POINTER(CLp), C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
+    L.b200pdlp_hipdlp_shard_layout_eval.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, _dp, _dp, _dp, _dp, _dp]
+    clp, keep = make_clp(lp)
+    h = C.c_void_p()
+    _check(L.b200pdlp_hipdlp_form_create(C.byref(clp), scaling_mode, ruiz_iterations, C.byref(h)), "b200pdlp_hipdlp_form_create")
+    try:
+        d = (C.c_int32 * 5)()
+        sc = (C.c_double * 3)()
+        _check(L.b200pdlp_form_dims(h, d, sc), "b200pdlp_form_dims")
+        n, m = d[0], d[1]
+        rng = np.random.default_rng(seed)
+        x = rng.standard_normal(max(n, 1)) if x is None else np.ascontiguousarray(x, dtype=np.float64)
+        y = rng.standard_normal(max(m, 1)) if y is None else np.ascontiguousarray(y, dtype=np.float64)
+        ax, aty, stats = [], [], []
+        for g in range(world):
+            a, b, st = np.full(max(m, 1), np.nan), np.full(max(n, 1), np.nan), np.zeros(7)
+            _check(L.b200pdlp_hipdlp_shard_layout_eval(h, g, world, ordered_max, _p(x, _dp), _p(y, _dp), _p(a, _dp), _p(b, _dp),
+                                                       _p(st, _dp)), "b200pdlp_hipdlp_shard_layout_eval")
+            ax.append(a[:m])
+            aty.append(b[:n])
+            stats.append(st)
+        ref_ax, ref_aty, st = np.full(max(m, 1), np.nan), np.full(max(n, 1), np.nan), np.zeros(12)
+        _check(L.b200pdlp_form_layout_eval(h, 0, 1, ordered_max, _p(x, _dp), _p(y, _dp), _p(ref_ax, _dp), _p(ref_aty, _dp),
+                                           _p(st, _dp)), "b200pdlp_form_layout_eval")
+        return dict(n=n, m=m, x=x[:n], y=y[:m], ax=ax, aty=aty, stats=stats, ref_ax=ref_ax[:m], ref_aty=ref_aty[:n],
+                    ref_ordered=bool(st[2]))
+    finally:
+        L.b200pdlp_form_destroy(h)
 
 
 def solve_multi(lp: HighsLp, ngpus: int, devices=None, warm=None, **params) -> dict:

@@ -252,6 +252,16 @@ typedef struct {
 } b200pdlp_hipdlp_params;
 void b200pdlp_hipdlp_default_params(b200pdlp_hipdlp_params* p);
 int b200pdlp_solve_hipdlp(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params* params, b200pdlp_result* out);
+/* The HiPDLP solve on `ngpus` devices of THIS process (devices[g] or, if NULL, ordinals 0..ngpus-1; a device may repeat,
+ * which gives logical shards on one device): the host prologue once, then each rank computes contiguous blocks of the
+ * one-GPU device rows and columns, one host thread per rank, peer memory, no NCCL.  Returns the same bits as
+ * b200pdlp_solve_hipdlp with device_prep = -1 (iterations, termination and all four vectors), for every ngpus.
+ * ngpus <= 1 is b200pdlp_solve_hipdlp; ngpus > 16 or devices without peer access: B200PDLP_ERR_ARG; device_prep and
+ * device are ignored.  What the HiGHS shim uses for solver=hipdlp when B200PDLP_GPUS > 1.
+ * STATUS: runs on hardware as logical shards on one H100 (tests/test_gpu_hipdlp_shards.py, byte equality with one GPU);
+ * not yet run on two physical GPUs. */
+int b200pdlp_solve_hipdlp_multi(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params* params, b200pdlp_result* out,
+                                int32_t ngpus, const int32_t* devices);
 
 /* host-only (no GPU; parity tests): the HOST control of the HiPDLP loop -- step sizes, fixed-point error, convergence test,
  * restart criteria, PID primal weight (HipController, host_prep_hipdlp.cpp; hipdlp/pdhg.cc:494-707,901-927,1944-2050) --
@@ -272,6 +282,15 @@ int b200pdlp_hipdlp_power_method(const b200pdlp_form* f, double* lambda);
  *        [7] A' long rows [8] A' segments [9] shard_len [10] seg_len [11] layout build time, ms */
 int b200pdlp_form_layout_eval(b200pdlp_form* f, int32_t rank, int32_t world, int32_t ordered_max, const double* x,
                               const double* y, double* ax, double* aty, double stats[12]);
+
+/* host-only (no GPU): rank `rank` of `world` of b200pdlp_solve_hipdlp_multi -- its block of the one-GPU device rows and
+ * of the one-GPU device columns, A_g and A_g' built as the solve builds them -- evaluated on the host in the kernels'
+ * traversal order.  f from b200pdlp_hipdlp_form_create.  x[n], y[m] full, in standard-form order; ax[m] receives the
+ * rank's rows of A x, aty[n] the rank's columns of A'y, both in standard-form order (other entries untouched).
+ * stats: [0] R_g [1] R_g+1 (device rows) [2] C_g [3] C_g+1 (device columns) [4] ordered mode [5] A_g long rows
+ *        [6] A_g' long rows */
+int b200pdlp_hipdlp_shard_layout_eval(b200pdlp_form* f, int32_t rank, int32_t world, int32_t ordered_max, const double* x,
+                                      const double* y, double* ax, double* aty, double stats[7]);
 
 /* host-only helper (no GPU): nnz-balanced contiguous row partition of the
  * formulated LP; bounds[world+1] receives the row offsets (SURVEY.md 8(e)) */
