@@ -831,7 +831,7 @@ void DevicePrologue::run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, i
     DevForm F{n, m, nnz, cbeg, cidx, colof, cval, cost, lower, upper, colscale, rhs, rowscale};
     DevScaleScratch w{cs, cnorm, rs, rnorm, amax};
     if (do_scale && nnz > 0) {
-      device_scale_ruiz(s, F, w, /*have_colof=*/true);
+      device_scale_ruiz(s, F, w);
       device_scale_pock_chambolle(s, F, w, rptr, rpos);
     } else if (nnz > 0) {
       device_abs_max(s, nnz, cval, amax);

@@ -29,7 +29,6 @@
 #include "device_prep.hpp"
 #include "host_prep.hpp"
 #include "pdhg_kernels.hpp"
-#include "setup_kernels.hpp"
 
 namespace b200 {
 
@@ -132,26 +131,11 @@ struct DeviceMatrix {
   DevBuf<int> tile_lo, tile_w;   // tiled shape (DevSell::tiled): windows of the input vector per tile of kTileSlices slices
   int ntiles = 0, tiles_staged = 0;
   DevSell dev{};
-  // descriptors only; col/val/lcol/lval are allocated (lcol/lval zeroed) for a device-side fill
-  // (the long-row arrays are cleared on the stream the fill kernels run on: a cudaMemset on the legacy stream is not
-  //  ordered against a non-blocking stream)
-  void upload_plan(cudaStream_t s) {
-    col.alloc((size_t)host.padded + 32, false);
-    val.alloc((size_t)host.padded + 32, false);
-    lcol.alloc((size_t)host.lcount, false);
-    lval.alloc((size_t)host.lcount, false);
-    CUDA_OK(cudaMemsetAsync(lcol.p, 0, std::max<size_t>((size_t)host.lcount, 1) * sizeof(int), s));
-    CUDA_OK(cudaMemsetAsync(lval.p, 0, std::max<size_t>((size_t)host.lcount, 1) * sizeof(double), s));
-    finish_upload();
-  }
   void upload() {
     col.from(host.col);
     val.from(host.val);
     lcol.from(host.lcol);
     lval.from(host.lval);
-    finish_upload();
-  }
-  void finish_upload() {
     static_assert(sizeof(SellMatrix::Slice) == sizeof(int4) && sizeof(SellMatrix::Seg) == sizeof(int4) &&
                   sizeof(SellMatrix::LongRow) == sizeof(int4), "descriptor layouts");
     slices.alloc(host.slices.size(), false);
@@ -169,8 +153,6 @@ struct DeviceMatrix {
     dev.nsegs = (int)host.segs.size();
     dev.slices = slices.p; dev.col = col.p; dev.val = val.p; dev.segs = segs.p; dev.long_rows = long_rows.p;
     dev.lcol = lcol.p; dev.lval = lval.p; dev.long_partial = long_partial.p; dev.long_counter = long_counter.p;
-    dev.padded_total = (int)host.padded;
-    dev.prefetch_dist = 0;
     // the big host copies are not needed any more
     RawVec<int>().swap(host.col); RawVec<double>().swap(host.val);
     std::vector<int>().swap(host.lcol); std::vector<double>().swap(host.lval);
@@ -242,7 +224,6 @@ struct b200pdlp_problem {
   DevBuf<int> at_outpos;           // A_g^T body row -> position in the segmented partial vector
   // fused P2P path
   std::vector<int> row_bounds;     // row offsets of every rank's block
-  bool device_filled = false;      // the sliced-ELL arrays were filled on the device (params.device_scaling >= 2)
   // HiPDLP mode (reflected Halpern PDHG): its own iterate set; cost/lower/upper/colscale/rowscale/rhs (= row lower) are shared
   struct HipBuffers {
     DevBuf<double> x, y, xn, yn, rx, ry, xa, ya, aty, axp, atyp, dy, atdy, hslack, sp, sn, rup;
@@ -260,7 +241,6 @@ struct b200pdlp_problem {
   std::shared_ptr<b200::LocalGroup> group;   // their host-side rendezvous
   bool no_graph = false;           // B200PDLP_NO_GRAPH: every pass and check as direct launches (debugging aid)
   bool p2p = false;
-  int p2p_pull = 0;                // 1: the primal kernel reads the peers' partials over NVLink; 0: peers push them
   PeerPtrs peers{};
   std::vector<void*> ipc_opened;
   DevBuf<unsigned long long> flags, epochs;
@@ -299,9 +279,7 @@ struct b200pdlp_problem {
   DevBuf<double> trace_dev;
   cudaGraphExec_t graph_pow2[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // 1 << k passes
   cudaGraphExec_t graph_check = nullptr;
-  bool fuse_k4 = false;                           // B200PDLP_FUSE_K4=1: the step rule runs in K3's last CTA (tree mode, one GPU)
   int check_launches[2] = {0, 0};                 // kernels in graph_check / graph_check_light
-  bool fused_check = false;                       // B200PDLP_FUSED_CHECK=1: residual sums in the SpMV epilogues (C2/C3) instead of the split check
   cudaGraphExec_t graph_check_light = nullptr;   // the dense-check phase's check: two sweeps instead of two SpMV (see kDenseChecks)
   DevBuf<double> axsum, atysum;                   // A xSum (ml), A'ySum (n): carried by the passes while iter < kDenseChecks
   long long launches = 0;
@@ -330,9 +308,8 @@ struct b200pdlp_problem {
   ReduceScratch rs(int slot, int len) const {
     // slot-private partial arrays: 16 accumulators x kMaxEwBlocks-or-nblocks each
     double* t = (ordered && len <= ordered_cap) ? terms.p + (size_t)slot * 16 * ordered_cap : nullptr;
-    return ReduceScratch{partials.p + (size_t)slot * scratch_stride, counters.p + slot, t, len, pass_flags};
+    return ReduceScratch{partials.p + (size_t)slot * scratch_stride, counters.p + slot, t, len};
   }
-  int pass_flags = 0;              // ReduceScratch::flags of the pass kernels (B200PDLP_PDL experiment: 2 or 6)
   size_t scratch_stride = 0;
   DevBuf<double> terms;            // ordered-mode term scratch
   bool ordered = false;
@@ -392,76 +369,10 @@ struct Laps {
   }
 };
 
-
-// params.device_scaling >= 1: PDHG_Scale_Data on the GPU (setup_kernels.cu).  The unscaled column-major matrix and the
-// vectors go up once, the 10 Ruiz passes run while the host builds the row-major index of the nonzeros (which the
-// Pock-Chambolle row sums and, later, the row-major layout need anyway), and the scaled data come back into `f`, so the
-// rest of the prologue is unchanged.  Bit-identical to host_prep.cpp::scale.
-// params.device_scaling >= 2 (one GPU): the scaled matrix stays in HBM and the sliced-ELL bodies of A and A' are
-// filled there from the host's PLAN (fill_layouts), so neither layout is built on the host or sent over PCIe.
-struct DeviceSetup {
-  cudaStream_t s = nullptr;
-  int n = 0, m = 0, nnz = 0;
-  DevBuf<int> cbeg, cidx, colof, rptr, rpos;
-  DevBuf<double> cval, cost, lower, upper, colscale, rhs, rowscale, cs, cnorm, rs, rnorm, amax;
-  DeviceSetup() { CUDA_OK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking)); }
-  ~DeviceSetup() { if (s) cudaStreamDestroy(s); }
-  DeviceSetup(const DeviceSetup&) = delete;
-  DeviceSetup& operator=(const DeviceSetup&) = delete;
-
-  template <class Lap>
-  void scale(StdForm& f, Lap& lap) {
-    n = f.n; m = f.m; nnz = f.nnz;
-    cbeg.from(f.cbeg); cidx.from(f.cidx); cval.from(f.cval);
-    cost.from(f.cost); lower.from(f.lower); upper.from(f.upper); colscale.from(f.col_scale);
-    rhs.from(f.rhs); rowscale.from(f.row_scale);
-    colof.alloc(nnz, false);
-    cs.alloc(n, false); cnorm.alloc(n, false); rs.alloc(m, false); rnorm.alloc(m, false); amax.alloc(1, false);
-    lap("scale: upload");
-    DevForm F{n, m, nnz, cbeg.p, cidx.p, colof.p, cval.p, cost.p, lower.p, upper.p, colscale.p, rhs.p, rowscale.p};
-    DevScaleScratch w{cs.p, cnorm.p, rs.p, rnorm.p, amax.p};
-    device_scale_ruiz(s, F, w);
-    CUDA_OK(cudaGetLastError());
-    if (f.rptr.empty()) build_row_index(f);          // host threads, while the device runs the Ruiz passes
-    rptr.from(f.rptr); rpos.from(f.rpos);
-    lap("scale: row index (host) + Ruiz (device)");
-    device_scale_pock_chambolle(s, F, w, rptr.p, rpos.p);
-    CUDA_OK(cudaGetLastError());
-    auto down = [&](auto& dst, const auto& src) {
-      if (!dst.empty()) CUDA_OK(cudaMemcpyAsync(dst.data(), src.p, dst.size() * sizeof(dst[0]), cudaMemcpyDeviceToHost, s));
-    };
-    down(f.cval, cval); down(f.cost, cost); down(f.lower, lower); down(f.upper, upper); down(f.col_scale, colscale);
-    down(f.rhs, rhs); down(f.row_scale, rowscale);
-    double am = 0.0;
-    CUDA_OK(cudaMemcpyAsync(&am, amax.p, sizeof(double), cudaMemcpyDeviceToHost, s));
-    CUDA_OK(cudaStreamSynchronize(s));
-    f.amax = am;
-    lap("scale: Pock-Chambolle + download");
-  }
-
-  // device-side fill of one planned matrix (world == 1): which = 0: A from the row-major index, 1: A' from the columns
-  void fill(DeviceMatrix& M, int which, const std::vector<int>& perm, const std::vector<int>& colmap) {
-    const SellMatrix& h = M.host;
-    DevBuf<int> dperm, dcolmap;
-    dperm.from(perm); dcolmap.from(colmap);
-    M.upload_plan(s);
-    SellSource S{};
-    if (which == 0) { S.beg = rptr.p; S.end = rptr.p + 1; S.pos = rpos.p; S.idx = colof.p; }
-    else { S.beg = cbeg.p; S.end = cbeg.p + 1; S.pos = nullptr; S.idx = cidx.p; }
-    S.val = cval.p; S.idx_offset = 0; S.colmap = dcolmap.p;
-    device_fill_sell(s, h.nrows, (int)h.slices.size(), M.slices.p, dperm.p, S, M.col.p, M.val.p, h.padded,
-                     (int)h.long_rows.size(), M.long_rows.p, M.segs.p, M.lcol.p, M.lval.p);
-    CUDA_OK(cudaGetLastError());
-    CUDA_OK(cudaStreamSynchronize(s));   // dperm / dcolmap go out of scope
-  }
-};
-
 // experiment (B200PDLP_SPMV_CTAS_PER_SM=k, one GPU, tree mode): the SpMV bodies run on a persistent grid of k CTAs per SM and
 // walk their slices in a software pipeline (spmv_sell_kernel<Epi, true>) instead of one CTA per 8 slices
-// hipdlp: the HiPDLP mode's SpMVs (the fused step rule B200PDLP_FUSE_K4 is a pdlp-mode kernel: it stays off)
-static void apply_spmv_grid(b200pdlp_problem* p, bool hipdlp = false) {
+static void apply_spmv_grid(b200pdlp_problem* p) {
   if (p->world != 1 || p->ordered) return;
-  if (const char* e = getenv("B200PDLP_FUSE_K4"); e && !hipdlp) p->fuse_k4 = atoi(e) != 0 && p->AT.grid() > 0;
   auto val = [](const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; };
   const int both = val("B200PDLP_SPMV_CTAS_PER_SM", -1);
   // measured on one H100 (S3, DESIGN.md section 6): the pipelined walk at 3 CTAs per SM helps A'y a little (K3 87.3 -> 85.8
@@ -480,10 +391,10 @@ static void apply_spmv_grid(b200pdlp_problem* p, bool hipdlp = false) {
   };
   // Tiled shape (shared-memory staged gathers, spmv_sell_tile_kernel): B200PDLP_TILE=1 (bulk copy by the TMA unit) or 2
   // (cooperative loads) for both matrices, B200PDLP_TILE_A / _AT for one.  Only where every tile's window fits the staging
-  // buffer and there are enough tiles to occupy the device; not together with the fused step rule or PDL launches.
+  // buffer and there are enough tiles to occupy the device.
   auto tile = [&](DeviceMatrix& M, int mode) {
     // (a few tiles may miss -- wrap-around patterns put both ends of the vector into one window: those gather from global memory)
-    if (mode <= 0 || M.ntiles <= 0 || 10 * M.tiles_staged < 9 * M.ntiles || p->fuse_k4 || p->pass_flags) return false;
+    if (mode <= 0 || M.ntiles <= 0 || 10 * M.tiles_staged < 9 * M.ntiles) return false;
     if (2 * M.ntiles < sms && !getenv("B200PDLP_TILE_FORCE")) return false;   // fewer than half the SMs would have a tile (tests force it)
     M.dev.tiled = mode; M.dev.tile_lo = M.tile_lo.p; M.dev.tile_w = M.tile_w.p;
     M.dev.nblocks_body = M.ntiles; M.dev.pipelined = 0;
@@ -566,9 +477,6 @@ static void create_problem(const b200pdlp_lp& lp, const b200pdlp_params& prm, in
     fprintf(stderr, "[b200pdlp setup] %-28s %8.1f ms\n", what, std::chrono::duration<double, std::milli>(t1 - t0).count());
     t0 = t1;
   };
-  std::unique_ptr<DeviceSetup> dev_setup;
-  int dev_level = prm.device_scaling;
-  if (const char* e = getenv("B200PDLP_DEVICE_SETUP")) dev_level = atoi(e);   // experiments: same switch from the environment
   bool mg_dev_form = false;
   if (!shared_form && world > 1 && lp.num_row > 0 && lp.num_col > 0 && lp.a_start[lp.num_col] > 0) {
     // default (the ranks do not compete for the host's cores and memory bandwidth): B200PDLP_MG_DEVICE_PREP=0 keeps the host
@@ -586,23 +494,13 @@ static void create_problem(const b200pdlp_lp& lp, const b200pdlp_params& prm, in
     formulate(lp, p->form);
     lap("formulate");
   }
-  if (shared_form || mg_dev_form) {
-    // nothing to scale
-  } else if (prm.scaling != 0 && dev_level != 0 && p->form.nnz > 0) {
-    dev_setup.reset(new DeviceSetup());
-    dev_setup->scale(p->form, lap);
-  } else {
-    scale(p->form, prm.scaling != 0);
-  }
+  if (!shared_form && !mg_dev_form) scale(p->form, prm.scaling != 0);
   lap("scale");
   StdForm& f = p->form;
   {
     // host layout (row block, device orderings, sliced-ELL of A_g and A_g^T): host_prep.cpp build_layout
     HostLayout L;
-    // (unsorted columns: the host path re-sorts them, the device fill reads storage order -- stay on the host then)
-    const bool device_fill = dev_setup && dev_level >= 2 && world == 1 && columns_sorted(f);
-    p->device_filled = device_fill;
-    build_layout(f, rank, world, prm.ordered_max, L, lap, /*plan_only=*/device_fill);
+    build_layout(f, rank, world, prm.ordered_max, L, lap);
     p->r0 = L.r0; p->r1 = L.r1; p->ml = L.ml; p->neq_local = L.neq_local; p->ordered = L.ordered;
     p->row_bounds = L.bounds;
     p->n = f.n; p->m = f.m;
@@ -616,21 +514,9 @@ static void create_problem(const b200pdlp_lp& lp, const b200pdlp_params& prm, in
   const int n = p->n, ml = p->ml;
   CUDA_OK(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
   if (world == 1) ensure_side_stream(p);
-  if (p->device_filled) {
-    dev_setup->fill(p->A, 0, p->rperm, p->cinv);
-    dev_setup->fill(p->AT, 1, p->cperm, p->rinv);
-    lap("sliced-ELL fill (device)");
-  } else {
-    p->A.upload();
-    p->AT.upload();
-    lap("matrix upload");
-  }
-  dev_setup.reset();
-  if (const char* e = getenv("B200PDLP_PDL")) {   // experiment, single GPU only: programmatic dependent launch of the pass kernels
-    const int v = atoi(e);
-    if (world == 1) p->pass_flags = v >= 2 ? 6 : (v == 1 ? 2 : 0);
-  }
-  if (const char* e = getenv("B200PDLP_PREFETCH")) { p->A.dev.prefetch_dist = atoi(e); p->AT.dev.prefetch_dist = atoi(e); }
+  p->A.upload();
+  p->AT.upload();
+  lap("matrix upload");
   apply_spmv_grid(p);
   const int nl = p->nl;
   for (int k = 0; k < 2; k++) { p->x[k].alloc(nl); p->aty[k].alloc(nl); p->y[k].alloc(ml); p->ax[k].alloc(ml); }
@@ -674,13 +560,13 @@ static void create_problem(const b200pdlp_lp& lp, const b200pdlp_params& prm, in
   lap("vectors + scratch");
 }
 
-// One GPU, tree mode: the whole prologue on the device (device_prep.cu).  B200PDLP_DEVICE_PREP=0 keeps the host
-// prologue (its tested twin); ordered mode (small problems, bit-identical trajectories) and several GPUs always do.
+// One GPU, tree mode: the whole prologue on the device (device_prep.cu).  params.device_scaling = -1 or
+// B200PDLP_DEVICE_PREP=0 keeps the host prologue (its tested twin); ordered mode (small problems, bit-identical
+// trajectories) and several GPUs always do.
 static bool use_device_prep(const b200pdlp_lp& lp, const b200pdlp_params& prm, int world) {
   if (world != 1) return false;
   if (const char* e = getenv("B200PDLP_DEVICE_PREP")) { if (atoi(e) == 0) return false; }
-  else if (prm.device_scaling != 0) return false;   // -1: host prologue; 1, 2: the staged variants of create_problem
-  if (getenv("B200PDLP_DEVICE_SETUP")) return false;        // the round-1 staged variants (host formulate + device scaling)
+  else if (prm.device_scaling == -1) return false;   // the host prologue on request (check_params allows 0 and -1 only)
   const int omax = prm.ordered_max == 0 ? 4096 : prm.ordered_max;
   // ordered mode (host_prep.cpp::build_layout) is decided on the STANDARD FORM's size: n = num_col + #BOUND rows
   // (ranged and free rows get a slack column, CupdlpWrapper.cpp:328-345) -- count them when the answer depends on it
@@ -711,7 +597,6 @@ static void adopt_matrix(DeviceMatrix& M, DevSellOwned& O) {
   M.dev.nsegs = O.nsegs;
   M.dev.slices = M.slices.p; M.dev.col = M.col.p; M.dev.val = M.val.p; M.dev.segs = M.segs.p; M.dev.long_rows = M.long_rows.p;
   M.dev.lcol = M.lcol.p; M.dev.lval = M.lval.p; M.dev.long_partial = M.long_partial.p; M.dev.long_counter = M.long_counter.p;
-  M.dev.padded_total = (int)O.padded; M.dev.prefetch_dist = 0;
   O = DevSellOwned();   // ownership moved
 }
 
@@ -753,15 +638,12 @@ static void create_problem_device(const b200pdlp_lp& lp, const b200pdlp_params& 
   p->n = n; p->m = m; p->ml = m; p->r0 = 0; p->r1 = m; p->neq_local = f.neq; p->ordered = false;
   p->row_bounds = {0, m};
   p->nl = p->nl_real = n; p->c0 = 0; p->shard_len = n; p->seg_len = n;
-  p->device_filled = true;
   p->csr_local.nrows = m; p->csr_local.ncols = n; p->csr_local.nnz = f.nnz;   // dimensions only (built on demand)
   adopt_matrix(p->A, P.A);
   adopt_matrix(p->AT, P.AT);
   p->cost.adopt(P.arr.cost, n); p->lower.adopt(P.arr.lower, n); p->upper.adopt(P.arr.upper, n); p->colscale.adopt(P.arr.colscale, n);
   p->rhs.adopt(P.arr.rhs, m); p->rowscale.adopt(P.arr.rowscale, m);
   P.arr.cost = P.arr.lower = P.arr.upper = P.arr.colscale = P.arr.rhs = P.arr.rowscale = nullptr;
-  if (const char* ev = getenv("B200PDLP_PDL")) { const int v = atoi(ev); p->pass_flags = v >= 2 ? 6 : (v == 1 ? 2 : 0); }
-  if (const char* ev = getenv("B200PDLP_PREFETCH")) { p->A.dev.prefetch_dist = atoi(ev); p->AT.dev.prefetch_dist = atoi(ev); }
   apply_spmv_grid(p);
   // iterates and scratch: uninitialised (the solve's initial-point kernels write every entry they read)
   for (int k = 0; k < 2; k++) { p->x[k].alloc(n, false); p->aty[k].alloc(n, false); p->y[k].alloc(m, false); p->ax[k].alloc(m, false); }
@@ -827,11 +709,6 @@ static void enqueue_pass(b200pdlp_problem* p) {
                      p->upper.p, p->xsum.p, r1);
   launch_spmv_dual(s, p->A.dev, st, p->x[0].p, p->x[1].p, p->y[0].p, p->y[1].p, p->ax[0].p, p->ax[1].p,
                    p->rhs.p, p->ysum.p, p->neq_local, 0, r2, p->axsum.p);
-  if (p->fuse_k4) {   // B200PDLP_FUSE_K4=1 (experiment): K3's last CTA applies the step rule, three launches per pass
-    launch_spmv_primal(s, p->AT.dev, st, p->y[0].p, p->y[1].p, p->x[0].p, p->x[1].p, p->aty[0].p, p->aty[1].p, r3, p->atysum.p,
-                       r1.partials, primal_step_grid(p->n), r2.partials, p->A.grid());
-    return;
-  }
   launch_spmv_primal(s, p->AT.dev, st, p->y[0].p, p->y[1].p, p->x[0].p, p->x[1].p, p->aty[0].p, p->aty[1].p, r3, p->atysum.p);
   launch_step_rule(s, st, r1, primal_step_grid(p->n), r2, p->A.grid(), r3, p->AT.grid(), nullptr);
 }
@@ -844,13 +721,12 @@ static void enqueue_pass_mg(b200pdlp_problem* p) {
   if (p->p2p) {
     // fused compute + collective over NVLink peer memory (5 launches, no NCCL)
     launch_primal_shard_p2p(s, p->nl, st, p->x[0].p, p->x[1].p, p->aty[0].p, p->peers, p->world, p->rank, p->seg_len,
-                            p->p2p_pull, p->cost.p, p->lower.p, p->upper.p, p->xsum.p, r1, p->atysum.p);
+                            p->cost.p, p->lower.p, p->upper.p, p->xsum.p, r1, p->atysum.p);
     launch_p2p_barrier(s, 0, st, r1.partials, primal_shard_p2p_grid(p->nl), p->peers, p->world, p->rank, p->seg_len,
                        p->shard_len, p->epochs.p, p->fault.p);
     launch_spmv_dual_mg(s, p->A.dev, st, p->xfull.p, p->y[0].p, p->y[1].p, p->ax[0].p, p->ax[1].p, p->rhs.p,
                         p->ysum.p, p->neq_local, r2, p->axsum.p);
     launch_spmv_partial_aty(s, p->AT.dev, st, p->y[0].p, p->y[1].p, p->part.p, p->at_outpos.p);
-    if (!p->p2p_pull) launch_push_part(s, st, p->part.p, p->peers, p->world, p->rank, p->seg_len);
     launch_p2p_barrier(s, 1, st, r2.partials, p->A.grid(), p->peers, p->world, p->rank, p->seg_len, p->shard_len,
                        p->epochs.p, p->fault.p);
     return;
@@ -913,11 +789,10 @@ static void full_aty(b200pdlp_problem* p, const double* y, double* aty) {
     launch_spmv_partial_aty(p->stream, p->AT.dev, nullptr, y, y, p->part.p, p->at_outpos.p);
     p->launches++;
     if (p->p2p) {
-      if (!p->p2p_pull) launch_push_part(p->stream, nullptr, p->part.p, p->peers, p->world, p->rank, p->seg_len);
       launch_p2p_exchange(p->stream, p->outs.p + 60, 0, p->peers, p->world, p->rank, p->epochs.p, p->fault.p);
-      launch_reduce_part_p2p(p->stream, p->nl, aty, p->peers, p->world, p->rank, p->seg_len, p->p2p_pull);
-      // (pull mode: the peers' `part` buffers stay untouched until their next partial SpMV, which comes after a
-      //  barrier that this rank only passes once it has finished reading)
+      launch_reduce_part_p2p(p->stream, p->nl, aty, p->peers, p->world, p->rank, p->seg_len, 1);
+      // (the peers' `part` buffers stay untouched until their next partial SpMV, which comes after a barrier that this
+      //  rank only passes once it has finished reading)
       p->launches += 3;
     } else {
       reduce_scatter_part(p);
@@ -977,7 +852,7 @@ static CheckResult parse_fused_check(b200pdlp_problem* p, bool timed_out_local) 
 // state block and does nothing unless state.iter has reached state.stop_iter.  The host launch overhead of the ~10
 // kernels hides behind the running pass graph, one synchronisation per check interval remains, and on several GPUs
 // the barriers inside the check no longer wait for every rank's host thread.
-static bool can_speculate_check(const b200pdlp_problem* p) { return !p->ordered && (p->world == 1 || (p->p2p && p->p2p_pull)); }
+static bool can_speculate_check(const b200pdlp_problem* p) { return !p->ordered && (p->world == 1 || p->p2p); }
 
 static void enqueue_check_dev(b200pdlp_problem* p, bool timed_out_local) {
   cudaStream_t s = p->stream;
@@ -1029,17 +904,12 @@ static CheckResult run_check(b200pdlp_problem* p, bool timed_out_local) {
   const int n = p->nl, ml = p->ml, cur = h->cur;   // n = column entries held by this rank
   const int acur = p->world == 1 ? cur : 0;        // multi-GPU keeps one current A^T y shard
   const double scale = h->sum_step > 0.0 ? 1.0 / h->sum_step : 1.0;
-  const bool fused_pull = p->world > 1 && p->p2p && p->p2p_pull;
+  const bool fused = p->world > 1 && p->p2p;
   if (p->world > 1 && h->accepted_last) {
     // the last accepted pass left its A^T y' un-reduced (P2P) / in the reduce-scatter buffer (NCCL): make it current
     if (p->p2p) {
-      launch_reduce_part_p2p(s, n, p->aty[0].p, p->peers, p->world, p->rank, p->seg_len, p->p2p_pull);
+      launch_reduce_part_p2p(s, n, p->aty[0].p, p->peers, p->world, p->rank, p->seg_len, 1);
       p->launches++;
-      if (!p->p2p_pull) {
-        // push mode: nobody may overwrite my receive slots (check-time A^T ybar) before I have consumed them
-        launch_p2p_exchange(s, p->outs.p + 60, 0, p->peers, p->world, p->rank, p->epochs.p, p->fault.p);
-        p->launches++;
-      }
     } else {
       CUDA_OK(cudaMemcpyAsync(p->aty[0].p, p->red.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, s));
     }
@@ -1050,7 +920,7 @@ static CheckResult run_check(b200pdlp_problem* p, bool timed_out_local) {
   launch_average(s, ml, p->y[cur].p, p->ysum.p, p->yavg.p, h->pending, h->w_pending, scale);
   p->launches += 2;
   if (h->pending) { h->pending = 0; push_state(p); }
-  if (fused_pull) {
+  if (fused) {
     // one barrier for both exchanges: x-bar shards are stored into every peer's xfull, the partial A_g^T y-bar is
     // parked in my `recv` buffer (so `part`, which a slower peer may still be reducing from, stays intact)
     launch_push_shard(s, p->xavg.p, p->nl, p->peers, p->world, p->rank, p->seg_len);
@@ -1274,7 +1144,7 @@ static bool use_device_checks(const b200pdlp_problem* p, const b200pdlp_params& 
   if (p->ordered || prm.log_level >= 2 || prm.iter_limit <= 0) return false;
   if (p->world != 1) {
     // several GPUs: only on the fused peer-memory path (the checks' collectives are our own barrier / exchange kernels)
-    if (!(p->p2p && p->p2p_pull)) return false;
+    if (!p->p2p) return false;
     // default since it passed on hardware against the oracle (2 GPUs: tests/test_gpu_multi.py; 2 / 3 / 4 logical shards:
     // tests/test_gpu_logical_shards.py; both run both settings).  B200PDLP_MG_DEVICE_CHECK=0: round 1's host-driven checks.
     const char* e = getenv("B200PDLP_MG_DEVICE_CHECK");
@@ -1351,8 +1221,8 @@ static void run_side_by_side(b200pdlp_problem* p, FA&& a, FB&& b) {
   CUDA_OK(cudaStreamWaitEvent(p->stream, p->ev_join, 0));
 }
 
-// the six launches of one check (pdhg_kernels.cu "device-side check iteration"); no-ops unless the check is due.
-// light: the dense-check phase's variant (five launches: two sweeps over the carried A xSum / A'ySum instead of C1-C3)
+// the eight launches of one check (pdhg_kernels.cu "device-side check iteration"); no-ops unless the check is due.
+// light: the dense-check phase's variant (five launches: the two sweeps use the carried A xSum / A'ySum, no C1 / C2)
 static int enqueue_check_device(b200pdlp_problem* p, bool light = false) {
   if (p->world > 1) return enqueue_check_device_mg(p, light);
   cudaStream_t s = p->stream;
@@ -1372,30 +1242,19 @@ static int enqueue_check_device(b200pdlp_problem* p, bool light = false) {
                                   p->yavg.p, p->axavg.p, p->rhs.p, p->rowscale.p, st, ctl, rrow);
         });
   };
-  if (light) {
-    sweeps();
-    launch_check_decide(s, st, ctl, rrow.partials, check_light_grid(ml, false), rcol.partials, check_light_grid(n, true), rrow.counter);
-  } else if (!p->fused_check) {
+  if (!light) {
     // split check: averages, two plain SpMV (as fast as the pass kernels), two vector sweeps for the 20 + 8 sums
     launch_check_avg_xy(s, n, ml, p->x[0].p, p->x[1].p, p->xsum.p, p->xavg.p, p->y[0].p, p->y[1].p, p->ysum.p, p->yavg.p, st, ctl);
     run_side_by_side(p, [&](cudaStream_t q) { launch_spmv_plain(q, p->A.dev, p->xavg.p, p->axavg.p, st); },
                      [&](cudaStream_t q) { launch_spmv_plain(q, p->AT.dev, p->yavg.p, p->atyavg.p, st); });
-    sweeps();
-    launch_check_decide(s, st, ctl, rrow.partials, check_light_grid(ml, false), rcol.partials, check_light_grid(n, true), rrow.counter);
-  } else {
-    // B200PDLP_FUSED_CHECK=1: the sums in the epilogues of the two averaging SpMV (three launches instead of five)
-    launch_check_avg_x(s, n, p->x[0].p, p->x[1].p, p->xsum.p, p->xavg.p, st, ctl);
-    launch_spmv_check_rows(s, p->A.dev, st, ctl, p->xavg.p, p->y[0].p, p->y[1].p, p->ax[0].p, p->ax[1].p, p->ysum.p,
-                           p->yavg.p, p->axavg.p, p->rhs.p, p->rowscale.p, p->neq_local, rrow, p->axsum.p);
-    launch_spmv_check_cols(s, p->AT.dev, st, ctl, p->yavg.p, p->x[0].p, p->x[1].p, p->aty[0].p, p->aty[1].p, p->xavg.p,
-                           p->atyavg.p, p->cost.p, p->lower.p, p->upper.p, p->colscale.p, rcol, p->atysum.p);
-    launch_check_decide(s, st, ctl, rrow.partials, p->A.grid_full(), rcol.partials, p->AT.grid_full(), rrow.counter);
   }
+  sweeps();
+  launch_check_decide(s, st, ctl, rrow.partials, check_light_grid(ml, false), rcol.partials, check_light_grid(n, true), rrow.counter);
   launch_restart_sweep(s, n, ml, p->x[0].p, p->x[1].p, p->aty[0].p, p->aty[1].p, p->xavg.p, p->atyavg.p, p->xsum.p,
                        p->xlr.p, p->y[0].p, p->y[1].p, p->ax[0].p, p->ax[1].p, p->yavg.p, p->axavg.p, p->ysum.p, p->ylr.p,
                        st, ctl, rrst, p->atysum.p, p->axsum.p);
   launch_check_finish(s, st, ctl, rrst.partials, restart_sweep_grid(n, ml));
-  return light ? 5 : (p->fused_check ? 6 : 8);
+  return light ? 5 : 8;
 }
 
 static cudaGraphExec_t capture_check(b200pdlp_problem* p, bool light, int* launches) {
@@ -1469,7 +1328,7 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
     // its peers (see LocalGroup)
     const int interval0 = prm.check_interval > 0 ? prm.check_interval : 40;
     const int want0 = std::min(prm.graph_passes > 0 ? prm.graph_passes : interval0 + 4, kPowTab - 16);
-    p->kernels_per_pass = (p->p2p && p->p2p_pull) ? 5 : 6;
+    p->kernels_per_pass = p->p2p ? 5 : 6;
     if (p->graph_main && p->graph_main_passes != want0) { cudaGraphExecDestroy(p->graph_main); p->graph_main = nullptr; }
     p->graph_main_passes = want0;
     if (!getenv("B200PDLP_NO_GRAPH")) {
@@ -1609,7 +1468,7 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
     if (!p->graph_main) p->graph_main = capture_passes(p, want_main);
     if (!p->graph_small) { p->graph_small_passes = 4; p->graph_small = capture_passes(p, 4); }
   }
-  p->kernels_per_pass = p->world == 1 ? (p->fuse_k4 ? 3 : 4) : ((p->p2p && p->p2p_pull) ? 5 : 6);   // ours; NCCL kernels not counted
+  p->kernels_per_pass = p->world == 1 ? 4 : (p->p2p ? 5 : 6);   // ours; NCCL kernels not counted
   lap("solve", "graph capture");
   nvtxRangePop();
   nvtxRangePushA("b200pdlp: PDHG loop");
@@ -1651,12 +1510,6 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
     c->term = -1;
     // dense-check phase (iterations 0 .. kDenseChecks-1 are all check iterations): the passes carry A xSum and A'ySum, the
     // checks are two vector sweeps.  B200PDLP_LIGHT_CHECK=0: every check multiplies the average iterate by A and A'.
-    {
-      const char* e = getenv("B200PDLP_FUSED_CHECK");
-      const bool fused = e && atoi(e) != 0;
-      if (fused != p->fused_check && p->graph_check) { cudaGraphExecDestroy(p->graph_check); p->graph_check = nullptr; }
-      p->fused_check = fused;
-    }
     const bool hot = warm && warm->col_value && warm->row_value && warm->row_dual;
     h_light = p->axsum.p && p->atysum.p && (p->world == 1 || !hot);   // (several GPUs: A_g xSum of a hot start would need the gathered xSum)
     if (const char* e = getenv("B200PDLP_LIGHT_CHECK")) if (atoi(e) == 0) h_light = false;
@@ -1856,7 +1709,7 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
   const double* dy = use_avg ? p->yavg.p : p->y[cur].p;
   const double* dax = use_avg ? p->axavg.p : p->ax[cur].p;
   if (p->world > 1 && h->accepted_last && !use_avg) {   // (only when the loop never ran a check, e.g. iter_limit <= 0)
-    if (p->p2p) launch_reduce_part_p2p(s, nl, p->aty[0].p, p->peers, p->world, p->rank, p->seg_len, p->p2p_pull);
+    if (p->p2p) launch_reduce_part_p2p(s, nl, p->aty[0].p, p->peers, p->world, p->rank, p->seg_len, 1);
     else CUDA_OK(cudaMemcpyAsync(p->aty[0].p, p->red.p, (size_t)nl * sizeof(double), cudaMemcpyDeviceToDevice, s));
   }
   if (p->p2p) {
@@ -2102,15 +1955,13 @@ static void create_problem_hipdlp_device(const b200pdlp_lp& lp, const b200pdlp_h
   p->n = n; p->m = m; p->ml = m; p->r0 = 0; p->r1 = m; p->neq_local = f.neq; p->ordered = false;
   p->row_bounds = {0, m};
   p->nl = p->nl_real = n; p->c0 = 0; p->shard_len = n; p->seg_len = n;
-  p->device_filled = true;
   p->csr_local.nrows = m; p->csr_local.ncols = n; p->csr_local.nnz = f.nnz;
   adopt_matrix(p->A, P.A);
   adopt_matrix(p->AT, P.AT);
   p->cost.adopt(P.arr.cost, n); p->lower.adopt(P.arr.lower, n); p->upper.adopt(P.arr.upper, n); p->colscale.adopt(P.arr.colscale, n);
   p->rhs.adopt(P.arr.rhs, m); p->rowscale.adopt(P.arr.rowscale, m); p->hip.rup.adopt(P.arr.rup, m);
   P.arr.cost = P.arr.lower = P.arr.upper = P.arr.colscale = P.arr.rhs = P.arr.rowscale = P.arr.rup = nullptr;
-  if (const char* ev = getenv("B200PDLP_PREFETCH")) { p->A.dev.prefetch_dist = atoi(ev); p->AT.dev.prefetch_dist = atoi(ev); }
-  apply_spmv_grid(p, /*hipdlp=*/true);
+  apply_spmv_grid(p);
   hipdlp_buffers(p);
   p->io_col.alloc((size_t)2 * std::max(f.n_orig, 1), false);
   p->io_row.alloc((size_t)2 * std::max(m, 1), false);
@@ -2534,6 +2385,11 @@ static int guarded(F&& fn) {
   }
 }
 
+static void check_params(const b200pdlp_params& prm) {
+  if (prm.device_scaling != 0 && prm.device_scaling != -1)
+    throw Error(B200PDLP_ERR_ARG, "b200pdlp: params.device_scaling must be 0 (default) or -1 (host prologue)");
+}
+
 // deep: also the O(n) / O(nnz) validation of a_start and a_index (the device prologue does both in its first sweep)
 static void check_lp(const b200pdlp_lp* lp, bool deep = true) {
   if (!lp || lp->num_col < 0 || lp->num_row < 0 || !lp->a_start || (lp->a_start[lp->num_col] > 0 && (!lp->a_index || !lp->a_value)) ||
@@ -2583,6 +2439,7 @@ int b200pdlp_problem_create(const b200pdlp_lp* lp, const b200pdlp_params* params
   DeviceGuard dg;
   return guarded([&] {
     if (!params || !out || world < 1 || rank < 0 || rank >= world) throw Error(B200PDLP_ERR_ARG, "b200pdlp_problem_create: bad arguments");
+    check_params(*params);
     check_lp(lp, false);
     check_lp(lp, !use_device_prep(*lp, *params, world));
     auto* p = new b200pdlp_problem();
@@ -2849,7 +2706,7 @@ int b200pdlp_bench_pass(b200pdlp_problem* p, int32_t reps, float ms[4]) {
     set_device(p);
     cudaStream_t s = p->stream;
     PdhgState* st = p->state.p;
-    p->kernels_per_pass = p->world == 1 ? 4 : ((p->p2p && p->p2p_pull) ? 5 : 6);
+    p->kernels_per_pass = p->world == 1 ? 4 : (p->p2p ? 5 : 6);
     pull_state(p);
     p->hstate->stop_iter = 2147483647;
     fill_pow_tables(p->hstate);
@@ -2878,7 +2735,7 @@ int b200pdlp_bench_pass(b200pdlp_problem* p, int32_t reps, float ms[4]) {
         if (p->p2p) {
           CUDA_OK(cudaEventRecord(ev[0], s));
           launch_primal_shard_p2p(s, p->nl, st, p->x[0].p, p->x[1].p, p->aty[0].p, p->peers, p->world, p->rank,
-                                  p->seg_len, p->p2p_pull, p->cost.p, p->lower.p, p->upper.p, p->xsum.p, r1);
+                                  p->seg_len, p->cost.p, p->lower.p, p->upper.p, p->xsum.p, r1);
           launch_p2p_barrier(s, 0, st, r1.partials, primal_shard_p2p_grid(p->nl), p->peers, p->world, p->rank, p->seg_len,
                              p->shard_len, p->epochs.p, p->fault.p);
           CUDA_OK(cudaEventRecord(ev[1], s));
@@ -2886,7 +2743,6 @@ int b200pdlp_bench_pass(b200pdlp_problem* p, int32_t reps, float ms[4]) {
                               p->ysum.p, p->neq_local, r2);
           CUDA_OK(cudaEventRecord(ev[2], s));
           launch_spmv_partial_aty(s, p->AT.dev, st, p->y[0].p, p->y[1].p, p->part.p, p->at_outpos.p);
-          if (!p->p2p_pull) launch_push_part(s, st, p->part.p, p->peers, p->world, p->rank, p->seg_len);
           CUDA_OK(cudaEventRecord(ev[3], s));
           launch_p2p_barrier(s, 1, st, r2.partials, p->A.grid(), p->peers, p->world, p->rank, p->seg_len, p->shard_len,
                              p->epochs.p, p->fault.p);
@@ -2940,6 +2796,7 @@ int b200pdlp_solve(const b200pdlp_lp* lp, const b200pdlp_params* params, const b
   DeviceGuard dg;
   return guarded([&] {
     if (!params || !out) throw Error(B200PDLP_ERR_ARG, "null argument");
+    check_params(*params);
     check_lp(lp, false);
     check_lp(lp, !use_device_prep(*lp, *params, 1));
     const auto t0 = std::chrono::steady_clock::now();
@@ -2975,6 +2832,7 @@ int b200pdlp_solve_multi(const b200pdlp_lp* lp, const b200pdlp_params* params, c
   const int rc = guarded([&] {
     check_lp(lp);
     if (!params || !out || ngpus > kMaxPeers) throw Error(B200PDLP_ERR_ARG, "b200pdlp_solve_multi: bad arguments");
+    check_params(*params);
     const auto t0 = std::chrono::steady_clock::now();
     for (int g = 0; g < ngpus; g++) {
       b200pdlp_params prm = *params;
@@ -3249,8 +3107,6 @@ int b200pdlp_p2p_import(b200pdlp_problem* p, const uint8_t* all_handles) {
       p->peers.recv[g] = (double*)q[3];
     }
     p->p2p = true;
-    p->p2p_pull = 1;   // pull variant by default (B200PDLP_P2P_PULL=0: push); the two have not been compared on H100s
-    if (const char* e = getenv("B200PDLP_P2P_PULL")) p->p2p_pull = atoi(e);
     // graphs captured for the NCCL path are stale now
     drop_graphs(p);
   });
@@ -3291,7 +3147,6 @@ int b200pdlp_p2p_link_local(b200pdlp_problem** probs, int32_t count) {
       p->p2p = true;
       p->local_link = true;
       p->group = group;
-      p->p2p_pull = 1;
       drop_graphs(p);
     }
   });

@@ -518,16 +518,6 @@ void build_col_major(const StdForm& f, int r0, int r1, Csr& at) {
   });
 }
 
-bool columns_sorted(const StdForm& f) {
-  std::atomic<bool> ok{true};
-  parallel_chunks(f.n, [&](int, long long j0, long long j1) {
-    for (int j = (int)j0; j < (int)j1 && ok.load(std::memory_order_relaxed); j++)
-      for (int p = f.cbeg[j] + 1; p < f.cbeg[j + 1]; p++)
-        if (f.cidx[p] < f.cidx[p - 1]) { ok.store(false, std::memory_order_relaxed); break; }
-  }, 4096);
-  return ok.load();
-}
-
 std::vector<int> make_perm(const std::vector<int>& rowptr, int boundary, bool sort) {
   const int n = (int)rowptr.size() - 1;
   std::vector<int> perm(n);

@@ -129,9 +129,6 @@ void build_row_major(const StdForm& f, int r0, int r1, Csr& a);
 void build_col_major(const StdForm& f, int r0, int r1, Csr& at);
 // new -> old ordering of `count` rows: identity, or (sort) by descending length inside windows that
 // do not straddle `boundary`
-// true if the row indices of every column ascend (the storage order is then the order in which the reference's
-// row-scatter adds into that column's output)
-bool columns_sorted(const StdForm& f);
 std::vector<int> make_perm(const std::vector<int>& rowptr, int boundary, bool sort);
 std::vector<int> invert_perm(const std::vector<int>& perm);
 // rows of `a` taken in `perm` order, column ids mapped through `colmap` (old -> new)

@@ -115,7 +115,7 @@ struct HipState {
 struct DevSell {
   int nrows, nslices;
   int nblocks_body;                       // CTAs that process slices (8 slices = 256 rows each; fewer when `pipelined`)
-  int nblocks_full;                       // one CTA per 8 slices, whatever nblocks_body says (the check kernels use this shape)
+  int nblocks_full;                       // one CTA per 8 slices, whatever nblocks_body says (sizes the partial-sum scratch)
   int nsegs;                              // + one CTA per long-row segment
   const int4* __restrict__ slices;        // {ptr, len, skipmask, -}
   const int* __restrict__ col;
@@ -126,8 +126,6 @@ struct DevSell {
   const double* __restrict__ lval;
   double* long_partial;
   unsigned* long_counter;
-  int prefetch_dist;                      // CTAs ahead whose col/val range is pulled into L2 (0 = off)
-  int padded_total;                       // elements in col/val (end of the last slice)
   int pipelined;                          // 1: nblocks_body is a persistent grid (a few CTAs per SM), slices walked in a software pipeline
   // TILED shape (structured matrices; spmv_sell_tile_kernel): one 1024-thread CTA per kTileSlices consecutive slices (= one
   // 8192-row sort window); the window of the input vector those rows touch, [tile_lo[t], tile_lo[t] + tile_w[t]), is staged in
@@ -160,19 +158,7 @@ struct ReduceScratch {
   // (cupdlp_linalg.c:111-126,320-336), which makes whole trajectories bit-identical.
   double* terms;      // nullptr = tree mode
   int len;            // elements per accumulator in terms[]
-  int flags;          // experiment switches (bit 0: skip the grid reduction -- timing experiments only;
-                      //  bit 1: the kernel was launched with programmatic dependent launch: wait for the preceding
-                      //  grid before the first global read; bit 2: additionally release the dependent grid early)
 };
-
-// Programmatic dependent launch (experiment, B200PDLP_PDL): the launch latency of kernel k+1 hides behind kernel k.
-// Every pass kernel calls this before it touches anything the preceding kernel wrote (the state block first of all).
-__device__ __forceinline__ void pdl_entry(int flags) {
-  if (flags & 2) {
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    if (flags & 4) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  }
-}
 
 // ----------------------------------------------------------------- reductions
 __device__ __forceinline__ double warp_sum(double v) {
@@ -238,7 +224,6 @@ __device__ __forceinline__ bool grid_reduce(const double (&acc)[NACC], ReduceScr
   __shared__ double sm[NACC][kWarps];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int nb = gridDim.x;
-  if (rs.flags & 1) return false;
 #pragma unroll
   for (int a = 0; a < NACC; a++) {
     const double s = warp_sum(acc[a]);

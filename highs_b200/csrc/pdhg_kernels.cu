@@ -1,8 +1,6 @@
 // highs_b200/csrc/pdhg_kernels.cu -- kernel definitions + launchers (see kernels.cuh).
 #include "pdhg_kernels.hpp"
 
-#include <utility>
-
 namespace b200 {
 
 // =============================================================== K1: primal step
@@ -15,7 +13,6 @@ primal_step_kernel(int n, PdhgState* __restrict__ st, double* __restrict__ x0, d
                    const double* __restrict__ aty0, const double* __restrict__ aty1,
                    const double* __restrict__ c, const double* __restrict__ lo, const double* __restrict__ up,
                    double* __restrict__ xsum, ReduceScratch rs) {
-  pdl_entry(rs.flags);
   if (st->iter >= st->stop_iter) return;
   const int cur = st->cur;
   const double tau = st->tau_try, ntau = -tau;
@@ -212,10 +209,6 @@ struct PrimalEpilogue {
   const double *x0, *x1;
   double *aty0, *aty1;
   double* atysum;              // A'ySum, carried while the checks are dense (PdhgState::light_on); may be nullptr
-  // fused step rule (B200PDLP_FUSE_K4): the last CTA of K3 to finish adds the block partials of K1, K2 and K3 and applies the
-  // step rule -- K4's work without K4's launch
-  const double *p1, *p2;
-  int nb1, nb2, fuse;
   const double *x, *xn, *aty;
   double* atyn;
   double w;
@@ -233,25 +226,6 @@ struct PrimalEpilogue {
   __device__ const double* input() const { return y0; }
   double p_x, p_xn, p_aty, p_as;
   __device__ void prefetch(int r) { p_x = x[r]; p_xn = xn[r]; p_aty = aty[r]; p_as = accum ? atysum[r] : 0.0; }
-  __device__ void tail(const ReduceScratch& rs, int nb3) const {
-    // same sums as step_rule_kernel (fixed order: thread-strided, lanes, warps), on this CTA's kThreads threads
-    __shared__ double smt[3][kThreads / 32];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    double s1 = 0.0, s2 = 0.0, s3 = 0.0;
-    for (int i = threadIdx.x; i < nb1; i += kThreads) s1 += __ldcg(p1 + i);
-    for (int i = threadIdx.x; i < nb2; i += kThreads) s2 += __ldcg(p2 + i);
-    for (int i = threadIdx.x; i < nb3; i += kThreads) s3 += __ldcg(rs.partials + i);   // other CTAs of THIS kernel wrote them
-    s1 = warp_sum(s1); s2 = warp_sum(s2); s3 = warp_sum(s3);
-    if (lane == 0) { smt[0][wid] = s1; smt[1][wid] = s2; smt[2][wid] = s3; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      double t1 = 0.0, t2 = 0.0, t3 = 0.0;
-      for (int q = 0; q < kThreads / 32; q++) { t1 += smt[0][q]; t2 += smt[1][q]; t3 += smt[2][q]; }
-      st->dx2 = t1;
-      st->dy2 = t2;
-      step_rule(st, t3);
-    }
-  }
   __device__ void row(int r, double s, double* t) const {
     atyn[r] = s;
     if (accum) atysum[r] = p_as + w * p_aty;   // A'ySum += w A'y
@@ -268,18 +242,17 @@ constexpr int kStepThreads = 1024;
 __global__ void __launch_bounds__(kStepThreads)
 step_rule_kernel(PdhgState* __restrict__ st, ReduceScratch r1, int nb1, ReduceScratch r2, int nb2, ReduceScratch r3,
                  int nb3, const double* __restrict__ dy2_override) {
-  pdl_entry(r1.flags);
   __shared__ double sm[3][kStepThreads / 32];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   double tot[3];
   if (r1.terms) {
     // ordered mode: thread a adds accumulator a's terms sequentially
     if (st->iter >= st->stop_iter) return;
-    const ReduceScratch* rr[3] = {&r1, &r2, &r3};
     double s = 0.0;
     if (threadIdx.x < 3) {
-      const double* t = rr[threadIdx.x]->terms;
-      const int len = rr[threadIdx.x]->len;
+      // (selected field by field: taking the parameters' addresses would copy all three to the stack first)
+      const double* t = threadIdx.x == 0 ? r1.terms : (threadIdx.x == 1 ? r2.terms : r3.terms);
+      const int len = threadIdx.x == 0 ? r1.len : (threadIdx.x == 1 ? r2.len : r3.len);
       for (int i = 0; i < len; i++) s += t[i];
       sm[threadIdx.x][0] = s;
     }
@@ -320,40 +293,21 @@ step_rule_kernel(PdhgState* __restrict__ st, ReduceScratch r1, int nb1, ReduceSc
   }
 }
 
-template <class E> struct HasTail { static constexpr bool value = false; };
-template <> struct HasTail<PrimalEpilogue> { static constexpr bool value = true; };
-
 // PIPE: persistent grid (DevSell::pipelined), slices walked in a software pipeline; !PIPE: one CTA per 8 slices
 template <class Epi, bool PIPE = false>
 __global__ void __launch_bounds__(kThreads) spmv_sell_kernel(DevSell A, Epi epi_arg, ReduceScratch rs) {
   Epi epi = epi_arg;
-  pdl_entry(rs.flags);
   if (!epi.begin()) return;
   const double* __restrict__ xin = epi.input();
-  // Epilogues with many sums (the check iteration's 8 / 20): in the one-slice-per-warp shape every thread finishes at most
-  // ONE row, so its terms go straight to a shared-memory row instead of living in 2 x NACC registers next to the gather
-  // pipeline (CheckColEpilogue: 128 -> ~48 registers, i.e. 2 -> 5 resident CTAs per SM); the block tree is the same.
+  // Epilogues with many sums (CheckRowEpilogue, the multi-GPU check's 8): in the one-slice-per-warp shape every thread
+  // finishes at most ONE row, so its terms go straight to a shared-memory row instead of living in 2 x NACC registers next
+  // to the gather pipeline; the block tree is the same.
   constexpr bool kSmemAcc = (Epi::NACC > 4) && !PIPE;
   __shared__ double sacc[kSmemAcc ? Epi::NACC : 1][kSmemAcc ? kThreads : 1];
   double acc[(Epi::NACC > 0 && !kSmemAcc) ? Epi::NACC : 1] = {0.0};
   if constexpr (kSmemAcc) {
 #pragma unroll
     for (int a = 0; a < Epi::NACC; a++) sacc[a][threadIdx.x] = 0.0;
-  }
-  if (A.prefetch_dist > 0 && threadIdx.x == 0) {
-    // pull the col/val range of a CTA that will run one residency wave later into L2, so that its
-    // streaming loads hold their L1 miss slots for an L2 round trip instead of an HBM one
-    const int b2 = blockIdx.x + A.prefetch_dist;
-    if (b2 < A.nblocks_body) {
-      const int s0 = b2 * (kThreads / 32), s1 = s0 + (kThreads / 32);
-      const int p0 = A.slices[s0].x;
-      const int p1 = s1 < A.nslices ? A.slices[s1].x : A.padded_total;
-      const unsigned nb4 = (unsigned)(p1 - p0) * 4u, nb8 = (unsigned)(p1 - p0) * 8u;
-      if (nb4) {
-        asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(A.col + p0), "r"(nb4) : "memory");
-        asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(A.val + p0), "r"(nb8) : "memory");
-      }
-    }
   }
   if (PIPE && (int)blockIdx.x < A.nblocks_body) {
     // A warp walks the slices  w, w + W, w + 2W, ...  (W = warps of the body CTAs).  With one CTA per 8 slices (the default
@@ -540,21 +494,6 @@ __global__ void __launch_bounds__(kThreads) spmv_sell_kernel(DevSell A, Epi epi_
     }
   } else if constexpr (Epi::NACC > 0) {
     block_partials<Epi::NACC>(acc, rs);
-  }
-  if constexpr (HasTail<Epi>::value) {
-    // last-CTA-done: the epilogue's tail runs once, after every CTA of this launch has published its partial sums
-    if (epi.fuse) {
-      __shared__ int is_last;
-      if (threadIdx.x == 0) {
-        __threadfence();
-        is_last = atomicAdd(rs.counter, 1u) == gridDim.x - 1u ? 1 : 0;
-      }
-      __syncthreads();
-      if (is_last) {
-        if (threadIdx.x == 0) { *rs.counter = 0u; __threadfence(); }
-        epi.tail(rs, (int)gridDim.x);
-      }
-    }
   }
 }
 
@@ -796,7 +735,7 @@ __device__ __forceinline__ double ld_sys(const double* p) {
 
 __global__ void __launch_bounds__(kThreads)
 primal_shard_p2p_kernel(int len, PdhgState* __restrict__ st, double* __restrict__ xs0, double* __restrict__ xs1,
-                        double* __restrict__ aty_s, PeerPtrs pp, int world, int rank, int seg_len, int pull,
+                        double* __restrict__ aty_s, PeerPtrs pp, int world, int rank, int seg_len,
                         const double* __restrict__ c, const double* __restrict__ lo, const double* __restrict__ up,
                         double* __restrict__ xsum, ReduceScratch rs, double* __restrict__ atysum) {
   if (st->iter >= st->stop_iter) return;
@@ -823,19 +762,14 @@ primal_shard_p2p_kernel(int len, PdhgState* __restrict__ st, double* __restrict_
   for (int i = blockIdx.x * kThreads + threadIdx.x; i < npair; i += stride) {
     double2 ai;
     if (take) {
-      // reduce-scatter, second half: the G partial A_h^T y' segments that the peers PUSHED into my receive
-      // slots (push_part_kernel), added in rank order
-      // (pull variant: read the peers' `part` segments over NVLink instead)
-      // all G loads are issued before the first add (with the loads inside the summing loop a thread would pay G NVLink
-      // round trips one after the other); the sum stays in rank order
+      // reduce-scatter: my segment of the G partial A_h^T y', read from the peers' `part` buffers over NVLink and added
+      // in rank order.  All G loads are issued before the first add (with the loads inside the summing loop a thread
+      // would pay G NVLink round trips one after the other).  The address is formed whole per element: written as
+      // (part[h] + seg) + i, the compiler keeps the 16 segment bases in registers (148 instead of 116)
       double2 q[kMaxPeers];
 #pragma unroll
-      for (int h = 0; h < kMaxPeers; h++) {
-        if (h < world) {
-          const double* src = pull ? pp.part[h] + seg : pp.recv[rank] + (size_t)h * seg_len;
-          q[h] = __ldcg(reinterpret_cast<const double2*>(src) + i);
-        }
-      }
+      for (int h = 0; h < kMaxPeers; h++)
+        if (h < world) q[h] = __ldcg(reinterpret_cast<const double2*>(pp.part[h] + seg + 2 * (size_t)i));
       ai = make_double2(0.0, 0.0);
 #pragma unroll
       for (int h = 0; h < kMaxPeers; h++) {
@@ -870,21 +804,6 @@ primal_shard_p2p_kernel(int len, PdhgState* __restrict__ st, double* __restrict_
   // no per-thread system fence: the kernel boundary completes the peer stores, and the barrier
   // kernel that follows fences at system scope before it signals
   block_partials<1>(acc, rs);
-}
-
-// reduce-scatter, first half: every rank stores segment r of its partial A_g^T y' into rank r's receive
-// slot (coalesced 128-bit stores over NVLink; posted writes need no round trip)
-__global__ void __launch_bounds__(kThreads)
-push_part_kernel(PdhgState* st, const double* __restrict__ part, PeerPtrs pp, int world, int rank, int seg_len) {
-  if (st && st->iter >= st->stop_iter) return;
-  const int npair = seg_len >> 1;   // includes the scalar tail
-  const int total = npair * world;
-  const int stride = gridDim.x * kThreads;
-  for (int t = blockIdx.x * kThreads + threadIdx.x; t < total; t += stride) {
-    const int r = t / npair, i = t - r * npair;
-    const double2 v = reinterpret_cast<const double2*>(part + (size_t)r * seg_len)[i];
-    reinterpret_cast<double2*>(pp.recv[r] + (size_t)rank * seg_len)[i] = v;
-  }
 }
 
 // check-iteration collectives of the fused path ------------------------------------------------------
@@ -972,13 +891,12 @@ reduce_part_p2p_kernel(int len, double* __restrict__ dst, PeerPtrs pp, int world
   const size_t seg = (size_t)rank * seg_len;
   const int stride = gridDim.x * kThreads;
   for (int i = blockIdx.x * kThreads + threadIdx.x; i < len; i += stride) {
-    // pull 0: the peers pushed into my receive slots; 1: read the peers' `part`; 2: read the peers' `recv`
-    // (check iterations park their partial A_g^T ybar there so that `part` keeps the last pass's data)
-    // (loads first, then the sum in rank order: see primal_shard_p2p_kernel)
+    // pull 1: read the peers' `part`; 2: read the peers' `recv` (check iterations park their partial A_g^T ybar there so
+    // that `part` keeps the last pass's data).  Loads first, then the sum in rank order: see primal_shard_p2p_kernel
     double q[kMaxPeers];
 #pragma unroll
     for (int h = 0; h < kMaxPeers; h++)
-      if (h < world) q[h] = __ldcg(pull == 0 ? pp.recv[rank] + (size_t)h * seg_len + i : (pull == 1 ? pp.part[h] : pp.recv[h]) + seg + i);
+      if (h < world) q[h] = __ldcg((pull == 1 ? pp.part[h] : pp.recv[h]) + seg + i);
     double ai = 0.0;
 #pragma unroll
     for (int h = 0; h < kMaxPeers; h++)
@@ -1417,10 +1335,10 @@ __global__ void __launch_bounds__(kThreads) fill_kernel(int len, double* __restr
 // ================================================== device-side check iteration (tree mode, one GPU)
 // The whole check -- averages, A xbar and A'ybar, residuals of both iterates, termination, infeasibility, restart --
 // without a host round trip (cupdlp_solver.c:953-1106 on the host in the reference; host_check path of engine.cu for
-// ordered mode / several GPUs).  Six launches:
-//   C1 check_avg_x_kernel          xbar = (xSum + w x) / sum(w)                  (cupdlp_step.c:377-420)
-//   C2 spmv<CheckRowEpilogue>      A xbar; ybar formed on the fly; row-side sums of BOTH iterates in the epilogue
-//   C3 spmv<CheckColEpilogue>      A'ybar; column-side sums of both iterates in the epilogue
+// ordered mode / several GPUs).  Eight launches (the split check):
+//   C1 check_avg_xy_kernel         xbar = (xSum + w x) / sum(w), ybar likewise   (cupdlp_step.c:377-420)
+//   C2 spmv<PlainEpilogue> x 2     A xbar and A'ybar, side by side
+//   C3 check_*_sweep_kernel x 2    column-side (20) and row-side (8) sums of BOTH iterates, side by side
 //   C4 check_decide_kernel         adds the block partials, forms the residuals, decides (1 CTA)
 //   C5 restart_sweep_kernel        only if C4 chose a restart: copies, clears the sums, |x - x_lr|^2, |y - y_lr|^2
 //   C6 check_finish_kernel         restart scalars (beta, tau, sigma), trace row, next check iteration, power tables
@@ -1475,94 +1393,41 @@ __device__ __forceinline__ void col_terms(double x, double aty, double ci, doubl
   t[6] = x * x; t[7] = k * k; t[8] = bl * bl; t[9] = bu * bu;
 }
 
-// FLUSH: ybar is formed here from ySum (one GPU).  !FLUSH (several GPUs: the partial A_g'ybar had to be launched before
-// this kernel could run, so ybar was formed by average_dev_kernel): ybar is read
-template <bool FLUSH>
-struct CheckRowEpilogueT {
+// Row side of the multi-GPU check (launch_spmv_check_rows_mg): A_g xbar, with the row-side sums of BOTH iterates in the
+// epilogue.  ybar is read: the partial A_g'ybar had to be launched before this kernel could run, so average_dev_kernel
+// formed ybar already.
+struct CheckRowEpilogue {
   static constexpr int NACC = 8;
   const PdhgState* st;
   const SolveCtl* ctl;
   const double* xavg;
   const double *y0, *y1, *ax0, *ax1;
-  double *ysum, *yavg, *axavg;
+  const double* yavg;
+  double* axavg;
   const double *b, *rsc;
   int neq;
-  double* axsum;   // one GPU, dense-check phase: kept consistent with ySum's flush (may be nullptr)
   const double *y, *ax;
-  double w, scale;
-  bool pend, accum;
   __device__ bool begin() {
     if (!check_live(st, ctl)) return false;
     const int cur = st->cur;
     y = cur ? y1 : y0; ax = cur ? ax1 : ax0;
-    w = st->w_pending; pend = st->pending != 0;
-    accum = FLUSH && pend && axsum && st->light_on && st->iter < kDenseChecks;
-    scale = st->sum_step > 0.0 ? 1.0 / st->sum_step : 1.0;
     return true;
   }
   __device__ const double* input() const { return xavg; }
-  double p_y, p_ax, p_ys, p_b, p_sc;
-  __device__ void prefetch(int r) { p_y = y[r]; p_ax = ax[r]; p_ys = FLUSH ? ysum[r] : yavg[r]; p_b = b[r]; p_sc = rsc[r]; }
+  double p_y, p_ax, p_ya, p_b, p_sc;
+  __device__ void prefetch(int r) { p_y = y[r]; p_ax = ax[r]; p_ya = yavg[r]; p_b = b[r]; p_sc = rsc[r]; }
   template <class T>
   __device__ void row(int r, double s, T t) const {
     axavg[r] = s;
-    double ya;
-    if (FLUSH) {
-      double ys = p_ys;
-      if (pend) { ys = ys + w * p_y; ysum[r] = ys; }
-      if (accum) axsum[r] = axsum[r] + w * p_ax;
-      ya = ys * scale;
-      yavg[r] = ya;
-    } else {
-      ya = p_ys;
-    }
     const bool ineq = r >= neq;
     row_terms(p_y, p_ax, p_b, p_sc, ineq, t);
-    row_terms(ya, s, p_b, p_sc, ineq, t + 4);
-  }
-};
-
-using CheckRowEpilogue = CheckRowEpilogueT<true>;
-
-struct CheckColEpilogue {
-  static constexpr int NACC = 20;
-  const PdhgState* st;
-  const SolveCtl* ctl;
-  const double* yavg;
-  const double *x0, *x1, *aty0, *aty1, *xavg;
-  double* atyavg;
-  const double *c, *lo, *up, *cs;
-  double* atysum;   // dense-check phase: kept consistent with xSum's flush (C1); may be nullptr
-  const double *x, *aty;
-  double w;
-  bool accum;
-  __device__ bool begin() {
-    if (!check_live(st, ctl)) return false;
-    const int cur = st->cur;
-    x = cur ? x1 : x0; aty = cur ? aty1 : aty0;
-    w = st->w_pending;
-    accum = st->pending != 0 && atysum && st->light_on && st->iter < kDenseChecks;
-    return true;
-  }
-  __device__ const double* input() const { return yavg; }
-  double p_x, p_aty, p_xa, p_c, p_lo, p_up, p_cs;
-  __device__ void prefetch(int j) {
-    p_x = x[j]; p_aty = aty[j]; p_xa = xavg[j]; p_c = c[j]; p_lo = lo[j]; p_up = up[j]; p_cs = cs[j];
-  }
-  template <class T>
-  __device__ void row(int j, double s, T t) const {
-    atyavg[j] = s;
-    if (accum) atysum[j] = atysum[j] + w * p_aty;
-    col_terms(p_x, p_aty, p_c, p_lo, p_up, p_cs, t);
-    col_terms(p_xa, s, p_c, p_lo, p_up, p_cs, t + 10);
+    row_terms(p_ya, s, p_b, p_sc, ineq, t + 4);
   }
 };
 
 // ---- the residual sweeps of a check as plain vector kernels (one GPU).  Two uses:
 //  * SPLIT check (GIVEN = true; the default from iteration kDenseChecks on): C1 forms xbar AND ybar, two PLAIN SpMV give
-//    A xbar and A'ybar at the speed of the pass kernels, and these sweeps add the 20 + 8 terms.  The fused epilogues
-//    (CheckRowEpilogue / CheckColEpilogue: the 20 accumulators cost the column kernel its occupancy) are replaced by plain
-//    SpMV at the speed of the pass kernels and two vector sweeps.
+//    A xbar and A'ybar at the speed of the pass kernels, and these sweeps add the 20 + 8 terms.
 //  * LIGHT check (GIVEN = false; dense-check phase, PdhgState::light_on && iter < kDenseChecks): A xbar = (A xSum) / sum(w)
 //    and A'ybar = (A'ySum) / sum(w) come from the sums the passes carried: no SpMV at all.
 // Same per-element terms (col_terms / row_terms) and the same downstream kernels (C4-C6) in both.
@@ -2034,20 +1899,6 @@ check_finish_kernel(PdhgState* __restrict__ st, SolveCtl* __restrict__ ctl, cons
 }
 
 // ==================================================================== launchers
-// plain <<<>>> launch, or (flags bit 1) a launch with the programmatic-stream-serialization attribute: the grid may be
-// scheduled while its predecessor in the stream is still running; the kernel then waits in pdl_entry()
-template <class... KArgs, class... Args>
-static void launch_k(void (*kernel)(KArgs...), int grid, int block, cudaStream_t s, int flags, Args&&... args) {
-  if (!(flags & 2)) { kernel<<<grid, block, 0, s>>>(std::forward<Args>(args)...); return; }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3((unsigned)block); cfg.dynamicSmemBytes = 0; cfg.stream = s;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = 1;
-  cudaLaunchKernelEx(&cfg, kernel, KArgs(std::forward<Args>(args))...);
-}
-
 static inline int ew_grid(int len) {
   int g = (len + kThreads - 1) / kThreads;
   if (g < 1) g = 1;
@@ -2057,15 +1908,15 @@ static inline int ew_grid(int len) {
 void launch_primal_step(cudaStream_t s, int n, PdhgState* st, double* x0, double* x1, const double* aty0,
                         const double* aty1, const double* c, const double* lo, const double* up, double* xsum,
                         ReduceScratch rs) {
-  launch_k(primal_step_kernel, ew_grid((n + 1) / 2), kThreads, s, rs.flags, n, st, x0, x1, aty0, aty1, c, lo, up, xsum, rs);
+  primal_step_kernel<<<ew_grid((n + 1) / 2), kThreads, 0, s>>>(n, st, x0, x1, aty0, aty1, c, lo, up, xsum, rs);
 }
 
 void launch_spmv_plain(cudaStream_t s, const DevSell& A, const double* in, double* out, const PdhgState* due) {
   if (A.nblocks_body + A.nsegs == 0) return;
   PlainEpilogue e{in, out, due};
-  if (A.tiled) { launch_tile(s, A, e, ReduceScratch{nullptr, nullptr, nullptr, 0, 0}); return; }
-  if (A.pipelined) spmv_sell_kernel<PlainEpilogue, true><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, ReduceScratch{nullptr, nullptr, nullptr, 0, 0});
-  else spmv_sell_kernel<PlainEpilogue, false><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, ReduceScratch{nullptr, nullptr, nullptr, 0, 0});
+  if (A.tiled) { launch_tile(s, A, e, ReduceScratch{nullptr, nullptr, nullptr, 0}); return; }
+  if (A.pipelined) spmv_sell_kernel<PlainEpilogue, true><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, ReduceScratch{nullptr, nullptr, nullptr, 0});
+  else spmv_sell_kernel<PlainEpilogue, false><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, ReduceScratch{nullptr, nullptr, nullptr, 0});
 }
 
 void launch_spmv_dual(cudaStream_t s, const DevSell& A, PdhgState* st, const double* x0, const double* x1,
@@ -2076,20 +1927,18 @@ void launch_spmv_dual(cudaStream_t s, const DevSell& A, PdhgState* st, const dou
   e.st = st; e.x0 = x0; e.x1 = x1; e.y0 = y0; e.y1 = y1; e.ax0 = ax0; e.ax1 = ax1; e.b = b; e.ysum = ysum;
   e.neq = neq; e.row_offset = row_offset; e.axsum = axsum;
   if (A.tiled) { launch_tile(s, A, e, rs); return; }   // (the engine tiles only in tree mode)
-  if (A.pipelined) launch_k(spmv_sell_kernel<DualEpilogue, true>, A.nblocks_body + A.nsegs, kThreads, s, rs.flags, A, e, rs);
-  else launch_k(spmv_sell_kernel<DualEpilogue, false>, A.nblocks_body + A.nsegs, kThreads, s, rs.flags, A, e, rs);
+  if (A.pipelined) spmv_sell_kernel<DualEpilogue, true><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, rs);
+  else spmv_sell_kernel<DualEpilogue, false><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, rs);
 }
 
 void launch_spmv_primal(cudaStream_t s, const DevSell& A, PdhgState* st, const double* y0, const double* y1,
-                        const double* x0, const double* x1, double* aty0, double* aty1, ReduceScratch rs, double* atysum,
-                        const double* p1, int nb1, const double* p2, int nb2) {
+                        const double* x0, const double* x1, double* aty0, double* aty1, ReduceScratch rs, double* atysum) {
   if (A.nblocks_body + A.nsegs == 0) return;   // no rows on this rank: nothing to launch, the partial count is 0
   PrimalEpilogue e{};
   e.st = st; e.y0 = y0; e.y1 = y1; e.x0 = x0; e.x1 = x1; e.aty0 = aty0; e.aty1 = aty1; e.atysum = atysum;
-  e.p1 = p1; e.nb1 = nb1; e.p2 = p2; e.nb2 = nb2; e.fuse = (p1 != nullptr && rs.terms == nullptr) ? 1 : 0;
-  if (A.tiled) { launch_tile(s, A, e, rs); return; }   // (tree mode only; never together with the fused step rule: engine.cu)
-  if (A.pipelined) launch_k(spmv_sell_kernel<PrimalEpilogue, true>, A.nblocks_body + A.nsegs, kThreads, s, rs.flags, A, e, rs);
-  else launch_k(spmv_sell_kernel<PrimalEpilogue, false>, A.nblocks_body + A.nsegs, kThreads, s, rs.flags, A, e, rs);
+  if (A.tiled) { launch_tile(s, A, e, rs); return; }   // (tree mode only: engine.cu)
+  if (A.pipelined) spmv_sell_kernel<PrimalEpilogue, true><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, rs);
+  else spmv_sell_kernel<PrimalEpilogue, false><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, rs);
 }
 
 // multi-GPU K3a: partial A_g' y' into buf (input chosen by the device state)
@@ -2119,7 +1968,7 @@ void launch_spmv_partial_aty(cudaStream_t s, const DevSell& A, PdhgState* st, co
                              double* part, const int* outpos, const PdhgState* due) {
   if (A.nblocks_body + A.nsegs == 0) return;
   PartialAtyEpilogue e{st, y0, y1, part, outpos, due};
-  spmv_sell_kernel<PartialAtyEpilogue><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, ReduceScratch{nullptr, nullptr, nullptr, 0, 0});
+  spmv_sell_kernel<PartialAtyEpilogue><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, ReduceScratch{nullptr, nullptr, nullptr, 0});
 }
 
 void launch_spmv_dual_mg(cudaStream_t s, const DevSell& A, PdhgState* st, const double* xfull, double* y0, double* y1,
@@ -2146,13 +1995,10 @@ void launch_stash_scalars(cudaStream_t s, int nv, PdhgState* st, const double* p
 }
 
 void launch_primal_shard_p2p(cudaStream_t s, int len, PdhgState* st, double* xs0, double* xs1, double* aty_s,
-                             const PeerPtrs& pp, int world, int rank, int seg_len, int pull, const double* c,
+                             const PeerPtrs& pp, int world, int rank, int seg_len, const double* c,
                              const double* lo, const double* up, double* xsum, ReduceScratch rs, double* atysum) {
   primal_shard_p2p_kernel<<<ew_grid((len + 1) / 2), kThreads, 0, s>>>(len, st, xs0, xs1, aty_s, pp, world, rank, seg_len,
-                                                                      pull, c, lo, up, xsum, rs, atysum);
-}
-void launch_push_part(cudaStream_t s, PdhgState* st, const double* part, const PeerPtrs& pp, int world, int rank, int seg_len) {
-  push_part_kernel<<<ew_grid((seg_len / 2) * world), kThreads, 0, s>>>(st, part, pp, world, rank, seg_len);
+                                                                      c, lo, up, xsum, rs, atysum);
 }
 void launch_push_shard(cudaStream_t s, const double* src, int len, const PeerPtrs& pp, int world, int rank, int seg_len,
                        const PdhgState* due) {
@@ -2182,7 +2028,7 @@ void launch_step_rule_mg(cudaStream_t s, PdhgState* st, const double* xfull, int
 
 void launch_step_rule(cudaStream_t s, PdhgState* st, ReduceScratch r1, int nb1, ReduceScratch r2, int nb2,
                       ReduceScratch r3, int nb3, const double* dy2_override) {
-  launch_k(step_rule_kernel, 1, kStepThreads, s, r1.flags, st, r1, nb1, r2, nb2, r3, nb3, dy2_override);
+  step_rule_kernel<<<1, kStepThreads, 0, s>>>(st, r1, nb1, r2, nb2, r3, nb3, dy2_override);
 }
 
 int primal_step_grid(int n) { return ew_grid((n + 1) / 2); }
@@ -2196,7 +2042,7 @@ int primal_step_grid(int n) { return ew_grid((n + 1) / 2); }
 void preload_multi_gpu_kernels() {
   const void* fns[] = {
       (const void*)primal_step_kernel, (const void*)primal_shard_kernel, (const void*)primal_shard_p2p_kernel,
-      (const void*)push_part_kernel, (const void*)push_shard_kernel, (const void*)push_rows_kernel,
+      (const void*)push_shard_kernel, (const void*)push_rows_kernel,
       (const void*)p2p_exchange_kernel, (const void*)reduce_part_p2p_kernel, (const void*)p2p_barrier_kernel,
       (const void*)stash_scalars_kernel<1>, (const void*)stash_scalars_kernel<2>, (const void*)step_rule_mg_kernel,
       (const void*)step_rule_kernel, (const void*)average_kernel, (const void*)average_dev_kernel,
@@ -2212,8 +2058,7 @@ void preload_multi_gpu_kernels() {
       (const void*)spmv_sell_kernel<DualEpilogue, false>, (const void*)spmv_sell_kernel<DualEpilogue, true>,
       (const void*)spmv_sell_kernel<PrimalEpilogue, false>, (const void*)spmv_sell_kernel<PrimalEpilogue, true>,
       (const void*)spmv_sell_kernel<DualEpilogueMg, false>, (const void*)spmv_sell_kernel<PartialAtyEpilogue, false>,
-      (const void*)spmv_sell_kernel<CheckRowEpilogue, false>, (const void*)spmv_sell_kernel<CheckColEpilogue, false>,
-      (const void*)spmv_sell_kernel<CheckRowEpilogueT<false>, false>,
+      (const void*)spmv_sell_kernel<CheckRowEpilogue, false>,
   };
   cudaFuncAttributes at;
   for (const void* f : fns) cudaFuncGetAttributes(&at, f);
@@ -2225,32 +2070,6 @@ void launch_check_avg_x(cudaStream_t s, int n, const double* x0, const double* x
                         const PdhgState* st, const SolveCtl* ctl) {
   if (n > 0) check_avg_x_kernel<<<ew_grid(n), kThreads, 0, s>>>(n, x0, x1, xsum, xavg, st, ctl);
 }
-void launch_spmv_check_rows(cudaStream_t s, const DevSell& A, const PdhgState* st, const SolveCtl* ctl, const double* xavg,
-                            const double* y0, const double* y1, const double* ax0, const double* ax1, double* ysum,
-                            double* yavg, double* axavg, const double* b, const double* rsc, int neq, ReduceScratch rs,
-                            double* axsum) {
-  if (A.nblocks_body + A.nsegs == 0) return;
-  CheckRowEpilogue e{};
-  e.st = st; e.ctl = ctl; e.xavg = xavg; e.y0 = y0; e.y1 = y1; e.ax0 = ax0; e.ax1 = ax1; e.ysum = ysum; e.yavg = yavg;
-  e.axavg = axavg; e.b = b; e.rsc = rsc; e.neq = neq; e.axsum = axsum;
-  rs.terms = nullptr; rs.flags = 0;
-  DevSell F = A;   // the check epilogues keep their sums in shared memory, which needs at most one row per thread
-  F.nblocks_body = A.nblocks_full; F.pipelined = 0; F.tiled = 0;
-  spmv_sell_kernel<CheckRowEpilogue, false><<<F.nblocks_body + F.nsegs, kThreads, 0, s>>>(F, e, rs);
-}
-void launch_spmv_check_cols(cudaStream_t s, const DevSell& AT, const PdhgState* st, const SolveCtl* ctl, const double* yavg,
-                            const double* x0, const double* x1, const double* aty0, const double* aty1, const double* xavg,
-                            double* atyavg, const double* c, const double* lo, const double* up, const double* cs,
-                            ReduceScratch rs, double* atysum) {
-  if (AT.nblocks_body + AT.nsegs == 0) return;
-  CheckColEpilogue e{};
-  e.st = st; e.ctl = ctl; e.yavg = yavg; e.x0 = x0; e.x1 = x1; e.aty0 = aty0; e.aty1 = aty1; e.xavg = xavg;
-  e.atyavg = atyavg; e.c = c; e.lo = lo; e.up = up; e.cs = cs; e.atysum = atysum;
-  rs.terms = nullptr; rs.flags = 0;
-  DevSell F = AT;
-  F.nblocks_body = AT.nblocks_full; F.pipelined = 0; F.tiled = 0;
-  spmv_sell_kernel<CheckColEpilogue, false><<<F.nblocks_body + F.nsegs, kThreads, 0, s>>>(F, e, rs);
-}
 void launch_check_decide(cudaStream_t s, PdhgState* st, SolveCtl* ctl, const double* prow, int nbr, const double* pcol,
                          int nbc, unsigned* ticket) {
   check_decide_kernel<<<kCheckSums, kDecideThreads, 0, s>>>(st, ctl, prow, nbr, pcol, nbc, ticket);
@@ -2260,7 +2079,7 @@ void launch_restart_sweep(cudaStream_t s, int n, int m, double* x0, double* x1, 
                           const double* xavg, const double* atyavg, double* xsum, double* xlr, double* y0, double* y1,
                           double* ax0, double* ax1, const double* yavg, const double* axavg, double* ysum, double* ylr,
                           const PdhgState* st, const SolveCtl* ctl, ReduceScratch rs, double* atysum, double* axsum) {
-  rs.terms = nullptr; rs.flags = 0;
+  rs.terms = nullptr;
   restart_sweep_kernel<<<restart_sweep_grid(n, m), kThreads, 0, s>>>(n, m, x0, x1, aty0, aty1, xavg, atyavg, xsum, xlr, y0,
                                                                     y1, ax0, ax1, yavg, axavg, ysum, ylr, st, ctl, rs, atysum,
                                                                     axsum);
@@ -2275,14 +2094,14 @@ void launch_check_cols_sweep(cudaStream_t s, bool given, int n, const double* x0
                              const double* aty1, double* xsum, double* atysum, double* xavg, double* atyavg, const double* c,
                              const double* lo, const double* up, const double* cs, const PdhgState* st, const SolveCtl* ctl,
                              ReduceScratch rs) {
-  rs.terms = nullptr; rs.flags = 0;
+  rs.terms = nullptr;
   if (given) check_cols_sweep_kernel<true><<<check_light_grid(n, true), kThreads, 0, s>>>(n, x0, x1, aty0, aty1, xsum, atysum, xavg, atyavg, c, lo, up, cs, st, ctl, rs);
   else check_cols_sweep_kernel<false><<<check_light_grid(n, true), kThreads, 0, s>>>(n, x0, x1, aty0, aty1, xsum, atysum, xavg, atyavg, c, lo, up, cs, st, ctl, rs);
 }
 void launch_check_rows_sweep(cudaStream_t s, bool given, int m, int neq, const double* y0, const double* y1, const double* ax0,
                              const double* ax1, double* ysum, double* axsum, double* yavg, double* axavg, const double* b,
                              const double* rsc, const PdhgState* st, const SolveCtl* ctl, ReduceScratch rs) {
-  rs.terms = nullptr; rs.flags = 0;
+  rs.terms = nullptr;
   if (given) check_rows_sweep_kernel<true><<<check_light_grid(m, false), kThreads, 0, s>>>(m, neq, y0, y1, ax0, ax1, ysum, axsum, yavg, axavg, b, rsc, st, ctl, rs);
   else check_rows_sweep_kernel<false><<<check_light_grid(m, false), kThreads, 0, s>>>(m, neq, y0, y1, ax0, ax1, ysum, axsum, yavg, axavg, b, rsc, st, ctl, rs);
 }
@@ -2299,11 +2118,11 @@ void launch_spmv_check_rows_mg(cudaStream_t s, const DevSell& A, const PdhgState
                                const double* y0, const double* y1, const double* ax0, const double* ax1, const double* yavg,
                                double* axavg, const double* b, const double* rsc, int neq, ReduceScratch rs) {
   if (A.nblocks_body + A.nsegs == 0) return;
-  CheckRowEpilogueT<false> e{};
-  e.st = st; e.ctl = ctl; e.xavg = xfull; e.y0 = y0; e.y1 = y1; e.ax0 = ax0; e.ax1 = ax1; e.ysum = nullptr;
-  e.yavg = const_cast<double*>(yavg); e.axavg = axavg; e.b = b; e.rsc = rsc; e.neq = neq;
-  rs.terms = nullptr; rs.flags = 0;
-  spmv_sell_kernel<CheckRowEpilogueT<false>><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, rs);
+  CheckRowEpilogue e{};
+  e.st = st; e.ctl = ctl; e.xavg = xfull; e.y0 = y0; e.y1 = y1; e.ax0 = ax0; e.ax1 = ax1;
+  e.yavg = yavg; e.axavg = axavg; e.b = b; e.rsc = rsc; e.neq = neq;
+  rs.terms = nullptr;
+  spmv_sell_kernel<CheckRowEpilogue><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, rs);
 }
 void launch_reduce_partials(cudaStream_t s, const PdhgState* st, const SolveCtl* ctl, int nacc, const double* partials, int nb,
                             double* out, int flag_slot, int need_restart, int nacc2, const double* partials2, int nb2,
@@ -2457,7 +2276,7 @@ void launch_hip_dual(cudaStream_t s, const DevSell& A, const HipState* st, int k
   e.yn = yn; e.ry = ry;
   // the launch shape the engine chose for A (apply_spmv_grid): a persistent grid must take the pipelined walk, which visits
   // every slice; the one-slice-per-warp kernel on that capped grid would skip slices
-  const ReduceScratch none{nullptr, nullptr, nullptr, 0, 0};
+  const ReduceScratch none{nullptr, nullptr, nullptr, 0};
   if (A.tiled) { launch_tile(s, A, e, none); return; }
   if (A.pipelined) spmv_sell_kernel<HipDualEpilogue, true><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, none);
   else spmv_sell_kernel<HipDualEpilogue, false><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, none);
@@ -2708,7 +2527,7 @@ void launch_hip_dual_shard(cudaStream_t s, const DevSell& A, const HipState* st,
   HipDualShardEpilogue e{};
   e.st = st; e.k_offset = k_offset; e.is_major = is_major; e.in = rx; e.y = y; e.ya = ya; e.rlo = rlo; e.rup = rup;
   e.yn = yn; e.ry = ry; e.y_peers = y_peers; e.world = world; e.rank = rank;
-  const ReduceScratch none{nullptr, nullptr, nullptr, 0, 0};
+  const ReduceScratch none{nullptr, nullptr, nullptr, 0};
   spmv_sell_kernel<HipDualShardEpilogue, false><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, none);
 }
 void launch_hip_gather(cudaStream_t s, const HipGather& g, int world, int rank) {

@@ -16,8 +16,7 @@ void launch_spmv_dual(cudaStream_t s, const DevSell& A, PdhgState* st, const dou
                       int neq, int row_offset, ReduceScratch rs, double* axsum = nullptr);
 void launch_spmv_primal(cudaStream_t s, const DevSell& A, PdhgState* st, const double* y0, const double* y1,
                         const double* x0, const double* x1, double* aty0, double* aty1, ReduceScratch rs,
-                        double* atysum = nullptr, const double* k1_partials = nullptr, int nb1 = 0,
-                        const double* k2_partials = nullptr, int nb2 = 0 /* non-null: the last CTA also applies the step rule */);
+                        double* atysum = nullptr);
 void launch_spmv_partial_aty(cudaStream_t s, const DevSell& A, PdhgState* st, const double* y0, const double* y1,
                              double* part, const int* outpos, const PdhgState* due = nullptr);
 void launch_spmv_dual_mg(cudaStream_t s, const DevSell& A, PdhgState* st, const double* xfull, double* y0, double* y1,
@@ -31,7 +30,7 @@ int primal_shard_p2p_grid(int len);
 void launch_stash_scalars(cudaStream_t s, int nv, PdhgState* st, const double* partials, int nb, double* dst, int copies,
                           int stride);
 void launch_primal_shard_p2p(cudaStream_t s, int len, PdhgState* st, double* xs0, double* xs1, double* aty_s,
-                             const PeerPtrs& pp, int world, int rank, int seg_len, int pull, const double* c,
+                             const PeerPtrs& pp, int world, int rank, int seg_len, const double* c,
                              const double* lo, const double* up, double* xsum, ReduceScratch rs, double* atysum = nullptr);
 void launch_push_shard(cudaStream_t s, const double* src, int len, const PeerPtrs& pp, int world, int rank, int seg_len,
                        const PdhgState* due = nullptr);
@@ -39,7 +38,7 @@ void launch_push_rows(cudaStream_t s, const double* src, int len, const PeerPtrs
 void launch_p2p_exchange(cudaStream_t s, double* vals, int k, const PeerPtrs& pp, int world, int rank,
                          unsigned long long* epochs, int* fault, const PdhgState* due = nullptr,
                          const SolveCtl* only_if_restart = nullptr /* skip (on every rank alike) unless the check chose a restart */);
-void launch_push_part(cudaStream_t s, PdhgState* st, const double* part, const PeerPtrs& pp, int world, int rank, int seg_len);
+// pull 1: add the peers' `part` segments (a pass's partial A_g^T y'); 2: their `recv` (a check's partial A_g^T ybar)
 void launch_reduce_part_p2p(cudaStream_t s, int len, double* dst, const PeerPtrs& pp, int world, int rank, int seg_len,
                             int pull, const PdhgState* due = nullptr, int only_if_accepted = 0);
 void launch_p2p_barrier(cudaStream_t s, int mode, PdhgState* st, const double* partials, int nb, const PeerPtrs& pp,
@@ -78,14 +77,6 @@ void launch_fill(cudaStream_t s, int len, double* v, double w);
 // ---- device-side check iteration (tree mode, one GPU): see pdhg_kernels.cu "device-side check iteration"
 void launch_check_avg_x(cudaStream_t s, int n, const double* x0, const double* x1, double* xsum, double* xavg,
                         const PdhgState* st, const SolveCtl* ctl);
-void launch_spmv_check_rows(cudaStream_t s, const DevSell& A, const PdhgState* st, const SolveCtl* ctl, const double* xavg,
-                            const double* y0, const double* y1, const double* ax0, const double* ax1, double* ysum,
-                            double* yavg, double* axavg, const double* b, const double* rsc, int neq, ReduceScratch rs,
-                            double* axsum = nullptr);
-void launch_spmv_check_cols(cudaStream_t s, const DevSell& AT, const PdhgState* st, const SolveCtl* ctl, const double* yavg,
-                            const double* x0, const double* x1, const double* aty0, const double* aty1, const double* xavg,
-                            double* atyavg, const double* c, const double* lo, const double* up, const double* cs,
-                            ReduceScratch rs, double* atysum = nullptr);
 void launch_check_decide(cudaStream_t s, PdhgState* st, SolveCtl* ctl, const double* prow, int nbr, const double* pcol,
                          int nbc, unsigned* ticket /* zero-initialised, self-resetting */);
 int restart_sweep_grid(int n, int m);

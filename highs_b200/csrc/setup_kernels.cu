@@ -1,4 +1,4 @@
-// highs_b200/csrc/setup_kernels.cu -- PDHG_Scale_Data on the device (opt-in: params.device_scaling).
+// highs_b200/csrc/setup_kernels.cu -- PDHG_Scale_Data on the device (the scaling stage of device_prep.cu).
 //
 // What cupdlp_scaling.c:47-120 (10 Ruiz passes), :174-231 (Pock-Chambolle, alpha = 1) and :17-45
 // (scale_problem) do in 44 host sweeps over the nonzeros, on the column-major matrix resident in HBM:
@@ -10,13 +10,13 @@
 //     order; a row's entries with the columns ascending).  One warp per column / row: the lanes load 32
 //     entries at once, then every lane adds the 32 values in index order (shuffle broadcast), so the
 //     loads are parallel and the additions sequential.  Rows go through the row-major index of the
-//     nonzeros (rptr / rpos), which the host builds while the Ruiz passes run.
+//     nonzeros (rptr / rpos).
 //   * sqrt and division are IEEE-correctly rounded on the device as on the host (nvcc defaults
 //     -prec-sqrt=true -prec-div=true; the file is compiled with -fmad=false like the rest), so the scaled
 //     data are bit-identical to host_prep.cpp::scale and to the reference.
 //
-// STATUS (round 2): runs on hardware -- as the staged variants (device_scaling = 1, 2; tests/test_gpu_device_scaling.py compares
-// them bit for bit with the host path) and as the scaling stage of the device prologue (device_prep.cu, the default).
+// STATUS: runs on hardware as the scaling stage of the device prologue (device_prep.cu, the default;
+// tests/test_gpu_device_prep.py compares it bit for bit with the host path).
 #include "setup_kernels.hpp"
 #include "kernels.cuh"
 
@@ -29,13 +29,6 @@ constexpr int kTpb = 256;
 
 __device__ __forceinline__ void atomic_max_nonneg(double* addr, double v) {
   atomicMax(reinterpret_cast<unsigned long long*>(addr), (unsigned long long)__double_as_longlong(v));
-}
-
-// colof[p] = column of nonzero p (one warp per column; a dense column is written 32 entries at a time)
-__global__ void __launch_bounds__(kTpb) colof_kernel(int n, const int* __restrict__ cbeg, int* __restrict__ colof) {
-  const int j = (blockIdx.x * kTpb + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (j >= n) return;
-  for (int p = cbeg[j] + lane; p < cbeg[j + 1]; p += 32) colof[p] = j;
 }
 
 // norms of the first Ruiz pass: max |a_ij| per column and per row
@@ -300,8 +293,7 @@ void device_abs_max(cudaStream_t s, int nnz, const double* val, double* amax) {
   if (nnz > 0) abs_max_kernel<<<grid_for(nnz), kTpb, 0, s>>>(nnz, val, amax);
 }
 
-void device_scale_ruiz(cudaStream_t s, const DevForm& F, DevScaleScratch& w, bool have_colof) {
-  if (F.n > 0 && !have_colof) colof_kernel<<<warp_grid(F.n), kTpb, 0, s>>>(F.n, F.cbeg, F.colof);
+void device_scale_ruiz(cudaStream_t s, const DevForm& F, DevScaleScratch& w) {
   cudaMemsetAsync(w.cnorm, 0, sizeof(double) * (size_t)(F.n > 0 ? F.n : 1), s);
   cudaMemsetAsync(w.rnorm, 0, sizeof(double) * (size_t)(F.m > 0 ? F.m : 1), s);
   if (F.nnz > 0) first_norms_kernel<<<grid_for(F.nnz), kTpb, 0, s>>>(F.nnz, F.cidx, F.colof, F.cval, w.cnorm, w.rnorm);

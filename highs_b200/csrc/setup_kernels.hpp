@@ -9,7 +9,7 @@ struct DevForm {
   int n, m, nnz;
   const int* cbeg;   // [n+1]
   const int* cidx;   // [nnz] row of each nonzero
-  int* colof;        // [nnz] column of each nonzero (filled by device_scale_ruiz)
+  int* colof;        // [nnz] column of each nonzero
   double* cval;      // [nnz] scaled in place
   double *cost, *lower, *upper, *colscale;   // [n]
   double *rhs, *rowscale;                    // [m]
@@ -20,9 +20,8 @@ struct DevScaleScratch {
   double* amax;         // [1] max |a_ij| of the scaled matrix
 };
 
-// the 10 Ruiz passes (cupdlp_scaling.c:47-120); needs nothing but the column-major matrix
-// have_colof: F.colof is filled already
-void device_scale_ruiz(cudaStream_t s, const DevForm& F, DevScaleScratch& w, bool have_colof = false);
+// the 10 Ruiz passes (cupdlp_scaling.c:47-120); needs nothing but the column-major matrix (and its colof)
+void device_scale_ruiz(cudaStream_t s, const DevForm& F, DevScaleScratch& w);
 // *amax = max |val[p]|
 void device_abs_max(cudaStream_t s, int nnz, const double* val, double* amax);
 // the Pock-Chambolle pass (:174-231); rptr[m+1] / rpos[nnz] = device copy of the row-major index of the nonzeros

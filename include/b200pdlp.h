@@ -79,8 +79,8 @@ typedef struct {
   int32_t ordered_max;       /* problems with max(cols,rows) <= this reduce in the reference's
                                 sequential order (bit-identical trajectories); 0 -> 4096, <0 -> off */
   int32_t device_scaling;    /* where the prologue (formulate, scaling, transposition, layouts) runs: 0 = on the device for one
-                                GPU in tree mode (device_prep.cu; host threads otherwise), -1 = always host threads,
-                                1 / 2 = round-1 staged variants (host formulate + device scaling [+ device ELL fill]) */
+                                GPU in tree mode (device_prep.cu; host threads otherwise), -1 = always host threads;
+                                any other value is rejected (B200PDLP_ERR_ARG) */
   int32_t reserved[2];
 } b200pdlp_params;
 

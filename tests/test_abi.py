@@ -73,6 +73,9 @@ def test_bad_arguments(engine_lib):
     lp.sense_ = 3
     with pytest.raises(engine.EngineError, match="sense"):
         engine.host_form(lp)
+    # checked with the other arguments, before any device is looked for
+    with pytest.raises(engine.EngineError, match="device_scaling"):
+        engine.solve(synthetic_lp(50, 40, 3, 1), device_scaling=2)
 
 
 def test_product_does_not_touch_oracle():

@@ -30,8 +30,7 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 _SHAPE_ENV = ("B200PDLP_TILE", "B200PDLP_TILE_A", "B200PDLP_TILE_AT", "B200PDLP_TILE_FORCE", "B200PDLP_SPMV_CTAS_PER_SM",
-              "B200PDLP_SPMV_A_CTAS_PER_SM", "B200PDLP_SPMV_AT_CTAS_PER_SM", "B200PDLP_FUSE_K4", "B200PDLP_PDL",
-              "B200PDLP_DEVICE_PREP", "B200PDLP_TIMING")
+              "B200PDLP_SPMV_A_CTAS_PER_SM", "B200PDLP_SPMV_AT_CTAS_PER_SM", "B200PDLP_DEVICE_PREP", "B200PDLP_TIMING")
 # arm -> (environment, shape the engine must report for A and A')
 SHAPES = {
     "one_slice_per_warp": ({"B200PDLP_TILE": "0", "B200PDLP_SPMV_CTAS_PER_SM": "0"}, "one slice per warp"),

@@ -31,7 +31,7 @@ REL_TRACE = 1e-6       # trajectories under different shapes: the block partial 
 TRACE_UNTIL = {"ragged": 40}
 
 _ENV = ("B200PDLP_TILE", "B200PDLP_TILE_A", "B200PDLP_TILE_AT", "B200PDLP_TILE_FORCE", "B200PDLP_SPMV_CTAS_PER_SM",
-        "B200PDLP_SPMV_A_CTAS_PER_SM", "B200PDLP_SPMV_AT_CTAS_PER_SM", "B200PDLP_FUSE_K4", "B200PDLP_PDL")
+        "B200PDLP_SPMV_A_CTAS_PER_SM", "B200PDLP_SPMV_AT_CTAS_PER_SM")
 
 # arm -> (environment, shape the engine must report, CTAs per SM of the persistent grid)
 ARMS = {
@@ -41,9 +41,6 @@ ARMS = {
                       "persistent", 1),
     "persistent_k2": ({"B200PDLP_TILE": "0", "B200PDLP_SPMV_A_CTAS_PER_SM": "2", "B200PDLP_SPMV_AT_CTAS_PER_SM": "2"},
                       "persistent", 2),
-    # the fused step rule: K3's last CTA runs the PrimalEpilogue tail
-    "persistent_k1_fused_k4": ({"B200PDLP_TILE": "0", "B200PDLP_SPMV_A_CTAS_PER_SM": "1", "B200PDLP_SPMV_AT_CTAS_PER_SM": "1",
-                                "B200PDLP_FUSE_K4": "1"}, "persistent", 1),
     "tiled_bulk_copy": ({"B200PDLP_TILE": "1", "B200PDLP_TILE_FORCE": "1", "B200PDLP_SPMV_A_CTAS_PER_SM": "0",
                          "B200PDLP_SPMV_AT_CTAS_PER_SM": "0"}, "tiled", 0),
     "tiled_cooperative_loads": ({"B200PDLP_TILE": "2", "B200PDLP_TILE_FORCE": "1", "B200PDLP_SPMV_A_CTAS_PER_SM": "0",
@@ -184,13 +181,11 @@ def _family(name, sms):
     raise KeyError(name)
 
 
-_ALL = tuple(ARMS)
-_NO_TILE = ("default", "persistent_k1", "persistent_k2", "persistent_k1_fused_k4")
 FAMILIES = {
-    "ragged": _NO_TILE,                         # random patterns: no window fits, the tiled shape is never chosen
-    "random": _NO_TILE,
-    "banded_staged": _ALL,
-    "banded_mixed": _ALL,
+    "ragged": ("default", "persistent_k1", "persistent_k2"),   # random patterns: no window fits, the tiled shape is never chosen
+    "random": ("default", "persistent_k1", "persistent_k2"),
+    "banded_staged": tuple(ARMS),
+    "banded_mixed": tuple(ARMS),
     "banded_synthetic": ("default", "tiled_bulk_copy", "tiled_cooperative_loads"),   # (too few rows for a persistent grid)
 }
 
