@@ -484,6 +484,30 @@ __global__ void long_plan_kernel(int nlong, const int* __restrict__ list, const 
   totals[1] = lpos + 8;
 }
 
+// ---- HiPDLP mode on several GPUs: nnz-balanced contiguous blocks of a device order (host twin: balanced_blocks).
+// w[i] = length of the i-th row in `perm` order + 5 (a per-row cost, as partition_rows charges), w[count] = 0; its exclusive
+// scan is the host's prefix array pre[0 .. count].
+__global__ void __launch_bounds__(kTpb)
+block_weight_kernel(int count, const int* __restrict__ perm, const int* __restrict__ ptr, long long* __restrict__ w) {
+  const int stride = gridDim.x * kTpb;
+  for (int i = blockIdx.x * kTpb + threadIdx.x; i <= count; i += stride)
+    w[i] = i < count ? (long long)(ptr[perm[i] + 1] - ptr[perm[i]]) + 5 : 0;
+}
+// b[0] = 0, b[world] = count, b[g] = min(lower_bound(pre[0 .. count], pre[count] g / world), count): one thread per g.  The
+// host searches from b[g-1]; every pre[i] before it is < the previous target <= this one, so the whole range gives the same.
+__global__ void block_bounds_kernel(int count, int world, const long long* __restrict__ pre, int* __restrict__ b) {
+  const int g = threadIdx.x;
+  if (g > world) return;
+  if (g == 0 || g == world) { b[g] = g == 0 ? 0 : count; return; }
+  const long long target = pre[count] * g / world;
+  int lo = 0, hi = count + 1;   // first i in [0, count] with pre[i] >= target (count + 1 if none)
+  while (lo < hi) {
+    const int mid = lo + (hi - lo) / 2;
+    if (pre[mid] < target) lo = mid + 1; else hi = mid;
+  }
+  b[g] = lo < count ? lo : count;
+}
+
 // ---- HiPDLP mode: entries of a column ordered by (new row, value), as std::sort of (row, value) pairs (pdhg.cc:300-333).
 // Columns stored with strictly ascending rows need nothing beyond the stable eq-like partition (the renumbering is
 // monotone inside each group); otherwise an LSD radix sort: first by value, then (stably) by (column, new row).
@@ -897,12 +921,31 @@ void DevicePrologue::run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, i
   arr.cperm = keep<int>(n); arr.cinv = keep<int>(n);
   make_perm_device(s, tmp, m, neq, rptr, arr.rperm, arr.rinv);
   make_perm_device(s, tmp, n, n, cbeg, arr.cperm, arr.cinv);
+  // HiPDLP mode on several GPUs: the partition of both device orders into `world` blocks (read-back 1b)
+  const bool blocks = world > 1;
+  if (blocks) {
+    int* bnd = tmp.get<int>(2 * (world + 1));
+    auto partition = [&](int count, const int* perm, const int* ptr, int* b) {
+      long long* w = tmp.get<long long>(count + 1);
+      long long* pre = tmp.get<long long>(count + 1);
+      block_weight_kernel<<<grid_for(count + 1), kTpb, 0, s>>>(count, perm, ptr, w);
+      exclusive_scan_ll(s, tmp, w, pre, count + 1);
+      block_bounds_kernel<<<1, 32, 0, s>>>(count, world, pre, b);
+    };
+    partition(m, arr.rperm, rptr, bnd);
+    partition(n, arr.cperm, cbeg, bnd + world + 1);
+    std::vector<int> hb((size_t)2 * (world + 1));
+    PREP_OK(cudaMemcpyAsync(hb.data(), bnd, hb.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+    PREP_OK(cudaStreamSynchronize(s));
+    rb.assign(hb.begin(), hb.begin() + world + 1);
+    cb.assign(hb.begin() + world + 1, hb.end());
+  }
   struct Plan {
     int nrows = 0, nslices = 0;
     int *slice_len = nullptr; unsigned* slice_mask = nullptr; long long *slots = nullptr, *slot_ex = nullptr;
     int *long_flag = nullptr, *long_list = nullptr, *nlong_dev = nullptr;
     long long* totals = nullptr;
-  } pa, pat;
+  };
   int* too_big = flags + 2;
   auto plan1 = [&](Plan& P, int nrows, const int* perm, const int* ptr) {
     P.nrows = nrows; P.nslices = (nrows + 31) / 32;
@@ -925,34 +968,62 @@ void DevicePrologue::run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, i
       PREP_OK(cudaMemsetAsync(P.slot_ex, 0, sizeof(long long), s));
     }
   };
-  plan1(pa, m, arr.rperm, rptr);
-  plan1(pat, n, arr.cperm, cbeg);
-  // read-back 2: sizes of the layouts
-  struct { long long a_slots, at_slots; int a_nlong, at_nlong; } hb;
-  memset(&hb, 0, sizeof(hb));
-  if (!stop_after_scaling) {
-    PREP_OK(cudaMemcpyAsync(&hb.a_slots, pa.slot_ex + pa.nslices, sizeof(long long), cudaMemcpyDeviceToHost, s));
-    PREP_OK(cudaMemcpyAsync(&hb.at_slots, pat.slot_ex + pat.nslices, sizeof(long long), cudaMemcpyDeviceToHost, s));
-    PREP_OK(cudaMemcpyAsync(&hb.a_nlong, pa.nlong_dev, sizeof(int), cudaMemcpyDeviceToHost, s));
-    PREP_OK(cudaMemcpyAsync(&hb.at_nlong, pat.nlong_dev, sizeof(int), cudaMemcpyDeviceToHost, s));
-    PREP_OK(cudaStreamSynchronize(s));
+  // One job per sliced-ELL matrix: rows perm[0 .. nrows) of a device order (perm = the order + the block's first row), their
+  // entries read from `src`.  One GPU: A and A'.  Block mode: A_g and A_g' of every rank on this device.
+  SellSource SA{rptr, rptr + 1, rpos, colof, cval, 0, arr.cinv};
+  SellSource SAT{cbeg, cbeg + 1, cpos, cidx, cval, 0, arr.rinv};
+  if (cpos) {
+    // cpos lists ALL positions ordered by (column, row): column j's entries are cpos[cbeg[j] .. cbeg[j+1]) since every
+    // column keeps its range
+    SAT.pos = cpos;
   }
-  sc.a_padded = hb.a_slots; sc.at_padded = hb.at_slots; sc.a_nlong = hb.a_nlong; sc.at_nlong = hb.at_nlong;
-  if (sc.a_padded > 2000000000LL || sc.at_padded > 2000000000LL)
-    throw std::runtime_error("b200pdlp: matrix too large for 32-bit slice offsets");
+  struct Job {
+    DevSellOwned* M; int nrows, ncols; const int* perm; const int* ptr; const SellSource* src;
+    Plan P; long long padded = 0, lcount = 8; int nlong = 0, nsegs = 0;
+  };
+  std::vector<Job> jobs;
+  if (blocks) {
+    block_A.assign(ranks.size(), DevSellOwned());
+    block_AT.assign(ranks.size(), DevSellOwned());
+    for (size_t k = 0; k < ranks.size(); k++) {
+      const int g = ranks[k];
+      jobs.push_back(Job{&block_A[k], rb[g + 1] - rb[g], n, arr.rperm + rb[g], rptr, &SA});
+      jobs.push_back(Job{&block_AT[k], cb[g + 1] - cb[g], m, arr.cperm + cb[g], cbeg, &SAT});
+    }
+  } else {
+    jobs.push_back(Job{&A, m, n, arr.rperm, rptr, &SA});
+    jobs.push_back(Job{&AT, n, m, arr.cperm, cbeg, &SAT});
+  }
+  for (Job& J : jobs) plan1(J.P, J.nrows, J.perm, J.ptr);
+  // read-back 2: sizes of the layouts (padded slots, long rows)
+  std::vector<long long> hsz(2 * jobs.size(), 0);
+  for (size_t k = 0; k < jobs.size(); k++) {
+    PREP_OK(cudaMemcpyAsync(&hsz[2 * k], jobs[k].P.slot_ex + jobs[k].P.nslices, sizeof(long long), cudaMemcpyDeviceToHost, s));
+    PREP_OK(cudaMemcpyAsync(&hsz[2 * k + 1], jobs[k].P.nlong_dev, sizeof(int), cudaMemcpyDeviceToHost, s));
+  }
+  PREP_OK(cudaStreamSynchronize(s));
+  for (size_t k = 0; k < jobs.size(); k++) {
+    jobs[k].padded = hsz[2 * k];
+    jobs[k].nlong = (int)hsz[2 * k + 1];
+    if (jobs[k].padded > 2000000000LL) throw std::runtime_error("b200pdlp: matrix too large for 32-bit slice offsets");
+  }
   // long rows: count the segments first (sizes), then write the descriptors
   auto long_sizes = [&](Plan& P, int nlong, const int* perm, const int* ptr) {
     long_plan_kernel<<<1, 32, 0, s>>>(nlong, P.long_list, perm, ptr, nullptr, nullptr, P.totals, 0);
   };
-  long_sizes(pa, sc.a_nlong, arr.rperm, rptr);
-  long_sizes(pat, sc.at_nlong, arr.cperm, cbeg);
-  long long ht[4] = {0, 8, 0, 8};
-  PREP_OK(cudaMemcpyAsync(&ht[0], pa.totals, 2 * sizeof(long long), cudaMemcpyDeviceToHost, s));
-  PREP_OK(cudaMemcpyAsync(&ht[2], pat.totals, 2 * sizeof(long long), cudaMemcpyDeviceToHost, s));
+  for (Job& J : jobs) long_sizes(J.P, J.nlong, J.perm, J.ptr);
+  for (size_t k = 0; k < jobs.size(); k++)
+    PREP_OK(cudaMemcpyAsync(&hsz[2 * k], jobs[k].P.totals, 2 * sizeof(long long), cudaMemcpyDeviceToHost, s));
   PREP_OK(cudaStreamSynchronize(s));
-  sc.a_nsegs = (int)ht[0]; sc.a_lcount = ht[1]; sc.at_nsegs = (int)ht[2]; sc.at_lcount = ht[3];
-  if (sc.a_lcount > 2000000000LL || sc.at_lcount > 2000000000LL)
-    throw std::runtime_error("b200pdlp: long rows too large for 32-bit offsets");
+  for (size_t k = 0; k < jobs.size(); k++) {
+    jobs[k].nsegs = (int)hsz[2 * k];
+    jobs[k].lcount = hsz[2 * k + 1];
+    if (jobs[k].lcount > 2000000000LL) throw std::runtime_error("b200pdlp: long rows too large for 32-bit offsets");
+  }
+  if (!blocks) {
+    sc.a_padded = jobs[0].padded; sc.a_nlong = jobs[0].nlong; sc.a_nsegs = jobs[0].nsegs; sc.a_lcount = jobs[0].lcount;
+    sc.at_padded = jobs[1].padded; sc.at_nlong = jobs[1].nlong; sc.at_nsegs = jobs[1].nsegs; sc.at_lcount = jobs[1].lcount;
+  }
 
   if (hip) values_and_scaling_hip();
   else values_and_scaling();
@@ -979,15 +1050,7 @@ void DevicePrologue::run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, i
     if (nlong > 0) long_plan_kernel<<<1, 32, 0, s>>>(nlong, P.long_list, perm, ptr, M.long_rows, M.segs, P.totals, 1);
     device_fill_sell(s, nrows, P.nslices, M.slices, perm, S, M.col, M.val, padded, nlong, M.long_rows, M.segs, M.lcol, M.lval);
   };
-  SellSource SA{rptr, rptr + 1, rpos, colof, cval, 0, arr.cinv};
-  SellSource SAT{cbeg, cbeg + 1, cpos, cidx, cval, 0, arr.rinv};
-  if (cpos) {
-    // cpos lists ALL positions ordered by (column, row): column j's entries are cpos[cbeg[j] .. cbeg[j+1]) since every
-    // column keeps its range
-    SAT.pos = cpos;
-  }
-  build(A, pa, m, n, sc.a_padded, sc.a_nlong, sc.a_nsegs, sc.a_lcount, arr.rperm, rptr, SA);
-  build(AT, pat, n, m, sc.at_padded, sc.at_nlong, sc.at_nsegs, sc.at_lcount, arr.cperm, cbeg, SAT);
+  for (Job& J : jobs) build(*J.M, J.P, J.nrows, J.ncols, J.padded, J.nlong, J.nsegs, J.lcount, J.perm, J.ptr, *J.src);
   int* sect = tmp.get<int>(4);
   PREP_OK(cudaMemsetAsync(sect, 0, 4 * sizeof(int), s));
   auto sample = [&](const DevSellOwned& M, int* out) {
@@ -995,8 +1058,10 @@ void DevicePrologue::run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, i
     const int step = std::max(1, M.nslices / 4096), nw = (M.nslices + step - 1) / step;
     sector_sharing_kernel<<<warp_grid(nw), kTpb, 0, s>>>(M.nslices, step, M.slices, M.col, out);
   };
-  sample(A, sect);
-  sample(AT, sect + 2);
+  if (!blocks) {   // (the shards run one slice per warp: no sampling, no tile windows)
+    sample(A, sect);
+    sample(AT, sect + 2);
+  }
   // tile windows for the shared-memory staged shape (decided by the engine from tiles_staged / ntiles)
   int* fit = tmp.get<int>(2);
   PREP_OK(cudaMemsetAsync(fit, 0, 2 * sizeof(int), s));
@@ -1007,8 +1072,10 @@ void DevicePrologue::run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, i
     M.tile_w = keep<int>(M.ntiles);
     tile_window_kernel<<<M.ntiles, kTpb, 0, s>>>(M.nslices, M.ncols, M.slices, M.col, M.val, M.tile_lo, M.tile_w, fit_out);
   };
-  windows(A, fit);
-  windows(AT, fit + 1);
+  if (!blocks) {
+    windows(A, fit);
+    windows(AT, fit + 1);
+  }
 
   // ---- vectors in device order
   arr.cost = keep<double>(n); arr.lower = keep<double>(n); arr.upper = keep<double>(n); arr.colscale = keep<double>(n);
@@ -1240,6 +1307,13 @@ void DevicePrologue::release_form() {
   dev_cache_free(form.rowscale); dev_cache_free(form.rptr); dev_cache_free(form.rpos); dev_cache_free(form.rcol);
   dev_cache_free(form.row_upper);
   form = DevStdForm();
+}
+
+void DevicePrologue::release_blocks() {
+  for (DevSellOwned& M : block_A) M.release();
+  for (DevSellOwned& M : block_AT) M.release();
+  block_A.clear();
+  block_AT.clear();
 }
 
 void DevicePrologue::release_arrays() {

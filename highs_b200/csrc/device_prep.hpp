@@ -5,13 +5,14 @@
 // (highs/pdlp/cupdlp/cupdlp_scaling.c:233-425), csc2csr (cupdlp_utils.c:1222-1254) -- and what host_prep.cpp does for
 // the engine on host threads (its tested twin: same arithmetic, same orders), here as kernels over the caller's
 // HighsLp arrays copied once to HBM.  The host touches O(1) data: three small read-backs (sizes of the standard form,
-// sizes of the layouts + scalars, long-row totals).  Scans, stable radix sorts and the stream compaction come from CUB
+// sizes of the layouts + scalars, long-row totals; block mode adds the partition's 2 (world + 1) offsets).  Scans, stable radix sorts and the stream compaction come from CUB
 // (part of the CUDA toolkit); everything that computes is a kernel of device_prep.cu / setup_kernels.cu.
 #pragma once
 #include <cuda_runtime.h>
 
 #include <cstddef>
 #include <cstdint>
+#include <vector>
 
 #include "../../include/b200pdlp.h"
 #include "kernels.cuh"
@@ -103,12 +104,22 @@ struct DevicePrologue {
   // layouts; `do_scale` is then ignored in favour of scaling_mode (bits 1 Ruiz, 4 Pock-Chambolle, 2 L2) / ruiz_iterations
   bool hipdlp = false;
   int scaling_mode = 0, ruiz_iterations = 0;
+  // Block mode (HiPDLP mode on several GPUs, world > 1): the HiPDLP front and the one-GPU orderings as above, then the
+  // nnz-balanced partition of the device rows and columns into `world` contiguous blocks (host twin: balanced_blocks in
+  // host_prep.cpp) and, for every rank in `ranks`, A_g (device rows [rb[g], rb[g+1]), columns through cinv) and A_g'
+  // (device columns [cb[g], cb[g+1]), columns through rinv) -- what build_hipdlp_shard builds on the host.  The one-GPU A / A',
+  // the sector sampling and the tile windows are not built.  block_A[k] / block_AT[k] belong to rank ranks[k].
+  int world = 1;
+  std::vector<int> ranks;
+  std::vector<int> rb, cb;                        // world + 1 block offsets each (read back)
+  std::vector<DevSellOwned> block_A, block_AT;
   size_t h2d_bytes = 0;
   // formulate + scale + row index + orderings + sliced-ELL layouts, all on stream `s`; returns with the stream idle.
   // Throws std::exception on bad input / CUDA errors (the caller releases what was produced so far).
   void run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, int long_threshold);
   void release_arrays();
   void release_form();
+  void release_blocks();   // whatever block_A / block_AT still own
 };
 
 // solve boundary for a device-resident problem: initial point (hot start / proj(0), start of the running sums) and

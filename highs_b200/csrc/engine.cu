@@ -2058,6 +2058,90 @@ static void create_problem_hipdlp_shard(const StdForm& f, const HipShards& S, in
   CUDA_OK(cudaDeviceSynchronize());
 }
 
+// The same problems from the device prologue in block mode (DevicePrologue::world > 1): one prologue per device, shared by
+// the ranks that live there.  What no problem adopted is released when the holder goes.
+struct ShardPrologue {
+  int device = 0;
+  cudaStream_t stream = nullptr;
+  DevicePrologue P;
+  ShardPrologue() = default;
+  ShardPrologue(const ShardPrologue&) = delete;
+  ShardPrologue& operator=(const ShardPrologue&) = delete;
+  ~ShardPrologue() {
+    if (stream) { cudaSetDevice(device); cudaStreamSynchronize(stream); cudaStreamDestroy(stream); }
+    P.release_blocks(); P.release_arrays(); P.release_form();
+  }
+};
+
+// formulate, scaling, orderings, the partition and A_g / A_g' of `ranks` on `device`; returns with the stream idle
+static void run_hipdlp_shard_prologue(const b200pdlp_lp& lp, int scaling_mode, int ruiz_iterations, int world, int device,
+                                      const std::vector<int>& ranks, ShardPrologue& SP) {
+  SP.device = device;
+  CUDA_OK(cudaSetDevice(device));
+  CUDA_OK(cudaStreamCreateWithFlags(&SP.stream, cudaStreamNonBlocking));
+  DevicePrologue& P = SP.P;
+  P.hipdlp = true;
+  P.scaling_mode = scaling_mode;
+  P.ruiz_iterations = ruiz_iterations;
+  P.world = world;
+  P.ranks = ranks;
+  try {
+    P.run(SP.stream, lp, true, /*long_threshold=*/512);
+  } catch (const std::invalid_argument& ex) {
+    throw Error(B200PDLP_ERR_ARG, ex.what());
+  } catch (const std::runtime_error& ex) {
+    throw Error(B200PDLP_ERR_CUDA, ex.what());
+  }
+}
+
+// rank P.ranks[k]'s problem: it adopts its A_g / A_g' and takes its own copies of the full-length device-order vectors
+static void create_problem_hipdlp_shard_device(const b200pdlp_lp& lp, ShardPrologue& SP, int k, b200pdlp_problem* p) {
+  DevicePrologue& P = SP.P;
+  const int g = P.ranks[k];
+  p->device = SP.device;
+  set_device(p);
+  p->rank = g; p->world = P.world;
+  p->dev_form = true;
+  StdForm& f = p->form;   // the scalars hip_form_scalars gives the host path's ranks
+  f = StdForm();
+  f.hipdlp = true; f.scaled = P.sc.scaled != 0;
+  f.n = P.arr.n; f.m = P.arr.m; f.nnz = P.arr.nnz; f.neq = P.arr.neq; f.n_orig = P.arr.n0;
+  f.sense = lp.sense; f.offset = lp.offset;
+  f.norm_cost = std::sqrt(P.sc.norm_cost_sq); f.norm_rhs = std::sqrt(P.sc.norm_rhs_sq);
+  f.amax = P.sc.amax;
+  const int n = f.n, m = f.m;
+  p->n = n; p->m = m; p->ml = m; p->r0 = 0; p->r1 = m; p->neq_local = f.neq; p->ordered = false;
+  p->nl = p->nl_real = n; p->c0 = 0; p->shard_len = n; p->seg_len = n;
+  p->hip_r0 = P.rb[g]; p->hip_r1 = P.rb[g + 1]; p->hip_c0 = P.cb[g]; p->hip_c1 = P.cb[g + 1];
+  CUDA_OK(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
+  adopt_matrix(p->A, P.block_A[k]);
+  adopt_matrix(p->AT, P.block_AT[k]);
+  auto dup = [&](DevBuf<double>& d, const double* src, int len) {
+    d.alloc(len, false);
+    if (len > 0) CUDA_OK(cudaMemcpyAsync(d.p, src, (size_t)len * sizeof(double), cudaMemcpyDeviceToDevice, p->stream));
+  };
+  dup(p->cost, P.arr.cost, n); dup(p->lower, P.arr.lower, n); dup(p->upper, P.arr.upper, n); dup(p->colscale, P.arr.colscale, n);
+  dup(p->rhs, P.arr.rhs, m); dup(p->hip.rup, P.arr.rup, m); dup(p->rowscale, P.arr.rowscale, m);
+  hipdlp_buffers(p);
+  p->flags.alloc(kMaxPeers);
+  p->epochs.alloc(1);
+  p->fault.alloc(1);
+  if (g == 0) {   // the postsolve's staging
+    p->io_col.alloc((size_t)2 * std::max(f.n_orig, 1), false);
+    p->io_row.alloc((size_t)2 * std::max(m, 1), false);
+  }
+  CUDA_OK(cudaStreamSynchronize(p->stream));
+}
+
+// rank 0 keeps the maps of the formulation and the row-major copy of the caller's matrix for the device postsolve; the
+// device-order vectors were copied by every rank
+static void hand_over_postsolve_maps(ShardPrologue& SP, b200pdlp_problem* p0) {
+  DevProblemArrays& a = SP.P.arr;
+  for (double** v : {&a.cost, &a.lower, &a.upper, &a.colscale, &a.rhs, &a.rowscale, &a.rup}) { dev_cache_free(*v); *v = nullptr; }
+  p0->prep.arr = a;
+  a = DevProblemArrays();
+}
+
 static void hip_barrier(b200pdlp_problem* p) {
   PeerFlags pf{};
   for (size_t g = 0; g < p->hip_peers.size(); g++) pf.f[g] = p->hip_peers[g]->flags.p;
@@ -2297,7 +2381,8 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
   const double solve_seconds = std::chrono::duration<double>(clk::now() - t_loop).count();
   // unscaleSolution + postprocess (pdhg.cc:1883-1897, :359-492): the iterate is copied out ONLY on convergence --
   // an iteration-limited run returns x = y = 0, like the reference
-  if (p->dev_form) {
+  // (several GPUs: rank 0 holds the whole iterate and slacks after the final check; the other ranks return no vectors)
+  if (p->dev_form && p->rank == 0) {
     // on the device (launch_hip_postsolve), one download of the four original-order vectors
     const int n0 = f.n_orig;
     double* cv = p->io_col.p;
@@ -2314,7 +2399,7 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
       dn(out->col_value, cv, n0); dn(out->col_dual, cd, n0); dn(out->row_value, rv, m); dn(out->row_dual, rd, m);
     }
     CUDA_OK(cudaStreamSynchronize(s));
-  } else if (p->rank == 0) {   // (several GPUs: rank 0 holds the whole iterate and slacks after the final check)
+  } else if (!p->dev_form && p->rank == 0) {
     std::vector<double> hx(std::max(n, 1), 0.0), hy(std::max(m, 1), 0.0), hsp(std::max(n, 1)), hsn(std::max(n, 1));
     {
       std::vector<double> t(std::max(std::max(n, m), 1));
@@ -2415,6 +2500,38 @@ struct DeviceGuard {
   DeviceGuard(const DeviceGuard&) = delete;
   DeviceGuard& operator=(const DeviceGuard&) = delete;
 };
+
+// b200pdlp_solve_hipdlp_multi's device prologue: one host thread per distinct device in `dev` runs the block-mode prologue
+// for the ranks on that device and creates their problems (probs[g], already allocated).  Every thread is joined, and its
+// device idle, before this returns: on one device an allocation or a lazy module load of a prologue would otherwise wait
+// behind a peer's spinning barrier (DESIGN section 5).
+static void create_hipdlp_shards_device(const b200pdlp_lp& lp, const b200pdlp_hipdlp_params& prm, const std::vector<int>& dev,
+                                        std::vector<b200pdlp_problem*>& probs) {
+  const int world = (int)dev.size();
+  std::vector<int> devices;   // distinct, in the order of their first rank
+  for (int d : dev)
+    if (std::find(devices.begin(), devices.end(), d) == devices.end()) devices.push_back(d);
+  std::vector<int> codes(devices.size(), B200PDLP_OK);
+  std::vector<std::string> msgs(devices.size());
+  std::vector<std::thread> th;
+  for (size_t i = 0; i < devices.size(); i++)
+    th.emplace_back([&, i] {
+      codes[i] = guarded([&] {
+        std::vector<int> ranks;
+        for (int g = 0; g < world; g++)
+          if (dev[g] == devices[i]) ranks.push_back(g);
+        ShardPrologue SP;
+        run_hipdlp_shard_prologue(lp, prm.scaling_mode, prm.ruiz_iterations, world, devices[i], ranks, SP);
+        for (size_t k = 0; k < ranks.size(); k++) create_problem_hipdlp_shard_device(lp, SP, (int)k, probs[ranks[k]]);
+        if (ranks[0] == 0) hand_over_postsolve_maps(SP, probs[0]);
+        CUDA_OK(cudaDeviceSynchronize());
+      });   // (SP has released the standard form, the orderings and the other temporaries of this device)
+      if (codes[i] != B200PDLP_OK) msgs[i] = g_last_error;   // thread-local: hand it to the caller's thread
+    });
+  for (auto& t : th) t.join();
+  for (size_t i = 0; i < devices.size(); i++)
+    if (codes[i] != B200PDLP_OK) throw Error(codes[i], "device " + std::to_string(devices[i]) + ": " + msgs[i]);
+}
 
 extern "C" {
 
@@ -2927,8 +3044,9 @@ int b200pdlp_solve_hipdlp(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params* p
   });
 }
 
-// The HiPDLP mode on several devices of this process: the host prologue once, then one problem per rank (its blocks of
-// the one-GPU device orders, build_hipdlp_shard), wired by peer pointers, one host thread per rank, no NCCL.
+// The HiPDLP mode on several devices of this process: the prologue once per device (device prologue in block mode) or once
+// on the host (ordered mode, device_prep = -1), then one problem per rank (its blocks of the one-GPU device orders), wired by
+// peer pointers, one host thread per rank, no NCCL.
 int b200pdlp_solve_hipdlp_multi(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params* params, b200pdlp_result* out,
                                 int32_t ngpus, const int32_t* devices) {
   if (ngpus <= 1) return b200pdlp_solve_hipdlp(lp, params, out);
@@ -2954,17 +3072,22 @@ int b200pdlp_solve_hipdlp_multi(const b200pdlp_lp* lp, const b200pdlp_hipdlp_par
           if (!ok) throw Error(B200PDLP_ERR_ARG, "b200pdlp_solve_hipdlp_multi: devices cannot access each other");
         }
     const auto t0 = std::chrono::steady_clock::now();
-    StdForm f;
-    formulate_hipdlp(*lp, f);
-    scale_hipdlp(f, params->scaling_mode, params->ruiz_iterations);
-    HipShards S;
-    plan_hipdlp_shards(f, ngpus, params->ordered_max, S);
+    Laps lap;
     probs.assign(ngpus, nullptr);
-    for (int g = 0; g < ngpus; g++) {
-      probs[g] = new b200pdlp_problem();
-      create_problem_hipdlp_shard(f, S, g, dev[g], probs[g]);
+    for (int g = 0; g < ngpus; g++) probs[g] = new b200pdlp_problem();
+    if (use_device_prep_hipdlp(*lp, *params)) {
+      create_hipdlp_shards_device(*lp, *params, dev, probs);
+      lap("setup", "HiPDLP shards: device prologue");
+    } else {
+      StdForm f;
+      formulate_hipdlp(*lp, f);
+      scale_hipdlp(f, params->scaling_mode, params->ruiz_iterations);
+      HipShards S;
+      plan_hipdlp_shards(f, ngpus, params->ordered_max, S);
+      for (int g = 0; g < ngpus; g++) create_problem_hipdlp_shard(f, S, g, dev[g], probs[g]);
+      probs[0]->form = std::move(f);
+      lap("setup", "HiPDLP shards: host prologue");
     }
-    probs[0]->form = std::move(f);
     auto group = std::make_shared<LocalGroup>();
     group->world = ngpus;
     for (b200pdlp_problem* p : probs) {
@@ -3316,6 +3439,17 @@ static double cmp_dev_d(const double* dev, const double* host, size_t cnt) {
   for (size_t i = 0; i < cnt; i++) bad += memcmp(&t[i], &host[i], sizeof(double)) != 0;
   return bad;
 }
+// one sliced-ELL matrix of the device prologue against the host's: *r_slices = -1 if the sizes differ
+static void cmp_sell(const DevSellOwned& D, const SellMatrix& H, double* r_slices, double* r_col, double* r_val, double* r_long) {
+  if ((size_t)D.nslices != H.slices.size() || D.padded != H.padded || (size_t)D.nlong != H.long_rows.size() ||
+      (size_t)D.nsegs != H.segs.size() || D.lcount != H.lcount) { *r_slices = -1; return; }
+  *r_slices = cmp_dev_i(reinterpret_cast<const int*>(D.slices), reinterpret_cast<const int*>(H.slices.data()), 4 * H.slices.size());
+  *r_col = cmp_dev_i(D.col, H.col.data(), (size_t)H.padded);
+  *r_val = cmp_dev_d(D.val, H.val.data(), (size_t)H.padded);
+  *r_long = cmp_dev_i(reinterpret_cast<const int*>(D.long_rows), reinterpret_cast<const int*>(H.long_rows.data()), 4 * H.long_rows.size()) +
+            cmp_dev_i(reinterpret_cast<const int*>(D.segs), reinterpret_cast<const int*>(H.segs.data()), 4 * H.segs.size()) +
+            cmp_dev_i(D.lcol, H.lcol.data(), H.lcol.size()) + cmp_dev_d(D.lval, H.lval.data(), H.lval.size());
+}
 static bool prep_compare_arrays(const DevicePrologue& P, const StdForm& f, const HostLayout& L, double* report) {
   const auto cmp_i = cmp_dev_i;
   const auto cmp_d = cmp_dev_d;
@@ -3338,16 +3472,6 @@ static bool prep_compare_arrays(const DevicePrologue& P, const StdForm& f, const
   report[16] = cmp_i(a.row_class, f.row_class.data(), m);
   report[17] = cmp_i(a.rperm, L.rperm.data(), m);
   report[18] = cmp_i(a.cperm, L.cperm.data(), n);
-  auto cmp_sell = [&](const DevSellOwned& D, const SellMatrix& H, double* r_slices, double* r_col, double* r_val, double* r_long) {
-    if ((size_t)D.nslices != H.slices.size() || D.padded != H.padded || (size_t)D.nlong != H.long_rows.size() ||
-        (size_t)D.nsegs != H.segs.size() || D.lcount != H.lcount) { *r_slices = -1; return; }
-    *r_slices = cmp_i(reinterpret_cast<const int*>(D.slices), reinterpret_cast<const int*>(H.slices.data()), 4 * H.slices.size());
-    *r_col = cmp_i(D.col, H.col.data(), (size_t)H.padded);
-    *r_val = cmp_d(D.val, H.val.data(), (size_t)H.padded);
-    *r_long = cmp_i(reinterpret_cast<const int*>(D.long_rows), reinterpret_cast<const int*>(H.long_rows.data()), 4 * H.long_rows.size()) +
-              cmp_i(reinterpret_cast<const int*>(D.segs), reinterpret_cast<const int*>(H.segs.data()), 4 * H.segs.size()) +
-              cmp_i(D.lcol, H.lcol.data(), H.lcol.size()) + cmp_d(D.lval, H.lval.data(), H.lval.size());
-  };
   cmp_sell(P.A, L.A, report + 19, report + 20, report + 21, report + 25);
   cmp_sell(P.AT, L.AT, report + 22, report + 23, report + 24, report + 26);
   report[27] = P.sc.amax != f.amax;
@@ -3442,6 +3566,59 @@ int b200pdlp_debug_prep_compare_hipdlp(const b200pdlp_lp* lp, int32_t scaling_mo
       report[35] = cmp_dev_i(P.arr.orow_col, col.data(), nnz0) + cmp_dev_d(P.arr.orow_val, val.data(), nnz0);
     }
     report[36] = (P.sc.scaled != 0) != f.scaled;
+  });
+}
+
+// The block-mode prologue of b200pdlp_solve_hipdlp_multi (run_hipdlp_shard_prologue, every rank on the current device)
+// against formulate_hipdlp + scale_hipdlp + plan_hipdlp_shards (ordered_max = -1) + build_hipdlp_shard, bit for bit;
+// report[8 + 9 world], see include/b200pdlp.h.
+int b200pdlp_debug_hipdlp_shard_prep_compare(const b200pdlp_lp* lp, int32_t scaling_mode, int32_t ruiz_iterations, int32_t world,
+                                             double* report) {
+  DeviceGuard dg;
+  return guarded([&] {
+    check_lp(lp);
+    if (!report || world < 2 || world > kMaxPeers || ruiz_iterations < 0) throw Error(B200PDLP_ERR_ARG, "bad argument");
+    for (int k = 0; k < 8 + 9 * world; k++) report[k] = 0.0;
+    StdForm f;
+    formulate_hipdlp(*lp, f);
+    scale_hipdlp(f, scaling_mode, ruiz_iterations);
+    HipShards S;
+    plan_hipdlp_shards(f, world, /*ordered_max=*/-1, S);
+    int device = 0;
+    CUDA_OK(cudaGetDevice(&device));
+    std::vector<int> ranks(world);
+    for (int g = 0; g < world; g++) ranks[g] = g;
+    ShardPrologue SP;
+    run_hipdlp_shard_prologue(*lp, scaling_mode, ruiz_iterations, world, device, ranks, SP);
+    const DevicePrologue& P = SP.P;
+    const DevProblemArrays& a = P.arr;
+    const int n = f.n, m = f.m;
+    report[0] = (a.n != n) + (a.m != m) + (a.nnz != f.nnz) + (a.neq != f.neq);
+    if (report[0] > 0) return;
+    {
+      std::vector<double> t(std::max(n, m));
+      auto cmp_perm = [&](const double* dev, const std::vector<double>& v, const std::vector<int>& perm, int len) {
+        for (int i = 0; i < len; i++) t[i] = v[perm[i]];
+        return cmp_dev_d(dev, t.data(), len);
+      };
+      report[1] = cmp_perm(a.cost, f.cost, S.cperm, n) + cmp_perm(a.lower, f.lower, S.cperm, n) + cmp_perm(a.upper, f.upper, S.cperm, n) +
+                  cmp_perm(a.colscale, f.col_scale, S.cperm, n) + cmp_perm(a.rhs, f.rhs, S.rperm, m) +
+                  cmp_perm(a.rowscale, f.row_scale, S.rperm, m);
+      report[2] = cmp_perm(a.rup, f.row_upper, S.rperm, m);
+    }
+    const double nc = std::sqrt(P.sc.norm_cost_sq), nr = std::sqrt(P.sc.norm_rhs_sq);
+    report[3] = memcmp(&nc, &f.norm_cost, sizeof(double)) != 0;
+    report[4] = memcmp(&nr, &f.norm_rhs, sizeof(double)) != 0;
+    report[5] = (P.sc.scaled != 0) != f.scaled;
+    report[6] = cmp_dev_i(a.rperm, S.rperm.data(), m) + cmp_dev_i(a.cperm, S.cperm.data(), n);
+    for (int g = 0; g < world; g++) {
+      double* r = report + 8 + 9 * g;
+      r[0] = (P.rb[g] != S.rb[g]) + (P.rb[g + 1] != S.rb[g + 1]) + (P.cb[g] != S.cb[g]) + (P.cb[g + 1] != S.cb[g + 1]);
+      SellMatrix A, AT;
+      build_hipdlp_shard(S, g, A, AT);
+      cmp_sell(P.block_A[g], A, r + 1, r + 2, r + 3, r + 4);
+      cmp_sell(P.block_AT[g], AT, r + 5, r + 6, r + 7, r + 8);
+    }
   });
 }
 

@@ -76,7 +76,7 @@ ABI_SYMBOLS = [
     "b200pdlp_hipdlp_form_create", "b200pdlp_hipdlp_power_method", "b200pdlp_hipdlp_default_params",
     "b200pdlp_solve_hipdlp", "b200pdlp_solve_hipdlp_multi", "b200pdlp_hipdlp_shard_layout_eval",
     "b200pdlp_hipdlp_controller_replay", "b200pdlp_debug_prep_compare",
-    "b200pdlp_debug_prep_compare_hipdlp", "b200pdlp_release_cache",
+    "b200pdlp_debug_prep_compare_hipdlp", "b200pdlp_debug_hipdlp_shard_prep_compare", "b200pdlp_release_cache",
     "b200pdlp_host_register", "b200pdlp_host_unregister", "b200pdlp_primal_step", "b200pdlp_dual_step", "b200pdlp_residuals",
     "b200pdlp_kkt_check", "b200pdlp_kkt_check_host", "b200pdlp_kkt_default_tolerances",
 ]
@@ -256,6 +256,25 @@ def prep_compare_hipdlp(lp: HighsLp, scaling_mode: int = 5, ruiz_iterations: int
     return dict(zip(PREP_ITEMS_HIPDLP, rep.tolist()))
 
 
+SHARD_PREP_ITEMS = ["dims", "device_order_vectors", "row_upper_device_order", "norm_cost_bits", "norm_rhs_bits", "scaled",
+                    "orderings", "unused7"]
+SHARD_PREP_RANK_ITEMS = ["bounds", "A.slices", "A.col", "A.val", "A.long", "AT.slices", "AT.col", "AT.val", "AT.long"]
+
+
+def hipdlp_shard_prep_compare(lp: HighsLp, world: int, scaling_mode: int = 5, ruiz_iterations: int = 10) -> dict:
+    """b200pdlp_debug_hipdlp_shard_prep_compare: the device prologue of solve_hipdlp_multi (every rank's A_g and A_g' on the
+    current device) against the host prologue and build_hipdlp_shard, mismatches per array; "ranks" holds one dict per rank."""
+    L = lib()
+    L.b200pdlp_debug_hipdlp_shard_prep_compare.argtypes = [C.POINTER(CLp), C.c_int32, C.c_int32, C.c_int32, _dp]
+    clp, keep = make_clp(lp)
+    rep = np.zeros(8 + 9 * max(world, 1))
+    _check(L.b200pdlp_debug_hipdlp_shard_prep_compare(C.byref(clp), scaling_mode, ruiz_iterations, world, _p(rep, _dp)),
+           "b200pdlp_debug_hipdlp_shard_prep_compare")
+    out = dict(zip(SHARD_PREP_ITEMS, rep[:8].tolist()))
+    out["ranks"] = [dict(zip(SHARD_PREP_RANK_ITEMS, rep[8 + 9 * g:17 + 9 * g].tolist())) for g in range(world)]
+    return out
+
+
 def lp_arrays(lp: HighsLp):
     a = lp.a_matrix_
     return [a.start_, a.index_, a.value_, lp.col_cost_, lp.col_lower_, lp.col_upper_, lp.row_lower_, lp.row_upper_]
@@ -355,7 +374,8 @@ def solve_hipdlp(lp: HighsLp, **params) -> dict:
 
 def solve_hipdlp_multi(lp: HighsLp, ngpus: int, devices=None, out_arrays=None, **params) -> dict:
     """b200pdlp_solve_hipdlp_multi: the HiPDLP mode on `ngpus` ranks of this process (devices may repeat: logical shards
-    on one device); the same bits as solve_hipdlp(lp, device_prep=-1, **params).
+    on one device).  device_prep is passed through: 0 (default) runs the device prologue once per device where it applies,
+    -1 the host prologue; either way the bits are those of solve_hipdlp(lp, device_prep=-1, **params).
     out_arrays = (col_value, col_dual, row_value, row_dual): caller-owned (e.g. page-locked) result storage."""
     L = lib()
     L.b200pdlp_solve_hipdlp_multi.argtypes = [C.POINTER(CLp), C.POINTER(CHipdlpParams), C.POINTER(CResult), C.c_int32, _ip]

@@ -247,19 +247,21 @@ typedef struct {
   int32_t ordered_max;        /* as in b200pdlp_params: checks add in the reference's order up to this size */
   int32_t device;             /* CUDA device ordinal; -1 = current */
   int32_t log_level;
-  int32_t device_prep;        /* 0 = device prologue where it applies (one GPU, tree mode), -1 = always the host prologue */
+  int32_t device_prep;        /* 0 = device prologue where it applies (tree mode; one GPU or shards), -1 = always the host prologue */
   int32_t reserved[2];
 } b200pdlp_hipdlp_params;
 void b200pdlp_hipdlp_default_params(b200pdlp_hipdlp_params* p);
 int b200pdlp_solve_hipdlp(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params* params, b200pdlp_result* out);
 /* The HiPDLP solve on `ngpus` devices of THIS process (devices[g] or, if NULL, ordinals 0..ngpus-1; a device may repeat,
- * which gives logical shards on one device): the host prologue once, then each rank computes contiguous blocks of the
- * one-GPU device rows and columns, one host thread per rank, peer memory, no NCCL.  Returns the same bits as
- * b200pdlp_solve_hipdlp with device_prep = -1 (iterations, termination and all four vectors), for every ngpus.
- * ngpus <= 1 is b200pdlp_solve_hipdlp; ngpus > 16 or devices without peer access: B200PDLP_ERR_ARG; device_prep and
- * device are ignored.  What the HiGHS shim uses for solver=hipdlp when B200PDLP_GPUS > 1.
- * STATUS: runs on hardware as logical shards on one H100 (tests/test_gpu_hipdlp_shards.py, byte equality with one GPU);
- * not yet run on two physical GPUs. */
+ * which gives logical shards on one device): the prologue, then each rank computes contiguous blocks of the one-GPU device
+ * rows and columns, one host thread per rank, peer memory, no NCCL.  device_prep is honoured as on one GPU: 0 runs the
+ * device prologue where it applies (tree mode, non-empty matrix) once per distinct device, which builds every rank's blocks
+ * there and leaves the postsolve to rank 0's device; -1 (or B200PDLP_DEVICE_PREP=0) runs the host prologue once.  Either
+ * way the result has the same bits as b200pdlp_solve_hipdlp with device_prep = -1 (iterations, termination and all four
+ * vectors), for every ngpus.  ngpus <= 1 is b200pdlp_solve_hipdlp; ngpus > 16 or devices without peer access:
+ * B200PDLP_ERR_ARG; device is ignored.  What the HiGHS shim uses for solver=hipdlp when B200PDLP_GPUS > 1.
+ * STATUS: runs on hardware as logical shards on one H100 with both prologues (tests/test_gpu_hipdlp_shards.py,
+ * tests/test_gpu_hipdlp_shard_prep.py, byte equality with one GPU); not yet run on two physical GPUs. */
 int b200pdlp_solve_hipdlp_multi(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params* params, b200pdlp_result* out,
                                 int32_t ngpus, const int32_t* devices);
 
@@ -311,6 +313,14 @@ int b200pdlp_debug_prep_compare(const b200pdlp_lp* lp, int32_t scaling, double r
  *  34 row pointer of the row-major copy of the caller's matrix  35 its column ids + values (a row's entries in column order)
  *  36 1 if the device and the host disagree on whether any scaling pass ran   37-39 unused (0) */
 int b200pdlp_debug_prep_compare_hipdlp(const b200pdlp_lp* lp, int32_t scaling_mode, int32_t ruiz_iterations, double report[40]);
+/* The device prologue of b200pdlp_solve_hipdlp_multi (block mode, all `world` ranks on the current device, 2 <= world <= 16)
+ * against formulate_hipdlp + scale_hipdlp + plan_hipdlp_shards (ordered_max = -1) + build_hipdlp_shard.  report[8 + 9 world]
+ * = mismatch counts:  0 n, m, nnz, neq (nothing else is compared if they differ)  1 vectors in device order (cost, lower,
+ *  upper, col_scale, rhs, row_scale)  2 row_upper in device order  3, 4 1 if |c|_2, |b|_2 differ in any bit  5 1 if the two
+ *  disagree on whether any scaling pass ran  6 row and column orderings  7 unused (0);  rank g at 8 + 9 g:  +0 its block
+ *  bounds (rows and columns)  +1..+4 A_g: slice descriptors (-1: sizes differ), col, val, long-row arrays  +5..+8 the same for A_g' */
+int b200pdlp_debug_hipdlp_shard_prep_compare(const b200pdlp_lp* lp, int32_t scaling_mode, int32_t ruiz_iterations, int32_t world,
+                                             double* report);
 
 /* The engine keeps the device blocks of finished solves in a process-wide cache (a solve allocates ~60 buffers; cudaMalloc /
  * cudaFree would cost more than the prologue).  This returns them to the driver.  B200PDLP_CACHE_MB caps the cache. */

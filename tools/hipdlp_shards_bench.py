@@ -5,10 +5,13 @@ arm runs a fixed number of iterations (no tolerance is reached at 1e-12): one wa
 the median is reported.  Arms:
   one_gpu            solve_hipdlp, default (device prologue, engine-chosen SpMV shapes)
   one_gpu_host_prep  solve_hipdlp(device_prep=-1): host prologue, one slice per warp -- what the shards reproduce bit for bit
-  shards_G           G logical shards on device 0 (a correctness vehicle: G ranks share one GPU, so expect it slower)
+  shards_G           G logical shards on device 0 (a correctness vehicle: G ranks share one GPU, so expect it slower), device
+                     prologue (one per device, every rank's blocks built there)
+  shards_G_host_prep the same with device_prep=-1: the host prologue and host-built blocks, same layouts, same bits
   gpus_G             G physical GPUs, where the box has them
 One JSON line per (workload, arm): us_per_step = loop_device_ms / iterations (checks included), setup_seconds (the engine's
-clock: everything before the loop), the GPU's name and power limit.
+clock: everything before the loop), the GPU's name and power limit.  The arms run in alternating order: forward for the
+first workload, reversed for the second, and so on, so that no arm always runs first.
 usage: python tools/hipdlp_shards_bench.py [--workloads S3,S3B,S3D] [--iters 800] [--reps 3] [--world 2]
 """
 import argparse
@@ -32,6 +35,8 @@ def run_arm(workload, arm, iters, reps, world):
         call = lambda: engine.solve_hipdlp(lp, **prm)   # noqa: E731
     elif arm == "one_gpu_host_prep":
         call = lambda: engine.solve_hipdlp(lp, device_prep=-1, **prm)   # noqa: E731
+    elif arm.startswith("shards_") and arm.endswith("_host_prep"):
+        call = lambda: engine.solve_hipdlp_multi(lp, world, devices=[0] * world, device_prep=-1, **prm)   # noqa: E731
     elif arm.startswith("shards_"):
         call = lambda: engine.solve_hipdlp_multi(lp, world, devices=[0] * world, **prm)   # noqa: E731
     else:
@@ -42,9 +47,11 @@ def run_arm(workload, arm, iters, reps, world):
             res = call()
             if r:
                 rows.append((1e3 * res["loop_device_ms"] / max(res["iters"], 1), res["setup_seconds"], res["solve_seconds"]))
-        med = np.median(np.array(rows), axis=0)
+        a = np.array(rows)
+        med = np.median(a, axis=0)
         return dict(workload=workload, arm=arm, iters=int(res["iters"]), us_per_step=float(med[0]), setup_seconds=float(med[1]),
-                    solve_seconds=float(med[2]), reps=reps)
+                    solve_seconds=float(med[2]), reps=reps, us_per_step_range=[float(a[:, 0].min()), float(a[:, 0].max())],
+                    setup_seconds_range=[float(a[:, 1].min()), float(a[:, 1].max())])
     finally:
         engine.unpin_arrays(pinned)
 
@@ -64,11 +71,11 @@ def main():
     from highs_b200 import engine
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
     gpu = q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown"
-    arms = ["one_gpu", "one_gpu_host_prep", f"shards_{args.world}"]
+    arms = ["one_gpu", "one_gpu_host_prep", f"shards_{args.world}", f"shards_{args.world}_host_prep"]
     if engine.device_count() >= args.world:
         arms.append(f"gpus_{args.world}")
-    for wl in args.workloads.split(","):
-        for arm in arms:
+    for i, wl in enumerate(args.workloads.split(",")):
+        for arm in (arms if i % 2 == 0 else arms[::-1]):
             r = subprocess.run([sys.executable, os.path.abspath(__file__), "--child", f"{wl}:{arm}", "--iters", str(args.iters),
                                 "--reps", str(args.reps), "--world", str(args.world)], capture_output=True, text=True, cwd=ROOT)
             lines = [ln for ln in r.stdout.splitlines() if ln.startswith("{")]
