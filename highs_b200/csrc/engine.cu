@@ -417,10 +417,181 @@ static void apply_spmv_grid(b200pdlp_problem* p) {
             p->AT.tiles_staged, p->AT.ntiles);
 }
 
+// ---- problem construction.  Every creator below is a sequence of these steps plus what is its own.
+
+// the number of CUDA devices; none is an error: the engine has no CPU fallback
+static int device_count_checked() {
+  int ndev = 0;
+  const cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev == 0)
+    throw Error(B200PDLP_ERR_CUDA, std::string("no CUDA device: the engine has no CPU fallback (") + cudaGetErrorString(e) + ")");
+  return ndev;
+}
+
+// rank `rank` of `world` on `device` (< 0: the caller's current device): selects the device and creates the problem's stream
+static void open_problem(b200pdlp_problem* p, int device, int rank, int world) {
+  device_count_checked();
+  if (device >= 0) p->device = device; else CUDA_OK(cudaGetDevice(&p->device));
+  set_device(p);
+  p->rank = rank; p->world = world;
+  CUDA_OK(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
+}
+
+// the only caller of DevicePrologue::run: bad input -> ERR_ARG, CUDA errors -> ERR_CUDA; a host std::bad_alloc passes
+// through (guarded: ERR_ALLOC)
+static void run_prologue(DevicePrologue& P, cudaStream_t s, const b200pdlp_lp& lp, bool do_scale) {
+  try {
+    P.run(s, lp, do_scale, /*long_threshold=*/512);
+  } catch (const std::invalid_argument& ex) {
+    throw Error(B200PDLP_ERR_ARG, ex.what());
+  } catch (const std::runtime_error& ex) {
+    throw Error(B200PDLP_ERR_CUDA, ex.what());
+  }
+}
+
+// A prologue run on the current device that no single problem holds: its stream, and whatever no problem adopted (A / A',
+// the rank blocks, the arrays, the kept form), released when the holder goes.
+struct TempPrologue {
+  int device = 0;
+  cudaStream_t stream = nullptr;
+  DevicePrologue P;
+  TempPrologue() {
+    CUDA_OK(cudaGetDevice(&device));
+    CUDA_OK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+  }
+  TempPrologue(const TempPrologue&) = delete;
+  TempPrologue& operator=(const TempPrologue&) = delete;
+  ~TempPrologue() {
+    cudaSetDevice(device);
+    cudaStreamSynchronize(stream);
+    cudaStreamDestroy(stream);
+    P.A.release(); P.AT.release(); P.release_blocks(); P.release_arrays(); P.release_form();
+  }
+};
+
+// the scalars of the standard form a device prologue built (the form itself stays on the device)
+static StdForm form_scalars(const b200pdlp_lp& lp, const DevicePrologue& P) {
+  StdForm f;
+  f.hipdlp = P.hipdlp; f.scaled = P.sc.scaled != 0;
+  f.n = P.arr.n; f.m = P.arr.m; f.nnz = P.arr.nnz; f.neq = P.arr.neq; f.n_orig = P.arr.n0;
+  f.sense = lp.sense; f.offset = lp.offset;
+  f.norm_cost = std::sqrt(P.sc.norm_cost_sq); f.norm_rhs = std::sqrt(P.sc.norm_rhs_sq);
+  f.amax = P.sc.amax;
+  return f;
+}
+
+// the standard form the prologue kept on the device (DevicePrologue::keep_form) into f, whose sizes are set
+static void download_form(const DevStdForm& d, StdForm& f, cudaStream_t s) {
+  const int n = f.n, m = f.m, nnz = f.nnz;
+  f.cbeg.resize(n + 1); f.cidx.resize(nnz); f.cval.resize(nnz);
+  f.cost.resize(n); f.lower.resize(n); f.upper.resize(n); f.col_scale.resize(n); f.rhs.resize(m); f.row_scale.resize(m);
+  f.rptr.resize(m + 1); f.rpos.resize(nnz); f.rcol.resize(nnz);
+  auto dn = [&](auto& h, const auto* dv) {
+    if (!h.empty()) CUDA_OK(cudaMemcpyAsync(h.data(), dv, h.size() * sizeof(h[0]), cudaMemcpyDeviceToHost, s));
+  };
+  dn(f.cbeg, d.cbeg); dn(f.cidx, d.cidx); dn(f.cval, d.cval);
+  dn(f.cost, d.cost); dn(f.lower, d.lower); dn(f.upper, d.upper); dn(f.col_scale, d.colscale); dn(f.rhs, d.rhs); dn(f.row_scale, d.rowscale);
+  dn(f.rptr, d.rptr); dn(f.rpos, d.rpos); dn(f.rcol, d.rcol);
+  CUDA_OK(cudaStreamSynchronize(s));
+}
+
+// dimensions of a host layout (host_prep.cpp build_layout); p->form holds the standard form
+static void take_layout(b200pdlp_problem* p, HostLayout&& L) {
+  p->n = p->form.n; p->m = p->form.m;
+  p->r0 = L.r0; p->r1 = L.r1; p->ml = L.ml; p->neq_local = L.neq_local; p->ordered = L.ordered;
+  p->row_bounds = std::move(L.bounds);
+  p->nl = L.nl; p->nl_real = L.nl_real; p->c0 = L.c0; p->shard_len = L.shard_len; p->seg_len = L.seg_len;
+  p->csr_local = std::move(L.csr_local);
+  p->rperm = std::move(L.rperm); p->rinv = std::move(L.rinv);
+  p->cperm = std::move(L.cperm); p->cinv = std::move(L.cinv);
+  p->A.host = std::move(L.A); p->AT.host = std::move(L.AT);
+  if (L.world > 1) p->at_outpos.from(L.at_outpos);
+}
+
+// dimensions of a rank that holds every row and full-length vectors (one GPU, and the HiPDLP shards); p->form holds the scalars
+static void set_full_length_dims(b200pdlp_problem* p) {
+  const StdForm& f = p->form;
+  const int n = f.n, m = f.m;
+  p->n = n; p->m = m; p->ml = m; p->r0 = 0; p->r1 = m; p->neq_local = f.neq;
+  p->row_bounds = {0, m};
+  p->nl = p->nl_real = n; p->c0 = 0; p->shard_len = n; p->seg_len = n;
+  p->csr_local.nrows = m; p->csr_local.ncols = n; p->csr_local.nnz = f.nnz;   // dimensions only (built on demand)
+}
+
+// what a problem that holds every row takes from a device prologue: the form's scalars, the dimensions and the device-order
+// vectors, adopted on one GPU; in block mode every rank takes its own copy (the matrices are the caller's: A / A' or a block)
+static void take_prologue(const b200pdlp_lp& lp, DevicePrologue& P, b200pdlp_problem* p) {
+  p->form = form_scalars(lp, P);
+  set_full_length_dims(p);
+  DevProblemArrays& a = P.arr;
+  auto take = [&](DevBuf<double>& d, double*& src, int len) {
+    if (P.world == 1) { d.adopt(src, len); src = nullptr; return; }
+    d.alloc(len, false);
+    if (len > 0) CUDA_OK(cudaMemcpyAsync(d.p, src, (size_t)len * sizeof(double), cudaMemcpyDeviceToDevice, p->stream));
+  };
+  take(p->cost, a.cost, a.n); take(p->lower, a.lower, a.n); take(p->upper, a.upper, a.n); take(p->colscale, a.colscale, a.n);
+  take(p->rhs, a.rhs, a.m); take(p->rowscale, a.rowscale, a.m);
+  if (P.hipdlp) take(p->hip.rup, a.rup, a.m);
+}
+
+// a host vector into device order: d[i] = v[offset + perm[i]] for i < len, then `pad` up to `size` entries
+static void upload_permuted(DevBuf<double>& d, const std::vector<double>& v, const int* perm, int offset, int len, int size,
+                            double pad = 0.0) {
+  std::vector<double> t((size_t)std::max(size, 1), pad);
+  for (int i = 0; i < len; i++) t[i] = v[offset + perm[i]];
+  d.alloc(size, false);
+  d.upload(t.data(), size);
+}
+
+// reduction scratch (sized for the larger launch shape, so after apply_spmv_grid), the check's device scalars and their pinned
+// mirror.  The term scratch has p->ordered_cap entries per accumulator: set by pdlp in ordered mode, 0 for HiPDLP, whose check
+// reduces without it.  zero: every buffer zeroed at allocation; the counters are zero before the first launch either way.
+static void alloc_scratch(b200pdlp_problem* p, bool zero) {
+  const size_t maxgrid = std::max<size_t>(kMaxEwBlocks, std::max(p->A.grid_full(), p->AT.grid_full()));
+  p->scratch_stride = 24 * maxgrid;
+  p->partials.alloc(p->scratch_stride * kNumSlots, zero);
+  p->counters.alloc(kNumSlots, zero);
+  if (!zero) CUDA_OK(cudaMemsetAsync(p->counters.p, 0, kNumSlots * sizeof(unsigned), p->stream));
+  p->terms.alloc(p->ordered_cap > 0 ? (size_t)kNumSlots * 16 * p->ordered_cap : 1, zero);
+  p->outs.alloc(kOutsCount, zero);
+  p->houts = static_cast<double*>(pinned_cache_alloc(kOutsCount * sizeof(double), false));
+}
+
+// the PDHG solve's pinned mirrors, zeroed
 static void alloc_host_mirrors(b200pdlp_problem* p) {
   p->hstate = static_cast<PdhgState*>(pinned_cache_alloc(sizeof(PdhgState), false));
-  p->houts = static_cast<double*>(pinned_cache_alloc(kOutsCount * sizeof(double), false));
   p->hflag = static_cast<double*>(pinned_cache_alloc(4 * sizeof(double), false));   // [0] time-limit flag, [2] read-back of the barrier fault word
+  memset(p->hflag, 0, 4 * sizeof(double));
+  memset(p->hstate, 0, sizeof(PdhgState));
+}
+
+// the HiPDLP shards' arrival words, one per peer (hip_barrier_kernel), epoch and fault word
+static void alloc_peer_words(b200pdlp_problem* p) {
+  p->flags.alloc(kMaxPeers);
+  p->epochs.alloc(1);
+  p->fault.alloc(1);
+}
+
+// staging of the hot start and of the solution in original order (device postsolve)
+static void alloc_postsolve_staging(b200pdlp_problem* p) {
+  p->io_col.alloc((size_t)2 * std::max(p->form.n_orig, 1), false);
+  p->io_row.alloc((size_t)2 * std::max(p->m, 1), false);
+}
+
+// The size rule of both device prologues.  Ordered mode keeps the host prologue; it is decided on the STANDARD FORM's size,
+// n = num_col + one slack column per ranged or free row (CupdlpWrapper.cpp:328-345; `inf` is the mode's infinite row bound),
+// so count them when the answer depends on it.  An empty matrix keeps it too.
+static bool device_prep_fits(const b200pdlp_lp& lp, int ordered_max, double inf) {
+  const int omax = ordered_max == 0 ? 4096 : ordered_max;
+  if (omax > 0 && lp.num_col <= omax && lp.num_row <= omax) {
+    int nslack = 0;
+    for (int i = 0; i < lp.num_row; i++) {
+      const bool lo = lp.row_lower[i] > -inf, up = lp.row_upper[i] < inf;
+      nslack += (lo && up && lp.row_lower[i] != lp.row_upper[i]) || (!lo && !up);
+    }
+    if (lp.num_col + nslack <= omax) return false;
+  }
+  return lp.num_col > 0 && lp.num_row > 0 && lp.a_start[lp.num_col] > 0;
 }
 
 // Several GPUs (default; B200PDLP_MG_DEVICE_PREP=0 for the host path): every rank needs the whole scaled standard form to cut its shard out of
@@ -428,55 +599,25 @@ static void alloc_host_mirrors(b200pdlp_problem* p) {
 // each rank formulates and scales on ITS GPU (a few milliseconds, identical bits on every rank) and downloads the result;
 // the per-rank layouts are then built by the host as before.
 static void device_form_to_host(const b200pdlp_lp& lp, const b200pdlp_params& prm, StdForm& f) {
-  cudaStream_t s = nullptr;
-  CUDA_OK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
-  DevicePrologue P;
-  P.keep_form = true;
-  P.stop_after_scaling = true;
-  struct Cleanup { DevicePrologue& P; cudaStream_t s; ~Cleanup() { P.release_arrays(); P.release_form(); cudaStreamDestroy(s); } } cleanup{P, s};
-  try { P.run(s, lp, prm.scaling != 0, 512); }
-  catch (const std::invalid_argument& ex) { throw Error(B200PDLP_ERR_ARG, ex.what()); }
-  catch (const std::exception& ex) { throw Error(B200PDLP_ERR_CUDA, ex.what()); }
-  f = StdForm();
-  const DevProblemArrays& a = P.arr;
-  const int n = a.n, m = a.m, nnz = a.nnz;
-  f.n = n; f.m = m; f.nnz = nnz; f.neq = a.neq; f.n_orig = a.n0;
-  f.sense = lp.sense; f.offset = lp.offset;
-  f.norm_cost = std::sqrt(P.sc.norm_cost_sq); f.norm_rhs = std::sqrt(P.sc.norm_rhs_sq); f.amax = P.sc.amax;
-  f.cbeg.resize(n + 1); f.cidx.resize(nnz); f.cval.resize(nnz);
-  f.cost.resize(n); f.lower.resize(n); f.upper.resize(n); f.col_scale.resize(n); f.rhs.resize(m); f.row_scale.resize(m);
-  f.row_new_idx.resize(m); f.row_class.resize(m);
-  f.rptr.resize(m + 1); f.rpos.resize(nnz); f.rcol.resize(nnz);
-  auto dn = [&](void* h, const void* d, size_t bytes) { if (bytes) CUDA_OK(cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, s)); };
-  const DevStdForm& d = P.form;
-  dn(f.cbeg.data(), d.cbeg, (size_t)(n + 1) * 4); dn(f.cidx.data(), d.cidx, (size_t)nnz * 4); dn(f.cval.data(), d.cval, (size_t)nnz * 8);
-  dn(f.cost.data(), d.cost, (size_t)n * 8); dn(f.lower.data(), d.lower, (size_t)n * 8); dn(f.upper.data(), d.upper, (size_t)n * 8);
-  dn(f.col_scale.data(), d.colscale, (size_t)n * 8); dn(f.rhs.data(), d.rhs, (size_t)m * 8); dn(f.row_scale.data(), d.rowscale, (size_t)m * 8);
-  dn(f.rptr.data(), d.rptr, (size_t)(m + 1) * 4); dn(f.rpos.data(), d.rpos, (size_t)nnz * 4); dn(f.rcol.data(), d.rcol, (size_t)nnz * 4);
-  dn(f.row_new_idx.data(), a.row_new_idx, (size_t)m * 4); dn(f.row_class.data(), a.row_class, (size_t)m * 4);
-  CUDA_OK(cudaStreamSynchronize(s));
+  TempPrologue T;
+  T.P.keep_form = true;
+  T.P.stop_after_scaling = true;
+  run_prologue(T.P, T.stream, lp, prm.scaling != 0);
+  f = form_scalars(lp, T.P);
+  download_form(T.P.form, f, T.stream);
+  const DevProblemArrays& a = T.P.arr;
+  f.row_new_idx.resize(f.m); f.row_class.resize(f.m);
+  CUDA_OK(cudaMemcpy(f.row_new_idx.data(), a.row_new_idx, (size_t)f.m * sizeof(int), cudaMemcpyDeviceToHost));
+  CUDA_OK(cudaMemcpy(f.row_class.data(), a.row_class, (size_t)f.m * sizeof(int), cudaMemcpyDeviceToHost));
 }
 
 // shared_form != nullptr: the standard form was formulated and scaled already (by another rank of this process)
 static void create_problem(const b200pdlp_lp& lp, const b200pdlp_params& prm, int rank, int world, b200pdlp_problem* p,
                            const StdForm* shared_form = nullptr) {
   NvtxRange nvtx("b200pdlp: prologue (host threads) + upload");
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0)
-    throw Error(B200PDLP_ERR_CUDA, std::string("no CUDA device: the engine has no CPU fallback (") + cudaGetErrorString(e) + ")");
-  if (prm.device >= 0) p->device = prm.device; else CUDA_OK(cudaGetDevice(&p->device));
-  set_device(p);
-  p->rank = rank; p->world = world;
-  const bool timing = getenv("B200PDLP_TIMING") != nullptr;
-  auto tnow = [] { return std::chrono::steady_clock::now(); };
-  auto t0 = tnow();
-  auto lap = [&](const char* what) {
-    if (!timing) return;
-    auto t1 = tnow();
-    fprintf(stderr, "[b200pdlp setup] %-28s %8.1f ms\n", what, std::chrono::duration<double, std::milli>(t1 - t0).count());
-    t0 = t1;
-  };
+  open_problem(p, prm.device, rank, world);
+  Laps laps;
+  auto lap = [&](const char* what) { laps("setup", what); };
   bool mg_dev_form = false;
   if (!shared_form && world > 1 && lp.num_row > 0 && lp.num_col > 0 && lp.a_start[lp.num_col] > 0) {
     // default (the ranks do not compete for the host's cores and memory bandwidth): B200PDLP_MG_DEVICE_PREP=0 keeps the host
@@ -501,24 +642,14 @@ static void create_problem(const b200pdlp_lp& lp, const b200pdlp_params& prm, in
     // host layout (row block, device orderings, sliced-ELL of A_g and A_g^T): host_prep.cpp build_layout
     HostLayout L;
     build_layout(f, rank, world, prm.ordered_max, L, lap);
-    p->r0 = L.r0; p->r1 = L.r1; p->ml = L.ml; p->neq_local = L.neq_local; p->ordered = L.ordered;
-    p->row_bounds = L.bounds;
-    p->n = f.n; p->m = f.m;
-    p->nl = L.nl; p->nl_real = L.nl_real; p->c0 = L.c0; p->shard_len = L.shard_len; p->seg_len = L.seg_len;
-    p->csr_local = std::move(L.csr_local);
-    p->rperm = std::move(L.rperm); p->rinv = std::move(L.rinv);
-    p->cperm = std::move(L.cperm); p->cinv = std::move(L.cinv);
-    p->A.host = std::move(L.A); p->AT.host = std::move(L.AT);
-    if (world > 1) p->at_outpos.from(L.at_outpos);
+    take_layout(p, std::move(L));
   }
-  const int n = p->n, ml = p->ml;
-  CUDA_OK(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
+  const int n = p->n, ml = p->ml, nl = p->nl;
   if (world == 1) ensure_side_stream(p);
   p->A.upload();
   p->AT.upload();
   lap("matrix upload");
   apply_spmv_grid(p);
-  const int nl = p->nl;
   for (int k = 0; k < 2; k++) { p->x[k].alloc(nl); p->aty[k].alloc(nl); p->y[k].alloc(ml); p->ax[k].alloc(ml); }
   p->xsum.alloc(nl); p->xavg.alloc(nl); p->atyavg.alloc(nl); p->xlr.alloc(nl);
   p->ysum.alloc(ml); p->yavg.alloc(ml); p->axavg.alloc(ml); p->ylr.alloc(ml);
@@ -530,32 +661,16 @@ static void create_problem(const b200pdlp_lp& lp, const b200pdlp_params& prm, in
     p->flags.alloc(5 * kMaxPeers + 2 * kMaxPeers * 32);   // [3][16] flags, [16][2] pass mailbox, [2][16][32] check mailbox
     p->epochs.alloc(16); p->fault.alloc(1);
   }
-  {
-    std::vector<double> t(std::max(std::max(n, nl), ml));
-    auto up_col = [&](DevBuf<double>& d, const std::vector<double>& v, double pad) {
-      // my shard of the column vector in device order (padding: cost 0, bounds [0,0], scale 1)
-      for (int i = 0; i < nl; i++) t[i] = i < p->nl_real ? v[p->cperm[p->c0 + i]] : pad;
-      d.alloc(nl, false); d.upload(t.data(), nl);
-    };
-    auto up_row = [&](DevBuf<double>& d, const std::vector<double>& v) {
-      for (int i = 0; i < ml; i++) t[i] = v[p->r0 + p->rperm[i]];
-      d.alloc(ml, false); d.upload(t.data(), ml);
-    };
-    up_col(p->cost, f.cost, 0.0); up_col(p->lower, f.lower, 0.0); up_col(p->upper, f.upper, 0.0); up_col(p->colscale, f.col_scale, 1.0);
-    up_row(p->rhs, f.rhs); up_row(p->rowscale, f.row_scale);
-  }
+  // my shard of the column vectors in device order (padding: cost 0, bounds [0,0], scale 1) and my rows
+  const int* cperm = p->cperm.data() + p->c0;
+  upload_permuted(p->cost, f.cost, cperm, 0, p->nl_real, nl); upload_permuted(p->lower, f.lower, cperm, 0, p->nl_real, nl);
+  upload_permuted(p->upper, f.upper, cperm, 0, p->nl_real, nl); upload_permuted(p->colscale, f.col_scale, cperm, 0, p->nl_real, nl, 1.0);
+  upload_permuted(p->rhs, f.rhs, p->rperm.data(), p->r0, ml, ml); upload_permuted(p->rowscale, f.row_scale, p->rperm.data(), p->r0, ml, ml);
   p->redbuf.alloc((size_t)std::max(n, p->m) + 16);
-  size_t maxgrid = std::max<size_t>(kMaxEwBlocks, std::max(p->A.grid_full(), p->AT.grid_full()));
-  p->scratch_stride = 24 * maxgrid;
-  p->partials.alloc(p->scratch_stride * kNumSlots);
-  p->counters.alloc(kNumSlots);
   p->ordered_cap = p->ordered ? std::max(std::max(p->n, p->m), 1) : 0;
-  p->terms.alloc(p->ordered ? (size_t)kNumSlots * 16 * p->ordered_cap : 1);
-  p->outs.alloc(kOutsCount);
+  alloc_scratch(p, true);
   p->state.alloc(1);
-  alloc_host_mirrors(p);   // [0] time-limit flag, [2] read-back of the barrier fault word
-  memset(p->hflag, 0, 4 * sizeof(double));
-  memset(p->hstate, 0, sizeof(PdhgState));
+  alloc_host_mirrors(p);
   CUDA_OK(cudaDeviceSynchronize());
   lap("vectors + scratch");
 }
@@ -567,19 +682,7 @@ static bool use_device_prep(const b200pdlp_lp& lp, const b200pdlp_params& prm, i
   if (world != 1) return false;
   if (const char* e = getenv("B200PDLP_DEVICE_PREP")) { if (atoi(e) == 0) return false; }
   else if (prm.device_scaling == -1) return false;   // the host prologue on request (check_params allows 0 and -1 only)
-  const int omax = prm.ordered_max == 0 ? 4096 : prm.ordered_max;
-  // ordered mode (host_prep.cpp::build_layout) is decided on the STANDARD FORM's size: n = num_col + #BOUND rows
-  // (ranged and free rows get a slack column, CupdlpWrapper.cpp:328-345) -- count them when the answer depends on it
-  if (omax > 0 && lp.num_col <= omax && lp.num_row <= omax) {
-    int nbound = 0;
-    for (int i = 0; i < lp.num_row; i++) {
-      const bool lo = lp.row_lower[i] > -1e20, up = lp.row_upper[i] < 1e20;
-      nbound += (lo && up && lp.row_lower[i] != lp.row_upper[i]) || (!lo && !up);
-    }
-    if (lp.num_col + nbound <= omax) return false;
-  }
-  if (lp.num_col <= 0 || lp.num_row <= 0 || lp.a_start[lp.num_col] <= 0) return false;
-  return true;
+  return device_prep_fits(lp, prm.ordered_max, 1e20);
 }
 
 // the engine takes over one sliced-ELL matrix the device prologue built
@@ -602,69 +705,33 @@ static void adopt_matrix(DeviceMatrix& M, DevSellOwned& O) {
 
 static void create_problem_device(const b200pdlp_lp& lp, const b200pdlp_params& prm, b200pdlp_problem* p) {
   NvtxRange nvtx("b200pdlp: prologue (device)");
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0)
-    throw Error(B200PDLP_ERR_CUDA, std::string("no CUDA device: the engine has no CPU fallback (") + cudaGetErrorString(e) + ")");
-  if (prm.device >= 0) p->device = prm.device; else CUDA_OK(cudaGetDevice(&p->device));
-  set_device(p);
-  p->rank = 0; p->world = 1;
+  open_problem(p, prm.device, 0, 1);
   Laps lap;
-  CUDA_OK(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
   ensure_side_stream(p);
-  cudaStream_t s = p->stream;
   p->dev_form = true;
   if (getenv("B200PDLP_KEEP_FORM")) p->prep.keep_form = true;
-  try {
-    p->prep.run(s, lp, prm.scaling != 0, /*long_threshold=*/512);
-  } catch (const std::invalid_argument& ex) {
-    throw Error(B200PDLP_ERR_ARG, ex.what());
-  } catch (const std::runtime_error& ex) {
-    throw Error(B200PDLP_ERR_CUDA, ex.what());
-  }
-  lap("setup", "device prologue");
   DevicePrologue& P = p->prep;
-  if (getenv("B200PDLP_TIMING"))
+  run_prologue(P, p->stream, lp, prm.scaling != 0);
+  lap("setup", "device prologue");
+  if (lap.on)
     fprintf(stderr, "[b200pdlp setup] sectors per gathered lane (sampled): A %.3f  A' %.3f\n",
             P.sc.a_lanes ? (double)P.sc.a_sectors / P.sc.a_lanes : 0.0, P.sc.at_lanes ? (double)P.sc.at_sectors / P.sc.at_lanes : 0.0);
-  StdForm& f = p->form;
-  f = StdForm();
-  f.n = P.arr.n; f.m = P.arr.m; f.nnz = P.arr.nnz; f.neq = P.arr.neq; f.n_orig = P.arr.n0;
-  f.sense = lp.sense; f.offset = lp.offset;
-  f.norm_cost = std::sqrt(P.sc.norm_cost_sq); f.norm_rhs = std::sqrt(P.sc.norm_rhs_sq);
-  f.amax = P.sc.amax;
+  take_prologue(lp, P, p);
   p->beta_cost_sq = P.sc.beta_cost_sq; p->beta_rhs_sq = P.sc.beta_rhs_sq;
-  const int n = f.n, m = f.m;
-  p->n = n; p->m = m; p->ml = m; p->r0 = 0; p->r1 = m; p->neq_local = f.neq; p->ordered = false;
-  p->row_bounds = {0, m};
-  p->nl = p->nl_real = n; p->c0 = 0; p->shard_len = n; p->seg_len = n;
-  p->csr_local.nrows = m; p->csr_local.ncols = n; p->csr_local.nnz = f.nnz;   // dimensions only (built on demand)
+  const int n = p->n, m = p->m;
   adopt_matrix(p->A, P.A);
   adopt_matrix(p->AT, P.AT);
-  p->cost.adopt(P.arr.cost, n); p->lower.adopt(P.arr.lower, n); p->upper.adopt(P.arr.upper, n); p->colscale.adopt(P.arr.colscale, n);
-  p->rhs.adopt(P.arr.rhs, m); p->rowscale.adopt(P.arr.rowscale, m);
-  P.arr.cost = P.arr.lower = P.arr.upper = P.arr.colscale = P.arr.rhs = P.arr.rowscale = nullptr;
   apply_spmv_grid(p);
   // iterates and scratch: uninitialised (the solve's initial-point kernels write every entry they read)
   for (int k = 0; k < 2; k++) { p->x[k].alloc(n, false); p->aty[k].alloc(n, false); p->y[k].alloc(m, false); p->ax[k].alloc(m, false); }
   p->xsum.alloc(n, false); p->xavg.alloc(n, false); p->atyavg.alloc(n, false); p->xlr.alloc(n, false);
   p->ysum.alloc(m, false); p->yavg.alloc(m, false); p->axavg.alloc(m, false); p->ylr.alloc(m, false);
   p->axsum.alloc(m, false); p->atysum.alloc(n, false);
-  p->io_col.alloc((size_t)2 * std::max(f.n_orig, 1), false);
-  p->io_row.alloc((size_t)2 * std::max(m, 1), false);
-  size_t maxgrid = std::max<size_t>(kMaxEwBlocks, std::max(p->A.grid_full(), p->AT.grid_full()));
-  p->scratch_stride = 24 * maxgrid;
-  p->partials.alloc(p->scratch_stride * kNumSlots, false);
-  p->counters.alloc(kNumSlots, false);
-  CUDA_OK(cudaMemsetAsync(p->counters.p, 0, kNumSlots * sizeof(unsigned), s));
-  p->ordered_cap = 0;
-  p->terms.alloc(1, false);
-  p->outs.alloc(kOutsCount, false);
+  alloc_postsolve_staging(p);
+  alloc_scratch(p, false);
   p->state.alloc(1, false);
   p->redbuf.alloc(16, false);
   alloc_host_mirrors(p);
-  memset(p->hflag, 0, 4 * sizeof(double));
-  memset(p->hstate, 0, sizeof(PdhgState));
   lap("setup", "vectors + scratch");
 }
 
@@ -687,14 +754,7 @@ static void ensure_host_form(b200pdlp_problem* p) {
   if (!p->dev_form || !p->form.cbeg.empty()) return;
   const DevStdForm& d = p->prep.form;
   if (!d.cbeg) throw Error(B200PDLP_ERR_STATE, "the standard form was not kept on the device (one-shot solve)");
-  StdForm& f = p->form;
-  const int n = f.n, m = f.m, nnz = f.nnz;
-  f.cbeg.resize(n + 1); f.cidx.resize(nnz); f.cval.resize(nnz);
-  f.cost.resize(n); f.lower.resize(n); f.upper.resize(n); f.col_scale.resize(n); f.rhs.resize(m); f.row_scale.resize(m);
-  auto dn = [&](void* h, const void* dv, size_t bytes) { if (bytes) CUDA_OK(cudaMemcpy(h, dv, bytes, cudaMemcpyDeviceToHost)); };
-  dn(f.cbeg.data(), d.cbeg, (size_t)(n + 1) * 4); dn(f.cidx.data(), d.cidx, (size_t)nnz * 4); dn(f.cval.data(), d.cval, (size_t)nnz * 8);
-  dn(f.cost.data(), d.cost, (size_t)n * 8); dn(f.lower.data(), d.lower, (size_t)n * 8); dn(f.upper.data(), d.upper, (size_t)n * 8);
-  dn(f.col_scale.data(), d.colscale, (size_t)n * 8); dn(f.rhs.data(), d.rhs, (size_t)m * 8); dn(f.row_scale.data(), d.rowscale, (size_t)m * 8);
+  download_form(d, p->form, p->stream);
   ensure_host_maps(p);
 }
 
@@ -1891,20 +1951,10 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
 static bool use_device_prep_hipdlp(const b200pdlp_lp& lp, const b200pdlp_hipdlp_params& prm) {
   if (const char* e = getenv("B200PDLP_DEVICE_PREP")) { if (atoi(e) == 0) return false; }
   if (prm.device_prep == -1) return false;
-  const int omax = prm.ordered_max == 0 ? 4096 : prm.ordered_max;
-  if (omax > 0 && lp.num_col <= omax && lp.num_row <= omax) {
-    const double inf = std::numeric_limits<double>::infinity();
-    int nslack = 0;
-    for (int i = 0; i < lp.num_row; i++) {
-      const bool lo = lp.row_lower[i] > -inf, up = lp.row_upper[i] < inf;
-      nslack += (lo && up && lp.row_lower[i] != lp.row_upper[i]) || (!lo && !up);
-    }
-    if (lp.num_col + nslack <= omax) return false;
-  }
-  if (lp.num_col <= 0 || lp.num_row <= 0 || lp.a_start[lp.num_col] <= 0) return false;
-  return true;
+  return device_prep_fits(lp, prm.ordered_max, std::numeric_limits<double>::infinity());
 }
 
+// the HiPDLP iterate set, its pinned state mirror and the scratch, all zeroed
 static void hipdlp_buffers(b200pdlp_problem* p) {
   const int n = p->n, m = p->m;
   auto& h = p->hip;
@@ -1912,14 +1962,7 @@ static void hipdlp_buffers(b200pdlp_problem* p) {
   for (DevBuf<double>* b : {&h.y, &h.yn, &h.ry, &h.ya, &h.axp, &h.dy}) b->alloc(m);
   h.state.alloc(1);
   h.hstate = static_cast<HipState*>(pinned_cache_alloc(sizeof(HipState), false));
-  size_t maxgrid = std::max<size_t>(kMaxEwBlocks, std::max(p->A.grid_full(), p->AT.grid_full()));
-  p->scratch_stride = 24 * maxgrid;
-  p->partials.alloc(p->scratch_stride * kNumSlots);
-  p->counters.alloc(kNumSlots);
-  p->terms.alloc(1);
-  p->ordered_cap = 0;
-  p->outs.alloc(kOutsCount);
-  p->houts = static_cast<double*>(pinned_cache_alloc(kOutsCount * sizeof(double), false));
+  alloc_scratch(p, true);
 }
 
 // the whole HiPDLP prologue on the device: formulate, scale, unscaled norms, row index, orderings, both layouts, the
@@ -1927,87 +1970,47 @@ static void hipdlp_buffers(b200pdlp_problem* p) {
 static void create_problem_hipdlp_device(const b200pdlp_lp& lp, const b200pdlp_hipdlp_params& prm, b200pdlp_problem* p) {
   NvtxRange nvtx("b200pdlp: HiPDLP prologue (device)");
   Laps lap;
-  CUDA_OK(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
-  cudaStream_t s = p->stream;
   p->dev_form = true;
   DevicePrologue& P = p->prep;
   P.hipdlp = true;
   P.scaling_mode = prm.scaling_mode;
   P.ruiz_iterations = prm.ruiz_iterations;
-  try {
-    P.run(s, lp, true, /*long_threshold=*/512);
-  } catch (const std::invalid_argument& ex) {
-    throw Error(B200PDLP_ERR_ARG, ex.what());
-  } catch (const std::runtime_error& ex) {
-    throw Error(B200PDLP_ERR_CUDA, ex.what());
-  }
+  run_prologue(P, p->stream, lp, true);
   lap("setup", "device prologue (HiPDLP)");
   if (lap.on) fprintf(stderr, "[b200pdlp setup] ordered |c|^2, |b|^2 (side stream, under the layouts) %8.3f ms\n", P.sc.norms_ms);
-  StdForm& f = p->form;
-  f = StdForm();
-  f.hipdlp = true;
-  f.n = P.arr.n; f.m = P.arr.m; f.nnz = P.arr.nnz; f.neq = P.arr.neq; f.n_orig = P.arr.n0;
-  f.sense = lp.sense; f.offset = lp.offset;
-  f.norm_cost = std::sqrt(P.sc.norm_cost_sq); f.norm_rhs = std::sqrt(P.sc.norm_rhs_sq);
-  f.amax = P.sc.amax;
-  f.scaled = P.sc.scaled != 0;
-  const int n = f.n, m = f.m;
-  p->n = n; p->m = m; p->ml = m; p->r0 = 0; p->r1 = m; p->neq_local = f.neq; p->ordered = false;
-  p->row_bounds = {0, m};
-  p->nl = p->nl_real = n; p->c0 = 0; p->shard_len = n; p->seg_len = n;
-  p->csr_local.nrows = m; p->csr_local.ncols = n; p->csr_local.nnz = f.nnz;
+  take_prologue(lp, P, p);
   adopt_matrix(p->A, P.A);
   adopt_matrix(p->AT, P.AT);
-  p->cost.adopt(P.arr.cost, n); p->lower.adopt(P.arr.lower, n); p->upper.adopt(P.arr.upper, n); p->colscale.adopt(P.arr.colscale, n);
-  p->rhs.adopt(P.arr.rhs, m); p->rowscale.adopt(P.arr.rowscale, m); p->hip.rup.adopt(P.arr.rup, m);
-  P.arr.cost = P.arr.lower = P.arr.upper = P.arr.colscale = P.arr.rhs = P.arr.rowscale = P.arr.rup = nullptr;
   apply_spmv_grid(p);
   hipdlp_buffers(p);
-  p->io_col.alloc((size_t)2 * std::max(f.n_orig, 1), false);
-  p->io_row.alloc((size_t)2 * std::max(m, 1), false);
-  CUDA_OK(cudaStreamSynchronize(s));
+  alloc_postsolve_staging(p);
+  CUDA_OK(cudaStreamSynchronize(p->stream));
   lap("setup", "vectors + scratch");
 }
 
 static void create_problem_hipdlp(const b200pdlp_lp& lp, const b200pdlp_hipdlp_params& prm, b200pdlp_problem* p) {
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0)
-    throw Error(B200PDLP_ERR_CUDA, std::string("no CUDA device: the engine has no CPU fallback (") + cudaGetErrorString(e) + ")");
-  if (prm.device >= 0) p->device = prm.device; else CUDA_OK(cudaGetDevice(&p->device));
-  set_device(p);
-  p->rank = 0; p->world = 1;
+  open_problem(p, prm.device, 0, 1);
   if (use_device_prep_hipdlp(lp, prm)) { create_problem_hipdlp_device(lp, prm, p); return; }
   Laps lap;
   formulate_hipdlp(lp, p->form);
   scale_hipdlp(p->form, prm.scaling_mode, prm.ruiz_iterations);
   lap("setup", "formulate + scale (host)");
   StdForm& f = p->form;
-  HostLayout L;
-  build_layout(f, 0, 1, prm.ordered_max, L);
+  {
+    HostLayout L;
+    build_layout(f, 0, 1, prm.ordered_max, L);
+    take_layout(p, std::move(L));
+  }
   lap("setup", "layouts (host)");
-  p->r0 = L.r0; p->r1 = L.r1; p->ml = L.ml; p->neq_local = L.neq_local; p->ordered = L.ordered;
-  p->n = f.n; p->m = f.m;
-  p->nl = L.nl; p->nl_real = L.nl_real; p->c0 = 0; p->shard_len = L.shard_len; p->seg_len = L.seg_len;
-  p->csr_local = std::move(L.csr_local);
-  p->rperm = std::move(L.rperm); p->rinv = std::move(L.rinv);
-  p->cperm = std::move(L.cperm); p->cinv = std::move(L.cinv);
-  p->A.host = std::move(L.A); p->AT.host = std::move(L.AT);
-  CUDA_OK(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
   p->A.upload();
   p->AT.upload();
   const int n = p->n, m = p->m;
-  std::vector<double> t(std::max(std::max(n, m), 1));
-  auto up_col = [&](DevBuf<double>& d, const std::vector<double>& v) {
-    for (int i = 0; i < n; i++) t[i] = v[p->cperm[i]];
-    d.alloc(n, false); d.upload(t.data(), n);
-  };
-  auto up_row = [&](DevBuf<double>& d, const std::vector<double>& v) {
-    for (int i = 0; i < m; i++) t[i] = v[p->rperm[i]];
-    d.alloc(m, false); d.upload(t.data(), m);
-  };
-  up_col(p->cost, f.cost); up_col(p->lower, f.lower); up_col(p->upper, f.upper); up_col(p->colscale, f.col_scale);
-  up_row(p->rhs, f.rhs); up_row(p->hip.rup, f.row_upper); up_row(p->rowscale, f.row_scale);
+  const int* cperm = p->cperm.data();
+  const int* rperm = p->rperm.data();
+  upload_permuted(p->cost, f.cost, cperm, 0, n, n); upload_permuted(p->lower, f.lower, cperm, 0, n, n);
+  upload_permuted(p->upper, f.upper, cperm, 0, n, n); upload_permuted(p->colscale, f.col_scale, cperm, 0, n, n);
+  upload_permuted(p->rhs, f.rhs, rperm, 0, m, m); upload_permuted(p->hip.rup, f.row_upper, rperm, 0, m, m);
+  upload_permuted(p->rowscale, f.row_scale, rperm, 0, m, m);
   hipdlp_buffers(p);
   CUDA_OK(cudaDeviceSynchronize());
   lap("setup", "upload + scratch");
@@ -2031,112 +2034,59 @@ static StdForm hip_form_scalars(const StdForm& f) {
 
 // rank g's problem on `device`: A_g, A_g' (build_hipdlp_shard) and every vector full length in the one-GPU device order
 static void create_problem_hipdlp_shard(const StdForm& f, const HipShards& S, int rank, int device, b200pdlp_problem* p) {
-  p->device = device;
-  set_device(p);
-  p->rank = rank; p->world = S.world;
+  open_problem(p, device, rank, S.world);
   p->form = hip_form_scalars(f);
-  p->n = f.n; p->m = f.m; p->ml = f.m; p->r0 = 0; p->r1 = f.m; p->neq_local = f.neq; p->ordered = S.ordered;
-  p->nl = p->nl_real = f.n; p->c0 = 0; p->shard_len = f.n; p->seg_len = f.n;
+  set_full_length_dims(p);
+  p->ordered = S.ordered;
   p->hip_r0 = S.rb[rank]; p->hip_r1 = S.rb[rank + 1]; p->hip_c0 = S.cb[rank]; p->hip_c1 = S.cb[rank + 1];
   if (rank == 0) { p->rperm = S.rperm; p->cperm = S.cperm; }   // the postsolve's un-permutation
   build_hipdlp_shard(S, rank, p->A.host, p->AT.host);
-  CUDA_OK(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
   p->A.upload();
   p->AT.upload();
   const int n = f.n, m = f.m;
-  std::vector<double> t(std::max(std::max(n, m), 1));
-  auto up = [&](DevBuf<double>& d, const std::vector<double>& v, const std::vector<int>& perm) {
-    for (size_t i = 0; i < perm.size(); i++) t[i] = v[perm[i]];
-    d.alloc(perm.size(), false); d.upload(t.data(), perm.size());
-  };
-  up(p->cost, f.cost, S.cperm); up(p->lower, f.lower, S.cperm); up(p->upper, f.upper, S.cperm); up(p->colscale, f.col_scale, S.cperm);
-  up(p->rhs, f.rhs, S.rperm); up(p->hip.rup, f.row_upper, S.rperm); up(p->rowscale, f.row_scale, S.rperm);
+  upload_permuted(p->cost, f.cost, S.cperm.data(), 0, n, n); upload_permuted(p->lower, f.lower, S.cperm.data(), 0, n, n);
+  upload_permuted(p->upper, f.upper, S.cperm.data(), 0, n, n); upload_permuted(p->colscale, f.col_scale, S.cperm.data(), 0, n, n);
+  upload_permuted(p->rhs, f.rhs, S.rperm.data(), 0, m, m); upload_permuted(p->hip.rup, f.row_upper, S.rperm.data(), 0, m, m);
+  upload_permuted(p->rowscale, f.row_scale, S.rperm.data(), 0, m, m);
   hipdlp_buffers(p);
-  p->flags.alloc(kMaxPeers);   // arrival words, one per peer (hip_barrier_kernel)
-  p->epochs.alloc(1);
-  p->fault.alloc(1);
+  alloc_peer_words(p);
   CUDA_OK(cudaDeviceSynchronize());
 }
 
 // The same problems from the device prologue in block mode (DevicePrologue::world > 1): one prologue per device, shared by
-// the ranks that live there.  What no problem adopted is released when the holder goes.
-struct ShardPrologue {
-  int device = 0;
-  cudaStream_t stream = nullptr;
-  DevicePrologue P;
-  ShardPrologue() = default;
-  ShardPrologue(const ShardPrologue&) = delete;
-  ShardPrologue& operator=(const ShardPrologue&) = delete;
-  ~ShardPrologue() {
-    if (stream) { cudaSetDevice(device); cudaStreamSynchronize(stream); cudaStreamDestroy(stream); }
-    P.release_blocks(); P.release_arrays(); P.release_form();
-  }
-};
-
-// formulate, scaling, orderings, the partition and A_g / A_g' of `ranks` on `device`; returns with the stream idle
-static void run_hipdlp_shard_prologue(const b200pdlp_lp& lp, int scaling_mode, int ruiz_iterations, int world, int device,
-                                      const std::vector<int>& ranks, ShardPrologue& SP) {
-  SP.device = device;
-  CUDA_OK(cudaSetDevice(device));
-  CUDA_OK(cudaStreamCreateWithFlags(&SP.stream, cudaStreamNonBlocking));
-  DevicePrologue& P = SP.P;
+// the ranks that live there.  Formulate, scaling, orderings, the partition and A_g / A_g' of `ranks` on the current device;
+// returns with the stream idle.
+static void run_hipdlp_shard_prologue(const b200pdlp_lp& lp, int scaling_mode, int ruiz_iterations, int world,
+                                      const std::vector<int>& ranks, TempPrologue& T) {
+  DevicePrologue& P = T.P;
   P.hipdlp = true;
   P.scaling_mode = scaling_mode;
   P.ruiz_iterations = ruiz_iterations;
   P.world = world;
   P.ranks = ranks;
-  try {
-    P.run(SP.stream, lp, true, /*long_threshold=*/512);
-  } catch (const std::invalid_argument& ex) {
-    throw Error(B200PDLP_ERR_ARG, ex.what());
-  } catch (const std::runtime_error& ex) {
-    throw Error(B200PDLP_ERR_CUDA, ex.what());
-  }
+  run_prologue(P, T.stream, lp, true);
 }
 
 // rank P.ranks[k]'s problem: it adopts its A_g / A_g' and takes its own copies of the full-length device-order vectors
-static void create_problem_hipdlp_shard_device(const b200pdlp_lp& lp, ShardPrologue& SP, int k, b200pdlp_problem* p) {
-  DevicePrologue& P = SP.P;
+static void create_problem_hipdlp_shard_device(const b200pdlp_lp& lp, TempPrologue& T, int k, b200pdlp_problem* p) {
+  DevicePrologue& P = T.P;
   const int g = P.ranks[k];
-  p->device = SP.device;
-  set_device(p);
-  p->rank = g; p->world = P.world;
+  open_problem(p, T.device, g, P.world);
   p->dev_form = true;
-  StdForm& f = p->form;   // the scalars hip_form_scalars gives the host path's ranks
-  f = StdForm();
-  f.hipdlp = true; f.scaled = P.sc.scaled != 0;
-  f.n = P.arr.n; f.m = P.arr.m; f.nnz = P.arr.nnz; f.neq = P.arr.neq; f.n_orig = P.arr.n0;
-  f.sense = lp.sense; f.offset = lp.offset;
-  f.norm_cost = std::sqrt(P.sc.norm_cost_sq); f.norm_rhs = std::sqrt(P.sc.norm_rhs_sq);
-  f.amax = P.sc.amax;
-  const int n = f.n, m = f.m;
-  p->n = n; p->m = m; p->ml = m; p->r0 = 0; p->r1 = m; p->neq_local = f.neq; p->ordered = false;
-  p->nl = p->nl_real = n; p->c0 = 0; p->shard_len = n; p->seg_len = n;
+  take_prologue(lp, P, p);
   p->hip_r0 = P.rb[g]; p->hip_r1 = P.rb[g + 1]; p->hip_c0 = P.cb[g]; p->hip_c1 = P.cb[g + 1];
-  CUDA_OK(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
   adopt_matrix(p->A, P.block_A[k]);
   adopt_matrix(p->AT, P.block_AT[k]);
-  auto dup = [&](DevBuf<double>& d, const double* src, int len) {
-    d.alloc(len, false);
-    if (len > 0) CUDA_OK(cudaMemcpyAsync(d.p, src, (size_t)len * sizeof(double), cudaMemcpyDeviceToDevice, p->stream));
-  };
-  dup(p->cost, P.arr.cost, n); dup(p->lower, P.arr.lower, n); dup(p->upper, P.arr.upper, n); dup(p->colscale, P.arr.colscale, n);
-  dup(p->rhs, P.arr.rhs, m); dup(p->hip.rup, P.arr.rup, m); dup(p->rowscale, P.arr.rowscale, m);
   hipdlp_buffers(p);
-  p->flags.alloc(kMaxPeers);
-  p->epochs.alloc(1);
-  p->fault.alloc(1);
-  if (g == 0) {   // the postsolve's staging
-    p->io_col.alloc((size_t)2 * std::max(f.n_orig, 1), false);
-    p->io_row.alloc((size_t)2 * std::max(m, 1), false);
-  }
+  alloc_peer_words(p);
+  if (g == 0) alloc_postsolve_staging(p);
   CUDA_OK(cudaStreamSynchronize(p->stream));
 }
 
 // rank 0 keeps the maps of the formulation and the row-major copy of the caller's matrix for the device postsolve; the
 // device-order vectors were copied by every rank
-static void hand_over_postsolve_maps(ShardPrologue& SP, b200pdlp_problem* p0) {
-  DevProblemArrays& a = SP.P.arr;
+static void hand_over_postsolve_maps(TempPrologue& T, b200pdlp_problem* p0) {
+  DevProblemArrays& a = T.P.arr;
   for (double** v : {&a.cost, &a.lower, &a.upper, &a.colscale, &a.rhs, &a.rowscale, &a.rup}) { dev_cache_free(*v); *v = nullptr; }
   p0->prep.arr = a;
   a = DevProblemArrays();
@@ -2470,6 +2420,29 @@ static int guarded(F&& fn) {
   }
 }
 
+// fn(i) for i < count, one host thread each.  After every thread has joined, the first failure is rethrown with its code
+// and "<label> <id>: " before its message (id = ids[i], or i).
+template <class F>
+static void run_per_rank(int count, const char* label, F&& fn, const int* ids = nullptr) {
+  std::vector<int> codes((size_t)count, B200PDLP_OK);
+  std::vector<std::string> msgs((size_t)count);
+  std::vector<std::thread> th;
+  for (int i = 0; i < count; i++)
+    th.emplace_back([&, i] {
+      codes[i] = guarded([&] { fn(i); });
+      if (codes[i] != B200PDLP_OK) msgs[i] = g_last_error;   // thread-local: hand it to the caller's thread
+    });
+  for (auto& t : th) t.join();
+  for (int i = 0; i < count; i++)
+    if (codes[i] != B200PDLP_OK) throw Error(codes[i], std::string(label) + " " + std::to_string(ids ? ids[i] : i) + ": " + msgs[i]);
+}
+
+// owning handle of a problem: deleted with its own device selected
+struct ProblemDeleter {
+  void operator()(b200pdlp_problem* p) const { cudaSetDevice(p->device); delete p; }
+};
+using ProblemPtr = std::unique_ptr<b200pdlp_problem, ProblemDeleter>;
+
 static void check_params(const b200pdlp_params& prm) {
   if (prm.device_scaling != 0 && prm.device_scaling != -1)
     throw Error(B200PDLP_ERR_ARG, "b200pdlp: params.device_scaling must be 0 (default) or -1 (host prologue)");
@@ -2511,26 +2484,17 @@ static void create_hipdlp_shards_device(const b200pdlp_lp& lp, const b200pdlp_hi
   std::vector<int> devices;   // distinct, in the order of their first rank
   for (int d : dev)
     if (std::find(devices.begin(), devices.end(), d) == devices.end()) devices.push_back(d);
-  std::vector<int> codes(devices.size(), B200PDLP_OK);
-  std::vector<std::string> msgs(devices.size());
-  std::vector<std::thread> th;
-  for (size_t i = 0; i < devices.size(); i++)
-    th.emplace_back([&, i] {
-      codes[i] = guarded([&] {
-        std::vector<int> ranks;
-        for (int g = 0; g < world; g++)
-          if (dev[g] == devices[i]) ranks.push_back(g);
-        ShardPrologue SP;
-        run_hipdlp_shard_prologue(lp, prm.scaling_mode, prm.ruiz_iterations, world, devices[i], ranks, SP);
-        for (size_t k = 0; k < ranks.size(); k++) create_problem_hipdlp_shard_device(lp, SP, (int)k, probs[ranks[k]]);
-        if (ranks[0] == 0) hand_over_postsolve_maps(SP, probs[0]);
-        CUDA_OK(cudaDeviceSynchronize());
-      });   // (SP has released the standard form, the orderings and the other temporaries of this device)
-      if (codes[i] != B200PDLP_OK) msgs[i] = g_last_error;   // thread-local: hand it to the caller's thread
-    });
-  for (auto& t : th) t.join();
-  for (size_t i = 0; i < devices.size(); i++)
-    if (codes[i] != B200PDLP_OK) throw Error(codes[i], "device " + std::to_string(devices[i]) + ": " + msgs[i]);
+  run_per_rank((int)devices.size(), "device", [&](int i) {
+    std::vector<int> ranks;
+    for (int g = 0; g < world; g++)
+      if (dev[g] == devices[i]) ranks.push_back(g);
+    CUDA_OK(cudaSetDevice(devices[i]));
+    TempPrologue T;
+    run_hipdlp_shard_prologue(lp, prm.scaling_mode, prm.ruiz_iterations, world, ranks, T);
+    for (size_t k = 0; k < ranks.size(); k++) create_problem_hipdlp_shard_device(lp, T, (int)k, probs[ranks[k]]);
+    if (ranks[0] == 0) hand_over_postsolve_maps(T, probs[0]);
+    CUDA_OK(cudaDeviceSynchronize());
+  }, devices.data());   // (T has released the standard form, the orderings and the other temporaries of this device)
 }
 
 extern "C" {
@@ -2917,21 +2881,14 @@ int b200pdlp_solve(const b200pdlp_lp* lp, const b200pdlp_params* params, const b
     check_lp(lp, false);
     check_lp(lp, !use_device_prep(*lp, *params, 1));
     const auto t0 = std::chrono::steady_clock::now();
-    b200pdlp_problem* p = new b200pdlp_problem();
-    try {
-      if (use_device_prep(*lp, *params, 1)) create_problem_device(*lp, *params, p);
-      else create_problem(*lp, *params, 0, 1, p);
-      out->setup_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-      solve_on_device(p, *params, warm, out);
-      CUDA_OK(cudaGetLastError());
-    } catch (...) {
-      cudaSetDevice(p->device);
-      delete p;
-      throw;
-    }
-    cudaSetDevice(p->device);
+    ProblemPtr p(new b200pdlp_problem());
+    if (use_device_prep(*lp, *params, 1)) create_problem_device(*lp, *params, p.get());
+    else create_problem(*lp, *params, 0, 1, p.get());
+    out->setup_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    solve_on_device(p.get(), *params, warm, out);
+    CUDA_OK(cudaGetLastError());
     Laps lap;
-    delete p;
+    p.reset();
     lap("solve", "teardown");
   });
 }
@@ -2945,16 +2902,17 @@ int b200pdlp_solve_multi(const b200pdlp_lp* lp, const b200pdlp_params* params, c
   // fixed-step mode needs the power method, which is single-GPU (power_method): fall back instead of failing
   if (params && params->adaptive_step == 0) return b200pdlp_solve(lp, params, warm, out);
   DeviceGuard dg;
-  std::vector<b200pdlp_problem*> probs((size_t)ngpus, nullptr);
+  std::vector<ProblemPtr> owned;
   const int rc = guarded([&] {
     check_lp(lp);
     if (!params || !out || ngpus > kMaxPeers) throw Error(B200PDLP_ERR_ARG, "b200pdlp_solve_multi: bad arguments");
     check_params(*params);
     const auto t0 = std::chrono::steady_clock::now();
+    std::vector<b200pdlp_problem*> probs((size_t)ngpus, nullptr);
     for (int g = 0; g < ngpus; g++) {
       b200pdlp_params prm = *params;
       prm.device = devices ? devices[g] : g;
-      probs[g] = new b200pdlp_problem();
+      owned.emplace_back(probs[g] = new b200pdlp_problem());
       create_problem(*lp, prm, g, ngpus, probs[g], g == 0 ? nullptr : &probs[0]->form);
     }
     const int lrc = b200pdlp_p2p_link_local(probs.data(), ngpus);
@@ -2964,8 +2922,6 @@ int b200pdlp_solve_multi(const b200pdlp_lp* lp, const b200pdlp_params* params, c
     const size_t n = (size_t)std::max(lp->num_col, 1), m = (size_t)std::max(lp->num_row, 1);
     std::vector<std::vector<double>> scratch((size_t)ngpus);
     std::vector<b200pdlp_result> res((size_t)ngpus);
-    std::vector<int> codes((size_t)ngpus, B200PDLP_OK);
-    std::vector<std::string> msgs((size_t)ngpus);
     for (int g = 0; g < ngpus; g++) {
       res[g] = *out;
       res[g].setup_seconds = 0.0;
@@ -2976,22 +2932,16 @@ int b200pdlp_solve_multi(const b200pdlp_lp* lp, const b200pdlp_params* params, c
         res[g].trace = nullptr; res[g].trace_cap = 0;
       }
     }
-    std::vector<std::thread> th;
-    for (int g = 0; g < ngpus; g++)
-      th.emplace_back([&, g] {
-        b200pdlp_params prm = *params;
-        prm.device = probs[g]->device;
-        codes[g] = guarded([&] { solve_on_device(probs[g], prm, warm, &res[g]); CUDA_OK(cudaGetLastError()); });
-        if (codes[g] != B200PDLP_OK) msgs[g] = g_last_error;   // thread-local: hand it to the caller's thread
-      });
-    for (auto& t : th) t.join();
-    for (int g = 0; g < ngpus; g++)
-      if (codes[g] != B200PDLP_OK) throw Error(codes[g], "rank " + std::to_string(g) + ": " + msgs[g]);
+    run_per_rank(ngpus, "rank", [&](int g) {
+      b200pdlp_params prm = *params;
+      prm.device = probs[g]->device;
+      solve_on_device(probs[g], prm, warm, &res[g]);
+      CUDA_OK(cudaGetLastError());
+    });
     *out = res[0];
     out->setup_seconds += setup;
   });
-  for (b200pdlp_problem* p : probs)
-    if (p) { cudaSetDevice(p->device); p->p2p = false; delete p; }
+  for (ProblemPtr& p : owned) p->p2p = false;
   return rc;
 }
 
@@ -3028,19 +2978,11 @@ int b200pdlp_solve_hipdlp(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params* p
     check_lp(lp);
     if (!params || !out) throw Error(B200PDLP_ERR_ARG, "null argument");
     const auto t0 = std::chrono::steady_clock::now();
-    b200pdlp_problem* p = new b200pdlp_problem();
-    try {
-      create_problem_hipdlp(*lp, *params, p);
-      out->setup_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-      solve_hipdlp_on_device(p, *lp, *params, out);
-      CUDA_OK(cudaGetLastError());
-    } catch (...) {
-      cudaSetDevice(p->device);
-      delete p;
-      throw;
-    }
-    cudaSetDevice(p->device);
-    delete p;
+    ProblemPtr p(new b200pdlp_problem());
+    create_problem_hipdlp(*lp, *params, p.get());
+    out->setup_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    solve_hipdlp_on_device(p.get(), *lp, *params, out);
+    CUDA_OK(cudaGetLastError());
   });
 }
 
@@ -3051,14 +2993,10 @@ int b200pdlp_solve_hipdlp_multi(const b200pdlp_lp* lp, const b200pdlp_hipdlp_par
                                 int32_t ngpus, const int32_t* devices) {
   if (ngpus <= 1) return b200pdlp_solve_hipdlp(lp, params, out);
   DeviceGuard dg;
-  std::vector<b200pdlp_problem*> probs;
-  const int rc = guarded([&] {
+  return guarded([&] {
     check_lp(lp);
     if (!params || !out || ngpus > kMaxPeers) throw Error(B200PDLP_ERR_ARG, "b200pdlp_solve_hipdlp_multi: bad arguments");
-    int ndev = 0;
-    const cudaError_t e = cudaGetDeviceCount(&ndev);
-    if (e != cudaSuccess || ndev == 0)
-      throw Error(B200PDLP_ERR_CUDA, std::string("no CUDA device: the engine has no CPU fallback (") + cudaGetErrorString(e) + ")");
+    const int ndev = device_count_checked();
     std::vector<int> dev(ngpus);
     for (int g = 0; g < ngpus; g++) {
       dev[g] = devices ? devices[g] : g;
@@ -3073,8 +3011,9 @@ int b200pdlp_solve_hipdlp_multi(const b200pdlp_lp* lp, const b200pdlp_hipdlp_par
         }
     const auto t0 = std::chrono::steady_clock::now();
     Laps lap;
-    probs.assign(ngpus, nullptr);
-    for (int g = 0; g < ngpus; g++) probs[g] = new b200pdlp_problem();
+    std::vector<ProblemPtr> owned;
+    std::vector<b200pdlp_problem*> probs;
+    for (int g = 0; g < ngpus; g++) { owned.emplace_back(new b200pdlp_problem()); probs.push_back(owned.back().get()); }
     if (use_device_prep_hipdlp(*lp, *params)) {
       create_hipdlp_shards_device(*lp, *params, dev, probs);
       lap("setup", "HiPDLP shards: device prologue");
@@ -3106,27 +3045,17 @@ int b200pdlp_solve_hipdlp_multi(const b200pdlp_lp* lp, const b200pdlp_hipdlp_par
     const double setup = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
     // rank 0 writes the caller's arrays; the other ranks' results carry no vectors
     std::vector<b200pdlp_result> res((size_t)ngpus, *out);
-    std::vector<int> codes((size_t)ngpus, B200PDLP_OK);
-    std::vector<std::string> msgs((size_t)ngpus);
     for (int g = 0; g < ngpus; g++) {
       res[g].setup_seconds = 0.0;
       if (g > 0) { res[g].col_value = res[g].col_dual = res[g].row_value = res[g].row_dual = nullptr; res[g].trace = nullptr; res[g].trace_cap = 0; }
     }
-    std::vector<std::thread> th;
-    for (int g = 0; g < ngpus; g++)
-      th.emplace_back([&, g] {
-        codes[g] = guarded([&] { solve_hipdlp_on_device(probs[g], *lp, *params, &res[g]); CUDA_OK(cudaGetLastError()); });
-        if (codes[g] != B200PDLP_OK) msgs[g] = g_last_error;   // thread-local: hand it to the caller's thread
-      });
-    for (auto& t : th) t.join();
-    for (int g = 0; g < ngpus; g++)
-      if (codes[g] != B200PDLP_OK) throw Error(codes[g], "rank " + std::to_string(g) + ": " + msgs[g]);
+    run_per_rank(ngpus, "rank", [&](int g) {
+      solve_hipdlp_on_device(probs[g], *lp, *params, &res[g]);
+      CUDA_OK(cudaGetLastError());
+    });
     *out = res[0];
     out->setup_seconds += setup;
   });
-  for (b200pdlp_problem* p : probs)
-    if (p) { cudaSetDevice(p->device); delete p; }
-  return rc;
 }
 
 int b200pdlp_hipdlp_shard_layout_eval(b200pdlp_form* fh, int32_t rank, int32_t world, int32_t ordered_max, const double* x,
@@ -3506,14 +3435,10 @@ int b200pdlp_debug_prep_compare(const b200pdlp_lp* lp, int32_t scaling, double r
     if (f.rptr.empty()) build_row_index(f);
     HostLayout L;
     build_layout(f, 0, 1, /*ordered_max=*/-1, L);
-    cudaStream_t s = nullptr;
-    CUDA_OK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
-    DevicePrologue P;
-    P.keep_form = true;
-    struct Cleanup { DevicePrologue& P; cudaStream_t s; ~Cleanup() { P.A.release(); P.AT.release(); P.release_arrays(); P.release_form(); cudaStreamDestroy(s); } } cleanup{P, s};
-    try { P.run(s, *lp, scaling != 0, 512); }
-    catch (const std::exception& ex) { throw Error(B200PDLP_ERR_CUDA, ex.what()); }
-    prep_compare_arrays(P, f, L, report);
+    TempPrologue T;
+    T.P.keep_form = true;
+    run_prologue(T.P, T.stream, *lp, scaling != 0);
+    prep_compare_arrays(T.P, f, L, report);
   });
 }
 
@@ -3531,16 +3456,13 @@ int b200pdlp_debug_prep_compare_hipdlp(const b200pdlp_lp* lp, int32_t scaling_mo
     if (f.rptr.empty()) build_row_index(f);
     HostLayout L;
     build_layout(f, 0, 1, /*ordered_max=*/-1, L);
-    cudaStream_t s = nullptr;
-    CUDA_OK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
-    DevicePrologue P;
+    TempPrologue T;
+    DevicePrologue& P = T.P;
     P.keep_form = true;
     P.hipdlp = true;
     P.scaling_mode = scaling_mode;
     P.ruiz_iterations = ruiz_iterations;
-    struct Cleanup { DevicePrologue& P; cudaStream_t s; ~Cleanup() { P.A.release(); P.AT.release(); P.release_arrays(); P.release_form(); cudaStreamDestroy(s); } } cleanup{P, s};
-    try { P.run(s, *lp, true, 512); }
-    catch (const std::exception& ex) { throw Error(B200PDLP_ERR_CUDA, ex.what()); }
+    run_prologue(P, T.stream, *lp, true);
     if (!prep_compare_arrays(P, f, L, report)) return;
     const int m = f.m, n0 = lp->num_col, nnz0 = lp->a_start[n0];
     // the norms set omega and both step sizes: bitwise
@@ -3584,13 +3506,11 @@ int b200pdlp_debug_hipdlp_shard_prep_compare(const b200pdlp_lp* lp, int32_t scal
     scale_hipdlp(f, scaling_mode, ruiz_iterations);
     HipShards S;
     plan_hipdlp_shards(f, world, /*ordered_max=*/-1, S);
-    int device = 0;
-    CUDA_OK(cudaGetDevice(&device));
     std::vector<int> ranks(world);
     for (int g = 0; g < world; g++) ranks[g] = g;
-    ShardPrologue SP;
-    run_hipdlp_shard_prologue(*lp, scaling_mode, ruiz_iterations, world, device, ranks, SP);
-    const DevicePrologue& P = SP.P;
+    TempPrologue T;
+    run_hipdlp_shard_prologue(*lp, scaling_mode, ruiz_iterations, world, ranks, T);
+    const DevicePrologue& P = T.P;
     const DevProblemArrays& a = P.arr;
     const int n = f.n, m = f.m;
     report[0] = (a.n != n) + (a.m != m) + (a.nnz != f.nnz) + (a.neq != f.neq);
