@@ -11,6 +11,7 @@
 #include <nccl.h>   // types only: the library is bound at run time (see NcclApi below)
 
 #include <algorithm>
+#include <atomic>
 #include <chrono>
 #include <cstddef>
 #include <cmath>
@@ -26,6 +27,7 @@
 #include <thread>
 #include <vector>
 
+#include "batch_kernels.hpp"
 #include "device_prep.hpp"
 #include "host_prep.hpp"
 #include "pdhg_kernels.hpp"
@@ -581,16 +583,17 @@ static void alloc_postsolve_staging(b200pdlp_problem* p) {
 // The size rule of both device prologues.  Ordered mode keeps the host prologue; it is decided on the STANDARD FORM's size,
 // n = num_col + one slack column per ranged or free row (CupdlpWrapper.cpp:328-345; `inf` is the mode's infinite row bound),
 // so count them when the answer depends on it.  An empty matrix keeps it too.
+static int std_form_cols(const b200pdlp_lp& lp, double inf) {
+  int nslack = 0;
+  for (int i = 0; i < lp.num_row; i++) {
+    const bool lo = lp.row_lower[i] > -inf, up = lp.row_upper[i] < inf;
+    nslack += (lo && up && lp.row_lower[i] != lp.row_upper[i]) || (!lo && !up);
+  }
+  return lp.num_col + nslack;
+}
 static bool device_prep_fits(const b200pdlp_lp& lp, int ordered_max, double inf) {
   const int omax = ordered_max == 0 ? 4096 : ordered_max;
-  if (omax > 0 && lp.num_col <= omax && lp.num_row <= omax) {
-    int nslack = 0;
-    for (int i = 0; i < lp.num_row; i++) {
-      const bool lo = lp.row_lower[i] > -inf, up = lp.row_upper[i] < inf;
-      nslack += (lo && up && lp.row_lower[i] != lp.row_upper[i]) || (!lo && !up);
-    }
-    if (lp.num_col + nslack <= omax) return false;
-  }
+  if (omax > 0 && lp.num_col <= omax && lp.num_row <= omax && std_form_cols(lp, inf) <= omax) return false;
   return lp.num_col > 0 && lp.num_row > 0 && lp.a_start[lp.num_col] > 0;
 }
 
@@ -954,6 +957,41 @@ static void enqueue_check_dev(b200pdlp_problem* p, bool timed_out_local) {
   CUDA_OK(cudaMemcpyAsync(p->houts, o, 29 * sizeof(double), cudaMemcpyDeviceToHost, s));
 }
 
+// Ordered-mode check, host arithmetic on the sums of sweeps A (o[0..20]: 7 column sums, then 3 row sums, per iterate):
+// residuals of both iterates and the ray scales sweeps B need
+static void assemble_check_a(const StdForm& f, const double* o, CheckResult& cr, double dscale[2], double pscale[2]) {
+  for (int t = 0; t < 2; t++) {
+    const double* a = o + 7 * t;
+    const double* r = o + 14 + 3 * t;
+    Residuals& R = cr.it[t];
+    R.pobj = a[0] * f.sense + f.offset;                        // cupdlp_solver.c:24
+    R.pfeas = std::sqrt(r[1]);
+    double d = r[0];                                           // :79
+    d += a[1];                                                 // :92 / :164
+    d -= a[2];                                                 // :98 / :180
+    R.dobj = d * f.sense + f.offset;                           // :100 / :182
+    R.dfeas = std::sqrt(a[3]);
+    R.gap = R.pobj - R.dobj;                                   // :513-516
+    R.relgap = std::fabs(R.pobj - R.dobj) / (1.0 + std::fabs(R.pobj) + std::fabs(R.dobj));
+    dscale[t] = std::sqrt(r[2] + a[4] + a[5]);                 // :262-266
+    if (dscale[t] < 1e-8) dscale[t] = 1.0;
+    pscale[t] = std::sqrt(a[6]);                               // :367-371
+    if (pscale[t] < 1e-8) pscale[t] = 1.0;
+  }
+}
+
+// ... and on the sums of sweeps B (o[24..29]: 3 column sums per iterate, o[30..31]: 1 row sum per iterate): the ray residuals
+static void assemble_check_b(const StdForm& f, const double* o, CheckResult& cr, const double dscale[2], const double pscale[2]) {
+  for (int t = 0; t < 2; t++) {
+    Residuals& R = cr.it[t];
+    const double* b = o + 24 + 3 * t;
+    R.pinf_obj = (R.dobj - f.offset) / f.sense / dscale[t];    // :282-283
+    R.pinf_res = std::sqrt(b[0]);
+    R.dinf_obj = (R.pobj - f.offset) / f.sense / pscale[t];    // :376-377
+    R.dinf_res = std::sqrt(o[30 + t] + b[1] + b[2]);           // :425
+  }
+}
+
 // PDHG_Compute_Average_Iterate + PDHG_Compute_Residuals + PDHG_Compute_Infeas_Residuals
 // (cupdlp_step.c:377-420, cupdlp_solver.c:473-529, :433-471) for current and average iterate
 static CheckResult run_check(b200pdlp_problem* p, bool timed_out_local) {
@@ -1023,23 +1061,8 @@ static CheckResult run_check(b200pdlp_problem* p, bool timed_out_local) {
   CheckResult cr;
   cr.timed_out = p->world > 1 ? p->houts[20] > 0.0 : timed_out_local;
   double inv_d[2], inv_p[2], dscale[2], pscale[2];
+  assemble_check_a(f, p->houts, cr, dscale, pscale);
   for (int t = 0; t < 2; t++) {
-    const double* a = p->houts + 7 * t;
-    const double* r = p->houts + 14 + 3 * t;
-    Residuals& R = cr.it[t];
-    R.pobj = a[0] * f.sense + f.offset;                        // cupdlp_solver.c:24
-    R.pfeas = std::sqrt(r[1]);
-    double d = r[0];                                           // :79
-    d += a[1];                                                 // :92 / :164
-    d -= a[2];                                                 // :98 / :180
-    R.dobj = d * f.sense + f.offset;                           // :100 / :182
-    R.dfeas = std::sqrt(a[3]);
-    R.gap = R.pobj - R.dobj;                                   // :513-516
-    R.relgap = std::fabs(R.pobj - R.dobj) / (1.0 + std::fabs(R.pobj) + std::fabs(R.dobj));
-    dscale[t] = std::sqrt(r[2] + a[4] + a[5]);                 // :262-266
-    if (dscale[t] < 1e-8) dscale[t] = 1.0;
-    pscale[t] = std::sqrt(a[6]);                               // :367-371
-    if (pscale[t] < 1e-8) pscale[t] = 1.0;
     inv_d[t] = 1 / dscale[t];
     inv_p[t] = 1.0 / pscale[t];
   }
@@ -1050,14 +1073,7 @@ static CheckResult run_check(b200pdlp_problem* p, bool timed_out_local) {
   if (p->world > 1) allreduce_inplace(p, o + 24, 8);
   CUDA_OK(cudaMemcpyAsync(p->houts + 24, o + 24, 8 * sizeof(double), cudaMemcpyDeviceToHost, s));
   CUDA_OK(cudaStreamSynchronize(s));
-  for (int t = 0; t < 2; t++) {
-    Residuals& R = cr.it[t];
-    const double* b = p->houts + 24 + 3 * t;
-    R.pinf_obj = (R.dobj - f.offset) / f.sense / dscale[t];    // :282-283
-    R.pinf_res = std::sqrt(b[0]);
-    R.dinf_obj = (R.pobj - f.offset) / f.sense / pscale[t];    // :376-377
-    R.dinf_res = std::sqrt(p->houts[30 + t] + b[1] + b[2]);    // :425
-  }
+  assemble_check_b(f, p->houts, cr, dscale, pscale);
   return cr;
 }
 
@@ -1093,6 +1109,24 @@ static int decide_restart(const PdhgState* h, const CheckResult& c, RestartMemo&
   return choice;
 }
 
+// the host part of a restart, given |x - x_lr|^2 and |y - y_lr|^2 of the iterate restarted to: the memo, the step sum, and
+// beta / tau / sigma (glibc log / exp, which the device's do not reproduce)
+static void restart_steps(PdhgState* h, int choice, const CheckResult& c, RestartMemo& mm, double dx2, double dy2) {
+  h->sum_step = 0.0;
+  const Residuals& R = choice == 1 ? c.it[1] : c.it[0];
+  mm.pf_lr = R.pfeas; mm.df_lr = R.dfeas; mm.gap_lr = R.gap;
+  const double mean = std::sqrt(h->tau * h->sigma);
+  const double dxn = std::sqrt(dx2), dyn = std::sqrt(dy2);
+  if (std::fmin(dxn, dyn) > 1e-10) {
+    const double upd = dyn / dxn;
+    const double lg = 0.5 * std::log(upd) + 0.5 * std::log(std::sqrt(h->beta));
+    h->beta = std::exp(lg) * std::exp(lg);
+  }
+  h->tau = mean / std::sqrt(h->beta);
+  h->sigma = h->tau * h->beta;
+  mm.last_iter = h->iter;
+}
+
 // PDHG_Restart_Iterate_GPU (cupdlp_proj.c:88-148) + PDHG_Compute_Step_Size_Ratio (cupdlp_step.c:147-176)
 static void do_restart(b200pdlp_problem* p, int choice, const CheckResult& c, RestartMemo& mm) {
   NvtxRange nvtx("b200pdlp: restart");
@@ -1100,11 +1134,8 @@ static void do_restart(b200pdlp_problem* p, int choice, const CheckResult& c, Re
   PdhgState* h = p->hstate;
   const int n = p->nl, ml = p->ml, cur = h->cur;
   const int acur = p->world == 1 ? cur : 0;
-  h->sum_step = 0.0;
   CUDA_OK(cudaMemsetAsync(p->xsum.p, 0, (size_t)n * sizeof(double), s));
   CUDA_OK(cudaMemsetAsync(p->ysum.p, 0, (size_t)std::max(ml, 1) * sizeof(double), s));
-  const Residuals& R = choice == 1 ? c.it[1] : c.it[0];
-  mm.pf_lr = R.pfeas; mm.df_lr = R.dfeas; mm.gap_lr = R.gap;
   if (choice == 1) {
     CUDA_OK(cudaMemcpyAsync(p->x[cur].p, p->xavg.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, s));
     CUDA_OK(cudaMemcpyAsync(p->y[cur].p, p->yavg.p, (size_t)ml * sizeof(double), cudaMemcpyDeviceToDevice, s));
@@ -1120,16 +1151,7 @@ static void do_restart(b200pdlp_problem* p, int choice, const CheckResult& c, Re
   CUDA_OK(cudaMemcpyAsync(p->xlr.p, p->x[cur].p, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, s));
   CUDA_OK(cudaMemcpyAsync(p->ylr.p, p->y[cur].p, (size_t)ml * sizeof(double), cudaMemcpyDeviceToDevice, s));
   CUDA_OK(cudaStreamSynchronize(s));
-  const double mean = std::sqrt(h->tau * h->sigma);
-  const double dxn = std::sqrt(p->houts[40]), dyn = std::sqrt(p->houts[41]);
-  if (std::fmin(dxn, dyn) > 1e-10) {
-    const double upd = dyn / dxn;
-    const double lg = 0.5 * std::log(upd) + 0.5 * std::log(std::sqrt(h->beta));
-    h->beta = std::exp(lg) * std::exp(lg);
-  }
-  h->tau = mean / std::sqrt(h->beta);
-  h->sigma = h->tau * h->beta;
-  mm.last_iter = h->iter;
+  restart_steps(h, choice, c, mm, p->houts[40], p->houts[41]);
 }
 
 // state for the next pass after the host touched tau/sigma/beta (start of
@@ -1175,6 +1197,119 @@ static double power_method(b200pdlp_problem* p) {
     lambda = vec_norm2_sq(p, p->aty[0].p, p->n, false);
   }
   return lambda;
+}
+
+// What a check decides (cupdlp_solver.c:939-1106): a termination code, or -1 to go on (then *choice = the restart decided,
+// 0 none, 1 to the average, 2 to the current iterate).  chk.timed_out: the time limit had passed when the check began.
+static int check_decision(const b200pdlp_params& prm, double tol_p, double tol_d, const PdhgState* h, const CheckResult& chk,
+                          RestartMemo& memo, int* term_iterate, int* choice) {
+  const Residuals &L = chk.it[0], &A = chk.it[1];
+  *choice = 0;
+  if (L.pfeas < tol_p && L.dfeas < tol_d && L.relgap < prm.tol_gap) { *term_iterate = 0; return B200PDLP_OPTIMAL; }
+  if (A.pfeas < tol_p && A.dfeas < tol_d && A.relgap < prm.tol_gap) { *term_iterate = 1; return B200PDLP_OPTIMAL; }
+  {  // PDHG_Check_Infeasibility, cupdlp_solver.c:740-795 (dFeasTol = 1e-8, cupdlp_utils.c:889)
+    const double ft = 1e-8;
+    bool inf = false;
+    for (int t = 0; t < 2; t++) {
+      const Residuals& R = chk.it[t];
+      if (R.pinf_obj > 0.0 && R.pinf_res < ft * R.pinf_obj) inf = true;
+      if (R.dinf_obj < 0.0 && R.dinf_res < -ft * R.dinf_obj) inf = true;
+    }
+    if (inf) return B200PDLP_INFEASIBLE_OR_UNBOUNDED;
+  }
+  if (chk.timed_out) return B200PDLP_TIMELIMIT_OR_ITERLIMIT;
+  if (h->iter >= prm.iter_limit - 1) return B200PDLP_TIMELIMIT_OR_ITERLIMIT;
+  if (prm.restart) *choice = decide_restart(h, chk, memo);
+  return -1;
+}
+
+// the next check iteration: < 10, multiple of the interval, or iter_limit - 1 (cupdlp_solver.c:953-962)
+static int next_check_iter(int iter, int interval, int iter_limit) {
+  int next = iter + 1;
+  while (!(next < 10 || next % interval == 0 || next == iter_limit - 1)) next++;
+  return next;
+}
+
+// PDHG_PreSolve's hot start (cupdlp_solver.c:1217-1279) + PDHG_Project_Bounds in standard-form order: x0[n], y0[m] (zero
+// without a complete hot start)
+static void host_start_point(const StdForm& f, const b200pdlp_warm* warm, std::vector<double>& x0, std::vector<double>& y0) {
+  const int n = f.n, m = f.m;
+  x0.assign(n, 0.0);
+  y0.assign(m, 0.0);
+  if (warm && warm->col_value && warm->row_value && warm->row_dual) {
+    int jc = 0;
+    for (; jc < f.n_orig; jc++) x0[jc] = warm->col_value[jc];
+    for (int i = 0; i < m; i++) {
+      const double mu = f.row_class[i] == kLeq ? -1 : 1;
+      y0[f.row_new_idx[i]] = f.sense * mu * warm->row_dual[i];
+      if (f.row_class[i] == kBound) x0[jc++] = warm->row_value[i];
+    }
+    for (int j = 0; j < n; j++) x0[j] *= f.col_scale[j];
+    for (int i = 0; i < m; i++) y0[i] *= f.row_scale[i];
+  }
+  for (int j = 0; j < n; j++) {  // PDHG_Project_Bounds: upper first, then lower
+    double v = x0[j];
+    v = v < f.upper[j] ? v : f.upper[j];
+    v = v > f.lower[j] ? v : f.lower[j];
+    x0[j] = v;
+  }
+}
+
+// proj(0) of column j: where xSum starts (PDHG_Init_Variables, cupdlp_solver.c:577-583)
+static double proj_zero(const StdForm& f, int j) {
+  double v = 0.0;
+  v = v < f.upper[j] ? v : f.upper[j];
+  v = v > f.lower[j] ? v : f.lower[j];
+  return v;
+}
+
+// PDHG_PostSolve (cupdlp_solver.c:1281-1435) on the host: x, y, A x, A'y of the returned iterate in standard-form order ->
+// the four HighsSolution vectors in `out` (scaled in place)
+static void host_postsolve(const StdForm& f, bool have_check, std::vector<double>& hx, std::vector<double>& hy,
+                           std::vector<double>& hax, const std::vector<double>& haty, b200pdlp_result* out) {
+  const int n = f.n, m = f.m;
+  const double inf = std::numeric_limits<double>::infinity();
+  if (!(out->col_value && out->col_dual && out->row_value && out->row_dual)) return;
+  std::vector<double> sp(n, 0.0), sn(n, 0.0);
+  if (have_check) {
+    for (int j = 0; j < n; j++) {   // dSlackPos / dSlackNeg of the returned iterate (cupdlp_solver.c:150-176)
+      double rc = haty[j] * -1.0;
+      rc = rc + 1.0 * f.cost[j];
+      double a = rc > 0.0 ? rc : 0.0;
+      a = a * (f.lower[j] > -inf ? 1.0 : 0.0);
+      double b = rc < 0.0 ? rc : 0.0;
+      b = b * -1.0;
+      b = b * (f.upper[j] < inf ? 1.0 : 0.0);
+      sp[j] = a; sn[j] = b;
+    }
+  }
+  for (int j = 0; j < n; j++) { hx[j] /= f.col_scale[j]; sp[j] *= f.col_scale[j]; sn[j] *= f.col_scale[j]; }
+  for (int i = 0; i < m; i++) { hy[i] /= f.row_scale[i]; hax[i] *= f.row_scale[i]; }
+  for (int j = 0; j < f.n_orig; j++) out->col_value[j] = hx[j];
+  for (int i = 0, j = 0; i < m; i++) {
+    double v = hax[f.row_new_idx[i]];
+    if (f.row_class[i] == kLeq) v = -v;
+    else if (f.row_class[i] == kBound) { v = v + hx[f.n_orig + j]; j++; }
+    out->row_value[i] = v;
+  }
+  for (int j = 0; j < f.n_orig; j++) { double v = sp[j] - sn[j]; out->col_dual[j] = v * f.sense; }
+  for (int i = 0; i < m; i++) {
+    double v = hy[f.row_new_idx[i]] * f.sense;
+    if (f.row_class[i] == kLeq) v = -v;
+    out->row_dual[i] = v;
+  }
+}
+
+// the per-solve fields of a result (the timings and kernel_launches are the caller's)
+static void fill_result(b200pdlp_result* out, const StdForm& f, const PdhgState* h, int term, int term_iterate, int restarts,
+                        const CheckResult& chk) {
+  out->value_valid = 1; out->dual_valid = 1;
+  out->term_code = term; out->term_iterate = term_iterate;
+  out->iters = h->iter; out->passes = h->passes; out->restarts = restarts;
+  const Residuals& R = chk.it[(term == B200PDLP_OPTIMAL && term_iterate == 1) ? 1 : 0];
+  out->primal_obj = R.pobj; out->dual_obj = R.dobj; out->primal_feas = R.pfeas; out->dual_feas = R.dfeas;
+  out->gap = R.gap; out->rel_gap = R.relgap;
+  out->form_cols = f.n; out->form_rows = f.m; out->form_nnz = f.nnz; out->form_neq = f.neq;
 }
 
 static void trace_row(b200pdlp_result* out, const PdhgState* h, const CheckResult& c, int restart) {
@@ -1414,24 +1549,8 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
 
   // ---- initial point: PDHG_PreSolve (hot start, cupdlp_solver.c:1217-1279) + PDHG_Init_Variables (:531-591)
   const bool dev_form = p->dev_form;
-  std::vector<double> x0(dev_form ? 0 : n, 0.0), y0(dev_form ? 0 : m, 0.0);
-  if (!dev_form && warm && warm->col_value && warm->row_value && warm->row_dual) {
-    int jc = 0;
-    for (; jc < f.n_orig; jc++) x0[jc] = warm->col_value[jc];
-    for (int i = 0; i < m; i++) {
-      const double mu = f.row_class[i] == kLeq ? -1 : 1;
-      y0[f.row_new_idx[i]] = f.sense * mu * warm->row_dual[i];
-      if (f.row_class[i] == kBound) x0[jc++] = warm->row_value[i];
-    }
-    for (int j = 0; j < n; j++) x0[j] *= f.col_scale[j];
-    for (int i = 0; i < m; i++) y0[i] *= f.row_scale[i];
-  }
-  for (int j = 0; j < (dev_form ? 0 : n); j++) {  // PDHG_Project_Bounds: upper first, then lower
-    double v = x0[j];
-    v = v < f.upper[j] ? v : f.upper[j];
-    v = v > f.lower[j] ? v : f.lower[j];
-    x0[j] = v;
-  }
+  std::vector<double> x0, y0;
+  if (!dev_form) host_start_point(f, warm, x0, y0);
   const int nl = p->nl;   // column entries held by this rank (== n on one GPU)
   for (int k = 0; k < 2; k++) {
     CUDA_OK(cudaMemsetAsync(p->x[k].p, 0, (size_t)nl * sizeof(double), s));
@@ -1496,10 +1615,7 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
     std::vector<double> z(std::max(nl, 1), 0.0);
     bool nz = false;
     for (int i = 0; i < p->nl_real; i++) {
-      const int j = p->cperm[p->c0 + i];
-      double v = 0.0;
-      v = v < f.upper[j] ? v : f.upper[j];
-      v = v > f.lower[j] ? v : f.lower[j];
+      const double v = proj_zero(f, p->cperm[p->c0 + i]);
       z[i] = v;
       nz |= (v != 0.0);
     }
@@ -1587,11 +1703,7 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
     CUDA_OK(cudaMemcpyAsync(p->ctl.p, c, sizeof(SolveCtl), cudaMemcpyHostToDevice, s));
     h->stop_iter = 0;   // the first check is due at once (iteration 0)
     push_state(p);
-    auto next_stop = [&](int it) {
-      int next = it + 1;
-      while (!(next < 10 || next % interval == 0 || next == prm.iter_limit - 1)) next++;
-      return next;
-    };
+    auto next_stop = [&](int it) { return next_check_iter(it, interval, prm.iter_limit); };
     std::vector<std::unique_ptr<CudaEvent>> evs;
     int pred_iter = 0, carry = 0;   // carry: passes still owed before the next check (after a re-synchronisation)
     while (true) {
@@ -1676,30 +1788,13 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
     if (prm.log_level >= 2)
       printf("[b200pdlp] it %8d  pobj %+.8e dobj %+.8e  pfeas %.2e dfeas %.2e | avg pobj %+.8e dobj %+.8e pfeas %.2e dfeas %.2e  tau %.3e sigma %.3e\n",
              h->iter, L.pobj, L.dobj, L.pfeas, L.dfeas, A.pobj, A.dobj, A.pfeas, A.dfeas, h->tau, h->sigma);
-    if (L.pfeas < tol_p && L.dfeas < tol_d && L.relgap < prm.tol_gap) { term = B200PDLP_OPTIMAL; term_iterate = 0; trace_row(out, h, chk, 0); break; }
-    if (A.pfeas < tol_p && A.dfeas < tol_d && A.relgap < prm.tol_gap) { term = B200PDLP_OPTIMAL; term_iterate = 1; trace_row(out, h, chk, 0); break; }
-    {  // PDHG_Check_Infeasibility, cupdlp_solver.c:740-795 (dFeasTol = 1e-8, cupdlp_utils.c:889)
-      const double ft = 1e-8;
-      bool inf = false;
-      for (int t = 0; t < 2; t++) {
-        const Residuals& R = chk.it[t];
-        if (R.pinf_obj > 0.0 && R.pinf_res < ft * R.pinf_obj) inf = true;
-        if (R.dinf_obj < 0.0 && R.dinf_res < -ft * R.dinf_obj) inf = true;
-      }
-      if (inf) { term = B200PDLP_INFEASIBLE_OR_UNBOUNDED; trace_row(out, h, chk, 0); break; }
-    }
-    if (chk.timed_out) { term = B200PDLP_TIMELIMIT_OR_ITERLIMIT; trace_row(out, h, chk, 0); break; }
-    if (h->iter >= prm.iter_limit - 1) { term = B200PDLP_TIMELIMIT_OR_ITERLIMIT; trace_row(out, h, chk, 0); break; }
-    bool dirty = false;
     int choice = 0;
-    if (prm.restart) {
-      choice = decide_restart(h, chk, memo);
-      if (choice) { do_restart(p, choice, chk, memo); restarts++; arm_step(h); dirty = true; }
-    }
+    const int t_code = check_decision(prm, tol_p, tol_d, h, chk, memo, &term_iterate, &choice);
+    if (t_code >= 0) { term = t_code; trace_row(out, h, chk, 0); break; }
+    bool dirty = false;
+    if (choice) { do_restart(p, choice, chk, memo); restarts++; arm_step(h); dirty = true; }
     trace_row(out, h, chk, choice);
-    // next check iteration: < 10, multiple of the interval, or iter_limit - 1 (cupdlp_solver.c:953-962)
-    int next = h->iter + 1;
-    while (!(next < 10 || next % interval == 0 || next == prm.iter_limit - 1)) next++;
+    const int next = next_check_iter(h->iter, interval, prm.iter_limit);
     h->stop_iter = next;
     fill_pow_tables(h);
     dirty = true;
@@ -1893,49 +1988,13 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
     }
   }
   lap("solve", "solution download");
-  const double inf = std::numeric_limits<double>::infinity();
-  if (out->col_value && out->col_dual && out->row_value && out->row_dual) {
-    std::vector<double> sp(n, 0.0), sn(n, 0.0);
-    if (have_check) {
-      for (int j = 0; j < n; j++) {   // dSlackPos / dSlackNeg of the returned iterate (cupdlp_solver.c:150-176)
-        double rc = haty[j] * -1.0;
-        rc = rc + 1.0 * f.cost[j];
-        double a = rc > 0.0 ? rc : 0.0;
-        a = a * (f.lower[j] > -inf ? 1.0 : 0.0);
-        double b = rc < 0.0 ? rc : 0.0;
-        b = b * -1.0;
-        b = b * (f.upper[j] < inf ? 1.0 : 0.0);
-        sp[j] = a; sn[j] = b;
-      }
-    }
-    for (int j = 0; j < n; j++) { hx[j] /= f.col_scale[j]; sp[j] *= f.col_scale[j]; sn[j] *= f.col_scale[j]; }
-    for (int i = 0; i < m; i++) { hy[i] /= f.row_scale[i]; hax[i] *= f.row_scale[i]; }
-    for (int j = 0; j < f.n_orig; j++) out->col_value[j] = hx[j];
-    for (int i = 0, j = 0; i < m; i++) {
-      double v = hax[f.row_new_idx[i]];
-      if (f.row_class[i] == kLeq) v = -v;
-      else if (f.row_class[i] == kBound) { v = v + hx[f.n_orig + j]; j++; }
-      out->row_value[i] = v;
-    }
-    for (int j = 0; j < f.n_orig; j++) { double v = sp[j] - sn[j]; out->col_dual[j] = v * f.sense; }
-    for (int i = 0; i < m; i++) {
-      double v = hy[f.row_new_idx[i]] * f.sense;
-      if (f.row_class[i] == kLeq) v = -v;
-      out->row_dual[i] = v;
-    }
-  }
+  host_postsolve(f, have_check, hx, hy, hax, haty, out);
   }   // host postsolve
-  out->value_valid = 1; out->dual_valid = 1;
-  out->term_code = term; out->term_iterate = term_iterate;
-  out->iters = h->iter; out->passes = h->passes; out->restarts = restarts;
+  fill_result(out, f, h, term, term_iterate, restarts, chk);
   out->kernel_launches = (int)std::min<long long>(p->launches - launches0, 2147483647LL);
-  const Residuals& R = chk.it[use_avg ? 1 : 0];
-  out->primal_obj = R.pobj; out->dual_obj = R.dobj; out->primal_feas = R.pfeas; out->dual_feas = R.dfeas;
-  out->gap = R.gap; out->rel_gap = R.relgap;
   out->solve_seconds = solve_seconds;
   out->iter_device_ms = iter_ms;
   out->setup_seconds += std::chrono::duration<double>(t_loop - t_begin).count();
-  out->form_cols = n; out->form_rows = m; out->form_nnz = f.nnz; out->form_neq = f.neq;
   lap("solve", "postsolve (host)");
 }
 
@@ -2497,6 +2556,315 @@ static void create_hipdlp_shards_device(const b200pdlp_lp& lp, const b200pdlp_hi
   }, devices.data());   // (T has released the standard form, the orderings and the other temporaries of this device)
 }
 
+// ====================================================================================== batch of small LPs, one GPU
+// b200pdlp_solve_batch: every member is an ordered-mode problem, solved by one CTA of batch_round_kernel (batch_kernels.cu).
+// The host runs each member's prologue (formulate, scale, build_layout with identity orderings) on its threads, packs every
+// member into a few pooled buffers, then drives ROUNDS: one launch, one read-back of the control blocks and states, the
+// decisions of every member that checked (the same functions solve_on_device calls), one upload.  Each member returns the
+// bits b200pdlp_solve returns for it alone.
+
+// fn(i) for i < count on up to one host thread per core; after all have run, the failure of the lowest index is rethrown
+// with "member i: " before its message
+template <class F>
+static void for_members(int count, F&& fn) {
+  std::vector<int> codes((size_t)count, B200PDLP_OK);
+  std::vector<std::string> msgs((size_t)count);
+  std::atomic<int> next{0};
+  auto work = [&] {
+    for (int i; (i = next++) < count;) {
+      codes[i] = guarded([&] { fn(i); });
+      if (codes[i] != B200PDLP_OK) msgs[i] = g_last_error;
+    }
+  };
+  const int T = std::max(1, std::min<int>(count, (int)std::thread::hardware_concurrency()));
+  std::vector<std::thread> th;
+  for (int t = 1; t < T; t++) th.emplace_back(work);
+  work();
+  for (auto& t : th) t.join();
+  for (int i = 0; i < count; i++)
+    if (codes[i] != B200PDLP_OK) throw Error(codes[i], "member " + std::to_string(i) + ": " + msgs[i]);
+}
+
+// a batch member's standard form must be an ordered-mode problem (max(n, m) <= ordered_max): checked before any device work
+static void check_batch_member(const b200pdlp_lp* lp, const b200pdlp_params& prm, int i) {
+  const int rc = guarded([&] {
+    check_lp(lp);
+    const int omax = prm.ordered_max == 0 ? 4096 : prm.ordered_max;
+    if (omax < 0) throw Error(B200PDLP_ERR_ARG, "ordered_max < 0: a batch solves ordered-mode problems only");
+    const int n = std_form_cols(*lp, 1e20);
+    if (std::max(n, lp->num_row) > omax)
+      throw Error(B200PDLP_ERR_ARG, "standard form " + std::to_string(lp->num_row) + " x " + std::to_string(n) +
+                                        " exceeds ordered_max = " + std::to_string(omax));
+  });
+  if (rc != B200PDLP_OK) throw Error(rc, "b200pdlp_solve_batch: member " + std::to_string(i) + ": " + g_last_error);
+}
+
+struct BatchHost {   // one member on the host
+  StdForm f;
+  HostLayout L;
+  std::vector<double> x0, y0;
+  size_t vec = 0, sl_a = 0, sl_at = 0, e_a = 0, e_at = 0;   // offsets in the pools
+  RestartMemo memo;
+  CheckResult chk;
+  int term = B200PDLP_TIMELIMIT_OR_ITERLIMIT, term_iterate = 0, restarts = 0;
+  bool have_check = false;
+  double tol_p = 0.0, tol_d = 0.0;
+};
+
+// pinned host array, returned to the pinned cache
+template <class T>
+struct PinnedArray {
+  T* p = nullptr;
+  explicit PinnedArray(size_t count) { p = static_cast<T*>(pinned_cache_alloc(std::max<size_t>(count, 1) * sizeof(T), false)); }
+  ~PinnedArray() { if (p) pinned_cache_free(p); }
+  PinnedArray(const PinnedArray&) = delete;
+  PinnedArray& operator=(const PinnedArray&) = delete;
+};
+
+struct StreamHolder {
+  cudaStream_t s = nullptr;
+  StreamHolder() { CUDA_OK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking)); }
+  ~StreamHolder() { if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); } }
+  StreamHolder(const StreamHolder&) = delete;
+  StreamHolder& operator=(const StreamHolder&) = delete;
+};
+
+// doubles of a member's vector block: cost, lower, upper, colscale, then x0 x1 aty0 aty1 xsum xavg atyavg xlr (n each);
+// rhs, rowscale, then y0 y1 ax0 ax1 ysum yavg axavg ylr (m each)
+static size_t batch_vec_len(int n, int m) { return (size_t)12 * n + (size_t)10 * m; }
+
+static void solve_batch(int count, const b200pdlp_lp* lps, const b200pdlp_params& prm, const b200pdlp_warm* warms,
+                        b200pdlp_result* outs) {
+  using clk = std::chrono::steady_clock;
+  const auto t_begin = clk::now();
+  Laps lap;
+  device_count_checked();
+  if (prm.device >= 0) CUDA_OK(cudaSetDevice(prm.device));
+  StreamHolder sh;
+  cudaStream_t s = sh.s;
+  std::vector<BatchHost> B((size_t)count);
+  {
+    NvtxRange nvtx("b200pdlp: batch prologue (host threads)");
+    for_members(count, [&](int i) {
+      BatchHost& b = B[i];
+      formulate(lps[i], b.f);
+      scale(b.f, prm.scaling != 0);
+      build_layout(b.f, 0, 1, prm.ordered_max, b.L);
+      if (!b.L.ordered || !b.L.A.segs.empty() || !b.L.AT.segs.empty())
+        throw Error(B200PDLP_ERR_STATE, "the layout is not an ordered-mode layout");
+      host_start_point(b.f, warms ? &warms[i] : nullptr, b.x0, b.y0);
+      b.tol_p = prm.tol_primal * (1.0 + b.f.norm_rhs);
+      b.tol_d = prm.tol_dual * (1.0 + b.f.norm_cost);
+    });
+  }
+  lap("batch", "prologue (host threads)");
+
+  // ---- pooled device buffers: vectors, slice descriptors, column ids and values of A and A'; one descriptor per member
+  size_t nvec = 0, nsl = 0, nent = 0;
+  for (BatchHost& b : B) {
+    b.vec = nvec; nvec += batch_vec_len(b.f.n, b.f.m);
+    b.sl_a = nsl; nsl += b.L.A.slices.size();
+    b.sl_at = nsl; nsl += b.L.AT.slices.size();
+    b.e_a = nent; nent += b.L.A.col.size();
+    b.e_at = nent; nent += b.L.AT.col.size();
+  }
+  std::vector<double> hvec(std::max<size_t>(nvec, 1), 0.0), hval(std::max<size_t>(nent, 1), 0.0);
+  std::vector<int> hcol(std::max<size_t>(nent, 1), 0);
+  std::vector<int4> hsl(std::max<size_t>(nsl, 1));
+  for_members(count, [&](int i) {
+    const BatchHost& b = B[i];
+    const StdForm& f = b.f;
+    const int n = f.n, m = f.m;
+    double* v = hvec.data() + b.vec;
+    // identity orderings (ordered mode): standard-form order is device order
+    std::copy(f.cost.begin(), f.cost.end(), v);
+    std::copy(f.lower.begin(), f.lower.end(), v + n);
+    std::copy(f.upper.begin(), f.upper.end(), v + 2 * n);
+    std::copy(f.col_scale.begin(), f.col_scale.end(), v + 3 * n);
+    std::copy(b.x0.begin(), b.x0.end(), v + 4 * n);
+    for (int j = 0; j < n; j++) v[8 * n + j] = proj_zero(f, j);   // xsum
+    double* w = v + 12 * n;
+    std::copy(f.rhs.begin(), f.rhs.end(), w);
+    std::copy(f.row_scale.begin(), f.row_scale.end(), w + m);
+    std::copy(b.y0.begin(), b.y0.end(), w + 2 * m);
+    static_assert(sizeof(SellMatrix::Slice) == sizeof(int4), "descriptor layout");
+    memcpy(hsl.data() + b.sl_a, b.L.A.slices.data(), b.L.A.slices.size() * sizeof(int4));
+    memcpy(hsl.data() + b.sl_at, b.L.AT.slices.data(), b.L.AT.slices.size() * sizeof(int4));
+    std::copy(b.L.A.col.begin(), b.L.A.col.end(), hcol.begin() + b.e_a);
+    std::copy(b.L.AT.col.begin(), b.L.AT.col.end(), hcol.begin() + b.e_at);
+    std::copy(b.L.A.val.begin(), b.L.A.val.end(), hval.begin() + b.e_a);
+    std::copy(b.L.AT.val.begin(), b.L.AT.val.end(), hval.begin() + b.e_at);
+  });
+  DevBuf<double> dvec, dval;
+  DevBuf<int> dcol;
+  DevBuf<int4> dsl;
+  DevBuf<BatchMember> dmem;
+  DevBuf<PdhgState> dst;
+  DevBuf<BatchCtl> dctl;
+  dvec.alloc(hvec.size(), false); dval.alloc(hval.size(), false); dcol.alloc(hcol.size(), false); dsl.alloc(hsl.size(), false);
+  dmem.alloc(count, false); dst.alloc(count, false); dctl.alloc(count, false);
+  std::vector<BatchMember> hmem((size_t)count);
+  for (int i = 0; i < count; i++) {
+    const BatchHost& b = B[i];
+    const int n = b.f.n, m = b.f.m;
+    double* v = dvec.p + b.vec;
+    double* w = v + 12 * n;
+    BatchMember& M = hmem[i];
+    M.n = n; M.m = m; M.neq = b.L.neq_local;
+    M.a_slices = dsl.p + b.sl_a; M.a_col = dcol.p + b.e_a; M.a_val = dval.p + b.e_a;
+    M.at_slices = dsl.p + b.sl_at; M.at_col = dcol.p + b.e_at; M.at_val = dval.p + b.e_at;
+    M.cost = v; M.lower = v + n; M.upper = v + 2 * n; M.colscale = v + 3 * n;
+    M.x0 = v + 4 * n; M.x1 = v + 5 * n; M.aty0 = v + 6 * n; M.aty1 = v + 7 * n;
+    M.xsum = v + 8 * n; M.xavg = v + 9 * n; M.atyavg = v + 10 * n; M.xlr = v + 11 * n;
+    M.rhs = w; M.rowscale = w + m;
+    M.y0 = w + 2 * m; M.y1 = w + 3 * m; M.ax0 = w + 4 * m; M.ax1 = w + 5 * m;
+    M.ysum = w + 6 * m; M.yavg = w + 7 * m; M.axavg = w + 8 * m; M.ylr = w + 9 * m;
+  }
+  // ---- initial states: PDHG_Init_Step_Sizes (cupdlp_step.c:312-375); a fixed step takes tau, sigma after round 0's power method
+  PinnedArray<PdhgState> hst((size_t)count);
+  PinnedArray<BatchCtl> hctl((size_t)count);
+  for (int i = 0; i < count; i++) {
+    const StdForm& f = B[i].f;
+    PdhgState* h = hst.p + i;
+    memset(h, 0, sizeof(PdhgState));
+    h->adaptive = prm.adaptive_step != 0;
+    double a = 0.0, b = 0.0;
+    for (int j = 0; j < f.n; j++) a += f.cost[j] * f.cost[j];
+    for (int r = 0; r < f.m; r++) b += f.rhs[r] * f.rhs[r];
+    h->beta = std::fmin(a, b) > 1e-6 ? a / b : 1.0;
+    if (h->adaptive) {
+      h->tau = (1.0 / f.amax) / std::sqrt(h->beta);
+      h->sigma = h->tau * h->beta;
+    }
+    arm_step(h);
+    fill_pow_tables(h);
+    h->stop_iter = 0;   // the first check is due at once (iteration 0)
+    BatchCtl& c = hctl.p[i];
+    memset(&c, 0, sizeof(BatchCtl));
+    c.active = 1; c.first = 1; c.fixed_step = !h->adaptive; c.no_check = prm.iter_limit <= 0;
+    outs[i].trace_len = 0;
+  }
+  CUDA_OK(cudaMemcpyAsync(dvec.p, hvec.data(), hvec.size() * sizeof(double), cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaMemcpyAsync(dval.p, hval.data(), hval.size() * sizeof(double), cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaMemcpyAsync(dcol.p, hcol.data(), hcol.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaMemcpyAsync(dsl.p, hsl.data(), hsl.size() * sizeof(int4), cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaMemcpyAsync(dmem.p, hmem.data(), (size_t)count * sizeof(BatchMember), cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaStreamSynchronize(s));
+  lap("batch", "pools + upload");
+
+  // ---- rounds
+  const int interval = prm.check_interval > 0 ? prm.check_interval : 40;
+  const double t_lim = (prm.time_limit >= 0 && std::isfinite(prm.time_limit)) ? prm.time_limit : -1.0;   // < 0: none
+  CudaEvent evl0, evl1, ev0, ev1;
+  double iter_ms = 0.0;
+  long long rounds = 0;
+  int active = count;
+  CUDA_OK(cudaEventRecord(evl0, s));
+  const auto t_loop = clk::now();
+  while (active > 0) {
+    NvtxRange nvtx("b200pdlp: batch round");
+    const bool timed_out = t_lim >= 0 && std::chrono::duration<double>(clk::now() - t_loop).count() > t_lim;
+    CUDA_OK(cudaMemcpyAsync(dctl.p, hctl.p, (size_t)count * sizeof(BatchCtl), cudaMemcpyHostToDevice, s));
+    CUDA_OK(cudaMemcpyAsync(dst.p, hst.p, (size_t)count * sizeof(PdhgState), cudaMemcpyHostToDevice, s));
+    CUDA_OK(cudaEventRecord(ev0, s));
+    launch_batch_round(s, count, dmem.p, dst.p, dctl.p);
+    CUDA_OK(cudaEventRecord(ev1, s));
+    CUDA_OK(cudaMemcpyAsync(hctl.p, dctl.p, (size_t)count * sizeof(BatchCtl), cudaMemcpyDeviceToHost, s));
+    // the scalars of every state (the power tables are the host's own)
+    CUDA_OK(cudaMemcpy2DAsync(hst.p, sizeof(PdhgState), dst.p, sizeof(PdhgState), offsetof(PdhgState, pow_red), count,
+                              cudaMemcpyDeviceToHost, s));
+    CUDA_OK(cudaStreamSynchronize(s));
+    float ms = 0.f;
+    CUDA_OK(cudaEventElapsedTime(&ms, ev0, ev1));
+    iter_ms += ms;
+    const bool first = rounds == 0;
+    rounds++;
+    for (int i = 0; i < count; i++) {
+      BatchCtl& c = hctl.p[i];
+      if (!c.active) continue;
+      BatchHost& b = B[i];
+      PdhgState* h = hst.p + i;
+      b200pdlp_result* out = outs + i;
+      if (!c.checked) {
+        if (first && c.no_check) { c.active = 0; active--; continue; }   // iter_limit <= 0: no check at all
+        fill_pow_tables(h);   // the tables ran out before the check iteration: refill, the next round goes on
+        continue;
+      }
+      if (first && c.fixed_step) {
+        const double lambda = c.outs[kBatchLambda];
+        h->tau = 0.8 / std::sqrt(lambda);
+        h->sigma = h->tau;
+        h->tau /= std::sqrt(h->beta);
+        h->sigma *= std::sqrt(h->beta);
+        arm_step(h);
+      }
+      CheckResult& chk = b.chk;
+      double dscale[2], pscale[2];
+      assemble_check_a(b.f, c.outs, chk, dscale, pscale);
+      assemble_check_b(b.f, c.outs, chk, dscale, pscale);
+      chk.timed_out = timed_out;
+      b.have_check = true;
+      int choice = 0;
+      const int t_code = check_decision(prm, b.tol_p, b.tol_d, h, chk, b.memo, &b.term_iterate, &choice);
+      if (t_code >= 0) {
+        b.term = t_code;
+        trace_row(out, h, chk, 0);
+        c.active = 0;
+        active--;
+        continue;
+      }
+      if (choice) {
+        restart_steps(h, choice, chk, b.memo, c.outs[choice == 1 ? kBatchDxAvg : kBatchDxCur],
+                      c.outs[choice == 1 ? kBatchDyAvg : kBatchDyCur]);
+        b.restarts++;
+        arm_step(h);
+        c.restart = choice;
+      }
+      trace_row(out, h, chk, choice);
+      h->stop_iter = next_check_iter(h->iter, interval, prm.iter_limit);
+      fill_pow_tables(h);
+    }
+  }
+  CUDA_OK(cudaEventRecord(evl1, s));
+  CUDA_OK(cudaEventSynchronize(evl1));
+  float loop_ms = 0.f;
+  CUDA_OK(cudaEventElapsedTime(&loop_ms, evl0, evl1));
+  const double solve_seconds = std::chrono::duration<double>(clk::now() - t_loop).count();
+  lap("batch", "rounds");
+
+  // ---- PDHG_PostSolve of every member, on the host
+  NvtxRange nvtx_post("b200pdlp: batch postsolve + download");
+  CUDA_OK(cudaMemcpyAsync(hvec.data(), dvec.p, hvec.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaStreamSynchronize(s));
+  const double setup_seconds = std::chrono::duration<double>(t_loop - t_begin).count();
+  for_members(count, [&](int i) {
+    BatchHost& b = B[i];
+    const StdForm& f = b.f;
+    const PdhgState* h = hst.p + i;
+    const int n = f.n, m = f.m, cur = h->cur;
+    const bool use_avg = b.term == B200PDLP_OPTIMAL && b.term_iterate == 1;
+    const double* v = hvec.data() + b.vec;
+    const double* w = v + 12 * n;
+    const double* dx = use_avg ? v + 9 * n : v + (4 + cur) * n;
+    const double* daty = use_avg ? v + 10 * n : v + (6 + cur) * n;
+    const double* dy = use_avg ? w + 7 * m : w + (2 + cur) * m;
+    const double* dax = use_avg ? w + 8 * m : w + (4 + cur) * m;
+    std::vector<double> hx(n), hy(m), hax(m), haty(n);
+    for (int j = 0; j < n; j++) { hx[b.L.cperm[j]] = dx[j]; haty[b.L.cperm[j]] = daty[j]; }
+    for (int r = 0; r < m; r++) { hy[b.L.rperm[r]] = dy[r]; hax[b.L.rperm[r]] = dax[r]; }
+    b200pdlp_result* out = outs + i;
+    host_postsolve(f, b.have_check, hx, hy, hax, haty, out);
+    fill_result(out, f, h, b.term, b.term_iterate, b.restarts, b.chk);
+    out->kernel_launches = (int)std::min<long long>(rounds, 2147483647LL);
+    out->setup_seconds = setup_seconds;
+    out->solve_seconds = solve_seconds;
+    out->loop_device_ms = loop_ms;
+    out->iter_device_ms = iter_ms;
+  });
+  lap("batch", "postsolve (host threads)");
+}
+
+
 extern "C" {
 
 const char* b200pdlp_last_error(void) { return g_last_error.c_str(); }
@@ -2890,6 +3258,20 @@ int b200pdlp_solve(const b200pdlp_lp* lp, const b200pdlp_params* params, const b
     Laps lap;
     p.reset();
     lap("solve", "teardown");
+  });
+}
+
+int b200pdlp_solve_batch(int32_t count, const b200pdlp_lp* lps, const b200pdlp_params* params, const b200pdlp_warm* warms,
+                         b200pdlp_result* outs) {
+  DeviceGuard dg;
+  return guarded([&] {
+    if (count < 0) throw Error(B200PDLP_ERR_ARG, "b200pdlp_solve_batch: count < 0");
+    if (count == 0) return;
+    if (!lps || !params || !outs) throw Error(B200PDLP_ERR_ARG, "b200pdlp_solve_batch: null argument");
+    check_params(*params);
+    for (int i = 0; i < count; i++) check_batch_member(&lps[i], *params, i);
+    solve_batch(count, lps, *params, warms, outs);
+    CUDA_OK(cudaGetLastError());
   });
 }
 

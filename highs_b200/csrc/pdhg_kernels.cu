@@ -1,4 +1,5 @@
 // highs_b200/csrc/pdhg_kernels.cu -- kernel definitions + launchers (see kernels.cuh).
+#include "pdhg_arith.cuh"
 #include "pdhg_kernels.hpp"
 
 namespace b200 {
@@ -23,13 +24,7 @@ primal_step_kernel(int n, PdhgState* __restrict__ st, double* __restrict__ x0, d
   const double* __restrict__ aty = cur ? aty1 : aty0;
   double acc[1] = {0.0};
   auto one = [&](double xc, double ci, double ai, double u, double l, double& out) {
-    double v = xc + ntau * ci;
-    v = v + tau * ai;
-    v = v < u ? v : u;
-    v = v > l ? v : l;
-    out = v;
-    const double d = xc - v;
-    return d * d;
+    return primal_update(xc, ci, ai, u, l, tau, ntau, out);
   };
   // pairs of elements with 128-bit loads/stores (all vectors are cudaMalloc-aligned)
   const int npair = n >> 1;
@@ -138,10 +133,7 @@ struct DualEpilogueT {
     const double yc = p_y;
     if (pend) ysum[r] = p_ys + w * yc;
     if (accum) axsum[r] = p_axs + w * p_ax;   // A xSum += w A x  (x = the iterate accepted by the previous pass)
-    double v = yc + sigma * p_b;
-    v = v + (-2.0 * sigma) * s;
-    v = v + sigma * p_ax;
-    if (r >= neq) v = v > 0.0 ? v : 0.0;
+    const double v = dual_update(yc, p_b, s, p_ax, sigma, r >= neq);
     yn[r] = v;
     const double d = yc - v;
     t[0] = d * d;
@@ -150,55 +142,6 @@ struct DualEpilogueT {
 };
 using DualEpilogue = DualEpilogueT<1>;
 using DualEpilogueMg = DualEpilogueT<2>;
-
-// device-side adaptive step rule, PDHG_Update_Iterate_Adaptive_Step_Size
-// (cupdlp_step.c:236-307) + the bookkeeping of PDHG_Update_Average (:422-442)
-__device__ void step_rule(PdhgState* st, double inter) {
-  const double rb = sqrt(st->beta);
-  const double mov = st->dx2 * 0.5 * rb + st->dy2 / (2.0 * rb);   // cupdlp_linalg.c:800
-  st->inter = inter;
-  st->mov = mov;
-  st->passes++;
-  if (st->adaptive) {
-    const int k = ++st->step_iter;
-    const double eta = st->eta;
-    const double lim = (inter != 0.0) ? mov / fabs(inter) : INFINITY;
-    st->lim = lim;
-    const bool accept = eta <= lim;
-    int t = k - st->pow_base - 1;
-    double pr, pg;
-    if (t >= 0 && t < kPowTab) { pr = st->pow_red[t]; pg = st->pow_grow[t]; }
-    else { pr = pow(k + 1.0, -0.3); pg = pow(k + 1.0, -0.6); }   // never hit: host refills the tables
-    const double first = (1.0 - pr) * lim;
-    const double second = (1.0 + pg) * eta;
-    const double eta_new = fmin(first, second);
-    if (accept) {
-      st->tau = eta_new / rb;
-      st->sigma = eta_new * rb;
-      const double w = sqrt(st->tau * st->sigma);
-      st->sum_step += w;
-      st->w_pending = w;
-      st->pending = 1;
-      st->cur ^= 1;
-      st->iter++;
-      st->eta = w;   // next iteration starts from sqrt(dPrimalStep*dDualStep), cupdlp_step.c:230-231
-    } else {
-      st->eta = eta_new;
-      st->pending = 0;
-      st->rejects++;
-    }
-    st->tau_try = st->eta / rb;
-    st->sigma_try = st->eta * rb;
-  } else {
-    // fixed step (PDHG_Update_Iterate_Constant_Step_Size): always accepted, steps unchanged
-    const double w = sqrt(st->tau * st->sigma);
-    st->sum_step += w;
-    st->w_pending = w;
-    st->pending = 1;
-    st->cur ^= 1;
-    st->iter++;
-  }
-}
 
 // K3: aty' = A'y' fused with the interaction (x - x').(aty - aty')
 // (cupdlp_compute_interaction_and_movement, cupdlp_linalg.c:772-801); K4 adds the block partials.
@@ -1096,25 +1039,9 @@ col_check_a_kernel(int n, int nit, ColIter it0, ColIter it1, const double* __res
     for (int t = 0; t < 2; t++) {
       if (t >= nit) break;
       const ColIter& it = t ? it1 : it0;
-      const double x = it.x[i], aty = it.aty[i];
-      double rc = aty * -1.0;
-      rc = rc + 1.0 * ci;
-      double sp = rc > 0.0 ? rc : 0.0;
-      sp = sp * (hl ? 1.0 : 0.0);
-      double sn = rc < 0.0 ? rc : 0.0;
-      sn = sn * -1.0;
-      sn = sn * (hu ? 1.0 : 0.0);
-      double rr = rc + -1.0 * sp;
-      rr = rr + 1.0 * sn;
-      rr = rr * sc;
       double* a = acc + 7 * t;
-      add_term(a[0], x * ci, rs, 7 * t + 0, i);
-      add_term(a[1], sp * lf, rs, 7 * t + 1, i);
-      add_term(a[2], sn * uf, rs, 7 * t + 2, i);
-      add_term(a[3], rr * rr, rs, 7 * t + 3, i);
-      add_term(a[4], sp * sp, rs, 7 * t + 4, i);
-      add_term(a[5], sn * sn, rs, 7 * t + 5, i);
-      add_term(a[6], x * x, rs, 7 * t + 6, i);
+      col_check_a_terms(it.x[i], it.aty[i], ci, hl, hu, lf, uf, sc,
+                        [&](int k, double v) { add_term(a[k], v, rs, 7 * t + k, i); });
     }
   }
   double res[14];
@@ -1219,14 +1146,8 @@ row_check_a_kernel(int m, int nit, RowIter it0, RowIter it1, const double* __res
     for (int t = 0; t < 2; t++) {
       if (t >= nit) break;
       const RowIter& it = t ? it1 : it0;
-      const double y = it.y[i], ax = it.ax[i];
-      double r = ax + -1.0 * bi;
-      if (ineq) r = r < 0.0 ? r : 0.0;
-      r = r * sc;
       double* a = acc + 3 * t;
-      add_term(a[0], y * bi, rs, 3 * t + 0, i);
-      add_term(a[1], r * r, rs, 3 * t + 1, i);
-      add_term(a[2], y * y, rs, 3 * t + 2, i);
+      row_check_a_terms(it.y[i], it.ax[i], bi, sc, ineq, [&](int k, double v) { add_term(a[k], v, rs, 3 * t + k, i); });
     }
   }
   double res[6];
@@ -1254,29 +1175,8 @@ col_check_b_kernel(int n, int nit, ColIter it0, ColIter it1, double inv_dscale0,
       if (t >= nit) break;
       const ColIter& it = t ? it1 : it0;
       const double ids = t ? inv_dscale1 : inv_dscale0, ips = t ? inv_pscale1 : inv_pscale0;
-      const double x = it.x[i], aty = it.aty[i];
-      double rc = aty * -1.0;
-      rc = rc + 1.0 * ci;
-      double sp = rc > 0.0 ? rc : 0.0;
-      sp = sp * hl;
-      double sn = rc < 0.0 ? rc : 0.0;
-      sn = sn * -1.0;
-      sn = sn * hu;
-      double k = aty * ids;
-      k = k + 1.0 * (sp * ids);
-      k = k + -1.0 * (sn * ids);
-      k = k * sc;
-      const double ray = x * ips;
-      double bl = ray < 0.0 ? ray : 0.0;
-      bl = bl * hl;
-      bl = bl / sc;
-      double bu = ray > 0.0 ? ray : 0.0;
-      bu = bu * hu;
-      bu = bu / sc;
       double* a = acc + 3 * t;
-      add_term(a[0], k * k, rs, 3 * t + 0, i);
-      add_term(a[1], bl * bl, rs, 3 * t + 1, i);
-      add_term(a[2], bu * bu, rs, 3 * t + 2, i);
+      col_check_b_terms(it.x[i], it.aty[i], ci, hl, hu, sc, ids, ips, [&](int k, double v) { add_term(a[k], v, rs, 3 * t + k, i); });
     }
   }
   double res[6];
@@ -1298,10 +1198,7 @@ row_check_b_kernel(int m, int nit, RowIter it0, RowIter it1, double inv_pscale0,
     for (int t = 0; t < 2; t++) {
       if (t >= nit) break;
       const RowIter& it = t ? it1 : it0;
-      double k = it.ax[i] * (t ? inv_pscale1 : inv_pscale0);
-      if (ineq) k = k < 0.0 ? k : 0.0;
-      k = k * sc;
-      add_term(acc[t], k * k, rs, t, i);
+      add_term(acc[t], row_check_b_term(it.ax[i], t ? inv_pscale1 : inv_pscale0, sc, ineq), rs, t, i);
     }
   }
   double res[2];

@@ -78,7 +78,7 @@ ABI_SYMBOLS = [
     "b200pdlp_hipdlp_controller_replay", "b200pdlp_debug_prep_compare",
     "b200pdlp_debug_prep_compare_hipdlp", "b200pdlp_debug_hipdlp_shard_prep_compare", "b200pdlp_release_cache",
     "b200pdlp_host_register", "b200pdlp_host_unregister", "b200pdlp_primal_step", "b200pdlp_dual_step", "b200pdlp_residuals",
-    "b200pdlp_kkt_check", "b200pdlp_kkt_check_host", "b200pdlp_kkt_default_tolerances",
+    "b200pdlp_kkt_check", "b200pdlp_kkt_check_host", "b200pdlp_kkt_default_tolerances", "b200pdlp_solve_batch",
 ]
 
 _lib = None
@@ -115,6 +115,7 @@ def lib():
         L.b200pdlp_default_params.argtypes = [C.POINTER(CParams)]
         L.b200pdlp_default_params.restype = None
         L.b200pdlp_solve.argtypes = [C.POINTER(CLp), C.POINTER(CParams), C.POINTER(CWarm), C.POINTER(CResult)]
+        L.b200pdlp_solve_batch.argtypes = [C.c_int32, C.POINTER(CLp), C.POINTER(CParams), C.POINTER(CWarm), C.POINTER(CResult)]
         L.b200pdlp_problem_create.argtypes = [C.POINTER(CLp), C.POINTER(CParams), C.c_int32, C.c_int32,
                                               C.POINTER(C.c_void_p)]
         L.b200pdlp_problem_destroy.argtypes = [C.c_void_p]
@@ -226,6 +227,33 @@ def solve(lp: HighsLp, warm=None, trace_cap: int = 0, out_arrays=None, **params)
     w, wk = _mk_warm(warm)
     _check(L.b200pdlp_solve(C.byref(clp), C.byref(prm), C.byref(w) if w else None, C.byref(res)), "b200pdlp_solve")
     return _result_dict(res, arrays)
+
+
+def solve_batch(lps, warms=None, trace_cap: int = 0, **params) -> list:
+    """b200pdlp_solve_batch: every LP of `lps` (ordered-mode problems) solved on one GPU in one call, one CTA per LP.
+    warms: None, or one entry per LP -- None (cold start) or (col_value, row_value, row_dual).  Returns the dicts solve()
+    returns, in order; each holds the bits solve() returns for that LP alone (the timings and kernel_launches are the
+    batch's)."""
+    lps = list(lps)
+    if warms is not None:
+        warms = list(warms)
+        if len(warms) != len(lps):
+            raise ValueError(f"solve_batch: {len(warms)} warm starts for {len(lps)} LPs")
+    L = lib()
+    count = len(lps)
+    clps, cres, keep, arrays = (CLp * max(count, 1))(), (CResult * max(count, 1))(), [], []
+    cwarm = (CWarm * max(count, 1))() if warms is not None and any(w is not None for w in warms) else None
+    for i, lp in enumerate(lps):
+        clps[i], k = make_clp(lp)
+        keep.append(k)
+        cres[i], a = _mk_result(lp, trace_cap)
+        arrays.append(a)
+        if cwarm is not None and warms[i] is not None:
+            cwarm[i], wk = _mk_warm(warms[i])
+            keep.append(wk)
+    prm = make_params(**params)
+    _check(L.b200pdlp_solve_batch(count, clps, C.byref(prm), cwarm, cres), "b200pdlp_solve_batch")
+    return [_result_dict(cres[i], arrays[i]) for i in range(count)]
 
 
 PREP_ITEMS = ["n", "m", "nnz", "neq", "cbeg", "cidx", "cval", "cost", "lower", "upper", "col_scale", "rhs", "row_scale", "rptr",

@@ -135,6 +135,22 @@ int b200pdlp_solve(const b200pdlp_lp* lp, const b200pdlp_params* params,
 int b200pdlp_solve_multi(const b200pdlp_lp* lp, const b200pdlp_params* params, const b200pdlp_warm* warm,
                          b200pdlp_result* out, int32_t ngpus, const int32_t* devices);
 
+/* Solve `count` independent LPs on one GPU in one call.  Every member must be an ordered-mode problem of `params`
+ * (standard form max(n, m) <= ordered_max); each returns exactly what b200pdlp_solve(lps[i], params, warms[i]) returns:
+ * term_code, term_iterate, iters, passes, restarts, the residual scalars, the trace rows and all four vectors, bit for bit.
+ * All members share `params` (tolerances, limits, check_interval, scaling, adaptive step, restart); `device` selects the GPU.
+ * One CTA solves one member; the members' host prologues run on host threads.  The time limit counts from the start of the
+ * batch's PDHG loop.  These fields are batch-wide, the same in every outs[i]: setup_seconds, solve_seconds, loop_device_ms,
+ * iter_device_ms and kernel_launches (= the batch's rounds, one launch each).
+ * Returns B200PDLP_ERR_ARG before any device work for count < 0, NULL arrays, a member that the checks of b200pdlp_solve
+ * reject, ordered_max < 0, or a member whose standard form exceeds ordered_max; b200pdlp_last_error() names the member's
+ * index, and no result is written.  count == 0: B200PDLP_OK.  No device: B200PDLP_ERR_CUDA.  The whole batch must fit in
+ * device memory (B200PDLP_ERR_ALLOC otherwise).
+ * STATUS: runs on hardware; tests/test_gpu_batch.py (byte equality with b200pdlp_solve and with the oracle), tools/batch_bench.py. */
+int b200pdlp_solve_batch(int32_t count, const b200pdlp_lp* lps, const b200pdlp_params* params,
+                         const b200pdlp_warm* warms /* [count] or NULL; a member whose pointers are NULL starts cold */,
+                         b200pdlp_result* outs /* [count], caller-allocated like b200pdlp_result */);
+
 /* ---- persistent problem handle (bench + kernel-level parity tests) --------- */
 typedef struct b200pdlp_problem b200pdlp_problem;
 
