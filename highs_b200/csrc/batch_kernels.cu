@@ -295,10 +295,189 @@ batch_round_kernel(const BatchMember* __restrict__ members, PdhgState* __restric
   }
 }
 
+// ============================================================================================ HiPDLP batch
+// b200pdlp_solve_hipdlp_batch: one round of one member = what solve_hipdlp_on_device (engine.cu) enqueues between two of
+// its host decisions, with the same per-element arithmetic (pdhg_arith.cuh):
+//   round 0    the power method (n > 0 and m > 0), x = xa = proj_[l,u](0), y = ya = 0, A'y, the iteration-0 check;
+//   round k    the restart decided after block k - 1 (anchors and iterates <- (xn, yn), A'y), step 1 (major), the three
+//              fixed-point sums of that step when the restart's reference error is due (step 2 overwrites rx, so they
+//              cannot wait for the check), steps 2..39 (minor) and 40 (major), the block-end check.
+// Every SpMV row is summed in entry order (sell_row over the ordered layout, as spmv_sell_kernel sums it), and every sum of
+// a check or of the power method adds its terms in index order in one thread from the same init, as warp_ordered_sum
+// does; the reducing thread forms the terms from the stored vectors.  The independent sums of one phase run on lane 0 of
+// different warps.
+
+// the sum of term(i), i < len, in index order from init (warp_ordered_sum's order), one thread
+template <class Term>
+__device__ __forceinline__ double seq_sum(int len, double init, Term term) {
+  double s = init;
+  for (int i = 0; i < len; i++) s = s + term(i);
+  return s;
+}
+
+// PDLPSolver::powerMethod (pdhg.cc:1529-1671) as solve_hipdlp_on_device runs it in ordered mode: q = 1; 20 times w = A'q,
+// z = A w, z = z / |z|, w' = A'z, lambda = |w'|^2, q = z.  q in dy, z in axp, w in atdy, w' in atyp (all set again later).
+__device__ double hip_power_method(const HipBatchMember& M, double* sw) {
+  const int n = M.n, m = M.m;
+  double* q = M.dy;
+  double* z = M.axp;
+  for (int i = threadIdx.x; i < m; i += kThreads) q[i] = 1.0;
+  double lambda = 0.0;
+  for (int it = 0; it < 20; it++) {
+    __syncthreads();
+    spmv(M.at_slices, M.at_col, M.at_val, n, q, M.atdy);
+    __syncthreads();
+    spmv(M.a_slices, M.a_col, M.a_val, m, M.atdy, z);
+    __syncthreads();
+    if (threadIdx.x == 0) sw[0] = seq_sum(m, 0.0, [&](int i) { return z[i] * z[i]; });
+    __syncthreads();
+    const double nrm = sqrt(sw[0]);   // hip_div_norm_kernel
+    for (int i = threadIdx.x; i < m; i += kThreads) z[i] = z[i] / nrm;
+    __syncthreads();
+    spmv(M.at_slices, M.at_col, M.at_val, n, z, M.atyp);
+    __syncthreads();
+    if (threadIdx.x == 0) sw[1] = seq_sum(n, 0.0, [&](int i) { return M.atyp[i] * M.atyp[i]; });
+    for (int i = threadIdx.x; i < m; i += kThreads) q[i] = z[i];
+    __syncthreads();
+    lambda = sw[1];
+  }
+  return lambda;
+}
+
+// Halpern step k_offset of the block (hip_step: hip_primal_kernel, A * reflected x with HipDualEpilogue, A'y)
+__device__ void hip_batch_step(const HipBatchMember& M, double ps, double ds, int hi, int k_offset, int is_major) {
+  const int k = hi + k_offset;
+  const double w = (double)k / (k + 1.0);
+  for (int i = threadIdx.x; i < M.n; i += kThreads)
+    hip_primal_col(i, ps, w, is_major, M.x, M.xa, M.cost, M.aty, M.lower, M.upper, M.rx, M.xn, M.hslack);
+  __syncthreads();
+  for (int r = threadIdx.x; r < M.m; r += kThreads) {
+    const double s = sell_row(M.a_slices, M.a_col, M.a_val, r, M.rx);
+    M.y[r] = hip_dual_blend(r, M.y[r], M.ya[r], M.rlo[r], M.rup[r], s, ds, w, is_major, M.yn, M.ry);
+  }
+  __syncthreads();
+  spmv(M.at_slices, M.at_col, M.at_val, M.n, M.y, M.aty);
+  __syncthreads();
+}
+
+// dy = yn - ry and A'dy: the dual movement of the last major step (hip_diff_kernel, then A')
+__device__ void hip_batch_atdy(const HipBatchMember& M) {
+  for (int r = threadIdx.x; r < M.m; r += kThreads) M.dy[r] = M.yn[r] - M.ry[r];
+  __syncthreads();
+  spmv(M.at_slices, M.at_col, M.at_val, M.n, M.dy, M.atdy);
+}
+
+// the check arguments of hip_check for (x, y), or with `major` for (xn, yn); thread 0 writes them
+__device__ void hip_batch_args(const HipBatchMember& M, int major, HipCheckArgs& a) {
+  a.n = M.n; a.m = M.m; a.neq = M.neq; a.scaled = M.scaled; a.offset = M.offset;
+  a.x = major ? M.xn : M.x; a.y = major ? M.yn : M.y; a.ax = M.axp; a.aty = M.atyp; a.rx = M.rx; a.ry = M.ry; a.atdy = M.atdy;
+  a.xa = M.xa; a.ya = M.ya; a.c = M.cost; a.lo = M.lower; a.up = M.upper; a.rlo = M.rlo;
+  a.colscale = M.colscale; a.rowscale = M.rowscale; a.sp = M.sp; a.sn = M.sn;
+}
+
+// hip_check: A x and A'y of the checked iterate (and A'dy with `major`), the dual slacks (cached on a major step), then the
+// nine sums of hip_check_ordered_kernel into out[0..8] (0..2 stay 0 without `major`); `a` is hip_batch_args(major)
+__device__ void hip_batch_check(const HipBatchMember& M, int major, const HipCheckArgs& a, double* __restrict__ out) {
+  if (major) hip_batch_atdy(M);
+  spmv(M.a_slices, M.a_col, M.a_val, M.m, a.x, M.axp);
+  spmv(M.at_slices, M.at_col, M.at_val, M.n, a.y, M.atyp);
+  __syncthreads();
+  for (int i = threadIdx.x; i < M.n; i += kThreads) {
+    double sp, sn;
+    hip_dual_slacks(i, major, M.hslack, M.cost, M.atyp, M.lower, M.upper, sp, sn);
+    M.sp[i] = sp;
+    M.sn[i] = sn;
+  }
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) {
+    switch (threadIdx.x >> 5) {   // 9 sums on 8 warps: warp 1 adds two m-length sums one after the other
+      case 0: out[0] = major ? seq_sum(a.n, 0.0, [&](int i) { return hip_fpe_x_term(a, i); }) : 0.0; break;
+      case 1:
+        out[1] = major ? seq_sum(a.m, 0.0, [&](int i) { return hip_fpe_y_term(a, i); }) : 0.0;
+        out[8] = seq_sum(a.m, 0.0, [&](int i) { return hip_anchor_y_term(a, i); });
+        break;
+      case 2: out[2] = major ? seq_sum(a.n, 0.0, [&](int i) { return hip_fpe_inter_term(a, i); }) : 0.0; break;
+      case 3: out[3] = seq_sum(a.m, 0.0, [&](int i) { return hip_primal_res_term(a, i); }); break;
+      case 4: out[4] = seq_sum(a.n, 0.0, [&](int i) { return hip_dual_res_term(a, i); }); break;
+      case 5: out[5] = seq_sum(a.n, a.offset, [&](int i) { return hip_pobj_term(a, i); }); break;
+      case 6: {
+        double v = seq_sum(a.m, a.offset, [&](int i) { return hip_dobj_row_term(a, i); });
+        v = seq_sum(a.n, v, [&](int i) { return hip_dobj_lo_term(a, i); });
+        out[6] = seq_sum(a.n, v, [&](int i) { return hip_dobj_up_term(a, i); });
+        break;
+      }
+      default: out[7] = seq_sum(a.n, 0.0, [&](int i) { return hip_anchor_x_term(a, i); }); break;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kThreads, 3)
+hip_batch_round_kernel(const HipBatchMember* __restrict__ members, const HipState* __restrict__ states,
+                       HipBatchCtl* __restrict__ ctls) {
+  HipBatchCtl* ctl = ctls + blockIdx.x;
+  if (!ctl->active) return;
+  __shared__ HipBatchMember M;
+  __shared__ HipCheckArgs args;
+  __shared__ double sw[2];
+  copy_words(&M, members + blockIdx.x);
+  const HipState st = states[blockIdx.x];
+  const int first = ctl->first, restart = ctl->restart, fpe = ctl->fpe;
+  double* out = ctl->outs;
+  __syncthreads();
+  if (first) {
+    if (M.n > 0 && M.m > 0) {
+      const double lambda = hip_power_method(M, sw);
+      if (threadIdx.x == 0) out[kHipBatchLambda] = lambda;
+    }
+    // x = xa = proj_[l,u](0) (hip_init_kernel: upper first, then lower), y = ya = 0, the other iterate vectors 0
+    for (int i = threadIdx.x; i < M.n; i += kThreads) {
+      double v = 0.0;
+      if (v > M.upper[i]) v = M.upper[i];
+      if (v < M.lower[i]) v = M.lower[i];
+      M.x[i] = v; M.xa[i] = v;
+      M.xn[i] = 0.0; M.rx[i] = 0.0; M.hslack[i] = 0.0; M.sp[i] = 0.0; M.sn[i] = 0.0; M.atdy[i] = 0.0;
+    }
+    for (int r = threadIdx.x; r < M.m; r += kThreads) {
+      M.y[r] = 0.0; M.ya[r] = 0.0; M.yn[r] = 0.0; M.ry[r] = 0.0; M.dy[r] = 0.0;
+    }
+    if (threadIdx.x == 0) hip_batch_args(M, 0, args);
+    __syncthreads();
+    spmv(M.at_slices, M.at_col, M.at_val, M.n, M.y, M.aty);
+    __syncthreads();
+    hip_batch_check(M, 0, args, out);
+    return;
+  }
+  if (restart) {   // anchors and iterates <- the PDHG iterate of the last major step (:664-688)
+    for (int i = threadIdx.x; i < M.n; i += kThreads) { const double v = M.xn[i]; M.xa[i] = v; M.x[i] = v; }
+    for (int r = threadIdx.x; r < M.m; r += kThreads) { const double v = M.yn[r]; M.ya[r] = v; M.y[r] = v; }
+    __syncthreads();
+    spmv(M.at_slices, M.at_col, M.at_val, M.n, M.y, M.aty);
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) hip_batch_args(M, 1, args);
+  hip_batch_step(M, st.primal_step, st.dual_step, st.halpern_iteration, 1, 1);
+  if (fpe) {   // the restart's reference fixed-point error is that of the first step after it (:600-608)
+    hip_batch_atdy(M);
+    __syncthreads();
+    if (threadIdx.x == 0) out[kHipBatchFpe] = seq_sum(M.n, 0.0, [&](int i) { return hip_fpe_x_term(args, i); });
+    else if (threadIdx.x == 32) out[kHipBatchFpe + 1] = seq_sum(M.m, 0.0, [&](int i) { return hip_fpe_y_term(args, i); });
+    else if (threadIdx.x == 64) out[kHipBatchFpe + 2] = seq_sum(M.n, 0.0, [&](int i) { return hip_fpe_inter_term(args, i); });
+    __syncthreads();
+  }
+  for (int k = 2; k <= 39; k++) hip_batch_step(M, st.primal_step, st.dual_step, st.halpern_iteration, k, 0);
+  hip_batch_step(M, st.primal_step, st.dual_step, st.halpern_iteration, 40, 1);
+  hip_batch_check(M, 1, args, out);
+}
+
 }  // namespace
 
 void launch_batch_round(cudaStream_t s, int count, const BatchMember* members, PdhgState* states, BatchCtl* ctls) {
   if (count > 0) batch_round_kernel<<<count, kThreads, 0, s>>>(members, states, ctls);
+}
+
+void launch_hip_batch_round(cudaStream_t s, int count, const HipBatchMember* members, const HipState* states,
+                            HipBatchCtl* ctls) {
+  if (count > 0) hip_batch_round_kernel<<<count, kThreads, 0, s>>>(members, states, ctls);
 }
 
 }  // namespace b200

@@ -1,4 +1,5 @@
-// highs_b200/csrc/batch_kernels.hpp -- the batched ordered-mode solve (b200pdlp_solve_batch): one CTA per LP.
+// highs_b200/csrc/batch_kernels.hpp -- the batched ordered-mode solves (b200pdlp_solve_batch, b200pdlp_solve_hipdlp_batch):
+// one CTA per LP.
 #pragma once
 #include "kernels.cuh"
 
@@ -37,5 +38,38 @@ struct BatchCtl {
 
 // One round for every active member: blockIdx.x = member
 void launch_batch_round(cudaStream_t s, int count, const BatchMember* members, PdhgState* states, BatchCtl* ctls);
+
+// ---- the batched HiPDLP solve (b200pdlp_solve_hipdlp_batch): one CTA per LP, one round = one block of 40 Halpern steps
+
+// One member of a HiPDLP batch on the device: its ordered-mode sliced-ELL layouts and its vectors, inside the pooled buffers
+struct HipBatchMember {
+  int n, m, neq, scaled;
+  double offset;
+  const int4* a_slices;  const int* a_col;  const double* a_val;    // A  (m rows)
+  const int4* at_slices; const int* at_col; const double* at_val;   // A' (n rows)
+  const double *cost, *lower, *upper, *colscale, *rlo, *rup, *rowscale;
+  double *x, *xa, *xn, *rx, *aty, *hslack, *atyp, *atdy, *sp, *sn;   // n-vectors
+  double *y, *ya, *yn, *ry, *axp, *dy;                                // m-vectors
+};
+
+// Sums a round leaves in HipBatchCtl::outs
+//   0..8    the nine sums of the round's closing check (HipController's s[0..8]; 0..2 are 0 in round 0)
+//   9..11   the fixed-point sums of the round's first step (HipController::restart_reference), when HipBatchCtl::fpe is set
+//   12      the power method's estimate of |A|_2^2 (round 0, when n > 0 and m > 0)
+constexpr int kHipBatchOuts = 16;
+constexpr int kHipBatchFpe = 9, kHipBatchLambda = 12;
+
+// Per member, written by the host before a round and read back after it
+struct HipBatchCtl {
+  int active;    // 0: finished (its CTA returns at once)
+  int first;     // 1: round 0 -- power method, initial point, A'y, the iteration-0 check
+  int restart;   // a restart decided after the last block, applied first thing in this round: anchors and iterates <- (xn, yn)
+  int fpe;       // the restart's reference fixed-point error is due: the three sums of this round's first step
+  double outs[kHipBatchOuts];
+};
+
+// One round for every active member: blockIdx.x = member; states[i] holds the steps and halpern_iteration of the round
+void launch_hip_batch_round(cudaStream_t s, int count, const HipBatchMember* members, const HipState* states,
+                            HipBatchCtl* ctls);
 
 }  // namespace b200

@@ -2249,6 +2249,38 @@ static void hip_check(b200pdlp_problem* p, int major) {
   }
 }
 
+// unscaleSolution + postprocess (pdhg.cc:1883-1897, :359-492) of a host-prologue form on the host: x, y in device order
+// (cperm / rperm: device -> standard-form order), or nullptr when the run did not converge (the reference then returns
+// x = y = 0), and the dual slacks sp, sn of the last check in device order -> the four vectors of `out`, when it has them
+static void hip_host_postsolve(const b200pdlp_lp& lp, const StdForm& f, const int* cperm, const int* rperm, const double* x,
+                               const double* y, const double* sp, const double* sn, b200pdlp_result* out) {
+  const int n = f.n, m = f.m;
+  std::vector<double> hx(std::max(n, 1), 0.0), hy(std::max(m, 1), 0.0), hsp(std::max(n, 1)), hsn(std::max(n, 1));
+  if (x) {
+    for (int i = 0; i < n; i++) hx[cperm[i]] = x[i];
+    for (int i = 0; i < m; i++) hy[rperm[i]] = y[i];
+  }
+  for (int i = 0; i < n; i++) { hsp[cperm[i]] = sp[i]; hsn[cperm[i]] = sn[i]; }
+  if (f.scaled) {
+    for (int i = 0; i < n; i++) hx[i] /= f.col_scale[i];
+    for (int i = 0; i < m; i++) hy[i] /= f.row_scale[i];
+  }
+  for (int i = 0; i < n; i++) { hsp[i] *= f.col_scale[i]; hsn[i] *= f.col_scale[i]; }
+  if (out->col_value && out->col_dual && out->row_value && out->row_dual) {
+    for (int j = 0; j < f.n_orig; j++) out->col_value[j] = hx[j];
+    for (int i = 0; i < m; i++) {
+      const double d = hy[f.row_new_idx[i]];
+      out->row_dual[i] = f.row_class[i] == kLeq ? -d : d;
+    }
+    for (int i = 0; i < m; i++) out->row_value[i] = 0.0;
+    for (int c = 0; c < lp.num_col; c++) {
+      const double xv = hx[c];
+      for (int q = lp.a_start[c]; q < lp.a_start[c + 1]; q++) out->row_value[lp.a_index[q]] += lp.a_value[q] * xv;
+    }
+    for (int j = 0; j < f.n_orig; j++) { double v = hsp[j] - hsn[j]; v *= f.sense; out->col_dual[j] = v; }
+  }
+}
+
 static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, const b200pdlp_hipdlp_params& prm, b200pdlp_result* out) {
   NvtxRange nvtx("b200pdlp: solve (HiPDLP mode)");
   using clk = std::chrono::steady_clock;
@@ -2409,40 +2441,17 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
     }
     CUDA_OK(cudaStreamSynchronize(s));
   } else if (!p->dev_form && p->rank == 0) {
-    std::vector<double> hx(std::max(n, 1), 0.0), hy(std::max(m, 1), 0.0), hsp(std::max(n, 1)), hsn(std::max(n, 1));
-    {
-      std::vector<double> t(std::max(std::max(n, m), 1));
-      auto down_col = [&](const double* d, std::vector<double>& v) {
-        CUDA_OK(cudaMemcpyAsync(t.data(), d, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, s));
-        CUDA_OK(cudaStreamSynchronize(s));
-        for (int i = 0; i < n; i++) v[p->cperm[i]] = t[i];
-      };
-      if (converged) {
-        down_col(sol_x, hx);
-        if (m) CUDA_OK(cudaMemcpyAsync(t.data(), sol_y, (size_t)m * sizeof(double), cudaMemcpyDeviceToHost, s));
-        CUDA_OK(cudaStreamSynchronize(s));
-        for (int i = 0; i < m; i++) hy[p->rperm[i]] = t[i];
-      }
-      down_col(h.sp.p, hsp); down_col(h.sn.p, hsn);
-    }
-    if (f.scaled) {
-      for (int i = 0; i < n; i++) hx[i] /= f.col_scale[i];
-      for (int i = 0; i < m; i++) hy[i] /= f.row_scale[i];
-    }
-    for (int i = 0; i < n; i++) { hsp[i] *= f.col_scale[i]; hsn[i] *= f.col_scale[i]; }
-    if (out->col_value && out->col_dual && out->row_value && out->row_dual) {
-      for (int j = 0; j < f.n_orig; j++) out->col_value[j] = hx[j];
-      for (int i = 0; i < m; i++) {
-        const double d = hy[f.row_new_idx[i]];
-        out->row_dual[i] = f.row_class[i] == kLeq ? -d : d;
-      }
-      for (int i = 0; i < m; i++) out->row_value[i] = 0.0;
-      for (int c = 0; c < lp.num_col; c++) {
-        const double xv = hx[c];
-        for (int q = lp.a_start[c]; q < lp.a_start[c + 1]; q++) out->row_value[lp.a_index[q]] += lp.a_value[q] * xv;
-      }
-      for (int j = 0; j < f.n_orig; j++) { double v = hsp[j] - hsn[j]; v *= f.sense; out->col_dual[j] = v; }
-    }
+    // one download of the device-order vectors, then the host postsolve
+    std::vector<double> dx, dy, dsp, dsn;
+    auto down = [&](const double* d, std::vector<double>& v, int len) {
+      v.resize(std::max(len, 1));
+      if (len > 0) CUDA_OK(cudaMemcpyAsync(v.data(), d, (size_t)len * sizeof(double), cudaMemcpyDeviceToHost, s));
+    };
+    if (converged) { down(sol_x, dx, n); down(sol_y, dy, m); }
+    down(h.sp.p, dsp, n); down(h.sn.p, dsn, n);
+    CUDA_OK(cudaStreamSynchronize(s));
+    hip_host_postsolve(lp, f, p->cperm.data(), p->rperm.data(), converged ? dx.data() : nullptr,
+                       converged ? dy.data() : nullptr, dsp.data(), dsn.data(), out);
   }
   if (getenv("B200PDLP_TIMING"))
     fprintf(stderr, "[b200pdlp solve] postsolve (%s) %8.3f ms\n", p->dev_form ? "device" : "host",
@@ -2865,6 +2874,236 @@ static void solve_batch(int count, const b200pdlp_lp* lps, const b200pdlp_params
 }
 
 
+// ----------------------------------------------------------------------------------- batch of small LPs, HiPDLP mode
+// b200pdlp_solve_hipdlp_batch: every member is an ordered-mode HiPDLP problem, solved by one CTA of hip_batch_round_kernel
+// (batch_kernels.cu).  The host prologue (formulate_hipdlp, scale_hipdlp, build_layout) runs on host threads; the members are
+// packed into pooled buffers, one descriptor each.  A round is one block of 40 Halpern steps for every unfinished member
+// (round 0: the power method, the initial point and the iteration-0 check): one upload of the control blocks and states, one
+// launch, one read-back, then each member's HipController decisions in the order solve_hipdlp_on_device takes them.  The
+// PID weight's log / exp / log10 stay on the host.  Each member returns the bits b200pdlp_solve_hipdlp returns for it alone.
+
+// a member's standard form under HiPDLP's classification (std_form_cols with infinite thresholds, as use_device_prep_hipdlp)
+// must be an ordered-mode problem: checked before any device work
+static void check_hipdlp_batch_member(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params& prm, int i) {
+  const int rc = guarded([&] {
+    check_lp(lp);
+    const int omax = prm.ordered_max == 0 ? 4096 : prm.ordered_max;
+    if (omax < 0) throw Error(B200PDLP_ERR_ARG, "ordered_max < 0: a batch solves ordered-mode problems only");
+    const int n = std_form_cols(*lp, std::numeric_limits<double>::infinity());
+    if (std::max(n, lp->num_row) > omax)
+      throw Error(B200PDLP_ERR_ARG, "standard form " + std::to_string(lp->num_row) + " x " + std::to_string(n) +
+                                        " exceeds ordered_max = " + std::to_string(omax));
+  });
+  if (rc != B200PDLP_OK) throw Error(rc, "b200pdlp_solve_hipdlp_batch: member " + std::to_string(i) + ": " + g_last_error);
+}
+
+struct HipBatchHost {   // one member on the host
+  StdForm f;
+  HostLayout L;
+  size_t vec = 0, sl_a = 0, sl_at = 0, e_a = 0, e_at = 0;   // offsets in the pools
+  HipController ctl;
+  bool converged = false, timed_out = false;
+  int sol = 0;   // converged: 0 at the iteration-0 check (x, y), 1 after a block (xn, yn)
+};
+
+// doubles of a HiPDLP member's vector block: cost, lower, upper, colscale, then x xa xn rx aty hslack atyp atdy sp sn (n each);
+// rlo, rup, rowscale, then y ya yn ry axp dy (m each)
+static size_t hip_batch_vec_len(int n, int m) { return (size_t)14 * n + (size_t)9 * m; }
+
+static void solve_hipdlp_batch(int count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params& prm, b200pdlp_result* outs) {
+  using clk = std::chrono::steady_clock;
+  const auto t_begin = clk::now();
+  Laps lap;
+  device_count_checked();
+  if (prm.device >= 0) CUDA_OK(cudaSetDevice(prm.device));
+  StreamHolder sh;
+  cudaStream_t s = sh.s;
+  std::vector<HipBatchHost> B((size_t)count);
+  {
+    NvtxRange nvtx("b200pdlp: HiPDLP batch prologue (host threads)");
+    for_members(count, [&](int i) {
+      HipBatchHost& b = B[i];
+      formulate_hipdlp(lps[i], b.f);
+      scale_hipdlp(b.f, prm.scaling_mode, prm.ruiz_iterations);
+      build_layout(b.f, 0, 1, prm.ordered_max, b.L);
+      if (!b.L.ordered || !b.L.A.segs.empty() || !b.L.AT.segs.empty())
+        throw Error(B200PDLP_ERR_STATE, "the layout is not an ordered-mode layout");
+    });
+  }
+  lap("batch", "HiPDLP prologue (host threads)");
+
+  // ---- pooled device buffers: vectors, slice descriptors, column ids and values of A and A'; one descriptor per member
+  size_t nvec = 0, nsl = 0, nent = 0;
+  for (HipBatchHost& b : B) {
+    b.vec = nvec; nvec += hip_batch_vec_len(b.f.n, b.f.m);
+    b.sl_a = nsl; nsl += b.L.A.slices.size();
+    b.sl_at = nsl; nsl += b.L.AT.slices.size();
+    b.e_a = nent; nent += b.L.A.col.size();
+    b.e_at = nent; nent += b.L.AT.col.size();
+  }
+  std::vector<double> hvec(std::max<size_t>(nvec, 1), 0.0), hval(std::max<size_t>(nent, 1), 0.0);
+  std::vector<int> hcol(std::max<size_t>(nent, 1), 0);
+  std::vector<int4> hsl(std::max<size_t>(nsl, 1));
+  for_members(count, [&](int i) {
+    const HipBatchHost& b = B[i];
+    const StdForm& f = b.f;
+    const int n = f.n, m = f.m;
+    const int* cperm = b.L.cperm.data();
+    const int* rperm = b.L.rperm.data();
+    double* v = hvec.data() + b.vec;
+    double* w = v + 14 * n;
+    for (int j = 0; j < n; j++) {   // device order, as create_problem_hipdlp uploads them
+      v[j] = f.cost[cperm[j]]; v[n + j] = f.lower[cperm[j]]; v[2 * n + j] = f.upper[cperm[j]]; v[3 * n + j] = f.col_scale[cperm[j]];
+    }
+    for (int r = 0; r < m; r++) { w[r] = f.rhs[rperm[r]]; w[m + r] = f.row_upper[rperm[r]]; w[2 * m + r] = f.row_scale[rperm[r]]; }
+    static_assert(sizeof(SellMatrix::Slice) == sizeof(int4), "descriptor layout");
+    memcpy(hsl.data() + b.sl_a, b.L.A.slices.data(), b.L.A.slices.size() * sizeof(int4));
+    memcpy(hsl.data() + b.sl_at, b.L.AT.slices.data(), b.L.AT.slices.size() * sizeof(int4));
+    std::copy(b.L.A.col.begin(), b.L.A.col.end(), hcol.begin() + b.e_a);
+    std::copy(b.L.AT.col.begin(), b.L.AT.col.end(), hcol.begin() + b.e_at);
+    std::copy(b.L.A.val.begin(), b.L.A.val.end(), hval.begin() + b.e_a);
+    std::copy(b.L.AT.val.begin(), b.L.AT.val.end(), hval.begin() + b.e_at);
+  });
+  DevBuf<double> dvec, dval;
+  DevBuf<int> dcol;
+  DevBuf<int4> dsl;
+  DevBuf<HipBatchMember> dmem;
+  DevBuf<HipState> dst;
+  DevBuf<HipBatchCtl> dctl;
+  dvec.alloc(hvec.size(), false); dval.alloc(hval.size(), false); dcol.alloc(hcol.size(), false); dsl.alloc(hsl.size(), false);
+  dmem.alloc(count, false); dst.alloc(count, false); dctl.alloc(count, false);
+  std::vector<HipBatchMember> hmem((size_t)count);
+  for (int i = 0; i < count; i++) {
+    const HipBatchHost& b = B[i];
+    const int n = b.f.n, m = b.f.m;
+    double* v = dvec.p + b.vec;
+    double* w = v + 14 * n;
+    HipBatchMember& M = hmem[i];
+    M.n = n; M.m = m; M.neq = b.L.neq_local; M.scaled = b.f.scaled ? 1 : 0; M.offset = b.f.offset;
+    M.a_slices = dsl.p + b.sl_a; M.a_col = dcol.p + b.e_a; M.a_val = dval.p + b.e_a;
+    M.at_slices = dsl.p + b.sl_at; M.at_col = dcol.p + b.e_at; M.at_val = dval.p + b.e_at;
+    M.cost = v; M.lower = v + n; M.upper = v + 2 * n; M.colscale = v + 3 * n;
+    M.x = v + 4 * n; M.xa = v + 5 * n; M.xn = v + 6 * n; M.rx = v + 7 * n; M.aty = v + 8 * n; M.hslack = v + 9 * n;
+    M.atyp = v + 10 * n; M.atdy = v + 11 * n; M.sp = v + 12 * n; M.sn = v + 13 * n;
+    M.rlo = w; M.rup = w + m; M.rowscale = w + 2 * m;
+    M.y = w + 3 * m; M.ya = w + 4 * m; M.yn = w + 5 * m; M.ry = w + 6 * m; M.axp = w + 7 * m; M.dy = w + 8 * m;
+  }
+  PinnedArray<HipState> hst((size_t)count);
+  PinnedArray<HipBatchCtl> hctl((size_t)count);
+  memset(hst.p, 0, (size_t)count * sizeof(HipState));
+  for (int i = 0; i < count; i++) {
+    HipBatchCtl& c = hctl.p[i];
+    memset(&c, 0, sizeof(HipBatchCtl));
+    c.active = 1; c.first = 1;
+  }
+  CUDA_OK(cudaMemcpyAsync(dvec.p, hvec.data(), hvec.size() * sizeof(double), cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaMemcpyAsync(dval.p, hval.data(), hval.size() * sizeof(double), cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaMemcpyAsync(dcol.p, hcol.data(), hcol.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaMemcpyAsync(dsl.p, hsl.data(), hsl.size() * sizeof(int4), cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaMemcpyAsync(dmem.p, hmem.data(), (size_t)count * sizeof(HipBatchMember), cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaStreamSynchronize(s));
+  lap("batch", "pools + upload");
+
+  // ---- rounds
+  const double t_lim = (prm.time_limit >= 0 && std::isfinite(prm.time_limit)) ? prm.time_limit : -1.0;   // < 0: none
+  CudaEvent evl0, evl1, ev0, ev1;
+  double iter_ms = 0.0;
+  long long rounds = 0;
+  int active = count;
+  CUDA_OK(cudaEventRecord(evl0, s));
+  const auto t_loop = clk::now();
+  while (active > 0) {
+    NvtxRange nvtx("b200pdlp: HiPDLP batch round");
+    // solve_hipdlp_on_device reads its clock before every block.  There a restart decided after the last block copies the
+    // iterates before that test; here the copy is the first thing of the next round, so a member that times out never
+    // makes it.  That cannot show: the copy writes x, xa, y, ya and A'y only, an unconverged run returns x = y = 0, and the
+    // slacks sp / sn the postsolve reads are those of the last check in both solves.
+    if (rounds > 0 && t_lim >= 0 && std::chrono::duration<double>(clk::now() - t_loop).count() > t_lim) {
+      for (int i = 0; i < count; i++)
+        if (hctl.p[i].active) { B[i].timed_out = true; hctl.p[i].active = 0; }
+      break;
+    }
+    CUDA_OK(cudaMemcpyAsync(dctl.p, hctl.p, (size_t)count * sizeof(HipBatchCtl), cudaMemcpyHostToDevice, s));
+    CUDA_OK(cudaMemcpyAsync(dst.p, hst.p, (size_t)count * sizeof(HipState), cudaMemcpyHostToDevice, s));
+    CUDA_OK(cudaEventRecord(ev0, s));
+    launch_hip_batch_round(s, count, dmem.p, dst.p, dctl.p);
+    CUDA_OK(cudaEventRecord(ev1, s));
+    CUDA_OK(cudaMemcpyAsync(hctl.p, dctl.p, (size_t)count * sizeof(HipBatchCtl), cudaMemcpyDeviceToHost, s));
+    CUDA_OK(cudaStreamSynchronize(s));
+    float ms = 0.f;
+    CUDA_OK(cudaEventElapsedTime(&ms, ev0, ev1));
+    iter_ms += ms;
+    const bool first = rounds == 0;
+    rounds++;
+    for (int i = 0; i < count; i++) {
+      HipBatchCtl& c = hctl.p[i];
+      if (!c.active) continue;
+      HipBatchHost& b = B[i];
+      HipController& ctl = b.ctl;
+      const StdForm& f = b.f;
+      bool done = false, restart = false;
+      if (first) {   // iteration 0 (:566-572)
+        const double op_norm_sq = (f.n > 0 && f.m > 0) ? c.outs[kHipBatchLambda] : 1.0;
+        ctl.init(f.norm_cost, f.norm_rhs, op_norm_sq, prm.tolerance, prm.step_size_strategy);
+        if (ctl.converged(c.outs)) { b.converged = true; b.sol = 0; done = true; }
+        else done = ctl.iters >= prm.iter_limit;
+      } else {
+        if (c.fpe) ctl.restart_reference(c.outs + kHipBatchFpe);
+        restart = ctl.after_block(c.outs);
+        if (ctl.pfeas < ctl.tol * (1.0 + f.norm_rhs) && ctl.dfeas < ctl.tol * (1.0 + f.norm_cost) && ctl.relgap < ctl.tol) {
+          b.converged = true; b.sol = 1; done = true;
+        } else {
+          done = ctl.iters >= prm.iter_limit;
+        }
+      }
+      if (done) { c.active = 0; active--; continue; }
+      c.first = 0;
+      c.restart = restart ? 1 : 0;
+      c.fpe = ctl.pending_restart_fpe ? 1 : 0;
+      HipState& st = hst.p[i];
+      st.primal_step = ctl.primal_step; st.dual_step = ctl.dual_step; st.halpern_iteration = ctl.halpern_iteration;
+    }
+  }
+  CUDA_OK(cudaEventRecord(evl1, s));
+  CUDA_OK(cudaEventSynchronize(evl1));
+  float loop_ms = 0.f;
+  CUDA_OK(cudaEventElapsedTime(&loop_ms, evl0, evl1));
+  const double solve_seconds = std::chrono::duration<double>(clk::now() - t_loop).count();
+  lap("batch", "rounds");
+
+  // ---- the host postsolve of every member (hip_host_postsolve, as the single solve's host prologue path), one download
+  NvtxRange nvtx_post("b200pdlp: HiPDLP batch postsolve + download");
+  CUDA_OK(cudaMemcpyAsync(hvec.data(), dvec.p, hvec.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaStreamSynchronize(s));
+  const double setup_seconds = std::chrono::duration<double>(t_loop - t_begin).count();
+  for_members(count, [&](int i) {
+    const HipBatchHost& b = B[i];
+    const StdForm& f = b.f;
+    const HipController& ctl = b.ctl;
+    const int n = f.n, m = f.m;
+    const double* v = hvec.data() + b.vec;
+    const double* w = v + 14 * n;
+    const double* x = b.converged ? v + (b.sol ? 6 : 4) * n : nullptr;   // xn or x
+    const double* y = b.converged ? w + (b.sol ? 5 : 3) * m : nullptr;   // yn or y
+    b200pdlp_result* out = outs + i;
+    hip_host_postsolve(lps[i], f, b.L.cperm.data(), b.L.rperm.data(), x, y, v + 12 * n, v + 13 * n, out);
+    out->value_valid = 1; out->dual_valid = 1;
+    out->term_code = b.converged ? B200PDLP_OPTIMAL : B200PDLP_TIMELIMIT_OR_ITERLIMIT;
+    out->term_iterate = b.timed_out ? 2 : 0;
+    out->iters = ctl.iters; out->passes = ctl.iters; out->restarts = ctl.restarts;
+    out->kernel_launches = (int)std::min<long long>(rounds, 2147483647LL);
+    out->primal_obj = ctl.pobj; out->dual_obj = ctl.dobj; out->primal_feas = ctl.pfeas; out->dual_feas = ctl.dfeas;
+    out->gap = ctl.pobj - ctl.dobj; out->rel_gap = ctl.relgap;
+    out->setup_seconds = setup_seconds;
+    out->solve_seconds = solve_seconds;
+    out->loop_device_ms = loop_ms;
+    out->iter_device_ms = iter_ms;
+    out->form_cols = n; out->form_rows = m; out->form_nnz = f.nnz; out->form_neq = f.neq;
+  });
+  lap("batch", "postsolve (host threads)");
+}
+
+
 extern "C" {
 
 const char* b200pdlp_last_error(void) { return g_last_error.c_str(); }
@@ -3271,6 +3510,19 @@ int b200pdlp_solve_batch(int32_t count, const b200pdlp_lp* lps, const b200pdlp_p
     check_params(*params);
     for (int i = 0; i < count; i++) check_batch_member(&lps[i], *params, i);
     solve_batch(count, lps, *params, warms, outs);
+    CUDA_OK(cudaGetLastError());
+  });
+}
+
+int b200pdlp_solve_hipdlp_batch(int32_t count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params* params,
+                                b200pdlp_result* outs) {
+  DeviceGuard dg;
+  return guarded([&] {
+    if (count < 0) throw Error(B200PDLP_ERR_ARG, "b200pdlp_solve_hipdlp_batch: count < 0");
+    if (count == 0) return;
+    if (!lps || !params || !outs) throw Error(B200PDLP_ERR_ARG, "b200pdlp_solve_hipdlp_batch: null argument");
+    for (int i = 0; i < count; i++) check_hipdlp_batch_member(&lps[i], *params, i);
+    solve_hipdlp_batch(count, lps, *params, outs);
     CUDA_OK(cudaGetLastError());
   });
 }

@@ -1,8 +1,10 @@
-// highs_b200/csrc/pdhg_arith.cuh -- per-element arithmetic of the PDHG pass and of the ordered-mode check, shared by the
-// one-problem kernels (pdhg_kernels.cu) and the batch kernel (batch_kernels.cu), so that both produce the same bits.
+// highs_b200/csrc/pdhg_arith.cuh -- per-element arithmetic of the PDHG pass and of the ordered-mode check, and of the HiPDLP
+// step and check, shared by the one-problem kernels (pdhg_kernels.cu) and the batch kernels (batch_kernels.cu), so that both
+// produce the same bits.
 // Every function keeps the reference CPU path's operation order (see kernels.cuh; compiled with -fmad=false).
 #pragma once
 #include "kernels.cuh"
+#include "pdhg_kernels.hpp"
 
 namespace b200 {
 
@@ -148,5 +150,89 @@ __device__ __forceinline__ double row_check_b_term(double ax, double ips, double
   k = k * sc;
   return k * k;
 }
+
+// ---- HiPDLP mode (reflected Halpern PDHG, hipdlp/pdhg.cc): the one-problem kernels of pdhg_kernels.cu and the HiPDLP batch
+// kernel (batch_kernels.cu)
+
+__device__ __forceinline__ double std_max(double a, double b) { return a < b ? b : a; }   // std::max / std::min semantics
+__device__ __forceinline__ double std_min(double a, double b) { return b < a ? b : a; }
+
+// x-side of performHalpernPdhgStep (:974-986, :1006-1009) for column i; returns the reflected x
+__device__ __forceinline__ double hip_primal_col(int i, double ps, double w, int is_major, double* __restrict__ x,
+                                                 const double* __restrict__ xa, const double* __restrict__ c,
+                                                 const double* __restrict__ aty, const double* __restrict__ lo,
+                                                 const double* __restrict__ up, double* __restrict__ rx,
+                                                 double* __restrict__ xn, double* __restrict__ hslack) {
+  const double rho = 1.0;
+  const double xc = x[i];
+  const double temp = xc - ps * (c[i] - aty[i]);
+  const double proj = std_max(lo[i], std_min(temp, up[i]));
+  if (is_major) { xn[i] = proj; hslack[i] = (proj - temp) / ps; }
+  const double r = 2.0 * proj - xc;
+  rx[i] = r;
+  const double blended = rho * r + (1.0 - rho) * xc;
+  x[i] = w * blended + (1.0 - w) * xa[i];
+  return r;
+}
+
+// y-side (:992-1003, :1010-1013) of row r, given s = (A * reflected x)[r] and the row's y, anchor ya and bounds: returns the
+// blended y; a major step also stores the projected dual (y_next) in yn[r] and the reflected y in ry[r]
+__device__ __forceinline__ double hip_dual_blend(int r, double y, double ya, double lo, double up, double s, double ds, double w,
+                                                 int is_major, double* yn, double* ry) {
+  const double rho = 1.0;
+  const double temp = y / ds - s;
+  const double proj = std_max(-up, std_min(temp, -lo));
+  const double pd = (temp - proj) * ds;
+  const double refl = 2.0 * pd - y;
+  if (is_major) { yn[r] = pd; ry[r] = refl; }
+  const double blended = rho * refl + (1.0 - rho) * y;
+  return w * blended + (1.0 - w) * ya;
+}
+
+// dual slack of column i (computeDualSlacks, :1322-1378): the cached major-step slack when there is one, otherwise the
+// residual projected by the signs of the bounds; sp / sn are its positive and negative parts
+__device__ __forceinline__ void hip_dual_slacks(int i, int use_cached, const double* __restrict__ hslack,
+                                                const double* __restrict__ c, const double* __restrict__ aty,
+                                                const double* __restrict__ lo, const double* __restrict__ up, double& sp,
+                                                double& sn) {
+  double slack = 0.0;
+  if (use_cached) slack = hslack[i];
+  else {
+    const double dres = c[i] - aty[i];
+    const bool hl = lo[i] > -INFINITY, hu = up[i] < INFINITY;
+    if (hl && hu) slack = dres;
+    else if (hl) slack = std_max(0.0, dres);
+    else if (hu) slack = std_min(0.0, dres);
+  }
+  sp = std_max(0.0, slack);
+  sn = std_max(0.0, -slack);
+}
+
+// The terms of the nine sums of a HiPDLP check (hip_check_ordered_kernel; each sum adds its terms in index order):
+//   0 |x_next - refl_x|^2  1 |y_next - refl_y|^2  2 (x_next - refl_x).(A' dy)        (fixed-point error, :709-740)
+//   3 |primal residual|^2 (:1297-1320)  4 |dual residual|^2 (:1380-1408)  5 offset + c.x (:1496-1500)
+//   6 offset + b.y + l.sp - u.sn (:1447-1472): rows, then lower bounds, then upper bounds, one running sum
+//   7 |x_next - x_anchor|^2  8 |y_next - y_anchor|^2                                    (PID weight, :1984-1999)
+__device__ __forceinline__ double hip_fpe_x_term(const HipCheckArgs& a, int i) { const double d = a.x[i] - a.rx[i]; return d * d; }
+__device__ __forceinline__ double hip_fpe_y_term(const HipCheckArgs& a, int i) { const double d = a.y[i] - a.ry[i]; return d * d; }
+__device__ __forceinline__ double hip_fpe_inter_term(const HipCheckArgs& a, int i) { return (a.x[i] - a.rx[i]) * a.atdy[i]; }
+__device__ __forceinline__ double hip_primal_res_term(const HipCheckArgs& a, int i) {
+  double r = a.ax[i] - a.rlo[i];
+  if (i >= a.neq) r = std_min(0.0, r);
+  if (a.scaled) r = r * a.rowscale[i];
+  return r * r;
+}
+__device__ __forceinline__ double hip_dual_res_term(const HipCheckArgs& a, int i) {
+  double r = (a.c[i] - a.aty[i]) - a.sp[i] + a.sn[i];
+  if (a.scaled) r = r * a.colscale[i];
+  return r * r;
+}
+__device__ __forceinline__ double hip_pobj_term(const HipCheckArgs& a, int i) { return a.c[i] * a.x[i]; }
+__device__ __forceinline__ double hip_dobj_row_term(const HipCheckArgs& a, int i) { return a.rlo[i] * a.y[i]; }
+// skipped (infinite-bound) columns add nothing in the reference: + 0.0 leaves the running sum unchanged
+__device__ __forceinline__ double hip_dobj_lo_term(const HipCheckArgs& a, int i) { return a.lo[i] > -INFINITY ? a.lo[i] * a.sp[i] : 0.0; }
+__device__ __forceinline__ double hip_dobj_up_term(const HipCheckArgs& a, int i) { return a.up[i] < INFINITY ? -(a.up[i] * a.sn[i]) : 0.0; }
+__device__ __forceinline__ double hip_anchor_x_term(const HipCheckArgs& a, int i) { const double d = a.x[i] - a.xa[i]; return d * d; }
+__device__ __forceinline__ double hip_anchor_y_term(const HipCheckArgs& a, int i) { const double d = a.y[i] - a.ya[i]; return d * d; }
 
 }  // namespace b200

@@ -2094,26 +2094,6 @@ void launch_fill(cudaStream_t s, int len, double* v, double w) {
 // STATUS (round 2): bit-exact against the oracle on hardware (tests/test_gpu_hipdlp.py, ~160 solves).
 namespace b200 {
 
-__device__ __forceinline__ double std_max(double a, double b) { return a < b ? b : a; }   // std::max / std::min semantics
-__device__ __forceinline__ double std_min(double a, double b) { return b < a ? b : a; }
-
-// x-side of performHalpernPdhgStep (:974-986, :1006-1009) for column i; returns the reflected x
-__device__ __forceinline__ double hip_primal_col(int i, double ps, double w, int is_major, double* __restrict__ x,
-                                                 const double* __restrict__ xa, const double* __restrict__ c,
-                                                 const double* __restrict__ aty, const double* __restrict__ lo,
-                                                 const double* __restrict__ up, double* __restrict__ rx,
-                                                 double* __restrict__ xn, double* __restrict__ hslack) {
-  const double rho = 1.0;
-  const double xc = x[i];
-  const double temp = xc - ps * (c[i] - aty[i]);
-  const double proj = std_max(lo[i], std_min(temp, up[i]));
-  if (is_major) { xn[i] = proj; hslack[i] = (proj - temp) / ps; }
-  const double r = 2.0 * proj - xc;
-  rx[i] = r;
-  const double blended = rho * r + (1.0 - rho) * xc;
-  x[i] = w * blended + (1.0 - w) * xa[i];
-  return r;
-}
 __global__ void __launch_bounds__(kThreads)
 hip_primal_kernel(int n, const HipState* __restrict__ st, int k_offset, int is_major, double* __restrict__ x,
                   const double* __restrict__ xa, const double* __restrict__ c, const double* __restrict__ aty,
@@ -2147,16 +2127,7 @@ struct HipDualEpilogue {
   double p_y, p_ya, p_lo, p_up;
   __device__ void prefetch(int r) { p_y = y[r]; p_ya = ya[r]; p_lo = rlo[r]; p_up = rup[r]; }
   // the blended y of row r, given s = (A * reflected x)[r]
-  __device__ double blend(int r, double s) const {
-    const double rho = 1.0;
-    const double temp = p_y / ds - s;
-    const double proj = std_max(-p_up, std_min(temp, -p_lo));
-    const double pd = (temp - proj) * ds;
-    const double refl = 2.0 * pd - p_y;
-    if (is_major) { yn[r] = pd; ry[r] = refl; }
-    const double blended = rho * refl + (1.0 - rho) * p_y;
-    return w * blended + (1.0 - w) * p_ya;
-  }
+  __device__ double blend(int r, double s) const { return hip_dual_blend(r, p_y, p_ya, p_lo, p_up, s, ds, w, is_major, yn, ry); }
   __device__ void row(int r, double s, double*) const { y[r] = blend(r, s); }
 };
 
@@ -2196,17 +2167,10 @@ hip_slack_kernel(int n, int use_cached, const double* __restrict__ hslack, const
                  const double* __restrict__ lo, const double* __restrict__ up, double* __restrict__ sp, double* __restrict__ sn) {
   const int stride = gridDim.x * kThreads;
   for (int i = blockIdx.x * kThreads + threadIdx.x; i < n; i += stride) {
-    double slack = 0.0;
-    if (use_cached) slack = hslack[i];
-    else {
-      const double dres = c[i] - aty[i];
-      const bool hl = lo[i] > -INFINITY, hu = up[i] < INFINITY;
-      if (hl && hu) slack = dres;
-      else if (hl) slack = std_max(0.0, dres);
-      else if (hu) slack = std_min(0.0, dres);
-    }
-    sp[i] = std_max(0.0, slack);
-    sn[i] = std_max(0.0, -slack);
+    double a, b;
+    hip_dual_slacks(i, use_cached, hslack, c, aty, lo, up, a, b);
+    sp[i] = a;
+    sn[i] = b;
   }
 }
 void launch_hip_slack(cudaStream_t s, int n, int use_cached, const double* hslack, const double* c, const double* aty,
@@ -2236,30 +2200,20 @@ __global__ void __launch_bounds__(9 * 32) hip_check_ordered_kernel(HipCheckArgs 
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   double v = 0.0;
   switch (w) {
-    case 0: if (with_fpe) v = warp_ordered_sum(a.n, 0.0, [&](int i) { const double d = a.x[i] - a.rx[i]; return d * d; }); break;
-    case 1: if (with_fpe) v = warp_ordered_sum(a.m, 0.0, [&](int i) { const double d = a.y[i] - a.ry[i]; return d * d; }); break;
-    case 2: if (with_fpe) v = warp_ordered_sum(a.n, 0.0, [&](int i) { return (a.x[i] - a.rx[i]) * a.atdy[i]; }); break;
-    case 3: v = warp_ordered_sum(a.m, 0.0, [&](int i) {
-              double r = a.ax[i] - a.rlo[i];
-              if (i >= a.neq) r = std_min(0.0, r);
-              if (a.scaled) r = r * a.rowscale[i];
-              return r * r; });
-            break;
-    case 4: v = warp_ordered_sum(a.n, 0.0, [&](int i) {
-              double r = (a.c[i] - a.aty[i]) - a.sp[i] + a.sn[i];
-              if (a.scaled) r = r * a.colscale[i];
-              return r * r; });
-            break;
-    case 5: v = warp_ordered_sum(a.n, a.offset, [&](int i) { return a.c[i] * a.x[i]; }); break;
+    case 0: if (with_fpe) v = warp_ordered_sum(a.n, 0.0, [&](int i) { return hip_fpe_x_term(a, i); }); break;
+    case 1: if (with_fpe) v = warp_ordered_sum(a.m, 0.0, [&](int i) { return hip_fpe_y_term(a, i); }); break;
+    case 2: if (with_fpe) v = warp_ordered_sum(a.n, 0.0, [&](int i) { return hip_fpe_inter_term(a, i); }); break;
+    case 3: v = warp_ordered_sum(a.m, 0.0, [&](int i) { return hip_primal_res_term(a, i); }); break;
+    case 4: v = warp_ordered_sum(a.n, 0.0, [&](int i) { return hip_dual_res_term(a, i); }); break;
+    case 5: v = warp_ordered_sum(a.n, a.offset, [&](int i) { return hip_pobj_term(a, i); }); break;
     case 6: {
-      v = warp_ordered_sum(a.m, a.offset, [&](int i) { return a.rlo[i] * a.y[i]; });
-      // skipped (infinite-bound) columns add nothing in the reference: + 0.0 leaves the running sum unchanged
-      v = warp_ordered_sum(a.n, v, [&](int i) { return a.lo[i] > -INFINITY ? a.lo[i] * a.sp[i] : 0.0; });
-      v = warp_ordered_sum(a.n, v, [&](int i) { return a.up[i] < INFINITY ? -(a.up[i] * a.sn[i]) : 0.0; });
+      v = warp_ordered_sum(a.m, a.offset, [&](int i) { return hip_dobj_row_term(a, i); });
+      v = warp_ordered_sum(a.n, v, [&](int i) { return hip_dobj_lo_term(a, i); });
+      v = warp_ordered_sum(a.n, v, [&](int i) { return hip_dobj_up_term(a, i); });
       break;
     }
-    case 7: v = warp_ordered_sum(a.n, 0.0, [&](int i) { const double d = a.x[i] - a.xa[i]; return d * d; }); break;
-    case 8: v = warp_ordered_sum(a.m, 0.0, [&](int i) { const double d = a.y[i] - a.ya[i]; return d * d; }); break;
+    case 7: v = warp_ordered_sum(a.n, 0.0, [&](int i) { return hip_anchor_x_term(a, i); }); break;
+    case 8: v = warp_ordered_sum(a.m, 0.0, [&](int i) { return hip_anchor_y_term(a, i); }); break;
   }
   if (lane == 0) out[w] = v;
 }

@@ -79,6 +79,7 @@ ABI_SYMBOLS = [
     "b200pdlp_debug_prep_compare_hipdlp", "b200pdlp_debug_hipdlp_shard_prep_compare", "b200pdlp_release_cache",
     "b200pdlp_host_register", "b200pdlp_host_unregister", "b200pdlp_primal_step", "b200pdlp_dual_step", "b200pdlp_residuals",
     "b200pdlp_kkt_check", "b200pdlp_kkt_check_host", "b200pdlp_kkt_default_tolerances", "b200pdlp_solve_batch",
+    "b200pdlp_solve_hipdlp_batch",
 ]
 
 _lib = None
@@ -398,6 +399,26 @@ def solve_hipdlp(lp: HighsLp, **params) -> dict:
     res, arrays = _mk_result(lp, 0)
     _check(L.b200pdlp_solve_hipdlp(C.byref(clp), C.byref(prm), C.byref(res)), "b200pdlp_solve_hipdlp")
     return _result_dict(res, arrays)
+
+
+def solve_hipdlp_batch(lps, **params) -> list:
+    """b200pdlp_solve_hipdlp_batch: every LP of `lps` (ordered-mode problems under HiPDLP's classification) solved in the
+    HiPDLP mode on one GPU in one call, one CTA per LP.  Takes the parameters of solve_hipdlp (device_prep is ignored) and
+    returns the dicts solve_hipdlp returns, in order; each holds the bits solve_hipdlp returns for that LP alone (the timings
+    and kernel_launches are the batch's)."""
+    lps = list(lps)
+    L = lib()
+    L.b200pdlp_solve_hipdlp_batch.argtypes = [C.c_int32, C.POINTER(CLp), C.POINTER(CHipdlpParams), C.POINTER(CResult)]
+    count = len(lps)
+    clps, cres, keep, arrays = (CLp * max(count, 1))(), (CResult * max(count, 1))(), [], []
+    for i, lp in enumerate(lps):
+        clps[i], k = make_clp(lp)
+        keep.append(k)
+        cres[i], a = _mk_result(lp, 0)
+        arrays.append(a)
+    prm = _hipdlp_params(params)
+    _check(L.b200pdlp_solve_hipdlp_batch(count, clps, C.byref(prm), cres), "b200pdlp_solve_hipdlp_batch")
+    return [_result_dict(cres[i], arrays[i]) for i in range(count)]
 
 
 def solve_hipdlp_multi(lp: HighsLp, ngpus: int, devices=None, out_arrays=None, **params) -> dict:

@@ -268,6 +268,23 @@ typedef struct {
 } b200pdlp_hipdlp_params;
 void b200pdlp_hipdlp_default_params(b200pdlp_hipdlp_params* p);
 int b200pdlp_solve_hipdlp(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params* params, b200pdlp_result* out);
+/* Solve `count` independent LPs in the HiPDLP mode on one GPU in one call.  Every member must be an ordered-mode problem of
+ * `params` under HiPDLP's classification (standard form max(n, m) <= ordered_max, a slack column for every ranged and free
+ * row, rows bounded by +-infinity only); each returns exactly what b200pdlp_solve_hipdlp(lps[i], params) returns: term_code,
+ * term_iterate, iters, passes, restarts, the residual scalars, the form dimensions and all four vectors, bit for bit.
+ * All members share `params` (tolerance, limits, scaling, step-size strategy); `device` selects the GPU; `device_prep` is
+ * ignored (ordered mode always takes the host prologue); log_level prints nothing per block.  One CTA solves one member;
+ * the members' host prologues and postsolves run on host threads.  The time limit counts from the start of the batch's
+ * loop.  These fields are batch-wide, the same in every outs[i]: setup_seconds, solve_seconds, loop_device_ms,
+ * iter_device_ms and kernel_launches (= the batch's rounds, one launch each; a round is one block of 40 steps).
+ * Returns B200PDLP_ERR_ARG before any device work for count < 0, NULL arrays, a member that the checks of
+ * b200pdlp_solve_hipdlp reject, ordered_max < 0, or a member whose standard form exceeds ordered_max; b200pdlp_last_error()
+ * names the member's index, and no result is written.  count == 0: B200PDLP_OK.  No device: B200PDLP_ERR_CUDA.  The whole
+ * batch must fit in device memory (B200PDLP_ERR_ALLOC otherwise).
+ * STATUS: runs on hardware; tests/test_gpu_hipdlp_batch.py (byte equality with b200pdlp_solve_hipdlp and with the HiPDLP
+ * oracle), tools/batch_bench.py --solver hipdlp. */
+int b200pdlp_solve_hipdlp_batch(int32_t count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params* params,
+                                b200pdlp_result* outs /* [count], caller-allocated like b200pdlp_result */);
 /* The HiPDLP solve on `ngpus` devices of THIS process (devices[g] or, if NULL, ordinals 0..ngpus-1; a device may repeat,
  * which gives logical shards on one device): the prologue, then each rank computes contiguous blocks of the one-GPU device
  * rows and columns, one host thread per rank, peer memory, no NCCL.  device_prep is honoured as on one GPU: 0 runs the

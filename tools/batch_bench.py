@@ -6,7 +6,9 @@ iterations at the default tolerances; the bound keeps the loop arm to minutes). 
 in alternating order --repeats times; the two must return identical bits.  Prints one JSON line: per workload the best
 time of each arm, LPs/s, summed PDHG iterations/s, the batch's rounds, its host time per round beside its kernel time per
 round, and the speed-up, with the card's name and power limit read in the same run.
-    python tools/batch_bench.py [--replicas 8] [--iter-limit 500] [--repeats 2]
+--solver hipdlp: the same measurement for the HiPDLP mode, b200pdlp_solve_hipdlp_batch against a loop of
+b200pdlp_solve_hipdlp, on the instances whose HiPDLP standard form is ordered, at the default tolerance and at 1e-4.
+    python tools/batch_bench.py [--solver pdlp|hipdlp] [--replicas 8] [--iter-limit 500] [--repeats 2]
 """
 import argparse
 import glob
@@ -52,31 +54,34 @@ def main():
     ap.add_argument("--replicas", type=int, default=8)
     ap.add_argument("--iter-limit", type=int, default=500)
     ap.add_argument("--repeats", type=int, default=2)
+    ap.add_argument("--solver", choices=("pdlp", "hipdlp"), default="pdlp")
     a = ap.parse_args()
+    hip = a.solver == "hipdlp"
     if engine.device_count() == 0:
         sys.exit("batch_bench.py needs a CUDA device")
     lps = []
     for p in sorted(glob.glob(os.path.join(ROOT, "tests", "golden", "instances", "*.b2lp"))):
         lp = read_b2lp(p)
-        f = engine.host_form(lp, 1)
+        f = engine.host_form_hipdlp(lp) if hip else engine.host_form(lp, 1)
         if max(f["n"], f["m"]) <= 4096:
             lps.append(lp)
     work = lps * a.replicas
-    result = dict(card(), instances=len(lps), replicas=a.replicas, members=len(work), iter_limit=a.iter_limit,
-                  repeats=a.repeats, workloads=[])
+    result = dict(card(), **({"solver": "hipdlp"} if hip else {}), instances=len(lps), replicas=a.replicas, members=len(work),
+                  iter_limit=a.iter_limit, repeats=a.repeats, workloads=[])
     for name, tol in (("default", None), ("kkt1e-4", 1e-4)):
         kw = dict(iter_limit=a.iter_limit)
         if tol:
-            kw.update(tol_primal=tol, tol_dual=tol, tol_gap=tol)
+            kw.update(dict(tolerance=tol) if hip else dict(tol_primal=tol, tol_dual=tol, tol_gap=tol))
+        solve_batch, solve = (engine.solve_hipdlp_batch, engine.solve_hipdlp) if hip else (engine.solve_batch, engine.solve)
 
         def run_batch():
             t = time.perf_counter()
-            r = engine.solve_batch(work, **kw)
+            r = solve_batch(work, **kw)
             return time.perf_counter() - t, r
 
         def run_loop():
             t = time.perf_counter()
-            r = [engine.solve(lp, **kw) for lp in work]
+            r = [solve(lp, **kw) for lp in work]
             return time.perf_counter() - t, r
 
         run_batch(); run_loop()   # warm-up (module loads, allocation caches)
