@@ -28,6 +28,7 @@
 #include <vector>
 
 #include "batch_kernels.hpp"
+#include "batch_prep.hpp"
 #include "device_prep.hpp"
 #include "host_prep.hpp"
 #include "pdhg_kernels.hpp"
@@ -2516,10 +2517,15 @@ static void check_params(const b200pdlp_params& prm) {
     throw Error(B200PDLP_ERR_ARG, "b200pdlp: params.device_scaling must be 0 (default) or -1 (host prologue)");
 }
 
+// what check_lp checks without reading an array: the sizes, and the arrays the sizes call for are present
+static bool lp_fields_ok(const b200pdlp_lp* lp) {
+  return lp && lp->num_col >= 0 && lp->num_row >= 0 && lp->a_start && (lp->num_col == 0 || (lp->col_cost && lp->col_lower && lp->col_upper)) &&
+         (lp->num_row == 0 || (lp->row_lower && lp->row_upper));
+}
+
 // deep: also the O(n) / O(nnz) validation of a_start and a_index (the device prologue does both in its first sweep)
 static void check_lp(const b200pdlp_lp* lp, bool deep = true) {
-  if (!lp || lp->num_col < 0 || lp->num_row < 0 || !lp->a_start || (lp->a_start[lp->num_col] > 0 && (!lp->a_index || !lp->a_value)) ||
-      (lp->num_col > 0 && (!lp->col_cost || !lp->col_lower || !lp->col_upper)) || (lp->num_row > 0 && (!lp->row_lower || !lp->row_upper)))
+  if (!lp_fields_ok(lp) || (lp->a_start[lp->num_col] > 0 && (!lp->a_index || !lp->a_value)))
     throw Error(B200PDLP_ERR_ARG, "b200pdlp: malformed b200pdlp_lp");
   if (lp->sense != 1.0 && lp->sense != -1.0) throw Error(B200PDLP_ERR_ARG, "b200pdlp: sense must be +1 or -1");
   // formulate() indexes per-row arrays with a_index and walks a_start: validate both once (O(nnz), a few ms at 8M nonzeros)
@@ -2608,16 +2614,20 @@ static void check_batch_member(const b200pdlp_lp* lp, const b200pdlp_params& prm
   if (rc != B200PDLP_OK) throw Error(rc, "b200pdlp_solve_batch: member " + std::to_string(i) + ": " + g_last_error);
 }
 
-struct BatchHost {   // one member on the host
-  StdForm f;
-  HostLayout L;
-  std::vector<double> x0, y0;
-  size_t vec = 0, sl_a = 0, sl_at = 0, e_a = 0, e_at = 0;   // offsets in the pools
+struct BatchRun {   // one member's host control over the rounds
+  StdForm f;        // b200pdlp_solve_batch_device fills the scalars only: dimensions, sense, offset, norms, amax
+  double cost_sq = 0.0, rhs_sq = 0.0;   // |c|^2 and |b|^2 of the scaled form, index order: what sets beta
   RestartMemo memo;
   CheckResult chk;
   int term = B200PDLP_TIMELIMIT_OR_ITERLIMIT, term_iterate = 0, restarts = 0;
   bool have_check = false;
   double tol_p = 0.0, tol_d = 0.0;
+};
+
+struct BatchHost : BatchRun {   // one member of b200pdlp_solve_batch on the host
+  HostLayout L;
+  std::vector<double> x0, y0;
+  size_t vec = 0, sl_a = 0, sl_at = 0, e_a = 0, e_at = 0;   // offsets in the pools
 };
 
 // pinned host array, returned to the pinned cache
@@ -2642,6 +2652,144 @@ struct StreamHolder {
 // rhs, rowscale, then y0 y1 ax0 ax1 ysum yavg axavg ylr (m each)
 static size_t batch_vec_len(int n, int m) { return (size_t)12 * n + (size_t)10 * m; }
 
+// the vectors of a member's block `v` (batch_vec_len) as BatchMember pointers
+static void batch_member_vectors(BatchMember& M, double* v, int n, int m) {
+  double* w = v + 12 * (size_t)n;
+  M.n = n; M.m = m;
+  M.cost = v; M.lower = v + n; M.upper = v + 2 * n; M.colscale = v + 3 * n;
+  M.x0 = v + 4 * n; M.x1 = v + 5 * n; M.aty0 = v + 6 * n; M.aty1 = v + 7 * n;
+  M.xsum = v + 8 * n; M.xavg = v + 9 * n; M.atyavg = v + 10 * n; M.xlr = v + 11 * n;
+  M.rhs = w; M.rowscale = w + m;
+  M.y0 = w + 2 * m; M.y1 = w + 3 * m; M.ax0 = w + 4 * m; M.ax1 = w + 5 * m;
+  M.ysum = w + 6 * m; M.yavg = w + 7 * m; M.axavg = w + 8 * m; M.ylr = w + 9 * m;
+}
+
+struct BatchLoop {
+  std::chrono::steady_clock::time_point t_loop;   // the start of the rounds (the time limit counts from here)
+  long long rounds = 0;
+  double iter_ms = 0.0, solve_seconds = 0.0;
+  float loop_ms = 0.f;
+};
+
+// The rounds of a batch, for both entry points: each member's initial state from its form's scalars, then per round one
+// upload of the control blocks and states, one launch, one read-back and the decisions of every member that checked (the
+// functions solve_on_device calls), until no member is active.  hst: `count` pinned states, the final ones on return.
+static BatchLoop batch_rounds(cudaStream_t s, int count, const b200pdlp_params& prm, const BatchMember* dmem,
+                              const std::vector<BatchRun*>& R, PdhgState* hst, b200pdlp_result* outs) {
+  using clk = std::chrono::steady_clock;
+  // ---- initial states: PDHG_Init_Step_Sizes (cupdlp_step.c:312-375); a fixed step takes tau, sigma after round 0's power method
+  PinnedArray<BatchCtl> hctl((size_t)count);
+  for (int i = 0; i < count; i++) {
+    const BatchRun& r = *R[i];
+    PdhgState* h = hst + i;
+    memset(h, 0, sizeof(PdhgState));
+    h->adaptive = prm.adaptive_step != 0;
+    const double a = r.cost_sq, b = r.rhs_sq;
+    h->beta = std::fmin(a, b) > 1e-6 ? a / b : 1.0;
+    if (h->adaptive) {
+      h->tau = (1.0 / r.f.amax) / std::sqrt(h->beta);
+      h->sigma = h->tau * h->beta;
+    }
+    arm_step(h);
+    fill_pow_tables(h);
+    h->stop_iter = 0;   // the first check is due at once (iteration 0)
+    BatchCtl& c = hctl.p[i];
+    memset(&c, 0, sizeof(BatchCtl));
+    c.active = 1; c.first = 1; c.fixed_step = !h->adaptive; c.no_check = prm.iter_limit <= 0;
+    outs[i].trace_len = 0;
+  }
+  DevBuf<PdhgState> dst;
+  DevBuf<BatchCtl> dctl;
+  dst.alloc(count, false); dctl.alloc(count, false);
+
+  const int interval = prm.check_interval > 0 ? prm.check_interval : 40;
+  const double t_lim = (prm.time_limit >= 0 && std::isfinite(prm.time_limit)) ? prm.time_limit : -1.0;   // < 0: none
+  CudaEvent evl0, evl1, ev0, ev1;
+  BatchLoop L;
+  int active = count;
+  CUDA_OK(cudaEventRecord(evl0, s));
+  L.t_loop = clk::now();
+  while (active > 0) {
+    NvtxRange nvtx("b200pdlp: batch round");
+    const bool timed_out = t_lim >= 0 && std::chrono::duration<double>(clk::now() - L.t_loop).count() > t_lim;
+    CUDA_OK(cudaMemcpyAsync(dctl.p, hctl.p, (size_t)count * sizeof(BatchCtl), cudaMemcpyHostToDevice, s));
+    CUDA_OK(cudaMemcpyAsync(dst.p, hst, (size_t)count * sizeof(PdhgState), cudaMemcpyHostToDevice, s));
+    CUDA_OK(cudaEventRecord(ev0, s));
+    launch_batch_round(s, count, dmem, dst.p, dctl.p);
+    CUDA_OK(cudaEventRecord(ev1, s));
+    CUDA_OK(cudaMemcpyAsync(hctl.p, dctl.p, (size_t)count * sizeof(BatchCtl), cudaMemcpyDeviceToHost, s));
+    // the scalars of every state (the power tables are the host's own)
+    CUDA_OK(cudaMemcpy2DAsync(hst, sizeof(PdhgState), dst.p, sizeof(PdhgState), offsetof(PdhgState, pow_red), count,
+                              cudaMemcpyDeviceToHost, s));
+    CUDA_OK(cudaStreamSynchronize(s));
+    float ms = 0.f;
+    CUDA_OK(cudaEventElapsedTime(&ms, ev0, ev1));
+    L.iter_ms += ms;
+    const bool first = L.rounds == 0;
+    L.rounds++;
+    for (int i = 0; i < count; i++) {
+      BatchCtl& c = hctl.p[i];
+      if (!c.active) continue;
+      BatchRun& b = *R[i];
+      PdhgState* h = hst + i;
+      b200pdlp_result* out = outs + i;
+      if (!c.checked) {
+        if (first && c.no_check) { c.active = 0; active--; continue; }   // iter_limit <= 0: no check at all
+        fill_pow_tables(h);   // the tables ran out before the check iteration: refill, the next round goes on
+        continue;
+      }
+      if (first && c.fixed_step) {
+        const double lambda = c.outs[kBatchLambda];
+        h->tau = 0.8 / std::sqrt(lambda);
+        h->sigma = h->tau;
+        h->tau /= std::sqrt(h->beta);
+        h->sigma *= std::sqrt(h->beta);
+        arm_step(h);
+      }
+      CheckResult& chk = b.chk;
+      double dscale[2], pscale[2];
+      assemble_check_a(b.f, c.outs, chk, dscale, pscale);
+      assemble_check_b(b.f, c.outs, chk, dscale, pscale);
+      chk.timed_out = timed_out;
+      b.have_check = true;
+      int choice = 0;
+      const int t_code = check_decision(prm, b.tol_p, b.tol_d, h, chk, b.memo, &b.term_iterate, &choice);
+      if (t_code >= 0) {
+        b.term = t_code;
+        trace_row(out, h, chk, 0);
+        c.active = 0;
+        active--;
+        continue;
+      }
+      if (choice) {
+        restart_steps(h, choice, chk, b.memo, c.outs[choice == 1 ? kBatchDxAvg : kBatchDxCur],
+                      c.outs[choice == 1 ? kBatchDyAvg : kBatchDyCur]);
+        b.restarts++;
+        arm_step(h);
+        c.restart = choice;
+      }
+      trace_row(out, h, chk, choice);
+      h->stop_iter = next_check_iter(h->iter, interval, prm.iter_limit);
+      fill_pow_tables(h);
+    }
+  }
+  CUDA_OK(cudaEventRecord(evl1, s));
+  CUDA_OK(cudaEventSynchronize(evl1));
+  CUDA_OK(cudaEventElapsedTime(&L.loop_ms, evl0, evl1));
+  L.solve_seconds = std::chrono::duration<double>(clk::now() - L.t_loop).count();
+  return L;
+}
+
+// the per-member fields of a batch result besides the vectors; the timings and kernel_launches are the batch's
+static void batch_result(b200pdlp_result* out, const BatchRun& b, const PdhgState* h, const BatchLoop& L, double setup_seconds) {
+  fill_result(out, b.f, h, b.term, b.term_iterate, b.restarts, b.chk);
+  out->kernel_launches = (int)std::min<long long>(L.rounds, 2147483647LL);
+  out->setup_seconds = setup_seconds;
+  out->solve_seconds = L.solve_seconds;
+  out->loop_device_ms = L.loop_ms;
+  out->iter_device_ms = L.iter_ms;
+}
+
 static void solve_batch(int count, const b200pdlp_lp* lps, const b200pdlp_params& prm, const b200pdlp_warm* warms,
                         b200pdlp_result* outs) {
   using clk = std::chrono::steady_clock;
@@ -2664,6 +2812,8 @@ static void solve_batch(int count, const b200pdlp_lp* lps, const b200pdlp_params
       host_start_point(b.f, warms ? &warms[i] : nullptr, b.x0, b.y0);
       b.tol_p = prm.tol_primal * (1.0 + b.f.norm_rhs);
       b.tol_d = prm.tol_dual * (1.0 + b.f.norm_cost);
+      for (int j = 0; j < b.f.n; j++) b.cost_sq += b.f.cost[j] * b.f.cost[j];
+      for (int r = 0; r < b.f.m; r++) b.rhs_sq += b.f.rhs[r] * b.f.rhs[r];
     });
   }
   lap("batch", "prologue (host threads)");
@@ -2708,50 +2858,16 @@ static void solve_batch(int count, const b200pdlp_lp* lps, const b200pdlp_params
   DevBuf<int> dcol;
   DevBuf<int4> dsl;
   DevBuf<BatchMember> dmem;
-  DevBuf<PdhgState> dst;
-  DevBuf<BatchCtl> dctl;
   dvec.alloc(hvec.size(), false); dval.alloc(hval.size(), false); dcol.alloc(hcol.size(), false); dsl.alloc(hsl.size(), false);
-  dmem.alloc(count, false); dst.alloc(count, false); dctl.alloc(count, false);
+  dmem.alloc(count, false);
   std::vector<BatchMember> hmem((size_t)count);
   for (int i = 0; i < count; i++) {
     const BatchHost& b = B[i];
-    const int n = b.f.n, m = b.f.m;
-    double* v = dvec.p + b.vec;
-    double* w = v + 12 * n;
     BatchMember& M = hmem[i];
-    M.n = n; M.m = m; M.neq = b.L.neq_local;
+    batch_member_vectors(M, dvec.p + b.vec, b.f.n, b.f.m);
+    M.neq = b.L.neq_local;
     M.a_slices = dsl.p + b.sl_a; M.a_col = dcol.p + b.e_a; M.a_val = dval.p + b.e_a;
     M.at_slices = dsl.p + b.sl_at; M.at_col = dcol.p + b.e_at; M.at_val = dval.p + b.e_at;
-    M.cost = v; M.lower = v + n; M.upper = v + 2 * n; M.colscale = v + 3 * n;
-    M.x0 = v + 4 * n; M.x1 = v + 5 * n; M.aty0 = v + 6 * n; M.aty1 = v + 7 * n;
-    M.xsum = v + 8 * n; M.xavg = v + 9 * n; M.atyavg = v + 10 * n; M.xlr = v + 11 * n;
-    M.rhs = w; M.rowscale = w + m;
-    M.y0 = w + 2 * m; M.y1 = w + 3 * m; M.ax0 = w + 4 * m; M.ax1 = w + 5 * m;
-    M.ysum = w + 6 * m; M.yavg = w + 7 * m; M.axavg = w + 8 * m; M.ylr = w + 9 * m;
-  }
-  // ---- initial states: PDHG_Init_Step_Sizes (cupdlp_step.c:312-375); a fixed step takes tau, sigma after round 0's power method
-  PinnedArray<PdhgState> hst((size_t)count);
-  PinnedArray<BatchCtl> hctl((size_t)count);
-  for (int i = 0; i < count; i++) {
-    const StdForm& f = B[i].f;
-    PdhgState* h = hst.p + i;
-    memset(h, 0, sizeof(PdhgState));
-    h->adaptive = prm.adaptive_step != 0;
-    double a = 0.0, b = 0.0;
-    for (int j = 0; j < f.n; j++) a += f.cost[j] * f.cost[j];
-    for (int r = 0; r < f.m; r++) b += f.rhs[r] * f.rhs[r];
-    h->beta = std::fmin(a, b) > 1e-6 ? a / b : 1.0;
-    if (h->adaptive) {
-      h->tau = (1.0 / f.amax) / std::sqrt(h->beta);
-      h->sigma = h->tau * h->beta;
-    }
-    arm_step(h);
-    fill_pow_tables(h);
-    h->stop_iter = 0;   // the first check is due at once (iteration 0)
-    BatchCtl& c = hctl.p[i];
-    memset(&c, 0, sizeof(BatchCtl));
-    c.active = 1; c.first = 1; c.fixed_step = !h->adaptive; c.no_check = prm.iter_limit <= 0;
-    outs[i].trace_len = 0;
   }
   CUDA_OK(cudaMemcpyAsync(dvec.p, hvec.data(), hvec.size() * sizeof(double), cudaMemcpyHostToDevice, s));
   CUDA_OK(cudaMemcpyAsync(dval.p, hval.data(), hval.size() * sizeof(double), cudaMemcpyHostToDevice, s));
@@ -2761,91 +2877,17 @@ static void solve_batch(int count, const b200pdlp_lp* lps, const b200pdlp_params
   CUDA_OK(cudaStreamSynchronize(s));
   lap("batch", "pools + upload");
 
-  // ---- rounds
-  const int interval = prm.check_interval > 0 ? prm.check_interval : 40;
-  const double t_lim = (prm.time_limit >= 0 && std::isfinite(prm.time_limit)) ? prm.time_limit : -1.0;   // < 0: none
-  CudaEvent evl0, evl1, ev0, ev1;
-  double iter_ms = 0.0;
-  long long rounds = 0;
-  int active = count;
-  CUDA_OK(cudaEventRecord(evl0, s));
-  const auto t_loop = clk::now();
-  while (active > 0) {
-    NvtxRange nvtx("b200pdlp: batch round");
-    const bool timed_out = t_lim >= 0 && std::chrono::duration<double>(clk::now() - t_loop).count() > t_lim;
-    CUDA_OK(cudaMemcpyAsync(dctl.p, hctl.p, (size_t)count * sizeof(BatchCtl), cudaMemcpyHostToDevice, s));
-    CUDA_OK(cudaMemcpyAsync(dst.p, hst.p, (size_t)count * sizeof(PdhgState), cudaMemcpyHostToDevice, s));
-    CUDA_OK(cudaEventRecord(ev0, s));
-    launch_batch_round(s, count, dmem.p, dst.p, dctl.p);
-    CUDA_OK(cudaEventRecord(ev1, s));
-    CUDA_OK(cudaMemcpyAsync(hctl.p, dctl.p, (size_t)count * sizeof(BatchCtl), cudaMemcpyDeviceToHost, s));
-    // the scalars of every state (the power tables are the host's own)
-    CUDA_OK(cudaMemcpy2DAsync(hst.p, sizeof(PdhgState), dst.p, sizeof(PdhgState), offsetof(PdhgState, pow_red), count,
-                              cudaMemcpyDeviceToHost, s));
-    CUDA_OK(cudaStreamSynchronize(s));
-    float ms = 0.f;
-    CUDA_OK(cudaEventElapsedTime(&ms, ev0, ev1));
-    iter_ms += ms;
-    const bool first = rounds == 0;
-    rounds++;
-    for (int i = 0; i < count; i++) {
-      BatchCtl& c = hctl.p[i];
-      if (!c.active) continue;
-      BatchHost& b = B[i];
-      PdhgState* h = hst.p + i;
-      b200pdlp_result* out = outs + i;
-      if (!c.checked) {
-        if (first && c.no_check) { c.active = 0; active--; continue; }   // iter_limit <= 0: no check at all
-        fill_pow_tables(h);   // the tables ran out before the check iteration: refill, the next round goes on
-        continue;
-      }
-      if (first && c.fixed_step) {
-        const double lambda = c.outs[kBatchLambda];
-        h->tau = 0.8 / std::sqrt(lambda);
-        h->sigma = h->tau;
-        h->tau /= std::sqrt(h->beta);
-        h->sigma *= std::sqrt(h->beta);
-        arm_step(h);
-      }
-      CheckResult& chk = b.chk;
-      double dscale[2], pscale[2];
-      assemble_check_a(b.f, c.outs, chk, dscale, pscale);
-      assemble_check_b(b.f, c.outs, chk, dscale, pscale);
-      chk.timed_out = timed_out;
-      b.have_check = true;
-      int choice = 0;
-      const int t_code = check_decision(prm, b.tol_p, b.tol_d, h, chk, b.memo, &b.term_iterate, &choice);
-      if (t_code >= 0) {
-        b.term = t_code;
-        trace_row(out, h, chk, 0);
-        c.active = 0;
-        active--;
-        continue;
-      }
-      if (choice) {
-        restart_steps(h, choice, chk, b.memo, c.outs[choice == 1 ? kBatchDxAvg : kBatchDxCur],
-                      c.outs[choice == 1 ? kBatchDyAvg : kBatchDyCur]);
-        b.restarts++;
-        arm_step(h);
-        c.restart = choice;
-      }
-      trace_row(out, h, chk, choice);
-      h->stop_iter = next_check_iter(h->iter, interval, prm.iter_limit);
-      fill_pow_tables(h);
-    }
-  }
-  CUDA_OK(cudaEventRecord(evl1, s));
-  CUDA_OK(cudaEventSynchronize(evl1));
-  float loop_ms = 0.f;
-  CUDA_OK(cudaEventElapsedTime(&loop_ms, evl0, evl1));
-  const double solve_seconds = std::chrono::duration<double>(clk::now() - t_loop).count();
+  std::vector<BatchRun*> R((size_t)count);
+  for (int i = 0; i < count; i++) R[i] = &B[i];
+  PinnedArray<PdhgState> hst((size_t)count);
+  const BatchLoop loop = batch_rounds(s, count, prm, dmem.p, R, hst.p, outs);
   lap("batch", "rounds");
 
   // ---- PDHG_PostSolve of every member, on the host
   NvtxRange nvtx_post("b200pdlp: batch postsolve + download");
   CUDA_OK(cudaMemcpyAsync(hvec.data(), dvec.p, hvec.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
   CUDA_OK(cudaStreamSynchronize(s));
-  const double setup_seconds = std::chrono::duration<double>(t_loop - t_begin).count();
+  const double setup_seconds = std::chrono::duration<double>(loop.t_loop - t_begin).count();
   for_members(count, [&](int i) {
     BatchHost& b = B[i];
     const StdForm& f = b.f;
@@ -2863,16 +2905,386 @@ static void solve_batch(int count, const b200pdlp_lp* lps, const b200pdlp_params
     for (int r = 0; r < m; r++) { hy[b.L.rperm[r]] = dy[r]; hax[b.L.rperm[r]] = dax[r]; }
     b200pdlp_result* out = outs + i;
     host_postsolve(f, b.have_check, hx, hy, hax, haty, out);
-    fill_result(out, f, h, b.term, b.term_iterate, b.restarts, b.chk);
-    out->kernel_launches = (int)std::min<long long>(rounds, 2147483647LL);
-    out->setup_seconds = setup_seconds;
-    out->solve_seconds = solve_seconds;
-    out->loop_device_ms = loop_ms;
-    out->iter_device_ms = iter_ms;
+    batch_result(out, b, h, loop, setup_seconds);
   });
   lap("batch", "postsolve (host threads)");
 }
 
+// ------------------------------------------------------------------------------ batch of small LPs already on the GPU
+// b200pdlp_solve_batch_device: every array of every member is device memory.  The prologue and the postsolve run on the
+// device, one CTA per member (batch_prep.cu); the rounds are solve_batch's (batch_rounds).  The host reads one sizing record
+// and one scalar record per member, never an array, and the members return solve_batch's bits.
+
+// the checks of a member that read no array (the device checks the arrays: batch_size_kernel)
+static void check_batch_device_member(const b200pdlp_lp* lp, const b200pdlp_params& prm, int i) {
+  const int rc = guarded([&] {
+    if (!lp_fields_ok(lp)) throw Error(B200PDLP_ERR_ARG, "b200pdlp: malformed b200pdlp_lp");
+    if (lp->sense != 1.0 && lp->sense != -1.0) throw Error(B200PDLP_ERR_ARG, "b200pdlp: sense must be +1 or -1");
+    if (prm.ordered_max < 0) throw Error(B200PDLP_ERR_ARG, "ordered_max < 0: a batch solves ordered-mode problems only");
+  });
+  if (rc != B200PDLP_OK) throw Error(rc, "b200pdlp_solve_batch_device: member " + std::to_string(i) + ": " + g_last_error);
+}
+
+// ptr (NULL: not given) must be device or managed memory of `device`
+static void check_device_array(const void* ptr, int device, int i, const char* field) {
+  if (!ptr) return;
+  cudaPointerAttributes a{};
+  const cudaError_t e = cudaPointerGetAttributes(&a, ptr);
+  if (e != cudaSuccess) cudaGetLastError();
+  if (e != cudaSuccess || !((a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == device))
+    throw Error(B200PDLP_ERR_ARG, "b200pdlp_solve_batch_device: member " + std::to_string(i) + ": " + field +
+                                      " is not device memory of device " + std::to_string(device));
+}
+
+// A device-resident batch after its prologue: the descriptors (pool pointers set), the sizing and scalar records, the pools
+struct DeviceBatch {
+  std::vector<BatchPrep> hp;
+  std::vector<BatchSize> size;
+  std::vector<double> rec;   // [count][kPrepRec]
+  DevBuf<BatchPrep> prep;
+  DevBuf<BatchSize> dsize;
+  DevBuf<double> drec;
+  DevBuf<int> rows;          // the sizing's row maps and row lengths: 4 m + 1 per member
+  DevBuf<int> ints, col;     // the form's index arrays: 3 nnz + n + m + 1 per member; the layouts' column ids
+  DevBuf<double> dbls, vec, val;   // the form's values and the scaling factors: nnz + 2 n + m; batch_vec_len; the layouts' values
+  DevBuf<int4> slices;
+};
+
+static const char* prep_error_text(int err) {
+  switch (err) {
+    case kPrepStart0: return "b200pdlp: a_start[0] must be 0 and a_start[num_col] >= 0";
+    case kPrepDecreasing: return "b200pdlp: a_start must be non-decreasing";
+    case kPrepIndex: return "b200pdlp: a_index entry outside [0, num_row)";
+    default: return "b200pdlp: malformed b200pdlp_lp";
+  }
+}
+
+// Validation and sizing (one read-back of `count` records), the pools, then the prologue (one read-back of the scalar
+// records), on stream s of the current device.  lps[i] / warms[i]: host structs whose arrays are device memory.
+static void device_batch_prologue(cudaStream_t s, int count, const b200pdlp_lp* lps, const b200pdlp_warm* warms, int scaling,
+                                  int ordered_max, const char* who, DeviceBatch& D, Laps& lap) {
+  const int omax = ordered_max == 0 ? 4096 : ordered_max;
+  D.hp.assign((size_t)count, BatchPrep{});
+  size_t nrows = 0;
+  for (int i = 0; i < count; i++) nrows += 4 * (size_t)lps[i].num_row + 1;
+  D.rows.alloc(nrows, false);
+  nrows = 0;
+  for (int i = 0; i < count; i++) {
+    const b200pdlp_lp& lp = lps[i];
+    BatchPrep& P = D.hp[i];
+    const int m = lp.num_row;
+    P.n0 = lp.num_col; P.m = m; P.sense = lp.sense;
+    P.a_start = lp.a_start; P.a_index = lp.a_index; P.a_value = lp.a_value;
+    P.col_cost = lp.col_cost; P.col_lower = lp.col_lower; P.col_upper = lp.col_upper;
+    P.row_lower = lp.row_lower; P.row_upper = lp.row_upper;
+    if (warms && warms[i].col_value && warms[i].row_value && warms[i].row_dual) {
+      P.warm_x = warms[i].col_value; P.warm_rv = warms[i].row_value; P.warm_rd = warms[i].row_dual;
+    }
+    int* q = D.rows.p + nrows;
+    P.row_class = q; P.row_new_idx = q + m; P.slack = q + 2 * m; P.rptr = q + 3 * m;
+    nrows += 4 * (size_t)m + 1;
+  }
+  D.prep.alloc(count, false); D.dsize.alloc(count, false); D.drec.alloc((size_t)count * kPrepRec, false);
+  CUDA_OK(cudaMemcpyAsync(D.prep.p, D.hp.data(), (size_t)count * sizeof(BatchPrep), cudaMemcpyHostToDevice, s));
+  launch_batch_size(s, count, D.prep.p, D.dsize.p);
+  CUDA_OK(cudaGetLastError());
+  D.size.resize((size_t)count);
+  CUDA_OK(cudaMemcpyAsync(D.size.data(), D.dsize.p, (size_t)count * sizeof(BatchSize), cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaStreamSynchronize(s));
+  for (int i = 0; i < count; i++) {   // the lowest failing member
+    const BatchSize& z = D.size[i];
+    const std::string at = std::string(who) + ": member " + std::to_string(i) + ": ";
+    if (z.err != kPrepOk) throw Error(B200PDLP_ERR_ARG, at + prep_error_text(z.err));
+    if (std::max(z.n, lps[i].num_row) > omax)
+      throw Error(B200PDLP_ERR_ARG, at + "standard form " + std::to_string(lps[i].num_row) + " x " + std::to_string(z.n) +
+                                        " exceeds ordered_max = " + std::to_string(omax));
+    if (z.pad_a >= 2000000000 || z.pad_at >= 2000000000)
+      throw Error(B200PDLP_ERR_ARG, at + "b200pdlp: matrix too large for 32-bit slice offsets");
+  }
+  lap("batch device", "validation + sizing");
+
+  // ---- the pools: each member's slices of them
+  size_t ni = 0, nd = 0, nv = 0, nsl = 0, ne = 0;
+  for (int i = 0; i < count; i++) {
+    const BatchSize& z = D.size[i];
+    const size_t n = z.n, m = lps[i].num_row, nnz = z.nnz;
+    ni += 3 * nnz + n + m + 1;
+    nd += nnz + 2 * n + m;
+    nv += batch_vec_len(z.n, lps[i].num_row);
+    nsl += (m + 31) / 32 + (n + 31) / 32;
+    ne += (size_t)z.pad_a + 32 + (size_t)z.pad_at + 32;
+  }
+  D.ints.alloc(ni, false); D.dbls.alloc(nd, false); D.vec.alloc(nv, false); D.slices.alloc(nsl, false);
+  D.col.alloc(ne, false); D.val.alloc(ne, false);
+  CUDA_OK(cudaMemsetAsync(D.vec.p, 0, std::max<size_t>(nv, 1) * sizeof(double), s));   // the iterates' other halves, sums
+  ni = nd = nv = nsl = ne = 0;
+  for (int i = 0; i < count; i++) {
+    const BatchSize& z = D.size[i];
+    BatchPrep& P = D.hp[i];
+    const int n = z.n, m = lps[i].num_row, nnz = z.nnz;
+    P.n = n; P.nnz = nnz; P.neq = z.neq;
+    int* q = D.ints.p + ni;
+    P.cbeg = q; P.cidx = q + n + 1; P.pcol = P.cidx + nnz; P.rpos = P.pcol + nnz; P.rwork = P.rpos + nnz;
+    ni += 3 * (size_t)nnz + n + m + 1;
+    double* d = D.dbls.p + nd;
+    P.cval = d; P.cs = d + nnz; P.cs_next = P.cs + n; P.rs = P.cs_next + n;
+    nd += (size_t)nnz + 2 * (size_t)n + m;
+    P.vec = D.vec.p + nv;
+    nv += batch_vec_len(n, m);
+    P.a_slices = D.slices.p + nsl; nsl += (m + 31) / 32;
+    P.at_slices = D.slices.p + nsl; nsl += (n + 31) / 32;
+    P.a_col = D.col.p + ne; P.a_val = D.val.p + ne; ne += (size_t)z.pad_a + 32;
+    P.at_col = D.col.p + ne; P.at_val = D.val.p + ne; ne += (size_t)z.pad_at + 32;
+    P.rec = D.drec.p + (size_t)kPrepRec * i;
+  }
+  CUDA_OK(cudaMemcpyAsync(D.prep.p, D.hp.data(), (size_t)count * sizeof(BatchPrep), cudaMemcpyHostToDevice, s));
+  launch_batch_prep(s, count, D.prep.p, scaling != 0);
+  CUDA_OK(cudaGetLastError());
+  D.rec.resize((size_t)count * kPrepRec);
+  CUDA_OK(cudaMemcpyAsync(D.rec.data(), D.drec.p, D.rec.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaStreamSynchronize(s));
+  lap("batch device", "prologue (device)");
+}
+
+static void solve_batch_device(int count, const b200pdlp_lp* lps, const b200pdlp_params& prm, const b200pdlp_warm* warms,
+                               b200pdlp_result* outs) {
+  using clk = std::chrono::steady_clock;
+  const auto t_begin = clk::now();
+  Laps lap;
+  device_count_checked();
+  if (prm.device >= 0) CUDA_OK(cudaSetDevice(prm.device));
+  int device = 0;
+  CUDA_OK(cudaGetDevice(&device));
+  for (int i = 0; i < count; i++) {
+    const b200pdlp_lp& lp = lps[i];
+    check_device_array(lp.a_start, device, i, "a_start");
+    check_device_array(lp.a_index, device, i, "a_index");
+    check_device_array(lp.a_value, device, i, "a_value");
+    check_device_array(lp.col_cost, device, i, "col_cost");
+    check_device_array(lp.col_lower, device, i, "col_lower");
+    check_device_array(lp.col_upper, device, i, "col_upper");
+    check_device_array(lp.row_lower, device, i, "row_lower");
+    check_device_array(lp.row_upper, device, i, "row_upper");
+    if (warms) {
+      check_device_array(warms[i].col_value, device, i, "warm col_value");
+      check_device_array(warms[i].row_value, device, i, "warm row_value");
+      check_device_array(warms[i].row_dual, device, i, "warm row_dual");
+    }
+    check_device_array(outs[i].col_value, device, i, "result col_value");
+    check_device_array(outs[i].col_dual, device, i, "result col_dual");
+    check_device_array(outs[i].row_value, device, i, "result row_value");
+    check_device_array(outs[i].row_dual, device, i, "result row_dual");
+  }
+  StreamHolder sh;
+  cudaStream_t s = sh.s;
+  DeviceBatch D;
+  {
+    NvtxRange nvtx("b200pdlp: batch prologue (device)");
+    device_batch_prologue(s, count, lps, warms, prm.scaling, prm.ordered_max, "b200pdlp_solve_batch_device", D, lap);
+  }
+  std::vector<BatchRun> runs((size_t)count);
+  std::vector<BatchRun*> R((size_t)count);
+  std::vector<BatchMember> hmem((size_t)count);
+  for (int i = 0; i < count; i++) {
+    BatchRun& b = runs[i];
+    const BatchPrep& P = D.hp[i];
+    const double* r = D.rec.data() + (size_t)kPrepRec * i;
+    StdForm& f = b.f;
+    f.n = P.n; f.m = P.m; f.nnz = P.nnz; f.neq = P.neq; f.n_orig = P.n0;
+    f.sense = lps[i].sense; f.offset = lps[i].offset;
+    f.norm_cost = std::sqrt(r[0]); f.norm_rhs = std::sqrt(r[1]); f.amax = r[2];
+    b.cost_sq = r[3]; b.rhs_sq = r[4];
+    b.tol_p = prm.tol_primal * (1.0 + f.norm_rhs);
+    b.tol_d = prm.tol_dual * (1.0 + f.norm_cost);
+    R[i] = &b;
+    BatchMember& M = hmem[i];
+    batch_member_vectors(M, P.vec, P.n, P.m);
+    M.neq = P.neq;
+    M.a_slices = P.a_slices; M.a_col = P.a_col; M.a_val = P.a_val;
+    M.at_slices = P.at_slices; M.at_col = P.at_col; M.at_val = P.at_val;
+  }
+  DevBuf<BatchMember> dmem;
+  dmem.alloc(count, false);
+  CUDA_OK(cudaMemcpyAsync(dmem.p, hmem.data(), (size_t)count * sizeof(BatchMember), cudaMemcpyHostToDevice, s));
+  PinnedArray<PdhgState> hst((size_t)count);
+  const BatchLoop loop = batch_rounds(s, count, prm, dmem.p, R, hst.p, outs);
+  lap("batch device", "rounds");
+
+  // ---- PDHG_PostSolve of every member on the device, into the caller's vectors
+  NvtxRange nvtx_post("b200pdlp: batch postsolve (device)");
+  std::vector<BatchPost> hpost((size_t)count);
+  for (int i = 0; i < count; i++) {
+    const BatchRun& b = runs[i];
+    BatchPost& q = hpost[i];
+    q.col_value = outs[i].col_value; q.col_dual = outs[i].col_dual; q.row_value = outs[i].row_value; q.row_dual = outs[i].row_dual;
+    q.sel = (b.term == B200PDLP_OPTIMAL && b.term_iterate == 1) ? 2 : hst.p[i].cur;
+    q.have_check = b.have_check;
+  }
+  DevBuf<BatchPost> dpost;
+  dpost.alloc(count, false);
+  CUDA_OK(cudaMemcpyAsync(dpost.p, hpost.data(), (size_t)count * sizeof(BatchPost), cudaMemcpyHostToDevice, s));
+  launch_batch_post(s, count, D.prep.p, dpost.p);
+  CUDA_OK(cudaGetLastError());
+  CUDA_OK(cudaStreamSynchronize(s));
+  const double setup_seconds = std::chrono::duration<double>(loop.t_loop - t_begin).count();
+  for (int i = 0; i < count; i++) batch_result(outs + i, runs[i], hst.p + i, loop, setup_seconds);
+  lap("batch device", "postsolve (device)");
+}
+
+// ---- b200pdlp_debug_batch_prep_compare: the device prologue and postsolve against their host twins
+static const int kBatchPrepItems = 27;
+
+template <class T>
+static std::vector<T> download_vec(const T* d, size_t count) {
+  std::vector<T> h(count);
+  if (count) CUDA_OK(cudaMemcpy(h.data(), d, count * sizeof(T), cudaMemcpyDeviceToHost));
+  return h;
+}
+// elements of a[0..count) whose bytes differ from b's
+template <class T>
+static double bit_mismatches(const T* a, const T* b, size_t count) {
+  double k = 0;
+  for (size_t i = 0; i < count; i++) k += memcmp(a + i, b + i, sizeof(T)) != 0;
+  return k;
+}
+// a fixed pseudo-random value in [-1, 1) for (member, index)
+static double batch_probe(int i, int k) {
+  unsigned long long h = (0x9E3779B97F4A7C15ull * (unsigned long long)(i + 1)) ^ (0x94D049BB133111EBull * (unsigned long long)(k + 3));
+  h ^= h >> 31; h *= 0xD6E8FEB86659FD93ull; h ^= h >> 32;
+  return (double)(h >> 11) * 0x1p-52 - 1.0;
+}
+
+static void batch_prep_compare(int count, const b200pdlp_lp* lps, int scaling, double* report) {
+  device_count_checked();
+  // the raw LPs, uploaded as they are
+  size_t ni = 0, nd = 0;
+  for (int i = 0; i < count; i++) {
+    const b200pdlp_lp& lp = lps[i];
+    const size_t nnz = lp.a_start[lp.num_col];
+    ni += lp.num_col + 1 + nnz;
+    nd += nnz + 3 * (size_t)lp.num_col + 2 * (size_t)lp.num_row;
+  }
+  DevBuf<int> ri;
+  DevBuf<double> rd;
+  ri.alloc(ni, false); rd.alloc(nd, false);
+  std::vector<b200pdlp_lp> dl(lps, lps + count);
+  ni = nd = 0;
+  for (int i = 0; i < count; i++) {
+    const b200pdlp_lp& lp = lps[i];
+    b200pdlp_lp& d = dl[i];
+    const int n0 = lp.num_col, m = lp.num_row, nnz = lp.a_start[n0];
+    auto up_i = [&](const int* src, size_t len) { int* p = ri.p + ni; if (len) CUDA_OK(cudaMemcpy(p, src, len * sizeof(int), cudaMemcpyHostToDevice)); ni += len; return p; };
+    auto up_d = [&](const double* src, size_t len) { double* p = rd.p + nd; if (len) CUDA_OK(cudaMemcpy(p, src, len * sizeof(double), cudaMemcpyHostToDevice)); nd += len; return p; };
+    d.a_start = up_i(lp.a_start, n0 + 1); d.a_index = up_i(lp.a_index, nnz); d.a_value = up_d(lp.a_value, nnz);
+    d.col_cost = up_d(lp.col_cost, n0); d.col_lower = up_d(lp.col_lower, n0); d.col_upper = up_d(lp.col_upper, n0);
+    d.row_lower = up_d(lp.row_lower, m); d.row_upper = up_d(lp.row_upper, m);
+  }
+  StreamHolder sh;
+  DeviceBatch D;
+  Laps lap;
+  device_batch_prologue(sh.s, count, dl.data(), nullptr, scaling, std::numeric_limits<int>::max(), "b200pdlp_debug_batch_prep_compare",
+                        D, lap);
+  std::vector<StdForm> F((size_t)count);
+  for (int i = 0; i < count; i++) {
+    const BatchPrep& P = D.hp[i];
+    StdForm& f = F[i];
+    HostLayout L;
+    formulate(lps[i], f);
+    scale(f, scaling != 0);
+    build_layout(f, 0, 1, std::numeric_limits<int>::max(), L);
+    std::vector<double> x0, y0;
+    host_start_point(f, nullptr, x0, y0);
+    double* rep = report + (size_t)kBatchPrepItems * i;
+    for (int k = 0; k < kBatchPrepItems; k++) rep[k] = 0.0;
+    rep[0] = (P.n != f.n) + (P.m != f.m) + (P.nnz != f.nnz) + (P.neq != f.neq);
+    if (rep[0] != 0.0) {   // nothing else lines up
+      for (int k = 1; k < kBatchPrepItems; k++) rep[k] = -1.0;
+      continue;
+    }
+    const int n = f.n, m = f.m;
+    const std::vector<double> v = download_vec(P.vec, batch_vec_len(n, m));
+    const double* w = v.data() + 12 * (size_t)n;
+    rep[1] = bit_mismatches(v.data(), f.cost.data(), n);
+    rep[2] = bit_mismatches(v.data() + n, f.lower.data(), n);
+    rep[3] = bit_mismatches(v.data() + 2 * n, f.upper.data(), n);
+    rep[4] = bit_mismatches(w, f.rhs.data(), m);
+    rep[5] = bit_mismatches(v.data() + 3 * n, f.col_scale.data(), n);
+    rep[6] = bit_mismatches(w + m, f.row_scale.data(), m);
+    rep[7] = bit_mismatches(download_vec(P.row_new_idx, m).data(), f.row_new_idx.data(), m);
+    rep[8] = bit_mismatches(download_vec(P.row_class, m).data(), reinterpret_cast<const int*>(f.row_class.data()), m);
+    static_assert(sizeof(RowClass) == sizeof(int), "row classes are ints");
+    auto sell = [&](const SellMatrix& H, const int4* sl, const int* col, const double* val, double* r) {
+      const size_t ns = H.slices.size(), ne = H.col.size();
+      const std::vector<int4> ds = download_vec(sl, ns);
+      r[0] = bit_mismatches(reinterpret_cast<const int4*>(H.slices.data()), ds.data(), ns);
+      if (r[0] != 0.0) { r[1] = r[2] = -1.0; return; }
+      r[1] = bit_mismatches(download_vec(col, ne).data(), H.col.data(), ne);
+      r[2] = bit_mismatches(download_vec(val, ne).data(), H.val.data(), ne);
+    };
+    sell(L.A, P.a_slices, P.a_col, P.a_val, rep + 9);
+    sell(L.AT, P.at_slices, P.at_col, P.at_val, rep + 12);
+    rep[15] = bit_mismatches(v.data() + 4 * n, x0.data(), n);
+    rep[16] = bit_mismatches(w + 2 * m, y0.data(), m);
+    std::vector<double> xsum(n);
+    for (int j = 0; j < n; j++) xsum[j] = proj_zero(f, j);
+    rep[17] = bit_mismatches(v.data() + 8 * n, xsum.data(), n);
+    const double* r = D.rec.data() + (size_t)kPrepRec * i;
+    double cost_sq = 0.0, rhs_sq = 0.0;
+    for (int j = 0; j < n; j++) cost_sq += f.cost[j] * f.cost[j];
+    for (int q = 0; q < m; q++) rhs_sq += f.rhs[q] * f.rhs[q];
+    const double got[5] = {std::sqrt(r[0]), std::sqrt(r[1]), r[2], r[3], r[4]};
+    const double want[5] = {f.norm_cost, f.norm_rhs, f.amax, cost_sq, rhs_sq};
+    for (int k = 0; k < 5; k++) rep[18 + k] = bit_mismatches(got + k, want + k, 1);
+  }
+  // the postsolve of a probe iterate (x, A'y, y, A x in half 0 of every block, a check assumed) into fresh device vectors
+  std::vector<BatchPost> hpost((size_t)count);
+  std::vector<std::vector<double>> probes((size_t)count);
+  size_t nout = 0;
+  for (int i = 0; i < count; i++) nout += 2 * (size_t)D.hp[i].n0 + 2 * (size_t)D.hp[i].m;
+  DevBuf<double> dout;
+  dout.alloc(nout, false);
+  nout = 0;
+  for (int i = 0; i < count; i++) {
+    const BatchPrep& P = D.hp[i];
+    const int n = P.n, m = P.m, n0 = P.n0;
+    std::vector<double>& pr = probes[i];   // x, A'y (n each), y, A x (m each)
+    pr.resize(2 * (size_t)n + 2 * (size_t)m);
+    for (size_t k = 0; k < pr.size(); k++) pr[k] = batch_probe(i, (int)k);
+    double* v = P.vec;
+    double* w = v + 12 * (size_t)n;
+    CUDA_OK(cudaMemcpy(v + 4 * (size_t)n, pr.data(), n * sizeof(double), cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemcpy(v + 6 * (size_t)n, pr.data() + n, n * sizeof(double), cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemcpy(w + 2 * (size_t)m, pr.data() + 2 * n, m * sizeof(double), cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemcpy(w + 4 * (size_t)m, pr.data() + 2 * n + m, m * sizeof(double), cudaMemcpyHostToDevice));
+    double* o = dout.p + nout;
+    hpost[i] = BatchPost{o, o + n0, o + 2 * n0, o + 2 * n0 + m, 0, 1};
+    nout += 2 * (size_t)n0 + 2 * (size_t)m;
+  }
+  DevBuf<BatchPost> dpost;
+  dpost.alloc(count, false);
+  dpost.upload(hpost.data(), count);
+  launch_batch_post(sh.s, count, D.prep.p, dpost.p);
+  CUDA_OK(cudaGetLastError());
+  CUDA_OK(cudaStreamSynchronize(sh.s));
+  for (int i = 0; i < count; i++) {
+    double* rep = report + (size_t)kBatchPrepItems * i;
+    if (rep[0] != 0.0) continue;
+    const StdForm& f = F[i];
+    const int n = f.n, m = f.m, n0 = f.n_orig;
+    const std::vector<double>& pr = probes[i];
+    std::vector<double> hx(pr.begin(), pr.begin() + n), haty(pr.begin() + n, pr.begin() + 2 * n);
+    std::vector<double> hy(pr.begin() + 2 * n, pr.begin() + 2 * n + m), hax(pr.begin() + 2 * n + m, pr.end());
+    std::vector<double> cv(n0), cd(n0), rv(m), rdual(m);
+    b200pdlp_result res{};
+    res.col_value = cv.data(); res.col_dual = cd.data(); res.row_value = rv.data(); res.row_dual = rdual.data();
+    host_postsolve(f, true, hx, hy, hax, haty, &res);
+    const BatchPost& q = hpost[i];
+    rep[23] = bit_mismatches(download_vec(q.col_value, n0).data(), cv.data(), n0);
+    rep[24] = bit_mismatches(download_vec(q.col_dual, n0).data(), cd.data(), n0);
+    rep[25] = bit_mismatches(download_vec(q.row_value, m).data(), rv.data(), m);
+    rep[26] = bit_mismatches(download_vec(q.row_dual, m).data(), rdual.data(), m);
+  }
+}
 
 // ----------------------------------------------------------------------------------- batch of small LPs, HiPDLP mode
 // b200pdlp_solve_hipdlp_batch: every member is an ordered-mode HiPDLP problem, solved by one CTA of hip_batch_round_kernel
@@ -3511,6 +3923,29 @@ int b200pdlp_solve_batch(int32_t count, const b200pdlp_lp* lps, const b200pdlp_p
     for (int i = 0; i < count; i++) check_batch_member(&lps[i], *params, i);
     solve_batch(count, lps, *params, warms, outs);
     CUDA_OK(cudaGetLastError());
+  });
+}
+
+int b200pdlp_solve_batch_device(int32_t count, const b200pdlp_lp* lps, const b200pdlp_params* params, const b200pdlp_warm* warms,
+                                b200pdlp_result* outs) {
+  DeviceGuard dg;
+  return guarded([&] {
+    if (count < 0) throw Error(B200PDLP_ERR_ARG, "b200pdlp_solve_batch_device: count < 0");
+    if (count == 0) return;
+    if (!lps || !params || !outs) throw Error(B200PDLP_ERR_ARG, "b200pdlp_solve_batch_device: null argument");
+    check_params(*params);
+    for (int i = 0; i < count; i++) check_batch_device_member(&lps[i], *params, i);
+    solve_batch_device(count, lps, *params, warms, outs);
+    CUDA_OK(cudaGetLastError());
+  });
+}
+
+int b200pdlp_debug_batch_prep_compare(int32_t count, const b200pdlp_lp* lps, int32_t scaling, double* report) {
+  DeviceGuard dg;
+  return guarded([&] {
+    if (count < 0 || (count > 0 && (!lps || !report))) throw Error(B200PDLP_ERR_ARG, "b200pdlp_debug_batch_prep_compare: bad arguments");
+    for (int i = 0; i < count; i++) check_lp(&lps[i]);
+    if (count > 0) batch_prep_compare(count, lps, scaling, report);
   });
 }
 

@@ -79,7 +79,7 @@ ABI_SYMBOLS = [
     "b200pdlp_debug_prep_compare_hipdlp", "b200pdlp_debug_hipdlp_shard_prep_compare", "b200pdlp_release_cache",
     "b200pdlp_host_register", "b200pdlp_host_unregister", "b200pdlp_primal_step", "b200pdlp_dual_step", "b200pdlp_residuals",
     "b200pdlp_kkt_check", "b200pdlp_kkt_check_host", "b200pdlp_kkt_default_tolerances", "b200pdlp_solve_batch",
-    "b200pdlp_solve_hipdlp_batch",
+    "b200pdlp_solve_hipdlp_batch", "b200pdlp_solve_batch_device", "b200pdlp_debug_batch_prep_compare",
 ]
 
 _lib = None
@@ -255,6 +255,104 @@ def solve_batch(lps, warms=None, trace_cap: int = 0, **params) -> list:
     prm = make_params(**params)
     _check(L.b200pdlp_solve_batch(count, clps, C.byref(prm), cwarm, cres), "b200pdlp_solve_batch")
     return [_result_dict(cres[i], arrays[i]) for i in range(count)]
+
+
+_LP_INDEX_ARRAYS = ("a_start", "a_index")
+_LP_VALUE_ARRAYS = ("a_value", "col_cost", "col_lower", "col_upper", "row_lower", "row_upper")
+
+
+def lp_to_device(lp: HighsLp, device: int = 0) -> dict:
+    """The arrays of `lp` as torch CUDA tensors on `device` (int32 indices, float64 values), with num_col, num_row, sense and
+    offset: one member of solve_batch_device."""
+    import torch
+    dev = torch.device("cuda", device)
+    arrs = dict(zip(_LP_INDEX_ARRAYS + _LP_VALUE_ARRAYS, lp_arrays(lp)))
+    out = {k: torch.as_tensor(np.ascontiguousarray(v, dtype=np.int32 if k in _LP_INDEX_ARRAYS else np.float64)).to(dev)
+           for k, v in arrs.items()}
+    out.update(num_col=int(lp.num_col_), num_row=int(lp.num_row_), sense=float(lp.sense_), offset=float(lp.offset_))
+    return out
+
+
+def _dev_ptr(t, dtype, ptype, what):
+    """the device address of a contiguous CUDA tensor of `dtype` (NULL when empty)"""
+    if t is None:
+        return None
+    if not (t.is_cuda and t.dtype == dtype and t.is_contiguous()):
+        raise TypeError(f"{what} must be a contiguous CUDA tensor of {dtype}")
+    return C.cast(C.c_void_p(t.data_ptr() if t.numel() else 0), ptype)
+
+
+def make_clp_device(d: dict) -> CLp:
+    """the b200pdlp_lp of an lp_to_device dict: every array pointer is device memory"""
+    import torch
+    ptrs = [_dev_ptr(d[k], torch.int32, _ip, k) for k in _LP_INDEX_ARRAYS] + \
+           [_dev_ptr(d[k], torch.float64, _dp, k) for k in _LP_VALUE_ARRAYS]
+    return CLp(d["num_col"], d["num_row"], *ptrs, float(d["sense"]), float(d["offset"]))
+
+
+def solve_batch_device(dlps, warms=None, trace_cap: int = 0, **params) -> list:
+    """b200pdlp_solve_batch_device: solve_batch for LPs already in GPU memory (dicts of lp_to_device), prologue and postsolve
+    on the device.  warms: None, or one entry per LP -- None or (col_value, row_value, row_dual) as float64 CUDA tensors.
+    Returns the dicts solve_batch returns, with the four vectors as float64 CUDA tensors; each member's bits are those
+    solve_batch returns for it.  `device` defaults to the device of the first LP's tensors.  torch's current stream is
+    synchronised first, so that inputs it is still writing are complete."""
+    dlps = list(dlps)
+    if warms is not None:
+        warms = list(warms)
+        if len(warms) != len(dlps):
+            raise ValueError(f"solve_batch_device: {len(warms)} warm starts for {len(dlps)} LPs")
+    L = lib()
+    L.b200pdlp_solve_batch_device.argtypes = [C.c_int32, C.POINTER(CLp), C.POINTER(CParams), C.POINTER(CWarm), C.POINTER(CResult)]
+    count = len(dlps)
+    if count == 0:
+        _check(L.b200pdlp_solve_batch_device(0, None, C.byref(make_params(**params)), None, None), "b200pdlp_solve_batch_device")
+        return []
+    import torch
+    dev = dlps[0]["a_start"].device
+    params.setdefault("device", dev.index)
+    prm = make_params(**params)
+    dev = torch.device("cuda", prm.device if prm.device >= 0 else torch.cuda.current_device())
+    clps, cres, arrays = (CLp * count)(), (CResult * count)(), []
+    cwarm = (CWarm * count)() if warms is not None and any(w is not None for w in warms) else None
+    for i, d in enumerate(dlps):
+        clps[i] = make_clp_device(d)
+        vecs = (torch.empty(d["num_col"], dtype=torch.float64, device=dev), torch.empty(d["num_col"], dtype=torch.float64, device=dev),
+                torch.empty(d["num_row"], dtype=torch.float64, device=dev), torch.empty(d["num_row"], dtype=torch.float64, device=dev))
+        res = CResult()
+        res.col_value, res.col_dual, res.row_value, res.row_dual = (_dev_ptr(v, torch.float64, _dp, "result") for v in vecs)
+        if trace_cap > 0:
+            tr = np.zeros((trace_cap, 16))
+            res.trace, res.trace_cap = _p(tr, _dp), trace_cap
+            vecs = vecs + (tr,)
+        cres[i] = res
+        arrays.append(vecs)
+        if cwarm is not None and warms[i] is not None:
+            cwarm[i] = CWarm(*(_dev_ptr(w, torch.float64, _dp, "warm start") for w in warms[i]))
+    torch.cuda.current_stream(dev).synchronize()
+    _check(L.b200pdlp_solve_batch_device(count, clps, C.byref(prm), cwarm, cres), "b200pdlp_solve_batch_device")
+    return [_result_dict(cres[i], arrays[i]) for i in range(count)]
+
+
+BATCH_PREP_ITEMS = ["dims", "cost", "lower", "upper", "rhs", "col_scale", "row_scale", "row_new_idx", "row_class", "A.slices",
+                    "A.col", "A.val", "AT.slices", "AT.col", "AT.val", "x0", "y0", "xsum", "norm_cost", "norm_rhs", "amax",
+                    "beta_cost_sq", "beta_rhs_sq", "col_value", "col_dual", "row_value", "row_dual"]
+
+
+def batch_prep_compare(lps, scaling: int = 1) -> list:
+    """b200pdlp_debug_batch_prep_compare: the device prologue and postsolve of solve_batch_device against their host twins on
+    host LPs; one dict of mismatch counts per LP (BATCH_PREP_ITEMS)."""
+    lps = list(lps)
+    L = lib()
+    L.b200pdlp_debug_batch_prep_compare.argtypes = [C.c_int32, C.POINTER(CLp), C.c_int32, _dp]
+    count = len(lps)
+    clps, keep = (CLp * max(count, 1))(), []
+    for i, lp in enumerate(lps):
+        clps[i], k = make_clp(lp)
+        keep.append(k)
+    k = len(BATCH_PREP_ITEMS)
+    rep = np.zeros(max(count, 1) * k)
+    _check(L.b200pdlp_debug_batch_prep_compare(count, clps, scaling, _p(rep, _dp)), "b200pdlp_debug_batch_prep_compare")
+    return [dict(zip(BATCH_PREP_ITEMS, rep[k * i:k * (i + 1)].tolist())) for i in range(count)]
 
 
 PREP_ITEMS = ["n", "m", "nnz", "neq", "cbeg", "cidx", "cval", "cost", "lower", "upper", "col_scale", "rhs", "row_scale", "rptr",

@@ -151,6 +151,29 @@ int b200pdlp_solve_batch(int32_t count, const b200pdlp_lp* lps, const b200pdlp_p
                          const b200pdlp_warm* warms /* [count] or NULL; a member whose pointers are NULL starts cold */,
                          b200pdlp_result* outs /* [count], caller-allocated like b200pdlp_result */);
 
+/* b200pdlp_solve_batch for LPs that are already in GPU memory.  `lps`, `warms` and `outs` are host arrays of the usual
+ * structs, but every array pointer inside them is device (or managed) memory of params->device (< 0: the current device):
+ * the LP's eight arrays, the three warm vectors and the four result vectors.  num_col, num_row, sense and offset are host
+ * scalars; `trace` stays a host pointer.  Each member returns exactly what b200pdlp_solve_batch returns for it with the same
+ * arrays on the host (and so what b200pdlp_solve returns for it alone): term_code, term_iterate, iters, passes, restarts, the
+ * residual scalars, the trace rows, the form dimensions and the four vectors, bit for bit.  Batch-wide fields as in
+ * b200pdlp_solve_batch; setup_seconds covers validation, sizing and the device prologue.
+ * The prologue (formulate, scaling, layouts, start point) and the postsolve run on the device, one CTA per member; the host
+ * reads a few scalars per member, never an array.  The call returns once the outputs are complete on the device; it never
+ * writes an input array.  The caller must have finished writing the inputs before the call (the library uses a stream of
+ * its own).
+ * Returns B200PDLP_ERR_ARG before any device work for count < 0, NULL arrays, ordered_max < 0, a bad device_scaling or a
+ * sense other than +-1; then, naming the member and the field, for a pointer that is not device memory of the device; then,
+ * before any solve work and naming the lowest failing member, for what b200pdlp_solve's checks reject in the arrays
+ * (a_start[0] != 0, a decreasing a_start, an a_index outside [0, num_row)) and for a standard form larger than ordered_max.
+ * No result field or array is written on an error.  count == 0: B200PDLP_OK.  No device: B200PDLP_ERR_CUDA.  The whole batch
+ * must fit in device memory (B200PDLP_ERR_ALLOC otherwise).
+ * STATUS: runs on hardware; tests/test_gpu_batch_device.py (byte equality with b200pdlp_solve_batch),
+ * tools/batch_device_bench.py. */
+int b200pdlp_solve_batch_device(int32_t count, const b200pdlp_lp* lps, const b200pdlp_params* params,
+                                const b200pdlp_warm* warms /* [count] or NULL; device vectors; a member whose pointers are NULL starts cold */,
+                                b200pdlp_result* outs /* [count]; vectors in device memory */);
+
 /* ---- persistent problem handle (bench + kernel-level parity tests) --------- */
 typedef struct b200pdlp_problem b200pdlp_problem;
 
@@ -346,6 +369,14 @@ int b200pdlp_debug_prep_compare(const b200pdlp_lp* lp, int32_t scaling, double r
  *  34 row pointer of the row-major copy of the caller's matrix  35 its column ids + values (a row's entries in column order)
  *  36 1 if the device and the host disagree on whether any scaling pass ran   37-39 unused (0) */
 int b200pdlp_debug_prep_compare_hipdlp(const b200pdlp_lp* lp, int32_t scaling_mode, int32_t ruiz_iterations, double report[40]);
+/* The device prologue and postsolve of b200pdlp_solve_batch_device (highs_b200/csrc/batch_prep.cu) against their host twins:
+ * the `count` host LPs are uploaded as they are, prepared on the device (cold start, no ordered_max limit) and compared with
+ * formulate + scale + build_layout + host_start_point; then a fixed pseudo-random iterate is postsolved on both sides.
+ * report[27 * i + k] = mismatching entries (bit for bit) of member i:  0 n, m, nnz, neq (-1 everywhere else if they differ)
+ *  1 cost 2 lower 3 upper 4 rhs 5 col_scale 6 row_scale  7 row_new_idx 8 row_class  9-11 A: slice descriptors (-1 for the
+ *  rest if they differ), col, val  12-14 the same for A'  15 x0 16 y0 17 xsum  18 |c|_2 19 |b|_2 20 max|a_ij|  21, 22 the
+ *  scaled |c|^2, |b|^2 that set beta  23 col_value 24 col_dual 25 row_value 26 row_dual */
+int b200pdlp_debug_batch_prep_compare(int32_t count, const b200pdlp_lp* lps, int32_t scaling, double* report);
 /* The device prologue of b200pdlp_solve_hipdlp_multi (block mode, all `world` ranks on the current device, 2 <= world <= 16)
  * against formulate_hipdlp + scale_hipdlp + plan_hipdlp_shards (ordered_max = -1) + build_hipdlp_shard.  report[8 + 9 world]
  * = mismatch counts:  0 n, m, nnz, neq (nothing else is compared if they differ)  1 vectors in device order (cost, lower,
