@@ -6,6 +6,11 @@
 //   batch_prep_kernel   formulate, the row-major index, scale, the sliced-ELL bodies of A and A', host_start_point, xSum = proj(0)
 //                       and the sums that set the tolerances and beta
 //   batch_post_kernel   host_postsolve of the returned iterate, into the caller's device vectors
+// and their HiPDLP twins for b200pdlp_solve_hipdlp_batch_device (engine.cu solve_hipdlp_batch_device):
+//   hip_batch_size_kernel   the same checks and sizes under formulate_hipdlp's row classes
+//   hip_batch_prep_kernel   formulate_hipdlp, the row-major indexes of the form and of the caller's matrix, scale_hipdlp, the
+//                           sliced-ELL bodies of A and A', |c|^2 and |b|^2 of the unscaled form
+//   hip_batch_post_kernel   hip_host_postsolve of the returned iterate, into the caller's device vectors
 //
 // Bits: every value is the host prologue's (host_prep.cpp formulate / build_row_index / scale / build_layout, engine.cu
 // host_start_point / host_postsolve) with the same operations on the same operands: the build compiles this file with
@@ -443,7 +448,400 @@ __global__ void __launch_bounds__(kThreads) batch_post_kernel(const BatchPrep* _
   }
 }
 
+// ===================================================================================== HiPDLP batch
+// the row-major index by one warp (build_row_index): position p of row[p] goes to slot rwork[row[p]]++, positions ascending.
+// The warp walks the positions in order, 32 at a time; lanes that hit the same row take consecutive slots in lane order.
+// (batch_prep_kernel keeps this walk and form_layouts' two bodies written out in place, so that its machine code stays as
+// it was; the HiPDLP kernel calls them.)
+__device__ __forceinline__ void row_walk(int nnz, const int* row, int* rwork, int* rpos) {
+  const int lane = threadIdx.x & 31;
+  for (int base = 0; base < nnz; base += 32) {
+    const int p = base + lane;
+    const int i = p < nnz ? row[p] : -1 - lane;
+    const unsigned same = __match_any_sync(0xffffffffu, i);
+    int q = 0;
+    if (p < nnz) q = rwork[i] + __popc(same & ((1u << lane) - 1u));
+    __syncwarp();
+    if (p < nnz) {
+      rpos[q] = p;
+      if (lane == __ffs(same) - 1) rwork[i] += __popc(same);
+    }
+    __syncwarp();
+  }
+}
+
+// the ordered sliced-ELL bodies of the form (build_layout, identity orderings, no long rows): A's rows in the row-major
+// index's order; A' row j = column j sorted by row, stably (build_col_major)
+__device__ __forceinline__ void form_layouts(const BatchPrep& P, int m, int n, int* sm) {
+  sell_body(m, P.a_slices, P.a_col, P.a_val, sm, [&](int r) { return P.rptr[r + 1] - P.rptr[r]; },
+            [&](int r, int* c, double* v) {
+              const int q0 = P.rptr[r], len = P.rptr[r + 1] - q0;
+              for (int k = 0; k < len; k++) { const int p = P.rpos[q0 + k]; c[32 * k] = P.pcol[p]; v[32 * k] = P.cval[p]; }
+              return len;
+            });
+  __syncthreads();
+  sell_body(n, P.at_slices, P.at_col, P.at_val, sm, [&](int j) { return P.cbeg[j + 1] - P.cbeg[j]; },
+            [&](int j, int* c, double* v) {
+              const int p0 = P.cbeg[j], len = P.cbeg[j + 1] - p0;
+              bool sorted = true;
+              for (int k = 0; k < len; k++) {
+                c[32 * k] = P.cidx[p0 + k]; v[32 * k] = P.cval[p0 + k];
+                if (k > 0 && P.cidx[p0 + k] < P.cidx[p0 + k - 1]) sorted = false;
+              }
+              if (!sorted)   // stable insertion sort by row
+                for (int k = 1; k < len; k++) {
+                  const int ck = c[32 * k];
+                  const double vk = v[32 * k];
+                  int h = k - 1;
+                  for (; h >= 0 && c[32 * h] > ck; h--) { c[32 * (h + 1)] = c[32 * h]; v[32 * (h + 1)] = v[32 * h]; }
+                  c[32 * (h + 1)] = ck; v[32 * (h + 1)] = vk;
+                }
+              return len;
+            });
+}
+
+// The twins of host_prep_hipdlp.cpp formulate_hipdlp / scale_hipdlp, build_layout and engine.cu hip_host_postsolve.
+
+// batch_size_kernel under formulate_hipdlp's classification: +-infinity thresholds (a bound of 1e25 is finite), FREE rows a
+// class of their own, BOUND and FREE rows equality-like, each with a slack column
+__global__ void __launch_bounds__(kThreads) hip_batch_size_kernel(const BatchPrep* __restrict__ prep, BatchSize* __restrict__ sizes) {
+  __shared__ int flag[4];
+  __shared__ int sm_eq[kThreads + 1], sm_bnd[kThreads + 1];
+  __shared__ unsigned long long acc;
+  const BatchPrep& P = prep[blockIdx.x];
+  BatchSize& S = sizes[blockIdx.x];
+  const int t = threadIdx.x, n0 = P.n0, m = P.m;
+  if (t < 4) flag[t] = 0;
+  __syncthreads();
+  // check_lp(deep): a_start[0] == 0, a_start non-decreasing, the matrix arrays present, a_index in [0, num_row)
+  if (t == 0 && P.a_start[0] != 0) flag[0] = kPrepStart0;
+  for (int j = t; j < n0; j += kThreads)
+    if (P.a_start[j + 1] < P.a_start[j]) flag[1] = kPrepDecreasing;
+  __syncthreads();
+  const int nnz0 = P.a_start[n0];
+  if (t == 0 && nnz0 > 0 && (!P.a_index || !P.a_value)) flag[2] = kPrepNull;
+  __syncthreads();
+  const int early = flag[0] ? flag[0] : flag[1] ? flag[1] : flag[2];
+  if (early) {
+    if (t == 0) S.err = early;
+    return;
+  }
+  for (int p = t; p < nnz0; p += kThreads)
+    if ((unsigned)P.a_index[p] >= (unsigned)m) flag[3] = kPrepIndex;
+  __syncthreads();
+  if (flag[3]) {
+    if (t == 0) S.err = kPrepIndex;
+    return;
+  }
+  // formulate_hipdlp's row classes
+  for (int i = t; i < m; i += kThreads) {
+    const double rl = P.row_lower[i], ru = P.row_upper[i];
+    const bool lo = rl > -kInf, up = ru < kInf;
+    int c;
+    if (lo && up) c = (rl == ru) ? kEq : kBound;
+    else if (lo) c = kGeq;
+    else if (up) c = kLeq;
+    else c = kFreeRow;
+    P.row_class[i] = c;
+  }
+  for (int i = t; i <= m; i += kThreads) P.rptr[i] = 0;
+  __syncthreads();
+  // the new row order: equality-like rows (EQ / BOUND / FREE) first, then LEQ / GEQ, each in original order;
+  // slack columns in the order of their rows
+  const int chunk = (m + kThreads - 1) / kThreads;
+  const int b = min(t * chunk, m), e = min(b + chunk, m);
+  int eq = 0, bnd = 0;
+  for (int i = b; i < e; i++) {
+    const int c = P.row_class[i];
+    eq += (c == kEq || c == kBound || c == kFreeRow);
+    bnd += (c == kBound || c == kFreeRow);
+  }
+  sm_eq[t] = eq; sm_bnd[t] = bnd;
+  __syncthreads();
+  if (t == 0) {
+    int re = 0, rb = 0;
+    for (int k = 0; k < kThreads; k++) {
+      const int ve = sm_eq[k], vb = sm_bnd[k];
+      sm_eq[k] = re; sm_bnd[k] = rb;
+      re += ve; rb += vb;
+    }
+    sm_eq[kThreads] = re; sm_bnd[kThreads] = rb;
+  }
+  __syncthreads();
+  const int neq = sm_eq[kThreads], nb = sm_bnd[kThreads];
+  {
+    int head = sm_eq[t], tail = neq + (b - sm_eq[t]), sl = sm_bnd[t];
+    for (int i = b; i < e; i++) {
+      const int c = P.row_class[i];
+      P.row_new_idx[i] = (c == kEq || c == kBound || c == kFreeRow) ? head++ : tail++;
+      P.slack[i] = (c == kBound || c == kFreeRow) ? sl++ : -1;
+    }
+  }
+  __syncthreads();
+  // the standard form's row lengths (integer counts: order-free), a slack row's slack entry included
+  for (int p = t; p < nnz0; p += kThreads) atomicAdd(&P.rptr[P.row_new_idx[P.a_index[p]]], 1);
+  for (int i = t; i < m; i += kThreads)
+    if (P.slack[i] >= 0) atomicAdd(&P.rptr[P.row_new_idx[i]], 1);
+  __syncthreads();
+  const long long pa = padded(m, [&](int r) { return P.rptr[r]; }, &acc);
+  const long long pat = padded(n0 + nb, [&](int j) { return j < n0 ? P.a_start[j + 1] - P.a_start[j] : 1; }, &acc);
+  if (t == 0) {
+    S.err = kPrepOk;
+    S.n = n0 + nb; S.nnz = nnz0 + nb; S.neq = neq;
+    // (ordered_max keeps these far below 2^31; the host checks the dimensions before it trusts them)
+    S.pad_a = (int)min(pa, 2000000000ll); S.pad_at = (int)min(pat, 2000000000ll);
+  }
+}
+
+// a double as a radix key: ascending numeric order, -0.0 before +0.0 (device_prep.cu value_key_kernel's convention)
+__device__ __forceinline__ unsigned long long value_key(double v) {
+  const unsigned long long u = (unsigned long long)__double_as_longlong(v);
+  return (u >> 63) ? ~u : (u | 0x8000000000000000ull);
+}
+
+// The fold of one scaling pass over a column's or a row's terms, and its factor (Scaling::scaleProblem).  OP 0: Ruiz, max |v|
+// -> sqrt, 0 -> 1; 1: Pock-Chambolle with alpha = 1, sum |v| -> sqrt; 2: L2, sum v^2 -> sqrt(sqrt).  The host evaluates the
+// Pock-Chambolle terms and factors as std::pow(x, 1.0), which glibc returns exactly as x, so the identity is used here.
+template <int OP> __device__ __forceinline__ double hip_fold(double a, double v) {
+  if (OP == 0) { const double t = fabs(v); return (a < t) ? t : a; }   // std::max(a, t)
+  return OP == 1 ? a + fabs(v) : a + v * v;
+}
+template <int OP> __device__ __forceinline__ double hip_factor(double a) {
+  if (OP == 0) { const double f = sqrt(a); return f == 0.0 ? 1.0 : f; }
+  return a > 0.0 ? (OP == 1 ? sqrt(a) : sqrt(sqrt(a))) : 1.0;
+}
+
+// one scaling pass (scale_hipdlp's pass + apply_hipdlp): column folds in cbeg order, row folds in row-major order, then
+// every entry divided once by the product rs[i] * cs[j]; only finite bounds, rhs and row upper bounds are scaled
+template <int OP>
+__device__ void hip_scale_pass(const BatchPrep& P, double* cost, double* lower, double* upper, double* colscale, double* rlo,
+                               double* rup, double* rowscale) {
+  const int t = threadIdx.x, n = P.n, m = P.m;
+  for (int j = t; j < n; j += kThreads) {
+    double a = 0.0;
+    for (int p = P.cbeg[j]; p < P.cbeg[j + 1]; p++) a = hip_fold<OP>(a, P.cval[p]);
+    P.cs[j] = hip_factor<OP>(a);
+  }
+  for (int i = t; i < m; i += kThreads) {
+    double a = 0.0;
+    for (int q = P.rptr[i]; q < P.rptr[i + 1]; q++) a = hip_fold<OP>(a, P.cval[P.rpos[q]]);
+    P.rs[i] = hip_factor<OP>(a);
+  }
+  __syncthreads();
+  for (int j = t; j < n; j += kThreads) {
+    const double c = P.cs[j];
+    cost[j] /= c;
+    if (lower[j] > -kInf) lower[j] *= c;
+    if (upper[j] < kInf) upper[j] *= c;
+    colscale[j] *= c;
+    for (int p = P.cbeg[j]; p < P.cbeg[j + 1]; p++) P.cval[p] /= (P.rs[P.cidx[p]] * c);
+  }
+  for (int i = t; i < m; i += kThreads) {
+    const double r = P.rs[i];
+    if (rlo[i] > -kInf) rlo[i] /= r;
+    if (rup[i] < kInf) rup[i] /= r;
+    rowscale[i] *= r;
+  }
+  __syncthreads();
+}
+
+__global__ void __launch_bounds__(kThreads)
+hip_batch_prep_kernel(const BatchPrep* __restrict__ prep, const HipBatchPrep* __restrict__ hprep, int scaling_mode,
+                      int ruiz_iterations) {
+  __shared__ int sm[kThreads + 1];
+  __shared__ int s_row[kThreads];
+  __shared__ unsigned long long s_key[kThreads];
+  __shared__ int nsort;
+  const BatchPrep& P = prep[blockIdx.x];
+  const HipBatchPrep& H = hprep[blockIdx.x];
+  const int t = threadIdx.x, wid = t >> 5;
+  const int n0 = P.n0, m = P.m, n = P.n, nnz = P.nnz;
+  const int nnz0 = nnz - (n - n0);
+  double* cost = P.vec;   // the member's block (hip_batch_vec_len): cost, lower, upper, colscale ... rlo, rup, rowscale ...
+  double* lower = cost + n;
+  double* upper = cost + 2 * n;
+  double* colscale = cost + 3 * n;
+  double* rlo = cost + 14 * n;
+  double* rup = rlo + m;
+  double* rowscale = rlo + 2 * m;
+  const int* rni = P.row_new_idx;
+  const int* rcl = P.row_class;
+  if (t == 0) nsort = 0;
+  __syncthreads();
+
+  // ---- formulate_hipdlp.  A structural column keeps cbeg[j] = a_start[j], its entries ordered by (new row, value) with LEQ
+  // rows negated.  Stored rows strictly ascending: the new rows ascend inside the equality-like group and inside the rest, so
+  // that order is the stable partition.  Other columns go on the work list for the sort below.  Costs keep their sign and
+  // bounds are not clamped.
+  for (int j = t; j < n0; j += kThreads) {
+    const int p0 = P.a_start[j], p1 = P.a_start[j + 1];
+    P.cbeg[j] = p0;
+    bool ascending = true;
+    for (int p = p0 + 1; p < p1; p++)
+      if (P.a_index[p] <= P.a_index[p - 1]) ascending = false;
+    if (ascending) {
+      int k = p0;
+      for (int p = p0; p < p1; p++) {
+        const int i = P.a_index[p];
+        if (rni[i] < P.neq) { P.cidx[k] = rni[i]; P.cval[k] = rcl[i] == kLeq ? -P.a_value[p] : P.a_value[p]; P.pcol[k] = j; k++; }
+      }
+      for (int p = p0; p < p1; p++) {
+        const int i = P.a_index[p];
+        if (rni[i] >= P.neq) { P.cidx[k] = rni[i]; P.cval[k] = rcl[i] == kLeq ? -P.a_value[p] : P.a_value[p]; P.pcol[k] = j; k++; }
+      }
+    } else {
+      H.sortcols[atomicAdd(&nsort, 1)] = j;
+    }
+    cost[j] = P.col_cost[j];
+    lower[j] = P.col_lower[j];
+    upper[j] = P.col_upper[j];
+    colscale[j] = 1.0;
+  }
+  for (int i = t; i < m; i += kThreads) {
+    const int r = rni[i], c = rcl[i];
+    rlo[r] = (c == kEq || c == kGeq) ? P.row_lower[i] : c == kLeq ? -P.row_upper[i] : 0.0;
+    rup[r] = c == kEq ? P.row_upper[i] : (c == kGeq || c == kLeq) ? kInf : 0.0;
+    rowscale[r] = 1.0;
+    H.optr[i] = P.rptr[r] - (P.slack[i] >= 0);   // the caller's row length (rptr: the form's, before its scan)
+    if (P.slack[i] >= 0) {   // one -1 slack column per BOUND / FREE row, in row order, with the row's raw bounds
+      const int j = n0 + P.slack[i], q = nnz0 + P.slack[i];
+      P.cbeg[j] = q; P.cidx[q] = r; P.cval[q] = -1.0; P.pcol[q] = j;
+      cost[j] = 0.0;
+      lower[j] = P.row_lower[i];
+      upper[j] = P.row_upper[i];
+      colscale[j] = 1.0;
+    }
+  }
+  if (t == 0) P.cbeg[n] = nnz;
+  __syncthreads();
+  // the listed columns, sorted by the whole CTA: an entry's slot is its rank under (new row, value key, stored index), the
+  // other entries streamed through shared memory a tile at a time.  (value_key orders -0.0 before +0.0, which std::sort
+  // leaves in either order.)
+  const int ns = nsort;
+  for (int s = 0; s < ns; s++) {
+    const int j = H.sortcols[s];
+    const int p0 = P.a_start[j], len = P.a_start[j + 1] - p0;
+    for (int k0 = 0; k0 < len; k0 += kThreads) {
+      const int k = k0 + t;
+      int row = 0;
+      double v = 0.0;
+      unsigned long long key = 0;
+      if (k < len) {
+        const int i = P.a_index[p0 + k];
+        row = rni[i];
+        v = rcl[i] == kLeq ? -P.a_value[p0 + k] : P.a_value[p0 + k];
+        key = value_key(v);
+      }
+      int rank = 0;
+      for (int h0 = 0; h0 < len; h0 += kThreads) {
+        __syncthreads();
+        if (h0 + t < len) {
+          const int i = P.a_index[p0 + h0 + t];
+          s_row[t] = rni[i];
+          s_key[t] = value_key(rcl[i] == kLeq ? -P.a_value[p0 + h0 + t] : P.a_value[p0 + h0 + t]);
+        }
+        __syncthreads();
+        if (k < len) {
+          const int cnt = min(kThreads, len - h0);
+          for (int h = 0; h < cnt; h++) {
+            const int rh = s_row[h];
+            const unsigned long long kh = s_key[h];
+            rank += rh < row || (rh == row && (kh < key || (kh == key && h0 + h < k)));
+          }
+        }
+      }
+      if (k < len) { const int q = p0 + rank; P.cidx[q] = row; P.cval[q] = v; P.pcol[q] = j; }
+    }
+  }
+  __syncthreads();
+
+  // ---- the row-major indexes (build_row_index) of the form and of the caller's matrix (the postsolve's row sums)
+  const int rtotal = block_scan(P.rptr, 1, m, sm);
+  if (t == 0) P.rptr[m] = rtotal;
+  const int ototal = block_scan(H.optr, 1, m, sm);
+  if (t == 0) H.optr[m] = ototal;
+  for (int i = t; i < m; i += kThreads) P.rwork[i] = P.rptr[i];
+  __syncthreads();
+  if (wid == 0) {
+    row_walk(nnz, P.cidx, P.rwork, P.rpos);
+    for (int i = t; i < m; i += 32) P.rwork[i] = H.optr[i];
+    __syncwarp();
+    row_walk(nnz0, P.a_index, P.rwork, H.opos);
+  } else if (t == 32 || t == 64) {   // |c|^2 and |b|^2 of the unscaled form, index order (formulate_hipdlp's norms, squared)
+    const double* v = t == 32 ? cost : rlo;
+    const int len = t == 32 ? n : m;
+    double s = 0.0;
+    for (int q = 0; q < len; q++) s += v[q] * v[q];
+    P.rec[t == 32 ? 0 : 1] = s;
+  }
+  __syncthreads();
+
+  // ---- scale_hipdlp: Ruiz x ruiz_iterations, then Pock-Chambolle, then L2, each pass as its bit of scaling_mode says
+  if (scaling_mode & 1)
+    for (int it = 0; it < ruiz_iterations; it++) hip_scale_pass<0>(P, cost, lower, upper, colscale, rlo, rup, rowscale);
+  if (scaling_mode & 4) hip_scale_pass<1>(P, cost, lower, upper, colscale, rlo, rup, rowscale);
+  if (scaling_mode & 2) hip_scale_pass<2>(P, cost, lower, upper, colscale, rlo, rup, rowscale);
+
+  // ---- the ordered sliced-ELL bodies (every column is already sorted by row)
+  form_layouts(P, m, n, sm);
+}
+
+__global__ void __launch_bounds__(kThreads)
+hip_batch_post_kernel(const BatchPrep* __restrict__ prep, const HipBatchPrep* __restrict__ hprep,
+                      const HipBatchPost* __restrict__ post, int scaled) {
+  const BatchPrep& P = prep[blockIdx.x];
+  const HipBatchPrep& H = hprep[blockIdx.x];
+  const HipBatchPost& Q = post[blockIdx.x];
+  if (!(Q.col_value && Q.col_dual && Q.row_value && Q.row_dual)) return;
+  const int n0 = P.n0, m = P.m, n = P.n;
+  const double* v = P.vec;
+  const double* w = v + 14 * n;
+  const double* x = Q.sol == 1 ? v + 6 * n : v + 4 * n;   // xn or x
+  const double* y = Q.sol == 1 ? w + 5 * m : w + 3 * m;   // yn or y
+  const double *colscale = v + 3 * n, *sp = v + 12 * n, *sn = v + 13 * n, *rowscale = w + 2 * m;
+  const bool conv = Q.sol >= 0;
+  const double sense = P.sense;
+  // the unscaled primal value of structural column j (hip_host_postsolve's hx[j])
+  const auto xval = [&](int j) {
+    double xv = conv ? x[j] : 0.0;
+    if (scaled) xv /= colscale[j];
+    return xv;
+  };
+  for (int j = threadIdx.x; j < n0; j += kThreads) {
+    const double cs = colscale[j];
+    Q.col_value[j] = xval(j);
+    const double a = sp[j] * cs, b = sn[j] * cs;
+    double d = a - b;
+    d *= sense;
+    Q.col_dual[j] = d;
+  }
+  for (int i = threadIdx.x; i < m; i += kThreads) {
+    const int r = P.row_new_idx[i];
+    double d = conv ? y[r] : 0.0;
+    if (scaled) d /= rowscale[r];
+    Q.row_dual[i] = P.row_class[i] == kLeq ? -d : d;
+    double s = 0.0;   // A x along the caller's row: columns ascending, then stored order
+    for (int q = H.optr[i]; q < H.optr[i + 1]; q++) {
+      const int p = H.opos[q];
+      s += P.a_value[p] * xval(P.pcol[p]);
+    }
+    Q.row_value[i] = s;
+  }
+}
+
 }  // namespace
+
+void launch_hip_batch_size(cudaStream_t s, int count, const BatchPrep* prep, BatchSize* sizes) {
+  if (count > 0) hip_batch_size_kernel<<<count, kThreads, 0, s>>>(prep, sizes);
+}
+void launch_hip_batch_prep(cudaStream_t s, int count, const BatchPrep* prep, const HipBatchPrep* hprep, int scaling_mode,
+                           int ruiz_iterations) {
+  if (count > 0) hip_batch_prep_kernel<<<count, kThreads, 0, s>>>(prep, hprep, scaling_mode, ruiz_iterations);
+}
+void launch_hip_batch_post(cudaStream_t s, int count, const BatchPrep* prep, const HipBatchPrep* hprep,
+                           const HipBatchPost* post, int scaled) {
+  if (count > 0) hip_batch_post_kernel<<<count, kThreads, 0, s>>>(prep, hprep, post, scaled);
+}
 
 void launch_batch_size(cudaStream_t s, int count, const BatchPrep* prep, BatchSize* sizes) {
   if (count > 0) batch_size_kernel<<<count, kThreads, 0, s>>>(prep, sizes);

@@ -1,4 +1,5 @@
-// highs_b200/csrc/batch_prep.hpp -- the device prologue and postsolve of b200pdlp_solve_batch_device: one CTA per member.
+// highs_b200/csrc/batch_prep.hpp -- the device prologue and postsolve of b200pdlp_solve_batch_device and
+// b200pdlp_solve_hipdlp_batch_device: one CTA per member.
 #pragma once
 #include "kernels.cuh"
 
@@ -51,5 +52,28 @@ struct BatchPost {
 void launch_batch_size(cudaStream_t s, int count, const BatchPrep* prep, BatchSize* sizes);
 void launch_batch_prep(cudaStream_t s, int count, const BatchPrep* prep, int do_scale);
 void launch_batch_post(cudaStream_t s, int count, const BatchPrep* prep, const BatchPost* post);
+
+// ---- the HiPDLP batch (b200pdlp_solve_hipdlp_batch_device): the same BatchPrep per member, read with HiPDLP's meaning --
+// row_class under formulate_hipdlp's rule (FREE rows a class of their own), slack[i] >= 0 for BOUND and FREE rows, vec a
+// block of hip_batch_vec_len doubles (engine.cu), rec[0..1] = |c|^2, |b|^2 of the unscaled form -- plus these arrays
+// (pooled, like BatchPrep's):
+struct HipBatchPrep {
+  int* optr;       // [m + 1] row pointer of the row-major index of the caller's matrix
+  int* opos;       // [nnz0]  its positions into a_index / a_value: per row columns ascending, then stored order
+  int* sortcols;   // [num_col] structural columns whose stored rows do not ascend strictly (the prologue's work list)
+};
+
+// Per member, for the HiPDLP postsolve: the caller's device vectors (any NULL: none written) and the iterate to return
+struct HipBatchPost {
+  double *col_value, *col_dual, *row_value, *row_dual;
+  int sol;          // -1: not converged (x = y = 0); 0: (x, y) of the iteration-0 check; 1: (xn, yn) after a block
+  int pad;
+};
+
+void launch_hip_batch_size(cudaStream_t s, int count, const BatchPrep* prep, BatchSize* sizes);
+void launch_hip_batch_prep(cudaStream_t s, int count, const BatchPrep* prep, const HipBatchPrep* hprep, int scaling_mode,
+                           int ruiz_iterations);
+void launch_hip_batch_post(cudaStream_t s, int count, const BatchPrep* prep, const HipBatchPrep* hprep,
+                           const HipBatchPost* post, int scaled);
 
 }  // namespace b200

@@ -2652,6 +2652,10 @@ struct StreamHolder {
 // rhs, rowscale, then y0 y1 ax0 ax1 ysum yavg axavg ylr (m each)
 static size_t batch_vec_len(int n, int m) { return (size_t)12 * n + (size_t)10 * m; }
 
+// doubles of a HiPDLP member's vector block: cost, lower, upper, colscale, then x xa xn rx aty hslack atyp atdy sp sn (n each);
+// rlo, rup, rowscale, then y ya yn ry axp dy (m each)
+static size_t hip_batch_vec_len(int n, int m) { return (size_t)14 * n + (size_t)9 * m; }
+
 // the vectors of a member's block `v` (batch_vec_len) as BatchMember pointers
 static void batch_member_vectors(BatchMember& M, double* v, int n, int m) {
   double* w = v + 12 * (size_t)n;
@@ -2916,24 +2920,50 @@ static void solve_batch(int count, const b200pdlp_lp* lps, const b200pdlp_params
 // and one scalar record per member, never an array, and the members return solve_batch's bits.
 
 // the checks of a member that read no array (the device checks the arrays: batch_size_kernel)
-static void check_batch_device_member(const b200pdlp_lp* lp, const b200pdlp_params& prm, int i) {
+// (both device-pointer batches; who: the entry point, for the message)
+static void check_batch_device_member(const b200pdlp_lp* lp, int ordered_max, int i, const char* who) {
   const int rc = guarded([&] {
     if (!lp_fields_ok(lp)) throw Error(B200PDLP_ERR_ARG, "b200pdlp: malformed b200pdlp_lp");
     if (lp->sense != 1.0 && lp->sense != -1.0) throw Error(B200PDLP_ERR_ARG, "b200pdlp: sense must be +1 or -1");
-    if (prm.ordered_max < 0) throw Error(B200PDLP_ERR_ARG, "ordered_max < 0: a batch solves ordered-mode problems only");
+    if (ordered_max < 0) throw Error(B200PDLP_ERR_ARG, "ordered_max < 0: a batch solves ordered-mode problems only");
   });
-  if (rc != B200PDLP_OK) throw Error(rc, "b200pdlp_solve_batch_device: member " + std::to_string(i) + ": " + g_last_error);
+  if (rc != B200PDLP_OK) throw Error(rc, std::string(who) + ": member " + std::to_string(i) + ": " + g_last_error);
 }
 
 // ptr (NULL: not given) must be device or managed memory of `device`
-static void check_device_array(const void* ptr, int device, int i, const char* field) {
+static void check_device_array(const void* ptr, int device, int i, const char* field, const char* who) {
   if (!ptr) return;
   cudaPointerAttributes a{};
   const cudaError_t e = cudaPointerGetAttributes(&a, ptr);
   if (e != cudaSuccess) cudaGetLastError();
   if (e != cudaSuccess || !((a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == device))
-    throw Error(B200PDLP_ERR_ARG, "b200pdlp_solve_batch_device: member " + std::to_string(i) + ": " + field +
+    throw Error(B200PDLP_ERR_ARG, std::string(who) + ": member " + std::to_string(i) + ": " + field +
                                       " is not device memory of device " + std::to_string(device));
+}
+
+// every array pointer of the batch (warms: NULL for none) must be device memory of `device`: the lowest failing member, field
+static void check_device_arrays(int count, const b200pdlp_lp* lps, const b200pdlp_warm* warms, const b200pdlp_result* outs,
+                                int device, const char* who) {
+  for (int i = 0; i < count; i++) {
+    const b200pdlp_lp& lp = lps[i];
+    check_device_array(lp.a_start, device, i, "a_start", who);
+    check_device_array(lp.a_index, device, i, "a_index", who);
+    check_device_array(lp.a_value, device, i, "a_value", who);
+    check_device_array(lp.col_cost, device, i, "col_cost", who);
+    check_device_array(lp.col_lower, device, i, "col_lower", who);
+    check_device_array(lp.col_upper, device, i, "col_upper", who);
+    check_device_array(lp.row_lower, device, i, "row_lower", who);
+    check_device_array(lp.row_upper, device, i, "row_upper", who);
+    if (warms) {
+      check_device_array(warms[i].col_value, device, i, "warm col_value", who);
+      check_device_array(warms[i].row_value, device, i, "warm row_value", who);
+      check_device_array(warms[i].row_dual, device, i, "warm row_dual", who);
+    }
+    check_device_array(outs[i].col_value, device, i, "result col_value", who);
+    check_device_array(outs[i].col_dual, device, i, "result col_dual", who);
+    check_device_array(outs[i].row_value, device, i, "result row_value", who);
+    check_device_array(outs[i].row_dual, device, i, "result row_dual", who);
+  }
 }
 
 // A device-resident batch after its prologue: the descriptors (pool pointers set), the sizing and scalar records, the pools
@@ -2948,6 +2978,15 @@ struct DeviceBatch {
   DevBuf<int> ints, col;     // the form's index arrays: 3 nnz + n + m + 1 per member; the layouts' column ids
   DevBuf<double> dbls, vec, val;   // the form's values and the scaling factors: nnz + 2 n + m; batch_vec_len; the layouts' values
   DevBuf<int4> slices;
+  std::vector<HipBatchPrep> hx;    // HiPDLP members only: their arrays in `ints`
+  DevBuf<HipBatchPrep> dhx;
+};
+
+// which prologue a device batch runs: formulate + scale (PDLP mode), or formulate_hipdlp + scale_hipdlp (HiPDLP mode)
+struct PrepMode {
+  bool hip = false;
+  int scaling = 0;           // PDLP: b200pdlp_params::scaling; HiPDLP: scaling_mode
+  int ruiz_iterations = 0;   // HiPDLP only
 };
 
 static const char* prep_error_text(int err) {
@@ -2961,8 +3000,8 @@ static const char* prep_error_text(int err) {
 
 // Validation and sizing (one read-back of `count` records), the pools, then the prologue (one read-back of the scalar
 // records), on stream s of the current device.  lps[i] / warms[i]: host structs whose arrays are device memory.
-static void device_batch_prologue(cudaStream_t s, int count, const b200pdlp_lp* lps, const b200pdlp_warm* warms, int scaling,
-                                  int ordered_max, const char* who, DeviceBatch& D, Laps& lap) {
+static void device_batch_prologue(cudaStream_t s, int count, const b200pdlp_lp* lps, const b200pdlp_warm* warms,
+                                  const PrepMode& mode, int ordered_max, const char* who, DeviceBatch& D, Laps& lap) {
   const int omax = ordered_max == 0 ? 4096 : ordered_max;
   D.hp.assign((size_t)count, BatchPrep{});
   size_t nrows = 0;
@@ -2986,7 +3025,8 @@ static void device_batch_prologue(cudaStream_t s, int count, const b200pdlp_lp* 
   }
   D.prep.alloc(count, false); D.dsize.alloc(count, false); D.drec.alloc((size_t)count * kPrepRec, false);
   CUDA_OK(cudaMemcpyAsync(D.prep.p, D.hp.data(), (size_t)count * sizeof(BatchPrep), cudaMemcpyHostToDevice, s));
-  launch_batch_size(s, count, D.prep.p, D.dsize.p);
+  if (mode.hip) launch_hip_batch_size(s, count, D.prep.p, D.dsize.p);
+  else launch_batch_size(s, count, D.prep.p, D.dsize.p);
   CUDA_OK(cudaGetLastError());
   D.size.resize((size_t)count);
   CUDA_OK(cudaMemcpyAsync(D.size.data(), D.dsize.p, (size_t)count * sizeof(BatchSize), cudaMemcpyDeviceToHost, s));
@@ -3009,8 +3049,9 @@ static void device_batch_prologue(cudaStream_t s, int count, const b200pdlp_lp* 
     const BatchSize& z = D.size[i];
     const size_t n = z.n, m = lps[i].num_row, nnz = z.nnz;
     ni += 3 * nnz + n + m + 1;
+    if (mode.hip) ni += m + 1 + (nnz - n) + 2 * (size_t)lps[i].num_col;   // optr, opos (nnz0), sortcols
     nd += nnz + 2 * n + m;
-    nv += batch_vec_len(z.n, lps[i].num_row);
+    nv += mode.hip ? hip_batch_vec_len(z.n, lps[i].num_row) : batch_vec_len(z.n, lps[i].num_row);
     nsl += (m + 31) / 32 + (n + 31) / 32;
     ne += (size_t)z.pad_a + 32 + (size_t)z.pad_at + 32;
   }
@@ -3018,6 +3059,7 @@ static void device_batch_prologue(cudaStream_t s, int count, const b200pdlp_lp* 
   D.col.alloc(ne, false); D.val.alloc(ne, false);
   CUDA_OK(cudaMemsetAsync(D.vec.p, 0, std::max<size_t>(nv, 1) * sizeof(double), s));   // the iterates' other halves, sums
   ni = nd = nv = nsl = ne = 0;
+  if (mode.hip) D.hx.assign((size_t)count, HipBatchPrep{});
   for (int i = 0; i < count; i++) {
     const BatchSize& z = D.size[i];
     BatchPrep& P = D.hp[i];
@@ -3026,11 +3068,17 @@ static void device_batch_prologue(cudaStream_t s, int count, const b200pdlp_lp* 
     int* q = D.ints.p + ni;
     P.cbeg = q; P.cidx = q + n + 1; P.pcol = P.cidx + nnz; P.rpos = P.pcol + nnz; P.rwork = P.rpos + nnz;
     ni += 3 * (size_t)nnz + n + m + 1;
+    if (mode.hip) {
+      const int n0 = lps[i].num_col;
+      HipBatchPrep& X = D.hx[i];
+      X.optr = D.ints.p + ni; X.opos = X.optr + m + 1; X.sortcols = X.opos + (nnz - n + n0);
+      ni += (size_t)m + 1 + (nnz - n + n0) + n0;
+    }
     double* d = D.dbls.p + nd;
     P.cval = d; P.cs = d + nnz; P.cs_next = P.cs + n; P.rs = P.cs_next + n;
     nd += (size_t)nnz + 2 * (size_t)n + m;
     P.vec = D.vec.p + nv;
-    nv += batch_vec_len(n, m);
+    nv += mode.hip ? hip_batch_vec_len(n, m) : batch_vec_len(n, m);
     P.a_slices = D.slices.p + nsl; nsl += (m + 31) / 32;
     P.at_slices = D.slices.p + nsl; nsl += (n + 31) / 32;
     P.a_col = D.col.p + ne; P.a_val = D.val.p + ne; ne += (size_t)z.pad_a + 32;
@@ -3038,10 +3086,20 @@ static void device_batch_prologue(cudaStream_t s, int count, const b200pdlp_lp* 
     P.rec = D.drec.p + (size_t)kPrepRec * i;
   }
   CUDA_OK(cudaMemcpyAsync(D.prep.p, D.hp.data(), (size_t)count * sizeof(BatchPrep), cudaMemcpyHostToDevice, s));
-  launch_batch_prep(s, count, D.prep.p, scaling != 0);
-  CUDA_OK(cudaGetLastError());
-  D.rec.resize((size_t)count * kPrepRec);
-  CUDA_OK(cudaMemcpyAsync(D.rec.data(), D.drec.p, D.rec.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+  D.rec.assign((size_t)count * kPrepRec, 0.0);
+  if (mode.hip) {
+    D.dhx.alloc(count, false);
+    CUDA_OK(cudaMemcpyAsync(D.dhx.p, D.hx.data(), (size_t)count * sizeof(HipBatchPrep), cudaMemcpyHostToDevice, s));
+    launch_hip_batch_prep(s, count, D.prep.p, D.dhx.p, mode.scaling, mode.ruiz_iterations);
+    CUDA_OK(cudaGetLastError());
+    // rec[0..1] of every member: |c|^2 and |b|^2 of the unscaled form
+    CUDA_OK(cudaMemcpy2DAsync(D.rec.data(), kPrepRec * sizeof(double), D.drec.p, kPrepRec * sizeof(double), 2 * sizeof(double),
+                              count, cudaMemcpyDeviceToHost, s));
+  } else {
+    launch_batch_prep(s, count, D.prep.p, mode.scaling != 0);
+    CUDA_OK(cudaGetLastError());
+    CUDA_OK(cudaMemcpyAsync(D.rec.data(), D.drec.p, D.rec.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+  }
   CUDA_OK(cudaStreamSynchronize(s));
   lap("batch device", "prologue (device)");
 }
@@ -3055,32 +3113,15 @@ static void solve_batch_device(int count, const b200pdlp_lp* lps, const b200pdlp
   if (prm.device >= 0) CUDA_OK(cudaSetDevice(prm.device));
   int device = 0;
   CUDA_OK(cudaGetDevice(&device));
-  for (int i = 0; i < count; i++) {
-    const b200pdlp_lp& lp = lps[i];
-    check_device_array(lp.a_start, device, i, "a_start");
-    check_device_array(lp.a_index, device, i, "a_index");
-    check_device_array(lp.a_value, device, i, "a_value");
-    check_device_array(lp.col_cost, device, i, "col_cost");
-    check_device_array(lp.col_lower, device, i, "col_lower");
-    check_device_array(lp.col_upper, device, i, "col_upper");
-    check_device_array(lp.row_lower, device, i, "row_lower");
-    check_device_array(lp.row_upper, device, i, "row_upper");
-    if (warms) {
-      check_device_array(warms[i].col_value, device, i, "warm col_value");
-      check_device_array(warms[i].row_value, device, i, "warm row_value");
-      check_device_array(warms[i].row_dual, device, i, "warm row_dual");
-    }
-    check_device_array(outs[i].col_value, device, i, "result col_value");
-    check_device_array(outs[i].col_dual, device, i, "result col_dual");
-    check_device_array(outs[i].row_value, device, i, "result row_value");
-    check_device_array(outs[i].row_dual, device, i, "result row_dual");
-  }
+  check_device_arrays(count, lps, warms, outs, device, "b200pdlp_solve_batch_device");
   StreamHolder sh;
   cudaStream_t s = sh.s;
   DeviceBatch D;
   {
     NvtxRange nvtx("b200pdlp: batch prologue (device)");
-    device_batch_prologue(s, count, lps, warms, prm.scaling, prm.ordered_max, "b200pdlp_solve_batch_device", D, lap);
+    PrepMode mode;
+    mode.scaling = prm.scaling;
+    device_batch_prologue(s, count, lps, warms, mode, prm.ordered_max, "b200pdlp_solve_batch_device", D, lap);
   }
   std::vector<BatchRun> runs((size_t)count);
   std::vector<BatchRun*> R((size_t)count);
@@ -3154,9 +3195,16 @@ static double batch_probe(int i, int k) {
   return (double)(h >> 11) * 0x1p-52 - 1.0;
 }
 
-static void batch_prep_compare(int count, const b200pdlp_lp* lps, int scaling, double* report) {
-  device_count_checked();
-  // the raw LPs, uploaded as they are
+// host LPs uploaded as they are: dl[i] is lps[i] with its arrays in ri / rd
+struct RawLps {
+  DevBuf<int> ri;
+  DevBuf<double> rd;
+  std::vector<b200pdlp_lp> dl;
+};
+static void upload_raw_lps(int count, const b200pdlp_lp* lps, RawLps& R) {
+  DevBuf<int>& ri = R.ri;
+  DevBuf<double>& rd = R.rd;
+  std::vector<b200pdlp_lp>& dl = R.dl;
   size_t ni = 0, nd = 0;
   for (int i = 0; i < count; i++) {
     const b200pdlp_lp& lp = lps[i];
@@ -3164,10 +3212,8 @@ static void batch_prep_compare(int count, const b200pdlp_lp* lps, int scaling, d
     ni += lp.num_col + 1 + nnz;
     nd += nnz + 3 * (size_t)lp.num_col + 2 * (size_t)lp.num_row;
   }
-  DevBuf<int> ri;
-  DevBuf<double> rd;
   ri.alloc(ni, false); rd.alloc(nd, false);
-  std::vector<b200pdlp_lp> dl(lps, lps + count);
+  dl.assign(lps, lps + count);
   ni = nd = 0;
   for (int i = 0; i < count; i++) {
     const b200pdlp_lp& lp = lps[i];
@@ -3179,10 +3225,18 @@ static void batch_prep_compare(int count, const b200pdlp_lp* lps, int scaling, d
     d.col_cost = up_d(lp.col_cost, n0); d.col_lower = up_d(lp.col_lower, n0); d.col_upper = up_d(lp.col_upper, n0);
     d.row_lower = up_d(lp.row_lower, m); d.row_upper = up_d(lp.row_upper, m);
   }
+}
+
+static void batch_prep_compare(int count, const b200pdlp_lp* lps, int scaling, double* report) {
+  device_count_checked();
+  RawLps raw;
+  upload_raw_lps(count, lps, raw);
   StreamHolder sh;
   DeviceBatch D;
   Laps lap;
-  device_batch_prologue(sh.s, count, dl.data(), nullptr, scaling, std::numeric_limits<int>::max(), "b200pdlp_debug_batch_prep_compare",
+  PrepMode mode;
+  mode.scaling = scaling;
+  device_batch_prologue(sh.s, count, raw.dl.data(), nullptr, mode, std::numeric_limits<int>::max(), "b200pdlp_debug_batch_prep_compare",
                         D, lap);
   std::vector<StdForm> F((size_t)count);
   for (int i = 0; i < count; i++) {
@@ -3309,18 +3363,134 @@ static void check_hipdlp_batch_member(const b200pdlp_lp* lp, const b200pdlp_hipd
   if (rc != B200PDLP_OK) throw Error(rc, "b200pdlp_solve_hipdlp_batch: member " + std::to_string(i) + ": " + g_last_error);
 }
 
-struct HipBatchHost {   // one member on the host
-  StdForm f;
-  HostLayout L;
-  size_t vec = 0, sl_a = 0, sl_at = 0, e_a = 0, e_at = 0;   // offsets in the pools
+struct HipBatchRun {   // one member's host control over the rounds
+  StdForm f;           // b200pdlp_solve_hipdlp_batch_device fills the scalars only: dimensions, sense, offset, norms, scaled
   HipController ctl;
   bool converged = false, timed_out = false;
   int sol = 0;   // converged: 0 at the iteration-0 check (x, y), 1 after a block (xn, yn)
 };
 
-// doubles of a HiPDLP member's vector block: cost, lower, upper, colscale, then x xa xn rx aty hslack atyp atdy sp sn (n each);
-// rlo, rup, rowscale, then y ya yn ry axp dy (m each)
-static size_t hip_batch_vec_len(int n, int m) { return (size_t)14 * n + (size_t)9 * m; }
+struct HipBatchHost : HipBatchRun {   // one member of b200pdlp_solve_hipdlp_batch on the host
+  HostLayout L;
+  size_t vec = 0, sl_a = 0, sl_at = 0, e_a = 0, e_at = 0;   // offsets in the pools
+};
+
+// the HipBatchMember of a member with block `v` (hip_batch_vec_len) and the given layouts
+static HipBatchMember hip_batch_member(const StdForm& f, int neq, double* v, const int4* a_slices, const int* a_col,
+                                       const double* a_val, const int4* at_slices, const int* at_col, const double* at_val) {
+  const int n = f.n, m = f.m;
+  double* w = v + 14 * (size_t)n;
+  HipBatchMember M;
+  M.n = n; M.m = m; M.neq = neq; M.scaled = f.scaled ? 1 : 0; M.offset = f.offset;
+  M.a_slices = a_slices; M.a_col = a_col; M.a_val = a_val;
+  M.at_slices = at_slices; M.at_col = at_col; M.at_val = at_val;
+  M.cost = v; M.lower = v + n; M.upper = v + 2 * n; M.colscale = v + 3 * n;
+  M.x = v + 4 * n; M.xa = v + 5 * n; M.xn = v + 6 * n; M.rx = v + 7 * n; M.aty = v + 8 * n; M.hslack = v + 9 * n;
+  M.atyp = v + 10 * n; M.atdy = v + 11 * n; M.sp = v + 12 * n; M.sn = v + 13 * n;
+  M.rlo = w; M.rup = w + m; M.rowscale = w + 2 * m;
+  M.y = w + 3 * m; M.ya = w + 4 * m; M.yn = w + 5 * m; M.ry = w + 6 * m; M.axp = w + 7 * m; M.dy = w + 8 * m;
+  return M;
+}
+
+// The rounds of a HiPDLP batch, for both entry points: one upload of the control blocks and states, one launch, one
+// read-back, then each member's HipController decisions in the order solve_hipdlp_on_device takes them, until no member is
+// active or the time limit has passed.
+static BatchLoop hip_batch_rounds(cudaStream_t s, int count, const b200pdlp_hipdlp_params& prm, const HipBatchMember* dmem,
+                                  const std::vector<HipBatchRun*>& B) {
+  using clk = std::chrono::steady_clock;
+  DevBuf<HipState> dst;
+  DevBuf<HipBatchCtl> dctl;
+  dst.alloc(count, false); dctl.alloc(count, false);
+  PinnedArray<HipState> hst((size_t)count);
+  PinnedArray<HipBatchCtl> hctl((size_t)count);
+  memset(hst.p, 0, (size_t)count * sizeof(HipState));
+  for (int i = 0; i < count; i++) {
+    HipBatchCtl& c = hctl.p[i];
+    memset(&c, 0, sizeof(HipBatchCtl));
+    c.active = 1; c.first = 1;
+  }
+  const double t_lim = (prm.time_limit >= 0 && std::isfinite(prm.time_limit)) ? prm.time_limit : -1.0;   // < 0: none
+  CudaEvent evl0, evl1, ev0, ev1;
+  BatchLoop L;
+  int active = count;
+  CUDA_OK(cudaEventRecord(evl0, s));
+  L.t_loop = clk::now();
+  while (active > 0) {
+    NvtxRange nvtx("b200pdlp: HiPDLP batch round");
+    // solve_hipdlp_on_device reads its clock before every block.  There a restart decided after the last block copies the
+    // iterates before that test; here the copy is the first thing of the next round, so a member that times out never
+    // makes it.  That cannot show: the copy writes x, xa, y, ya and A'y only, an unconverged run returns x = y = 0, and the
+    // slacks sp / sn the postsolve reads are those of the last check in both solves.
+    if (L.rounds > 0 && t_lim >= 0 && std::chrono::duration<double>(clk::now() - L.t_loop).count() > t_lim) {
+      for (int i = 0; i < count; i++)
+        if (hctl.p[i].active) { B[i]->timed_out = true; hctl.p[i].active = 0; }
+      break;
+    }
+    CUDA_OK(cudaMemcpyAsync(dctl.p, hctl.p, (size_t)count * sizeof(HipBatchCtl), cudaMemcpyHostToDevice, s));
+    CUDA_OK(cudaMemcpyAsync(dst.p, hst.p, (size_t)count * sizeof(HipState), cudaMemcpyHostToDevice, s));
+    CUDA_OK(cudaEventRecord(ev0, s));
+    launch_hip_batch_round(s, count, dmem, dst.p, dctl.p);
+    CUDA_OK(cudaEventRecord(ev1, s));
+    CUDA_OK(cudaMemcpyAsync(hctl.p, dctl.p, (size_t)count * sizeof(HipBatchCtl), cudaMemcpyDeviceToHost, s));
+    CUDA_OK(cudaStreamSynchronize(s));
+    float ms = 0.f;
+    CUDA_OK(cudaEventElapsedTime(&ms, ev0, ev1));
+    L.iter_ms += ms;
+    const bool first = L.rounds == 0;
+    L.rounds++;
+    for (int i = 0; i < count; i++) {
+      HipBatchCtl& c = hctl.p[i];
+      if (!c.active) continue;
+      HipBatchRun& b = *B[i];
+      HipController& ctl = b.ctl;
+      const StdForm& f = b.f;
+      bool done = false, restart = false;
+      if (first) {   // iteration 0 (:566-572)
+        const double op_norm_sq = (f.n > 0 && f.m > 0) ? c.outs[kHipBatchLambda] : 1.0;
+        ctl.init(f.norm_cost, f.norm_rhs, op_norm_sq, prm.tolerance, prm.step_size_strategy);
+        if (ctl.converged(c.outs)) { b.converged = true; b.sol = 0; done = true; }
+        else done = ctl.iters >= prm.iter_limit;
+      } else {
+        if (c.fpe) ctl.restart_reference(c.outs + kHipBatchFpe);
+        restart = ctl.after_block(c.outs);
+        if (ctl.pfeas < ctl.tol * (1.0 + f.norm_rhs) && ctl.dfeas < ctl.tol * (1.0 + f.norm_cost) && ctl.relgap < ctl.tol) {
+          b.converged = true; b.sol = 1; done = true;
+        } else {
+          done = ctl.iters >= prm.iter_limit;
+        }
+      }
+      if (done) { c.active = 0; active--; continue; }
+      c.first = 0;
+      c.restart = restart ? 1 : 0;
+      c.fpe = ctl.pending_restart_fpe ? 1 : 0;
+      HipState& st = hst.p[i];
+      st.primal_step = ctl.primal_step; st.dual_step = ctl.dual_step; st.halpern_iteration = ctl.halpern_iteration;
+    }
+  }
+  CUDA_OK(cudaEventRecord(evl1, s));
+  CUDA_OK(cudaEventSynchronize(evl1));
+  CUDA_OK(cudaEventElapsedTime(&L.loop_ms, evl0, evl1));
+  L.solve_seconds = std::chrono::duration<double>(clk::now() - L.t_loop).count();
+  return L;
+}
+
+// the fields of a HiPDLP batch result besides the vectors; the timings and kernel_launches are the batch's
+static void hip_batch_result(b200pdlp_result* out, const HipBatchRun& b, const BatchLoop& L, double setup_seconds) {
+  const StdForm& f = b.f;
+  const HipController& ctl = b.ctl;
+  out->value_valid = 1; out->dual_valid = 1;
+  out->term_code = b.converged ? B200PDLP_OPTIMAL : B200PDLP_TIMELIMIT_OR_ITERLIMIT;
+  out->term_iterate = b.timed_out ? 2 : 0;
+  out->iters = ctl.iters; out->passes = ctl.iters; out->restarts = ctl.restarts;
+  out->kernel_launches = (int)std::min<long long>(L.rounds, 2147483647LL);
+  out->primal_obj = ctl.pobj; out->dual_obj = ctl.dobj; out->primal_feas = ctl.pfeas; out->dual_feas = ctl.dfeas;
+  out->gap = ctl.pobj - ctl.dobj; out->rel_gap = ctl.relgap;
+  out->setup_seconds = setup_seconds;
+  out->solve_seconds = L.solve_seconds;
+  out->loop_device_ms = L.loop_ms;
+  out->iter_device_ms = L.iter_ms;
+  out->form_cols = f.n; out->form_rows = f.m; out->form_nnz = f.nnz; out->form_neq = f.neq;
+}
 
 static void solve_hipdlp_batch(int count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params& prm, b200pdlp_result* outs) {
   using clk = std::chrono::steady_clock;
@@ -3380,33 +3550,13 @@ static void solve_hipdlp_batch(int count, const b200pdlp_lp* lps, const b200pdlp
   DevBuf<int> dcol;
   DevBuf<int4> dsl;
   DevBuf<HipBatchMember> dmem;
-  DevBuf<HipState> dst;
-  DevBuf<HipBatchCtl> dctl;
   dvec.alloc(hvec.size(), false); dval.alloc(hval.size(), false); dcol.alloc(hcol.size(), false); dsl.alloc(hsl.size(), false);
-  dmem.alloc(count, false); dst.alloc(count, false); dctl.alloc(count, false);
+  dmem.alloc(count, false);
   std::vector<HipBatchMember> hmem((size_t)count);
   for (int i = 0; i < count; i++) {
     const HipBatchHost& b = B[i];
-    const int n = b.f.n, m = b.f.m;
-    double* v = dvec.p + b.vec;
-    double* w = v + 14 * n;
-    HipBatchMember& M = hmem[i];
-    M.n = n; M.m = m; M.neq = b.L.neq_local; M.scaled = b.f.scaled ? 1 : 0; M.offset = b.f.offset;
-    M.a_slices = dsl.p + b.sl_a; M.a_col = dcol.p + b.e_a; M.a_val = dval.p + b.e_a;
-    M.at_slices = dsl.p + b.sl_at; M.at_col = dcol.p + b.e_at; M.at_val = dval.p + b.e_at;
-    M.cost = v; M.lower = v + n; M.upper = v + 2 * n; M.colscale = v + 3 * n;
-    M.x = v + 4 * n; M.xa = v + 5 * n; M.xn = v + 6 * n; M.rx = v + 7 * n; M.aty = v + 8 * n; M.hslack = v + 9 * n;
-    M.atyp = v + 10 * n; M.atdy = v + 11 * n; M.sp = v + 12 * n; M.sn = v + 13 * n;
-    M.rlo = w; M.rup = w + m; M.rowscale = w + 2 * m;
-    M.y = w + 3 * m; M.ya = w + 4 * m; M.yn = w + 5 * m; M.ry = w + 6 * m; M.axp = w + 7 * m; M.dy = w + 8 * m;
-  }
-  PinnedArray<HipState> hst((size_t)count);
-  PinnedArray<HipBatchCtl> hctl((size_t)count);
-  memset(hst.p, 0, (size_t)count * sizeof(HipState));
-  for (int i = 0; i < count; i++) {
-    HipBatchCtl& c = hctl.p[i];
-    memset(&c, 0, sizeof(HipBatchCtl));
-    c.active = 1; c.first = 1;
+    hmem[i] = hip_batch_member(b.f, b.L.neq_local, dvec.p + b.vec, dsl.p + b.sl_a, dcol.p + b.e_a, dval.p + b.e_a,
+                               dsl.p + b.sl_at, dcol.p + b.e_at, dval.p + b.e_at);
   }
   CUDA_OK(cudaMemcpyAsync(dvec.p, hvec.data(), hvec.size() * sizeof(double), cudaMemcpyHostToDevice, s));
   CUDA_OK(cudaMemcpyAsync(dval.p, hval.data(), hval.size() * sizeof(double), cudaMemcpyHostToDevice, s));
@@ -3416,82 +3566,19 @@ static void solve_hipdlp_batch(int count, const b200pdlp_lp* lps, const b200pdlp
   CUDA_OK(cudaStreamSynchronize(s));
   lap("batch", "pools + upload");
 
-  // ---- rounds
-  const double t_lim = (prm.time_limit >= 0 && std::isfinite(prm.time_limit)) ? prm.time_limit : -1.0;   // < 0: none
-  CudaEvent evl0, evl1, ev0, ev1;
-  double iter_ms = 0.0;
-  long long rounds = 0;
-  int active = count;
-  CUDA_OK(cudaEventRecord(evl0, s));
-  const auto t_loop = clk::now();
-  while (active > 0) {
-    NvtxRange nvtx("b200pdlp: HiPDLP batch round");
-    // solve_hipdlp_on_device reads its clock before every block.  There a restart decided after the last block copies the
-    // iterates before that test; here the copy is the first thing of the next round, so a member that times out never
-    // makes it.  That cannot show: the copy writes x, xa, y, ya and A'y only, an unconverged run returns x = y = 0, and the
-    // slacks sp / sn the postsolve reads are those of the last check in both solves.
-    if (rounds > 0 && t_lim >= 0 && std::chrono::duration<double>(clk::now() - t_loop).count() > t_lim) {
-      for (int i = 0; i < count; i++)
-        if (hctl.p[i].active) { B[i].timed_out = true; hctl.p[i].active = 0; }
-      break;
-    }
-    CUDA_OK(cudaMemcpyAsync(dctl.p, hctl.p, (size_t)count * sizeof(HipBatchCtl), cudaMemcpyHostToDevice, s));
-    CUDA_OK(cudaMemcpyAsync(dst.p, hst.p, (size_t)count * sizeof(HipState), cudaMemcpyHostToDevice, s));
-    CUDA_OK(cudaEventRecord(ev0, s));
-    launch_hip_batch_round(s, count, dmem.p, dst.p, dctl.p);
-    CUDA_OK(cudaEventRecord(ev1, s));
-    CUDA_OK(cudaMemcpyAsync(hctl.p, dctl.p, (size_t)count * sizeof(HipBatchCtl), cudaMemcpyDeviceToHost, s));
-    CUDA_OK(cudaStreamSynchronize(s));
-    float ms = 0.f;
-    CUDA_OK(cudaEventElapsedTime(&ms, ev0, ev1));
-    iter_ms += ms;
-    const bool first = rounds == 0;
-    rounds++;
-    for (int i = 0; i < count; i++) {
-      HipBatchCtl& c = hctl.p[i];
-      if (!c.active) continue;
-      HipBatchHost& b = B[i];
-      HipController& ctl = b.ctl;
-      const StdForm& f = b.f;
-      bool done = false, restart = false;
-      if (first) {   // iteration 0 (:566-572)
-        const double op_norm_sq = (f.n > 0 && f.m > 0) ? c.outs[kHipBatchLambda] : 1.0;
-        ctl.init(f.norm_cost, f.norm_rhs, op_norm_sq, prm.tolerance, prm.step_size_strategy);
-        if (ctl.converged(c.outs)) { b.converged = true; b.sol = 0; done = true; }
-        else done = ctl.iters >= prm.iter_limit;
-      } else {
-        if (c.fpe) ctl.restart_reference(c.outs + kHipBatchFpe);
-        restart = ctl.after_block(c.outs);
-        if (ctl.pfeas < ctl.tol * (1.0 + f.norm_rhs) && ctl.dfeas < ctl.tol * (1.0 + f.norm_cost) && ctl.relgap < ctl.tol) {
-          b.converged = true; b.sol = 1; done = true;
-        } else {
-          done = ctl.iters >= prm.iter_limit;
-        }
-      }
-      if (done) { c.active = 0; active--; continue; }
-      c.first = 0;
-      c.restart = restart ? 1 : 0;
-      c.fpe = ctl.pending_restart_fpe ? 1 : 0;
-      HipState& st = hst.p[i];
-      st.primal_step = ctl.primal_step; st.dual_step = ctl.dual_step; st.halpern_iteration = ctl.halpern_iteration;
-    }
-  }
-  CUDA_OK(cudaEventRecord(evl1, s));
-  CUDA_OK(cudaEventSynchronize(evl1));
-  float loop_ms = 0.f;
-  CUDA_OK(cudaEventElapsedTime(&loop_ms, evl0, evl1));
-  const double solve_seconds = std::chrono::duration<double>(clk::now() - t_loop).count();
+  std::vector<HipBatchRun*> R((size_t)count);
+  for (int i = 0; i < count; i++) R[i] = &B[i];
+  const BatchLoop loop = hip_batch_rounds(s, count, prm, dmem.p, R);
   lap("batch", "rounds");
 
   // ---- the host postsolve of every member (hip_host_postsolve, as the single solve's host prologue path), one download
   NvtxRange nvtx_post("b200pdlp: HiPDLP batch postsolve + download");
   CUDA_OK(cudaMemcpyAsync(hvec.data(), dvec.p, hvec.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
   CUDA_OK(cudaStreamSynchronize(s));
-  const double setup_seconds = std::chrono::duration<double>(t_loop - t_begin).count();
+  const double setup_seconds = std::chrono::duration<double>(loop.t_loop - t_begin).count();
   for_members(count, [&](int i) {
     const HipBatchHost& b = B[i];
     const StdForm& f = b.f;
-    const HipController& ctl = b.ctl;
     const int n = f.n, m = f.m;
     const double* v = hvec.data() + b.vec;
     const double* w = v + 14 * n;
@@ -3499,20 +3586,186 @@ static void solve_hipdlp_batch(int count, const b200pdlp_lp* lps, const b200pdlp
     const double* y = b.converged ? w + (b.sol ? 5 : 3) * m : nullptr;   // yn or y
     b200pdlp_result* out = outs + i;
     hip_host_postsolve(lps[i], f, b.L.cperm.data(), b.L.rperm.data(), x, y, v + 12 * n, v + 13 * n, out);
-    out->value_valid = 1; out->dual_valid = 1;
-    out->term_code = b.converged ? B200PDLP_OPTIMAL : B200PDLP_TIMELIMIT_OR_ITERLIMIT;
-    out->term_iterate = b.timed_out ? 2 : 0;
-    out->iters = ctl.iters; out->passes = ctl.iters; out->restarts = ctl.restarts;
-    out->kernel_launches = (int)std::min<long long>(rounds, 2147483647LL);
-    out->primal_obj = ctl.pobj; out->dual_obj = ctl.dobj; out->primal_feas = ctl.pfeas; out->dual_feas = ctl.dfeas;
-    out->gap = ctl.pobj - ctl.dobj; out->rel_gap = ctl.relgap;
-    out->setup_seconds = setup_seconds;
-    out->solve_seconds = solve_seconds;
-    out->loop_device_ms = loop_ms;
-    out->iter_device_ms = iter_ms;
-    out->form_cols = n; out->form_rows = m; out->form_nnz = f.nnz; out->form_neq = f.neq;
+    hip_batch_result(out, b, loop, setup_seconds);
   });
   lap("batch", "postsolve (host threads)");
+}
+
+// ------------------------------------------------------------------ HiPDLP batch of small LPs already on the GPU
+// b200pdlp_solve_hipdlp_batch_device: solve_hipdlp_batch for LPs whose arrays are device memory.  The prologue and the
+// postsolve run on the device, one CTA per member (batch_prep.cu hip_batch_*_kernel); the rounds are solve_hipdlp_batch's
+// (hip_batch_rounds).  The host reads one sizing record and |c|^2, |b|^2 per member, never an array.
+
+static void solve_hipdlp_batch_device(int count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params& prm, b200pdlp_result* outs) {
+  using clk = std::chrono::steady_clock;
+  const char* who = "b200pdlp_solve_hipdlp_batch_device";
+  const auto t_begin = clk::now();
+  Laps lap;
+  device_count_checked();
+  if (prm.device >= 0) CUDA_OK(cudaSetDevice(prm.device));
+  int device = 0;
+  CUDA_OK(cudaGetDevice(&device));
+  check_device_arrays(count, lps, nullptr, outs, device, who);
+  StreamHolder sh;
+  cudaStream_t s = sh.s;
+  DeviceBatch D;
+  PrepMode mode;
+  mode.hip = true; mode.scaling = prm.scaling_mode; mode.ruiz_iterations = prm.ruiz_iterations;
+  {
+    NvtxRange nvtx("b200pdlp: HiPDLP batch prologue (device)");
+    device_batch_prologue(s, count, lps, nullptr, mode, prm.ordered_max, who, D, lap);
+  }
+  const bool scaled = (prm.scaling_mode & 7) != 0;   // scale_hipdlp: any of its passes is switched on
+  std::vector<HipBatchRun> runs((size_t)count);
+  std::vector<HipBatchRun*> R((size_t)count);
+  std::vector<HipBatchMember> hmem((size_t)count);
+  for (int i = 0; i < count; i++) {
+    HipBatchRun& b = runs[i];
+    const BatchPrep& P = D.hp[i];
+    const double* r = D.rec.data() + (size_t)kPrepRec * i;
+    StdForm& f = b.f;
+    f.hipdlp = true;
+    f.n = P.n; f.m = P.m; f.nnz = P.nnz; f.neq = P.neq; f.n_orig = P.n0;
+    f.sense = lps[i].sense; f.offset = lps[i].offset;
+    f.norm_cost = std::sqrt(r[0]); f.norm_rhs = std::sqrt(r[1]);
+    f.scaled = scaled;
+    R[i] = &b;
+    hmem[i] = hip_batch_member(f, P.neq, P.vec, P.a_slices, P.a_col, P.a_val, P.at_slices, P.at_col, P.at_val);
+  }
+  DevBuf<HipBatchMember> dmem;
+  dmem.alloc(count, false);
+  CUDA_OK(cudaMemcpyAsync(dmem.p, hmem.data(), (size_t)count * sizeof(HipBatchMember), cudaMemcpyHostToDevice, s));
+  const BatchLoop loop = hip_batch_rounds(s, count, prm, dmem.p, R);
+  lap("batch device", "rounds");
+
+  // ---- the postsolve of every member on the device, into the caller's vectors
+  NvtxRange nvtx_post("b200pdlp: HiPDLP batch postsolve (device)");
+  std::vector<HipBatchPost> hpost((size_t)count);
+  for (int i = 0; i < count; i++) {
+    HipBatchPost& q = hpost[i];
+    q.col_value = outs[i].col_value; q.col_dual = outs[i].col_dual; q.row_value = outs[i].row_value; q.row_dual = outs[i].row_dual;
+    q.sol = runs[i].converged ? runs[i].sol : -1;
+    q.pad = 0;
+  }
+  DevBuf<HipBatchPost> dpost;
+  dpost.alloc(count, false);
+  CUDA_OK(cudaMemcpyAsync(dpost.p, hpost.data(), (size_t)count * sizeof(HipBatchPost), cudaMemcpyHostToDevice, s));
+  launch_hip_batch_post(s, count, D.prep.p, D.dhx.p, dpost.p, scaled ? 1 : 0);
+  CUDA_OK(cudaGetLastError());
+  CUDA_OK(cudaStreamSynchronize(s));
+  const double setup_seconds = std::chrono::duration<double>(loop.t_loop - t_begin).count();
+  for (int i = 0; i < count; i++) hip_batch_result(outs + i, runs[i], loop, setup_seconds);
+  lap("batch device", "postsolve (device)");
+}
+
+// ---- b200pdlp_debug_hipdlp_batch_prep_compare: the HiPDLP device prologue and postsolve against their host twins
+static const int kHipBatchPrepItems = 24;
+
+static void hipdlp_batch_prep_compare(int count, const b200pdlp_lp* lps, int scaling_mode, int ruiz_iterations, double* report) {
+  device_count_checked();
+  RawLps raw;
+  upload_raw_lps(count, lps, raw);
+  StreamHolder sh;
+  DeviceBatch D;
+  Laps lap;
+  PrepMode mode;
+  mode.hip = true; mode.scaling = scaling_mode; mode.ruiz_iterations = ruiz_iterations;
+  device_batch_prologue(sh.s, count, raw.dl.data(), nullptr, mode, std::numeric_limits<int>::max(),
+                        "b200pdlp_debug_hipdlp_batch_prep_compare", D, lap);
+  const bool scaled = (scaling_mode & 7) != 0;
+  std::vector<StdForm> F((size_t)count);
+  std::vector<HostLayout> Ls((size_t)count);
+  for (int i = 0; i < count; i++) {
+    const BatchPrep& P = D.hp[i];
+    StdForm& f = F[i];
+    HostLayout& L = Ls[i];
+    formulate_hipdlp(lps[i], f);
+    scale_hipdlp(f, scaling_mode, ruiz_iterations);
+    build_layout(f, 0, 1, std::numeric_limits<int>::max(), L);
+    double* rep = report + (size_t)kHipBatchPrepItems * i;
+    for (int k = 0; k < kHipBatchPrepItems; k++) rep[k] = 0.0;
+    rep[0] = (P.n != f.n) + (P.m != f.m) + (P.nnz != f.nnz) + (P.neq != f.neq);
+    if (rep[0] != 0.0) {   // nothing else lines up
+      for (int k = 1; k < kHipBatchPrepItems; k++) rep[k] = -1.0;
+      continue;
+    }
+    const int n = f.n, m = f.m;
+    const std::vector<double> v = download_vec(P.vec, hip_batch_vec_len(n, m));
+    const double* w = v.data() + 14 * (size_t)n;
+    rep[1] = bit_mismatches(v.data(), f.cost.data(), n);
+    rep[2] = bit_mismatches(v.data() + n, f.lower.data(), n);
+    rep[3] = bit_mismatches(v.data() + 2 * n, f.upper.data(), n);
+    rep[4] = bit_mismatches(w, f.rhs.data(), m);
+    rep[5] = bit_mismatches(w + m, f.row_upper.data(), m);
+    rep[6] = bit_mismatches(v.data() + 3 * n, f.col_scale.data(), n);
+    rep[7] = bit_mismatches(w + 2 * m, f.row_scale.data(), m);
+    rep[8] = bit_mismatches(download_vec(P.row_new_idx, m).data(), f.row_new_idx.data(), m);
+    rep[9] = bit_mismatches(download_vec(P.row_class, m).data(), reinterpret_cast<const int*>(f.row_class.data()), m);
+    auto sell = [&](const SellMatrix& H, const int4* sl, const int* col, const double* val, double* r) {
+      const size_t ns = H.slices.size(), ne = H.col.size();
+      const std::vector<int4> ds = download_vec(sl, ns);
+      r[0] = bit_mismatches(reinterpret_cast<const int4*>(H.slices.data()), ds.data(), ns);
+      if (r[0] != 0.0) { r[1] = r[2] = -1.0; return; }
+      r[1] = bit_mismatches(download_vec(col, ne).data(), H.col.data(), ne);
+      r[2] = bit_mismatches(download_vec(val, ne).data(), H.val.data(), ne);
+    };
+    sell(L.A, P.a_slices, P.a_col, P.a_val, rep + 10);
+    sell(L.AT, P.at_slices, P.at_col, P.at_val, rep + 13);
+    const double* r = D.rec.data() + (size_t)kPrepRec * i;
+    const double got[2] = {std::sqrt(r[0]), std::sqrt(r[1])};
+    const double want[2] = {f.norm_cost, f.norm_rhs};
+    for (int k = 0; k < 2; k++) rep[16 + k] = bit_mismatches(got + k, want + k, 1);
+    rep[18] = scaled != f.scaled;
+    for (int j = 0; j < n; j++) rep[19] += L.cperm[j] != j;   // the batch assumes identity orderings
+    for (int q = 0; q < m; q++) rep[19] += L.rperm[q] != q;
+  }
+  // the postsolve of a probe iterate (x, y, sp, sn; a converged member at the iteration-0 check) into fresh device vectors
+  std::vector<HipBatchPost> hpost((size_t)count);
+  std::vector<std::vector<double>> probes((size_t)count);
+  size_t nout = 0;
+  for (int i = 0; i < count; i++) nout += 2 * (size_t)D.hp[i].n0 + 2 * (size_t)D.hp[i].m;
+  DevBuf<double> dout;
+  dout.alloc(nout, false);
+  nout = 0;
+  for (int i = 0; i < count; i++) {
+    const BatchPrep& P = D.hp[i];
+    const int n = P.n, m = P.m, n0 = P.n0;
+    std::vector<double>& pr = probes[i];   // x, sp, sn (n each), y (m)
+    pr.resize(3 * (size_t)n + m);
+    for (size_t k = 0; k < pr.size(); k++) pr[k] = batch_probe(i, (int)k);
+    double* v = P.vec;
+    double* w = v + 14 * (size_t)n;
+    CUDA_OK(cudaMemcpy(v + 4 * (size_t)n, pr.data(), n * sizeof(double), cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemcpy(v + 12 * (size_t)n, pr.data() + n, 2 * (size_t)n * sizeof(double), cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemcpy(w + 3 * (size_t)m, pr.data() + 3 * n, m * sizeof(double), cudaMemcpyHostToDevice));
+    double* o = dout.p + nout;
+    hpost[i] = HipBatchPost{o, o + n0, o + 2 * n0, o + 2 * n0 + m, 0, 0};
+    nout += 2 * (size_t)n0 + 2 * (size_t)m;
+  }
+  DevBuf<HipBatchPost> dpost;
+  dpost.alloc(count, false);
+  dpost.upload(hpost.data(), count);
+  launch_hip_batch_post(sh.s, count, D.prep.p, D.dhx.p, dpost.p, scaled ? 1 : 0);
+  CUDA_OK(cudaGetLastError());
+  CUDA_OK(cudaStreamSynchronize(sh.s));
+  for (int i = 0; i < count; i++) {
+    double* rep = report + (size_t)kHipBatchPrepItems * i;
+    if (rep[0] != 0.0) continue;
+    const StdForm& f = F[i];
+    const HostLayout& L = Ls[i];
+    const int n = f.n, m = f.m, n0 = f.n_orig;
+    const double* pr = probes[i].data();
+    // (at least one element each: hip_host_postsolve writes nothing when a vector pointer is NULL)
+    std::vector<double> cv(std::max(n0, 1)), cd(std::max(n0, 1)), rv(std::max(m, 1)), rdual(std::max(m, 1));
+    b200pdlp_result res{};
+    res.col_value = cv.data(); res.col_dual = cd.data(); res.row_value = rv.data(); res.row_dual = rdual.data();
+    hip_host_postsolve(lps[i], f, L.cperm.data(), L.rperm.data(), pr, pr + 3 * n, pr + n, pr + 2 * n, &res);
+    const HipBatchPost& q = hpost[i];
+    rep[20] = bit_mismatches(download_vec(q.col_value, n0).data(), cv.data(), n0);
+    rep[21] = bit_mismatches(download_vec(q.col_dual, n0).data(), cd.data(), n0);
+    rep[22] = bit_mismatches(download_vec(q.row_value, m).data(), rv.data(), m);
+    rep[23] = bit_mismatches(download_vec(q.row_dual, m).data(), rdual.data(), m);
+  }
 }
 
 
@@ -3934,7 +4187,7 @@ int b200pdlp_solve_batch_device(int32_t count, const b200pdlp_lp* lps, const b20
     if (count == 0) return;
     if (!lps || !params || !outs) throw Error(B200PDLP_ERR_ARG, "b200pdlp_solve_batch_device: null argument");
     check_params(*params);
-    for (int i = 0; i < count; i++) check_batch_device_member(&lps[i], *params, i);
+    for (int i = 0; i < count; i++) check_batch_device_member(&lps[i], params->ordered_max, i, "b200pdlp_solve_batch_device");
     solve_batch_device(count, lps, *params, warms, outs);
     CUDA_OK(cudaGetLastError());
   });
@@ -3959,6 +4212,31 @@ int b200pdlp_solve_hipdlp_batch(int32_t count, const b200pdlp_lp* lps, const b20
     for (int i = 0; i < count; i++) check_hipdlp_batch_member(&lps[i], *params, i);
     solve_hipdlp_batch(count, lps, *params, outs);
     CUDA_OK(cudaGetLastError());
+  });
+}
+
+int b200pdlp_solve_hipdlp_batch_device(int32_t count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params* params,
+                                       b200pdlp_result* outs) {
+  DeviceGuard dg;
+  return guarded([&] {
+    const char* who = "b200pdlp_solve_hipdlp_batch_device";
+    if (count < 0) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": count < 0");
+    if (count == 0) return;
+    if (!lps || !params || !outs) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": null argument");
+    for (int i = 0; i < count; i++) check_batch_device_member(&lps[i], params->ordered_max, i, who);
+    solve_hipdlp_batch_device(count, lps, *params, outs);
+    CUDA_OK(cudaGetLastError());
+  });
+}
+
+int b200pdlp_debug_hipdlp_batch_prep_compare(int32_t count, const b200pdlp_lp* lps, int32_t scaling_mode, int32_t ruiz_iterations,
+                                             double* report) {
+  DeviceGuard dg;
+  return guarded([&] {
+    if (count < 0 || (count > 0 && (!lps || !report)))
+      throw Error(B200PDLP_ERR_ARG, "b200pdlp_debug_hipdlp_batch_prep_compare: bad arguments");
+    for (int i = 0; i < count; i++) check_lp(&lps[i]);
+    if (count > 0) hipdlp_batch_prep_compare(count, lps, scaling_mode, ruiz_iterations, report);
   });
 }
 

@@ -308,6 +308,29 @@ int b200pdlp_solve_hipdlp(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params* p
  * oracle), tools/batch_bench.py --solver hipdlp. */
 int b200pdlp_solve_hipdlp_batch(int32_t count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params* params,
                                 b200pdlp_result* outs /* [count], caller-allocated like b200pdlp_result */);
+/* b200pdlp_solve_hipdlp_batch for LPs that are already in GPU memory.  `lps` and `outs` are host arrays of the usual structs,
+ * but every array pointer inside them is device (or managed) memory of params->device (< 0: the current device): the LP's
+ * eight arrays and the four result vectors.  num_col, num_row, sense and offset are host scalars.  Each member returns exactly
+ * what b200pdlp_solve_hipdlp_batch returns for it with the same arrays on the host (and so what b200pdlp_solve_hipdlp returns
+ * for it alone): term_code, term_iterate, iters, passes, restarts, the residual scalars, the form dimensions and the four
+ * vectors, bit for bit.  Batch-wide fields as in b200pdlp_solve_hipdlp_batch; setup_seconds covers validation, sizing and
+ * the device prologue.  device_prep is ignored.
+ * The prologue (formulate_hipdlp, scale_hipdlp, the ordered layouts) and the postsolve run on the device, one CTA per member;
+ * the host reads one sizing record and two scalars per member, never an array.  A column whose stored rows repeat or descend
+ * is sorted by (row, value) on the device; should one row of a column hold both +0.0 and -0.0, -0.0 goes first (std::sort
+ * leaves that order unspecified; either order gives the same sums).  The call returns once the outputs are complete on the
+ * device; it never writes an input array.  The caller must have finished writing the inputs before the call (the library
+ * uses a stream of its own).
+ * Returns B200PDLP_ERR_ARG before any device work for count < 0, NULL arrays, ordered_max < 0 or a sense other than +-1;
+ * then, naming the member and the field, for a pointer that is not device memory of the device; then, before any solve
+ * work and naming the lowest failing member, for what b200pdlp_solve_hipdlp's checks reject in the arrays (a_start[0] != 0,
+ * a decreasing a_start, an a_index outside [0, num_row)) and for a standard form under HiPDLP's classification larger than
+ * ordered_max.  No result field or array is written on an error.  count == 0: B200PDLP_OK.  No device: B200PDLP_ERR_CUDA.
+ * The whole batch must fit in device memory (B200PDLP_ERR_ALLOC otherwise).
+ * STATUS: runs on hardware; tests/test_gpu_hipdlp_batch_device.py (byte equality with b200pdlp_solve_hipdlp_batch),
+ * tools/batch_device_bench.py --solver hipdlp. */
+int b200pdlp_solve_hipdlp_batch_device(int32_t count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params* params,
+                                       b200pdlp_result* outs /* [count]; vectors in device memory */);
 /* The HiPDLP solve on `ngpus` devices of THIS process (devices[g] or, if NULL, ordinals 0..ngpus-1; a device may repeat,
  * which gives logical shards on one device): the prologue, then each rank computes contiguous blocks of the one-GPU device
  * rows and columns, one host thread per rank, peer memory, no NCCL.  device_prep is honoured as on one GPU: 0 runs the
@@ -377,6 +400,17 @@ int b200pdlp_debug_prep_compare_hipdlp(const b200pdlp_lp* lp, int32_t scaling_mo
  *  rest if they differ), col, val  12-14 the same for A'  15 x0 16 y0 17 xsum  18 |c|_2 19 |b|_2 20 max|a_ij|  21, 22 the
  *  scaled |c|^2, |b|^2 that set beta  23 col_value 24 col_dual 25 row_value 26 row_dual */
 int b200pdlp_debug_batch_prep_compare(int32_t count, const b200pdlp_lp* lps, int32_t scaling, double* report);
+/* The device prologue and postsolve of b200pdlp_solve_hipdlp_batch_device (batch_prep.cu hip_batch_*_kernel) against their
+ * host twins: the `count` host LPs are uploaded as they are, prepared on the device (no ordered_max limit) and compared with
+ * formulate_hipdlp + scale_hipdlp + build_layout; then a fixed pseudo-random iterate (x, y and the slacks sp, sn of a member
+ * converged at iteration 0) is postsolved on both sides (hip_host_postsolve).
+ * report[24 * i + k] = mismatching entries (bit for bit) of member i:  0 n, m, nnz, neq (-1 everywhere else if they differ)
+ *  1 cost 2 lower 3 upper 4 rhs 5 row_upper 6 col_scale 7 row_scale  8 row_new_idx 9 row_class  10-12 A: slice descriptors
+ *  (-1 for the rest if they differ), col, val  13-15 the same for A'  16 |c|_2 17 |b|_2 of the unscaled form  18 1 if the
+ *  device batch and scale_hipdlp disagree on whether the form is scaled  19 entries of build_layout's column and row orderings
+ *  that are not the identity the batch assumes  20 col_value 21 col_dual 22 row_value 23 row_dual */
+int b200pdlp_debug_hipdlp_batch_prep_compare(int32_t count, const b200pdlp_lp* lps, int32_t scaling_mode, int32_t ruiz_iterations,
+                                             double* report);
 /* The device prologue of b200pdlp_solve_hipdlp_multi (block mode, all `world` ranks on the current device, 2 <= world <= 16)
  * against formulate_hipdlp + scale_hipdlp + plan_hipdlp_shards (ordered_max = -1) + build_hipdlp_shard.  report[8 + 9 world]
  * = mismatch counts:  0 n, m, nnz, neq (nothing else is compared if they differ)  1 vectors in device order (cost, lower,

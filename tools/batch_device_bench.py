@@ -1,7 +1,9 @@
-"""The batch on host arrays against the batch on LPs already in GPU memory: b200pdlp_solve_batch vs b200pdlp_solve_batch_device.
+"""The batch on host arrays against the batch on LPs already in GPU memory: b200pdlp_solve_batch vs b200pdlp_solve_batch_device
+(--solver hipdlp: b200pdlp_solve_hipdlp_batch vs b200pdlp_solve_hipdlp_batch_device).
 
 Workload (as tools/batch_bench.py): every ordered-mode instance of tests/golden/instances (standard form max(n, m) <= 4096),
 replicated R times, at the default tolerances and at kkt_tolerance 1e-4, each bounded by --iter-limit PDHG iterations.
+With --solver hipdlp the instances are those whose HiPDLP standard form is ordered, and 1e-4 is HiPDLP's tolerance.
 Three arms:
   host      solve_batch on host arrays (prologue and postsolve on host threads)
   device    solve_batch_device on LPs already resident on the GPU (prologue and postsolve on the device)
@@ -9,7 +11,7 @@ Three arms:
 After one warm-up of each arm, the arms run in alternating order --repeats times; all must return identical bits.  One more
 call of the device arm with B200PDLP_TIMING=1 gives its laps (validation + sizing, device prologue, rounds, postsolve).
 Prints one JSON line with the card's name, power limit and max SM clock read in the same run.
-    python tools/batch_device_bench.py [--replicas 8] [--iter-limit 500] [--repeats 2]
+    python tools/batch_device_bench.py [--solver pdlp|hipdlp] [--replicas 8] [--iter-limit 500] [--repeats 2]
 """
 import argparse
 import glob
@@ -82,39 +84,45 @@ def main():
     ap.add_argument("--replicas", type=int, default=8)
     ap.add_argument("--iter-limit", type=int, default=500)
     ap.add_argument("--repeats", type=int, default=2)
+    ap.add_argument("--solver", choices=("pdlp", "hipdlp"), default="pdlp")
     a = ap.parse_args()
+    hip = a.solver == "hipdlp"
+    solve_host = engine.solve_hipdlp_batch if hip else engine.solve_batch
+    solve_device = engine.solve_hipdlp_batch_device if hip else engine.solve_batch_device
     if engine.device_count() == 0:
         sys.exit("batch_device_bench.py needs a CUDA device")
     import torch
     lps = []
     for p in sorted(glob.glob(os.path.join(ROOT, "tests", "golden", "instances", "*.b2lp"))):
         lp = read_b2lp(p)
-        f = engine.host_form(lp, 1)
+        f = engine.host_form_hipdlp(lp) if hip else engine.host_form(lp, 1)
         if max(f["n"], f["m"]) <= 4096:
             lps.append(lp)
     work = lps * a.replicas
     resident = [engine.lp_to_device(lp, 0) for lp in work]
     torch.cuda.synchronize()
-    result = dict(card(), instances=len(lps), replicas=a.replicas, members=len(work), iter_limit=a.iter_limit,
-                  repeats=a.repeats, workloads=[])
+    result = dict(card(), **(dict(solver="hipdlp") if hip else {}), instances=len(lps), replicas=a.replicas, members=len(work),
+                  iter_limit=a.iter_limit, repeats=a.repeats, workloads=[])
     for name, tol in (("default", None), ("kkt1e-4", 1e-4)):
         kw = dict(iter_limit=a.iter_limit)
-        if tol:
+        if tol and hip:
+            kw.update(tolerance=tol)
+        elif tol:
             kw.update(tol_primal=tol, tol_dual=tol, tol_gap=tol)
 
         def run_host():
             t = time.perf_counter()
-            r = engine.solve_batch(work, **kw)
+            r = solve_host(work, **kw)
             return time.perf_counter() - t, r
 
         def run_device():
             t = time.perf_counter()
-            r = engine.solve_batch_device(resident, **kw)
+            r = solve_device(resident, **kw)
             return time.perf_counter() - t, r
 
         def run_upload():
             t = time.perf_counter()
-            r = engine.solve_batch_device([engine.lp_to_device(lp, 0) for lp in work], **kw)
+            r = solve_device([engine.lp_to_device(lp, 0) for lp in work], **kw)
             r = [host_vectors(x) for x in r]
             return time.perf_counter() - t, r
 
@@ -133,8 +141,8 @@ def main():
             ref = got["host"]
             for k in ("device", "upload"):
                 same = same and all(identical(host_vectors(x), y) for x, y in zip(got[k], ref))
-        dev_result = engine.solve_batch_device(resident, **kw)
-        laps = timing_laps(lambda: engine.solve_batch_device(resident, **kw))
+        dev_result = solve_device(resident, **kw)
+        laps = timing_laps(lambda: solve_device(resident, **kw))
         best = {k: min(v) for k, v in times.items()}
         result["workloads"].append(dict(
             name=name, identical_bits=same, pdhg_iterations=sum(r["iters"] for r in dev_result),
