@@ -18,34 +18,14 @@
 // 1-norm column-ascending by the thread that owns the row, |c|^2 and |b|^2 in index order by one thread.
 #include "batch_prep.hpp"
 #include "host_prep.hpp"
+#include "row_index.cuh"
 
 namespace b200 {
 namespace {
 
 constexpr double kInf = __builtin_huge_val();
 
-// in-place exclusive scan of a[0], a[stride], ... a[(len - 1) * stride] by one CTA (each thread owns a contiguous chunk);
-// returns the total in every thread.  sm: kThreads + 1 ints of shared memory.
-__device__ int block_scan(int* a, int stride, int len, int* sm) {
-  const int t = threadIdx.x;
-  const int chunk = (len + kThreads - 1) / kThreads;
-  const int b = min(t * chunk, len), e = min(b + chunk, len);
-  int s = 0;
-  for (int i = b; i < e; i++) s += a[(size_t)i * stride];
-  sm[t] = s;
-  __syncthreads();
-  if (t == 0) {
-    int run = 0;
-    for (int k = 0; k < kThreads; k++) { const int v = sm[k]; sm[k] = run; run += v; }
-    sm[kThreads] = run;
-  }
-  __syncthreads();
-  int run = sm[t];
-  for (int i = b; i < e; i++) { const int v = a[(size_t)i * stride]; a[(size_t)i * stride] = run; run += v; }
-  const int total = sm[kThreads];
-  __syncthreads();
-  return total;
-}
+// (block_scan and row_walk, which build the row-major indexes: row_index.cuh)
 
 // max over the CTA with std::max's comparison ((a < b) ? b : a); result in every thread
 __device__ double block_max(double v, double* sm) {
@@ -449,29 +429,9 @@ __global__ void __launch_bounds__(kThreads) batch_post_kernel(const BatchPrep* _
 }
 
 // ===================================================================================== HiPDLP batch
-// the row-major index by one warp (build_row_index): position p of row[p] goes to slot rwork[row[p]]++, positions ascending.
-// The warp walks the positions in order, 32 at a time; lanes that hit the same row take consecutive slots in lane order.
-// (batch_prep_kernel keeps this walk and form_layouts' two bodies written out in place, so that its machine code stays as
-// it was; the HiPDLP kernel calls them.)
-__device__ __forceinline__ void row_walk(int nnz, const int* row, int* rwork, int* rpos) {
-  const int lane = threadIdx.x & 31;
-  for (int base = 0; base < nnz; base += 32) {
-    const int p = base + lane;
-    const int i = p < nnz ? row[p] : -1 - lane;
-    const unsigned same = __match_any_sync(0xffffffffu, i);
-    int q = 0;
-    if (p < nnz) q = rwork[i] + __popc(same & ((1u << lane) - 1u));
-    __syncwarp();
-    if (p < nnz) {
-      rpos[q] = p;
-      if (lane == __ffs(same) - 1) rwork[i] += __popc(same);
-    }
-    __syncwarp();
-  }
-}
-
 // the ordered sliced-ELL bodies of the form (build_layout, identity orderings, no long rows): A's rows in the row-major
-// index's order; A' row j = column j sorted by row, stably (build_col_major)
+// index's order; A' row j = column j sorted by row, stably (build_col_major).  (batch_prep_kernel keeps the two bodies written
+// out in place, so that its machine code stays as it was; the HiPDLP kernel calls this.)
 __device__ __forceinline__ void form_layouts(const BatchPrep& P, int m, int n, int* sm) {
   sell_body(m, P.a_slices, P.a_col, P.a_val, sm, [&](int r) { return P.rptr[r + 1] - P.rptr[r]; },
             [&](int r, int* c, double* v) {

@@ -31,6 +31,7 @@
 #include "batch_prep.hpp"
 #include "device_prep.hpp"
 #include "host_prep.hpp"
+#include "kkt_batch.hpp"
 #include "pdhg_kernels.hpp"
 
 namespace b200 {
@@ -3768,6 +3769,194 @@ static void hipdlp_batch_prep_compare(int count, const b200pdlp_lp* lps, int sca
   }
 }
 
+// ====================================================================================== KKT assessment of a batch
+// b200pdlp_kkt_check_batch / _device: kkt_batch.cu's kernel assesses every member at once (one CTA each); the host reads one
+// record per member and runs finalize_kkt on it, so the derived fields and the status rules are those of the single checks.
+
+// the checks of a member that read no array: its lengths, and no NULL array whose length is positive (the matrix arrays,
+// whose length is a_start[num_col], are checked with the other array checks)
+static void check_kkt_batch_member(const b200pdlp_lp& lp, const b200pdlp_solution& x, int i, const char* who) {
+  const std::string at = std::string(who) + ": member " + std::to_string(i) + ": ";
+  if (lp.num_col < 0 || lp.num_row < 0) throw Error(B200PDLP_ERR_ARG, at + "num_col < 0 or num_row < 0");
+  const bool cols = lp.num_col > 0, rows = lp.num_row > 0;
+  if (!lp.a_start || (cols && !(lp.col_cost && lp.col_lower && lp.col_upper && x.col_value && x.col_dual)) ||
+      (rows && !(lp.row_lower && lp.row_upper && x.row_value && x.row_dual)))
+    throw Error(B200PDLP_ERR_ARG, at + "NULL array of positive length");
+}
+
+// the array checks of kkt_batch_check_kernel on host arrays (a BatchPrepErr)
+static int kkt_batch_host_arrays(const b200pdlp_lp& lp) {
+  if (lp.a_start[0] != 0) return kPrepStart0;
+  for (int j = 0; j < lp.num_col; j++)
+    if (lp.a_start[j + 1] < lp.a_start[j]) return kPrepDecreasing;
+  const int nnz = lp.a_start[lp.num_col];
+  if (nnz > 0 && (!lp.a_index || !lp.a_value)) return kPrepNull;
+  for (int p = 0; p < nnz; p++)
+    if ((unsigned)lp.a_index[p] >= (unsigned)lp.num_row) return kPrepIndex;
+  return kPrepOk;
+}
+
+// device_arrays: every array of lps / sols is device memory of the device (b200pdlp_kkt_check_batch_device).  Otherwise they
+// are host arrays that have passed kkt_batch_host_arrays, and the call uploads them with the members' descriptors in one copy.
+static void kkt_check_batch(int count, const b200pdlp_lp* lps, const b200pdlp_solution* sols, const KktTolerances& t,
+                            int device, bool device_arrays, const char* who, b200pdlp_kkt_info* inout, Laps& lap) {
+  device_count_checked();
+  if (device >= 0) CUDA_OK(cudaSetDevice(device));
+  int dev = 0;
+  CUDA_OK(cudaGetDevice(&dev));
+  NvtxRange nvtx("b200pdlp: KKT check batch");
+  StreamHolder sh;
+  cudaStream_t s = sh.s;
+  std::vector<KktBatchMember> hm((size_t)count);
+  for (int i = 0; i < count; i++) {
+    const b200pdlp_lp& lp = lps[i];
+    const b200pdlp_solution& x = sols[i];
+    KktBatchMember& M = hm[i];
+    M.n = lp.num_col; M.m = lp.num_row; M.sense = lp.sense;
+    M.a_start = lp.a_start; M.a_index = lp.a_index; M.a_value = lp.a_value;
+    M.col_cost = lp.col_cost; M.col_lower = lp.col_lower; M.col_upper = lp.col_upper;
+    M.row_lower = lp.row_lower; M.row_upper = lp.row_upper;
+    M.col_value = x.col_value; M.col_dual = x.col_dual; M.row_value = x.row_value; M.row_dual = x.row_dual;
+  }
+  const size_t head = (size_t)count * sizeof(KktBatchMember);
+  DevBuf<char> pack;   // the descriptors, then (host arrays) every member's doubles and ints
+  std::vector<int> nnz((size_t)count);
+  if (device_arrays) {
+    for (int i = 0; i < count; i++) {
+      const b200pdlp_lp& lp = lps[i];
+      const b200pdlp_solution& x = sols[i];
+      check_device_array(lp.a_start, dev, i, "a_start", who);
+      check_device_array(lp.a_index, dev, i, "a_index", who);
+      check_device_array(lp.a_value, dev, i, "a_value", who);
+      check_device_array(lp.col_cost, dev, i, "col_cost", who);
+      check_device_array(lp.col_lower, dev, i, "col_lower", who);
+      check_device_array(lp.col_upper, dev, i, "col_upper", who);
+      check_device_array(lp.row_lower, dev, i, "row_lower", who);
+      check_device_array(lp.row_upper, dev, i, "row_upper", who);
+      check_device_array(x.col_value, dev, i, "col_value", who);
+      check_device_array(x.col_dual, dev, i, "col_dual", who);
+      check_device_array(x.row_value, dev, i, "row_value", who);
+      check_device_array(x.row_dual, dev, i, "row_dual", who);
+    }
+    // the array checks on the device, and nnz for the workspace: one record per member
+    pack.alloc(head, false);
+    DevBuf<KktBatchSize> dsize;
+    dsize.alloc(count, false);
+    CUDA_OK(cudaMemcpyAsync(pack.p, hm.data(), head, cudaMemcpyHostToDevice, s));
+    launch_kkt_batch_check(s, count, reinterpret_cast<const KktBatchMember*>(pack.p), dsize.p);
+    CUDA_OK(cudaGetLastError());
+    std::vector<KktBatchSize> sz((size_t)count);
+    CUDA_OK(cudaMemcpyAsync(sz.data(), dsize.p, (size_t)count * sizeof(KktBatchSize), cudaMemcpyDeviceToHost, s));
+    CUDA_OK(cudaStreamSynchronize(s));
+    for (int i = 0; i < count; i++) {   // the lowest failing member
+      if (sz[i].err != kPrepOk)
+        throw Error(B200PDLP_ERR_ARG, std::string(who) + ": member " + std::to_string(i) + ": " + prep_error_text(sz[i].err));
+      nnz[i] = sz[i].nnz;
+    }
+    lap("kkt batch", "validation");
+  } else {
+    for (int i = 0; i < count; i++) nnz[i] = lps[i].a_start[lps[i].num_col];
+  }
+
+  // ---- the workspace: rptr [m + 1], rpos and colof [nnz] (ints); rres [m], cres [n] (doubles)
+  size_t ni = 0, nd = 0;
+  for (int i = 0; i < count; i++) {
+    ni += (size_t)hm[i].m + 1 + 2 * (size_t)nnz[i];
+    nd += (size_t)hm[i].n + hm[i].m;
+  }
+  DevBuf<int> wi;
+  DevBuf<double> wd;
+  DevBuf<KktBatchRec> drec;
+  wi.alloc(ni, false); wd.alloc(nd, false); drec.alloc(count, false);
+  ni = nd = 0;
+  for (int i = 0; i < count; i++) {
+    KktBatchMember& M = hm[i];
+    M.rptr = wi.p + ni; M.rpos = M.rptr + M.m + 1; M.colof = M.rpos + nnz[i];
+    ni += (size_t)M.m + 1 + 2 * (size_t)nnz[i];
+    M.rres = wd.p + nd; M.cres = M.rres + M.m;
+    nd += (size_t)M.n + M.m;
+  }
+  if (device_arrays) {
+    CUDA_OK(cudaMemcpyAsync(pack.p, hm.data(), head, cudaMemcpyHostToDevice, s));
+  } else {
+    // one packed copy (per-array copies would cost more than the kernel): the descriptors, the doubles, the ints
+    size_t dbl = 0, ints = 0;
+    for (int i = 0; i < count; i++) {
+      dbl += (size_t)nnz[i] + 5 * (size_t)hm[i].n + 4 * (size_t)hm[i].m;
+      ints += (size_t)hm[i].n + 1 + nnz[i];
+    }
+    const size_t bytes = head + 8 * dbl + 4 * ints;
+    pack.alloc(bytes, false);
+    PinnedArray<char> stage(bytes);
+    double* hd = reinterpret_cast<double*>(stage.p + head);
+    int* hi = reinterpret_cast<int*>(stage.p + head + 8 * dbl);
+    const double* dd = reinterpret_cast<const double*>(pack.p + head);
+    const int* di = reinterpret_cast<const int*>(pack.p + head + 8 * dbl);
+    size_t od = 0, oi = 0;
+    auto put_d = [&](const double* src, size_t len) {
+      if (len) memcpy(hd + od, src, len * sizeof(double));
+      od += len;
+      return dd + od - len;
+    };
+    auto put_i = [&](const int* src, size_t len) {
+      if (len) memcpy(hi + oi, src, len * sizeof(int));
+      oi += len;
+      return di + oi - len;
+    };
+    for (int i = 0; i < count; i++) {
+      KktBatchMember& M = hm[i];
+      const size_t n = M.n, m = M.m, z = nnz[i];
+      M.a_start = put_i(M.a_start, n + 1); M.a_index = put_i(M.a_index, z); M.a_value = put_d(M.a_value, z);
+      M.col_cost = put_d(M.col_cost, n); M.col_lower = put_d(M.col_lower, n); M.col_upper = put_d(M.col_upper, n);
+      M.row_lower = put_d(M.row_lower, m); M.row_upper = put_d(M.row_upper, m);
+      M.col_value = put_d(M.col_value, n); M.col_dual = put_d(M.col_dual, n);
+      M.row_value = put_d(M.row_value, m); M.row_dual = put_d(M.row_dual, m);
+    }
+    memcpy(stage.p, hm.data(), head);
+    CUDA_OK(cudaMemcpyAsync(pack.p, stage.p, bytes, cudaMemcpyHostToDevice, s));
+    CUDA_OK(cudaStreamSynchronize(s));   // (`stage` goes back to the pinned cache at the end of this block)
+  }
+  lap("kkt batch", "upload");
+  launch_kkt_batch(s, count, reinterpret_cast<const KktBatchMember*>(pack.p), t, drec.p);
+  CUDA_OK(cudaGetLastError());
+  if (lap.on) CUDA_OK(cudaStreamSynchronize(s));
+  lap("kkt batch", "kernel");
+  PinnedArray<KktBatchRec> rec((size_t)count);
+  CUDA_OK(cudaMemcpyAsync(rec.p, drec.p, (size_t)count * sizeof(KktBatchRec), cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaStreamSynchronize(s));
+  lap("kkt batch", "read-back");
+  // inout is written only now, when nothing can fail any more
+  std::vector<b200pdlp_kkt_info> out(inout, inout + count);
+  for (int i = 0; i < count; i++) {
+    out[i].norm_bounds = rec.p[i].norm_bounds;
+    out[i].norm_costs = rec.p[i].norm_costs;
+    finalize_kkt(rec.p[i].sums, lps[i].offset, t, &out[i]);
+  }
+  std::copy(out.begin(), out.end(), inout);
+}
+
+static int kkt_check_batch_entry(bool device_arrays, int count, const b200pdlp_lp* lps, const b200pdlp_solution* sols,
+                                 const b200pdlp_kkt_tolerances* tol, int device, b200pdlp_kkt_info* inout) {
+  DeviceGuard dg;
+  const char* who = device_arrays ? "b200pdlp_kkt_check_batch_device" : "b200pdlp_kkt_check_batch";
+  return guarded([&] {
+    Laps lap;
+    if (count < 0) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": count < 0");
+    if (count == 0) return;
+    if (!lps || !sols || !tol || !inout) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": null argument");
+    for (int i = 0; i < count; i++) check_kkt_batch_member(lps[i], sols[i], i, who);
+    if (!device_arrays) {   // the array checks of host arrays: on the host, before any device work
+      for (int i = 0; i < count; i++) {
+        const int err = kkt_batch_host_arrays(lps[i]);
+        if (err != kPrepOk)
+          throw Error(B200PDLP_ERR_ARG, std::string(who) + ": member " + std::to_string(i) + ": " + prep_error_text(err));
+      }
+      lap("kkt batch", "validation");
+    }
+    kkt_check_batch(count, lps, sols, tolerances_of(tol), device, device_arrays, who, inout, lap);
+  });
+}
+
 
 extern "C" {
 
@@ -4227,6 +4416,16 @@ int b200pdlp_solve_hipdlp_batch_device(int32_t count, const b200pdlp_lp* lps, co
     solve_hipdlp_batch_device(count, lps, *params, outs);
     CUDA_OK(cudaGetLastError());
   });
+}
+
+int b200pdlp_kkt_check_batch(int32_t count, const b200pdlp_lp* lps, const b200pdlp_solution* sols,
+                             const b200pdlp_kkt_tolerances* tol, int32_t device, b200pdlp_kkt_info* inout) {
+  return kkt_check_batch_entry(false, count, lps, sols, tol, device, inout);
+}
+
+int b200pdlp_kkt_check_batch_device(int32_t count, const b200pdlp_lp* lps, const b200pdlp_solution* sols,
+                                    const b200pdlp_kkt_tolerances* tol, int32_t device, b200pdlp_kkt_info* inout) {
+  return kkt_check_batch_entry(true, count, lps, sols, tol, device, inout);
 }
 
 int b200pdlp_debug_hipdlp_batch_prep_compare(int32_t count, const b200pdlp_lp* lps, int32_t scaling_mode, int32_t ruiz_iterations,

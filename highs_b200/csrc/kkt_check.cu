@@ -16,12 +16,14 @@
 
 #include "../../include/b200pdlp.h"
 #include "device_prep.hpp"
+#include "kkt_batch.hpp"
 #include "kkt_logic.hpp"
 
 namespace b200 {
 
-// ---- shared epilogue: HighsInfo fields + lpKktCheck's status rules for a solution without a basis (:1207-1323)
-static void finalize_kkt(const KktSums& s, double offset, const KktTolerances& t, b200pdlp_kkt_info* out) {
+// ---- shared epilogue (also of the batch, kkt_batch.hpp): HighsInfo fields + lpKktCheck's status rules for a solution
+// without a basis (:1207-1323)
+void finalize_kkt(const KktSums& s, double offset, const KktTolerances& t, b200pdlp_kkt_info* out) {
   out->objective_function_value = offset + s.objective;
   out->num_primal_infeasibilities = s.num_primal_infeasibility;
   out->max_primal_infeasibility = s.max_primal_infeasibility;
@@ -65,7 +67,7 @@ static void finalize_kkt(const KktSums& s, double offset, const KktTolerances& t
   out->model_status = status;
 }
 
-static KktTolerances tolerances_of(const b200pdlp_kkt_tolerances* t) {
+KktTolerances tolerances_of(const b200pdlp_kkt_tolerances* t) {
   return KktTolerances{t->primal_feasibility_tolerance, t->dual_feasibility_tolerance, t->primal_residual_tolerance,
                        t->dual_residual_tolerance, t->optimality_tolerance};
 }

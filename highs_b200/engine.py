@@ -80,7 +80,8 @@ ABI_SYMBOLS = [
     "b200pdlp_host_register", "b200pdlp_host_unregister", "b200pdlp_primal_step", "b200pdlp_dual_step", "b200pdlp_residuals",
     "b200pdlp_kkt_check", "b200pdlp_kkt_check_host", "b200pdlp_kkt_default_tolerances", "b200pdlp_solve_batch",
     "b200pdlp_solve_hipdlp_batch", "b200pdlp_solve_batch_device", "b200pdlp_debug_batch_prep_compare",
-    "b200pdlp_solve_hipdlp_batch_device", "b200pdlp_debug_hipdlp_batch_prep_compare",
+    "b200pdlp_solve_hipdlp_batch_device", "b200pdlp_debug_hipdlp_batch_prep_compare", "b200pdlp_kkt_check_batch",
+    "b200pdlp_kkt_check_batch_device",
 ]
 
 _lib = None
@@ -440,24 +441,99 @@ class CKktInfo(C.Structure):
             "primal_solution_status", "dual_solution_status", "model_status")])
 
 
+class CSolution(C.Structure):
+    _fields_ = [("col_value", _dp), ("col_dual", _dp), ("row_value", _dp), ("row_dual", _dp)]
+
+
+_SOLUTION_VECTORS = ("col_value", "col_dual", "row_value", "row_dual")
+
+
+def _kkt_tolerances(kkt_tolerance: float) -> CKktTolerances:
+    L = lib()
+    tol = CKktTolerances()
+    L.b200pdlp_kkt_default_tolerances.argtypes = [C.POINTER(CKktTolerances), C.c_double]
+    L.b200pdlp_kkt_default_tolerances.restype = None
+    L.b200pdlp_kkt_default_tolerances(C.byref(tol), float(kkt_tolerance))
+    return tol
+
+
 def kkt_check(lp: HighsLp, solution, kkt_tolerance: float = 0.0, model_status: int = 7, on_device: bool = True) -> dict:
     """lpKktCheck of a HighsSolution (b200pdlp_kkt_check on the GPU, b200pdlp_kkt_check_host = its host twin).
     `solution`: mapping with col_value, col_dual, row_value, row_dual; model_status: HighsModelStatus code from the solver."""
     L = lib()
     clp, keep = make_clp(lp)
-    tol = CKktTolerances()
-    L.b200pdlp_kkt_default_tolerances.argtypes = [C.POINTER(CKktTolerances), C.c_double]
-    L.b200pdlp_kkt_default_tolerances.restype = None
-    L.b200pdlp_kkt_default_tolerances(C.byref(tol), float(kkt_tolerance))
+    tol = _kkt_tolerances(kkt_tolerance)
     info = CKktInfo()
     info.model_status = int(model_status)
-    arrs = [np.ascontiguousarray(solution[k], dtype=np.float64) for k in ("col_value", "col_dual", "row_value", "row_dual")]
+    arrs = [np.ascontiguousarray(solution[k], dtype=np.float64) for k in _SOLUTION_VECTORS]
     fn = L.b200pdlp_kkt_check if on_device else L.b200pdlp_kkt_check_host
     fn.argtypes = [C.POINTER(CLp), _dp, _dp, _dp, _dp, C.POINTER(CKktTolerances), C.POINTER(CKktInfo)]
     rc = fn(C.byref(clp), *(_p(a, _dp) for a in arrs), C.byref(tol), C.byref(info))
     if rc != 0:
         raise EngineError(f"b200pdlp_kkt_check{'_host' if not on_device else ''} failed ({rc})")
     return {k: getattr(info, k) for k, _ in CKktInfo._fields_}
+
+
+def _kkt_statuses(model_status, count: int, what: str) -> list:
+    """model_status (one int, or one per LP) as a list of `count` ints"""
+    if isinstance(model_status, (int, np.integer)):
+        return [int(model_status)] * count
+    statuses = [int(s) for s in model_status]
+    if len(statuses) != count:
+        raise ValueError(f"{what}: {len(statuses)} model statuses for {count} LPs")
+    return statuses
+
+
+def _kkt_batch_call(name: str, count: int, clps, csols, kkt_tolerance: float, statuses, device: int) -> list:
+    L = lib()
+    fn = getattr(L, name)
+    fn.argtypes = [C.c_int32, C.POINTER(CLp), C.POINTER(CSolution), C.POINTER(CKktTolerances), C.c_int32, C.POINTER(CKktInfo)]
+    infos = (CKktInfo * max(count, 1))()
+    for i, s in enumerate(statuses):
+        infos[i].model_status = s
+    _check(fn(count, clps, csols, C.byref(_kkt_tolerances(kkt_tolerance)), device, infos), name)
+    return [{k: getattr(infos[i], k) for k, _ in CKktInfo._fields_} for i in range(count)]
+
+
+def kkt_check_batch(lps, sols, kkt_tolerance: float = 0.0, model_status=7, device: int = -1) -> list:
+    """b200pdlp_kkt_check_batch: kkt_check for every (LP, solution) pair in one call on one GPU, one CTA per LP.  `sols`:
+    mappings holding the four vectors as numpy arrays (the dicts of solve_batch and solve_hipdlp_batch work as they are);
+    model_status: one HighsModelStatus code for all, or one per LP.  Returns the dicts kkt_check returns, in order; each
+    equals kkt_check(lp, sol, on_device=False) for that pair, bit for bit (any NaN matching any NaN)."""
+    lps, sols = list(lps), list(sols)
+    if len(sols) != len(lps):
+        raise ValueError(f"kkt_check_batch: {len(sols)} solutions for {len(lps)} LPs")
+    count = len(lps)
+    statuses = _kkt_statuses(model_status, count, "kkt_check_batch")
+    clps, csols, keep = (CLp * max(count, 1))(), (CSolution * max(count, 1))(), []
+    for i, (lp, sol) in enumerate(zip(lps, sols)):
+        clps[i], k = make_clp(lp)
+        arrs = [np.ascontiguousarray(sol[v], dtype=np.float64) for v in _SOLUTION_VECTORS]
+        csols[i] = CSolution(*(_p(a, _dp) for a in arrs))
+        keep += [k, arrs]
+    return _kkt_batch_call("b200pdlp_kkt_check_batch", count, clps, csols, kkt_tolerance, statuses, device)
+
+
+def kkt_check_batch_device(dlps, sols, kkt_tolerance: float = 0.0, model_status=7) -> list:
+    """b200pdlp_kkt_check_batch_device: kkt_check_batch for LPs and solutions already in GPU memory -- `dlps` from
+    lp_to_device, `sols` mappings holding the four vectors as float64 CUDA tensors (the dicts of solve_batch_device and
+    solve_hipdlp_batch_device work as they are).  The device is that of the tensors.  torch's current stream is synchronised
+    first, so that inputs it is still writing are complete.  Returns the dicts kkt_check_batch returns."""
+    dlps, sols = list(dlps), list(sols)
+    if len(sols) != len(dlps):
+        raise ValueError(f"kkt_check_batch_device: {len(sols)} solutions for {len(dlps)} LPs")
+    count = len(dlps)
+    statuses = _kkt_statuses(model_status, count, "kkt_check_batch_device")
+    if count == 0:
+        return _kkt_batch_call("b200pdlp_kkt_check_batch_device", 0, None, None, kkt_tolerance, [], -1)
+    import torch
+    dev = dlps[0]["a_start"].device
+    clps, csols = (CLp * count)(), (CSolution * count)()
+    for i, (d, sol) in enumerate(zip(dlps, sols)):
+        clps[i] = make_clp_device(d)
+        csols[i] = CSolution(*(_dev_ptr(sol[v], torch.float64, _dp, v) for v in _SOLUTION_VECTORS))
+    torch.cuda.current_stream(dev).synchronize()
+    return _kkt_batch_call("b200pdlp_kkt_check_batch_device", count, clps, csols, kkt_tolerance, statuses, dev.index)
 
 
 def hipdlp_controller_replay(norm_cost, norm_rhs, op_norm_sq, tolerance, strategy, sums, restart_sums) -> np.ndarray:

@@ -455,6 +455,37 @@ int b200pdlp_kkt_check(const b200pdlp_lp* lp, const double* col_value, const dou
 int b200pdlp_kkt_check_host(const b200pdlp_lp* lp, const double* col_value, const double* col_dual, const double* row_value,
                             const double* row_dual, const b200pdlp_kkt_tolerances* tol, b200pdlp_kkt_info* inout);
 
+/* The four vectors of a HighsSolution, original LP space, HiGHS signs (what b200pdlp_result returns) */
+typedef struct {
+  const double* col_value;   /* [num_col] */
+  const double* col_dual;    /* [num_col] */
+  const double* row_value;   /* [num_row] */
+  const double* row_dual;    /* [num_row] */
+} b200pdlp_solution;
+
+/* The KKT assessment of `count` LP solutions in one call on one GPU (device < 0: the current device), one CTA per member:
+ * the output side of the batch solves.  inout[i].model_status is read (the HighsModelStatus code from the solver, as for
+ * b200pdlp_kkt_check); every other field is written.  `tol` is shared by all members.  Every member's b200pdlp_kkt_info
+ * equals what b200pdlp_kkt_check_host returns for it alone, field for field and bit for bit, except that a NaN may have
+ * another bit pattern.  There is no size limit: a large member only takes longer.
+ * b200pdlp_kkt_check_batch takes host arrays and uploads the whole batch in one copy; b200pdlp_kkt_check_batch_device
+ * requires every array pointer in lps[i] and sols[i] to be device (or managed) memory of the device, so the results of
+ * b200pdlp_solve_batch_device and b200pdlp_solve_hipdlp_batch_device can be passed as they are (num_col, num_row, sense and
+ * offset stay host scalars).  Neither call writes an input.  The caller must have finished writing device inputs before the
+ * call (the library uses a stream of its own).
+ * Errors, with nothing written to inout: B200PDLP_ERR_ARG before any device work for count < 0, NULL lps / sols / tol /
+ * inout, a member with num_col < 0 or num_row < 0, or a NULL array whose length is positive, naming the member (count == 0:
+ * B200PDLP_OK; no device: B200PDLP_ERR_CUDA); _device only: a pointer that is not device memory of the device, naming the
+ * member and the field; then, naming the lowest failing member, a_start[0] != 0, a decreasing a_start or an a_index outside
+ * [0, num_row) (the host variant checks these on the host before any device lookup); B200PDLP_ERR_ALLOC if the batch's
+ * workspace (about 4 (m + 1) + 8 nnz + 8 (n + m) bytes per member, and the uploaded arrays for the host variant) does not fit.
+ * STATUS: runs on hardware; tests/test_gpu_kkt_batch.py (bit equality with b200pdlp_kkt_check_host for every member),
+ * tools/kkt_batch_bench.py. */
+int b200pdlp_kkt_check_batch(int32_t count, const b200pdlp_lp* lps, const b200pdlp_solution* sols,
+                             const b200pdlp_kkt_tolerances* tol, int32_t device, b200pdlp_kkt_info* inout);
+int b200pdlp_kkt_check_batch_device(int32_t count, const b200pdlp_lp* lps, const b200pdlp_solution* sols,
+                                    const b200pdlp_kkt_tolerances* tol, int32_t device, b200pdlp_kkt_info* inout);
+
 /* Page-lock / unlock caller memory (cudaHostRegister) so that the copies of b200pdlp_solve run at PCIe speed; optional
  * (pageable buffers work, staged by the driver).  A host application that keeps its HighsLp / HighsSolution vectors for
  * many solves registers them once. */
