@@ -2283,6 +2283,60 @@ static void hip_host_postsolve(const b200pdlp_lp& lp, const StdForm& f, const in
   }
 }
 
+// PDLPSolver::powerMethod (pdhg.cc:1529-1671) on the device: 20 iterations of q <- A A'q / |A A'q| from the ones vector,
+// lambda = |A'q|^2; no host round trip inside (the norm stays on the device), one read-back at the end.  Several GPUs:
+// every rank holds q and z whole, forms its columns of w and its rows of z, and gathers them; the norms are then the
+// one-GPU sums over full vectors.  Uses dy, axp, atdy (and atyp on several GPUs) as scratch.
+static double hip_power_method(b200pdlp_problem* p) {
+  auto& h = p->hip;
+  cudaStream_t s = p->stream;
+  const int n = p->n, m = p->m;
+  const bool shard = hip_sharded(p);
+  const int r0 = p->hip_r0, c0 = p->hip_c0;
+  if (n == 0 || m == 0) return 1.0;
+  double* xq = h.dy.p;      // m-vectors: q (dy), z (axp); n-vector: w = A'q (atdy)
+  double* zq = h.axp.p;
+  double* wq = h.atdy.p;
+  // several GPUs: A'z goes to a second buffer, so that a rank's next A'q cannot overwrite a peer's A'z while that peer
+  // still sums it (no barrier lies between the two)
+  const HipVec wzv = shard ? &HipBufs::atyp : &HipBufs::atdy;
+  double* wz = (h.*wzv).p;
+  double* sc = p->outs.p + 16;
+  launch_fill(s, m, xq, 1.0);
+  for (int it = 0; it < 20; it++) {
+    launch_spmv_plain(s, p->AT.dev, xq, wq + c0);
+    if (shard) { hip_gather(p, true, {&HipBufs::atdy}); hip_barrier(p); }
+    launch_spmv_plain(s, p->A.dev, wq, zq + r0);
+    if (shard) { hip_gather(p, false, {&HipBufs::axp}); hip_barrier(p); }
+    launch_hip_dot(s, m, zq, zq, p->ordered ? 1 : 0, p->rs(kSlotChk, m), sc);
+    launch_hip_div_norm(s, m, zq, sc);
+    launch_spmv_plain(s, p->AT.dev, zq, wz + c0);
+    if (shard) { hip_gather(p, true, {wzv}); hip_barrier(p); }
+    launch_hip_dot(s, n, wz, wz, p->ordered ? 1 : 0, p->rs(kSlotChk, n), sc + 1);
+    CUDA_OK(cudaMemcpyAsync(xq, zq, (size_t)m * sizeof(double), cudaMemcpyDeviceToDevice, s));
+    p->launches += 6;
+  }
+  CUDA_OK(cudaMemcpyAsync(p->houts + 16, sc + 1, sizeof(double), cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaStreamSynchronize(s));
+  return p->houts[16];
+}
+
+// one row of b200pdlp_result::trace per block (B200PDLP_HIP_TRACE_COLS, include/b200pdlp.h) from the block-end check's sums
+// and the controller's decisions: host values the loop already holds, no device work
+static void hip_trace_row(b200pdlp_result* out, const HipController& ctl, const double* sums, bool restart, bool converged) {
+  if (!out->trace || out->trace_len >= out->trace_cap) return;
+  double* t = out->trace + (size_t)out->trace_len * B200PDLP_HIP_TRACE_COLS;
+  t[0] = ctl.iters;
+  for (int q = 0; q < 9; q++) t[1 + q] = sums[q];
+  t[10] = restart ? 1.0 : 0.0;
+  t[11] = restart ? ctl.primal_weight : 0.0;
+  t[12] = restart ? ctl.primal_step : 0.0;
+  t[13] = restart ? ctl.dual_step : 0.0;
+  t[14] = ctl.fpe;
+  t[15] = converged ? 1.0 : 0.0;
+  out->trace_len++;
+}
+
 static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, const b200pdlp_hipdlp_params& prm, b200pdlp_result* out) {
   NvtxRange nvtx("b200pdlp: solve (HiPDLP mode)");
   using clk = std::chrono::steady_clock;
@@ -2294,7 +2348,8 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
   const int n = p->n, m = p->m;
   const long long launches0 = p->launches;
   const bool shard = hip_sharded(p);
-  const int r0 = p->hip_r0, c0 = p->hip_c0;
+  const int c0 = p->hip_c0;
+  out->trace_len = 0;
   CudaEvent evl0, evl1;
   if (!h.graph) {   // steps 2 .. 40 of a block: 38 minor steps and the closing major step (:629-632)
     const long long l0 = p->launches;
@@ -2320,38 +2375,7 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
     CUDA_OK(cudaStreamSynchronize(s));
     p->group->arrive_and_wait();
   }
-  // PDLPSolver::powerMethod (pdhg.cc:1529-1671) on the device: 20 iterations of q <- A A'q / |A A'q| from the ones vector,
-  // lambda = |A'q|^2; no host round trip inside (the norm stays on the device), one read-back at the end.  Several GPUs:
-  // every rank holds q and z whole, forms its columns of w and its rows of z, and gathers them; the norms are then the
-  // one-GPU sums over full vectors.
-  double op_norm_sq = 1.0;
-  if (n > 0 && m > 0) {
-    double* xq = h.dy.p;      // m-vectors: q (dy), z (axp); n-vector: w = A'q (atdy)
-    double* zq = h.axp.p;
-    double* wq = h.atdy.p;
-    // several GPUs: A'z goes to a second buffer, so that a rank's next A'q cannot overwrite a peer's A'z while that peer
-    // still sums it (no barrier lies between the two)
-    const HipVec wzv = shard ? &HipBufs::atyp : &HipBufs::atdy;
-    double* wz = (h.*wzv).p;
-    double* sc = p->outs.p + 16;
-    launch_fill(s, m, xq, 1.0);
-    for (int it = 0; it < 20; it++) {
-      launch_spmv_plain(s, p->AT.dev, xq, wq + c0);
-      if (shard) { hip_gather(p, true, {&HipBufs::atdy}); hip_barrier(p); }
-      launch_spmv_plain(s, p->A.dev, wq, zq + r0);
-      if (shard) { hip_gather(p, false, {&HipBufs::axp}); hip_barrier(p); }
-      launch_hip_dot(s, m, zq, zq, p->ordered ? 1 : 0, p->rs(kSlotChk, m), sc);
-      launch_hip_div_norm(s, m, zq, sc);
-      launch_spmv_plain(s, p->AT.dev, zq, wz + c0);
-      if (shard) { hip_gather(p, true, {wzv}); hip_barrier(p); }
-      launch_hip_dot(s, n, wz, wz, p->ordered ? 1 : 0, p->rs(kSlotChk, n), sc + 1);
-      CUDA_OK(cudaMemcpyAsync(xq, zq, (size_t)m * sizeof(double), cudaMemcpyDeviceToDevice, s));
-      p->launches += 6;
-    }
-    CUDA_OK(cudaMemcpyAsync(p->houts + 16, sc + 1, sizeof(double), cudaMemcpyDeviceToHost, s));
-    CUDA_OK(cudaStreamSynchronize(s));
-    op_norm_sq = p->houts[16];
-  }
+  const double op_norm_sq = hip_power_method(p);
   HipController ctl;   // step sizes, fixed-point error, convergence test, restart criteria, PID weight (host_prep_hipdlp.cpp)
   ctl.init(f.norm_cost, f.norm_rhs, op_norm_sq, prm.tolerance, prm.step_size_strategy);
   // x = xa = proj_[l,u](0) (a kernel on the device-order bounds, upper first, then lower), y = ya = 0; A'y (:512-552)
@@ -2396,9 +2420,10 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
       if (prm.log_level >= 2)
         printf("[b200pdlp hipdlp] it %8d  pobj %+.8e dobj %+.8e  pfeas %.2e dfeas %.2e  fpe %.3e  weight %.3e\n", ctl.iters,
                ctl.pobj, ctl.dobj, ctl.pfeas, ctl.dfeas, ctl.fpe, ctl.primal_weight);
-      if (ctl.pfeas < ctl.tol * (1.0 + f.norm_rhs) && ctl.dfeas < ctl.tol * (1.0 + f.norm_cost) && ctl.relgap < ctl.tol) {
-        converged = true; sol_x = h.xn.p; sol_y = h.yn.p; break;
-      }
+      const bool block_converged =
+          ctl.pfeas < ctl.tol * (1.0 + f.norm_rhs) && ctl.dfeas < ctl.tol * (1.0 + f.norm_cost) && ctl.relgap < ctl.tol;
+      hip_trace_row(out, ctl, p->houts, restart, block_converged);
+      if (block_converged) { converged = true; sol_x = h.xn.p; sol_y = h.yn.p; break; }
       if (restart) {   // anchors and iterates <- the PDHG iterate of the last major step (:664-688)
         // (several GPUs: xn and yn were gathered by the check, so every rank copies them whole and holds full anchors)
         CUDA_OK(cudaMemcpyAsync(h.xa.p, h.xn.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, s));
@@ -4053,10 +4078,20 @@ int b200pdlp_problem_get_csr(const b200pdlp_problem* p, int32_t* rowptr, int32_t
   return B200PDLP_OK;
 }
 
+// A problem of b200pdlp_hipdlp_problem_create holds the HiPDLP iterate set only (hipdlp_buffers), and one of
+// b200pdlp_problem_create the pdlp one only: each family of entry points rejects the other's problems.
+static bool is_hipdlp_problem(const b200pdlp_problem* p) { return p->hip.state.p != nullptr; }
+static void require_mode(const b200pdlp_problem* p, bool hipdlp, const char* who) {
+  if (is_hipdlp_problem(p) == hipdlp) return;
+  throw Error(B200PDLP_ERR_ARG, std::string(who) + (hipdlp ? ": not a HiPDLP problem (create it with b200pdlp_hipdlp_problem_create)"
+                                                           : ": a HiPDLP problem (use the b200pdlp_hipdlp_* entry points)"));
+}
+
 int b200pdlp_spmv_ax(b200pdlp_problem* p, const double* x, double* ax) {
   DeviceGuard dg;
   return guarded([&] {
     if (!p || !x || !ax) throw Error(B200PDLP_ERR_ARG, "null argument");
+    require_mode(p, false, "b200pdlp_spmv_ax");
     set_device(p);
     ensure_host_maps(p);
     const size_t full = p->world == 1 ? (size_t)p->n : p->xfull.n;
@@ -4077,6 +4112,7 @@ int b200pdlp_spmv_aty(b200pdlp_problem* p, const double* y, double* aty) {
   DeviceGuard dg;
   return guarded([&] {
     if (!p || !y || !aty) throw Error(B200PDLP_ERR_ARG, "null argument");
+    require_mode(p, false, "b200pdlp_spmv_aty");
     set_device(p);
     ensure_host_maps(p);
     const size_t full = p->world == 1 ? (size_t)p->n : p->part.n;
@@ -4124,6 +4160,7 @@ int b200pdlp_primal_step(b200pdlp_problem* p, const double* x, const double* aty
   DeviceGuard dg;
   return guarded([&] {
     if (!p || !x || !aty || !x_new) throw Error(B200PDLP_ERR_ARG, "null argument");
+    require_mode(p, false, "b200pdlp_primal_step");
     if (p->world != 1) throw Error(B200PDLP_ERR_ARG, "kernel-level entry points are single-GPU");
     set_device(p);
     ensure_host_maps(p);
@@ -4152,6 +4189,7 @@ int b200pdlp_dual_step(b200pdlp_problem* p, const double* x_new, const double* y
   DeviceGuard dg;
   return guarded([&] {
     if (!p || !x_new || !y || !ax || !y_new || !ax_new) throw Error(B200PDLP_ERR_ARG, "null argument");
+    require_mode(p, false, "b200pdlp_dual_step");
     if (p->world != 1) throw Error(B200PDLP_ERR_ARG, "kernel-level entry points are single-GPU");
     set_device(p);
     ensure_host_maps(p);
@@ -4188,6 +4226,7 @@ int b200pdlp_residuals(b200pdlp_problem* p, const double* x, const double* y, do
   DeviceGuard dg;
   return guarded([&] {
     if (!p || !x || !y || !out) throw Error(B200PDLP_ERR_ARG, "null argument");
+    require_mode(p, false, "b200pdlp_residuals");
     if (p->world != 1) throw Error(B200PDLP_ERR_ARG, "kernel-level entry points are single-GPU");
     set_device(p);
     ensure_host_maps(p);
@@ -4221,6 +4260,7 @@ int b200pdlp_bench_spmv(b200pdlp_problem* p, int32_t which, int32_t reps, float*
   DeviceGuard dg;
   return guarded([&] {
     if (!p || !ms_total || reps < 1) throw Error(B200PDLP_ERR_ARG, "bad argument");
+    require_mode(p, false, "b200pdlp_bench_spmv");
     set_device(p);
     cudaEvent_t e0, e1;
     CUDA_OK(cudaEventCreate(&e0));
@@ -4245,6 +4285,7 @@ int b200pdlp_bench_pass(b200pdlp_problem* p, int32_t reps, float ms[4]) {
   DeviceGuard dg;
   return guarded([&] {
     if (!p || !ms || reps < 1) throw Error(B200PDLP_ERR_ARG, "bad argument");
+    require_mode(p, false, "b200pdlp_bench_pass");
     set_device(p);
     cudaStream_t s = p->stream;
     PdhgState* st = p->state.p;
@@ -4328,6 +4369,7 @@ int b200pdlp_problem_solve(b200pdlp_problem* p, const b200pdlp_params* params, c
   DeviceGuard dg;
   return guarded([&] {
     if (!p || !params || !out) throw Error(B200PDLP_ERR_ARG, "null argument");
+    require_mode(p, false, "b200pdlp_problem_solve");
     out->setup_seconds = 0.0;
     solve_on_device(p, *params, warm, out);
     CUDA_OK(cudaGetLastError());
@@ -4528,6 +4570,103 @@ int b200pdlp_solve_hipdlp(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params* p
     create_problem_hipdlp(*lp, *params, p.get());
     out->setup_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
     solve_hipdlp_on_device(p.get(), *lp, *params, out);
+    CUDA_OK(cudaGetLastError());
+  });
+}
+
+// ---- HiPDLP kernel-level entry points (tests): one Halpern step (hip_step), one check (hip_check) and the power method
+// (hip_power_method) of the solve, on host vectors in standard-form order, single GPU.  Like the pdlp ones they use the
+// problem's iterate buffers as scratch.
+static void hip_kernel_api(b200pdlp_problem* p, const char* who) {
+  if (!p) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": null problem");
+  require_mode(p, true, who);
+  if (p->world != 1 || hip_sharded(p)) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": kernel-level entry points are single-GPU");
+  set_device(p);
+  ensure_host_maps(p);
+  if ((int)p->cperm.size() != p->n || (int)p->rperm.size() != p->m)
+    throw Error(B200PDLP_ERR_STATE, std::string(who) + ": the problem has no host copy of its orderings");
+}
+// d[i] = v[perm[i]]: standard-form order -> device order
+static void hip_upload(b200pdlp_problem* p, double* d, const double* v, const std::vector<int>& perm) {
+  const int len = (int)perm.size();
+  if (len == 0) return;
+  std::vector<double> t(len);
+  for (int i = 0; i < len; i++) t[i] = v[perm[i]];
+  CUDA_OK(cudaMemcpyAsync(d, t.data(), (size_t)len * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+  CUDA_OK(cudaStreamSynchronize(p->stream));
+}
+static void hip_download(b200pdlp_problem* p, double* v, const double* d, const std::vector<int>& perm) {
+  const int len = (int)perm.size();
+  if (len == 0) return;
+  std::vector<double> t(len);
+  CUDA_OK(cudaMemcpyAsync(t.data(), d, (size_t)len * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+  CUDA_OK(cudaStreamSynchronize(p->stream));
+  for (int i = 0; i < len; i++) v[perm[i]] = t[i];
+}
+
+int b200pdlp_hipdlp_problem_create(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params* params, b200pdlp_problem** out) {
+  DeviceGuard dg;
+  return guarded([&] {
+    if (!params || !out) throw Error(B200PDLP_ERR_ARG, "b200pdlp_hipdlp_problem_create: null argument");
+    check_lp(lp);
+    ProblemPtr p(new b200pdlp_problem());
+    create_problem_hipdlp(*lp, *params, p.get());
+    *out = p.release();
+  });
+}
+
+int b200pdlp_hipdlp_step(b200pdlp_problem* p, double primal_step, double dual_step, int32_t halpern_iteration, int32_t k_offset,
+                         int32_t is_major, double* x, const double* xa, double* aty, double* y, const double* ya, double* rx,
+                         double* xn, double* hslack, double* yn, double* ry) {
+  DeviceGuard dg;
+  return guarded([&] {
+    if (!x || !xa || !aty || !y || !ya || !rx || !xn || !hslack || !yn || !ry)
+      throw Error(B200PDLP_ERR_ARG, "b200pdlp_hipdlp_step: null argument");
+    hip_kernel_api(p, "b200pdlp_hipdlp_step");
+    auto& h = p->hip;
+    const std::vector<int>&cp = p->cperm, &rp = p->rperm;
+    hip_upload(p, h.x.p, x, cp); hip_upload(p, h.xa.p, xa, cp); hip_upload(p, h.aty.p, aty, cp);
+    hip_upload(p, h.xn.p, xn, cp); hip_upload(p, h.hslack.p, hslack, cp);
+    hip_upload(p, h.y.p, y, rp); hip_upload(p, h.ya.p, ya, rp); hip_upload(p, h.yn.p, yn, rp); hip_upload(p, h.ry.p, ry, rp);
+    h.hstate->primal_step = primal_step; h.hstate->dual_step = dual_step; h.hstate->halpern_iteration = halpern_iteration;
+    CUDA_OK(cudaMemcpyAsync(h.state.p, h.hstate, sizeof(HipState), cudaMemcpyHostToDevice, p->stream));
+    hip_step(p, k_offset, is_major ? 1 : 0);
+    CUDA_OK(cudaGetLastError());
+    hip_download(p, x, h.x.p, cp); hip_download(p, rx, h.rx.p, cp); hip_download(p, aty, h.aty.p, cp);
+    hip_download(p, xn, h.xn.p, cp); hip_download(p, hslack, h.hslack.p, cp);
+    hip_download(p, y, h.y.p, rp); hip_download(p, yn, h.yn.p, rp); hip_download(p, ry, h.ry.p, rp);
+  });
+}
+
+int b200pdlp_hipdlp_check(b200pdlp_problem* p, int32_t major, const double* x, const double* y, const double* xa,
+                          const double* ya, const double* rx, const double* ry, const double* hslack, double out[9],
+                          double* sp, double* sn, double* ax, double* aty, double* atdy) {
+  DeviceGuard dg;
+  return guarded([&] {
+    if (!x || !y || !xa || !ya || !out || !sp || !sn || !ax || !aty || !atdy || (major && (!rx || !ry || !hslack)))
+      throw Error(B200PDLP_ERR_ARG, "b200pdlp_hipdlp_check: null argument");
+    hip_kernel_api(p, "b200pdlp_hipdlp_check");
+    auto& h = p->hip;
+    const std::vector<int>&cp = p->cperm, &rp = p->rperm;
+    hip_upload(p, major ? h.xn.p : h.x.p, x, cp); hip_upload(p, h.xa.p, xa, cp);
+    hip_upload(p, major ? h.yn.p : h.y.p, y, rp); hip_upload(p, h.ya.p, ya, rp);
+    if (major) { hip_upload(p, h.rx.p, rx, cp); hip_upload(p, h.hslack.p, hslack, cp); hip_upload(p, h.ry.p, ry, rp); }
+    hip_check(p, major ? 1 : 0);
+    CUDA_OK(cudaGetLastError());
+    for (int q = 0; q < 9; q++) out[q] = p->houts[q];
+    hip_download(p, sp, h.sp.p, cp); hip_download(p, sn, h.sn.p, cp);
+    hip_download(p, ax, h.axp.p, rp); hip_download(p, aty, h.atyp.p, cp);
+    if (major) hip_download(p, atdy, h.atdy.p, cp);
+    else std::fill(atdy, atdy + p->n, 0.0);
+  });
+}
+
+int b200pdlp_hipdlp_problem_power_method(b200pdlp_problem* p, double* lambda) {
+  DeviceGuard dg;
+  return guarded([&] {
+    if (!lambda) throw Error(B200PDLP_ERR_ARG, "b200pdlp_hipdlp_problem_power_method: null argument");
+    hip_kernel_api(p, "b200pdlp_hipdlp_problem_power_method");
+    *lambda = hip_power_method(p);
     CUDA_OK(cudaGetLastError());
   });
 }

@@ -81,8 +81,10 @@ ABI_SYMBOLS = [
     "b200pdlp_kkt_check", "b200pdlp_kkt_check_host", "b200pdlp_kkt_default_tolerances", "b200pdlp_solve_batch",
     "b200pdlp_solve_hipdlp_batch", "b200pdlp_solve_batch_device", "b200pdlp_debug_batch_prep_compare",
     "b200pdlp_solve_hipdlp_batch_device", "b200pdlp_debug_hipdlp_batch_prep_compare", "b200pdlp_kkt_check_batch",
-    "b200pdlp_kkt_check_batch_device",
+    "b200pdlp_kkt_check_batch_device", "b200pdlp_hipdlp_problem_create", "b200pdlp_hipdlp_step", "b200pdlp_hipdlp_check",
+    "b200pdlp_hipdlp_problem_power_method",
 ]
+HIP_TRACE_COLS = 16   # B200PDLP_HIP_TRACE_COLS: the per-block trace of the HiPDLP solves
 
 _lib = None
 
@@ -563,15 +565,16 @@ def _hipdlp_params(params) -> CHipdlpParams:
     return prm
 
 
-def solve_hipdlp(lp: HighsLp, **params) -> dict:
+def solve_hipdlp(lp: HighsLp, trace_cap: int = 0, **params) -> dict:
     """b200pdlp_solve_hipdlp: the HiPDLP mode (reflected Halpern PDHG, solver=hipdlp) on one GPU; parameters are the
     HighsOptions of the same meaning (tolerance, iter_limit, scaling_mode, ruiz_iterations, step_size_strategy ...), and
-    device_prep=-1 for the host prologue instead of the device-resident one."""
+    device_prep=-1 for the host prologue instead of the device-resident one.  trace_cap > 0: "trace" holds one row of
+    HIP_TRACE_COLS per block of 40 steps (include/b200pdlp.h, B200PDLP_HIP_TRACE_COLS)."""
     L = lib()
     L.b200pdlp_solve_hipdlp.argtypes = [C.POINTER(CLp), C.POINTER(CHipdlpParams), C.POINTER(CResult)]
     clp, keep = make_clp(lp)
     prm = _hipdlp_params(params)
-    res, arrays = _mk_result(lp, 0)
+    res, arrays = _mk_result(lp, trace_cap)
     _check(L.b200pdlp_solve_hipdlp(C.byref(clp), C.byref(prm), C.byref(res)), "b200pdlp_solve_hipdlp")
     return _result_dict(res, arrays)
 
@@ -838,6 +841,73 @@ class Problem:
         _check(lib().b200pdlp_problem_solve(self._h, C.byref(prm), C.byref(w) if w else None, C.byref(res)),
                "b200pdlp_problem_solve")
         return _result_dict(res, arrays)
+
+
+class HipProblem:
+    """Persistent HiPDLP problem for kernel-level tests (b200pdlp_hipdlp_problem_create): built as solve_hipdlp builds it
+    (same prologue choice and SpMV launch shapes), one GPU.  Vectors are numpy arrays in standard-form order."""
+
+    def __init__(self, lp: HighsLp, **params):
+        L = lib()
+        L.b200pdlp_hipdlp_problem_create.argtypes = [C.POINTER(CLp), C.POINTER(CHipdlpParams), C.POINTER(C.c_void_p)]
+        L.b200pdlp_hipdlp_step.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_int32, C.c_int32, C.c_int32] + [_dp] * 10
+        L.b200pdlp_hipdlp_check.argtypes = [C.c_void_p, C.c_int32] + [_dp] * 13
+        L.b200pdlp_hipdlp_problem_power_method.argtypes = [C.c_void_p, _dp]
+        self.lp = lp
+        self._clp, self._keep = make_clp(lp)
+        self._prm = _hipdlp_params(params)
+        self._h = C.c_void_p()
+        _check(L.b200pdlp_hipdlp_problem_create(C.byref(self._clp), C.byref(self._prm), C.byref(self._h)),
+               "b200pdlp_hipdlp_problem_create")
+        d = (C.c_int32 * 8)()
+        _check(L.b200pdlp_problem_dims(self._h, d), "b200pdlp_problem_dims")
+        self.n, self.m, self.nnz, self.neq = list(d)[:4]
+
+    def close(self):
+        if self._h:
+            lib().b200pdlp_problem_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _vec(self, v, length):
+        v = np.array(v, dtype=np.float64, copy=True)
+        assert v.shape == (length,), (v.shape, length)
+        return v
+
+    def step(self, primal_step, dual_step, halpern_iteration, k_offset, is_major, x, xa, aty, y, ya, xn=None, hslack=None,
+             yn=None, ry=None) -> dict:
+        """One Halpern step (b200pdlp_hipdlp_step).  xn, hslack, yn, ry default to NaN, which a minor step returns as
+        given.  Returns x, rx, xn, hslack, y, yn, ry and aty (= A'y of the new y)."""
+        n, m = self.n, self.m
+        v = dict(x=self._vec(x, n), xa=self._vec(xa, n), aty=self._vec(aty, n), y=self._vec(y, m), ya=self._vec(ya, m),
+                 rx=np.zeros(n), xn=self._vec(np.full(n, np.nan) if xn is None else xn, n),
+                 hslack=self._vec(np.full(n, np.nan) if hslack is None else hslack, n),
+                 yn=self._vec(np.full(m, np.nan) if yn is None else yn, m), ry=self._vec(np.full(m, np.nan) if ry is None else ry, m))
+        _check(lib().b200pdlp_hipdlp_step(self._h, float(primal_step), float(dual_step), int(halpern_iteration), int(k_offset),
+                                          int(is_major), *(_p(v[k], _dp) for k in ("x", "xa", "aty", "y", "ya", "rx", "xn",
+                                                                                   "hslack", "yn", "ry"))), "b200pdlp_hipdlp_step")
+        return {k: v[k] for k in ("x", "rx", "xn", "hslack", "y", "yn", "ry", "aty")}
+
+    def check(self, major, x, y, xa, ya, rx=None, ry=None, hslack=None) -> dict:
+        """One check (b200pdlp_hipdlp_check): "sums" = the nine sums, and the vectors sp, sn, ax, aty, atdy."""
+        n, m = self.n, self.m
+        ins = [self._vec(x, n), self._vec(y, m), self._vec(xa, n), self._vec(ya, m)]
+        ins += [self._vec(v, ln) if v is not None else None for v, ln in ((rx, n), (ry, m), (hslack, n))]
+        out = dict(sums=np.zeros(9), sp=np.zeros(n), sn=np.zeros(n), ax=np.zeros(m), aty=np.zeros(n), atdy=np.zeros(n))
+        _check(lib().b200pdlp_hipdlp_check(self._h, int(major), *(_p(v, _dp) if v is not None else None for v in ins),
+                                           *(_p(out[k], _dp) for k in ("sums", "sp", "sn", "ax", "aty", "atdy"))),
+               "b200pdlp_hipdlp_check")
+        return out
+
+    def power_method(self) -> float:
+        lam = C.c_double()
+        _check(lib().b200pdlp_hipdlp_problem_power_method(self._h, C.byref(lam)), "b200pdlp_hipdlp_problem_power_method")
+        return lam.value
 
 
 def nccl_unique_id() -> bytes:

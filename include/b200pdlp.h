@@ -123,6 +123,13 @@ typedef struct {
   int32_t trace_cap, trace_len;
 } b200pdlp_result;
 #define B200PDLP_TRACE_COLS 16
+/* The HiPDLP solves (b200pdlp_solve_hipdlp, _multi) write one row of B200PDLP_HIP_TRACE_COLS doubles per block of 40 steps
+ * instead, from the block-end check (no extra device work): 0 iterations, 1-9 the nine sums of the check (|x_next - refl_x|^2,
+ * |y_next - refl_y|^2, the fixed-point cross term, |primal residual|^2, |dual residual|^2, primal objective, dual objective,
+ * |x_next - x_anchor|^2, |y_next - y_anchor|^2; see b200pdlp_hipdlp_check), 10 restart decided, 11-13 primal weight, primal
+ * step, dual step after the restart's update (0 when there is no restart), 14 fixed-point error, 15 converged.  These are
+ * columns 0-9 and 14-19 of the HiPDLP oracle's trace (oracle/hipdlp_oracle.h). */
+#define B200PDLP_HIP_TRACE_COLS 16
 
 /* ---- whole solve: the function the HiGHS shim calls ------------------------ */
 void b200pdlp_default_params(b200pdlp_params* p);
@@ -354,6 +361,33 @@ int b200pdlp_hipdlp_controller_replay(double norm_cost, double norm_rhs, double 
 
 /* PDLPSolver::powerMethod (hipdlp/pdhg.cc:1529-1671): 20 iterations on A A' from the ones vector -> estimate of |A|_2^2 */
 int b200pdlp_hipdlp_power_method(const b200pdlp_form* f, double* lambda);
+
+/* ---- HiPDLP kernel-level entry points (parity tests; one GPU) ----------------------------------------------------------
+ * A persistent HiPDLP problem, built exactly as b200pdlp_solve_hipdlp builds it: the same prologue choice (ordered_max,
+ * device_prep, B200PDLP_DEVICE_PREP) and the same SpMV launch shapes (B200PDLP_TILE*, B200PDLP_SPMV_*; B200PDLP_TIMING=1
+ * prints the `SpMV shapes:` line).  b200pdlp_problem_destroy and b200pdlp_problem_dims serve it.  The pdlp entry points on a
+ * problem (spmv, primal / dual step, residuals, bench, problem_solve) reject it, and the functions below reject a problem of
+ * b200pdlp_problem_create: B200PDLP_ERR_ARG.  Every vector is a host array in standard-form order (the problem's device
+ * orderings are applied inside); the problem's iterate buffers serve as scratch.  No device: B200PDLP_ERR_CUDA. */
+int b200pdlp_hipdlp_problem_create(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params* params, b200pdlp_problem** out);
+/* One Halpern step of the solve (performHalpernPdhgStep, hipdlp/pdhg.cc:961-1018): the primal kernel, A * reflected x fused
+ * with the dual update, then A'y.  Weight w = k / (k + 1) with k = halpern_iteration + k_offset.  In/out: x, y (the blended
+ * iterate), aty (A'y of the input y on entry, of the new y on return); xn, hslack, yn, ry (written by a major step only, a
+ * minor step returns them as given).  Out: rx (the reflected x).  In: xa, ya (the anchors). */
+int b200pdlp_hipdlp_step(b200pdlp_problem* p, double primal_step, double dual_step, int32_t halpern_iteration, int32_t k_offset,
+                         int32_t is_major, double* x, const double* xa, double* aty, double* y, const double* ya, double* rx,
+                         double* xn, double* hslack, double* yn, double* ry);
+/* One check of the solve (the fixed-point error, convergence and PID sums) for the iterate (x, y) with anchors (xa, ya);
+ * major = 1 checks a major step's x_next = x, y_next = y with its reflected rx, ry and cached slack hslack (otherwise those
+ * may be NULL: the sums 0-2 are then 0 and the slacks are the projected dual residual).  out[9] = the nine sums
+ * (B200PDLP_HIP_TRACE_COLS columns 1-9; 5 and 6 include the objective offset), in the reference's order in ordered mode,
+ * as tree sums otherwise.  Also returns the vectors they were formed from: the slacks sp, sn, ax = A x, aty = A'y, and
+ * atdy = A'(y - ry) (zeros when major = 0). */
+int b200pdlp_hipdlp_check(b200pdlp_problem* p, int32_t major, const double* x, const double* y, const double* xa,
+                          const double* ya, const double* rx, const double* ry, const double* hslack, double out[9],
+                          double* sp, double* sn, double* ax, double* aty, double* atdy);
+/* The solve's device power method (20 iterations on A A' from the ones vector) -> its estimate of |A|_2^2 */
+int b200pdlp_hipdlp_problem_power_method(b200pdlp_problem* p, double* lambda);
 
 /* host-only (no GPU): build the device layout of rank `rank` of `world` exactly as b200pdlp_problem_create does
  * (row block, length-sorted device orderings, sliced ELL of A_g and A_g', long-row segments, segmented column

@@ -157,6 +157,15 @@ def hipdlp_solve(lp, tolerance=1e-7, max_iterations=2147483647, scaling_mode=5, 
                 trace=tr[: res.trace_len].copy())
 
 
+def hipdlp_set_sum_block(k: int):
+    """Test switch of the HiPDLP restatement (hip_set_sum_block): k > 0 adds its dot products in blocks of k, 0 restores
+    the reference's sequential order."""
+    L = lib()
+    L.hip_set_sum_block.argtypes = [C.c_int]
+    L.hip_set_sum_block.restype = None
+    L.hip_set_sum_block(int(k))
+
+
 class HipForm(C.Structure):
     _fields_ = [("n", C.c_int), ("m", C.c_int), ("nnz", C.c_int), ("neq", C.c_int),
                 ("cost", _dp), ("lower", _dp), ("upper", _dp), ("rlo", _dp), ("rup", _dp),

@@ -53,8 +53,23 @@ static void l_aty(const hip* s, const double* y, double* r) {          /* linalg
   for (int c = 0; c < s->n; c++)
     for (int p = s->cbeg[c]; p < s->cbeg[c + 1]; p++) r[c] += s->cval[p] * y[s->cidx[p]];
 }
+/* TEST SWITCH (not the reference's behaviour), like orc_set_sum_block in pdlp_oracle.c: hip_set_sum_block(k > 0) makes l_dot
+ * (and so l_norm2, the power method's norms and the residual norms of the checks) add in blocks of k elements and then add
+ * the block sums -- a different, equally valid rounding order, like the GPU engine's tree reductions.  Used to measure how
+ * far a mere change of summation order moves a HiPDLP trajectory (tests/test_gpu_hipdlp_kernels.py).  0: sequential. */
+static int g_sum_block = 0;
+void hip_set_sum_block(int k) { g_sum_block = k; }
 static double l_dot(int k, const double* a, const double* b) {         /* linalg.cc:63-73 */
   double r = 0.0;
+  if (g_sum_block > 0) {
+    for (int i0 = 0; i0 < k; i0 += g_sum_block) {
+      double t = 0.0;
+      const int i1 = i0 + g_sum_block < k ? i0 + g_sum_block : k;
+      for (int i = i0; i < i1; i++) t += a[i] * b[i];
+      r += t;
+    }
+    return r;
+  }
   for (int i = 0; i < k; i++) r += a[i] * b[i];
   return r;
 }

@@ -56,6 +56,9 @@ typedef struct {
 } hip_form;
 int hip_form_build(const orc_lp* lp, const hip_params* prm, hip_form* f);
 
+/* test switch: k > 0 makes the dot products add in blocks of k (another rounding order); 0 (default) = the reference's */
+void hip_set_sum_block(int k);
+
 #ifdef __cplusplus
 }
 #endif
