@@ -1,6 +1,6 @@
 // highs_b200/csrc/batch_kernels.cu -- batched ordered-mode PDHG (b200pdlp_solve_batch): one CTA owns one LP.
 //
-// A launch runs one ROUND for every unfinished member (engine.cu solve_batch drives the rounds):
+// A launch runs one ROUND for every unfinished member (engine_batch.cu solve_batch drives the rounds):
 //   1. the host's decision from the last check: a restart (average -> current when chosen, sums cleared, last-restart point
 //      taken) -- or, in round 0, the initial products A x0, A'y0 (after the power method of a fixed-step solve);
 //   2. PDHG passes until state.iter == state.stop_iter (K1..K4 of pdhg_kernels.cu, same arithmetic through pdhg_arith.cuh);
@@ -296,7 +296,7 @@ batch_round_kernel(const BatchMember* __restrict__ members, PdhgState* __restric
 }
 
 // ============================================================================================ HiPDLP batch
-// b200pdlp_solve_hipdlp_batch: one round of one member = what solve_hipdlp_on_device (engine.cu) enqueues between two of
+// b200pdlp_solve_hipdlp_batch: one round of one member = what solve_hipdlp_on_device (engine_hipdlp.cu) enqueues between two of
 // its host decisions, with the same per-element arithmetic (pdhg_arith.cuh):
 //   round 0    the power method (n > 0 and m > 0), x = xa = proj_[l,u](0), y = ya = 0, A'y, the iteration-0 check;
 //   round k    the restart decided after block k - 1 (anchors and iterates <- (xn, yn), A'y), step 1 (major), the three

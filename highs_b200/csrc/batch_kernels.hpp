@@ -16,6 +16,18 @@ struct BatchMember {
   double *y0, *y1, *ax0, *ax1, *ysum, *yavg, *axavg, *ylr;         // m-vectors
 };
 
+// A member's vectors lie in one block of doubles: its n-vectors, one slot of n doubles each, then its m-vectors, one slot of
+// m doubles each.  These slots are the only place the order is written; the host (engine_batch.cu) and the kernels of
+// batch_prep.cu address a block through them.  The two halves of each double buffer (x0 / x1, aty0 / aty1, y0 / y1,
+// ax0 / ax1) are adjacent, so the half of parity cur is slot k0 + cur.
+struct BatchVec {
+  enum Col { kCost, kLower, kUpper, kColscale, kX0, kX1, kAty0, kAty1, kXsum, kXavg, kAtyavg, kXlr, kCols };
+  enum Row { kRhs, kRowscale, kY0, kY1, kAx0, kAx1, kYsum, kYavg, kAxavg, kYlr, kRows };
+  static size_t len(int n, int m) { return (size_t)kCols * n + (size_t)kRows * m; }
+  template <class T> __host__ __device__ static T* col(T* v, int n, int k) { return v + k * n; }
+  template <class T> __host__ __device__ static T* row(T* v, int n, int m, int k) { return v + kCols * n + k * m; }
+};
+
 // Sums a check leaves in BatchCtl::outs (indices 0..31 are those of the one-problem ordered check in engine.cu run_check)
 //   0..13   column sweep A, 7 per iterate (current, average)     14..19  row sweep A, 3 per iterate
 //   24..29  column sweep B, 3 per iterate                         30..31  row sweep B, 1 per iterate
@@ -50,6 +62,15 @@ struct HipBatchMember {
   const double *cost, *lower, *upper, *colscale, *rlo, *rup, *rowscale;
   double *x, *xa, *xn, *rx, *aty, *hslack, *atyp, *atdy, *sp, *sn;   // n-vectors
   double *y, *ya, *yn, *ry, *axp, *dy;                                // m-vectors
+};
+
+// A HiPDLP member's vector block, laid out as BatchVec's
+struct HipBatchVec {
+  enum Col { kCost, kLower, kUpper, kColscale, kX, kXa, kXn, kRx, kAty, kHslack, kAtyp, kAtdy, kSp, kSn, kCols };
+  enum Row { kRlo, kRup, kRowscale, kY, kYa, kYn, kRy, kAxp, kDy, kRows };
+  static size_t len(int n, int m) { return (size_t)kCols * n + (size_t)kRows * m; }
+  template <class T> __host__ __device__ static T* col(T* v, int n, int k) { return v + k * n; }
+  template <class T> __host__ __device__ static T* row(T* v, int n, int m, int k) { return v + kCols * n + k * m; }
 };
 
 // Sums a round leaves in HipBatchCtl::outs

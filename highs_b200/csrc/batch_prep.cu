@@ -1,4 +1,4 @@
-// highs_b200/csrc/batch_prep.cu -- the device prologue and postsolve of b200pdlp_solve_batch_device (engine.cu
+// highs_b200/csrc/batch_prep.cu -- the device prologue and postsolve of b200pdlp_solve_batch_device (engine_batch.cu
 // solve_batch_device): one CTA per member, and no CTA waits on another, so any number of members runs.
 //
 //   batch_size_kernel   check_lp(deep) on the device, formulate's row classes and row order, the standard form's dimensions
@@ -6,7 +6,7 @@
 //   batch_prep_kernel   formulate, the row-major index, scale, the sliced-ELL bodies of A and A', host_start_point, xSum = proj(0)
 //                       and the sums that set the tolerances and beta
 //   batch_post_kernel   host_postsolve of the returned iterate, into the caller's device vectors
-// and their HiPDLP twins for b200pdlp_solve_hipdlp_batch_device (engine.cu solve_hipdlp_batch_device):
+// and their HiPDLP twins for b200pdlp_solve_hipdlp_batch_device (engine_batch.cu solve_hipdlp_batch_device):
 //   hip_batch_size_kernel   the same checks and sizes under formulate_hipdlp's row classes
 //   hip_batch_prep_kernel   formulate_hipdlp, the row-major indexes of the form and of the caller's matrix, scale_hipdlp, the
 //                           sliced-ELL bodies of A and A', |c|^2 and |b|^2 of the unscaled form
@@ -16,6 +16,7 @@
 // host_start_point / host_postsolve) with the same operations on the same operands: the build compiles this file with
 // -fmad=false and IEEE division and square root.  Maxima are order-free; every sum is taken in the host's order -- a row's
 // 1-norm column-ascending by the thread that owns the row, |c|^2 and |b|^2 in index order by one thread.
+#include "batch_kernels.hpp"
 #include "batch_prep.hpp"
 #include "host_prep.hpp"
 #include "row_index.cuh"
@@ -189,15 +190,16 @@ __global__ void __launch_bounds__(kThreads) batch_prep_kernel(const BatchPrep* _
   const int n0 = P.n0, m = P.m, n = P.n, nnz = P.nnz;
   const int nnz0 = nnz - (n - n0);
   const double sense = P.sense;
-  double* cost = P.vec;
-  double* lower = cost + n;
-  double* upper = cost + 2 * n;
-  double* colscale = cost + 3 * n;
-  double* x0 = cost + 4 * n;
-  double* xsum = cost + 8 * n;
-  double* rhs = cost + 12 * n;
-  double* rowscale = rhs + m;
-  double* y0 = rhs + 2 * m;
+  using V = BatchVec;
+  double* cost = V::col(P.vec, n, V::kCost);
+  double* lower = V::col(P.vec, n, V::kLower);
+  double* upper = V::col(P.vec, n, V::kUpper);
+  double* colscale = V::col(P.vec, n, V::kColscale);
+  double* x0 = V::col(P.vec, n, V::kX0);
+  double* xsum = V::col(P.vec, n, V::kXsum);
+  double* rhs = V::row(P.vec, n, m, V::kRhs);
+  double* rowscale = V::row(P.vec, n, m, V::kRowscale);
+  double* y0 = V::row(P.vec, n, m, V::kY0);
   const int* rni = P.row_new_idx;
   const int* rcl = P.row_class;
 
@@ -259,7 +261,7 @@ __global__ void __launch_bounds__(kThreads) batch_prep_kernel(const BatchPrep* _
     const int len = t == 32 ? n : m;
     double s = 0.0;
     for (int q = 0; q < len; q++) s += v[q] * v[q];
-    P.rec[t == 32 ? 0 : 1] = s;
+    P.rec[t == 32 ? kRecCostSq : kRecRhsSq] = s;
   }
   __syncthreads();
 
@@ -378,8 +380,8 @@ __global__ void __launch_bounds__(kThreads) batch_prep_kernel(const BatchPrep* _
     const int len = t == 0 ? n : m;
     double s = 0.0;
     for (int q = 0; q < len; q++) s += v[q] * v[q];
-    P.rec[t == 0 ? 3 : 4] = s;
-    if (t == 0) P.rec[2] = amax;
+    P.rec[t == 0 ? kRecScaledCostSq : kRecScaledRhsSq] = s;
+    if (t == 0) P.rec[kRecAmax] = amax;
   }
 }
 
@@ -388,14 +390,15 @@ __global__ void __launch_bounds__(kThreads) batch_post_kernel(const BatchPrep* _
   const BatchPost& Q = post[blockIdx.x];
   if (!(Q.col_value && Q.col_dual && Q.row_value && Q.row_dual)) return;
   const int n0 = P.n0, m = P.m, n = P.n;
+  using V = BatchVec;
   const double* v = P.vec;
-  const double* w = v + 12 * n;
   const bool avg = Q.sel == 2;
-  const double* dx = avg ? v + 9 * n : v + (4 + Q.sel) * n;
-  const double* daty = avg ? v + 10 * n : v + (6 + Q.sel) * n;
-  const double* dy = avg ? w + 7 * m : w + (2 + Q.sel) * m;
-  const double* dax = avg ? w + 8 * m : w + (4 + Q.sel) * m;
-  const double *cost = v, *lower = v + n, *upper = v + 2 * n, *colscale = v + 3 * n, *rowscale = w + m;
+  const double* dx = V::col(v, n, avg ? V::kXavg : V::kX0 + Q.sel);
+  const double* daty = V::col(v, n, avg ? V::kAtyavg : V::kAty0 + Q.sel);
+  const double* dy = V::row(v, n, m, avg ? V::kYavg : V::kY0 + Q.sel);
+  const double* dax = V::row(v, n, m, avg ? V::kAxavg : V::kAx0 + Q.sel);
+  const double *cost = V::col(v, n, V::kCost), *lower = V::col(v, n, V::kLower), *upper = V::col(v, n, V::kUpper);
+  const double *colscale = V::col(v, n, V::kColscale), *rowscale = V::row(v, n, m, V::kRowscale);
   const double sense = P.sense;
   for (int j = threadIdx.x; j < n0; j += kThreads) {
     double sp = 0.0, sn = 0.0;
@@ -460,7 +463,7 @@ __device__ __forceinline__ void form_layouts(const BatchPrep& P, int m, int n, i
             });
 }
 
-// The twins of host_prep_hipdlp.cpp formulate_hipdlp / scale_hipdlp, build_layout and engine.cu hip_host_postsolve.
+// The twins of host_prep_hipdlp.cpp formulate_hipdlp / scale_hipdlp, build_layout and engine_hipdlp.cu hip_host_postsolve.
 
 // batch_size_kernel under formulate_hipdlp's classification: +-infinity thresholds (a bound of 1e25 is finite), FREE rows a
 // class of their own, BOUND and FREE rows equality-like, each with a slack column
@@ -617,13 +620,14 @@ hip_batch_prep_kernel(const BatchPrep* __restrict__ prep, const HipBatchPrep* __
   const int t = threadIdx.x, wid = t >> 5;
   const int n0 = P.n0, m = P.m, n = P.n, nnz = P.nnz;
   const int nnz0 = nnz - (n - n0);
-  double* cost = P.vec;   // the member's block (hip_batch_vec_len): cost, lower, upper, colscale ... rlo, rup, rowscale ...
-  double* lower = cost + n;
-  double* upper = cost + 2 * n;
-  double* colscale = cost + 3 * n;
-  double* rlo = cost + 14 * n;
-  double* rup = rlo + m;
-  double* rowscale = rlo + 2 * m;
+  using V = HipBatchVec;
+  double* cost = V::col(P.vec, n, V::kCost);
+  double* lower = V::col(P.vec, n, V::kLower);
+  double* upper = V::col(P.vec, n, V::kUpper);
+  double* colscale = V::col(P.vec, n, V::kColscale);
+  double* rlo = V::row(P.vec, n, m, V::kRlo);
+  double* rup = V::row(P.vec, n, m, V::kRup);
+  double* rowscale = V::row(P.vec, n, m, V::kRowscale);
   const int* rni = P.row_new_idx;
   const int* rcl = P.row_class;
   if (t == 0) nsort = 0;
@@ -732,7 +736,7 @@ hip_batch_prep_kernel(const BatchPrep* __restrict__ prep, const HipBatchPrep* __
     const int len = t == 32 ? n : m;
     double s = 0.0;
     for (int q = 0; q < len; q++) s += v[q] * v[q];
-    P.rec[t == 32 ? 0 : 1] = s;
+    P.rec[t == 32 ? kRecCostSq : kRecRhsSq] = s;
   }
   __syncthreads();
 
@@ -754,11 +758,12 @@ hip_batch_post_kernel(const BatchPrep* __restrict__ prep, const HipBatchPrep* __
   const HipBatchPost& Q = post[blockIdx.x];
   if (!(Q.col_value && Q.col_dual && Q.row_value && Q.row_dual)) return;
   const int n0 = P.n0, m = P.m, n = P.n;
+  using V = HipBatchVec;
   const double* v = P.vec;
-  const double* w = v + 14 * n;
-  const double* x = Q.sol == 1 ? v + 6 * n : v + 4 * n;   // xn or x
-  const double* y = Q.sol == 1 ? w + 5 * m : w + 3 * m;   // yn or y
-  const double *colscale = v + 3 * n, *sp = v + 12 * n, *sn = v + 13 * n, *rowscale = w + 2 * m;
+  const double* x = Q.sol == 1 ? V::col(v, n, V::kXn) : V::col(v, n, V::kX);
+  const double* y = Q.sol == 1 ? V::row(v, n, m, V::kYn) : V::row(v, n, m, V::kY);
+  const double *colscale = V::col(v, n, V::kColscale), *sp = V::col(v, n, V::kSp), *sn = V::col(v, n, V::kSn);
+  const double* rowscale = V::row(v, n, m, V::kRowscale);
   const bool conv = Q.sol >= 0;
   const double sense = P.sense;
   // the unscaled primal value of structural column j (hip_host_postsolve's hx[j])

@@ -23,7 +23,7 @@ struct BatchPrep {
   int n, nnz, neq;
   int* cbeg; int* cidx; int* pcol; int* rpos; int* rwork;   // [n + 1], [nnz] x 3, [m]
   double* cval; double* cs; double* cs_next; double* rs;    // [nnz], [n], [n], [m]
-  double* vec;                                              // the member's vector block (engine.cu batch_vec_len)
+  double* vec;                                              // the member's vector block (batch_kernels.hpp BatchVec)
   int4* a_slices; int* a_col; double* a_val;                // the ordered sliced-ELL layouts in the pooled format
   int4* at_slices; int* at_col; double* at_val;             //   batch_round_kernel reads (BatchMember)
   double* rec;                                              // [kPrepRec]
@@ -38,9 +38,9 @@ struct BatchSize {
   int pad[2];
 };
 
-// What the prologue reads back per member: rec[0..4] = |c|^2, |b|^2 of the unscaled form (index order), amax, and |c|^2,
+// What the prologue reads back per member, rec[kPrepRec]: |c|^2, |b|^2 of the unscaled form (index order), amax, and |c|^2,
 // |b|^2 of the scaled form (index order: what sets beta)
-constexpr int kPrepRec = 5;
+enum PrepRec { kRecCostSq, kRecRhsSq, kRecAmax, kRecScaledCostSq, kRecScaledRhsSq, kPrepRec };
 
 // Per member, for the postsolve: which iterate to return and where (the caller's device vectors; any NULL: none written)
 struct BatchPost {
@@ -55,7 +55,7 @@ void launch_batch_post(cudaStream_t s, int count, const BatchPrep* prep, const B
 
 // ---- the HiPDLP batch (b200pdlp_solve_hipdlp_batch_device): the same BatchPrep per member, read with HiPDLP's meaning --
 // row_class under formulate_hipdlp's rule (FREE rows a class of their own), slack[i] >= 0 for BOUND and FREE rows, vec a
-// block of hip_batch_vec_len doubles (engine.cu), rec[0..1] = |c|^2, |b|^2 of the unscaled form -- plus these arrays
+// block laid out as HipBatchVec (batch_kernels.hpp), rec[kRecCostSq], rec[kRecRhsSq] = |c|^2, |b|^2 of the unscaled form -- plus these arrays
 // (pooled, like BatchPrep's):
 struct HipBatchPrep {
   int* optr;       // [m + 1] row pointer of the row-major index of the caller's matrix

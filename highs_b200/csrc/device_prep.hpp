@@ -131,7 +131,7 @@ void launch_postsolve(cudaStream_t s, const DevProblemArrays& a, double sense, i
                       const double* y, const double* ax, const double* cost, const double* lower, const double* upper,
                       const double* colscale, const double* rowscale, double* col_value, double* col_dual, double* row_value,
                       double* row_dual);
-// HiPDLP mode (host twins: engine.cu solve_hipdlp_on_device).  Initial point x = xa = proj_[l,u](0) (upper bound first,
+// HiPDLP mode (host twins: engine_hipdlp.cu solve_hipdlp_on_device).  Initial point x = xa = proj_[l,u](0) (upper bound first,
 // then lower, pdhg.cc:512-552), device order.
 void launch_hip_init_point(cudaStream_t s, int n, const double* lower, const double* upper, double* x, double* xa);
 // unscaleSolution + postprocess (pdhg.cc:1883-1897, :359-492) into original-order arrays on the device: x, y only when

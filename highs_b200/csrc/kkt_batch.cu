@@ -1,5 +1,5 @@
 // highs_b200/csrc/kkt_batch.cu -- HiGHS's post-solve KKT assessment (lpKktCheck) for many LP solutions in one launch
-// (engine.cu kkt_check_batch): one CTA per member, and no CTA waits on another, so any number of members of any size runs.
+// (engine_batch.cu kkt_check_batch): one CTA per member, and no CTA waits on another, so any number of members of any size runs.
 //
 //   kkt_batch_check_kernel   the device-pointer variant only: a_start[0] == 0, a_start non-decreasing, a_index in
 //                            [0, num_row), and a_start[num_col], which the host needs to lay out the workspace

@@ -2290,7 +2290,7 @@ void launch_hip_div_norm(cudaStream_t s, int len, double* v, const double* norm_
 }
 }  // namespace b200
 
-// ---- HiPDLP shards: the Halpern step on several GPUs (engine.cu, "HiPDLP on several GPUs").  Rank g owns device columns
+// ---- HiPDLP shards: the Halpern step on several GPUs (engine_hipdlp.cu, "HiPDLP on several GPUs").  Rank g owns device columns
 // [c0, c1) and device rows [r0, r1); every vector is held full length in the one-GPU device order.  The step's two
 // exchanged vectors are stored straight into the peers' copies: the reflected x by the primal kernel, the blended y by the
 // dual epilogue.  The flag barrier carries no data: a Halpern step has no reduction, so nothing but arrival is exchanged.

@@ -1,5 +1,5 @@
 """The HiPDLP mode's device-resident prologue, initial point and postsolve (device_prep.cu, DevicePrologue::hipdlp) against
-the host path it replaces (host_prep_hipdlp.cpp + the host boundary steps of engine.cu solve_hipdlp_on_device).
+the host path it replaces (host_prep_hipdlp.cpp + the host boundary steps of engine_hipdlp.cu solve_hipdlp_on_device).
 
 1. Prologue parity: b200pdlp_debug_prep_compare_hipdlp reports no mismatch in any array -- the scaled standard form, the row
    upper bounds, both orderings and layouts, the row-major copy of the caller's matrix, and both unscaled norms bit for bit --

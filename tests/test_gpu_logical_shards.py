@@ -8,7 +8,7 @@ Each case runs in a child process with a hard timeout (a stuck barrier must not 
 
 Round 2: the path deadlocked on hardware because CUDA loads kernels lazily and a load can need a context-wide synchronisation,
 which never comes while a peer rank's barrier kernel spins on the same device; the kernels of the multi-GPU path are now
-loaded (and the graphs instantiated) before any rank launches a kernel that waits for its peers (engine.cu LocalGroup,
+loaded (and the graphs instantiated) before any rank launches a kernel that waits for its peers (engine.hpp LocalGroup,
 pdhg_kernels.cu preload_multi_gpu_kernels).  Both check-iteration modes run: host-driven (round 1) and device-side."""
 import json
 import os
