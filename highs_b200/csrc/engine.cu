@@ -88,12 +88,31 @@ void apply_spmv_grid(b200pdlp_problem* p) {
   const int tat = val("B200PDLP_TILE_AT", tboth >= 0 ? tboth : tdef);
   if (!tile(p->A, ta)) apply(p->A, ka);
   if (!tile(p->AT, tat)) apply(p->AT, kat);
-  if (getenv("B200PDLP_TIMING"))
+  // Zero-skip shape of the PDLP pass SpMVs (spmv_sell_zskip_kernel: the nonzero bitmap of the input staged in shared memory,
+  // only the entries that may be nonzero gathered; same sums as the shape chosen above) wherever the matrix is not tiled and
+  // the bitmap of its input fits in a CTA's shared memory.  Measured on one H100 (DESIGN.md section 6).
+  // B200PDLP_ZERO_SKIP=0 turns it off to compare the two shapes; it changes no result.
+  if (!p->form.hipdlp && val("B200PDLP_ZERO_SKIP", 1) != 0) {
+    auto zskip = [&](DeviceMatrix& M, int len) {
+      if (M.dev.tiled || M.dev.nslices == 0) return;
+      const int bytes = (int)(((size_t)len + 127) / 128 * 16);
+      const int per_sm = zskip_ctas_per_sm(bytes);
+      if (per_sm <= 0) return;
+      M.nz.alloc((size_t)bytes / 4, false);
+      M.dev.nzmap = M.nz.p; M.dev.nz_bytes = bytes; M.dev.zskip_grid = per_sm * sms;
+    };
+    zskip(p->A, p->n);
+    zskip(p->AT, p->m);
+  }
+  if (getenv("B200PDLP_TIMING")) {
     fprintf(stderr, "[b200pdlp setup] SpMV shapes: A %s (%d CTAs, tiles staged %d/%d)  A' %s (%d CTAs, tiles staged %d/%d)\n",
             p->A.dev.tiled ? "tiled" : (p->A.dev.pipelined ? "persistent" : "one slice per warp"), p->A.dev.nblocks_body,
             p->A.tiles_staged, p->A.ntiles,
             p->AT.dev.tiled ? "tiled" : (p->AT.dev.pipelined ? "persistent" : "one slice per warp"), p->AT.dev.nblocks_body,
             p->AT.tiles_staged, p->AT.ntiles);
+    fprintf(stderr, "[b200pdlp setup] zero-skip pass SpMVs: A %d CTAs  A' %d CTAs (0: off)\n", p->A.dev.zskip_grid,
+            p->AT.dev.zskip_grid);
+  }
 }
 
 // ---- problem construction.  Every creator below is a sequence of these steps plus what is its own.
@@ -426,9 +445,9 @@ static void enqueue_pass(b200pdlp_problem* p) {
   PdhgState* st = p->state.p;
   const ReduceScratch r1 = p->rs(kSlotK1, p->n), r2 = p->rs(kSlotK2, p->ml), r3 = p->rs(kSlotK3, p->n);
   launch_primal_step(s, p->n, st, p->x[0].p, p->x[1].p, p->aty[0].p, p->aty[1].p, p->cost.p, p->lower.p,
-                     p->upper.p, p->xsum.p, r1);
+                     p->upper.p, p->xsum.p, r1, p->A.dev.nzmap);
   launch_spmv_dual(s, p->A.dev, st, p->x[0].p, p->x[1].p, p->y[0].p, p->y[1].p, p->ax[0].p, p->ax[1].p,
-                   p->rhs.p, p->ysum.p, p->neq_local, 0, r2, p->axsum.p);
+                   p->rhs.p, p->ysum.p, p->neq_local, 0, r2, p->axsum.p, p->AT.dev.nzmap);
   launch_spmv_primal(s, p->AT.dev, st, p->y[0].p, p->y[1].p, p->x[0].p, p->x[1].p, p->aty[0].p, p->aty[1].p, r3, p->atysum.p);
   launch_step_rule(s, st, r1, primal_step_grid(p->n), r2, p->A.grid(), r3, p->AT.grid(), nullptr);
 }
@@ -1910,7 +1929,7 @@ int b200pdlp_primal_step(b200pdlp_problem* p, const double* x, const double* aty
     kernel_api_state(p, tau, tau);
     const ReduceScratch r1 = p->rs(kSlotK1, n);
     launch_primal_step(p->stream, n, p->state.p, p->x[0].p, p->x[1].p, p->aty[0].p, p->aty[1].p, p->cost.p, p->lower.p,
-                       p->upper.p, p->xsum.p, r1);
+                       p->upper.p, p->xsum.p, r1, p->A.dev.nzmap);
     p->launches++;
     download_perm(p, x_new, p->x[1].p, p->cperm);
     if (dx2) *dx2 = sum_partials(p, r1, primal_step_grid(n));
@@ -1934,8 +1953,9 @@ int b200pdlp_dual_step(b200pdlp_problem* p, const double* x_new, const double* y
     upload_perm(p, p->ax[0].p, ax, p->rperm);
     kernel_api_state(p, sigma, sigma);
     const ReduceScratch r2 = p->rs(kSlotK2, m);
+    if (p->A.dev.nzmap) launch_nz_bitmap(s, p->n, p->x[1].p, p->A.dev.nzmap);   // x' came from the caller, not from K1
     launch_spmv_dual(s, p->A.dev, p->state.p, p->x[0].p, p->x[1].p, p->y[0].p, p->y[1].p, p->ax[0].p, p->ax[1].p, p->rhs.p,
-                     p->ysum.p, p->neq_local, 0, r2);
+                     p->ysum.p, p->neq_local, 0, r2, nullptr, p->AT.dev.nzmap);
     p->launches++;
     download_perm(p, y_new, p->y[1].p, p->rperm);
     download_perm(p, ax_new, p->ax[1].p, p->rperm);
@@ -2022,10 +2042,10 @@ int b200pdlp_bench_pass(b200pdlp_problem* p, int32_t reps, float ms[4]) {
         const ReduceScratch r1 = p->rs(kSlotK1, p->n), r2 = p->rs(kSlotK2, p->ml), r3 = p->rs(kSlotK3, p->n);
         CUDA_OK(cudaEventRecord(ev[0], s));
         launch_primal_step(s, p->n, st, p->x[0].p, p->x[1].p, p->aty[0].p, p->aty[1].p, p->cost.p, p->lower.p,
-                           p->upper.p, p->xsum.p, r1);
+                           p->upper.p, p->xsum.p, r1, p->A.dev.nzmap);
         CUDA_OK(cudaEventRecord(ev[1], s));
         launch_spmv_dual(s, p->A.dev, st, p->x[0].p, p->x[1].p, p->y[0].p, p->y[1].p, p->ax[0].p, p->ax[1].p,
-                         p->rhs.p, p->ysum.p, p->neq_local, 0, r2);
+                         p->rhs.p, p->ysum.p, p->neq_local, 0, r2, nullptr, p->AT.dev.nzmap);
         CUDA_OK(cudaEventRecord(ev[2], s));
         launch_spmv_primal(s, p->AT.dev, st, p->y[0].p, p->y[1].p, p->x[0].p, p->x[1].p, p->aty[0].p,
                            p->aty[1].p, r3);

@@ -130,6 +130,7 @@ struct DeviceMatrix {
   DevBuf<unsigned> long_counter;
   DevBuf<int> tile_lo, tile_w;   // tiled shape (DevSell::tiled): windows of the input vector per tile of kTileSlices slices
   int ntiles = 0, tiles_staged = 0;
+  DevBuf<unsigned> nz;           // zero-skip shape (DevSell::zskip_grid): nonzero bitmap of the input vector
   DevSell dev{};
   void upload() {
     col.from(host.col);

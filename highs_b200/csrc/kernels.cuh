@@ -134,10 +134,21 @@ struct DevSell {
   int tiled;                              // 0 off, 1 staged by cp.async.bulk (TMA unit) + mbarrier, 2 staged by cooperative loads
   const int* __restrict__ tile_lo;
   const int* __restrict__ tile_w;
+  // ZERO-SKIP shape (the PDHG pass SpMVs only, one GPU, tree mode; spmv_sell_zskip_kernel): a nonzero bitmap of the input
+  // vector, written by the kernel that produces that vector in the same pass (K1 for x', K2's epilogue for y').  Bit i is
+  // word i >> 5, bit i & 31; 0 means "entry i is exactly +-0.0", 1 means "may be nonzero" (whoever cannot tell writes 1).
+  // Every CTA stages the bitmap in shared memory and gathers only the entries whose bit is 1.  zskip_grid > 0: K2 / K3 of
+  // this matrix run that kernel on zskip_grid CTAs; nblocks_body / pipelined keep describing the shape whose partial sums it
+  // reproduces (and the one every other launch of this matrix uses).
+  int zskip_grid;
+  int nz_bytes;                           // staged bytes: the bitmap rounded up to 16 bytes
+  unsigned* nzmap;
 };
 constexpr int kTileSlices = 256;          // slices per tile (8192 rows)
 constexpr int kTileThreads = 1024;
 constexpr int kTileMaxWindow = 24576;     // doubles staged per tile (192 KB of the 227 KB a CTA may use)
+constexpr int kZThreads = 768;            // threads of a zero-skip CTA: kZGroups groups of kThreads, each one CTA of the walk
+constexpr int kZGroups = kZThreads / kThreads;
 
 // peer-memory view for the fused multi-GPU path (one process per GPU, buffers mapped with CUDA IPC)
 constexpr int kMaxPeers = 16;
@@ -211,6 +222,31 @@ __device__ __forceinline__ void block_partials(const double (&acc)[NACC], const 
       rs.partials[(size_t)a * gridDim.x + blockIdx.x] = s;
     }
   }
+}
+
+// block_partials for one group of kThreads threads inside a wider CTA (threads [g kThreads, (g + 1) kThreads)): the same tree,
+// synchronised by named barrier 1 + g, into slot `slot` of partials arrays `nslots` long.  smp: [groups][NACC][kThreads / 32].
+template <int NACC>
+__device__ __forceinline__ void group_partials(const double (&acc)[NACC], const ReduceScratch& rs, int slot, int nslots,
+                                               double (*smp)[NACC][kThreads / 32]) {
+  constexpr int kWarps = kThreads / 32;
+  const int lane = threadIdx.x & 31, g = threadIdx.x / kThreads, wid = (threadIdx.x % kThreads) >> 5;
+#pragma unroll
+  for (int a = 0; a < NACC; a++) {
+    const double s = warp_sum(acc[a]);
+    if (lane == 0) smp[g][a][wid] = s;
+  }
+  asm volatile("bar.sync %0, %1;" ::"r"(1 + g), "r"(kThreads) : "memory");
+  if (threadIdx.x % kThreads == 0) {
+#pragma unroll
+    for (int a = 0; a < NACC; a++) {
+      double s = 0.0;
+#pragma unroll
+      for (int w = 0; w < kWarps; w++) s += smp[g][a][w];
+      rs.partials[(size_t)a * nslots + slot] = s;
+    }
+  }
+  asm volatile("bar.sync %0, %1;" ::"r"(1 + g), "r"(kThreads) : "memory");   // smp is the group's again
 }
 
 // Two-stage deterministic sum over the grid.  Every warp parks its shuffle-reduced partials in

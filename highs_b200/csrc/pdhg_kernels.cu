@@ -13,7 +13,7 @@ __global__ void __launch_bounds__(kThreads)
 primal_step_kernel(int n, PdhgState* __restrict__ st, double* __restrict__ x0, double* __restrict__ x1,
                    const double* __restrict__ aty0, const double* __restrict__ aty1,
                    const double* __restrict__ c, const double* __restrict__ lo, const double* __restrict__ up,
-                   double* __restrict__ xsum, ReduceScratch rs) {
+                   double* __restrict__ xsum, ReduceScratch rs, unsigned* __restrict__ xnz) {
   if (st->iter >= st->stop_iter) return;
   const int cur = st->cur;
   const double tau = st->tau_try, ntau = -tau;
@@ -26,27 +26,48 @@ primal_step_kernel(int n, PdhgState* __restrict__ st, double* __restrict__ x0, d
   auto one = [&](double xc, double ci, double ai, double u, double l, double& out) {
     return primal_update(xc, ci, ai, u, l, tau, ntau, out);
   };
-  // pairs of elements with 128-bit loads/stores (all vectors are cudaMalloc-aligned)
-  const int npair = n >> 1;
+  // pairs of elements with 128-bit loads/stores (all vectors are cudaMalloc-aligned); the loop runs warp-uniformly so that
+  // a warp's 64 entries give two words of the nonzero bitmap (DevSell::nzmap) of x'
+  const int npair = n >> 1, nq = (n + 1) >> 1;
+  const int lane = threadIdx.x & 31;
   const int stride = gridDim.x * kThreads;
-  for (int i = blockIdx.x * kThreads + threadIdx.x; i < npair; i += stride) {
-    const double2 xc = reinterpret_cast<const double2*>(x)[i];
-    const double2 ci = reinterpret_cast<const double2*>(c)[i];
-    const double2 ai = reinterpret_cast<const double2*>(aty)[i];
-    const double2 u = reinterpret_cast<const double2*>(up)[i];
-    const double2 l = reinterpret_cast<const double2*>(lo)[i];
-    if (pend) {
-      double2 sm = reinterpret_cast<double2*>(xsum)[i];
-      sm.x = sm.x + w * xc.x;
-      sm.y = sm.y + w * xc.y;
-      reinterpret_cast<double2*>(xsum)[i] = sm;
+  for (int i0 = blockIdx.x * kThreads + (threadIdx.x & ~31); i0 < nq; i0 += stride) {
+    const int i = i0 + lane;
+    unsigned nz = 3u;   // two bits: entries 2i, 2i + 1 (1 = may be nonzero; past the end nothing reads them)
+    if (i < npair) {
+      const double2 xc = reinterpret_cast<const double2*>(x)[i];
+      const double2 ci = reinterpret_cast<const double2*>(c)[i];
+      const double2 ai = reinterpret_cast<const double2*>(aty)[i];
+      const double2 u = reinterpret_cast<const double2*>(up)[i];
+      const double2 l = reinterpret_cast<const double2*>(lo)[i];
+      if (pend) {
+        double2 sm = reinterpret_cast<double2*>(xsum)[i];
+        sm.x = sm.x + w * xc.x;
+        sm.y = sm.y + w * xc.y;
+        reinterpret_cast<double2*>(xsum)[i] = sm;
+      }
+      double2 o;
+      const double t0 = one(xc.x, ci.x, ai.x, u.x, l.x, o.x);
+      const double t1 = one(xc.y, ci.y, ai.y, u.y, l.y, o.y);
+      reinterpret_cast<double2*>(xn)[i] = o;
+      add_term(acc[0], t0, rs, 0, 2 * i);
+      add_term(acc[0], t1, rs, 0, 2 * i + 1);
+      nz = (o.x != 0.0 ? 1u : 0u) | (o.y != 0.0 ? 2u : 0u);
+    } else if (i < nq && xnz) {
+      // odd n: x'[n - 1] is written (and summed) by block 0 below; the same arithmetic here gives its bit without a race
+      // on the bitmap word
+      double o;
+      one(x[n - 1], c[n - 1], aty[n - 1], up[n - 1], lo[n - 1], o);
+      nz = (o != 0.0 ? 1u : 0u) | 2u;
     }
-    double2 o;
-    const double t0 = one(xc.x, ci.x, ai.x, u.x, l.x, o.x);
-    const double t1 = one(xc.y, ci.y, ai.y, u.y, l.y, o.y);
-    reinterpret_cast<double2*>(xn)[i] = o;
-    add_term(acc[0], t0, rs, 0, 2 * i);
-    add_term(acc[0], t1, rs, 0, 2 * i + 1);
+    if (xnz) {
+      const unsigned sh = nz << (2 * (lane & 15));
+      const unsigned w_lo = __reduce_or_sync(0xffffffffu, lane < 16 ? sh : 0u);
+      const unsigned w_hi = __reduce_or_sync(0xffffffffu, lane < 16 ? 0u : sh);
+      const int wd = i0 >> 4;   // entries 2 i0 .. 2 i0 + 63
+      if (lane == 0) xnz[wd] = w_lo;
+      if (lane == 16 && 32 * (wd + 1) < n) xnz[wd + 1] = w_hi;
+    }
   }
   if ((n & 1) && blockIdx.x == 0 && threadIdx.x == 0) {
     const int i = n - 1;
@@ -68,6 +89,13 @@ struct StridedOut {
   __device__ __forceinline__ double& operator[](int a) const { return p[a * kThreads]; }
   __device__ __forceinline__ StridedOut operator+(int k) const { return StridedOut{p + k * kThreads}; }
 };
+// an epilogue that has slice_end(slice, live) gets it after every slice of the body, with the whole warp converged
+template <class E, class = void> struct HasSliceEnd { static constexpr bool value = false; };
+template <class E> struct HasSliceEnd<E, decltype(void(&E::slice_end))> { static constexpr bool value = true; };
+template <class Epi>
+__device__ __forceinline__ void slice_end(const Epi& e, int slice, bool live) {
+  if constexpr (HasSliceEnd<Epi>::value) e.slice_end(slice, live);
+}
 // ===================================================================== SpMV
 // Sliced-ELL body: one warp per slice of 32 rows, one lane per row.  A warp reads the slice's
 // col / val arrays fully coalesced (k-major, lane-minor), every lane gathers its dense-vector
@@ -105,6 +133,7 @@ struct DualEpilogueT {
   double* ysum;
   int neq, row_offset;         // neq = number of LOCAL equality rows (they come first); row_offset unused
   double* axsum;               // A xSum, carried while the checks are dense (PdhgState::light_on); may be nullptr
+  unsigned* ynz;               // nonzero bitmap of y' (DevSell::nzmap of A'), one word per slice; may be nullptr
   // cached from the state block by begin()
   const double *y, *ax;
   double *yn, *axn;
@@ -128,16 +157,25 @@ struct DualEpilogueT {
     p_ys = pend ? ysum[r] : 0.0;
     p_axs = accum ? axsum[r] : 0.0;
   }
-  __device__ void row(int r, double s, double* t) const {
+  bool nz;
+  __device__ void row(int r, double s, double* t) {
     axn[r] = s;
     const double yc = p_y;
     if (pend) ysum[r] = p_ys + w * yc;
     if (accum) axsum[r] = p_axs + w * p_ax;   // A xSum += w A x  (x = the iterate accepted by the previous pass)
     const double v = dual_update(yc, p_b, s, p_ax, sigma, r >= neq);
     yn[r] = v;
+    nz = v != 0.0;
     const double d = yc - v;
     t[0] = d * d;
     if (NACC > 1) t[NACC - 1] = (p_ax - s) * d;   // row-side interaction (AΔx)·Δy, multi-GPU only
+  }
+  // after a slice's rows (the whole warp, lane = row of the slice): the slice's word of the bitmap.  Lanes without a live
+  // row write 1 -- among them the long rows, whose y' the segment finisher writes later in this launch.
+  __device__ void slice_end(int slice, bool live) const {
+    if (!ynz) return;
+    const unsigned bits = __ballot_sync(0xffffffffu, !live || nz);
+    if ((threadIdx.x & 31) == 0) ynz[slice] = bits;
   }
 };
 using DualEpilogue = DualEpilogueT<1>;
@@ -329,6 +367,7 @@ __global__ void __launch_bounds__(kThreads) spmv_sell_kernel(DevSell A, Epi epi_
           }
         }
       }
+      slice_end(epi, slice, live);
       d = dn;
       dn = dnn;
 #pragma unroll
@@ -381,6 +420,7 @@ __global__ void __launch_bounds__(kThreads) spmv_sell_kernel(DevSell A, Epi epi_
           }
         }
       }
+      slice_end(epi, slice, live);
     }
   } else {
     // one segment of a long row
@@ -451,6 +491,35 @@ __global__ void __launch_bounds__(kThreads) spmv_sell_kernel(DevSell A, Epi epi_
 // multiplies its 0 by 0 instead of by x[0] (the sum is unchanged; the sign of an all-zero row's zero may differ).
 __device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 
+// `bytes` (a multiple of 16, from a 16-byte aligned address) into shared memory by the TMA unit: bulk copies of <= 32 KB
+// completed on one mbarrier, which every thread of the CTA waits for (SASS: UBLKCP / SYNCS).  Contains a __syncthreads.
+__device__ __forceinline__ void bulk_stage(void* dst, const void* src, unsigned bytes, unsigned long long* mbar) {
+  const unsigned bar = smem_u32(mbar);
+  if (threadIdx.x == 0) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(1) : "memory");
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");   // the init, visible to the async proxy that completes on it
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+    for (unsigned off = 0; off < bytes; off += 32768u) {   // chunks of 32 KB (each a multiple of 16 bytes)
+      const unsigned n = bytes - off < 32768u ? bytes - off : 32768u;
+      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
+                       smem_u32(dst) + off),
+                   "l"(reinterpret_cast<const char*>(src) + off), "r"(n), "r"(bar)
+                   : "memory");
+    }
+  }
+  unsigned done = 0;
+  do {
+    asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
+                 : "=r"(done)
+                 : "r"(bar), "r"(0)
+                 : "memory");
+  } while (!done);
+}
+
 template <class Epi>
 __global__ void __launch_bounds__(kTileThreads, 1) spmv_sell_tile_kernel(DevSell A, Epi epi_arg, ReduceScratch rs) {
   extern __shared__ __align__(16) double xs[];
@@ -502,31 +571,7 @@ __global__ void __launch_bounds__(kTileThreads, 1) spmv_sell_tile_kernel(DevSell
   const bool staged = w > 0;
   if (staged) {
     if (A.tiled == 1) {
-      const unsigned bar = smem_u32(&mbar);
-      if (threadIdx.x == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(1) : "memory");
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");   // the init, visible to the async proxy that completes on it
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      }
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        const unsigned bytes = (unsigned)w * 8u;
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-        for (unsigned off = 0; off < bytes; off += 32768u) {   // chunks of 32 KB (each a multiple of 16 bytes)
-          const unsigned n = bytes - off < 32768u ? bytes - off : 32768u;
-          asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                           smem_u32(xs) + off),
-                       "l"(reinterpret_cast<const char*>(xin + lo) + off), "r"(n), "r"(bar)
-                       : "memory");
-        }
-      }
-      unsigned done = 0;
-      do {
-        asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                     : "=r"(done)
-                     : "r"(bar), "r"(0)
-                     : "memory");
-      } while (!done);
+      bulk_stage(xs, xin + lo, (unsigned)w * 8u, &mbar);
     } else {
       for (int i = threadIdx.x; i < w; i += kTileThreads) xs[i] = xin[lo + i];
       __syncthreads();
@@ -584,6 +629,7 @@ __global__ void __launch_bounds__(kTileThreads, 1) spmv_sell_tile_kernel(DevSell
         for (int a = 0; a < Epi::NACC; a++) acc[a] += t[a];
       }
     }
+    slice_end(epi, slice, live);
   }
   if constexpr (Epi::NACC > 0) {
     // lanes, then the CTA's 32 warps in order: a fixed tree
@@ -615,6 +661,154 @@ static void launch_tile(cudaStream_t s, const DevSell& A, const Epi& e, const Re
     if (dev >= 0 && dev < 64) attr_set[dev] = true;
   }
   spmv_sell_tile_kernel<Epi><<<A.nblocks_body + A.nsegs, kTileThreads, smem, s>>>(A, e, rs);
+}
+
+// ============================================================ zero-skip SpMV (the PDHG pass, one GPU)
+// DevSell::zskip_grid.  K2 gathers x', K3 gathers y', and a PDLP iterate is full of exact zeros (x' = max(x', l) with
+// l = 0, y' = max(y', 0) on inequality rows).  A term v * (+-0.0) is +-0.0, and s + (+-0.0) == s for every s that is not
+// -0.0; a row sum starts at +0.0 and +0 + -0 = +0, so it never is.  Skipping those terms therefore leaves every row sum
+// bit-identical, and it saves their gathers, which bound these kernels on random columns (one 32-byte sector per
+// gathered double).  The producers of x' / y' write the nonzero bitmap (DevSell::nzmap); every CTA stages it in shared
+// memory with one bulk copy and tests a bit before it gathers.
+// The block partial sums are those of the shape described by nblocks_body / pipelined: a CTA is kZGroups groups of
+// kThreads, and group q of the grid does the work of that shape's CTAs q, q + Q, q + 2Q, ... (Q = groups in the grid) --
+// warp w of the group walks the slices 8c + w, 8c + w + W, ... (W = 8 nblocks_body) of CTA c, in the same order, and the
+// group writes CTA c's partials with the same tree.  Then the long-row segments, one per group, likewise.
+template <class Epi>
+__global__ void __launch_bounds__(kZThreads, 1) spmv_sell_zskip_kernel(DevSell A, Epi epi_arg, ReduceScratch rs) {
+  extern __shared__ __align__(16) unsigned nzs[];
+  __shared__ __align__(8) unsigned long long mbar;
+  __shared__ double smp[kZGroups][Epi::NACC][kThreads / 32];
+  __shared__ double sseg[kZGroups][kThreads / 32];
+  Epi epi = epi_arg;
+  if (!epi.begin()) return;
+  const double* __restrict__ xin = epi.input();
+  bulk_stage(nzs, A.nzmap, (unsigned)A.nz_bytes, &mbar);
+  auto bit = [&](int c) { return (nzs[c >> 5] >> (c & 31)) & 1u; };
+  const int lane = threadIdx.x & 31, grp = threadIdx.x / kThreads, w = (threadIdx.x % kThreads) >> 5;
+  const int ngroups = gridDim.x * kZGroups, gid = grp * gridDim.x + blockIdx.x;
+  const int nb = A.nblocks_body, ns = A.nslices, W = nb * (kThreads / 32);
+  const int nslots = A.nblocks_body + A.nsegs;
+  // this warp's walk: descriptor and the first (up to) 8 column ids one slice ahead
+  int s = gid * 8 + w;
+  int4 d = make_int4(0, 0, -1, 0);
+  int cpre[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  if (gid < nb && s < ns) {
+    d = A.slices[s];
+#pragma unroll
+    for (int u = 0; u < 8; u++) if (u < d.y) cpre[u] = A.col[d.x + lane + 32 * u];
+  }
+  for (int c = gid; c < nb; c += ngroups) {   // group-uniform
+    double acc[Epi::NACC] = {};
+    bool more = s < ns;
+    while (more) {
+      int sn = s + W;
+      more = sn < ns;
+      if (!more) sn = c + ngroups < nb ? (c + ngroups) * 8 + w : ns;
+      int4 dn = make_int4(0, 0, -1, 0);
+      int cnx[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+      if (sn < ns) {
+        dn = A.slices[sn];
+#pragma unroll
+        for (int u = 0; u < 8; u++) if (u < dn.y) cnx[u] = A.col[dn.x + lane + 32 * u];
+      }
+      const int row = s * 32 + lane;
+      const bool live = !((unsigned)d.z >> lane & 1u);
+      if (live) epi.prefetch(row);
+      const int* __restrict__ cp = A.col + d.x + lane;
+      const double* __restrict__ vp = A.val + d.x + lane;
+      double sum = 0.0;
+      int k = 0;
+      {
+        double v[8], g[8];
+#pragma unroll
+        for (int u = 0; u < 8; u++) g[u] = (u < d.y && bit(cpre[u])) ? xin[cpre[u]] : 0.0;
+#pragma unroll
+        for (int u = 0; u < 8; u++) v[u] = u < d.y ? vp[32 * u] : 0.0;
+#pragma unroll
+        for (int u = 0; u < 8; u++) if (u < d.y) sum += v[u] * g[u];
+        k = d.y < 8 ? d.y : 8;
+      }
+      for (; k + 8 <= d.y; k += 8) {
+        int cc[8];
+        double v[8], g[8];
+#pragma unroll
+        for (int u = 0; u < 8; u++) cc[u] = cp[32 * (k + u)];
+#pragma unroll
+        for (int u = 0; u < 8; u++) g[u] = bit(cc[u]) ? xin[cc[u]] : 0.0;
+#pragma unroll
+        for (int u = 0; u < 8; u++) v[u] = vp[32 * (k + u)];
+#pragma unroll
+        for (int u = 0; u < 8; u++) sum += v[u] * g[u];
+      }
+      for (; k < d.y; k++) {
+        const int cc = cp[32 * k];
+        sum += vp[32 * k] * (bit(cc) ? xin[cc] : 0.0);
+      }
+      if (live) {
+        double t[Epi::NACC];
+        epi.row(row, sum, t);
+#pragma unroll
+        for (int a = 0; a < Epi::NACC; a++) acc[a] += t[a];
+      }
+      slice_end(epi, s, live);
+      d = dn;
+#pragma unroll
+      for (int u = 0; u < 8; u++) cpre[u] = cnx[u];
+      s = sn;
+    }
+    group_partials<Epi::NACC>(acc, rs, c, nslots, smp);
+  }
+  // long-row segments: as one kThreads CTA of spmv_sell_kernel does them (block_sum's tree, the ticket, the finisher's term)
+  const int t = threadIdx.x % kThreads;
+  for (int q = gid; q < A.nsegs; q += ngroups) {
+    const int4 sg = A.segs[q];
+    double sv = 0.0;
+    for (int e = sg.y + t; e < sg.z; e += kThreads) sv += A.lval[e] * xin[A.lcol[e]];
+    sv = warp_sum(sv);
+    if (lane == 0) sseg[grp][w] = sv;
+    asm volatile("bar.sync %0, %1;" ::"r"(1 + grp), "r"(kThreads) : "memory");
+    double acc[Epi::NACC] = {};
+    if (w == 0) {
+      double r = lane < kThreads / 32 ? sseg[grp][lane] : 0.0;
+      r = warp_sum(r);
+      if (lane == 0) {
+        const int4 lr = A.long_rows[sg.w];
+        A.long_partial[lr.w + q - lr.y] = r;
+        __threadfence();
+        const unsigned tk = atomicAdd(&A.long_counter[sg.w], 1u);
+        if (tk == (unsigned)lr.z - 1u) {
+          __threadfence();
+          const volatile double* pp = A.long_partial + lr.w;
+          double tot = 0.0;
+          for (int i = 0; i < lr.z; i++) tot += pp[i];
+          A.long_counter[sg.w] = 0u;
+          epi.prefetch(lr.x);
+          double tt[Epi::NACC];
+          epi.row(lr.x, tot, tt);
+#pragma unroll
+          for (int a = 0; a < Epi::NACC; a++) acc[a] += tt[a];
+        }
+      }
+    }
+    group_partials<Epi::NACC>(acc, rs, nb + q, nslots, smp);   // (its first barrier also ends the group's use of sseg)
+  }
+}
+
+template <class Epi>
+static void launch_zskip(cudaStream_t s, const DevSell& A, const Epi& e, const ReduceScratch& rs) {
+  static bool attr_set[64] = {false};   // per instantiation AND per device (see launch_tile)
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= 64 || !attr_set[dev]) {
+    int cap = 0;
+    cudaDeviceGetAttribute(&cap, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+    cudaFuncAttributes fa;
+    cudaFuncGetAttributes(&fa, spmv_sell_zskip_kernel<Epi>);
+    cudaFuncSetAttribute(spmv_sell_zskip_kernel<Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap - (int)fa.sharedSizeBytes);
+    if (dev >= 0 && dev < 64) attr_set[dev] = true;
+  }
+  spmv_sell_zskip_kernel<Epi><<<A.zskip_grid, kZThreads, A.nz_bytes, s>>>(A, e, rs);
 }
 
 // ============================================================ multi-GPU kernels
@@ -1804,8 +1998,39 @@ static inline int ew_grid(int len) {
 
 void launch_primal_step(cudaStream_t s, int n, PdhgState* st, double* x0, double* x1, const double* aty0,
                         const double* aty1, const double* c, const double* lo, const double* up, double* xsum,
-                        ReduceScratch rs) {
-  primal_step_kernel<<<ew_grid((n + 1) / 2), kThreads, 0, s>>>(n, st, x0, x1, aty0, aty1, c, lo, up, xsum, rs);
+                        ReduceScratch rs, unsigned* xnz) {
+  primal_step_kernel<<<ew_grid((n + 1) / 2), kThreads, 0, s>>>(n, st, x0, x1, aty0, aty1, c, lo, up, xsum, rs, xnz);
+}
+
+// the nonzero bitmap (DevSell::nzmap) of a vector that no pass kernel produced (kernel-level entry points)
+__global__ void __launch_bounds__(kThreads) nz_bitmap_kernel(int len, const double* __restrict__ v, unsigned* __restrict__ out) {
+  for (int i0 = blockIdx.x * kThreads + (threadIdx.x & ~31); i0 < len; i0 += gridDim.x * kThreads) {
+    const int i = i0 + (threadIdx.x & 31);
+    const unsigned bits = __ballot_sync(0xffffffffu, i >= len || v[i] != 0.0);
+    if ((threadIdx.x & 31) == 0) out[i0 >> 5] = bits;
+  }
+}
+void launch_nz_bitmap(cudaStream_t s, int len, const double* v, unsigned* out) {
+  if (len > 0) nz_bitmap_kernel<<<ew_grid(len), kThreads, 0, s>>>(len, v, out);
+}
+
+// CTAs of spmv_sell_zskip_kernel that fit on one SM with nz_bytes of bitmap staged (both pass epilogues); 0: none
+int zskip_ctas_per_sm(int nz_bytes) {
+  int best = 1 << 30;
+  auto one = [&](auto kern) {
+    int dev = 0, cap = 0, k = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&cap, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+    cudaFuncAttributes fa;
+    if (cudaFuncGetAttributes(&fa, kern) != cudaSuccess || (size_t)nz_bytes + fa.sharedSizeBytes > (size_t)cap) { best = 0; return; }
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, cap - (int)fa.sharedSizeBytes);
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&k, kern, kZThreads, (size_t)nz_bytes) != cudaSuccess) k = 0;
+    best = k < best ? k : best;
+  };
+  one(spmv_sell_zskip_kernel<DualEpilogue>);
+  one(spmv_sell_zskip_kernel<PrimalEpilogue>);
+  cudaGetLastError();
+  return best;
 }
 
 void launch_spmv_plain(cudaStream_t s, const DevSell& A, const double* in, double* out, const PdhgState* due) {
@@ -1818,11 +2043,12 @@ void launch_spmv_plain(cudaStream_t s, const DevSell& A, const double* in, doubl
 
 void launch_spmv_dual(cudaStream_t s, const DevSell& A, PdhgState* st, const double* x0, const double* x1,
                       double* y0, double* y1, double* ax0, double* ax1, const double* b, double* ysum,
-                      int neq, int row_offset, ReduceScratch rs, double* axsum) {
+                      int neq, int row_offset, ReduceScratch rs, double* axsum, unsigned* ynz) {
   if (A.nblocks_body + A.nsegs == 0) return;   // no rows on this rank: nothing to launch, the partial count is 0
   DualEpilogue e{};
   e.st = st; e.x0 = x0; e.x1 = x1; e.y0 = y0; e.y1 = y1; e.ax0 = ax0; e.ax1 = ax1; e.b = b; e.ysum = ysum;
-  e.neq = neq; e.row_offset = row_offset; e.axsum = axsum;
+  e.neq = neq; e.row_offset = row_offset; e.axsum = axsum; e.ynz = ynz;
+  if (A.zskip_grid) { launch_zskip(s, A, e, rs); return; }
   if (A.tiled) { launch_tile(s, A, e, rs); return; }   // (the engine tiles only in tree mode)
   if (A.pipelined) spmv_sell_kernel<DualEpilogue, true><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, rs);
   else spmv_sell_kernel<DualEpilogue, false><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, rs);
@@ -1833,6 +2059,7 @@ void launch_spmv_primal(cudaStream_t s, const DevSell& A, PdhgState* st, const d
   if (A.nblocks_body + A.nsegs == 0) return;   // no rows on this rank: nothing to launch, the partial count is 0
   PrimalEpilogue e{};
   e.st = st; e.y0 = y0; e.y1 = y1; e.x0 = x0; e.x1 = x1; e.aty0 = aty0; e.aty1 = aty1; e.atysum = atysum;
+  if (A.zskip_grid) { launch_zskip(s, A, e, rs); return; }
   if (A.tiled) { launch_tile(s, A, e, rs); return; }   // (tree mode only: engine.cu)
   if (A.pipelined) spmv_sell_kernel<PrimalEpilogue, true><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, rs);
   else spmv_sell_kernel<PrimalEpilogue, false><<<A.nblocks_body + A.nsegs, kThreads, 0, s>>>(A, e, rs);

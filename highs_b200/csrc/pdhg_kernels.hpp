@@ -9,11 +9,14 @@ struct RowIter { const double* y; const double* ax; };    // one dual-side itera
 
 void launch_primal_step(cudaStream_t s, int n, PdhgState* st, double* x0, double* x1, const double* aty0,
                         const double* aty1, const double* c, const double* lo, const double* up, double* xsum,
-                        ReduceScratch rs);
+                        ReduceScratch rs, unsigned* xnz = nullptr);
+// xnz / ynz: where K1 / K2 write the nonzero bitmap of x' / y' (DevSell::nzmap of A / A'), nullptr: nowhere
+void launch_nz_bitmap(cudaStream_t s, int len, const double* v, unsigned* out);
+int zskip_ctas_per_sm(int nz_bytes);
 void launch_spmv_plain(cudaStream_t s, const DevSell& A, const double* in, double* out, const PdhgState* due = nullptr);
 void launch_spmv_dual(cudaStream_t s, const DevSell& A, PdhgState* st, const double* x0, const double* x1,
                       double* y0, double* y1, double* ax0, double* ax1, const double* b, double* ysum,
-                      int neq, int row_offset, ReduceScratch rs, double* axsum = nullptr);
+                      int neq, int row_offset, ReduceScratch rs, double* axsum = nullptr, unsigned* ynz = nullptr);
 void launch_spmv_primal(cudaStream_t s, const DevSell& A, PdhgState* st, const double* y0, const double* y1,
                         const double* x0, const double* x1, double* aty0, double* aty1, ReduceScratch rs,
                         double* atysum = nullptr);
