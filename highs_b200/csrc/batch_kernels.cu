@@ -469,6 +469,347 @@ hip_batch_round_kernel(const HipBatchMember* __restrict__ members, const HipStat
   hip_batch_check(M, 1, args, out);
 }
 
+// ============================================================================================ HiPDLP tree-mode members
+// b200pdlp_solve_hipdlp_batch_mixed's members past ordered_max: one thread-block cluster of C CTAs per LP runs the rounds of
+// hip_batch_round_kernel (same control blocks, states and round semantics) over the member's tree-mode layouts.  A tree-mode
+// solve_hipdlp_on_device has two kinds of sums, and neither depends on its launch shapes:
+//   * SpMV rows: a body row is summed in its entry order (lane = row, k ascending, padding adds 0 * in[0]); a long row is
+//     cut into segments of kNnzBlk entries, each summed by one kThreads CTA (thread t adds entries nnz_begin + t, + kThreads,
+//     ..., then block_sum's tree), and the segment partials are added in segment order from 0.0.
+//   * check and power-method sums (hip_check_tree_kernel, hip_dot_tree_kernel): ew_grid(len) CTAs, a count capped by a
+//     constant, each with its one element per thread (len <= 262144 keeps the grid below kMaxEwBlocks), warp_sum, the 8 warp
+//     sums in order from 0.0, then grid_reduce's combine of the block partials.
+// So rank r of the cluster stands in for the one-problem kernels' CTAs b == r (mod C) -- 8-slice body blocks, long-row
+// segments, the check's blocks -- one after the other, with the same per-thread code; the partials go to the member's
+// scratch and every phase ends at a cluster barrier.  The bits do not depend on C.  No cluster waits on another cluster,
+// so any number of members runs, resident or not.
+// The vectors written inside a round are read through plain (coherent) loads: another CTA of the cluster wrote them, and the
+// barrier's release / acquire is what makes them visible.
+
+__device__ __forceinline__ unsigned cluster_id() { unsigned r; asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r)); return r; }
+__device__ __forceinline__ unsigned cluster_rank() { unsigned r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
+__device__ __forceinline__ unsigned cluster_size() { unsigned r; asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r)); return r; }
+// every thread of the cluster: writes before it (global and shared) visible to every thread of the cluster after it
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+
+// this CTA's place in its cluster
+struct TreeCta {
+  int rank, C;
+  __device__ int first() const { return rank * kThreads + (int)threadIdx.x; }   // element loops: i = first(), += stride()
+  __device__ int stride() const { return C * kThreads; }
+};
+
+// the body rows of a sliced-ELL matrix times `in`, over the 8-slice blocks b == rank (mod C) (spmv_sell_kernel's body CTA b:
+// warp w takes slice 8 b + w, lane = row, k ascending); epi(row, sum) for every row whose lane is not masked
+template <class Epi>
+__device__ __forceinline__ void tree_body(const TreeCta& t, const int4* slices, const int* col, const double* val, int rows,
+                                          const double* in, Epi epi) {
+  const int nsl = (rows + 31) >> 5, lane = threadIdx.x & 31;
+  for (int sl = 8 * t.rank + (threadIdx.x >> 5); sl < nsl; sl += 8 * t.C) {
+    const int4 d = slices[sl];
+    if ((unsigned)d.z >> lane & 1u) continue;
+    const int* cp = col + d.x + lane;
+    const double* vp = val + d.x + lane;
+    double s = 0.0;
+    for (int k = 0; k < d.y; k++) s += vp[32 * k] * in[cp[32 * k]];
+    epi(sl * 32 + lane, s);
+  }
+}
+
+// the long-row segments q == rank (mod C), each as one segment CTA of spmv_sell_kernel sums it, into part[offset + segment]
+__device__ void tree_segs(const TreeCta& t, const HipTreeLong& L, const double* in, double* part, double* sm) {
+  for (int q = t.rank; q < L.nsegs; q += t.C) {
+    const int4 sg = L.segs[q];
+    double s = 0.0;
+    for (int e = sg.y + threadIdx.x; e < sg.z; e += kThreads) s += L.lval[e] * in[L.lcol[e]];
+    s = block_sum(s, sm);
+    if (threadIdx.x == 0) {
+      const int4 lr = L.long_rows[sg.w];
+      part[lr.w + q - lr.y] = s;
+    }
+  }
+}
+
+// the long rows (one thread each): the segment partials added in segment order from 0.0, then epi(row, total)
+template <class Epi>
+__device__ __forceinline__ void tree_finish(const TreeCta& t, const HipTreeLong& L, const double* part, Epi epi) {
+  for (int j = t.first(); j < L.nlong; j += t.stride()) {
+    const int4 lr = L.long_rows[j];
+    double tot = 0.0;
+    for (int q = 0; q < lr.z; q++) tot += part[lr.w + q];
+    epi(lr.x, tot);
+  }
+}
+
+// out = A' in (A' = the member's second layout), body and segments; the caller ends the phase
+__device__ __forceinline__ void tree_at_phase(const TreeCta& t, const HipTreeMember& T, const double* in, double* out, double* part,
+                                              double* sm) {
+  const HipBatchMember& M = T.b;
+  tree_body(t, M.at_slices, M.at_col, M.at_val, M.n, in, [&](int r, double s) { out[r] = s; });
+  tree_segs(t, T.lat, in, part, sm);
+}
+__device__ __forceinline__ void tree_a_phase(const TreeCta& t, const HipTreeMember& T, const double* in, double* out, double* sm) {
+  const HipBatchMember& M = T.b;
+  tree_body(t, M.a_slices, M.a_col, M.a_val, M.m, in, [&](int r, double s) { out[r] = s; });
+  tree_segs(t, T.la, in, T.a_part, sm);
+}
+
+// a whole plain SpMV, A (at = false) or A', ending at a cluster barrier
+__device__ void tree_spmv(const TreeCta& t, const HipTreeMember& T, bool at, const double* in, double* out, double* sm) {
+  if (at) tree_at_phase(t, T, in, out, T.at_part[0], sm);
+  else tree_a_phase(t, T, in, out, sm);
+  cluster_sync();
+  const HipTreeLong& L = at ? T.lat : T.la;
+  if (L.nlong == 0) return;
+  tree_finish(t, L, at ? T.at_part[0] : T.a_part, [&](int r, double s) { out[r] = s; });
+  cluster_sync();
+}
+
+// grid_reduce's combine of partials p[0 .. nb): lane l adds p[l], p[l + 32], ... in four chains, then warp_sum; lane 0 holds it
+__device__ __forceinline__ double tree_combine(const double* p, int nb) {
+  const int lane = threadIdx.x & 31;
+  double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0;
+  int i = lane;
+  for (; i + 96 < nb; i += 128) {
+    const double v0 = __ldcg(p + i), v1 = __ldcg(p + i + 32), v2 = __ldcg(p + i + 64), v3 = __ldcg(p + i + 96);
+    s0 += v0; s1 += v1; s2 += v2; s3 += v3;
+  }
+  for (; i < nb; i += 32) s0 += __ldcg(p + i);
+  return warp_sum((s0 + s1) + (s2 + s3));
+}
+
+// block b's partials of NQ accumulators: warp_sum, then the 8 warp sums in order from 0.0 -> partials[q nb + b]
+template <int NQ>
+__device__ __forceinline__ void tree_block_partials(const double (&acc)[NQ], double* partials, int nb, int b,
+                                                    double (*red)[kThreads / 32]) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+#pragma unroll
+  for (int q = 0; q < NQ; q++) {
+    const double s = warp_sum(acc[q]);
+    if (lane == 0) red[q][wid] = s;
+  }
+  __syncthreads();
+  if (threadIdx.x < NQ) {
+    double s = 0.0;
+#pragma unroll
+    for (int w = 0; w < kThreads / 32; w++) s += red[threadIdx.x][w];
+    partials[(size_t)threadIdx.x * nb + b] = s;
+  }
+  __syncthreads();
+}
+
+// hip_dot_tree_kernel: a.b over hip_tree_blocks(len) blocks; every CTA of the cluster combines the partials (the same bits)
+__device__ double tree_dot(const TreeCta& t, const HipTreeMember& T, int len, const double* a, const double* b,
+                           double (*red)[kThreads / 32], double* sw) {
+  const int nb = hip_tree_blocks(len);
+  for (int blk = t.rank; blk < nb; blk += t.C) {
+    double acc[1] = {0.0};
+    const int i = blk * kThreads + threadIdx.x;
+    if (i < len) acc[0] += a[i] * b[i];
+    tree_block_partials<1>(acc, T.partials, nb, blk, red);
+  }
+  cluster_sync();
+  if (threadIdx.x < 32) {
+    const double v = tree_combine(T.partials, nb);
+    if (threadIdx.x == 0) sw[0] = v;
+  }
+  __syncthreads();
+  return sw[0];
+}
+
+// hip_check_tree_kernel's sums for args `a` into out[0..NQ) (NQ = 3: the fixed-point sums 0..2 alone, whose accumulators
+// are independent of the others'); rank 0 writes out.  Ends at a cluster barrier only when the caller needs one.
+template <int NQ>
+__device__ void tree_check_sums(const TreeCta& t, const HipTreeMember& T, const HipCheckArgs& a, int with_fpe,
+                                double* __restrict__ out, double (*red)[kThreads / 32]) {
+  const int nb = T.nb;
+  for (int b = t.rank; b < nb; b += t.C) {
+    double acc[NQ];
+#pragma unroll
+    for (int q = 0; q < NQ; q++) acc[q] = 0.0;
+    const int i = b * kThreads + threadIdx.x;
+    if (i < a.n) {
+      if (with_fpe) { const double d = a.x[i] - a.rx[i]; acc[0] += d * d; acc[2] += d * a.atdy[i]; }
+      if constexpr (NQ == 9) {
+        double r = (a.c[i] - a.aty[i]) - a.sp[i] + a.sn[i];
+        if (a.scaled) r = r * a.colscale[i];
+        acc[4] += r * r;
+        acc[5] += a.c[i] * a.x[i];
+        if (a.lo[i] > -INFINITY) acc[6] += a.lo[i] * a.sp[i];
+        if (a.up[i] < INFINITY) acc[6] -= a.up[i] * a.sn[i];
+        const double d2 = a.x[i] - a.xa[i];
+        acc[7] += d2 * d2;
+      }
+    }
+    if (i < a.m) {
+      if (with_fpe) { const double d = a.y[i] - a.ry[i]; acc[1] += d * d; }
+      if constexpr (NQ == 9) {
+        double r = a.ax[i] - a.rlo[i];
+        if (i >= a.neq) r = std_min(0.0, r);
+        if (a.scaled) r = r * a.rowscale[i];
+        acc[3] += r * r;
+        acc[6] += a.rlo[i] * a.y[i];
+        const double d2 = a.y[i] - a.ya[i];
+        acc[8] += d2 * d2;
+      }
+    }
+    tree_block_partials<NQ>(acc, T.partials, nb, b, red);
+  }
+  cluster_sync();
+  const int wid = threadIdx.x >> 5;
+  if (t.rank == 0) {
+    for (int q = wid; q < NQ; q += kThreads / 32) {
+      double v = tree_combine(T.partials + (size_t)q * nb, nb);
+      if (q == 5 || q == 6) v += a.offset;
+      if ((threadIdx.x & 31) == 0) out[q] = v;
+    }
+  }
+}
+
+// dy = yn - ry and A'dy -> atdy (hip_diff_kernel, then A'), ending at a cluster barrier
+__device__ void tree_atdy(const TreeCta& t, const HipTreeMember& T, double* sm) {
+  const HipBatchMember& M = T.b;
+  for (int r = t.first(); r < M.m; r += t.stride()) M.dy[r] = M.yn[r] - M.ry[r];
+  cluster_sync();
+  tree_spmv(t, T, true, M.dy, M.atdy, sm);
+}
+
+// hip_check: (major) dy and A'dy; A x and A'y of the checked iterate; the dual slacks; the nine sums into out[0..8]
+__device__ void tree_check(const TreeCta& t, const HipTreeMember& T, int major, const HipCheckArgs& a, double* out, double* sm,
+                           double (*red)[kThreads / 32]) {
+  const HipBatchMember& M = T.b;
+  if (major) {
+    for (int r = t.first(); r < M.m; r += t.stride()) M.dy[r] = M.yn[r] - M.ry[r];
+    cluster_sync();
+    tree_at_phase(t, T, M.dy, M.atdy, T.at_part[1], sm);
+  }
+  tree_a_phase(t, T, a.x, M.axp, sm);
+  tree_at_phase(t, T, a.y, M.atyp, T.at_part[0], sm);
+  cluster_sync();
+  if (T.la.nlong + T.lat.nlong > 0) {
+    auto to = [](double* v) { return [v](int r, double s) { v[r] = s; }; };
+    if (major) tree_finish(t, T.lat, T.at_part[1], to(M.atdy));
+    tree_finish(t, T.la, T.a_part, to(M.axp));
+    tree_finish(t, T.lat, T.at_part[0], to(M.atyp));
+    cluster_sync();
+  }
+  for (int i = t.first(); i < M.n; i += t.stride()) {
+    double sp, sn;
+    hip_dual_slacks(i, major, M.hslack, M.cost, M.atyp, M.lower, M.upper, sp, sn);
+    M.sp[i] = sp;
+    M.sn[i] = sn;
+  }
+  cluster_sync();
+  tree_check_sums<9>(t, T, a, major, out, red);
+}
+
+// Halpern step k_offset of the block (hip_step: hip_primal_kernel, A * reflected x with HipDualEpilogue's blend, A'y)
+__device__ void tree_step(const TreeCta& t, const HipTreeMember& T, const HipState& st, int k_offset, int is_major, double* sm) {
+  const HipBatchMember& M = T.b;
+  const double ps = st.primal_step, ds = st.dual_step;
+  const int k = st.halpern_iteration + k_offset;
+  const double w = (double)k / (k + 1.0);
+  for (int i = t.first(); i < M.n; i += t.stride())
+    hip_primal_col(i, ps, w, is_major, M.x, M.xa, M.cost, M.aty, M.lower, M.upper, M.rx, M.xn, M.hslack);
+  cluster_sync();
+  auto blend = [&](int r, double s) {
+    M.y[r] = hip_dual_blend(r, M.y[r], M.ya[r], M.rlo[r], M.rup[r], s, ds, w, is_major, M.yn, M.ry);
+  };
+  tree_body(t, M.a_slices, M.a_col, M.a_val, M.m, M.rx, blend);
+  tree_segs(t, T.la, M.rx, T.a_part, sm);
+  cluster_sync();
+  if (T.la.nlong > 0) {
+    tree_finish(t, T.la, T.a_part, blend);
+    cluster_sync();
+  }
+  tree_spmv(t, T, true, M.y, M.aty, sm);
+}
+
+// PDLPSolver::powerMethod as solve_hipdlp_on_device runs it in tree mode: q = 1; 20 times w = A'q, z = A w, z = z / |z|,
+// w' = A'z, lambda = |w'|^2, q = z.  q in dy, z in axp, w and w' in atdy (all set again later).
+__device__ double tree_power_method(const TreeCta& t, const HipTreeMember& T, double* sm, double (*red)[kThreads / 32], double* sw) {
+  const HipBatchMember& M = T.b;
+  const int n = M.n, m = M.m;
+  double* q = M.dy;
+  double* z = M.axp;
+  double* w = M.atdy;
+  for (int i = t.first(); i < m; i += t.stride()) q[i] = 1.0;
+  cluster_sync();
+  double lambda = 0.0;
+  for (int it = 0; it < 20; it++) {
+    tree_spmv(t, T, true, q, w, sm);
+    tree_spmv(t, T, false, w, z, sm);
+    const double nrm = sqrt(tree_dot(t, T, m, z, z, red, sw));   // hip_div_norm_kernel
+    for (int i = t.first(); i < m; i += t.stride()) z[i] = z[i] / nrm;
+    cluster_sync();
+    tree_spmv(t, T, true, z, w, sm);
+    lambda = tree_dot(t, T, n, w, w, red, sw);
+    for (int i = t.first(); i < m; i += t.stride()) q[i] = z[i];
+    cluster_sync();
+  }
+  return lambda;
+}
+
+__global__ void __launch_bounds__(kThreads, 3)
+hip_tree_round_kernel(const HipTreeMember* __restrict__ members, const HipState* __restrict__ states,
+                      HipBatchCtl* __restrict__ ctls) {
+  const int id = (int)cluster_id();
+  HipBatchCtl* ctl = ctls + id;
+  if (!ctl->active) return;   // the same for every CTA of the cluster
+  __shared__ HipTreeMember T;
+  __shared__ HipCheckArgs args;
+  __shared__ double sm[kThreads / 32];
+  __shared__ double red[9][kThreads / 32];
+  __shared__ double sw[1];
+  copy_words(&T, members + id);
+  const HipState st = states[id];
+  const int first = ctl->first, restart = ctl->restart, fpe = ctl->fpe;
+  const TreeCta t{(int)cluster_rank(), (int)cluster_size()};
+  double* out = ctl->outs;
+  const HipBatchMember& M = T.b;
+  __syncthreads();
+  if (first) {
+    if (M.n > 0 && M.m > 0) {
+      const double lambda = tree_power_method(t, T, sm, red, sw);
+      if (t.rank == 0 && threadIdx.x == 0) out[kHipBatchLambda] = lambda;
+    }
+    // x = xa = proj_[l,u](0) (hip_init_kernel: upper first, then lower), y = ya = 0, the other iterate vectors 0
+    for (int i = t.first(); i < M.n; i += t.stride()) {
+      double v = 0.0;
+      if (v > M.upper[i]) v = M.upper[i];
+      if (v < M.lower[i]) v = M.lower[i];
+      M.x[i] = v; M.xa[i] = v;
+      M.xn[i] = 0.0; M.rx[i] = 0.0; M.hslack[i] = 0.0; M.sp[i] = 0.0; M.sn[i] = 0.0; M.atdy[i] = 0.0;
+    }
+    for (int r = t.first(); r < M.m; r += t.stride()) {
+      M.y[r] = 0.0; M.ya[r] = 0.0; M.yn[r] = 0.0; M.ry[r] = 0.0; M.dy[r] = 0.0;
+    }
+    if (threadIdx.x == 0) hip_batch_args(M, 0, args);
+    cluster_sync();
+    tree_spmv(t, T, true, M.y, M.aty, sm);
+    tree_check(t, T, 0, args, out, sm, red);
+    return;
+  }
+  if (restart) {   // anchors and iterates <- the PDHG iterate of the last major step (:664-688)
+    for (int i = t.first(); i < M.n; i += t.stride()) { const double v = M.xn[i]; M.xa[i] = v; M.x[i] = v; }
+    for (int r = t.first(); r < M.m; r += t.stride()) { const double v = M.yn[r]; M.ya[r] = v; M.y[r] = v; }
+    cluster_sync();
+    tree_spmv(t, T, true, M.y, M.aty, sm);
+  }
+  if (threadIdx.x == 0) hip_batch_args(M, 1, args);
+  tree_step(t, T, st, 1, 1, sm);
+  if (fpe) {   // the restart's reference fixed-point error is that of the first step after it (:600-608)
+    tree_atdy(t, T, sm);
+    tree_check_sums<3>(t, T, args, 1, out + kHipBatchFpe, red);   // (the steps' barriers lie between its reads and the next writes)
+  }
+  for (int k = 2; k <= 39; k++) tree_step(t, T, st, k, 0, sm);
+  tree_step(t, T, st, 40, 1, sm);
+  tree_check(t, T, 1, args, out, sm, red);
+}
+
 }  // namespace
 
 void launch_batch_round(cudaStream_t s, int count, const BatchMember* members, PdhgState* states, BatchCtl* ctls) {
@@ -478,6 +819,34 @@ void launch_batch_round(cudaStream_t s, int count, const BatchMember* members, P
 void launch_hip_batch_round(cudaStream_t s, int count, const HipBatchMember* members, const HipState* states,
                             HipBatchCtl* ctls) {
   if (count > 0) hip_batch_round_kernel<<<count, kThreads, 0, s>>>(members, states, ctls);
+}
+
+static cudaLaunchConfig_t tree_config(cudaStream_t s, int count, int cluster, cudaLaunchAttribute* attr) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)(count * cluster));
+  cfg.blockDim = dim3(kThreads);
+  cfg.stream = s;
+  attr->id = cudaLaunchAttributeClusterDimension;
+  attr->val.clusterDim.x = (unsigned)cluster;
+  attr->val.clusterDim.y = 1;
+  attr->val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  return cfg;
+}
+
+cudaError_t launch_hip_tree_round(cudaStream_t s, int count, int cluster, const HipTreeMember* members,
+                                  const HipState* states, HipBatchCtl* ctls) {
+  if (count <= 0) return cudaSuccess;
+  cudaLaunchAttribute attr;
+  const cudaLaunchConfig_t cfg = tree_config(s, count, cluster, &attr);
+  return cudaLaunchKernelEx(&cfg, hip_tree_round_kernel, members, states, ctls);
+}
+
+cudaError_t hip_tree_max_clusters(int count, int cluster, int* out) {
+  cudaLaunchAttribute attr;
+  const cudaLaunchConfig_t cfg = tree_config(nullptr, count, cluster, &attr);
+  return cudaOccupancyMaxActiveClusters(out, (const void*)hip_tree_round_kernel, &cfg);
 }
 
 }  // namespace b200

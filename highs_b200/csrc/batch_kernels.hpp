@@ -93,4 +93,41 @@ struct HipBatchCtl {
 void launch_hip_batch_round(cudaStream_t s, int count, const HipBatchMember* members, const HipState* states,
                             HipBatchCtl* ctls);
 
+// ---- tree-mode members of b200pdlp_solve_hipdlp_batch_mixed: one thread-block cluster of C CTAs per LP, the rounds of
+// hip_batch_round_kernel over the member's tree-mode layouts (length-sorted rows, long rows cut into segments)
+
+// ew_grid of pdhg_kernels.cu: the CTAs of the one-problem check and dot kernels over `len` elements
+__host__ __device__ inline int hip_tree_blocks(int len) {
+  int g = (len + kThreads - 1) / kThreads;
+  if (g < 1) g = 1;
+  return g > kMaxEwBlocks ? kMaxEwBlocks : g;
+}
+
+// the long rows of one matrix (SellMatrix::segs / long_rows / lcol / lval); the body's lanes of these rows are masked
+struct HipTreeLong {
+  int nsegs, nlong;
+  const int4* segs;        // {row, nnz_begin, nnz_end, long_id}
+  const int4* long_rows;   // {row, first_seg, nseg, partial_offset}
+  const int* lcol;
+  const double* lval;
+};
+
+// One tree-mode member: the HipBatchMember (vectors, scalars, sliced-ELL bodies) and the long rows of A and A', with its
+// scratch: the block partials of a check or a dot product ([9][nb], nb = hip_tree_blocks(max(n, m))), A's segment partials
+// and two sets of A''s (a check runs A'dy and A'y side by side)
+struct HipTreeMember {
+  HipBatchMember b;
+  HipTreeLong la, lat;
+  int nb, pad;
+  double* partials;
+  double* a_part;
+  double* at_part[2];
+};
+
+// One round for every active tree member: cluster `id` of `cluster` CTAs = member id; states / ctls indexed likewise
+cudaError_t launch_hip_tree_round(cudaStream_t s, int count, int cluster, const HipTreeMember* members,
+                                  const HipState* states, HipBatchCtl* ctls);
+// how many clusters of `cluster` CTAs of the round kernel the current device holds at once (cudaOccupancyMaxActiveClusters)
+cudaError_t hip_tree_max_clusters(int count, int cluster, int* out);
+
 }  // namespace b200

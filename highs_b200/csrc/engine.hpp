@@ -534,5 +534,6 @@ double dev_mismatches(const T* dev, const T* host, size_t count) {
 // engine_hipdlp.cu
 void hip_host_postsolve(const b200pdlp_lp& lp, const StdForm& f, const int* cperm, const int* rperm, const double* x,
                         const double* y, const double* sp, const double* sn, b200pdlp_result* out);
+void hip_trace_row(b200pdlp_result* out, const HipController& ctl, const double* sums, bool restart, bool converged);
 
 }  // namespace b200

@@ -35,6 +35,27 @@ static void check_ordered_member(const b200pdlp_lp* lp, int ordered_max, double 
   if (rc != B200PDLP_OK) throw Error(rc, std::string(who) + ": member " + std::to_string(i) + ": " + g_last_error);
 }
 
+// a member of b200pdlp_solve_hipdlp_batch_mixed: true for a tree member (HiPDLP's classification puts its standard form past
+// ordered_max, or ordered_max < 0), which must fit the cluster kernel (batch_kernels.cu: every check sum and dot product one
+// element per thread of hip_tree_blocks' grid); checked before any device work
+constexpr int kTreeMemberMax = 262144;
+static bool check_mixed_member(const b200pdlp_lp* lp, int ordered_max, int i, const char* who) {
+  bool tree = false;
+  const int rc = guarded([&] {
+    check_lp(lp);
+    const int omax = ordered_max == 0 ? 4096 : ordered_max;
+    const int n = std_form_cols(*lp, std::numeric_limits<double>::infinity());
+    const int big = std::max(n, lp->num_row);
+    tree = omax < 0 || big > omax;
+    if (tree && big > kTreeMemberMax)
+      throw Error(B200PDLP_ERR_ARG, "standard form " + std::to_string(lp->num_row) + " x " + std::to_string(n) +
+                                        " exceeds max(n, m) = " + std::to_string(kTreeMemberMax) +
+                                        " of a tree member: solve it with b200pdlp_solve_hipdlp");
+  });
+  if (rc != B200PDLP_OK) throw Error(rc, std::string(who) + ": member " + std::to_string(i) + ": " + g_last_error);
+  return tree;
+}
+
 struct BatchRun {   // one member's host control over the rounds
   StdForm f;        // b200pdlp_solve_batch_device fills the scalars only: dimensions, sense, offset, norms, amax
   double cost_sq = 0.0, rhs_sq = 0.0;   // |c|^2 and |b|^2 of the scaled form, index order: what sets beta
@@ -49,7 +70,16 @@ struct BatchRun {   // one member's host control over the rounds
 struct PooledMember {
   HostLayout L;
   size_t vec = 0, sl_a = 0, sl_at = 0, e_a = 0, e_at = 0;
+  // tree-mode layouts only (b200pdlp_solve_hipdlp_batch_mixed): the long rows' descriptors, entries and the scratch
+  size_t sg_a = 0, lr_a = 0, sg_at = 0, lr_at = 0, le_a = 0, le_at = 0, scr = 0;
 };
+
+// the scratch doubles of a tree-mode member (HipTreeMember): the check's block partials and the segment partials of A and,
+// twice, of A'; none for an ordered layout
+static size_t tree_scratch_len(const PooledMember& b) {
+  if (b.L.ordered) return 0;
+  return 9 * (size_t)hip_tree_blocks(std::max(b.L.A.ncols, b.L.A.nrows)) + (size_t)b.L.A.n_partials + 2 * (size_t)b.L.AT.n_partials;
+}
 
 struct BatchHost : BatchRun, PooledMember {   // one member of b200pdlp_solve_batch on the host
   std::vector<double> x0, y0;
@@ -76,6 +106,10 @@ static void set_layouts(D& M, const int4* a_slices, const int* a_col, const doub
   M.a_slices = a_slices; M.a_col = a_col; M.a_val = a_val;
   M.at_slices = at_slices; M.at_col = at_col; M.at_val = at_val;
 }
+static void set_layouts(HipTreeMember& M, const int4* a_slices, const int* a_col, const double* a_val, const int4* at_slices,
+                        const int* at_col, const double* at_val) {
+  set_layouts(M.b, a_slices, a_col, a_val, at_slices, at_col, at_val);
+}
 
 // The pooled device buffers of a host-array batch: every member's vector block, and the slice descriptors, column ids and
 // values of its A and A'
@@ -84,6 +118,9 @@ struct BatchPools {
   DevBuf<double> vec, val;
   DevBuf<int> col;
   DevBuf<int4> sl;
+  DevBuf<int4> lsg;           // tree-mode layouts: segs and long_rows of A and A'
+  DevBuf<int> lcol;
+  DevBuf<double> lval, scr;
 };
 
 // Lays the members out in the pools (block_len(n, m): the doubles of a vector block), packs their layouts, lets fill(i, v)
@@ -93,18 +130,27 @@ template <class D, class Member, class Fill, class Describe>
 static void upload_pools(cudaStream_t s, std::vector<Member>& B, size_t (*block_len)(int, int), Fill&& fill,
                          Describe&& describe, BatchPools& P, DevBuf<D>& dmem) {
   const int count = (int)B.size();
-  size_t nvec = 0, nsl = 0, nent = 0;
+  size_t nvec = 0, nsl = 0, nent = 0, nlsg = 0, nle = 0, nscr = 0;
   for (Member& b : B) {
     b.vec = nvec; nvec += block_len(b.f.n, b.f.m);
     b.sl_a = nsl; nsl += b.L.A.slices.size();
     b.sl_at = nsl; nsl += b.L.AT.slices.size();
     b.e_a = nent; nent += b.L.A.col.size();
     b.e_at = nent; nent += b.L.AT.col.size();
+    b.sg_a = nlsg; nlsg += b.L.A.segs.size();
+    b.lr_a = nlsg; nlsg += b.L.A.long_rows.size();
+    b.sg_at = nlsg; nlsg += b.L.AT.segs.size();
+    b.lr_at = nlsg; nlsg += b.L.AT.long_rows.size();
+    b.le_a = nle; nle += b.L.A.segs.empty() ? 0 : b.L.A.lcol.size();
+    b.le_at = nle; nle += b.L.AT.segs.empty() ? 0 : b.L.AT.lcol.size();
+    b.scr = nscr; nscr += tree_scratch_len(b);
   }
   P.hvec.assign(std::max<size_t>(nvec, 1), 0.0);
   std::vector<double> hval(std::max<size_t>(nent, 1), 0.0);
   std::vector<int> hcol(std::max<size_t>(nent, 1), 0);
-  std::vector<int4> hsl(std::max<size_t>(nsl, 1));
+  std::vector<int4> hsl(std::max<size_t>(nsl, 1)), hlsg(std::max<size_t>(nlsg, 1));
+  std::vector<int> hlcol(std::max<size_t>(nle, 1), 0);
+  std::vector<double> hlval(std::max<size_t>(nle, 1), 0.0);
   for_members(count, [&](int i) {
     const Member& b = B[i];
     fill(i, P.hvec.data() + b.vec);
@@ -115,8 +161,20 @@ static void upload_pools(cudaStream_t s, std::vector<Member>& B, size_t (*block_
     std::copy(b.L.AT.col.begin(), b.L.AT.col.end(), hcol.begin() + b.e_at);
     std::copy(b.L.A.val.begin(), b.L.A.val.end(), hval.begin() + b.e_a);
     std::copy(b.L.AT.val.begin(), b.L.AT.val.end(), hval.begin() + b.e_at);
+    static_assert(sizeof(SellMatrix::Seg) == sizeof(int4) && sizeof(SellMatrix::LongRow) == sizeof(int4), "descriptor layout");
+    auto longs = [&](const SellMatrix& S, size_t sg, size_t lr, size_t le) {
+      if (S.segs.empty()) return;
+      memcpy(hlsg.data() + sg, S.segs.data(), S.segs.size() * sizeof(int4));
+      memcpy(hlsg.data() + lr, S.long_rows.data(), S.long_rows.size() * sizeof(int4));
+      std::copy(S.lcol.begin(), S.lcol.end(), hlcol.begin() + le);
+      std::copy(S.lval.begin(), S.lval.end(), hlval.begin() + le);
+    };
+    longs(b.L.A, b.sg_a, b.lr_a, b.le_a);
+    longs(b.L.AT, b.sg_at, b.lr_at, b.le_at);
   });
   P.vec.alloc(P.hvec.size(), false); P.val.alloc(hval.size(), false); P.col.alloc(hcol.size(), false); P.sl.alloc(hsl.size(), false);
+  if (nlsg > 0) { P.lsg.alloc(hlsg.size(), false); P.lcol.alloc(hlcol.size(), false); P.lval.alloc(hlval.size(), false); }
+  if (nscr > 0) P.scr.alloc(nscr, false);
   dmem.alloc(count, false);
   std::vector<D> hmem((size_t)count);
   for (int i = 0; i < count; i++) {
@@ -128,6 +186,11 @@ static void upload_pools(cudaStream_t s, std::vector<Member>& B, size_t (*block_
   CUDA_OK(cudaMemcpyAsync(P.val.p, hval.data(), hval.size() * sizeof(double), cudaMemcpyHostToDevice, s));
   CUDA_OK(cudaMemcpyAsync(P.col.p, hcol.data(), hcol.size() * sizeof(int), cudaMemcpyHostToDevice, s));
   CUDA_OK(cudaMemcpyAsync(P.sl.p, hsl.data(), hsl.size() * sizeof(int4), cudaMemcpyHostToDevice, s));
+  if (nlsg > 0) {
+    CUDA_OK(cudaMemcpyAsync(P.lsg.p, hlsg.data(), hlsg.size() * sizeof(int4), cudaMemcpyHostToDevice, s));
+    CUDA_OK(cudaMemcpyAsync(P.lcol.p, hlcol.data(), hlcol.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    CUDA_OK(cudaMemcpyAsync(P.lval.p, hlval.data(), hlval.size() * sizeof(double), cudaMemcpyHostToDevice, s));
+  }
   CUDA_OK(cudaMemcpyAsync(dmem.p, hmem.data(), (size_t)count * sizeof(D), cudaMemcpyHostToDevice, s));
   CUDA_OK(cudaStreamSynchronize(s));
 }
@@ -778,6 +841,7 @@ struct HipBatchRun {   // one member's host control over the rounds
   HipController ctl;
   bool converged = false, timed_out = false;
   int sol = 0;   // converged: 0 at the iteration-0 check (x, y), 1 after a block (xn, yn)
+  b200pdlp_result* trace = nullptr;   // b200pdlp_solve_hipdlp_batch_mixed: the result whose trace rows the blocks write
 };
 
 struct HipBatchHost : HipBatchRun, PooledMember {};   // one member of b200pdlp_solve_hipdlp_batch on the host
@@ -796,11 +860,14 @@ static void hip_batch_member(HipBatchMember& M, const StdForm& f, int neq, doubl
   M.y = r(V::kY); M.ya = r(V::kYa); M.yn = r(V::kYn); M.ry = r(V::kRy); M.axp = r(V::kAxp); M.dy = r(V::kDy);
 }
 
-// The rounds of a HiPDLP batch, for both entry points: one upload of the control blocks and states, one launch, one
-// read-back, then each member's HipController decisions in the order solve_hipdlp_on_device takes them, until no member is
-// active or the time limit has passed.
+// The rounds of a HiPDLP batch, for every entry point: one upload of the control blocks and states, one launch per group,
+// one read-back, then each member's HipController decisions in the order solve_hipdlp_on_device takes them, until no member
+// is active or the time limit has passed.  Members [0, count - ntree) are ordered members (dmem, one CTA each), the rest
+// tree members (dtree, one cluster of `cluster` CTAs each).
 static BatchLoop hip_batch_rounds(cudaStream_t s, int count, const b200pdlp_hipdlp_params& prm, const HipBatchMember* dmem,
-                                  const std::vector<HipBatchRun*>& B) {
+                                  const std::vector<HipBatchRun*>& B, const HipTreeMember* dtree = nullptr, int ntree = 0,
+                                  int cluster = 1) {
+  const int nord = count - ntree;
   using clk = std::chrono::steady_clock;
   DevBuf<HipState> dst;
   DevBuf<HipBatchCtl> dctl;
@@ -833,7 +900,8 @@ static BatchLoop hip_batch_rounds(cudaStream_t s, int count, const b200pdlp_hipd
     CUDA_OK(cudaMemcpyAsync(dctl.p, hctl.p, (size_t)count * sizeof(HipBatchCtl), cudaMemcpyHostToDevice, s));
     CUDA_OK(cudaMemcpyAsync(dst.p, hst.p, (size_t)count * sizeof(HipState), cudaMemcpyHostToDevice, s));
     CUDA_OK(cudaEventRecord(ev0, s));
-    launch_hip_batch_round(s, count, dmem, dst.p, dctl.p);
+    launch_hip_batch_round(s, nord, dmem, dst.p, dctl.p);
+    CUDA_OK(launch_hip_tree_round(s, ntree, cluster, dtree, dst.p + nord, dctl.p + nord));
     CUDA_OK(cudaEventRecord(ev1, s));
     CUDA_OK(cudaMemcpyAsync(hctl.p, dctl.p, (size_t)count * sizeof(HipBatchCtl), cudaMemcpyDeviceToHost, s));
     CUDA_OK(cudaStreamSynchronize(s));
@@ -857,7 +925,10 @@ static BatchLoop hip_batch_rounds(cudaStream_t s, int count, const b200pdlp_hipd
       } else {
         if (c.fpe) ctl.restart_reference(c.outs + kHipBatchFpe);
         restart = ctl.after_block(c.outs);
-        if (ctl.pfeas < ctl.tol * (1.0 + f.norm_rhs) && ctl.dfeas < ctl.tol * (1.0 + f.norm_cost) && ctl.relgap < ctl.tol) {
+        const bool block_converged =
+            ctl.pfeas < ctl.tol * (1.0 + f.norm_rhs) && ctl.dfeas < ctl.tol * (1.0 + f.norm_cost) && ctl.relgap < ctl.tol;
+        if (b.trace) hip_trace_row(b.trace, ctl, c.outs, restart, block_converged);
+        if (block_converged) {
           b.converged = true; b.sol = 1; done = true;
         } else {
           done = ctl.iters >= prm.iter_limit;
@@ -896,23 +967,49 @@ static void hip_batch_result(b200pdlp_result* out, const HipBatchRun& b, const B
   out->form_cols = f.n; out->form_rows = f.m; out->form_nnz = f.nnz; out->form_neq = f.neq;
 }
 
-static void solve_hipdlp_batch(int count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params& prm, b200pdlp_result* outs) {
+// b200pdlp_solve_hipdlp_batch_mixed: the same rounds for members of any size up to kTreeMemberMax.  The tree-mode members
+// (past ordered_max) take their tree layouts from the same host prologue and run on hip_tree_round_kernel (batch_kernels.cu),
+// one thread-block cluster each, beside the ordered members' CTAs; each returns the bits b200pdlp_solve_hipdlp returns for it.
+// STATUS: runs on hardware; tests/test_gpu_hipdlp_batch_mixed.py, tools/hipdlp_batch_mixed_bench.py (DESIGN.md section 6).
+
+// B200PDLP_BATCH_CLUSTER=1|2|4|8 (tests, benchmarks), otherwise the largest C in {8, 4, 2} with which every one of the
+// `ntree` clusters of the round kernel is resident at once, otherwise 1.  C changes no result (see batch_kernels.cu).
+static int tree_cluster(int ntree) {
+  if (const char* e = getenv("B200PDLP_BATCH_CLUSTER")) {
+    const int c = atoi(e);
+    if (c != 1 && c != 2 && c != 4 && c != 8) throw Error(B200PDLP_ERR_ARG, "B200PDLP_BATCH_CLUSTER must be 1, 2, 4 or 8");
+    return c;
+  }
+  for (int c : {8, 4, 2}) {
+    int fit = 0;
+    if (hip_tree_max_clusters(ntree, c, &fit) != cudaSuccess) { cudaGetLastError(); continue; }
+    if (fit >= ntree) return c;
+  }
+  return 1;
+}
+
+// b200pdlp_solve_hipdlp_batch and _batch_mixed (`mixed`: the results take the blocks' trace rows): device member k is the
+// caller's member src[k]; members [0, count - ntree) are ordered members, the others tree members
+static void solve_hipdlp_batch(int count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params& prm, b200pdlp_result* outs,
+                               const std::vector<int>& src, int ntree, bool mixed) {
   using clk = std::chrono::steady_clock;
   const auto t_begin = clk::now();
   Laps lap;
   select_device(prm.device);
   StreamHolder sh;
   cudaStream_t s = sh.s;
+  const int nord = count - ntree;
   std::vector<HipBatchHost> B((size_t)count);
   {
     NvtxRange nvtx("b200pdlp: HiPDLP batch prologue (host threads)");
-    for_members(count, [&](int i) {
-      HipBatchHost& b = B[i];
-      formulate_hipdlp(lps[i], b.f);
+    for_members(count, [&](int k) {
+      HipBatchHost& b = B[k];
+      formulate_hipdlp(lps[src[k]], b.f);
       scale_hipdlp(b.f, prm.scaling_mode, prm.ruiz_iterations);
       build_layout(b.f, 0, 1, prm.ordered_max, b.L);
-      if (!b.L.ordered || !b.L.A.segs.empty() || !b.L.AT.segs.empty())
+      if (k < nord && (!b.L.ordered || !b.L.A.segs.empty() || !b.L.AT.segs.empty()))
         throw Error(B200PDLP_ERR_STATE, "the layout is not an ordered-mode layout");
+      if (k >= nord && b.L.ordered) throw Error(B200PDLP_ERR_STATE, "the layout is not a tree-mode layout");
     });
   }
   lap("batch", "HiPDLP prologue (host threads)");
@@ -920,9 +1017,9 @@ static void solve_hipdlp_batch(int count, const b200pdlp_lp* lps, const b200pdlp
   // ---- the pools, one descriptor per member; the vectors in device order, as create_problem_hipdlp uploads them
   using V = HipBatchVec;
   BatchPools pools;
-  DevBuf<HipBatchMember> dmem;
-  upload_pools(s, B, V::len, [&](int i, double* v) {
-    const HipBatchHost& b = B[i];
+  DevBuf<HipTreeMember> dtree;
+  upload_pools(s, B, V::len, [&](int k, double* v) {
+    const HipBatchHost& b = B[k];
     const StdForm& f = b.f;
     const int n = f.n, m = f.m;
     const int* cperm = b.L.cperm.data();
@@ -934,12 +1031,38 @@ static void solve_hipdlp_batch(int count, const b200pdlp_lp* lps, const b200pdlp
     }
     double *rlo = V::row(v, n, m, V::kRlo), *rup = V::row(v, n, m, V::kRup), *rowscale = V::row(v, n, m, V::kRowscale);
     for (int r = 0; r < m; r++) { rlo[r] = f.rhs[rperm[r]]; rup[r] = f.row_upper[rperm[r]]; rowscale[r] = f.row_scale[rperm[r]]; }
-  }, [&](HipBatchMember& M, int i, double* v) { hip_batch_member(M, B[i].f, B[i].L.neq_local, v); }, pools, dmem);
+  }, [&](HipTreeMember& M, int k, double* v) {
+    const HipBatchHost& b = B[k];
+    hip_batch_member(M.b, b.f, b.L.neq_local, v);
+    auto longs = [&](HipTreeLong& T, const SellMatrix& S, size_t sg, size_t lr, size_t le) {
+      T.nsegs = (int)S.segs.size(); T.nlong = (int)S.long_rows.size();
+      T.segs = pools.lsg.p + sg; T.long_rows = pools.lsg.p + lr; T.lcol = pools.lcol.p + le; T.lval = pools.lval.p + le;
+    };
+    longs(M.la, b.L.A, b.sg_a, b.lr_a, b.le_a);
+    longs(M.lat, b.L.AT, b.sg_at, b.lr_at, b.le_at);
+    M.nb = hip_tree_blocks(std::max(b.f.n, b.f.m));
+    if (b.L.ordered) return;
+    M.partials = pools.scr.p + b.scr;
+    M.a_part = M.partials + 9 * (size_t)M.nb;
+    M.at_part[0] = M.a_part + b.L.A.n_partials;
+    M.at_part[1] = M.at_part[0] + b.L.AT.n_partials;
+  }, pools, dtree);
+  // the ordered members' descriptors: the HipBatchMember that leads each of their HipTreeMember descriptors
+  DevBuf<HipBatchMember> dmem;
+  dmem.alloc(nord, false);
+  if (nord > 0)
+    CUDA_OK(cudaMemcpy2DAsync(dmem.p, sizeof(HipBatchMember), dtree.p, sizeof(HipTreeMember), sizeof(HipBatchMember), nord,
+                              cudaMemcpyDeviceToDevice, s));
+  const int cluster = ntree > 0 ? tree_cluster(ntree) : 1;
   lap("batch", "pools + upload");
+  if (lap.on && ntree > 0) fprintf(stderr, "[b200pdlp batch] tree members %d, cluster of C = %d CTAs each\n", ntree, cluster);
 
   std::vector<HipBatchRun*> R((size_t)count);
-  for (int i = 0; i < count; i++) R[i] = &B[i];
-  const BatchLoop loop = hip_batch_rounds(s, count, prm, dmem.p, R);
+  for (int k = 0; k < count; k++) {
+    R[k] = &B[k];
+    if (mixed) { B[k].trace = outs + src[k]; B[k].trace->trace_len = 0; }
+  }
+  const BatchLoop loop = hip_batch_rounds(s, count, prm, dmem.p, R, dtree.p + nord, ntree, cluster);
   lap("batch", "rounds");
 
   // ---- the host postsolve of every member (hip_host_postsolve, as the single solve's host prologue path), one download
@@ -947,15 +1070,15 @@ static void solve_hipdlp_batch(int count, const b200pdlp_lp* lps, const b200pdlp
   CUDA_OK(cudaMemcpyAsync(pools.hvec.data(), pools.vec.p, pools.hvec.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
   CUDA_OK(cudaStreamSynchronize(s));
   const double setup_seconds = std::chrono::duration<double>(loop.t_loop - t_begin).count();
-  for_members(count, [&](int i) {
-    const HipBatchHost& b = B[i];
+  for_members(count, [&](int k) {
+    const HipBatchHost& b = B[k];
     const StdForm& f = b.f;
     const int n = f.n, m = f.m;
     const double* v = pools.hvec.data() + b.vec;
     const double* x = b.converged ? V::col(v, n, b.sol ? V::kXn : V::kX) : nullptr;
     const double* y = b.converged ? V::row(v, n, m, b.sol ? V::kYn : V::kY) : nullptr;
-    b200pdlp_result* out = outs + i;
-    hip_host_postsolve(lps[i], f, b.L.cperm.data(), b.L.rperm.data(), x, y, V::col(v, n, V::kSp), V::col(v, n, V::kSn), out);
+    b200pdlp_result* out = outs + src[k];
+    hip_host_postsolve(lps[src[k]], f, b.L.cperm.data(), b.L.rperm.data(), x, y, V::col(v, n, V::kSp), V::col(v, n, V::kSn), out);
     hip_batch_result(out, b, loop, setup_seconds);
   });
   lap("batch", "postsolve (host threads)");
@@ -1348,7 +1471,21 @@ int b200pdlp_solve_hipdlp_batch(int32_t count, const b200pdlp_lp* lps, const b20
   return batch_entry(who, count, lps && params && outs, [&] {
     for (int i = 0; i < count; i++)
       check_ordered_member(&lps[i], params->ordered_max, std::numeric_limits<double>::infinity(), i, who);
-    solve_hipdlp_batch(count, lps, *params, outs);
+    std::vector<int> src((size_t)count);
+    for (int i = 0; i < count; i++) src[i] = i;
+    solve_hipdlp_batch(count, lps, *params, outs, src, 0, false);
+  });
+}
+
+int b200pdlp_solve_hipdlp_batch_mixed(int32_t count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params* params,
+                                      b200pdlp_result* outs) {
+  const char* who = "b200pdlp_solve_hipdlp_batch_mixed";
+  return batch_entry(who, count, lps && params && outs, [&] {
+    std::vector<int> src, tree;   // the ordered members first, then the tree members, each group in the caller's order
+    for (int i = 0; i < count; i++) (check_mixed_member(&lps[i], params->ordered_max, i, who) ? tree : src).push_back(i);
+    const int ntree = (int)tree.size();
+    src.insert(src.end(), tree.begin(), tree.end());
+    solve_hipdlp_batch(count, lps, *params, outs, src, ntree, true);
   });
 }
 

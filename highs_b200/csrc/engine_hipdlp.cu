@@ -325,7 +325,7 @@ static double hip_power_method(b200pdlp_problem* p) {
 
 // one row of b200pdlp_result::trace per block (B200PDLP_HIP_TRACE_COLS, include/b200pdlp.h) from the block-end check's sums
 // and the controller's decisions: host values the loop already holds, no device work
-static void hip_trace_row(b200pdlp_result* out, const HipController& ctl, const double* sums, bool restart, bool converged) {
+void hip_trace_row(b200pdlp_result* out, const HipController& ctl, const double* sums, bool restart, bool converged) {
   if (!out->trace || out->trace_len >= out->trace_cap) return;
   double* t = out->trace + (size_t)out->trace_len * B200PDLP_HIP_TRACE_COLS;
   t[0] = ctl.iters;

@@ -82,7 +82,7 @@ ABI_SYMBOLS = [
     "b200pdlp_solve_hipdlp_batch", "b200pdlp_solve_batch_device", "b200pdlp_debug_batch_prep_compare",
     "b200pdlp_solve_hipdlp_batch_device", "b200pdlp_debug_hipdlp_batch_prep_compare", "b200pdlp_kkt_check_batch",
     "b200pdlp_kkt_check_batch_device", "b200pdlp_hipdlp_problem_create", "b200pdlp_hipdlp_step", "b200pdlp_hipdlp_check",
-    "b200pdlp_hipdlp_problem_power_method",
+    "b200pdlp_hipdlp_problem_power_method", "b200pdlp_solve_hipdlp_batch_mixed",
 ]
 HIP_TRACE_COLS = 16   # B200PDLP_HIP_TRACE_COLS: the per-block trace of the HiPDLP solves
 
@@ -596,6 +596,26 @@ def solve_hipdlp_batch(lps, **params) -> list:
         arrays.append(a)
     prm = _hipdlp_params(params)
     _check(L.b200pdlp_solve_hipdlp_batch(count, clps, C.byref(prm), cres), "b200pdlp_solve_hipdlp_batch")
+    return [_result_dict(cres[i], arrays[i]) for i in range(count)]
+
+
+def solve_hipdlp_batch_mixed(lps, trace_cap: int = 0, **params) -> list:
+    """b200pdlp_solve_hipdlp_batch_mixed: solve_hipdlp_batch for LPs of any size up to max(n, m) = 262144, in any order.
+    Ordered-mode members return what solve_hipdlp_batch returns for them; every other member (a tree member: one
+    thread-block cluster of the GPU per LP) returns what solve_hipdlp returns for it alone, bit for bit, and with
+    trace_cap > 0 its "trace" rows too.  ordered_max=-1 makes every member a tree member."""
+    lps = list(lps)
+    L = lib()
+    L.b200pdlp_solve_hipdlp_batch_mixed.argtypes = [C.c_int32, C.POINTER(CLp), C.POINTER(CHipdlpParams), C.POINTER(CResult)]
+    count = len(lps)
+    clps, cres, keep, arrays = (CLp * max(count, 1))(), (CResult * max(count, 1))(), [], []
+    for i, lp in enumerate(lps):
+        clps[i], k = make_clp(lp)
+        keep.append(k)
+        cres[i], a = _mk_result(lp, trace_cap)
+        arrays.append(a)
+    prm = _hipdlp_params(params)
+    _check(L.b200pdlp_solve_hipdlp_batch_mixed(count, clps, C.byref(prm), cres), "b200pdlp_solve_hipdlp_batch_mixed")
     return [_result_dict(cres[i], arrays[i]) for i in range(count)]
 
 

@@ -315,6 +315,25 @@ int b200pdlp_solve_hipdlp(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params* p
  * oracle), tools/batch_bench.py --solver hipdlp. */
 int b200pdlp_solve_hipdlp_batch(int32_t count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params* params,
                                 b200pdlp_result* outs /* [count], caller-allocated like b200pdlp_result */);
+/* b200pdlp_solve_hipdlp_batch for members of any size up to a cap, in any order (host arrays).  A member whose standard form
+ * (HiPDLP's classification) has max(n, m) <= ordered_max is an ordered member and returns exactly what
+ * b200pdlp_solve_hipdlp_batch returns for it; every other member is a tree member and returns exactly what
+ * b200pdlp_solve_hipdlp(lps[i], params) returns for it alone: term_code, term_iterate, iters, passes, restarts, the residual
+ * scalars, the form dimensions and all four vectors, bit for bit.  ordered_max < 0 makes every member a tree member.  With
+ * trace storage (trace, trace_cap) every member writes the single solve's B200PDLP_HIP_TRACE_COLS rows.  Batch-wide fields
+ * as in b200pdlp_solve_hipdlp_batch (kernel_launches = the rounds).  One CTA solves an ordered member; one thread-block
+ * cluster of C CTAs (C in {1, 2, 4, 8}, the largest with which every tree member is resident at once, otherwise 1) solves a
+ * tree member; a round is one upload, up to two launches and one read-back.  The environment variable
+ * B200PDLP_BATCH_CLUSTER=1|2|4|8 forces C for tests and benchmarks; it changes no result.  B200PDLP_TIMING=1 prints the
+ * laps and the tree-member count with C.
+ * Returns B200PDLP_ERR_ARG before any device work, naming the lowest failing member, for count < 0, NULL arrays, a member
+ * that the checks of b200pdlp_solve_hipdlp reject, and a tree member whose standard form exceeds max(n, m) = 262144 (solve
+ * it with b200pdlp_solve_hipdlp); no result is written.  count == 0: B200PDLP_OK.  No device: B200PDLP_ERR_CUDA.  The whole
+ * batch must fit in device memory (B200PDLP_ERR_ALLOC otherwise).
+ * STATUS: runs on hardware; tests/test_gpu_hipdlp_batch_mixed.py (byte equality with b200pdlp_solve_hipdlp and with
+ * b200pdlp_solve_hipdlp_batch), tools/hipdlp_batch_mixed_bench.py. */
+int b200pdlp_solve_hipdlp_batch_mixed(int32_t count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params* params,
+                                      b200pdlp_result* outs /* [count], caller-allocated like b200pdlp_result */);
 /* b200pdlp_solve_hipdlp_batch for LPs that are already in GPU memory.  `lps` and `outs` are host arrays of the usual structs,
  * but every array pointer inside them is device (or managed) memory of params->device (< 0: the current device): the LP's
  * eight arrays and the four result vectors.  num_col, num_row, sense and offset are host scalars.  Each member returns exactly
