@@ -20,8 +20,8 @@ NVCC_FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17", "-fmad=false", "-Xcompile
                      "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 CXX_FLAGS = ["-O2", "-fPIC", "-std=c++17", "-ffp-contract=off", "-Wall", "-Wno-sign-compare"]
 
-SOURCES = [("host_prep.cpp", "cxx"), ("host_prep_hipdlp.cpp", "cxx"), ("pdhg_kernels.cu", "nvcc"), ("setup_kernels.cu", "nvcc"), ("device_prep.cu", "nvcc"), ("kkt_check.cu", "nvcc"), ("kkt_batch.cu", "nvcc"), ("batch_kernels.cu", "nvcc"), ("batch_prep.cu", "nvcc"), ("engine.cu", "nvcc"), ("engine_hipdlp.cu", "nvcc"), ("engine_batch.cu", "nvcc")]
-HEADERS = ["host_prep.hpp", "kernels.cuh", "pdhg_arith.cuh", "pdhg_kernels.hpp", "batch_kernels.hpp", "batch_prep.hpp", "row_index.cuh", "kkt_batch.hpp", "setup_kernels.hpp", "device_prep.hpp", "kkt_logic.hpp", "engine.hpp", os.path.join("..", "..", "include", "b200pdlp.h")]
+SOURCES = [("host_prep.cpp", "cxx"), ("host_prep_hipdlp.cpp", "cxx"), ("pdhg_kernels.cu", "nvcc"), ("setup_kernels.cu", "nvcc"), ("device_prep.cu", "nvcc"), ("kkt_check.cu", "nvcc"), ("kkt_batch.cu", "nvcc"), ("batch_kernels.cu", "nvcc"), ("batch_prep.cu", "nvcc"), ("batch_tree_prep.cu", "nvcc"), ("engine.cu", "nvcc"), ("engine_hipdlp.cu", "nvcc"), ("engine_batch.cu", "nvcc")]
+HEADERS = ["host_prep.hpp", "kernels.cuh", "pdhg_arith.cuh", "pdhg_kernels.hpp", "batch_kernels.hpp", "batch_prep.hpp", "row_index.cuh", "hip_form.cuh", "kkt_batch.hpp", "setup_kernels.hpp", "device_prep.hpp", "kkt_logic.hpp", "engine.hpp", os.path.join("..", "..", "include", "b200pdlp.h")]
 
 
 def _nvcc() -> str:

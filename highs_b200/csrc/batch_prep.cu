@@ -18,15 +18,15 @@
 // 1-norm column-ascending by the thread that owns the row, |c|^2 and |b|^2 in index order by one thread.
 #include "batch_kernels.hpp"
 #include "batch_prep.hpp"
+#include "hip_form.cuh"
 #include "host_prep.hpp"
 #include "row_index.cuh"
 
 namespace b200 {
 namespace {
 
-constexpr double kInf = __builtin_huge_val();
-
-// (block_scan and row_walk, which build the row-major indexes: row_index.cuh)
+// (block_scan and row_walk, which build the row-major indexes: row_index.cuh; kInf and the HiPDLP prologue's pieces:
+// hip_form.cuh)
 
 // max over the CTA with std::max's comparison ((a < b) ? b : a); result in every thread
 __device__ double block_max(double v, double* sm) {
@@ -556,58 +556,6 @@ __global__ void __launch_bounds__(kThreads) hip_batch_size_kernel(const BatchPre
   }
 }
 
-// a double as a radix key: ascending numeric order, -0.0 before +0.0 (device_prep.cu value_key_kernel's convention)
-__device__ __forceinline__ unsigned long long value_key(double v) {
-  const unsigned long long u = (unsigned long long)__double_as_longlong(v);
-  return (u >> 63) ? ~u : (u | 0x8000000000000000ull);
-}
-
-// The fold of one scaling pass over a column's or a row's terms, and its factor (Scaling::scaleProblem).  OP 0: Ruiz, max |v|
-// -> sqrt, 0 -> 1; 1: Pock-Chambolle with alpha = 1, sum |v| -> sqrt; 2: L2, sum v^2 -> sqrt(sqrt).  The host evaluates the
-// Pock-Chambolle terms and factors as std::pow(x, 1.0), which glibc returns exactly as x, so the identity is used here.
-template <int OP> __device__ __forceinline__ double hip_fold(double a, double v) {
-  if (OP == 0) { const double t = fabs(v); return (a < t) ? t : a; }   // std::max(a, t)
-  return OP == 1 ? a + fabs(v) : a + v * v;
-}
-template <int OP> __device__ __forceinline__ double hip_factor(double a) {
-  if (OP == 0) { const double f = sqrt(a); return f == 0.0 ? 1.0 : f; }
-  return a > 0.0 ? (OP == 1 ? sqrt(a) : sqrt(sqrt(a))) : 1.0;
-}
-
-// one scaling pass (scale_hipdlp's pass + apply_hipdlp): column folds in cbeg order, row folds in row-major order, then
-// every entry divided once by the product rs[i] * cs[j]; only finite bounds, rhs and row upper bounds are scaled
-template <int OP>
-__device__ void hip_scale_pass(const BatchPrep& P, double* cost, double* lower, double* upper, double* colscale, double* rlo,
-                               double* rup, double* rowscale) {
-  const int t = threadIdx.x, n = P.n, m = P.m;
-  for (int j = t; j < n; j += kThreads) {
-    double a = 0.0;
-    for (int p = P.cbeg[j]; p < P.cbeg[j + 1]; p++) a = hip_fold<OP>(a, P.cval[p]);
-    P.cs[j] = hip_factor<OP>(a);
-  }
-  for (int i = t; i < m; i += kThreads) {
-    double a = 0.0;
-    for (int q = P.rptr[i]; q < P.rptr[i + 1]; q++) a = hip_fold<OP>(a, P.cval[P.rpos[q]]);
-    P.rs[i] = hip_factor<OP>(a);
-  }
-  __syncthreads();
-  for (int j = t; j < n; j += kThreads) {
-    const double c = P.cs[j];
-    cost[j] /= c;
-    if (lower[j] > -kInf) lower[j] *= c;
-    if (upper[j] < kInf) upper[j] *= c;
-    colscale[j] *= c;
-    for (int p = P.cbeg[j]; p < P.cbeg[j + 1]; p++) P.cval[p] /= (P.rs[P.cidx[p]] * c);
-  }
-  for (int i = t; i < m; i += kThreads) {
-    const double r = P.rs[i];
-    if (rlo[i] > -kInf) rlo[i] /= r;
-    if (rup[i] < kInf) rup[i] /= r;
-    rowscale[i] *= r;
-  }
-  __syncthreads();
-}
-
 __global__ void __launch_bounds__(kThreads)
 hip_batch_prep_kernel(const BatchPrep* __restrict__ prep, const HipBatchPrep* __restrict__ hprep, int scaling_mode,
                       int ruiz_iterations) {
@@ -633,7 +581,9 @@ hip_batch_prep_kernel(const BatchPrep* __restrict__ prep, const HipBatchPrep* __
   if (t == 0) nsort = 0;
   __syncthreads();
 
-  // ---- formulate_hipdlp.  A structural column keeps cbeg[j] = a_start[j], its entries ordered by (new row, value) with LEQ
+  // ---- formulate_hipdlp (hip_form.cuh hip_formulate, hip_rank_entries, hip_row_indexes and hip_scale are these steps
+  // for the tree-mode prologue; this kernel keeps them written out in place, so that its machine code stays as it was).
+  // A structural column keeps cbeg[j] = a_start[j], its entries ordered by (new row, value) with LEQ
   // rows negated.  Stored rows strictly ascending: the new rows ascend inside the equality-like group and inside the rest, so
   // that order is the stable partition.  Other columns go on the work list for the sort below.  Costs keep their sign and
   // bounds are not clamped.
@@ -753,45 +703,8 @@ hip_batch_prep_kernel(const BatchPrep* __restrict__ prep, const HipBatchPrep* __
 __global__ void __launch_bounds__(kThreads)
 hip_batch_post_kernel(const BatchPrep* __restrict__ prep, const HipBatchPrep* __restrict__ hprep,
                       const HipBatchPost* __restrict__ post, int scaled) {
-  const BatchPrep& P = prep[blockIdx.x];
-  const HipBatchPrep& H = hprep[blockIdx.x];
-  const HipBatchPost& Q = post[blockIdx.x];
-  if (!(Q.col_value && Q.col_dual && Q.row_value && Q.row_dual)) return;
-  const int n0 = P.n0, m = P.m, n = P.n;
-  using V = HipBatchVec;
-  const double* v = P.vec;
-  const double* x = Q.sol == 1 ? V::col(v, n, V::kXn) : V::col(v, n, V::kX);
-  const double* y = Q.sol == 1 ? V::row(v, n, m, V::kYn) : V::row(v, n, m, V::kY);
-  const double *colscale = V::col(v, n, V::kColscale), *sp = V::col(v, n, V::kSp), *sn = V::col(v, n, V::kSn);
-  const double* rowscale = V::row(v, n, m, V::kRowscale);
-  const bool conv = Q.sol >= 0;
-  const double sense = P.sense;
-  // the unscaled primal value of structural column j (hip_host_postsolve's hx[j])
-  const auto xval = [&](int j) {
-    double xv = conv ? x[j] : 0.0;
-    if (scaled) xv /= colscale[j];
-    return xv;
-  };
-  for (int j = threadIdx.x; j < n0; j += kThreads) {
-    const double cs = colscale[j];
-    Q.col_value[j] = xval(j);
-    const double a = sp[j] * cs, b = sn[j] * cs;
-    double d = a - b;
-    d *= sense;
-    Q.col_dual[j] = d;
-  }
-  for (int i = threadIdx.x; i < m; i += kThreads) {
-    const int r = P.row_new_idx[i];
-    double d = conv ? y[r] : 0.0;
-    if (scaled) d /= rowscale[r];
-    Q.row_dual[i] = P.row_class[i] == kLeq ? -d : d;
-    double s = 0.0;   // A x along the caller's row: columns ascending, then stored order
-    for (int q = H.optr[i]; q < H.optr[i + 1]; q++) {
-      const int p = H.opos[q];
-      s += P.a_value[p] * xval(P.pcol[p]);
-    }
-    Q.row_value[i] = s;
-  }
+  const auto same = [](int k) { return k; };
+  hip_postsolve(prep[blockIdx.x], hprep[blockIdx.x], post[blockIdx.x], scaled, same, same);
 }
 
 }  // namespace

@@ -70,6 +70,42 @@ struct HipBatchPost {
   int pad;
 };
 
+// ---- tree members of b200pdlp_solve_hipdlp_batch_mixed_device (batch_tree_prep.cu): the same BatchPrep and HipBatchPrep
+// per member (P.a_slices / P.at_slices: the tree layouts' slice descriptors, P.a_col ... : their bodies; P.vec in device
+// order), plus the device orders and the long rows of A and A' (build_layout(f, 0, 1, -1): rows sorted by descending length
+// in windows, rows longer than kTreeLongRow cut into segments of kNnzPerBlock entries).
+constexpr int kTreeLongRow = 512;   // build_layout's long_threshold in tree mode
+constexpr int kTreeSortTile = 2048;   // unsorted columns: tiles ranked in shared memory, then merged in HipTreePrep::srt
+
+struct HipSortRec { int row, idx; unsigned long long key; };   // an entry of an unsorted column: (new row, stored index, value key)
+
+// What the orderings-and-plans kernel reads back per member.  err != 0: a layout past 32-bit offsets.
+struct HipTreePlan {
+  int err;
+  int pad_a, pad_at;        // padded body entries of A (m rows) and A' (n rows), before the 32 trailing zeros
+  int nseg_a, nlong_a;      // A's long-row segments (= its partial sums) and long rows
+  int nseg_at, nlong_at;
+  int maxcol;               // the longest structural column of the caller's matrix (the sort scratch)
+  long long lcount_a, lcount_at;   // entries of the long-row arrays (rows padded to multiples of 4, + 8)
+};
+
+struct HipTreePrep {
+  int* rperm; int* rinv;    // [m] device row order: rperm[device row] = form row; rinv its inverse
+  int* cperm; int* cinv;    // [n] the same for the columns
+  int cap;                  // capacity of each of the four descriptor arrays below (>= any count a plan can reach)
+  int4* a_segs; int4* a_long;     // {row, nnz_begin, nnz_end, long_id}, {row, first_seg, nseg, partial_offset}
+  int4* at_segs; int4* at_long;
+  int* a_lcol; double* a_lval;    // [lcount_a] (zeroed by the host), set after the plan
+  int* at_lcol; double* at_lval;
+  HipSortRec* srt;          // [2 maxcol] when maxcol > kTreeSortTile, else unused
+};
+
+void launch_hip_tree_plan(cudaStream_t s, int count, const BatchPrep* prep, const HipTreePrep* tprep, HipTreePlan* plans);
+void launch_hip_tree_prep(cudaStream_t s, int count, const BatchPrep* prep, const HipBatchPrep* hprep, const HipTreePrep* tprep,
+                          const HipTreePlan* plans, int scaling_mode, int ruiz_iterations);
+void launch_hip_tree_post(cudaStream_t s, int count, const BatchPrep* prep, const HipBatchPrep* hprep, const HipTreePrep* tprep,
+                          const HipBatchPost* post, int scaled);
+
 void launch_hip_batch_size(cudaStream_t s, int count, const BatchPrep* prep, BatchSize* sizes);
 void launch_hip_batch_prep(cudaStream_t s, int count, const BatchPrep* prep, const HipBatchPrep* hprep, int scaling_mode,
                            int ruiz_iterations);

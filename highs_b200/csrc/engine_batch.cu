@@ -492,11 +492,11 @@ static const char* prep_error_text(int err) {
   }
 }
 
-// Validation and sizing (one read-back of `count` records), the pools, then the prologue (one read-back of the scalar
-// records), on stream s of the current device.  lps[i] / warms[i]: host structs whose arrays are device memory.
-static void device_batch_prologue(cudaStream_t s, int count, const b200pdlp_lp* lps, const b200pdlp_warm* warms,
-                                  const PrepMode& mode, int ordered_max, const char* who, DeviceBatch& D, Laps& lap) {
-  const int omax = ordered_max == 0 ? 4096 : ordered_max;
+// The members' descriptors and the sizing kernel (the array checks, the row classes and orders, the form's dimensions):
+// one read-back of `count` records into D.size, on stream s of the current device.  lps[i] / warms[i]: host structs whose
+// arrays are device memory.
+static void device_batch_size(cudaStream_t s, int count, const b200pdlp_lp* lps, const b200pdlp_warm* warms,
+                              const PrepMode& mode, DeviceBatch& D) {
   D.hp.assign((size_t)count, BatchPrep{});
   size_t nrows = 0;
   for (int i = 0; i < count; i++) nrows += 4 * (size_t)lps[i].num_row + 1;
@@ -517,7 +517,7 @@ static void device_batch_prologue(cudaStream_t s, int count, const b200pdlp_lp* 
     P.row_class = q; P.row_new_idx = q + m; P.slack = q + 2 * m; P.rptr = q + 3 * m;
     nrows += 4 * (size_t)m + 1;
   }
-  D.prep.alloc(count, false); D.dsize.alloc(count, false); D.drec.alloc((size_t)count * kPrepRec, false);
+  D.prep.alloc(count, false); D.dsize.alloc(count, false);
   CUDA_OK(cudaMemcpyAsync(D.prep.p, D.hp.data(), (size_t)count * sizeof(BatchPrep), cudaMemcpyHostToDevice, s));
   if (mode.hip) launch_hip_batch_size(s, count, D.prep.p, D.dsize.p);
   else launch_batch_size(s, count, D.prep.p, D.dsize.p);
@@ -525,18 +525,13 @@ static void device_batch_prologue(cudaStream_t s, int count, const b200pdlp_lp* 
   D.size.resize((size_t)count);
   CUDA_OK(cudaMemcpyAsync(D.size.data(), D.dsize.p, (size_t)count * sizeof(BatchSize), cudaMemcpyDeviceToHost, s));
   CUDA_OK(cudaStreamSynchronize(s));
-  for (int i = 0; i < count; i++) {   // the lowest failing member
-    const BatchSize& z = D.size[i];
-    const std::string at = std::string(who) + ": member " + std::to_string(i) + ": ";
-    if (z.err != kPrepOk) throw Error(B200PDLP_ERR_ARG, at + prep_error_text(z.err));
-    if (std::max(z.n, lps[i].num_row) > omax)
-      throw Error(B200PDLP_ERR_ARG, at + "standard form " + std::to_string(lps[i].num_row) + " x " + std::to_string(z.n) +
-                                        " exceeds ordered_max = " + std::to_string(omax));
-    if (z.pad_a >= 2000000000 || z.pad_at >= 2000000000)
-      throw Error(B200PDLP_ERR_ARG, at + "b200pdlp: matrix too large for 32-bit slice offsets");
-  }
-  lap("batch device", "validation + sizing");
+}
 
+// The pools and the prologue kernel of ordered members whose sizing D holds (D.hp, D.size; D.prep is allocated anew when it
+// does not hold `count` descriptors), then one read-back of the scalar records, on stream s.
+static void device_batch_prep(cudaStream_t s, int count, const b200pdlp_lp* lps, const PrepMode& mode, DeviceBatch& D) {
+  if (D.prep.n != (size_t)count) D.prep.alloc(count, false);
+  D.drec.alloc((size_t)count * kPrepRec, false);
   // ---- the pools: each member's slices of them
   size_t ni = 0, nd = 0, nv = 0, nsl = 0, ne = 0;
   for (int i = 0; i < count; i++) {
@@ -595,6 +590,26 @@ static void device_batch_prologue(cudaStream_t s, int count, const b200pdlp_lp* 
     CUDA_OK(cudaMemcpyAsync(D.rec.data(), D.drec.p, D.rec.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
   }
   CUDA_OK(cudaStreamSynchronize(s));
+}
+
+// Validation and sizing (one read-back of `count` records), the pools, then the prologue (one read-back of the scalar
+// records), on stream s of the current device.  lps[i] / warms[i]: host structs whose arrays are device memory.
+static void device_batch_prologue(cudaStream_t s, int count, const b200pdlp_lp* lps, const b200pdlp_warm* warms,
+                                  const PrepMode& mode, int ordered_max, const char* who, DeviceBatch& D, Laps& lap) {
+  const int omax = ordered_max == 0 ? 4096 : ordered_max;
+  device_batch_size(s, count, lps, warms, mode, D);
+  for (int i = 0; i < count; i++) {   // the lowest failing member
+    const BatchSize& z = D.size[i];
+    const std::string at = std::string(who) + ": member " + std::to_string(i) + ": ";
+    if (z.err != kPrepOk) throw Error(B200PDLP_ERR_ARG, at + prep_error_text(z.err));
+    if (std::max(z.n, lps[i].num_row) > omax)
+      throw Error(B200PDLP_ERR_ARG, at + "standard form " + std::to_string(lps[i].num_row) + " x " + std::to_string(z.n) +
+                                        " exceeds ordered_max = " + std::to_string(omax));
+    if (z.pad_a >= 2000000000 || z.pad_at >= 2000000000)
+      throw Error(B200PDLP_ERR_ARG, at + "b200pdlp: matrix too large for 32-bit slice offsets");
+  }
+  lap("batch device", "validation + sizing");
+  device_batch_prep(s, count, lps, mode, D);
   lap("batch device", "prologue (device)");
 }
 
@@ -1241,6 +1256,419 @@ static void hipdlp_batch_prep_compare(int count, const b200pdlp_lp* lps, int sca
   }
 }
 
+// ----------------------------------------------------------- HiPDLP batch past ordered_max, LPs already on the GPU
+// b200pdlp_solve_hipdlp_batch_mixed_device: solve_hipdlp_batch_mixed for LPs whose arrays are device memory.  Every member's
+// prologue and postsolve run on the device, one CTA per member: the ordered members' in batch_prep.cu (as
+// b200pdlp_solve_hipdlp_batch_device), the tree members' in batch_tree_prep.cu.  The rounds are hip_batch_rounds with the
+// tree members on hip_tree_round_kernel.  The host reads fixed-size records per member, never an array.
+// STATUS: runs on hardware; tests/test_gpu_hipdlp_batch_mixed_device.py, tools/hipdlp_batch_mixed_device_bench.py
+// (DESIGN.md section 6).
+
+// The tree members' device prologue: the members' BatchPrep (from the sizing), HipBatchPrep, HipTreePrep and plans, and the
+// pools behind them
+struct TreeBatch {
+  std::vector<BatchPrep> hp;
+  std::vector<HipBatchPrep> hx;
+  std::vector<HipTreePrep> ht;
+  std::vector<HipTreePlan> plan;
+  std::vector<double> rec;   // [count][kPrepRec]: rec[kRecCostSq], rec[kRecRhsSq]
+  std::vector<size_t> scr;   // each member's offset in `scratch` (HipTreeMember::partials)
+  DevBuf<BatchPrep> prep;
+  DevBuf<HipBatchPrep> dhx;
+  DevBuf<HipTreePrep> dht;
+  DevBuf<HipTreePlan> dplan;
+  DevBuf<double> drec;
+  DevBuf<int> perms, ints, col, lcol;
+  DevBuf<int4> desc, slices;
+  DevBuf<double> dbls, vec, val, lval, scratch;
+  DevBuf<HipSortRec> srt;
+};
+
+// the descriptor arrays of one matrix hold at most this many long rows and segments (a long row has > kTreeLongRow entries,
+// a segment up to kNnzPerBlock)
+static int tree_desc_cap(int nnz) { return nnz / kTreeLongRow + nnz / kNnzPerBlock + 1; }
+
+// Orderings and plans of the tree members (hp: their descriptors from the sizing, lps their LPs; ids[k] names member k in
+// messages): one read-back of a HipTreePlan per member
+static void tree_batch_plan(cudaStream_t s, const std::vector<BatchPrep>& hp, const std::vector<BatchSize>& size,
+                            const std::vector<int>& ids, const char* who, TreeBatch& T) {
+  const int count = (int)hp.size();
+  T.hp = hp;
+  T.ht.assign((size_t)count, HipTreePrep{});
+  size_t np = 0, nd = 0, ns = 0;
+  for (int k = 0; k < count; k++) {
+    const size_t n = size[k].n, m = hp[k].m;
+    np += 2 * (n + m);
+    nd += 4 * (size_t)tree_desc_cap(size[k].nnz);
+    ns += (m + 31) / 32 + (n + 31) / 32;
+  }
+  T.perms.alloc(np, false); T.desc.alloc(nd, false); T.slices.alloc(ns, false);
+  np = nd = ns = 0;
+  for (int k = 0; k < count; k++) {
+    const BatchSize& z = size[k];
+    BatchPrep& P = T.hp[k];
+    HipTreePrep& H = T.ht[k];
+    const int n = z.n, m = P.m, cap = tree_desc_cap(z.nnz);
+    P.n = n; P.nnz = z.nnz; P.neq = z.neq;
+    H.rperm = T.perms.p + np; H.rinv = H.rperm + m; H.cperm = H.rinv + m; H.cinv = H.cperm + n;
+    np += 2 * ((size_t)n + m);
+    H.cap = cap;
+    H.a_segs = T.desc.p + nd; H.a_long = H.a_segs + cap; H.at_segs = H.a_long + cap; H.at_long = H.at_segs + cap;
+    nd += 4 * (size_t)cap;
+    P.a_slices = T.slices.p + ns; ns += (m + 31) / 32;
+    P.at_slices = T.slices.p + ns; ns += (n + 31) / 32;
+  }
+  T.prep.alloc(count, false); T.dht.alloc(count, false); T.dplan.alloc(count, false);
+  CUDA_OK(cudaMemcpyAsync(T.prep.p, T.hp.data(), (size_t)count * sizeof(BatchPrep), cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaMemcpyAsync(T.dht.p, T.ht.data(), (size_t)count * sizeof(HipTreePrep), cudaMemcpyHostToDevice, s));
+  launch_hip_tree_plan(s, count, T.prep.p, T.dht.p, T.dplan.p);
+  CUDA_OK(cudaGetLastError());
+  T.plan.resize((size_t)count);
+  CUDA_OK(cudaMemcpyAsync(T.plan.data(), T.dplan.p, (size_t)count * sizeof(HipTreePlan), cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaStreamSynchronize(s));
+  for (int k = 0; k < count; k++)
+    if (T.plan[k].err)
+      throw Error(B200PDLP_ERR_ARG, std::string(who) + ": member " + std::to_string(ids[k]) +
+                                        ": b200pdlp: matrix too large for 32-bit slice offsets");
+}
+
+// The pools of the tree members after their plans, then their prologue (formulate_hipdlp, scale_hipdlp, the device-order
+// vectors, the tree layouts) and one read-back of |c|^2, |b|^2 per member
+static void tree_batch_prep(cudaStream_t s, int scaling_mode, int ruiz_iterations, TreeBatch& T) {
+  const int count = (int)T.hp.size();
+  size_t ni = 0, nd = 0, nv = 0, ne = 0, nl = 0, nsrt = 0, nscr = 0;
+  T.scr.resize((size_t)count);
+  for (int k = 0; k < count; k++) {
+    const BatchPrep& P = T.hp[k];
+    const HipTreePlan& Z = T.plan[k];
+    const size_t n = P.n, m = P.m, nnz = P.nnz, n0 = P.n0;
+    ni += 3 * nnz + n + m + 1 + (m + 1) + (nnz - n + n0) + n0;
+    nd += nnz + 2 * n + m;
+    nv += HipBatchVec::len(P.n, P.m);
+    ne += (size_t)Z.pad_a + 32 + (size_t)Z.pad_at + 32;
+    nl += (size_t)Z.lcount_a + (size_t)Z.lcount_at;
+    nsrt += Z.maxcol > kTreeSortTile ? 2 * (size_t)Z.maxcol : 0;   // (each member sorts in its own scratch)
+    T.scr[k] = nscr;
+    nscr += 9 * (size_t)hip_tree_blocks(std::max(P.n, P.m)) + (size_t)Z.nseg_a + 2 * (size_t)Z.nseg_at;
+  }
+  T.ints.alloc(ni, false); T.dbls.alloc(nd, false); T.vec.alloc(nv, false);
+  T.col.alloc(ne, false); T.val.alloc(ne, false); T.lcol.alloc(nl, false); T.lval.alloc(nl, false);
+  T.scratch.alloc(nscr, false); T.srt.alloc(nsrt, false);
+  CUDA_OK(cudaMemsetAsync(T.vec.p, 0, std::max<size_t>(nv, 1) * sizeof(double), s));   // the iterates and sums start at 0
+  CUDA_OK(cudaMemsetAsync(T.lcol.p, 0, std::max<size_t>(nl, 1) * sizeof(int), s));       // fill_sell_host's zeroed lcol / lval
+  CUDA_OK(cudaMemsetAsync(T.lval.p, 0, std::max<size_t>(nl, 1) * sizeof(double), s));
+  T.hx.assign((size_t)count, HipBatchPrep{});
+  ni = nd = nv = ne = nl = nsrt = 0;
+  T.drec.alloc((size_t)count * kPrepRec, false);
+  for (int k = 0; k < count; k++) {
+    BatchPrep& P = T.hp[k];
+    HipBatchPrep& X = T.hx[k];
+    HipTreePrep& H = T.ht[k];
+    const HipTreePlan& Z = T.plan[k];
+    const int n = P.n, m = P.m, nnz = P.nnz, n0 = P.n0;
+    int* q = T.ints.p + ni;
+    P.cbeg = q; P.cidx = q + n + 1; P.pcol = P.cidx + nnz; P.rpos = P.pcol + nnz; P.rwork = P.rpos + nnz;
+    ni += 3 * (size_t)nnz + n + m + 1;
+    X.optr = T.ints.p + ni; X.opos = X.optr + m + 1; X.sortcols = X.opos + (nnz - n + n0);
+    ni += (size_t)m + 1 + (nnz - n + n0) + n0;
+    double* d = T.dbls.p + nd;
+    P.cval = d; P.cs = d + nnz; P.cs_next = P.cs + n; P.rs = P.cs_next + n;
+    nd += (size_t)nnz + 2 * (size_t)n + m;
+    P.vec = T.vec.p + nv; nv += HipBatchVec::len(n, m);
+    P.a_col = T.col.p + ne; P.a_val = T.val.p + ne; ne += (size_t)Z.pad_a + 32;
+    P.at_col = T.col.p + ne; P.at_val = T.val.p + ne; ne += (size_t)Z.pad_at + 32;
+    H.a_lcol = T.lcol.p + nl; H.a_lval = T.lval.p + nl; nl += (size_t)Z.lcount_a;
+    H.at_lcol = T.lcol.p + nl; H.at_lval = T.lval.p + nl; nl += (size_t)Z.lcount_at;
+    H.srt = T.srt.p + nsrt; nsrt += Z.maxcol > kTreeSortTile ? 2 * (size_t)Z.maxcol : 0;
+    P.rec = T.drec.p + (size_t)kPrepRec * k;
+  }
+  T.dhx.alloc(count, false);
+  CUDA_OK(cudaMemcpyAsync(T.prep.p, T.hp.data(), (size_t)count * sizeof(BatchPrep), cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaMemcpyAsync(T.dhx.p, T.hx.data(), (size_t)count * sizeof(HipBatchPrep), cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaMemcpyAsync(T.dht.p, T.ht.data(), (size_t)count * sizeof(HipTreePrep), cudaMemcpyHostToDevice, s));
+  launch_hip_tree_prep(s, count, T.prep.p, T.dhx.p, T.dht.p, T.dplan.p, scaling_mode, ruiz_iterations);
+  CUDA_OK(cudaGetLastError());
+  T.rec.assign((size_t)count * kPrepRec, 0.0);
+  CUDA_OK(cudaMemcpy2DAsync(T.rec.data(), kPrepRec * sizeof(double), T.drec.p, kPrepRec * sizeof(double), 2 * sizeof(double),
+                            count, cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaStreamSynchronize(s));
+}
+
+// member k's HipTreeMember (its vectors, layouts, long rows and scratch), for the rounds
+static HipTreeMember tree_member(const TreeBatch& T, int k, const StdForm& f) {
+  const BatchPrep& P = T.hp[k];
+  const HipTreePrep& H = T.ht[k];
+  const HipTreePlan& Z = T.plan[k];
+  HipTreeMember M{};
+  hip_batch_member(M.b, f, P.neq, P.vec);
+  set_layouts(M.b, P.a_slices, P.a_col, P.a_val, P.at_slices, P.at_col, P.at_val);
+  M.la.nsegs = Z.nseg_a; M.la.nlong = Z.nlong_a; M.la.segs = H.a_segs; M.la.long_rows = H.a_long;
+  M.la.lcol = H.a_lcol; M.la.lval = H.a_lval;
+  M.lat.nsegs = Z.nseg_at; M.lat.nlong = Z.nlong_at; M.lat.segs = H.at_segs; M.lat.long_rows = H.at_long;
+  M.lat.lcol = H.at_lcol; M.lat.lval = H.at_lval;
+  M.nb = hip_tree_blocks(std::max(P.n, P.m));
+  M.partials = T.scratch.p + T.scr[k];
+  M.a_part = M.partials + 9 * (size_t)M.nb;
+  M.at_part[0] = M.a_part + Z.nseg_a;
+  M.at_part[1] = M.at_part[0] + Z.nseg_at;
+  return M;
+}
+
+// the scalars of a member's form after a device prologue (P: its descriptor, r: its record)
+static void device_form(StdForm& f, const BatchPrep& P, const b200pdlp_lp& lp, const double* r, bool scaled) {
+  f.hipdlp = true;
+  f.n = P.n; f.m = P.m; f.nnz = P.nnz; f.neq = P.neq; f.n_orig = P.n0;
+  f.sense = lp.sense; f.offset = lp.offset;
+  f.norm_cost = std::sqrt(r[kRecCostSq]); f.norm_rhs = std::sqrt(r[kRecRhsSq]);
+  f.scaled = scaled;
+}
+
+static void solve_hipdlp_batch_mixed_device(int count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params& prm,
+                                            b200pdlp_result* outs) {
+  using clk = std::chrono::steady_clock;
+  const char* who = "b200pdlp_solve_hipdlp_batch_mixed_device";
+  const auto t_begin = clk::now();
+  Laps lap;
+  const int device = select_device(prm.device);
+  check_device_arrays(count, lps, nullptr, outs, device, who);
+  StreamHolder sh;
+  cudaStream_t s = sh.s;
+  PrepMode mode;
+  mode.hip = true; mode.scaling = prm.scaling_mode; mode.ruiz_iterations = prm.ruiz_iterations;
+  DeviceBatch D;   // every member's sizing
+  std::vector<int> src;   // device member k is the caller's member src[k]: the ordered members, then the tree members
+  int ntree = 0;
+  {
+    NvtxRange nvtx("b200pdlp: HiPDLP mixed batch validation + sizing (device)");
+    device_batch_size(s, count, lps, nullptr, mode, D);
+    const int omax = prm.ordered_max == 0 ? 4096 : prm.ordered_max;
+    std::vector<int> tree;
+    for (int i = 0; i < count; i++) {   // the lowest failing member
+      const BatchSize& z = D.size[i];
+      const std::string at = std::string(who) + ": member " + std::to_string(i) + ": ";
+      if (z.err != kPrepOk) throw Error(B200PDLP_ERR_ARG, at + prep_error_text(z.err));
+      const int m = lps[i].num_row, big = std::max(z.n, m);
+      if (omax < 0 || big > omax) {   // (a tree member's pad_a / pad_at, the ordered layout's padding, mean nothing)
+        if (big > kTreeMemberMax)
+          throw Error(B200PDLP_ERR_ARG, at + "standard form " + std::to_string(m) + " x " + std::to_string(z.n) +
+                                            " exceeds max(n, m) = " + std::to_string(kTreeMemberMax) +
+                                            " of a tree member: solve it with b200pdlp_solve_hipdlp");
+        tree.push_back(i);
+      } else {
+        if (z.pad_a >= 2000000000 || z.pad_at >= 2000000000)
+          throw Error(B200PDLP_ERR_ARG, at + "b200pdlp: matrix too large for 32-bit slice offsets");
+        src.push_back(i);
+      }
+    }
+    ntree = (int)tree.size();
+    src.insert(src.end(), tree.begin(), tree.end());
+  }
+  const int nord = count - ntree;
+  lap("batch device", "validation + sizing");
+  auto group = [&](int k0, int k1, std::vector<BatchPrep>& hp, std::vector<BatchSize>& sz, std::vector<b200pdlp_lp>& gl,
+                   std::vector<int>& ids) {
+    for (int k = k0; k < k1; k++) {
+      hp.push_back(D.hp[src[k]]); sz.push_back(D.size[src[k]]); gl.push_back(lps[src[k]]); ids.push_back(src[k]);
+    }
+  };
+  DeviceBatch O;   // the ordered members' prologue (their row maps stay in D's pools)
+  std::vector<b200pdlp_lp> olps, tlps;
+  std::vector<int> oids, tids;
+  group(0, nord, O.hp, O.size, olps, oids);
+  TreeBatch T;
+  {
+    NvtxRange nvtx("b200pdlp: HiPDLP mixed batch orderings + plans (device)");
+    std::vector<BatchPrep> thp;
+    std::vector<BatchSize> tsz;
+    group(nord, count, thp, tsz, tlps, tids);
+    if (ntree > 0) tree_batch_plan(s, thp, tsz, tids, who, T);
+  }
+  lap("batch device", "orderings + plans");
+  {
+    NvtxRange nvtx("b200pdlp: HiPDLP mixed batch prologue (device)");
+    if (nord > 0) device_batch_prep(s, nord, olps.data(), mode, O);
+    if (ntree > 0) tree_batch_prep(s, prm.scaling_mode, prm.ruiz_iterations, T);
+  }
+  lap("batch device", "prologue (device)");
+
+  const bool scaled = (prm.scaling_mode & 7) != 0;   // scale_hipdlp: any of its passes is switched on
+  std::vector<HipBatchRun> runs((size_t)count);
+  std::vector<HipBatchRun*> R((size_t)count);
+  std::vector<HipBatchMember> hmem((size_t)nord);
+  std::vector<HipTreeMember> htree((size_t)ntree);
+  for (int k = 0; k < count; k++) {
+    HipBatchRun& b = runs[k];
+    R[k] = &b;
+    b.trace = outs + src[k];
+    b.trace->trace_len = 0;
+    if (k < nord) {
+      const BatchPrep& P = O.hp[k];
+      device_form(b.f, P, lps[src[k]], O.rec.data() + (size_t)kPrepRec * k, scaled);
+      hip_batch_member(hmem[k], b.f, P.neq, P.vec);
+      set_layouts(hmem[k], P.a_slices, P.a_col, P.a_val, P.at_slices, P.at_col, P.at_val);
+    } else {
+      const int t = k - nord;
+      device_form(b.f, T.hp[t], lps[src[k]], T.rec.data() + (size_t)kPrepRec * t, scaled);
+      htree[t] = tree_member(T, t, b.f);
+    }
+  }
+  DevBuf<HipBatchMember> dmem;
+  DevBuf<HipTreeMember> dtree;
+  dmem.alloc(nord, false); dtree.alloc(ntree, false);
+  if (nord > 0) CUDA_OK(cudaMemcpyAsync(dmem.p, hmem.data(), (size_t)nord * sizeof(HipBatchMember), cudaMemcpyHostToDevice, s));
+  if (ntree > 0) CUDA_OK(cudaMemcpyAsync(dtree.p, htree.data(), (size_t)ntree * sizeof(HipTreeMember), cudaMemcpyHostToDevice, s));
+  const int cluster = ntree > 0 ? tree_cluster(ntree) : 1;
+  if (lap.on && ntree > 0) fprintf(stderr, "[b200pdlp batch] tree members %d, cluster of C = %d CTAs each\n", ntree, cluster);
+  const BatchLoop loop = hip_batch_rounds(s, count, prm, dmem.p, R, dtree.p, ntree, cluster);
+  lap("batch device", "rounds");
+
+  // ---- the postsolve of every member on the device, into the caller's vectors
+  NvtxRange nvtx_post("b200pdlp: HiPDLP mixed batch postsolve (device)");
+  std::vector<HipBatchPost> hpost((size_t)count);
+  for (int k = 0; k < count; k++) {
+    HipBatchPost& q = hpost[k];
+    const b200pdlp_result& o = outs[src[k]];
+    q.col_value = o.col_value; q.col_dual = o.col_dual; q.row_value = o.row_value; q.row_dual = o.row_dual;
+    q.sol = runs[k].converged ? runs[k].sol : -1;
+    q.pad = 0;
+  }
+  DevBuf<HipBatchPost> dpost;
+  dpost.alloc(count, false);
+  CUDA_OK(cudaMemcpyAsync(dpost.p, hpost.data(), (size_t)count * sizeof(HipBatchPost), cudaMemcpyHostToDevice, s));
+  if (nord > 0) launch_hip_batch_post(s, nord, O.prep.p, O.dhx.p, dpost.p, scaled ? 1 : 0);
+  if (ntree > 0) launch_hip_tree_post(s, ntree, T.prep.p, T.dhx.p, T.dht.p, dpost.p + nord, scaled ? 1 : 0);
+  CUDA_OK(cudaGetLastError());
+  CUDA_OK(cudaStreamSynchronize(s));
+  const double setup_seconds = std::chrono::duration<double>(loop.t_loop - t_begin).count();
+  for (int k = 0; k < count; k++) hip_batch_result(outs + src[k], runs[k], loop, setup_seconds);
+  lap("batch device", "postsolve (device)");
+}
+
+// ---- b200pdlp_debug_hipdlp_tree_prep_compare: the tree members' device prologue and postsolve against
+// formulate_hipdlp + scale_hipdlp + build_layout(ordered_max = -1) and hip_host_postsolve
+static const int kHipTreePrepItems = 31;
+
+// one matrix's long rows (descriptors, entries) from the device against the host's: r[0..3] (all -1 when the counts differ)
+static void long_mismatches(const SellMatrix& H, int nseg, int nlong, long long lcount, const int4* segs, const int4* longs,
+                            const int* lcol, const double* lval, double* r) {
+  if (nseg != (int)H.segs.size() || nlong != (int)H.long_rows.size() || lcount != H.lcount) {
+    r[0] = r[1] = r[2] = r[3] = -1.0;
+    return;
+  }
+  r[0] = dev_mismatches(segs, reinterpret_cast<const int4*>(H.segs.data()), H.segs.size());
+  r[1] = dev_mismatches(longs, reinterpret_cast<const int4*>(H.long_rows.data()), H.long_rows.size());
+  r[2] = dev_mismatches(lcol, H.lcol.data(), H.lcol.size());
+  r[3] = dev_mismatches(lval, H.lval.data(), H.lval.size());
+}
+
+static void hipdlp_tree_prep_compare(int count, const b200pdlp_lp* lps, int scaling_mode, int ruiz_iterations, double* report) {
+  using V = HipBatchVec;
+  const char* who = "b200pdlp_debug_hipdlp_tree_prep_compare";
+  device_count_checked();
+  RawLps raw(count, lps);
+  StreamHolder sh;
+  DeviceBatch D;
+  PrepMode mode;
+  mode.hip = true;
+  device_batch_size(sh.s, count, raw.dl.data(), nullptr, mode, D);
+  std::vector<int> ids((size_t)count);
+  for (int i = 0; i < count; i++) {
+    const BatchSize& z = D.size[i];
+    if (z.err != kPrepOk) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": member " + std::to_string(i) + ": " + prep_error_text(z.err));
+    if (std::max(z.n, lps[i].num_row) > kTreeMemberMax)
+      throw Error(B200PDLP_ERR_ARG, std::string(who) + ": member " + std::to_string(i) + ": exceeds max(n, m) = " +
+                                        std::to_string(kTreeMemberMax) + " of a tree member");
+    ids[i] = i;
+  }
+  TreeBatch T;
+  tree_batch_plan(sh.s, D.hp, D.size, ids, who, T);
+  tree_batch_prep(sh.s, scaling_mode, ruiz_iterations, T);
+  const bool scaled = (scaling_mode & 7) != 0;
+  std::vector<StdForm> F((size_t)count);
+  std::vector<HostLayout> Ls((size_t)count);
+  for (int i = 0; i < count; i++) {
+    const BatchPrep& P = T.hp[i];
+    const HipTreePrep& H = T.ht[i];
+    const HipTreePlan& Z = T.plan[i];
+    StdForm& f = F[i];
+    HostLayout& L = Ls[i];
+    formulate_hipdlp(lps[i], f);
+    scale_hipdlp(f, scaling_mode, ruiz_iterations);
+    build_layout(f, 0, 1, -1, L);
+    double* rep = report + (size_t)kHipTreePrepItems * i;
+    for (int k = 0; k < kHipTreePrepItems; k++) rep[k] = 0.0;
+    rep[0] = (P.n != f.n) + (P.m != f.m) + (P.nnz != f.nnz) + (P.neq != f.neq) + L.ordered;
+    if (rep[0] != 0.0) {   // nothing else lines up
+      for (int k = 1; k < kHipTreePrepItems; k++) rep[k] = -1.0;
+      continue;
+    }
+    const int n = f.n, m = f.m;
+    const double* v = P.vec;
+    auto by_col = [&](const std::vector<double>& x) { std::vector<double> o(n); for (int k = 0; k < n; k++) o[k] = x[L.cperm[k]]; return o; };
+    auto by_row = [&](const std::vector<double>& x) { std::vector<double> o(m); for (int k = 0; k < m; k++) o[k] = x[L.rperm[k]]; return o; };
+    rep[1] = dev_mismatches(V::col(v, n, V::kCost), by_col(f.cost).data(), n);
+    rep[2] = dev_mismatches(V::col(v, n, V::kLower), by_col(f.lower).data(), n);
+    rep[3] = dev_mismatches(V::col(v, n, V::kUpper), by_col(f.upper).data(), n);
+    rep[4] = dev_mismatches(V::row(v, n, m, V::kRlo), by_row(f.rhs).data(), m);
+    rep[5] = dev_mismatches(V::row(v, n, m, V::kRup), by_row(f.row_upper).data(), m);
+    rep[6] = dev_mismatches(V::col(v, n, V::kColscale), by_col(f.col_scale).data(), n);
+    rep[7] = dev_mismatches(V::row(v, n, m, V::kRowscale), by_row(f.row_scale).data(), m);
+    rep[8] = dev_mismatches(H.rperm, L.rperm.data(), m);
+    rep[9] = dev_mismatches(H.cperm, L.cperm.data(), n);
+    sell_mismatches(L.A, P.a_slices, P.a_col, P.a_val, rep + 10);
+    sell_mismatches(L.AT, P.at_slices, P.at_col, P.at_val, rep + 13);
+    long_mismatches(L.A, Z.nseg_a, Z.nlong_a, Z.lcount_a, H.a_segs, H.a_long, H.a_lcol, H.a_lval, rep + 16);
+    long_mismatches(L.AT, Z.nseg_at, Z.nlong_at, Z.lcount_at, H.at_segs, H.at_long, H.at_lcol, H.at_lval, rep + 20);
+    const double* r = T.rec.data() + (size_t)kPrepRec * i;
+    const double got[2] = {std::sqrt(r[kRecCostSq]), std::sqrt(r[kRecRhsSq])};
+    const double want[2] = {f.norm_cost, f.norm_rhs};
+    for (int k = 0; k < 2; k++) rep[24 + k] = memcmp(got + k, want + k, sizeof(double)) != 0;
+    rep[26] = scaled != f.scaled;
+  }
+  // the postsolve of a probe iterate (x, y, sp, sn in device order; a converged member at the iteration-0 check)
+  std::vector<HipBatchPost> hpost;
+  DevBuf<double> dout;
+  DeviceBatch shape;   // probe_outputs reads the dimensions only
+  shape.hp = T.hp;
+  probe_outputs(shape, dout, hpost);
+  std::vector<std::vector<double>> probes((size_t)count);
+  for (int i = 0; i < count; i++) {
+    const BatchPrep& P = T.hp[i];
+    const int n = P.n, m = P.m;
+    std::vector<double>& pr = probes[i];   // x, sp, sn (n each), y (m)
+    pr.resize(3 * (size_t)n + m);
+    for (size_t k = 0; k < pr.size(); k++) pr[k] = batch_probe(i, (int)k);
+    double* v = P.vec;
+    CUDA_OK(cudaMemcpy(V::col(v, n, V::kX), pr.data(), n * sizeof(double), cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemcpy(V::col(v, n, V::kSp), pr.data() + n, n * sizeof(double), cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemcpy(V::col(v, n, V::kSn), pr.data() + 2 * n, n * sizeof(double), cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemcpy(V::row(v, n, m, V::kY), pr.data() + 3 * n, m * sizeof(double), cudaMemcpyHostToDevice));
+  }
+  DevBuf<HipBatchPost> dpost;
+  dpost.alloc(count, false);
+  dpost.upload(hpost.data(), count);
+  launch_hip_tree_post(sh.s, count, T.prep.p, T.dhx.p, T.dht.p, dpost.p, scaled ? 1 : 0);
+  CUDA_OK(cudaGetLastError());
+  CUDA_OK(cudaStreamSynchronize(sh.s));
+  for (int i = 0; i < count; i++) {
+    double* rep = report + (size_t)kHipTreePrepItems * i;
+    if (rep[0] != 0.0) continue;
+    const StdForm& f = F[i];
+    const HostLayout& L = Ls[i];
+    const int n = f.n, m = f.m, n0 = f.n_orig;
+    const double* pr = probes[i].data();
+    std::vector<double> cv(std::max(n0, 1)), cd(std::max(n0, 1)), rv(std::max(m, 1)), rdual(std::max(m, 1));
+    b200pdlp_result res{};
+    res.col_value = cv.data(); res.col_dual = cd.data(); res.row_value = rv.data(); res.row_dual = rdual.data();
+    hip_host_postsolve(lps[i], f, L.cperm.data(), L.rperm.data(), pr, pr + 3 * n, pr + n, pr + 2 * n, &res);
+    const HipBatchPost& q = hpost[i];
+    rep[27] = dev_mismatches(q.col_value, cv.data(), n0);
+    rep[28] = dev_mismatches(q.col_dual, cd.data(), n0);
+    rep[29] = dev_mismatches(q.row_value, rv.data(), m);
+    rep[30] = dev_mismatches(q.row_dual, rdual.data(), m);
+  }
+}
+
 // ====================================================================================== KKT assessment of a batch
 // b200pdlp_kkt_check_batch / _device: kkt_batch.cu's kernel assesses every member at once (one CTA each); the host reads one
 // record per member and runs finalize_kkt on it, so the derived fields and the status rules are those of the single checks.
@@ -1495,6 +1923,26 @@ int b200pdlp_solve_hipdlp_batch_device(int32_t count, const b200pdlp_lp* lps, co
   return batch_entry(who, count, lps && params && outs, [&] {
     for (int i = 0; i < count; i++) check_batch_device_member(&lps[i], params->ordered_max, i, who);
     solve_hipdlp_batch_device(count, lps, *params, outs);
+  });
+}
+
+int b200pdlp_solve_hipdlp_batch_mixed_device(int32_t count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params* params,
+                                             b200pdlp_result* outs) {
+  const char* who = "b200pdlp_solve_hipdlp_batch_mixed_device";
+  return batch_entry(who, count, lps && params && outs, [&] {
+    for (int i = 0; i < count; i++) check_batch_device_member(&lps[i], 0, i, who);   // (any ordered_max: tree members)
+    solve_hipdlp_batch_mixed_device(count, lps, *params, outs);
+  });
+}
+
+int b200pdlp_debug_hipdlp_tree_prep_compare(int32_t count, const b200pdlp_lp* lps, int32_t scaling_mode, int32_t ruiz_iterations,
+                                            double* report) {
+  DeviceGuard dg;
+  return guarded([&] {
+    if (count < 0 || (count > 0 && (!lps || !report)))
+      throw Error(B200PDLP_ERR_ARG, "b200pdlp_debug_hipdlp_tree_prep_compare: bad arguments");
+    for (int i = 0; i < count; i++) check_lp(&lps[i]);
+    if (count > 0) hipdlp_tree_prep_compare(count, lps, scaling_mode, ruiz_iterations, report);
   });
 }
 

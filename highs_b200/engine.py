@@ -83,6 +83,7 @@ ABI_SYMBOLS = [
     "b200pdlp_solve_hipdlp_batch_device", "b200pdlp_debug_hipdlp_batch_prep_compare", "b200pdlp_kkt_check_batch",
     "b200pdlp_kkt_check_batch_device", "b200pdlp_hipdlp_problem_create", "b200pdlp_hipdlp_step", "b200pdlp_hipdlp_check",
     "b200pdlp_hipdlp_problem_power_method", "b200pdlp_solve_hipdlp_batch_mixed",
+    "b200pdlp_solve_hipdlp_batch_mixed_device", "b200pdlp_debug_hipdlp_tree_prep_compare",
 ]
 HIP_TRACE_COLS = 16   # B200PDLP_HIP_TRACE_COLS: the per-block trace of the HiPDLP solves
 
@@ -674,6 +675,72 @@ def hipdlp_batch_prep_compare(lps, scaling_mode: int = 5, ruiz_iterations: int =
     _check(L.b200pdlp_debug_hipdlp_batch_prep_compare(count, clps, scaling_mode, ruiz_iterations, _p(rep, _dp)),
            "b200pdlp_debug_hipdlp_batch_prep_compare")
     return [dict(zip(HIPDLP_BATCH_PREP_ITEMS, rep[k * i:k * (i + 1)].tolist())) for i in range(count)]
+
+
+def solve_hipdlp_batch_mixed_device(dlps, trace_cap: int = 0, **params) -> list:
+    """b200pdlp_solve_hipdlp_batch_mixed_device: solve_hipdlp_batch_mixed for LPs already in GPU memory (dicts of
+    lp_to_device), every member's prologue and postsolve on the device.  Returns the dicts solve_hipdlp_batch_device returns,
+    with the four vectors as float64 CUDA tensors (and with trace_cap > 0 a host "trace" array); each member's bits are those
+    solve_hipdlp_batch_mixed returns for it.  `device` defaults to the device of the first LP's tensors.  torch's current
+    stream is synchronised first, so that inputs it is still writing are complete."""
+    dlps = list(dlps)
+    L = lib()
+    L.b200pdlp_solve_hipdlp_batch_mixed_device.argtypes = [C.c_int32, C.POINTER(CLp), C.POINTER(CHipdlpParams),
+                                                           C.POINTER(CResult)]
+    count = len(dlps)
+    if count == 0:
+        _check(L.b200pdlp_solve_hipdlp_batch_mixed_device(0, None, C.byref(_hipdlp_params(params)), None),
+               "b200pdlp_solve_hipdlp_batch_mixed_device")
+        return []
+    import torch
+    if getattr(dlps[0]["a_start"], "is_cuda", False):
+        params.setdefault("device", dlps[0]["a_start"].device.index)
+    prm = _hipdlp_params(params)
+    clps, cres, arrays = (CLp * count)(), (CResult * count)(), []
+    for i, d in enumerate(dlps):
+        clps[i] = make_clp_device(d)
+    dev = torch.device("cuda", prm.device if prm.device >= 0 else torch.cuda.current_device())
+    for i, d in enumerate(dlps):
+        # at least one element each, so that an LP without rows (or columns) still gets four non-NULL vectors
+        n, m = d["num_col"], d["num_row"]
+        vecs = [torch.empty(max(k, 1), dtype=torch.float64, device=dev) for k in (n, n, m, m)]
+        res = CResult()
+        res.col_value, res.col_dual, res.row_value, res.row_dual = (_dev_ptr(v, torch.float64, _dp, "result") for v in vecs)
+        out = tuple(v[:k] for v, k in zip(vecs, (n, n, m, m)))
+        if trace_cap > 0:
+            tr = np.zeros((trace_cap, HIP_TRACE_COLS))
+            res.trace, res.trace_cap = _p(tr, _dp), trace_cap
+            out = out + (tr,)
+        cres[i] = res
+        arrays.append(out)
+    torch.cuda.current_stream(dev).synchronize()
+    _check(L.b200pdlp_solve_hipdlp_batch_mixed_device(count, clps, C.byref(prm), cres), "b200pdlp_solve_hipdlp_batch_mixed_device")
+    return [_result_dict(cres[i], arrays[i]) for i in range(count)]
+
+
+HIPDLP_TREE_PREP_ITEMS = ["dims", "cost", "lower", "upper", "rhs", "row_upper", "col_scale", "row_scale", "rperm", "cperm",
+                          "A.slices", "A.col", "A.val", "AT.slices", "AT.col", "AT.val", "A.segs", "A.long_rows", "A.lcol",
+                          "A.lval", "AT.segs", "AT.long_rows", "AT.lcol", "AT.lval", "norm_cost", "norm_rhs", "scaled",
+                          "col_value", "col_dual", "row_value", "row_dual"]
+
+
+def hipdlp_tree_prep_compare(lps, scaling_mode: int = 5, ruiz_iterations: int = 10) -> list:
+    """b200pdlp_debug_hipdlp_tree_prep_compare: the tree-mode device prologue and postsolve of solve_hipdlp_batch_mixed_device
+    against formulate_hipdlp + scale_hipdlp + build_layout(ordered_max=-1) and the host postsolve, on host LPs (every one
+    treated as a tree member); one dict of mismatch counts per LP (HIPDLP_TREE_PREP_ITEMS)."""
+    lps = list(lps)
+    L = lib()
+    L.b200pdlp_debug_hipdlp_tree_prep_compare.argtypes = [C.c_int32, C.POINTER(CLp), C.c_int32, C.c_int32, _dp]
+    count = len(lps)
+    clps, keep = (CLp * max(count, 1))(), []
+    for i, lp in enumerate(lps):
+        clps[i], k = make_clp(lp)
+        keep.append(k)
+    k = len(HIPDLP_TREE_PREP_ITEMS)
+    rep = np.zeros(max(count, 1) * k)
+    _check(L.b200pdlp_debug_hipdlp_tree_prep_compare(count, clps, scaling_mode, ruiz_iterations, _p(rep, _dp)),
+           "b200pdlp_debug_hipdlp_tree_prep_compare")
+    return [dict(zip(HIPDLP_TREE_PREP_ITEMS, rep[k * i:k * (i + 1)].tolist())) for i in range(count)]
 
 
 def solve_hipdlp_multi(lp: HighsLp, ngpus: int, devices=None, out_arrays=None, **params) -> dict:

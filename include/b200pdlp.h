@@ -357,6 +357,41 @@ int b200pdlp_solve_hipdlp_batch_mixed(int32_t count, const b200pdlp_lp* lps, con
  * tools/batch_device_bench.py --solver hipdlp. */
 int b200pdlp_solve_hipdlp_batch_device(int32_t count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params* params,
                                        b200pdlp_result* outs /* [count]; vectors in device memory */);
+/* b200pdlp_solve_hipdlp_batch_mixed for LPs that are already in GPU memory.  Pointers follow
+ * b200pdlp_solve_hipdlp_batch_device's rules: the LP's eight arrays and the four result vectors are device (or managed)
+ * memory of params->device (< 0: the current device); num_col, num_row, sense and offset are host scalars; the trace storage
+ * (trace, trace_cap) stays in host memory.  Members are classified as in b200pdlp_solve_hipdlp_batch_mixed (ordered:
+ * max(n, m) <= ordered_max under HiPDLP's classification; every other member a tree member up to max(n, m) = 262144;
+ * ordered_max < 0 makes every member a tree member) and may come in any order.  Each member returns exactly what
+ * b200pdlp_solve_hipdlp_batch_mixed returns for it from the same arrays on the host -- a tree member what
+ * b200pdlp_solve_hipdlp returns for it alone, an ordered member what b200pdlp_solve_hipdlp_batch returns: term_code,
+ * term_iterate, iters, passes, restarts, the residual scalars, the form dimensions, the four vectors and the trace rows, bit
+ * for bit.  Batch-wide fields as in b200pdlp_solve_hipdlp_batch_mixed; setup_seconds covers validation, sizing and the
+ * device prologue.  device_prep is ignored.  B200PDLP_BATCH_CLUSTER works as there and changes no result.
+ * Every member's prologue and postsolve run on the device, one CTA per member: an ordered member's as in
+ * b200pdlp_solve_hipdlp_batch_device; a tree member's builds formulate_hipdlp, scale_hipdlp and the tree-mode layouts (rows
+ * and columns sorted by length in windows, long rows cut into segments) and packs the vectors in device order.  The host
+ * reads fixed-size records per member, never an array.  The call never writes an input, uses a stream of its own and
+ * returns once the outputs are complete.  B200PDLP_TIMING=1 prints the laps (validation + sizing, orderings + plans,
+ * prologue, rounds, postsolve) and the tree-member count with C.
+ * Returns B200PDLP_ERR_ARG, with nothing written, in b200pdlp_solve_hipdlp_batch_device's order: before any device work for
+ * count < 0, NULL arrays or a sense other than +-1; then, naming the member and the field, for a pointer that is not device
+ * memory of the device; then, naming the lowest failing member, for a malformed a_start or a_index and for a tree member
+ * whose standard form exceeds max(n, m) = 262144 (solve it with b200pdlp_solve_hipdlp).  count == 0: B200PDLP_OK.  No
+ * device: B200PDLP_ERR_CUDA.  The whole batch must fit in device memory (B200PDLP_ERR_ALLOC otherwise).
+ * STATUS: runs on hardware; tests/test_gpu_hipdlp_batch_mixed_device.py (byte equality with
+ * b200pdlp_solve_hipdlp_batch_mixed on host copies and with b200pdlp_solve_hipdlp), tools/hipdlp_batch_mixed_device_bench.py. */
+int b200pdlp_solve_hipdlp_batch_mixed_device(int32_t count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params* params,
+                                             b200pdlp_result* outs /* [count]; vectors in device memory */);
+/* debug (tests): the tree-mode device prologue of b200pdlp_solve_hipdlp_batch_mixed_device on host LPs (uploaded first),
+ * every member treated as a tree member, against formulate_hipdlp + scale_hipdlp(scaling_mode, ruiz_iterations) +
+ * build_layout(ordered_max = -1), then the device postsolve of a fixed pseudo-random iterate against hip_host_postsolve.
+ * report[count][31]: mismatch counts of dims; cost, lower, upper, rhs, row_upper, col_scale, row_scale (device order);
+ * rperm, cperm; slices, col, val of A and of A'; segs, long_rows, lcol, lval of A and of A'; |c|, |b|; the scaled flag;
+ * col_value, col_dual, row_value, row_dual (-1: not comparable).  B200PDLP_ERR_ARG for a malformed LP or one past
+ * max(n, m) = 262144. */
+int b200pdlp_debug_hipdlp_tree_prep_compare(int32_t count, const b200pdlp_lp* lps, int32_t scaling_mode,
+                                            int32_t ruiz_iterations, double* report);
 /* The HiPDLP solve on `ngpus` devices of THIS process (devices[g] or, if NULL, ordinals 0..ngpus-1; a device may repeat,
  * which gives logical shards on one device): the prologue, then each rank computes contiguous blocks of the one-GPU device
  * rows and columns, one host thread per rank, peer memory, no NCCL.  device_prep is honoured as on one GPU: 0 runs the
