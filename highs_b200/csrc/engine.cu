@@ -1995,6 +1995,125 @@ int b200pdlp_residuals(b200pdlp_problem* p, const double* x, const double* y, do
   });
 }
 
+// the restart sums |x - xlr|^2, |y - ylr|^2 from the restart sweep's block partials, added in check_finish_kernel's order:
+// thread t adds partials t, t + 128, ... from 0, a shuffle tree inside each warp, then the four warps in order
+static void finish_order_sums(const std::vector<double>& prst, int nbs, double d2[2]) {
+  constexpr int kT = 128;
+  for (int a = 0; a < 2; a++) {
+    double w[kT / 32];
+    for (int g = 0; g < kT / 32; g++) {
+      double v[32];
+      for (int l = 0; l < 32; l++) {
+        double s = 0.0;
+        for (int i = g * 32 + l; i < nbs; i += kT) s += prst[(size_t)a * nbs + i];
+        v[l] = s;
+      }
+      for (int o = 16; o > 0; o >>= 1)
+        for (int l = 0; l + o < 32; l++) v[l] = v[l] + v[l + o];   // (ascending l reads v[l + o] before it changes)
+      w[g] = v[0];
+    }
+    double s = 0.0;
+    for (int g = 0; g < kT / 32; g++) s += w[g];
+    d2[a] = s;
+  }
+}
+
+int b200pdlp_check_device(b200pdlp_problem* p, const b200pdlp_check_in* in, double* x, double* y, double* ax, double* aty,
+                          double* xsum, double* ysum, double* xlr, double* ylr, double* axsum, double* atysum, double* xavg,
+                          double* yavg, double* axavg, double* atyavg, b200pdlp_check_out* out) {
+  DeviceGuard dg;
+  return guarded([&] {
+    const char* who = "b200pdlp_check_device";
+    if (!p || !in || !x || !y || !ax || !aty || !xsum || !ysum || !xlr || !ylr || !xavg || !yavg || !axavg || !atyavg || !out ||
+        (in->light && (!axsum || !atysum)))
+      throw Error(B200PDLP_ERR_ARG, std::string(who) + ": null argument");
+    require_mode(p, false, who);
+    if (p->world != 1) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": kernel-level entry points are single-GPU");
+    if (p->ordered) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": an ordered-mode problem (its checks run on the host)");
+    if (in->interval < 1 || in->iter < 0 || in->step_iter < 0)
+      throw Error(B200PDLP_ERR_ARG, std::string(who) + ": interval must be >= 1, iter and step_iter >= 0");
+    if (in->light && (!p->axsum.p || !p->atysum.p || in->iter >= kDenseChecks))
+      throw Error(B200PDLP_ERR_ARG, std::string(who) + ": the light check needs iter < 10 and a problem that carries A xSum");
+    set_device(p);
+    ensure_host_maps(p);
+    const int n = p->n;
+    cudaStream_t s = p->stream;
+    const bool light = in->light != 0;
+    upload_perm(p, p->x[0].p, x, p->cperm); upload_perm(p, p->aty[0].p, aty, p->cperm);
+    upload_perm(p, p->xsum.p, xsum, p->cperm); upload_perm(p, p->xlr.p, xlr, p->cperm);
+    upload_perm(p, p->y[0].p, y, p->rperm); upload_perm(p, p->ax[0].p, ax, p->rperm);
+    upload_perm(p, p->ysum.p, ysum, p->rperm); upload_perm(p, p->ylr.p, ylr, p->rperm);
+    if (light) { upload_perm(p, p->atysum.p, atysum, p->cperm); upload_perm(p, p->axsum.p, axsum, p->rperm); }
+    // the state and control blocks of a solve at its check iteration
+    const double nan = std::numeric_limits<double>::quiet_NaN();
+    PdhgState* h = p->hstate;
+    memset(h, 0, sizeof(PdhgState));
+    h->iter = in->iter; h->step_iter = in->step_iter; h->adaptive = in->adaptive; h->pending = in->pending;
+    h->beta = in->beta; h->tau = in->tau; h->sigma = in->sigma; h->sum_step = in->sum_step; h->w_pending = in->w_pending;
+    h->eta = h->tau_try = h->sigma_try = nan;
+    for (int t = 0; t < kPowTab; t++) h->pow_red[t] = h->pow_grow[t] = nan;
+    h->pow_base = -1;
+    h->stop_iter = in->iter; h->cur = 0; h->light_on = light ? 1 : 0; h->done = 0;
+    push_state(p);
+    if (!p->hctl) {
+      p->hctl = static_cast<SolveCtl*>(pinned_cache_alloc(sizeof(SolveCtl), false));
+      p->htime = static_cast<int*>(pinned_cache_alloc(64, true));
+      p->ctl.alloc(1, false);
+    }
+    if (p->trace_dev.n < (size_t)B200PDLP_TRACE_COLS) p->trace_dev.alloc(B200PDLP_TRACE_COLS, false);
+    CUDA_OK(cudaMemsetAsync(p->trace_dev.p, 0, B200PDLP_TRACE_COLS * sizeof(double), s));
+    SolveCtl* c = p->hctl;
+    memset(c, 0, sizeof(SolveCtl));
+    c->tol_p = in->tol_p; c->tol_d = in->tol_d; c->tol_gap = in->tol_gap;
+    c->sense = p->form.sense; c->offset = p->form.offset;
+    c->iter_limit = in->iter_limit; c->interval = in->interval; c->restart_on = in->restart_on != 0; c->world = 1;
+    *p->htime = in->time_flag;
+    int* dflag = nullptr;
+    CUDA_OK(cudaHostGetDevicePointer(&dflag, p->htime, 0));
+    c->time_flag = dflag;
+    c->pf_lr = in->pf_lr; c->df_lr = in->df_lr; c->gap_lr = in->gap_lr;
+    c->pf_lc = in->pf_lc; c->df_lc = in->df_lc; c->gap_lc = in->gap_lc;
+    c->last_restart_iter = in->last_restart_iter;
+    c->term = -1;
+    c->trace = p->trace_dev.p; c->trace_cap = 1;
+    CUDA_OK(cudaMemcpyAsync(p->ctl.p, c, sizeof(SolveCtl), cudaMemcpyHostToDevice, s));
+    p->launches += enqueue_check_device(p, light);
+    CUDA_OK(cudaGetLastError());
+    CUDA_OK(cudaMemcpyAsync(c, p->ctl.p, sizeof(SolveCtl), cudaMemcpyDeviceToHost, s));
+    CUDA_OK(cudaMemcpyAsync(h, p->state.p, sizeof(PdhgState), cudaMemcpyDeviceToHost, s));
+    CUDA_OK(cudaMemcpyAsync(out->trace, p->trace_dev.p, B200PDLP_TRACE_COLS * sizeof(double), cudaMemcpyDeviceToHost, s));
+    const int nbs = restart_sweep_grid(n, p->ml);
+    std::vector<double> prst((size_t)2 * nbs);
+    CUDA_OK(cudaMemcpyAsync(prst.data(), p->rs(kSlotK1, n).partials, prst.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+    CUDA_OK(cudaStreamSynchronize(s));
+    for (int a = 0; a < 28; a++) out->sums[a] = c->sums[a];
+    for (int t = 0; t < 2; t++) {
+      const DevResiduals& R = c->res[t];
+      const double v[10] = {R.pobj, R.dobj, R.pfeas, R.dfeas, R.gap, R.relgap, R.pinf_obj, R.pinf_res, R.dinf_obj, R.dinf_res};
+      for (int k = 0; k < 10; k++) out->res[t][k] = v[k];
+    }
+    out->term = c->term; out->term_iterate = c->term_iterate;
+    out->restart_choice = c->trace_len > 0 ? (int)out->trace[12] : 0;
+    out->restarts = c->restarts; out->checks = c->checks; out->trace_len = c->trace_len; out->done = h->done;
+    out->stop_iter = h->stop_iter; out->pending = h->pending; out->pow_base = h->pow_base;
+    out->pf_lr = c->pf_lr; out->df_lr = c->df_lr; out->gap_lr = c->gap_lr;
+    out->pf_lc = c->pf_lc; out->df_lc = c->df_lc; out->gap_lc = c->gap_lc;
+    out->last_restart_iter = c->last_restart_iter; out->reserved = 0;
+    out->beta = h->beta; out->tau = h->tau; out->sigma = h->sigma; out->eta = h->eta;
+    out->tau_try = h->tau_try; out->sigma_try = h->sigma_try; out->sum_step = h->sum_step;
+    out->restart_sq[0] = out->restart_sq[1] = 0.0;
+    if (out->restart_choice) finish_order_sums(prst, nbs, out->restart_sq);
+    for (int t = 0; t < kPowTab; t++) { out->pow_red[t] = h->pow_red[t]; out->pow_grow[t] = h->pow_grow[t]; }
+    download_perm(p, x, p->x[0].p, p->cperm); download_perm(p, aty, p->aty[0].p, p->cperm);
+    download_perm(p, xsum, p->xsum.p, p->cperm); download_perm(p, xlr, p->xlr.p, p->cperm);
+    download_perm(p, xavg, p->xavg.p, p->cperm); download_perm(p, atyavg, p->atyavg.p, p->cperm);
+    download_perm(p, y, p->y[0].p, p->rperm); download_perm(p, ax, p->ax[0].p, p->rperm);
+    download_perm(p, ysum, p->ysum.p, p->rperm); download_perm(p, ylr, p->ylr.p, p->rperm);
+    download_perm(p, yavg, p->yavg.p, p->rperm); download_perm(p, axavg, p->axavg.p, p->rperm);
+    if (light) { download_perm(p, atysum, p->atysum.p, p->cperm); download_perm(p, axsum, p->axsum.p, p->rperm); }
+  });
+}
+
 int b200pdlp_bench_spmv(b200pdlp_problem* p, int32_t which, int32_t reps, float* ms_total) {
   DeviceGuard dg;
   return guarded([&] {

@@ -48,6 +48,32 @@ class CHipdlpParams(C.Structure):
                 ("reserved", C.c_int32 * 2)]
 
 
+class CCheckIn(C.Structure):
+    """b200pdlp_check_in: the PdhgState and SolveCtl scalars of one device check (b200pdlp_check_device)"""
+    _fields_ = [("iter", C.c_int32), ("step_iter", C.c_int32), ("adaptive", C.c_int32), ("pending", C.c_int32),
+                ("beta", C.c_double), ("tau", C.c_double), ("sigma", C.c_double), ("sum_step", C.c_double),
+                ("w_pending", C.c_double), ("tol_p", C.c_double), ("tol_d", C.c_double), ("tol_gap", C.c_double),
+                ("iter_limit", C.c_int32), ("interval", C.c_int32), ("restart_on", C.c_int32), ("time_flag", C.c_int32),
+                ("pf_lr", C.c_double), ("df_lr", C.c_double), ("gap_lr", C.c_double), ("pf_lc", C.c_double),
+                ("df_lc", C.c_double), ("gap_lc", C.c_double), ("last_restart_iter", C.c_int32), ("light", C.c_int32)]
+
+
+class CCheckOut(C.Structure):
+    """b200pdlp_check_out: what one device check leaves behind"""
+    _fields_ = [("sums", C.c_double * 28), ("res", (C.c_double * 10) * 2), ("term", C.c_int32), ("term_iterate", C.c_int32),
+                ("restart_choice", C.c_int32), ("restarts", C.c_int32), ("checks", C.c_int32), ("trace_len", C.c_int32),
+                ("done", C.c_int32), ("stop_iter", C.c_int32), ("pending", C.c_int32), ("pow_base", C.c_int32),
+                ("pf_lr", C.c_double), ("df_lr", C.c_double), ("gap_lr", C.c_double), ("pf_lc", C.c_double),
+                ("df_lc", C.c_double), ("gap_lc", C.c_double), ("last_restart_iter", C.c_int32), ("reserved", C.c_int32),
+                ("beta", C.c_double), ("tau", C.c_double), ("sigma", C.c_double), ("eta", C.c_double), ("tau_try", C.c_double),
+                ("sigma_try", C.c_double), ("sum_step", C.c_double), ("restart_sq", C.c_double * 2),
+                ("pow_red", C.c_double * 128), ("pow_grow", C.c_double * 128), ("trace", C.c_double * 16)]
+
+
+CHECK_VECTORS = ("x", "y", "ax", "aty", "xsum", "ysum", "xlr", "ylr", "axsum", "atysum", "xavg", "yavg", "axavg", "atyavg")
+RESIDUAL_NAMES = ("pobj", "dobj", "pfeas", "dfeas", "gap", "relgap", "pinf_obj", "pinf_res", "dinf_obj", "dinf_res")
+
+
 class CWarm(C.Structure):
     _fields_ = [("col_value", _dp), ("row_value", _dp), ("row_dual", _dp)]
 
@@ -83,7 +109,7 @@ ABI_SYMBOLS = [
     "b200pdlp_solve_hipdlp_batch_device", "b200pdlp_debug_hipdlp_batch_prep_compare", "b200pdlp_kkt_check_batch",
     "b200pdlp_kkt_check_batch_device", "b200pdlp_hipdlp_problem_create", "b200pdlp_hipdlp_step", "b200pdlp_hipdlp_check",
     "b200pdlp_hipdlp_problem_power_method", "b200pdlp_solve_hipdlp_batch_mixed",
-    "b200pdlp_solve_hipdlp_batch_mixed_device", "b200pdlp_debug_hipdlp_tree_prep_compare",
+    "b200pdlp_solve_hipdlp_batch_mixed_device", "b200pdlp_debug_hipdlp_tree_prep_compare", "b200pdlp_check_device",
 ]
 HIP_TRACE_COLS = 16   # B200PDLP_HIP_TRACE_COLS: the per-block trace of the HiPDLP solves
 
@@ -159,6 +185,7 @@ def lib():
         L.b200pdlp_primal_step.argtypes = [C.c_void_p, _dp, _dp, C.c_double, _dp, _dp]
         L.b200pdlp_dual_step.argtypes = [C.c_void_p, _dp, _dp, _dp, C.c_double, _dp, _dp, _dp]
         L.b200pdlp_residuals.argtypes = [C.c_void_p, _dp, _dp, _dp]
+        L.b200pdlp_check_device.argtypes = [C.c_void_p, C.POINTER(CCheckIn)] + [_dp] * 14 + [C.POINTER(CCheckOut)]
         _lib = L
     return _lib
 
@@ -888,6 +915,34 @@ class Problem:
         out = np.zeros(10)
         _check(lib().b200pdlp_residuals(self._h, _p(x, _dp), _p(y, _dp), _p(out, _dp)), "b200pdlp_residuals")
         return dict(zip(("pobj", "dobj", "pfeas", "dfeas", "gap", "relgap", "pinf_obj", "pinf_res", "dinf_obj", "dinf_res"), out.tolist()))
+
+    def check_device(self, x, y, ax, aty, xsum, ysum, xlr, ylr, axsum=None, atysum=None, **scalars) -> dict:
+        """One device check of a tree-mode solve (b200pdlp_check_device).  Vectors in standard-form order; scalars are the
+        fields of b200pdlp_check_in (iter, tau, ..., light, time_flag).  Returns the fields of b200pdlp_check_out as numbers
+        and arrays ("res" as two dicts keyed by RESIDUAL_NAMES) and every vector of CHECK_VECTORS after the check (axsum /
+        atysum only for light = 1)."""
+        n, m = self.n, self.m
+        cin = CCheckIn()
+        for k, v in scalars.items():
+            if not hasattr(cin, k):
+                raise TypeError(f"unknown check_device field {k}")
+            setattr(cin, k, v)
+        light = bool(cin.light)
+        vec = lambda v, ln: np.array(v, dtype=np.float64, copy=True).reshape(ln)
+        v = dict(x=vec(x, n), y=vec(y, m), ax=vec(ax, m), aty=vec(aty, n), xsum=vec(xsum, n), ysum=vec(ysum, m),
+                 xlr=vec(xlr, n), ylr=vec(ylr, m), xavg=np.zeros(n), yavg=np.zeros(m), axavg=np.zeros(m), atyavg=np.zeros(n))
+        if light:
+            v["axsum"], v["atysum"] = vec(axsum, m), vec(atysum, n)
+        out = CCheckOut()
+        ptrs = [_p(v[k], _dp) if k in v else None for k in CHECK_VECTORS]
+        _check(lib().b200pdlp_check_device(self._h, C.byref(cin), *ptrs, C.byref(out)), "b200pdlp_check_device")
+        r = {}
+        for k, t in CCheckOut._fields_:
+            a = getattr(out, k)
+            r[k] = np.ctypeslib.as_array(a).copy() if hasattr(t, "_length_") else a
+        r["res"] = [dict(zip(RESIDUAL_NAMES, r["res"][t].tolist())) for t in range(2)]
+        r.update(v)
+        return r
 
     def bench_spmv(self, which: int, reps: int) -> float:
         ms = C.c_float()

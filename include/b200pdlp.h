@@ -217,6 +217,49 @@ int b200pdlp_dual_step(b200pdlp_problem* p, const double* x_new, const double* y
                        double* y_new, double* ax_new, double* dy2);
 int b200pdlp_residuals(b200pdlp_problem* p, const double* x, const double* y, double out[10]);
 
+/* One check iteration of a tree-mode solve, on the device (parity tests; one GPU): the launches the solve's check graphs
+ * capture (engine.cu enqueue_check_device), run once without a graph.  C1 flushes the pending weight into xSum / ySum and
+ * forms the averages, C2 multiplies them by A and A' (split variant only), C3 adds the 8 row-side and 20 column-side sums of
+ * both iterates, C4 forms the residuals and decides (termination, infeasibility, limits, restart choice), C5 restarts the
+ * vectors, C6 updates the step sizes and primal weight, writes the trace row, sets the next check iteration and fills the
+ * step-rule power tables.  The scalars in `in` become the PdhgState / SolveCtl of the check (sense and offset are the
+ * problem's; stop_iter = iter, so the check is due).  light = 1 runs the dense-check phase's variant: A xbar and A'ybar come
+ * from the carried axsum = A xSum and atysum = A'ySum instead of two SpMVs.
+ * Vectors are host arrays in standard-form order, read on entry and overwritten with their values after the check:
+ * x, y (current iterate), ax, aty (its products, the caller's values), xsum, ysum, xlr, ylr (last restart point), and for
+ * light = 1 axsum, atysum (NULL otherwise).  Written only: xavg, yavg (the averages), axavg = A xavg, atyavg = A'yavg.
+ * Rejected with B200PDLP_ERR_ARG before anything is written: NULL arguments, a problem in ordered mode, on several GPUs or of
+ * b200pdlp_hipdlp_problem_create, interval < 1, iter or step_iter < 0, and light = 1 when iter >= 10 (the dense-check
+ * phase) or the problem carries no A xSum.  No device: B200PDLP_ERR_CUDA. */
+typedef struct {
+  int32_t iter, step_iter, adaptive, pending;    /* PdhgState */
+  double beta, tau, sigma, sum_step, w_pending;
+  double tol_p, tol_d, tol_gap;                  /* SolveCtl: tol_p / tol_d absolute (already times 1 + |b| / 1 + |c|) */
+  int32_t iter_limit, interval, restart_on;
+  int32_t time_flag;                             /* the value of the time-limit word the check reads */
+  double pf_lr, df_lr, gap_lr, pf_lc, df_lc, gap_lc;   /* restart memo: at the last restart, at the last candidate */
+  int32_t last_restart_iter;
+  int32_t light;
+} b200pdlp_check_in;
+typedef struct {
+  double sums[28];          /* 0-3 row side of the current iterate (y.b, |primal residual|^2, |y|^2, |ray residual|^2),
+                               4-7 the same for the average, 8-17 column side of the current iterate, 18-27 of the average */
+  double res[2][10];        /* current, average: pobj, dobj, pfeas, dfeas, gap, relgap, pinf_obj, pinf_res, dinf_obj, dinf_res */
+  int32_t term;             /* -1 the solve goes on, else a b200pdlp_term */
+  int32_t term_iterate;     /* 0 current, 1 average (term == OPTIMAL) */
+  int32_t restart_choice;   /* 0 none, 1 to the average, 2 to the current iterate (trace column 12) */
+  int32_t restarts, checks, trace_len, done, stop_iter, pending, pow_base;
+  double pf_lr, df_lr, gap_lr, pf_lc, df_lc, gap_lc;   /* the memo after the check */
+  int32_t last_restart_iter, reserved;
+  double beta, tau, sigma, eta, tau_try, sigma_try, sum_step;   /* eta, tau_try, sigma_try enter as NaN */
+  double restart_sq[2];     /* on a restart: |x - xlr|^2, |y - ylr|^2 as C6 added them (0 otherwise) */
+  double pow_red[128], pow_grow[128];   /* enter as NaN */
+  double trace[16];         /* the check's trace row (B200PDLP_TRACE_COLS) */
+} b200pdlp_check_out;
+int b200pdlp_check_device(b200pdlp_problem* p, const b200pdlp_check_in* in, double* x, double* y, double* ax, double* aty,
+                          double* xsum, double* ysum, double* xlr, double* ylr, double* axsum, double* atysum, double* xavg,
+                          double* yavg, double* axavg, double* atyavg, b200pdlp_check_out* out);
+
 /* device-pointer variants on the problem's stream (bench roofline loop):
  * time `reps` back-to-back launches with CUDA events; returns ms in *ms_total */
 int b200pdlp_bench_spmv(b200pdlp_problem* p, int32_t which /*0 Ax, 1 ATy*/, int32_t reps, float* ms_total);
