@@ -1,21 +1,23 @@
-// highs_b200/csrc/batch_prep.cu -- the device prologue and postsolve of b200pdlp_solve_batch_device (engine_batch.cu
-// solve_batch_device): one CTA per member, and no CTA waits on another, so any number of members runs.
+// highs_b200/csrc/batch_prep.cu -- the device prologue and postsolve of the ordered members of the device-array batches:
+// b200pdlp_solve_batch_device (engine_batch.cu solve_batch_device) and b200pdlp_solve_hipdlp_batch_device / _mixed_device
+// (engine_batch.cu solve_hipdlp_batch_device).  One CTA per member, and no CTA waits on another, so any number of members runs.
 //
-//   batch_size_kernel   check_lp(deep) on the device, formulate's row classes and row order, the standard form's dimensions
-//                       and the padded lengths of its ordered sliced-ELL layouts: what the host needs to lay out the pools
-//   batch_prep_kernel   formulate, the row-major index, scale, the sliced-ELL bodies of A and A', host_start_point, xSum = proj(0)
-//                       and the sums that set the tolerances and beta
-//   batch_post_kernel   host_postsolve of the returned iterate, into the caller's device vectors
-// and their HiPDLP twins for b200pdlp_solve_hipdlp_batch_device (engine_batch.cu solve_hipdlp_batch_device):
-//   hip_batch_size_kernel   the same checks and sizes under formulate_hipdlp's row classes
-//   hip_batch_prep_kernel   formulate_hipdlp, the row-major indexes of the form and of the caller's matrix, scale_hipdlp, the
-//                           sliced-ELL bodies of A and A', |c|^2 and |b|^2 of the unscaled form
+//   batch_size_kernel       check_lp(deep) on the device, formulate's row classes and row order, the standard form's
+//                           dimensions and the padded lengths of its ordered sliced-ELL layouts: what the host needs to lay
+//                           out the pools
+//   batch_prep_kernel       formulate, the row-major index, scale, the sliced-ELL bodies of A and A', host_start_point,
+//                           xSum = proj(0) and the sums that set the tolerances and beta
+//   batch_post_kernel       host_postsolve of the returned iterate, into the caller's device vectors
+//   hip_batch_size_kernel   batch_size_kernel under formulate_hipdlp's row classes (every HiPDLP member, tree members too)
+//   hip_batch_prep_kernel   hip_form.cuh hip_form (formulate_hipdlp, the row-major indexes of the form and of the caller's
+//                           matrix, scale_hipdlp, |c|^2 and |b|^2 of the unscaled form), then the sliced-ELL bodies of A and A'
 //   hip_batch_post_kernel   hip_host_postsolve of the returned iterate, into the caller's device vectors
 //
-// Bits: every value is the host prologue's (host_prep.cpp formulate / build_row_index / scale / build_layout, engine.cu
-// host_start_point / host_postsolve) with the same operations on the same operands: the build compiles this file with
-// -fmad=false and IEEE division and square root.  Maxima are order-free; every sum is taken in the host's order -- a row's
-// 1-norm column-ascending by the thread that owns the row, |c|^2 and |b|^2 in index order by one thread.
+// Bits: every value is the host prologue's (host_prep.cpp formulate / build_row_index / scale / build_layout,
+// host_prep_hipdlp.cpp formulate_hipdlp / scale_hipdlp, engine.cu host_start_point / host_postsolve, engine_hipdlp.cu
+// hip_host_postsolve) with the same operations on the same operands: the build compiles this file with -fmad=false and IEEE
+// division and square root.  Maxima are order-free; every sum is taken in the host's order -- a row's 1-norm column-ascending
+// by the thread that owns the row, |c|^2 and |b|^2 in index order by one thread.
 #include "batch_kernels.hpp"
 #include "batch_prep.hpp"
 #include "hip_form.cuh"
@@ -67,12 +69,39 @@ __device__ long long padded(int rows, Len len, unsigned long long* acc) {
   return total;
 }
 
-__global__ void __launch_bounds__(kThreads) batch_size_kernel(const BatchPrep* __restrict__ prep, BatchSize* __restrict__ sizes) {
+// formulate's row classes (host_prep.cpp formulate): +-1e20 thresholds; ranged and free rows are BOUND rows
+struct PdlpRows {
+  __device__ static int row_class(double rl, double ru) {
+    const bool lo = rl > -1e20, up = ru < 1e20;
+    int c;
+    if (lo && up && rl == ru) c = kEq;
+    else if (lo && !up) c = kGeq;
+    else if (!lo && up) c = kLeq;
+    else c = kBound;
+    return c;
+  }
+};
+// formulate_hipdlp's row classes: +-infinity thresholds (a bound of 1e25 is finite), FREE rows a class of their own
+struct HipRows {
+  __device__ static int row_class(double rl, double ru) {
+    const bool lo = rl > -kInf, up = ru < kInf;
+    int c;
+    if (lo && up) c = (rl == ru) ? kEq : kBound;
+    else if (lo) c = kGeq;
+    else if (up) c = kLeq;
+    else c = kFreeRow;
+    return c;
+  }
+};
+
+// check_lp(deep), the row classes under Rows, the row order, the standard form's dimensions and the padded lengths of its
+// ordered layouts, for one member.  BOUND and FREE rows are equality-like, each with a slack column (PdlpRows makes no FREE
+// rows).
+template <class Rows>
+__device__ __forceinline__ void batch_size(const BatchPrep& P, BatchSize& S) {
   __shared__ int flag[4];
   __shared__ int sm_eq[kThreads + 1], sm_bnd[kThreads + 1];
   __shared__ unsigned long long acc;
-  const BatchPrep& P = prep[blockIdx.x];
-  BatchSize& S = sizes[blockIdx.x];
   const int t = threadIdx.x, n0 = P.n0, m = P.m;
   if (t < 4) flag[t] = 0;
   __syncthreads();
@@ -96,27 +125,21 @@ __global__ void __launch_bounds__(kThreads) batch_size_kernel(const BatchPrep* _
     if (t == 0) S.err = kPrepIndex;
     return;
   }
-  // formulate's row classes (host_prep.cpp formulate)
   for (int i = t; i < m; i += kThreads) {
     const double rl = P.row_lower[i], ru = P.row_upper[i];
-    const bool lo = rl > -1e20, up = ru < 1e20;
-    int c;
-    if (lo && up && rl == ru) c = kEq;
-    else if (lo && !up) c = kGeq;
-    else if (!lo && up) c = kLeq;
-    else c = kBound;
-    P.row_class[i] = c;
+    P.row_class[i] = Rows::row_class(rl, ru);
   }
   for (int i = t; i <= m; i += kThreads) P.rptr[i] = 0;
   __syncthreads();
-  // the new row order: EQ / BOUND rows first, then LEQ / GEQ, each in original order; slack columns in BOUND-row order
+  // the new row order: equality-like rows (EQ / BOUND / FREE) first, then LEQ / GEQ, each in original order;
+  // slack columns in the order of their rows
   const int chunk = (m + kThreads - 1) / kThreads;
   const int b = min(t * chunk, m), e = min(b + chunk, m);
   int eq = 0, bnd = 0;
   for (int i = b; i < e; i++) {
     const int c = P.row_class[i];
-    eq += (c == kEq || c == kBound);
-    bnd += (c == kBound);
+    eq += (c == kEq || c == kBound || c == kFreeRow);
+    bnd += (c == kBound || c == kFreeRow);
   }
   sm_eq[t] = eq; sm_bnd[t] = bnd;
   __syncthreads();
@@ -135,12 +158,12 @@ __global__ void __launch_bounds__(kThreads) batch_size_kernel(const BatchPrep* _
     int head = sm_eq[t], tail = neq + (b - sm_eq[t]), sl = sm_bnd[t];
     for (int i = b; i < e; i++) {
       const int c = P.row_class[i];
-      P.row_new_idx[i] = (c == kEq || c == kBound) ? head++ : tail++;
-      P.slack[i] = c == kBound ? sl++ : -1;
+      P.row_new_idx[i] = (c == kEq || c == kBound || c == kFreeRow) ? head++ : tail++;
+      P.slack[i] = (c == kBound || c == kFreeRow) ? sl++ : -1;
     }
   }
   __syncthreads();
-  // the standard form's row lengths (integer counts: order-free), a BOUND row's slack entry included
+  // the standard form's row lengths (integer counts: order-free), a slack row's slack entry included
   for (int p = t; p < nnz0; p += kThreads) atomicAdd(&P.rptr[P.row_new_idx[P.a_index[p]]], 1);
   for (int i = t; i < m; i += kThreads)
     if (P.slack[i] >= 0) atomicAdd(&P.rptr[P.row_new_idx[i]], 1);
@@ -153,6 +176,14 @@ __global__ void __launch_bounds__(kThreads) batch_size_kernel(const BatchPrep* _
     // (ordered_max keeps these far below 2^31; the host checks the dimensions before it trusts them)
     S.pad_a = (int)min(pa, 2000000000ll); S.pad_at = (int)min(pat, 2000000000ll);
   }
+}
+
+__global__ void __launch_bounds__(kThreads) batch_size_kernel(const BatchPrep* __restrict__ prep, BatchSize* __restrict__ sizes) {
+  batch_size<PdlpRows>(prep[blockIdx.x], sizes[blockIdx.x]);
+}
+
+__global__ void __launch_bounds__(kThreads) hip_batch_size_kernel(const BatchPrep* __restrict__ prep, BatchSize* __restrict__ sizes) {
+  batch_size<HipRows>(prep[blockIdx.x], sizes[blockIdx.x]);
 }
 
 // one ordered sliced-ELL body: rows r < rows, 32 a slice, entry k of row r at ptr + 32 k + (r & 31); padding (0, 0), and 32
@@ -182,11 +213,41 @@ __device__ void sell_body(int rows, int4* slices, int* col, double* val, int* sm
   for (int q = threadIdx.x; q < 32; q += kThreads) { col[(size_t)total + q] = 0; val[(size_t)total + q] = 0.0; }
 }
 
+// the ordered sliced-ELL bodies of the form (build_layout, identity orderings, no long rows): A's rows in the row-major
+// index's order; A' row j = column j sorted by row, stably (build_col_major)
+__device__ __forceinline__ void form_layouts(const BatchPrep& P, int m, int n, int* sm) {
+  sell_body(m, P.a_slices, P.a_col, P.a_val, sm, [&](int r) { return P.rptr[r + 1] - P.rptr[r]; },
+            [&](int r, int* c, double* v) {
+              const int q0 = P.rptr[r], len = P.rptr[r + 1] - q0;
+              for (int k = 0; k < len; k++) { const int p = P.rpos[q0 + k]; c[32 * k] = P.pcol[p]; v[32 * k] = P.cval[p]; }
+              return len;
+            });
+  __syncthreads();
+  sell_body(n, P.at_slices, P.at_col, P.at_val, sm, [&](int j) { return P.cbeg[j + 1] - P.cbeg[j]; },
+            [&](int j, int* c, double* v) {
+              const int p0 = P.cbeg[j], len = P.cbeg[j + 1] - p0;
+              bool sorted = true;
+              for (int k = 0; k < len; k++) {
+                c[32 * k] = P.cidx[p0 + k]; v[32 * k] = P.cval[p0 + k];
+                if (k > 0 && P.cidx[p0 + k] < P.cidx[p0 + k - 1]) sorted = false;
+              }
+              if (!sorted)   // stable insertion sort by row
+                for (int k = 1; k < len; k++) {
+                  const int ck = c[32 * k];
+                  const double vk = v[32 * k];
+                  int h = k - 1;
+                  for (; h >= 0 && c[32 * h] > ck; h--) { c[32 * (h + 1)] = c[32 * h]; v[32 * (h + 1)] = v[32 * h]; }
+                  c[32 * (h + 1)] = ck; v[32 * (h + 1)] = vk;
+                }
+              return len;
+            });
+}
+
 __global__ void __launch_bounds__(kThreads) batch_prep_kernel(const BatchPrep* __restrict__ prep, int do_scale) {
   __shared__ int sm[kThreads + 1];
   __shared__ double smd[kThreads / 32];
   const BatchPrep& P = prep[blockIdx.x];
-  const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
+  const int t = threadIdx.x, wid = t >> 5;
   const int n0 = P.n0, m = P.m, n = P.n, nnz = P.nnz;
   const int nnz0 = nnz - (n - n0);
   const double sense = P.sense;
@@ -242,20 +303,7 @@ __global__ void __launch_bounds__(kThreads) batch_prep_kernel(const BatchPrep* _
   for (int i = t; i < m; i += kThreads) P.rwork[i] = P.rptr[i];
   __syncthreads();
   if (wid == 0) {
-    // one warp walks the positions in order, 32 at a time; lanes that hit the same row take consecutive slots in lane order
-    for (int base = 0; base < nnz; base += 32) {
-      const int p = base + lane;
-      const int i = p < nnz ? P.cidx[p] : -1 - lane;
-      const unsigned same = __match_any_sync(0xffffffffu, i);
-      int q = 0;
-      if (p < nnz) q = P.rwork[i] + __popc(same & ((1u << lane) - 1u));
-      __syncwarp();
-      if (p < nnz) {
-        P.rpos[q] = p;
-        if (lane == __ffs(same) - 1) P.rwork[i] += __popc(same);
-      }
-      __syncwarp();
-    }
+    row_walk(nnz, P.cidx, P.rwork, P.rpos);
   } else if (t == 32 || t == 64) {   // |c|^2 and |b|^2 of the unscaled form, index order (formulate's norms, squared)
     const double* v = t == 32 ? cost : rhs;
     const int len = t == 32 ? n : m;
@@ -329,33 +377,8 @@ __global__ void __launch_bounds__(kThreads) batch_prep_kernel(const BatchPrep* _
   }
   const double amax = block_max(am, smd);
 
-  // ---- the ordered sliced-ELL bodies (build_layout, identity orderings, no long rows): A's rows in the row-major index's
-  // order; A' row j = column j sorted by row, stably (build_col_major)
-  sell_body(m, P.a_slices, P.a_col, P.a_val, sm, [&](int r) { return P.rptr[r + 1] - P.rptr[r]; },
-            [&](int r, int* c, double* v) {
-              const int q0 = P.rptr[r], len = P.rptr[r + 1] - q0;
-              for (int k = 0; k < len; k++) { const int p = P.rpos[q0 + k]; c[32 * k] = P.pcol[p]; v[32 * k] = P.cval[p]; }
-              return len;
-            });
-  __syncthreads();
-  sell_body(n, P.at_slices, P.at_col, P.at_val, sm, [&](int j) { return P.cbeg[j + 1] - P.cbeg[j]; },
-            [&](int j, int* c, double* v) {
-              const int p0 = P.cbeg[j], len = P.cbeg[j + 1] - p0;
-              bool sorted = true;
-              for (int k = 0; k < len; k++) {
-                c[32 * k] = P.cidx[p0 + k]; v[32 * k] = P.cval[p0 + k];
-                if (k > 0 && P.cidx[p0 + k] < P.cidx[p0 + k - 1]) sorted = false;
-              }
-              if (!sorted)   // stable insertion sort by row
-                for (int k = 1; k < len; k++) {
-                  const int ck = c[32 * k];
-                  const double vk = v[32 * k];
-                  int h = k - 1;
-                  for (; h >= 0 && c[32 * h] > ck; h--) { c[32 * (h + 1)] = c[32 * h]; v[32 * (h + 1)] = v[32 * h]; }
-                  c[32 * (h + 1)] = ck; v[32 * (h + 1)] = vk;
-                }
-              return len;
-            });
+  // ---- the ordered sliced-ELL bodies
+  form_layouts(P, m, n, sm);
 
   // ---- the start point (engine.cu host_start_point) and xSum = proj(0)
   const bool warm = P.warm_x && P.warm_rv && P.warm_rd;
@@ -431,272 +454,20 @@ __global__ void __launch_bounds__(kThreads) batch_post_kernel(const BatchPrep* _
   }
 }
 
-// ===================================================================================== HiPDLP batch
-// the ordered sliced-ELL bodies of the form (build_layout, identity orderings, no long rows): A's rows in the row-major
-// index's order; A' row j = column j sorted by row, stably (build_col_major).  (batch_prep_kernel keeps the two bodies written
-// out in place, so that its machine code stays as it was; the HiPDLP kernel calls this.)
-__device__ __forceinline__ void form_layouts(const BatchPrep& P, int m, int n, int* sm) {
-  sell_body(m, P.a_slices, P.a_col, P.a_val, sm, [&](int r) { return P.rptr[r + 1] - P.rptr[r]; },
-            [&](int r, int* c, double* v) {
-              const int q0 = P.rptr[r], len = P.rptr[r + 1] - q0;
-              for (int k = 0; k < len; k++) { const int p = P.rpos[q0 + k]; c[32 * k] = P.pcol[p]; v[32 * k] = P.cval[p]; }
-              return len;
-            });
-  __syncthreads();
-  sell_body(n, P.at_slices, P.at_col, P.at_val, sm, [&](int j) { return P.cbeg[j + 1] - P.cbeg[j]; },
-            [&](int j, int* c, double* v) {
-              const int p0 = P.cbeg[j], len = P.cbeg[j + 1] - p0;
-              bool sorted = true;
-              for (int k = 0; k < len; k++) {
-                c[32 * k] = P.cidx[p0 + k]; v[32 * k] = P.cval[p0 + k];
-                if (k > 0 && P.cidx[p0 + k] < P.cidx[p0 + k - 1]) sorted = false;
-              }
-              if (!sorted)   // stable insertion sort by row
-                for (int k = 1; k < len; k++) {
-                  const int ck = c[32 * k];
-                  const double vk = v[32 * k];
-                  int h = k - 1;
-                  for (; h >= 0 && c[32 * h] > ck; h--) { c[32 * (h + 1)] = c[32 * h]; v[32 * (h + 1)] = v[32 * h]; }
-                  c[32 * (h + 1)] = ck; v[32 * (h + 1)] = vk;
-                }
-              return len;
-            });
-}
-
-// The twins of host_prep_hipdlp.cpp formulate_hipdlp / scale_hipdlp, build_layout and engine_hipdlp.cu hip_host_postsolve.
-
-// batch_size_kernel under formulate_hipdlp's classification: +-infinity thresholds (a bound of 1e25 is finite), FREE rows a
-// class of their own, BOUND and FREE rows equality-like, each with a slack column
-__global__ void __launch_bounds__(kThreads) hip_batch_size_kernel(const BatchPrep* __restrict__ prep, BatchSize* __restrict__ sizes) {
-  __shared__ int flag[4];
-  __shared__ int sm_eq[kThreads + 1], sm_bnd[kThreads + 1];
-  __shared__ unsigned long long acc;
-  const BatchPrep& P = prep[blockIdx.x];
-  BatchSize& S = sizes[blockIdx.x];
-  const int t = threadIdx.x, n0 = P.n0, m = P.m;
-  if (t < 4) flag[t] = 0;
-  __syncthreads();
-  // check_lp(deep): a_start[0] == 0, a_start non-decreasing, the matrix arrays present, a_index in [0, num_row)
-  if (t == 0 && P.a_start[0] != 0) flag[0] = kPrepStart0;
-  for (int j = t; j < n0; j += kThreads)
-    if (P.a_start[j + 1] < P.a_start[j]) flag[1] = kPrepDecreasing;
-  __syncthreads();
-  const int nnz0 = P.a_start[n0];
-  if (t == 0 && nnz0 > 0 && (!P.a_index || !P.a_value)) flag[2] = kPrepNull;
-  __syncthreads();
-  const int early = flag[0] ? flag[0] : flag[1] ? flag[1] : flag[2];
-  if (early) {
-    if (t == 0) S.err = early;
-    return;
-  }
-  for (int p = t; p < nnz0; p += kThreads)
-    if ((unsigned)P.a_index[p] >= (unsigned)m) flag[3] = kPrepIndex;
-  __syncthreads();
-  if (flag[3]) {
-    if (t == 0) S.err = kPrepIndex;
-    return;
-  }
-  // formulate_hipdlp's row classes
-  for (int i = t; i < m; i += kThreads) {
-    const double rl = P.row_lower[i], ru = P.row_upper[i];
-    const bool lo = rl > -kInf, up = ru < kInf;
-    int c;
-    if (lo && up) c = (rl == ru) ? kEq : kBound;
-    else if (lo) c = kGeq;
-    else if (up) c = kLeq;
-    else c = kFreeRow;
-    P.row_class[i] = c;
-  }
-  for (int i = t; i <= m; i += kThreads) P.rptr[i] = 0;
-  __syncthreads();
-  // the new row order: equality-like rows (EQ / BOUND / FREE) first, then LEQ / GEQ, each in original order;
-  // slack columns in the order of their rows
-  const int chunk = (m + kThreads - 1) / kThreads;
-  const int b = min(t * chunk, m), e = min(b + chunk, m);
-  int eq = 0, bnd = 0;
-  for (int i = b; i < e; i++) {
-    const int c = P.row_class[i];
-    eq += (c == kEq || c == kBound || c == kFreeRow);
-    bnd += (c == kBound || c == kFreeRow);
-  }
-  sm_eq[t] = eq; sm_bnd[t] = bnd;
-  __syncthreads();
-  if (t == 0) {
-    int re = 0, rb = 0;
-    for (int k = 0; k < kThreads; k++) {
-      const int ve = sm_eq[k], vb = sm_bnd[k];
-      sm_eq[k] = re; sm_bnd[k] = rb;
-      re += ve; rb += vb;
-    }
-    sm_eq[kThreads] = re; sm_bnd[kThreads] = rb;
-  }
-  __syncthreads();
-  const int neq = sm_eq[kThreads], nb = sm_bnd[kThreads];
-  {
-    int head = sm_eq[t], tail = neq + (b - sm_eq[t]), sl = sm_bnd[t];
-    for (int i = b; i < e; i++) {
-      const int c = P.row_class[i];
-      P.row_new_idx[i] = (c == kEq || c == kBound || c == kFreeRow) ? head++ : tail++;
-      P.slack[i] = (c == kBound || c == kFreeRow) ? sl++ : -1;
-    }
-  }
-  __syncthreads();
-  // the standard form's row lengths (integer counts: order-free), a slack row's slack entry included
-  for (int p = t; p < nnz0; p += kThreads) atomicAdd(&P.rptr[P.row_new_idx[P.a_index[p]]], 1);
-  for (int i = t; i < m; i += kThreads)
-    if (P.slack[i] >= 0) atomicAdd(&P.rptr[P.row_new_idx[i]], 1);
-  __syncthreads();
-  const long long pa = padded(m, [&](int r) { return P.rptr[r]; }, &acc);
-  const long long pat = padded(n0 + nb, [&](int j) { return j < n0 ? P.a_start[j + 1] - P.a_start[j] : 1; }, &acc);
-  if (t == 0) {
-    S.err = kPrepOk;
-    S.n = n0 + nb; S.nnz = nnz0 + nb; S.neq = neq;
-    // (ordered_max keeps these far below 2^31; the host checks the dimensions before it trusts them)
-    S.pad_a = (int)min(pa, 2000000000ll); S.pad_at = (int)min(pat, 2000000000ll);
-  }
-}
-
-__global__ void __launch_bounds__(kThreads)
+// formulate_hipdlp, the row-major indexes and scale_hipdlp (hip_form.cuh hip_form; every listed column ranked whole), then the
+// ordered sliced-ELL bodies (every column is already sorted by row)
+__global__ void __launch_bounds__(kThreads, 3)
 hip_batch_prep_kernel(const BatchPrep* __restrict__ prep, const HipBatchPrep* __restrict__ hprep, int scaling_mode,
                       int ruiz_iterations) {
   __shared__ int sm[kThreads + 1];
-  __shared__ int s_row[kThreads];
-  __shared__ unsigned long long s_key[kThreads];
-  __shared__ int nsort;
   const BatchPrep& P = prep[blockIdx.x];
-  const HipBatchPrep& H = hprep[blockIdx.x];
-  const int t = threadIdx.x, wid = t >> 5;
-  const int n0 = P.n0, m = P.m, n = P.n, nnz = P.nnz;
-  const int nnz0 = nnz - (n - n0);
+  const int m = P.m, n = P.n;
   using V = HipBatchVec;
-  double* cost = V::col(P.vec, n, V::kCost);
-  double* lower = V::col(P.vec, n, V::kLower);
-  double* upper = V::col(P.vec, n, V::kUpper);
-  double* colscale = V::col(P.vec, n, V::kColscale);
-  double* rlo = V::row(P.vec, n, m, V::kRlo);
-  double* rup = V::row(P.vec, n, m, V::kRup);
-  double* rowscale = V::row(P.vec, n, m, V::kRowscale);
-  const int* rni = P.row_new_idx;
-  const int* rcl = P.row_class;
-  if (t == 0) nsort = 0;
-  __syncthreads();
-
-  // ---- formulate_hipdlp (hip_form.cuh hip_formulate, hip_rank_entries, hip_row_indexes and hip_scale are these steps
-  // for the tree-mode prologue; this kernel keeps them written out in place, so that its machine code stays as it was).
-  // A structural column keeps cbeg[j] = a_start[j], its entries ordered by (new row, value) with LEQ
-  // rows negated.  Stored rows strictly ascending: the new rows ascend inside the equality-like group and inside the rest, so
-  // that order is the stable partition.  Other columns go on the work list for the sort below.  Costs keep their sign and
-  // bounds are not clamped.
-  for (int j = t; j < n0; j += kThreads) {
-    const int p0 = P.a_start[j], p1 = P.a_start[j + 1];
-    P.cbeg[j] = p0;
-    bool ascending = true;
-    for (int p = p0 + 1; p < p1; p++)
-      if (P.a_index[p] <= P.a_index[p - 1]) ascending = false;
-    if (ascending) {
-      int k = p0;
-      for (int p = p0; p < p1; p++) {
-        const int i = P.a_index[p];
-        if (rni[i] < P.neq) { P.cidx[k] = rni[i]; P.cval[k] = rcl[i] == kLeq ? -P.a_value[p] : P.a_value[p]; P.pcol[k] = j; k++; }
-      }
-      for (int p = p0; p < p1; p++) {
-        const int i = P.a_index[p];
-        if (rni[i] >= P.neq) { P.cidx[k] = rni[i]; P.cval[k] = rcl[i] == kLeq ? -P.a_value[p] : P.a_value[p]; P.pcol[k] = j; k++; }
-      }
-    } else {
-      H.sortcols[atomicAdd(&nsort, 1)] = j;
-    }
-    cost[j] = P.col_cost[j];
-    lower[j] = P.col_lower[j];
-    upper[j] = P.col_upper[j];
-    colscale[j] = 1.0;
-  }
-  for (int i = t; i < m; i += kThreads) {
-    const int r = rni[i], c = rcl[i];
-    rlo[r] = (c == kEq || c == kGeq) ? P.row_lower[i] : c == kLeq ? -P.row_upper[i] : 0.0;
-    rup[r] = c == kEq ? P.row_upper[i] : (c == kGeq || c == kLeq) ? kInf : 0.0;
-    rowscale[r] = 1.0;
-    H.optr[i] = P.rptr[r] - (P.slack[i] >= 0);   // the caller's row length (rptr: the form's, before its scan)
-    if (P.slack[i] >= 0) {   // one -1 slack column per BOUND / FREE row, in row order, with the row's raw bounds
-      const int j = n0 + P.slack[i], q = nnz0 + P.slack[i];
-      P.cbeg[j] = q; P.cidx[q] = r; P.cval[q] = -1.0; P.pcol[q] = j;
-      cost[j] = 0.0;
-      lower[j] = P.row_lower[i];
-      upper[j] = P.row_upper[i];
-      colscale[j] = 1.0;
-    }
-  }
-  if (t == 0) P.cbeg[n] = nnz;
-  __syncthreads();
-  // the listed columns, sorted by the whole CTA: an entry's slot is its rank under (new row, value key, stored index), the
-  // other entries streamed through shared memory a tile at a time.  (value_key orders -0.0 before +0.0, which std::sort
-  // leaves in either order.)
-  const int ns = nsort;
-  for (int s = 0; s < ns; s++) {
-    const int j = H.sortcols[s];
-    const int p0 = P.a_start[j], len = P.a_start[j + 1] - p0;
-    for (int k0 = 0; k0 < len; k0 += kThreads) {
-      const int k = k0 + t;
-      int row = 0;
-      double v = 0.0;
-      unsigned long long key = 0;
-      if (k < len) {
-        const int i = P.a_index[p0 + k];
-        row = rni[i];
-        v = rcl[i] == kLeq ? -P.a_value[p0 + k] : P.a_value[p0 + k];
-        key = value_key(v);
-      }
-      int rank = 0;
-      for (int h0 = 0; h0 < len; h0 += kThreads) {
-        __syncthreads();
-        if (h0 + t < len) {
-          const int i = P.a_index[p0 + h0 + t];
-          s_row[t] = rni[i];
-          s_key[t] = value_key(rcl[i] == kLeq ? -P.a_value[p0 + h0 + t] : P.a_value[p0 + h0 + t]);
-        }
-        __syncthreads();
-        if (k < len) {
-          const int cnt = min(kThreads, len - h0);
-          for (int h = 0; h < cnt; h++) {
-            const int rh = s_row[h];
-            const unsigned long long kh = s_key[h];
-            rank += rh < row || (rh == row && (kh < key || (kh == key && h0 + h < k)));
-          }
-        }
-      }
-      if (k < len) { const int q = p0 + rank; P.cidx[q] = row; P.cval[q] = v; P.pcol[q] = j; }
-    }
-  }
-  __syncthreads();
-
-  // ---- the row-major indexes (build_row_index) of the form and of the caller's matrix (the postsolve's row sums)
-  const int rtotal = block_scan(P.rptr, 1, m, sm);
-  if (t == 0) P.rptr[m] = rtotal;
-  const int ototal = block_scan(H.optr, 1, m, sm);
-  if (t == 0) H.optr[m] = ototal;
-  for (int i = t; i < m; i += kThreads) P.rwork[i] = P.rptr[i];
-  __syncthreads();
-  if (wid == 0) {
-    row_walk(nnz, P.cidx, P.rwork, P.rpos);
-    for (int i = t; i < m; i += 32) P.rwork[i] = H.optr[i];
-    __syncwarp();
-    row_walk(nnz0, P.a_index, P.rwork, H.opos);
-  } else if (t == 32 || t == 64) {   // |c|^2 and |b|^2 of the unscaled form, index order (formulate_hipdlp's norms, squared)
-    const double* v = t == 32 ? cost : rlo;
-    const int len = t == 32 ? n : m;
-    double s = 0.0;
-    for (int q = 0; q < len; q++) s += v[q] * v[q];
-    P.rec[t == 32 ? kRecCostSq : kRecRhsSq] = s;
-  }
-  __syncthreads();
-
-  // ---- scale_hipdlp: Ruiz x ruiz_iterations, then Pock-Chambolle, then L2, each pass as its bit of scaling_mode says
-  if (scaling_mode & 1)
-    for (int it = 0; it < ruiz_iterations; it++) hip_scale_pass<0>(P, cost, lower, upper, colscale, rlo, rup, rowscale);
-  if (scaling_mode & 4) hip_scale_pass<1>(P, cost, lower, upper, colscale, rlo, rup, rowscale);
-  if (scaling_mode & 2) hip_scale_pass<2>(P, cost, lower, upper, colscale, rlo, rup, rowscale);
-
-  // ---- the ordered sliced-ELL bodies (every column is already sorted by row)
+  HipFormVecs F;
+  F.cost = V::col(P.vec, n, V::kCost); F.lower = V::col(P.vec, n, V::kLower); F.upper = V::col(P.vec, n, V::kUpper);
+  F.colscale = V::col(P.vec, n, V::kColscale);
+  F.rlo = V::row(P.vec, n, m, V::kRlo); F.rup = V::row(P.vec, n, m, V::kRup); F.rowscale = V::row(P.vec, n, m, V::kRowscale);
+  hip_form(P, hprep[blockIdx.x], F, scaling_mode, ruiz_iterations, sm, [](auto&&...) { return false; });
   form_layouts(P, m, n, sm);
 }
 

@@ -1,19 +1,21 @@
 // highs_b200/csrc/batch_tree_prep.cu -- the device prologue and postsolve of the tree members of
-// b200pdlp_solve_hipdlp_batch_mixed_device (engine_batch.cu solve_hipdlp_batch_mixed_device): one CTA of kThreads threads
+// b200pdlp_solve_hipdlp_batch_mixed_device (engine_batch.cu solve_hipdlp_batch_device): one CTA of kThreads threads
 // per member, and no CTA waits on another, so any number of members runs.  After hip_batch_size_kernel (batch_prep.cu):
 //
 //   hip_tree_plan_kernel   make_perm of the form's rows and columns (stable sorts by descending length in windows of
 //                          kSortWindow that never straddle neq), their inverses, and plan_sell of A and A' (slice
 //                          descriptors, long rows, segments): what the host needs to lay out the bodies and the scratch
-//   hip_tree_form_kernel   formulate_hipdlp, the row-major indexes, scale_hipdlp (hip_form.cuh), in standard-form order
+//   hip_tree_form_kernel   formulate_hipdlp, the row-major indexes, scale_hipdlp (hip_form.cuh hip_form), in standard-form
+//                          order
 //   hip_tree_fill_kernel   the seven data vectors gathered into device order, and the tree sliced-ELL bodies and long-row
 //                          arrays of A and A'
 //   hip_tree_post_kernel   hip_host_postsolve of the returned iterate, its device-order vectors read through cinv / rinv
 //
 // Bits: every value is that of build_layout(f, 0, 1, -1) (host_prep.cpp make_perm / plan_sell / build_sell) after
 // formulate_hipdlp / scale_hipdlp, packed as solve_hipdlp_batch packs a tree member.  The orderings and plans are integer
-// work; the formulate and scale steps are hip_batch_prep_kernel's.  An unsorted column is ordered by (new row, value key,
-// stored index) as there, but in O(len log len): tiles of kTreeSortTile entries ranked in shared memory, then merged.
+// work; the formulate and scale steps are hip_batch_prep_kernel's (hip_form.cuh hip_form), in standard-form order.  An
+// unsorted column is ordered by (new row, value key, stored index) as there; one longer than kTreeSortTile entries in
+// O(len log len): tiles of kTreeSortTile entries ranked in shared memory, then merged.
 #include <cub/block/block_radix_sort.cuh>
 
 #include "hip_form.cuh"
@@ -229,40 +231,21 @@ __device__ __forceinline__ HipFormVecs std_order_vecs(const BatchPrep& P) {
   return F;
 }
 
-// formulate_hipdlp, the row-major indexes and scale_hipdlp (hip_batch_prep_kernel's steps), in standard-form order.
+// formulate_hipdlp, the row-major indexes and scale_hipdlp (hip_form.cuh hip_form), in standard-form order; a listed column
+// longer than kTreeSortTile is sorted by sort_long_column.
 // (__maxnreg__ instead of __launch_bounds__: under the latter ptxas keeps this kernel at 64 registers and spills.)
 __global__ void __maxnreg__(96)
 hip_tree_form_kernel(const BatchPrep* __restrict__ prep, const HipBatchPrep* __restrict__ hprep,
                      const HipTreePrep* __restrict__ tprep, int scaling_mode, int ruiz_iterations) {
   __shared__ int sm[kThreads + 1];
-  __shared__ int s_row[kThreads];
-  __shared__ unsigned long long s_key[kThreads];
-  __shared__ int nsort;
   const BatchPrep& P = prep[blockIdx.x];
-  const HipBatchPrep& H = hprep[blockIdx.x];
   const HipTreePrep& T = tprep[blockIdx.x];
-  const int t = threadIdx.x;
-  const HipFormVecs F = std_order_vecs(P);
-  if (t == 0) nsort = 0;
-  __syncthreads();
-  hip_formulate(P, H, F, &nsort);
-  __syncthreads();
-  const int ns = nsort;
-  for (int s = 0; s < ns; s++) {
-    const int j = H.sortcols[s];
-    const int p0 = P.a_start[j], len = P.a_start[j + 1] - p0;
-    if (len > kTreeSortTile) {
-      sort_long_column(P, T, j, s_row, s_key);
-      continue;
-    }
-    hip_rank_entries(P, j, 0, len, s_row, s_key, [&](int rank, int, int row, double val, unsigned long long) {
-      const int q = p0 + rank;
-      P.cidx[q] = row; P.cval[q] = val; P.pcol[q] = j;
-    });
-  }
-  __syncthreads();
-  hip_row_indexes(P, H, F, sm);
-  hip_scale(P, F, scaling_mode, ruiz_iterations);
+  hip_form(P, hprep[blockIdx.x], std_order_vecs(P), scaling_mode, ruiz_iterations, sm,
+           [&](int j, int len, int* s_row, unsigned long long* s_key) {
+             if (len <= kTreeSortTile) return false;
+             sort_long_column(P, T, j, s_row, s_key);
+             return true;
+           });
 }
 
 // the seven data vectors gathered into device order, and the tree layouts of A and A'

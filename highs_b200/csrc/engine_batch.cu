@@ -1099,71 +1099,8 @@ static void solve_hipdlp_batch(int count, const b200pdlp_lp* lps, const b200pdlp
   lap("batch", "postsolve (host threads)");
 }
 
-// ------------------------------------------------------------------ HiPDLP batch of small LPs already on the GPU
-// b200pdlp_solve_hipdlp_batch_device: solve_hipdlp_batch for LPs whose arrays are device memory.  The prologue and the
-// postsolve run on the device, one CTA per member (batch_prep.cu hip_batch_*_kernel); the rounds are solve_hipdlp_batch's
-// (hip_batch_rounds).  The host reads one sizing record and |c|^2, |b|^2 per member, never an array.
-
-static void solve_hipdlp_batch_device(int count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params& prm, b200pdlp_result* outs) {
-  using clk = std::chrono::steady_clock;
-  const char* who = "b200pdlp_solve_hipdlp_batch_device";
-  const auto t_begin = clk::now();
-  Laps lap;
-  const int device = select_device(prm.device);
-  check_device_arrays(count, lps, nullptr, outs, device, who);
-  StreamHolder sh;
-  cudaStream_t s = sh.s;
-  DeviceBatch D;
-  PrepMode mode;
-  mode.hip = true; mode.scaling = prm.scaling_mode; mode.ruiz_iterations = prm.ruiz_iterations;
-  {
-    NvtxRange nvtx("b200pdlp: HiPDLP batch prologue (device)");
-    device_batch_prologue(s, count, lps, nullptr, mode, prm.ordered_max, who, D, lap);
-  }
-  const bool scaled = (prm.scaling_mode & 7) != 0;   // scale_hipdlp: any of its passes is switched on
-  std::vector<HipBatchRun> runs((size_t)count);
-  std::vector<HipBatchRun*> R((size_t)count);
-  std::vector<HipBatchMember> hmem((size_t)count);
-  for (int i = 0; i < count; i++) {
-    HipBatchRun& b = runs[i];
-    const BatchPrep& P = D.hp[i];
-    const double* r = D.rec.data() + (size_t)kPrepRec * i;
-    StdForm& f = b.f;
-    f.hipdlp = true;
-    f.n = P.n; f.m = P.m; f.nnz = P.nnz; f.neq = P.neq; f.n_orig = P.n0;
-    f.sense = lps[i].sense; f.offset = lps[i].offset;
-    f.norm_cost = std::sqrt(r[kRecCostSq]); f.norm_rhs = std::sqrt(r[kRecRhsSq]);
-    f.scaled = scaled;
-    R[i] = &b;
-    hip_batch_member(hmem[i], f, P.neq, P.vec);
-    set_layouts(hmem[i], P.a_slices, P.a_col, P.a_val, P.at_slices, P.at_col, P.at_val);
-  }
-  DevBuf<HipBatchMember> dmem;
-  dmem.alloc(count, false);
-  CUDA_OK(cudaMemcpyAsync(dmem.p, hmem.data(), (size_t)count * sizeof(HipBatchMember), cudaMemcpyHostToDevice, s));
-  const BatchLoop loop = hip_batch_rounds(s, count, prm, dmem.p, R);
-  lap("batch device", "rounds");
-
-  // ---- the postsolve of every member on the device, into the caller's vectors
-  NvtxRange nvtx_post("b200pdlp: HiPDLP batch postsolve (device)");
-  std::vector<HipBatchPost> hpost((size_t)count);
-  for (int i = 0; i < count; i++) {
-    HipBatchPost& q = hpost[i];
-    q.col_value = outs[i].col_value; q.col_dual = outs[i].col_dual; q.row_value = outs[i].row_value; q.row_dual = outs[i].row_dual;
-    q.sol = runs[i].converged ? runs[i].sol : -1;
-    q.pad = 0;
-  }
-  DevBuf<HipBatchPost> dpost;
-  dpost.alloc(count, false);
-  CUDA_OK(cudaMemcpyAsync(dpost.p, hpost.data(), (size_t)count * sizeof(HipBatchPost), cudaMemcpyHostToDevice, s));
-  launch_hip_batch_post(s, count, D.prep.p, D.dhx.p, dpost.p, scaled ? 1 : 0);
-  CUDA_OK(cudaGetLastError());
-  CUDA_OK(cudaStreamSynchronize(s));
-  const double setup_seconds = std::chrono::duration<double>(loop.t_loop - t_begin).count();
-  for (int i = 0; i < count; i++) hip_batch_result(outs + i, runs[i], loop, setup_seconds);
-  lap("batch device", "postsolve (device)");
-}
-
+// ---- b200pdlp_debug_hipdlp_batch_prep_compare: the ordered members' device prologue and postsolve (batch_prep.cu
+// hip_batch_*_kernel) against formulate_hipdlp + scale_hipdlp + build_layout and hip_host_postsolve
 static void hipdlp_batch_prep_compare(int count, const b200pdlp_lp* lps, int scaling_mode, int ruiz_iterations, double* report) {
   using V = HipBatchVec;
   device_count_checked();
@@ -1256,13 +1193,13 @@ static void hipdlp_batch_prep_compare(int count, const b200pdlp_lp* lps, int sca
   }
 }
 
-// ----------------------------------------------------------- HiPDLP batch past ordered_max, LPs already on the GPU
-// b200pdlp_solve_hipdlp_batch_mixed_device: solve_hipdlp_batch_mixed for LPs whose arrays are device memory.  Every member's
-// prologue and postsolve run on the device, one CTA per member: the ordered members' in batch_prep.cu (as
-// b200pdlp_solve_hipdlp_batch_device), the tree members' in batch_tree_prep.cu.  The rounds are hip_batch_rounds with the
-// tree members on hip_tree_round_kernel.  The host reads fixed-size records per member, never an array.
-// STATUS: runs on hardware; tests/test_gpu_hipdlp_batch_mixed_device.py, tools/hipdlp_batch_mixed_device_bench.py
-// (DESIGN.md section 6).
+// ----------------------------------------------------------------------- HiPDLP batch of LPs already on the GPU
+// b200pdlp_solve_hipdlp_batch_device and _mixed_device: solve_hipdlp_batch for LPs whose arrays are device memory.  Every
+// member's prologue and postsolve run on the device, one CTA per member: the ordered members' in batch_prep.cu, the tree
+// members' (_mixed_device only) in batch_tree_prep.cu.  The rounds are hip_batch_rounds with the tree members on
+// hip_tree_round_kernel.  The host reads fixed-size records per member, never an array.
+// STATUS: runs on hardware; tests/test_gpu_hipdlp_batch_device.py, tests/test_gpu_hipdlp_batch_mixed_device.py,
+// tools/batch_device_bench.py, tools/hipdlp_batch_mixed_device_bench.py (DESIGN.md section 6).
 
 // The tree members' device prologue: the members' BatchPrep (from the sizing), HipBatchPrep, HipTreePrep and plans, and the
 // pools behind them
@@ -1423,10 +1360,13 @@ static void device_form(StdForm& f, const BatchPrep& P, const b200pdlp_lp& lp, c
   f.scaled = scaled;
 }
 
-static void solve_hipdlp_batch_mixed_device(int count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params& prm,
-                                            b200pdlp_result* outs) {
+// `mixed`: a member past ordered_max is a tree member and the results take the blocks' trace rows; otherwise such a member
+// is an error
+static void solve_hipdlp_batch_device(int count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params& prm,
+                                      b200pdlp_result* outs, bool mixed) {
   using clk = std::chrono::steady_clock;
-  const char* who = "b200pdlp_solve_hipdlp_batch_mixed_device";
+  const char* who = mixed ? "b200pdlp_solve_hipdlp_batch_mixed_device" : "b200pdlp_solve_hipdlp_batch_device";
+  const std::string nvtx_name = mixed ? "b200pdlp: HiPDLP mixed batch " : "b200pdlp: HiPDLP batch ";
   const auto t_begin = clk::now();
   Laps lap;
   const int device = select_device(prm.device);
@@ -1439,7 +1379,7 @@ static void solve_hipdlp_batch_mixed_device(int count, const b200pdlp_lp* lps, c
   std::vector<int> src;   // device member k is the caller's member src[k]: the ordered members, then the tree members
   int ntree = 0;
   {
-    NvtxRange nvtx("b200pdlp: HiPDLP mixed batch validation + sizing (device)");
+    NvtxRange nvtx((nvtx_name + "validation + sizing (device)").c_str());
     device_batch_size(s, count, lps, nullptr, mode, D);
     const int omax = prm.ordered_max == 0 ? 4096 : prm.ordered_max;
     std::vector<int> tree;
@@ -1449,6 +1389,9 @@ static void solve_hipdlp_batch_mixed_device(int count, const b200pdlp_lp* lps, c
       if (z.err != kPrepOk) throw Error(B200PDLP_ERR_ARG, at + prep_error_text(z.err));
       const int m = lps[i].num_row, big = std::max(z.n, m);
       if (omax < 0 || big > omax) {   // (a tree member's pad_a / pad_at, the ordered layout's padding, mean nothing)
+        if (!mixed)
+          throw Error(B200PDLP_ERR_ARG, at + "standard form " + std::to_string(m) + " x " + std::to_string(z.n) +
+                                            " exceeds ordered_max = " + std::to_string(omax));
         if (big > kTreeMemberMax)
           throw Error(B200PDLP_ERR_ARG, at + "standard form " + std::to_string(m) + " x " + std::to_string(z.n) +
                                             " exceeds max(n, m) = " + std::to_string(kTreeMemberMax) +
@@ -1476,16 +1419,16 @@ static void solve_hipdlp_batch_mixed_device(int count, const b200pdlp_lp* lps, c
   std::vector<int> oids, tids;
   group(0, nord, O.hp, O.size, olps, oids);
   TreeBatch T;
-  {
+  if (mixed) {
     NvtxRange nvtx("b200pdlp: HiPDLP mixed batch orderings + plans (device)");
     std::vector<BatchPrep> thp;
     std::vector<BatchSize> tsz;
     group(nord, count, thp, tsz, tlps, tids);
     if (ntree > 0) tree_batch_plan(s, thp, tsz, tids, who, T);
+    lap("batch device", "orderings + plans");
   }
-  lap("batch device", "orderings + plans");
   {
-    NvtxRange nvtx("b200pdlp: HiPDLP mixed batch prologue (device)");
+    NvtxRange nvtx((nvtx_name + "prologue (device)").c_str());
     if (nord > 0) device_batch_prep(s, nord, olps.data(), mode, O);
     if (ntree > 0) tree_batch_prep(s, prm.scaling_mode, prm.ruiz_iterations, T);
   }
@@ -1499,8 +1442,7 @@ static void solve_hipdlp_batch_mixed_device(int count, const b200pdlp_lp* lps, c
   for (int k = 0; k < count; k++) {
     HipBatchRun& b = runs[k];
     R[k] = &b;
-    b.trace = outs + src[k];
-    b.trace->trace_len = 0;
+    if (mixed) { b.trace = outs + src[k]; b.trace->trace_len = 0; }
     if (k < nord) {
       const BatchPrep& P = O.hp[k];
       device_form(b.f, P, lps[src[k]], O.rec.data() + (size_t)kPrepRec * k, scaled);
@@ -1523,7 +1465,7 @@ static void solve_hipdlp_batch_mixed_device(int count, const b200pdlp_lp* lps, c
   lap("batch device", "rounds");
 
   // ---- the postsolve of every member on the device, into the caller's vectors
-  NvtxRange nvtx_post("b200pdlp: HiPDLP mixed batch postsolve (device)");
+  NvtxRange nvtx_post((nvtx_name + "postsolve (device)").c_str());
   std::vector<HipBatchPost> hpost((size_t)count);
   for (int k = 0; k < count; k++) {
     HipBatchPost& q = hpost[k];
@@ -1860,6 +1802,18 @@ static int batch_entry(const char* who, int count, bool args_ok, F&& solve) {
   });
 }
 
+// The three prologue comparisons' entry: the caller's device restored on return, count >= 0, no NULL argument and every LP
+// well-formed (check_lp), then compare() when there is a member
+template <class F>
+static int prep_compare_entry(const char* who, int count, const b200pdlp_lp* lps, const double* report, F&& compare) {
+  DeviceGuard dg;
+  return guarded([&] {
+    if (count < 0 || (count > 0 && (!lps || !report))) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": bad arguments");
+    for (int i = 0; i < count; i++) check_lp(&lps[i]);
+    if (count > 0) compare();
+  });
+}
+
 }  // namespace b200
 
 extern "C" {
@@ -1885,12 +1839,8 @@ int b200pdlp_solve_batch_device(int32_t count, const b200pdlp_lp* lps, const b20
 }
 
 int b200pdlp_debug_batch_prep_compare(int32_t count, const b200pdlp_lp* lps, int32_t scaling, double* report) {
-  DeviceGuard dg;
-  return guarded([&] {
-    if (count < 0 || (count > 0 && (!lps || !report))) throw Error(B200PDLP_ERR_ARG, "b200pdlp_debug_batch_prep_compare: bad arguments");
-    for (int i = 0; i < count; i++) check_lp(&lps[i]);
-    if (count > 0) batch_prep_compare(count, lps, scaling, report);
-  });
+  return prep_compare_entry("b200pdlp_debug_batch_prep_compare", count, lps, report,
+                            [&] { batch_prep_compare(count, lps, scaling, report); });
 }
 
 int b200pdlp_solve_hipdlp_batch(int32_t count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params* params,
@@ -1922,7 +1872,7 @@ int b200pdlp_solve_hipdlp_batch_device(int32_t count, const b200pdlp_lp* lps, co
   const char* who = "b200pdlp_solve_hipdlp_batch_device";
   return batch_entry(who, count, lps && params && outs, [&] {
     for (int i = 0; i < count; i++) check_batch_device_member(&lps[i], params->ordered_max, i, who);
-    solve_hipdlp_batch_device(count, lps, *params, outs);
+    solve_hipdlp_batch_device(count, lps, *params, outs, false);
   });
 }
 
@@ -1931,19 +1881,14 @@ int b200pdlp_solve_hipdlp_batch_mixed_device(int32_t count, const b200pdlp_lp* l
   const char* who = "b200pdlp_solve_hipdlp_batch_mixed_device";
   return batch_entry(who, count, lps && params && outs, [&] {
     for (int i = 0; i < count; i++) check_batch_device_member(&lps[i], 0, i, who);   // (any ordered_max: tree members)
-    solve_hipdlp_batch_mixed_device(count, lps, *params, outs);
+    solve_hipdlp_batch_device(count, lps, *params, outs, true);
   });
 }
 
 int b200pdlp_debug_hipdlp_tree_prep_compare(int32_t count, const b200pdlp_lp* lps, int32_t scaling_mode, int32_t ruiz_iterations,
                                             double* report) {
-  DeviceGuard dg;
-  return guarded([&] {
-    if (count < 0 || (count > 0 && (!lps || !report)))
-      throw Error(B200PDLP_ERR_ARG, "b200pdlp_debug_hipdlp_tree_prep_compare: bad arguments");
-    for (int i = 0; i < count; i++) check_lp(&lps[i]);
-    if (count > 0) hipdlp_tree_prep_compare(count, lps, scaling_mode, ruiz_iterations, report);
-  });
+  return prep_compare_entry("b200pdlp_debug_hipdlp_tree_prep_compare", count, lps, report,
+                            [&] { hipdlp_tree_prep_compare(count, lps, scaling_mode, ruiz_iterations, report); });
 }
 
 int b200pdlp_kkt_check_batch(int32_t count, const b200pdlp_lp* lps, const b200pdlp_solution* sols,
@@ -1958,13 +1903,8 @@ int b200pdlp_kkt_check_batch_device(int32_t count, const b200pdlp_lp* lps, const
 
 int b200pdlp_debug_hipdlp_batch_prep_compare(int32_t count, const b200pdlp_lp* lps, int32_t scaling_mode, int32_t ruiz_iterations,
                                              double* report) {
-  DeviceGuard dg;
-  return guarded([&] {
-    if (count < 0 || (count > 0 && (!lps || !report)))
-      throw Error(B200PDLP_ERR_ARG, "b200pdlp_debug_hipdlp_batch_prep_compare: bad arguments");
-    for (int i = 0; i < count; i++) check_lp(&lps[i]);
-    if (count > 0) hipdlp_batch_prep_compare(count, lps, scaling_mode, ruiz_iterations, report);
-  });
+  return prep_compare_entry("b200pdlp_debug_hipdlp_batch_prep_compare", count, lps, report,
+                            [&] { hipdlp_batch_prep_compare(count, lps, scaling_mode, ruiz_iterations, report); });
 }
 
 }  // extern "C"

@@ -1,7 +1,9 @@
 // highs_b200/csrc/hip_form.cuh -- formulate_hipdlp, scale_hipdlp and hip_host_postsolve on device arrays, one CTA of kThreads
-// threads per LP: the pieces hip_batch_prep_kernel / hip_batch_post_kernel (batch_prep.cu, ordered members) and the tree-mode
-// prologue and postsolve (batch_tree_prep.cu) share.  Every value is the host's (host_prep_hipdlp.cpp) with the same
-// operations on the same operands; both files are compiled with -fmad=false and IEEE division and square root.
+// threads per LP.  hip_form (formulate_hipdlp, the row-major indexes, scale_hipdlp) is the prologue of both
+// hip_batch_prep_kernel (batch_prep.cu, ordered members) and hip_tree_form_kernel (batch_tree_prep.cu, tree members);
+// hip_postsolve is the postsolve of both hip_batch_post_kernel and hip_tree_post_kernel.  Every value is the host's
+// (host_prep_hipdlp.cpp) with the same operations on the same operands; both files are compiled with -fmad=false and IEEE
+// division and square root.
 #pragma once
 #include "batch_kernels.hpp"
 #include "batch_prep.hpp"
@@ -200,6 +202,34 @@ __device__ __forceinline__ void hip_scale(const BatchPrep& P, const HipFormVecs&
       hip_scale_pass<0>(P, F.cost, F.lower, F.upper, F.colscale, F.rlo, F.rup, F.rowscale);
   if (scaling_mode & 4) hip_scale_pass<1>(P, F.cost, F.lower, F.upper, F.colscale, F.rlo, F.rup, F.rowscale);
   if (scaling_mode & 2) hip_scale_pass<2>(P, F.cost, F.lower, F.upper, F.colscale, F.rlo, F.rup, F.rowscale);
+}
+
+// ---- the whole HiPDLP prologue up to the layouts: formulate_hipdlp with its listed columns ranked, the row-major indexes and
+// scale_hipdlp, the data vectors at F.  long_sort(j, len, s_row, s_key) sorts a listed column in its own way and returns
+// true, or returns false to have it ranked whole here.  sm: kThreads + 1 ints of shared memory.
+template <class LongSort>
+__device__ __forceinline__ void hip_form(const BatchPrep& P, const HipBatchPrep& H, const HipFormVecs& F, int scaling_mode,
+                                         int ruiz_iterations, int* sm, LongSort&& long_sort) {
+  __shared__ int s_row[kThreads];
+  __shared__ unsigned long long s_key[kThreads];
+  __shared__ int nsort;
+  if (threadIdx.x == 0) nsort = 0;
+  __syncthreads();
+  hip_formulate(P, H, F, &nsort);
+  __syncthreads();
+  const int ns = nsort;
+  for (int s = 0; s < ns; s++) {
+    const int j = H.sortcols[s];
+    const int p0 = P.a_start[j], len = P.a_start[j + 1] - p0;
+    if (long_sort(j, len, s_row, s_key)) continue;
+    hip_rank_entries(P, j, 0, len, s_row, s_key, [&](int rank, int, int row, double val, unsigned long long) {
+      const int q = p0 + rank;
+      P.cidx[q] = row; P.cval[q] = val; P.pcol[q] = j;
+    });
+  }
+  __syncthreads();
+  hip_row_indexes(P, H, F, sm);
+  hip_scale(P, F, scaling_mode, ruiz_iterations);
 }
 
 // ---- hip_host_postsolve of the returned iterate into the caller's device vectors.  The member's vectors are in device

@@ -31,8 +31,6 @@ static __device__ int block_scan(int* a, int stride, int len, int* sm) {
 
 // the row-major index by one warp (build_row_index): position p of row[p] goes to slot rwork[row[p]]++, positions ascending.
 // The warp walks the positions in order, 32 at a time; lanes that hit the same row take consecutive slots in lane order.
-// (batch_prep_kernel keeps this walk written out in place, so that its machine code stays as it was; the HiPDLP kernel and
-// the KKT batch kernel call it.)
 __device__ __forceinline__ void row_walk(int nnz, const int* row, int* rwork, int* rpos) {
   const int lane = threadIdx.x & 31;
   for (int base = 0; base < nnz; base += 32) {

@@ -365,6 +365,23 @@ def solve_batch_device(dlps, warms=None, trace_cap: int = 0, **params) -> list:
     return [_result_dict(cres[i], arrays[i]) for i in range(count)]
 
 
+def _prep_compare(name: str, items, lps, *ints) -> list:
+    """the call of a batch prologue comparison `name` on host LPs, with the int arguments `ints`: one dict of mismatch counts
+    per LP (`items`)"""
+    lps = list(lps)
+    fn = getattr(lib(), name)
+    fn.argtypes = [C.c_int32, C.POINTER(CLp)] + [C.c_int32] * len(ints) + [_dp]
+    count = len(lps)
+    clps, keep = (CLp * max(count, 1))(), []
+    for i, lp in enumerate(lps):
+        clps[i], k = make_clp(lp)
+        keep.append(k)
+    k = len(items)
+    rep = np.zeros(max(count, 1) * k)
+    _check(fn(count, clps, *ints, _p(rep, _dp)), name)
+    return [dict(zip(items, rep[k * i:k * (i + 1)].tolist())) for i in range(count)]
+
+
 BATCH_PREP_ITEMS = ["dims", "cost", "lower", "upper", "rhs", "col_scale", "row_scale", "row_new_idx", "row_class", "A.slices",
                     "A.col", "A.val", "AT.slices", "AT.col", "AT.val", "x0", "y0", "xsum", "norm_cost", "norm_rhs", "amax",
                     "beta_cost_sq", "beta_rhs_sq", "col_value", "col_dual", "row_value", "row_dual"]
@@ -373,18 +390,7 @@ BATCH_PREP_ITEMS = ["dims", "cost", "lower", "upper", "rhs", "col_scale", "row_s
 def batch_prep_compare(lps, scaling: int = 1) -> list:
     """b200pdlp_debug_batch_prep_compare: the device prologue and postsolve of solve_batch_device against their host twins on
     host LPs; one dict of mismatch counts per LP (BATCH_PREP_ITEMS)."""
-    lps = list(lps)
-    L = lib()
-    L.b200pdlp_debug_batch_prep_compare.argtypes = [C.c_int32, C.POINTER(CLp), C.c_int32, _dp]
-    count = len(lps)
-    clps, keep = (CLp * max(count, 1))(), []
-    for i, lp in enumerate(lps):
-        clps[i], k = make_clp(lp)
-        keep.append(k)
-    k = len(BATCH_PREP_ITEMS)
-    rep = np.zeros(max(count, 1) * k)
-    _check(L.b200pdlp_debug_batch_prep_compare(count, clps, scaling, _p(rep, _dp)), "b200pdlp_debug_batch_prep_compare")
-    return [dict(zip(BATCH_PREP_ITEMS, rep[k * i:k * (i + 1)].tolist())) for i in range(count)]
+    return _prep_compare("b200pdlp_debug_batch_prep_compare", BATCH_PREP_ITEMS, lps, scaling)
 
 
 PREP_ITEMS = ["n", "m", "nnz", "neq", "cbeg", "cidx", "cval", "cost", "lower", "upper", "col_scale", "rhs", "row_scale", "rptr",
@@ -607,34 +613,11 @@ def solve_hipdlp(lp: HighsLp, trace_cap: int = 0, **params) -> dict:
     return _result_dict(res, arrays)
 
 
-def solve_hipdlp_batch(lps, **params) -> list:
-    """b200pdlp_solve_hipdlp_batch: every LP of `lps` (ordered-mode problems under HiPDLP's classification) solved in the
-    HiPDLP mode on one GPU in one call, one CTA per LP.  Takes the parameters of solve_hipdlp (device_prep is ignored) and
-    returns the dicts solve_hipdlp returns, in order; each holds the bits solve_hipdlp returns for that LP alone (the timings
-    and kernel_launches are the batch's)."""
+def _hipdlp_batch(name: str, lps, trace_cap: int, params: dict) -> list:
+    """the call of the host-array HiPDLP batch `name`: the result dicts, in order"""
     lps = list(lps)
-    L = lib()
-    L.b200pdlp_solve_hipdlp_batch.argtypes = [C.c_int32, C.POINTER(CLp), C.POINTER(CHipdlpParams), C.POINTER(CResult)]
-    count = len(lps)
-    clps, cres, keep, arrays = (CLp * max(count, 1))(), (CResult * max(count, 1))(), [], []
-    for i, lp in enumerate(lps):
-        clps[i], k = make_clp(lp)
-        keep.append(k)
-        cres[i], a = _mk_result(lp, 0)
-        arrays.append(a)
-    prm = _hipdlp_params(params)
-    _check(L.b200pdlp_solve_hipdlp_batch(count, clps, C.byref(prm), cres), "b200pdlp_solve_hipdlp_batch")
-    return [_result_dict(cres[i], arrays[i]) for i in range(count)]
-
-
-def solve_hipdlp_batch_mixed(lps, trace_cap: int = 0, **params) -> list:
-    """b200pdlp_solve_hipdlp_batch_mixed: solve_hipdlp_batch for LPs of any size up to max(n, m) = 262144, in any order.
-    Ordered-mode members return what solve_hipdlp_batch returns for them; every other member (a tree member: one
-    thread-block cluster of the GPU per LP) returns what solve_hipdlp returns for it alone, bit for bit, and with
-    trace_cap > 0 its "trace" rows too.  ordered_max=-1 makes every member a tree member."""
-    lps = list(lps)
-    L = lib()
-    L.b200pdlp_solve_hipdlp_batch_mixed.argtypes = [C.c_int32, C.POINTER(CLp), C.POINTER(CHipdlpParams), C.POINTER(CResult)]
+    fn = getattr(lib(), name)
+    fn.argtypes = [C.c_int32, C.POINTER(CLp), C.POINTER(CHipdlpParams), C.POINTER(CResult)]
     count = len(lps)
     clps, cres, keep, arrays = (CLp * max(count, 1))(), (CResult * max(count, 1))(), [], []
     for i, lp in enumerate(lps):
@@ -643,81 +626,18 @@ def solve_hipdlp_batch_mixed(lps, trace_cap: int = 0, **params) -> list:
         cres[i], a = _mk_result(lp, trace_cap)
         arrays.append(a)
     prm = _hipdlp_params(params)
-    _check(L.b200pdlp_solve_hipdlp_batch_mixed(count, clps, C.byref(prm), cres), "b200pdlp_solve_hipdlp_batch_mixed")
+    _check(fn(count, clps, C.byref(prm), cres), name)
     return [_result_dict(cres[i], arrays[i]) for i in range(count)]
 
 
-def solve_hipdlp_batch_device(dlps, **params) -> list:
-    """b200pdlp_solve_hipdlp_batch_device: solve_hipdlp_batch for LPs already in GPU memory (dicts of lp_to_device), prologue
-    and postsolve on the device.  Returns the dicts solve_hipdlp_batch returns, with the four vectors as float64 CUDA tensors;
-    each member's bits are those solve_hipdlp_batch returns for it.  `device` defaults to the device of the first LP's
-    tensors.  torch's current stream is synchronised first, so that inputs it is still writing are complete."""
+def _hipdlp_batch_device(name: str, dlps, trace_cap: int, params: dict) -> list:
+    """the call of the device-array HiPDLP batch `name`: the result dicts, in order, their vectors float64 CUDA tensors"""
     dlps = list(dlps)
-    L = lib()
-    L.b200pdlp_solve_hipdlp_batch_device.argtypes = [C.c_int32, C.POINTER(CLp), C.POINTER(CHipdlpParams), C.POINTER(CResult)]
+    fn = getattr(lib(), name)
+    fn.argtypes = [C.c_int32, C.POINTER(CLp), C.POINTER(CHipdlpParams), C.POINTER(CResult)]
     count = len(dlps)
     if count == 0:
-        _check(L.b200pdlp_solve_hipdlp_batch_device(0, None, C.byref(_hipdlp_params(params)), None),
-               "b200pdlp_solve_hipdlp_batch_device")
-        return []
-    import torch
-    if getattr(dlps[0]["a_start"], "is_cuda", False):
-        params.setdefault("device", dlps[0]["a_start"].device.index)
-    prm = _hipdlp_params(params)
-    clps, cres, arrays = (CLp * count)(), (CResult * count)(), []
-    for i, d in enumerate(dlps):
-        clps[i] = make_clp_device(d)
-    dev = torch.device("cuda", prm.device if prm.device >= 0 else torch.cuda.current_device())
-    for i, d in enumerate(dlps):
-        # at least one element each, so that an LP without rows (or columns) still gets four non-NULL vectors
-        n, m = d["num_col"], d["num_row"]
-        vecs = [torch.empty(max(k, 1), dtype=torch.float64, device=dev) for k in (n, n, m, m)]
-        res = CResult()
-        res.col_value, res.col_dual, res.row_value, res.row_dual = (_dev_ptr(v, torch.float64, _dp, "result") for v in vecs)
-        cres[i] = res
-        arrays.append(tuple(v[:k] for v, k in zip(vecs, (n, n, m, m))))
-    torch.cuda.current_stream(dev).synchronize()
-    _check(L.b200pdlp_solve_hipdlp_batch_device(count, clps, C.byref(prm), cres), "b200pdlp_solve_hipdlp_batch_device")
-    return [_result_dict(cres[i], arrays[i]) for i in range(count)]
-
-
-HIPDLP_BATCH_PREP_ITEMS = ["dims", "cost", "lower", "upper", "rhs", "row_upper", "col_scale", "row_scale", "row_new_idx",
-                           "row_class", "A.slices", "A.col", "A.val", "AT.slices", "AT.col", "AT.val", "norm_cost", "norm_rhs",
-                           "scaled", "orderings", "col_value", "col_dual", "row_value", "row_dual"]
-
-
-def hipdlp_batch_prep_compare(lps, scaling_mode: int = 5, ruiz_iterations: int = 10) -> list:
-    """b200pdlp_debug_hipdlp_batch_prep_compare: the device prologue and postsolve of solve_hipdlp_batch_device against their
-    host twins on host LPs; one dict of mismatch counts per LP (HIPDLP_BATCH_PREP_ITEMS)."""
-    lps = list(lps)
-    L = lib()
-    L.b200pdlp_debug_hipdlp_batch_prep_compare.argtypes = [C.c_int32, C.POINTER(CLp), C.c_int32, C.c_int32, _dp]
-    count = len(lps)
-    clps, keep = (CLp * max(count, 1))(), []
-    for i, lp in enumerate(lps):
-        clps[i], k = make_clp(lp)
-        keep.append(k)
-    k = len(HIPDLP_BATCH_PREP_ITEMS)
-    rep = np.zeros(max(count, 1) * k)
-    _check(L.b200pdlp_debug_hipdlp_batch_prep_compare(count, clps, scaling_mode, ruiz_iterations, _p(rep, _dp)),
-           "b200pdlp_debug_hipdlp_batch_prep_compare")
-    return [dict(zip(HIPDLP_BATCH_PREP_ITEMS, rep[k * i:k * (i + 1)].tolist())) for i in range(count)]
-
-
-def solve_hipdlp_batch_mixed_device(dlps, trace_cap: int = 0, **params) -> list:
-    """b200pdlp_solve_hipdlp_batch_mixed_device: solve_hipdlp_batch_mixed for LPs already in GPU memory (dicts of
-    lp_to_device), every member's prologue and postsolve on the device.  Returns the dicts solve_hipdlp_batch_device returns,
-    with the four vectors as float64 CUDA tensors (and with trace_cap > 0 a host "trace" array); each member's bits are those
-    solve_hipdlp_batch_mixed returns for it.  `device` defaults to the device of the first LP's tensors.  torch's current
-    stream is synchronised first, so that inputs it is still writing are complete."""
-    dlps = list(dlps)
-    L = lib()
-    L.b200pdlp_solve_hipdlp_batch_mixed_device.argtypes = [C.c_int32, C.POINTER(CLp), C.POINTER(CHipdlpParams),
-                                                           C.POINTER(CResult)]
-    count = len(dlps)
-    if count == 0:
-        _check(L.b200pdlp_solve_hipdlp_batch_mixed_device(0, None, C.byref(_hipdlp_params(params)), None),
-               "b200pdlp_solve_hipdlp_batch_mixed_device")
+        _check(fn(0, None, C.byref(_hipdlp_params(params)), None), name)
         return []
     import torch
     if getattr(dlps[0]["a_start"], "is_cuda", False):
@@ -741,8 +661,53 @@ def solve_hipdlp_batch_mixed_device(dlps, trace_cap: int = 0, **params) -> list:
         cres[i] = res
         arrays.append(out)
     torch.cuda.current_stream(dev).synchronize()
-    _check(L.b200pdlp_solve_hipdlp_batch_mixed_device(count, clps, C.byref(prm), cres), "b200pdlp_solve_hipdlp_batch_mixed_device")
+    _check(fn(count, clps, C.byref(prm), cres), name)
     return [_result_dict(cres[i], arrays[i]) for i in range(count)]
+
+
+def solve_hipdlp_batch(lps, **params) -> list:
+    """b200pdlp_solve_hipdlp_batch: every LP of `lps` (ordered-mode problems under HiPDLP's classification) solved in the
+    HiPDLP mode on one GPU in one call, one CTA per LP.  Takes the parameters of solve_hipdlp (device_prep is ignored) and
+    returns the dicts solve_hipdlp returns, in order; each holds the bits solve_hipdlp returns for that LP alone (the timings
+    and kernel_launches are the batch's)."""
+    return _hipdlp_batch("b200pdlp_solve_hipdlp_batch", lps, 0, params)
+
+
+def solve_hipdlp_batch_mixed(lps, trace_cap: int = 0, **params) -> list:
+    """b200pdlp_solve_hipdlp_batch_mixed: solve_hipdlp_batch for LPs of any size up to max(n, m) = 262144, in any order.
+    Ordered-mode members return what solve_hipdlp_batch returns for them; every other member (a tree member: one
+    thread-block cluster of the GPU per LP) returns what solve_hipdlp returns for it alone, bit for bit, and with
+    trace_cap > 0 its "trace" rows too.  ordered_max=-1 makes every member a tree member."""
+    return _hipdlp_batch("b200pdlp_solve_hipdlp_batch_mixed", lps, trace_cap, params)
+
+
+def solve_hipdlp_batch_device(dlps, **params) -> list:
+    """b200pdlp_solve_hipdlp_batch_device: solve_hipdlp_batch for LPs already in GPU memory (dicts of lp_to_device), prologue
+    and postsolve on the device.  Returns the dicts solve_hipdlp_batch returns, with the four vectors as float64 CUDA tensors;
+    each member's bits are those solve_hipdlp_batch returns for it.  `device` defaults to the device of the first LP's
+    tensors.  torch's current stream is synchronised first, so that inputs it is still writing are complete."""
+    return _hipdlp_batch_device("b200pdlp_solve_hipdlp_batch_device", dlps, 0, params)
+
+
+HIPDLP_BATCH_PREP_ITEMS = ["dims", "cost", "lower", "upper", "rhs", "row_upper", "col_scale", "row_scale", "row_new_idx",
+                           "row_class", "A.slices", "A.col", "A.val", "AT.slices", "AT.col", "AT.val", "norm_cost", "norm_rhs",
+                           "scaled", "orderings", "col_value", "col_dual", "row_value", "row_dual"]
+
+
+def hipdlp_batch_prep_compare(lps, scaling_mode: int = 5, ruiz_iterations: int = 10) -> list:
+    """b200pdlp_debug_hipdlp_batch_prep_compare: the device prologue and postsolve of solve_hipdlp_batch_device against their
+    host twins on host LPs; one dict of mismatch counts per LP (HIPDLP_BATCH_PREP_ITEMS)."""
+    return _prep_compare("b200pdlp_debug_hipdlp_batch_prep_compare", HIPDLP_BATCH_PREP_ITEMS, lps, scaling_mode,
+                         ruiz_iterations)
+
+
+def solve_hipdlp_batch_mixed_device(dlps, trace_cap: int = 0, **params) -> list:
+    """b200pdlp_solve_hipdlp_batch_mixed_device: solve_hipdlp_batch_mixed for LPs already in GPU memory (dicts of
+    lp_to_device), every member's prologue and postsolve on the device.  Returns the dicts solve_hipdlp_batch_device returns,
+    with the four vectors as float64 CUDA tensors (and with trace_cap > 0 a host "trace" array); each member's bits are those
+    solve_hipdlp_batch_mixed returns for it.  `device` defaults to the device of the first LP's tensors.  torch's current
+    stream is synchronised first, so that inputs it is still writing are complete."""
+    return _hipdlp_batch_device("b200pdlp_solve_hipdlp_batch_mixed_device", dlps, trace_cap, params)
 
 
 HIPDLP_TREE_PREP_ITEMS = ["dims", "cost", "lower", "upper", "rhs", "row_upper", "col_scale", "row_scale", "rperm", "cperm",
@@ -755,19 +720,8 @@ def hipdlp_tree_prep_compare(lps, scaling_mode: int = 5, ruiz_iterations: int = 
     """b200pdlp_debug_hipdlp_tree_prep_compare: the tree-mode device prologue and postsolve of solve_hipdlp_batch_mixed_device
     against formulate_hipdlp + scale_hipdlp + build_layout(ordered_max=-1) and the host postsolve, on host LPs (every one
     treated as a tree member); one dict of mismatch counts per LP (HIPDLP_TREE_PREP_ITEMS)."""
-    lps = list(lps)
-    L = lib()
-    L.b200pdlp_debug_hipdlp_tree_prep_compare.argtypes = [C.c_int32, C.POINTER(CLp), C.c_int32, C.c_int32, _dp]
-    count = len(lps)
-    clps, keep = (CLp * max(count, 1))(), []
-    for i, lp in enumerate(lps):
-        clps[i], k = make_clp(lp)
-        keep.append(k)
-    k = len(HIPDLP_TREE_PREP_ITEMS)
-    rep = np.zeros(max(count, 1) * k)
-    _check(L.b200pdlp_debug_hipdlp_tree_prep_compare(count, clps, scaling_mode, ruiz_iterations, _p(rep, _dp)),
-           "b200pdlp_debug_hipdlp_tree_prep_compare")
-    return [dict(zip(HIPDLP_TREE_PREP_ITEMS, rep[k * i:k * (i + 1)].tolist())) for i in range(count)]
+    return _prep_compare("b200pdlp_debug_hipdlp_tree_prep_compare", HIPDLP_TREE_PREP_ITEMS, lps, scaling_mode,
+                         ruiz_iterations)
 
 
 def solve_hipdlp_multi(lp: HighsLp, ngpus: int, devices=None, out_arrays=None, **params) -> dict:
