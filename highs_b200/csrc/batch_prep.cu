@@ -12,6 +12,8 @@
 //   hip_batch_prep_kernel   hip_form.cuh hip_form (formulate_hipdlp, the row-major indexes of the form and of the caller's
 //                           matrix, scale_hipdlp, |c|^2 and |b|^2 of the unscaled form), then the sliced-ELL bodies of A and A'
 //   hip_batch_post_kernel   hip_host_postsolve of the returned iterate, into the caller's device vectors
+//   lp_size_kernel          check_lp(deep) and the slack rows of ONE LP of any size, grid-wide: what
+//                           b200pdlp_solve_device / _hipdlp_device need to choose their route (engine.cu device_lp_route)
 //
 // Bits: every value is the host prologue's (host_prep.cpp formulate / build_row_index / scale / build_layout,
 // host_prep_hipdlp.cpp formulate_hipdlp / scale_hipdlp, engine.cu host_start_point / host_postsolve, engine_hipdlp.cu
@@ -94,6 +96,15 @@ struct HipRows {
   }
 };
 
+// check_lp(deep)'s rules, one entry at a time, for every sizing kernel (batch_size per CTA, lp_size_kernel over a grid):
+// a_start[0] == 0, a_start non-decreasing, a_index in [0, num_row).  (The fourth, a_index and a_value present when
+// a_start[num_col] > 0, stays written out in both: as a function it changes batch_size's code.)
+__device__ __forceinline__ bool start_bad(const BatchPrep& P) { return P.a_start[0] != 0; }
+__device__ __forceinline__ bool descent_at(const BatchPrep& P, int j) { return P.a_start[j + 1] < P.a_start[j]; }
+__device__ __forceinline__ bool index_bad(const BatchPrep& P, int p) { return (unsigned)P.a_index[p] >= (unsigned)P.m; }
+// a row of class c has a slack column in the standard form
+__device__ __forceinline__ bool has_slack(int c) { return c == kBound || c == kFreeRow; }
+
 // check_lp(deep), the row classes under Rows, the row order, the standard form's dimensions and the padded lengths of its
 // ordered layouts, for one member.  BOUND and FREE rows are equality-like, each with a slack column (PdlpRows makes no FREE
 // rows).
@@ -105,10 +116,9 @@ __device__ __forceinline__ void batch_size(const BatchPrep& P, BatchSize& S) {
   const int t = threadIdx.x, n0 = P.n0, m = P.m;
   if (t < 4) flag[t] = 0;
   __syncthreads();
-  // check_lp(deep): a_start[0] == 0, a_start non-decreasing, the matrix arrays present, a_index in [0, num_row)
-  if (t == 0 && P.a_start[0] != 0) flag[0] = kPrepStart0;
+  if (t == 0 && start_bad(P)) flag[0] = kPrepStart0;
   for (int j = t; j < n0; j += kThreads)
-    if (P.a_start[j + 1] < P.a_start[j]) flag[1] = kPrepDecreasing;
+    if (descent_at(P, j)) flag[1] = kPrepDecreasing;
   __syncthreads();
   const int nnz0 = P.a_start[n0];
   if (t == 0 && nnz0 > 0 && (!P.a_index || !P.a_value)) flag[2] = kPrepNull;
@@ -119,7 +129,7 @@ __device__ __forceinline__ void batch_size(const BatchPrep& P, BatchSize& S) {
     return;
   }
   for (int p = t; p < nnz0; p += kThreads)
-    if ((unsigned)P.a_index[p] >= (unsigned)m) flag[3] = kPrepIndex;
+    if (index_bad(P, p)) flag[3] = kPrepIndex;
   __syncthreads();
   if (flag[3]) {
     if (t == 0) S.err = kPrepIndex;
@@ -139,7 +149,7 @@ __device__ __forceinline__ void batch_size(const BatchPrep& P, BatchSize& S) {
   for (int i = b; i < e; i++) {
     const int c = P.row_class[i];
     eq += (c == kEq || c == kBound || c == kFreeRow);
-    bnd += (c == kBound || c == kFreeRow);
+    bnd += has_slack(c);
   }
   sm_eq[t] = eq; sm_bnd[t] = bnd;
   __syncthreads();
@@ -184,6 +194,39 @@ __global__ void __launch_bounds__(kThreads) batch_size_kernel(const BatchPrep* _
 
 __global__ void __launch_bounds__(kThreads) hip_batch_size_kernel(const BatchPrep* __restrict__ prep, BatchSize* __restrict__ sizes) {
   batch_size<HipRows>(prep[blockIdx.x], sizes[blockIdx.x]);
+}
+
+// check_lp(deep) and the slack rows under Rows of one LP of any size, grid-stride, in two passes over one record zeroed by
+// the host.  Pass 0: a_start (a_start[0] == 0 and a_start[num_col] >= 0, no descent), the matrix arrays present, the slack
+// rows.  Pass 1, the next launch on the stream: a_index in [0, num_row), only when pass 0 found nothing -- as check_lp, which
+// reads a_index only once a_start has passed, so a malformed a_start never sends the sweep past a_index's end.  Every warp
+// ORs its broken rules and adds its slack rows with one atomic each.
+template <class Rows>
+__global__ void __launch_bounds__(kThreads) lp_size_kernel(const BatchPrep P, int index_pass, LpSize* __restrict__ out) {
+  const long long stride = (long long)gridDim.x * kThreads, t = (long long)blockIdx.x * kThreads + threadIdx.x;
+  const int n0 = P.n0, m = P.m, nnz0 = P.a_start[n0];
+  unsigned bits = 0;
+  int slack = 0;
+  if (index_pass) {
+    if (out->err_bits) return;
+    for (long long p = t; p < nnz0; p += stride)
+      if (index_bad(P, (int)p)) bits |= 1u << kPrepIndex;
+  } else {
+    if (t == 0) {
+      if (start_bad(P) || nnz0 < 0) bits |= 1u << kPrepStart0;
+      if (nnz0 > 0 && (!P.a_index || !P.a_value)) bits |= 1u << kPrepNull;
+      out->nnz = nnz0;
+    }
+    for (long long j = t; j < n0; j += stride)
+      if (descent_at(P, (int)j)) bits |= 1u << kPrepDecreasing;
+    for (long long i = t; i < m; i += stride) slack += has_slack(Rows::row_class(P.row_lower[i], P.row_upper[i]));
+  }
+  bits = __reduce_or_sync(0xffffffffu, bits);
+  slack = __reduce_add_sync(0xffffffffu, slack);
+  if ((threadIdx.x & 31) == 0) {
+    if (bits) atomicOr(&out->err_bits, bits);
+    if (slack) atomicAdd(&out->nslack, slack);
+  }
 }
 
 // one ordered sliced-ELL body: rows r < rows, 32 a slice, entry k of row r at ptr + 32 k + (r & 31); padding (0, 0), and 32
@@ -494,6 +537,12 @@ void launch_hip_batch_post(cudaStream_t s, int count, const BatchPrep* prep, con
 
 void launch_batch_size(cudaStream_t s, int count, const BatchPrep* prep, BatchSize* sizes) {
   if (count > 0) batch_size_kernel<<<count, kThreads, 0, s>>>(prep, sizes);
+}
+void launch_lp_size(cudaStream_t s, const BatchPrep& lp, bool hip, LpSize* out) {
+  for (int pass = 0; pass < 2; pass++) {
+    if (hip) lp_size_kernel<HipRows><<<kLpSizeBlocks, kThreads, 0, s>>>(lp, pass, out);
+    else lp_size_kernel<PdlpRows><<<kLpSizeBlocks, kThreads, 0, s>>>(lp, pass, out);
+  }
 }
 void launch_batch_prep(cudaStream_t s, int count, const BatchPrep* prep, int do_scale) {
   if (count > 0) batch_prep_kernel<<<count, kThreads, 0, s>>>(prep, do_scale);

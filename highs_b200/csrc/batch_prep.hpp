@@ -49,7 +49,17 @@ struct BatchPost {
   int have_check;   // 0: no check ran (iter_limit <= 0): the slacks are zero
 };
 
+// What lp_size_kernel reads back for one LP of b200pdlp_solve_device / _hipdlp_device (only lp's LP fields are read)
+struct LpSize {
+  unsigned err_bits;   // 1 << BatchPrepErr for every rule the LP breaks (0: well-formed, and the fields below are valid)
+  int nslack;          // rows with a slack column under the mode's classification (BOUND rows; HiPDLP: BOUND and FREE)
+  int nnz;             // a_start[num_col]
+  int pad;
+};
+constexpr int kLpSizeBlocks = 1024;   // lp_size_kernel's grid: about one resident wave of kThreads-thread CTAs on an H100
+
 void launch_batch_size(cudaStream_t s, int count, const BatchPrep* prep, BatchSize* sizes);
+void launch_lp_size(cudaStream_t s, const BatchPrep& lp, bool hip, LpSize* out);   // both passes; out: zeroed by the caller
 void launch_batch_prep(cudaStream_t s, int count, const BatchPrep* prep, int do_scale);
 void launch_batch_post(cudaStream_t s, int count, const BatchPrep* prep, const BatchPost* post);
 

@@ -639,16 +639,12 @@ void DevicePrologue::run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, i
   const bool hip = hipdlp;
   Tmp tmp;
   tmp.stream = s;
-  const int n0 = lp.num_col, m = lp.num_row, nnz0 = lp.a_start[n0];
-  // ---- the caller's arrays -> HBM (pinned sources stream at PCIe speed; pageable ones are staged by the driver)
-  int* a_start = tmp.get<int>(n0 + 1);
-  int* a_index = tmp.get<int>(nnz0);
-  double* a_value = tmp.get<double>(nnz0);
-  double* cc = tmp.get<double>(n0);
-  double* cl = tmp.get<double>(n0);
-  double* cu = tmp.get<double>(n0);
-  double* rl = tmp.get<double>(m);
-  double* ru = tmp.get<double>(m);
+  const int n0 = lp.num_col, m = lp.num_row, nnz0 = inputs_on_device ? device_nnz : lp.a_start[n0];
+  // ---- the caller's arrays in HBM: where they are, or copied there (pinned sources stream at PCIe speed; pageable ones are
+  // staged by the driver)
+  const int *a_start = lp.a_start, *a_index = lp.a_index;
+  const double *a_value = lp.a_value, *cc = lp.col_cost, *cl = lp.col_lower, *cu = lp.col_upper, *rl = lp.row_lower,
+               *ru = lp.row_upper;
   // Two copy streams: the STRUCTURE (column starts, row indices, row bounds: 4 n + 4 nnz + 16 m bytes) goes first on `s`; the
   // VALUES (coefficients, cost, column bounds: 8 nnz + 24 n bytes, two thirds of the traffic) follow on a second stream, and
   // everything that depends on the sparsity pattern alone -- classification, the stable partition, the row-major index
@@ -669,16 +665,30 @@ void DevicePrologue::run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, i
       for (cudaEvent_t e : {structure_up, values_up, norms_in, norms_t0, norms_t1}) if (e) cudaEventDestroy(e);
     }
   } side;
-  auto up = [&](cudaStream_t q, void* d, const void* h, size_t bytes) { if (bytes) PREP_OK(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, q)); };
-  up(s, a_start, lp.a_start, (size_t)(n0 + 1) * 4);
-  up(s, a_index, lp.a_index, (size_t)nnz0 * 4);
-  up(s, rl, lp.row_lower, (size_t)m * 8); up(s, ru, lp.row_upper, (size_t)m * 8);
-  PREP_OK(cudaEventRecord(side.structure_up, s));
-  PREP_OK(cudaStreamWaitEvent(side.st, side.structure_up, 0));   // the structure first: the copy engine is shared
-  up(side.st, a_value, lp.a_value, (size_t)nnz0 * 8);
-  up(side.st, cc, lp.col_cost, (size_t)n0 * 8); up(side.st, cl, lp.col_lower, (size_t)n0 * 8); up(side.st, cu, lp.col_upper, (size_t)n0 * 8);
-  PREP_OK(cudaEventRecord(side.values_up, side.st));
-  h2d_bytes = (size_t)(n0 + 1) * 4 + (size_t)nnz0 * 12 + (size_t)n0 * 24 + (size_t)m * 16;
+  if (inputs_on_device) {
+    PREP_OK(cudaEventRecord(side.values_up, s));   // (the values are there already)
+    h2d_bytes = 0;
+  } else {
+    int* d_start = tmp.get<int>(n0 + 1);
+    int* d_index = tmp.get<int>(nnz0);
+    double* d_value = tmp.get<double>(nnz0);
+    double* d_cc = tmp.get<double>(n0);
+    double* d_cl = tmp.get<double>(n0);
+    double* d_cu = tmp.get<double>(n0);
+    double* d_rl = tmp.get<double>(m);
+    double* d_ru = tmp.get<double>(m);
+    auto up = [&](cudaStream_t q, void* d, const void* h, size_t bytes) { if (bytes) PREP_OK(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, q)); };
+    up(s, d_start, lp.a_start, (size_t)(n0 + 1) * 4);
+    up(s, d_index, lp.a_index, (size_t)nnz0 * 4);
+    up(s, d_rl, lp.row_lower, (size_t)m * 8); up(s, d_ru, lp.row_upper, (size_t)m * 8);
+    PREP_OK(cudaEventRecord(side.structure_up, s));
+    PREP_OK(cudaStreamWaitEvent(side.st, side.structure_up, 0));   // the structure first: the copy engine is shared
+    up(side.st, d_value, lp.a_value, (size_t)nnz0 * 8);
+    up(side.st, d_cc, lp.col_cost, (size_t)n0 * 8); up(side.st, d_cl, lp.col_lower, (size_t)n0 * 8); up(side.st, d_cu, lp.col_upper, (size_t)n0 * 8);
+    PREP_OK(cudaEventRecord(side.values_up, side.st));
+    h2d_bytes = (size_t)(n0 + 1) * 4 + (size_t)nnz0 * 12 + (size_t)n0 * 24 + (size_t)m * 16;
+    a_start = d_start; a_index = d_index; a_value = d_value; cc = d_cc; cl = d_cl; cu = d_cu; rl = d_rl; ru = d_ru;
+  }
 
   // ---- classification, row order
   int* cls = arr.row_class = keep<int>(m);

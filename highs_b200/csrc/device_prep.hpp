@@ -4,7 +4,7 @@
 // (/root/reference/highs/pdlp/CupdlpWrapper.cpp:280-448), Init_Scaling + PDHG_Scale_Data
 // (highs/pdlp/cupdlp/cupdlp_scaling.c:233-425), csc2csr (cupdlp_utils.c:1222-1254) -- and what host_prep.cpp does for
 // the engine on host threads (its tested twin: same arithmetic, same orders), here as kernels over the caller's
-// HighsLp arrays copied once to HBM.  The host touches O(1) data: three small read-backs (sizes of the standard form,
+// HighsLp arrays, copied once to HBM or (inputs_on_device) read where they are.  The host touches O(1) data: three small read-backs (sizes of the standard form,
 // sizes of the layouts + scalars, long-row totals; block mode adds the partition's 2 (world + 1) offsets).  Scans, stable radix sorts and the stream compaction come from CUB
 // (part of the CUDA toolkit); everything that computes is a kernel of device_prep.cu / setup_kernels.cu.
 #pragma once
@@ -113,7 +113,12 @@ struct DevicePrologue {
   std::vector<int> ranks;
   std::vector<int> rb, cb;                        // world + 1 block offsets each (read back)
   std::vector<DevSellOwned> block_A, block_AT;
-  size_t h2d_bytes = 0;
+  // The caller's eight LP arrays are device memory of this device (b200pdlp_solve_device, _hipdlp_device): the kernels read
+  // them in place, with no staging copy and nothing on the side stream but the HiPDLP norms; h2d_bytes stays 0.  The host
+  // cannot read a_start[num_col] then: device_nnz holds it.  Every kernel of the prologue only reads these arrays.
+  bool inputs_on_device = false;
+  int device_nnz = 0;
+  size_t h2d_bytes = 0;   // bytes of the caller's arrays copied to the device
   // formulate + scale + row index + orderings + sliced-ELL layouts, all on stream `s`; returns with the stream idle.
   // Throws std::exception on bad input / CUDA errors (the caller releases what was produced so far).
   void run(cudaStream_t s, const b200pdlp_lp& lp, bool do_scale, int long_threshold);

@@ -273,6 +273,108 @@ bool device_prep_fits(const b200pdlp_lp& lp, int ordered_max, double inf) {
   return lp.num_col > 0 && lp.num_row > 0 && lp.a_start[lp.num_col] > 0;
 }
 
+// ---- LPs whose arrays are device memory (the device-array batches and single solves)
+// check_lp's message for a BatchPrepErr of a sizing kernel
+const char* prep_error_text(int err) {
+  switch (err) {
+    case kPrepStart0: return "b200pdlp: a_start[0] must be 0 and a_start[num_col] >= 0";
+    case kPrepDecreasing: return "b200pdlp: a_start must be non-decreasing";
+    case kPrepIndex: return "b200pdlp: a_index entry outside [0, num_row)";
+    default: return "b200pdlp: malformed b200pdlp_lp";
+  }
+}
+
+// ptr (NULL: not given) must be device or managed memory of `device`; i >= 0: the array belongs to member i of a batch
+void check_device_array(const void* ptr, int device, int i, const char* field, const char* who) {
+  if (!ptr) return;
+  cudaPointerAttributes a{};
+  const cudaError_t e = cudaPointerGetAttributes(&a, ptr);
+  if (e != cudaSuccess) cudaGetLastError();
+  if (e != cudaSuccess || !((a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == device))
+    throw Error(B200PDLP_ERR_ARG, std::string(who) + (i >= 0 ? ": member " + std::to_string(i) : std::string()) + ": " +
+                                      field + " is not device memory of device " + std::to_string(device));
+}
+
+// the arrays of an LP, in this order
+void check_device_lp(const b200pdlp_lp& lp, int device, int i, const char* who) {
+  check_device_array(lp.a_start, device, i, "a_start", who);
+  check_device_array(lp.a_index, device, i, "a_index", who);
+  check_device_array(lp.a_value, device, i, "a_value", who);
+  check_device_array(lp.col_cost, device, i, "col_cost", who);
+  check_device_array(lp.col_lower, device, i, "col_lower", who);
+  check_device_array(lp.col_upper, device, i, "col_upper", who);
+  check_device_array(lp.row_lower, device, i, "row_lower", who);
+  check_device_array(lp.row_upper, device, i, "row_upper", who);
+}
+
+// the four vectors of a result, in this order
+void check_device_result(const b200pdlp_result& out, int device, int i, const char* who) {
+  check_device_array(out.col_value, device, i, "result col_value", who);
+  check_device_array(out.col_dual, device, i, "result col_dual", who);
+  check_device_array(out.row_value, device, i, "result row_value", who);
+  check_device_array(out.row_dual, device, i, "result row_dual", who);
+}
+
+// The route of a single solve on device arrays, from the grid-wide sizing kernel's two passes on stream s (batch_prep.cu
+// lp_size_kernel: check_lp(deep) and the slack rows under the mode's classification) and one read-back of its record: Ordered when the
+// standard form is within ordered_max (device_prep_fits' rule), else Tree when it has rows, columns and nonzeros, else
+// Degenerate.  A malformed LP is ERR_ARG with check_lp's message, in check_lp's order.  *nnz = a_start[num_col].
+DeviceRoute device_lp_route(cudaStream_t s, const b200pdlp_lp& lp, bool hipdlp, int ordered_max, const char* who, int* nnz) {
+  BatchPrep P{};
+  P.n0 = lp.num_col; P.m = lp.num_row; P.sense = lp.sense;
+  P.a_start = lp.a_start; P.a_index = lp.a_index; P.a_value = lp.a_value;
+  P.col_cost = lp.col_cost; P.col_lower = lp.col_lower; P.col_upper = lp.col_upper;
+  P.row_lower = lp.row_lower; P.row_upper = lp.row_upper;
+  DevBuf<LpSize> d;
+  d.alloc(1, false);
+  PinnedArray<LpSize> z(1);
+  CUDA_OK(cudaMemsetAsync(d.p, 0, sizeof(LpSize), s));
+  launch_lp_size(s, P, hipdlp, d.p);
+  CUDA_OK(cudaGetLastError());
+  CUDA_OK(cudaMemcpyAsync(z.p, d.p, sizeof(LpSize), cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaStreamSynchronize(s));
+  for (int e : {kPrepNull, kPrepStart0, kPrepDecreasing, kPrepIndex})
+    if (z.p->err_bits & (1u << e)) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": " + prep_error_text(e));
+  *nnz = z.p->nnz;
+  const int omax = ordered_max == 0 ? 4096 : ordered_max;
+  if (omax > 0 && std::max<long long>((long long)lp.num_col + z.p->nslack, lp.num_row) <= omax) return DeviceRoute::Ordered;
+  return lp.num_col > 0 && lp.num_row > 0 && z.p->nnz > 0 ? DeviceRoute::Tree : DeviceRoute::Degenerate;
+}
+
+// A degenerate LP of a single device-array solve (no rows, no columns or no nonzeros: well-formed, it has no matrix) takes
+// the host prologue, as in the host-array solve: its vectors (and hot start) come down, solve() runs on host copies, and the
+// four result vectors go back up into the caller's device vectors (those given) on stream s.
+void solve_degenerate(cudaStream_t s, const b200pdlp_lp& lp, const b200pdlp_warm* warm, b200pdlp_result* out,
+                      const HostSolve& solve) {
+  const int n0 = lp.num_col, m = lp.num_row;
+  std::vector<int> start((size_t)n0 + 1);
+  std::vector<std::vector<double>> h(12);
+  auto down = [&](int k, const double* d, int len) {
+    h[k].assign((size_t)std::max(len, 1), 0.0);
+    if (d && len > 0) CUDA_OK(cudaMemcpyAsync(h[k].data(), d, (size_t)len * sizeof(double), cudaMemcpyDeviceToHost, s));
+    return h[k].data();
+  };
+  CUDA_OK(cudaMemcpyAsync(start.data(), lp.a_start, start.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+  b200pdlp_lp hl = lp;
+  hl.a_start = start.data(); hl.a_index = nullptr; hl.a_value = nullptr;
+  hl.col_cost = down(0, lp.col_cost, n0); hl.col_lower = down(1, lp.col_lower, n0); hl.col_upper = down(2, lp.col_upper, n0);
+  hl.row_lower = down(3, lp.row_lower, m); hl.row_upper = down(4, lp.row_upper, m);
+  b200pdlp_warm hw{};
+  const bool hot = warm && warm->col_value && warm->row_value && warm->row_dual;
+  if (hot) { hw.col_value = down(5, warm->col_value, n0); hw.row_value = down(6, warm->row_value, m); hw.row_dual = down(7, warm->row_dual, m); }
+  CUDA_OK(cudaStreamSynchronize(s));
+  b200pdlp_result r = *out;
+  r.col_value = down(8, nullptr, n0); r.col_dual = down(9, nullptr, n0); r.row_value = down(10, nullptr, m); r.row_dual = down(11, nullptr, m);
+  solve(hl, hot ? &hw : nullptr, &r);
+  auto up = [&](double* d, const double* v, int len) {
+    if (d && len > 0) CUDA_OK(cudaMemcpyAsync(d, v, (size_t)len * sizeof(double), cudaMemcpyHostToDevice, s));
+  };
+  up(out->col_value, r.col_value, n0); up(out->col_dual, r.col_dual, n0); up(out->row_value, r.row_value, m); up(out->row_dual, r.row_dual, m);
+  CUDA_OK(cudaStreamSynchronize(s));
+  r.col_value = out->col_value; r.col_dual = out->col_dual; r.row_value = out->row_value; r.row_dual = out->row_dual;
+  *out = r;
+}
+
 // Several GPUs (default; B200PDLP_MG_DEVICE_PREP=0 for the host path): every rank needs the whole scaled standard form to cut its shard out of
 // it.  Instead of G processes running the host prologue side by side (they share the host's cores and memory bandwidth),
 // each rank formulates and scales on ITS GPU (a few milliseconds, identical bits on every rank) and downloads the result;
@@ -382,9 +484,9 @@ void adopt_matrix(DeviceMatrix& M, DevSellOwned& O) {
   O = DevSellOwned();   // ownership moved
 }
 
+// p: opened on its device (open_problem)
 static void create_problem_device(const b200pdlp_lp& lp, const b200pdlp_params& prm, b200pdlp_problem* p) {
   NvtxRange nvtx("b200pdlp: prologue (device)");
-  open_problem(p, prm.device, 0, 1);
   Laps lap;
   ensure_side_stream(p);
   p->dev_form = true;
@@ -392,9 +494,11 @@ static void create_problem_device(const b200pdlp_lp& lp, const b200pdlp_params& 
   DevicePrologue& P = p->prep;
   run_prologue(P, p->stream, lp, prm.scaling != 0);
   lap("setup", "device prologue");
-  if (lap.on)
+  if (lap.on) {
     fprintf(stderr, "[b200pdlp setup] sectors per gathered lane (sampled): A %.3f  A' %.3f\n",
             P.sc.a_lanes ? (double)P.sc.a_sectors / P.sc.a_lanes : 0.0, P.sc.at_lanes ? (double)P.sc.at_sectors / P.sc.at_lanes : 0.0);
+    fprintf(stderr, "[b200pdlp setup] LP arrays copied to the device: %zu bytes\n", P.h2d_bytes);
+  }
   take_prologue(lp, P, p);
   p->beta_cost_sq = P.sc.beta_cost_sq; p->beta_rhs_sq = P.sc.beta_rhs_sq;
   const int n = p->n, m = p->m;
@@ -406,7 +510,7 @@ static void create_problem_device(const b200pdlp_lp& lp, const b200pdlp_params& 
   p->xsum.alloc(n, false); p->xavg.alloc(n, false); p->atyavg.alloc(n, false); p->xlr.alloc(n, false);
   p->ysum.alloc(m, false); p->yavg.alloc(m, false); p->axavg.alloc(m, false); p->ylr.alloc(m, false);
   p->axsum.alloc(m, false); p->atysum.alloc(n, false);
-  alloc_postsolve_staging(p);
+  if (!p->device_io) alloc_postsolve_staging(p);
   alloc_scratch(p, false);
   p->state.alloc(1, false);
   p->redbuf.alloc(16, false);
@@ -1242,7 +1346,9 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
   if (dev_form) {
     // maps and scales live in HBM: the hot start goes up in original order and is permuted / scaled / projected there
     const double *wc = nullptr, *wv = nullptr, *wd = nullptr;
-    if (warm && warm->col_value && warm->row_value && warm->row_dual) {
+    if (warm && warm->col_value && warm->row_value && warm->row_dual && p->device_io) {
+      wc = warm->col_value; wv = warm->row_value; wd = warm->row_dual;
+    } else if (warm && warm->col_value && warm->row_value && warm->row_dual) {
       CUDA_OK(cudaMemcpyAsync(p->io_col.p, warm->col_value, (size_t)f.n_orig * sizeof(double), cudaMemcpyHostToDevice, s));
       CUDA_OK(cudaMemcpyAsync(p->io_row.p, warm->row_value, (size_t)m * sizeof(double), cudaMemcpyHostToDevice, s));
       CUDA_OK(cudaMemcpyAsync(p->io_row.p + m, warm->row_dual, (size_t)m * sizeof(double), cudaMemcpyHostToDevice, s));
@@ -1547,7 +1653,11 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
   if (dev_form) {
     // PDHG_PostSolve on the device (device_prep.cu post_*_kernel): un-permute, un-scale, sign conventions, slacks of
     // BOUND rows; four original-order vectors come back
-    if (out->col_value && out->col_dual && out->row_value && out->row_dual) {
+    if (out->col_value && out->col_dual && out->row_value && out->row_dual && p->device_io) {
+      launch_postsolve(s, p->prep.arr, f.sense, have_check ? 1 : 0, dx, daty, dy, dax, p->cost.p, p->lower.p, p->upper.p,
+                       p->colscale.p, p->rowscale.p, out->col_value, out->col_dual, out->row_value, out->row_dual);
+      p->launches += 2;
+    } else if (out->col_value && out->col_dual && out->row_value && out->row_dual) {
       const int n0 = f.n_orig;
       launch_postsolve(s, p->prep.arr, f.sense, have_check ? 1 : 0, dx, daty, dy, dax, p->cost.p, p->lower.p, p->upper.p,
                        p->colscale.p, p->rowscale.p, p->io_col.p, p->io_col.p + n0, p->io_row.p, p->io_row.p + m);
@@ -1780,7 +1890,7 @@ int b200pdlp_problem_create(const b200pdlp_lp* lp, const b200pdlp_params* params
     auto* p = new b200pdlp_problem();
     try {
       p->prep.keep_form = true;   // persistent handle: the accessors below may ask for the standard form
-      if (use_device_prep(*lp, *params, world)) create_problem_device(*lp, *params, p);
+      if (use_device_prep(*lp, *params, world)) { open_problem(p, params->device, 0, 1); create_problem_device(*lp, *params, p); }
       else create_problem(*lp, *params, rank, world, p);
     } catch (...) { delete p; throw; }
     *out = p;
@@ -2243,7 +2353,7 @@ int b200pdlp_solve(const b200pdlp_lp* lp, const b200pdlp_params* params, const b
     check_lp(lp, !use_device_prep(*lp, *params, 1));
     const auto t0 = std::chrono::steady_clock::now();
     ProblemPtr p(new b200pdlp_problem());
-    if (use_device_prep(*lp, *params, 1)) create_problem_device(*lp, *params, p.get());
+    if (use_device_prep(*lp, *params, 1)) { open_problem(p.get(), params->device, 0, 1); create_problem_device(*lp, *params, p.get()); }
     else create_problem(*lp, *params, 0, 1, p.get());
     out->setup_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
     solve_on_device(p.get(), *params, warm, out);
@@ -2251,6 +2361,50 @@ int b200pdlp_solve(const b200pdlp_lp* lp, const b200pdlp_params* params, const b
     Laps lap;
     p.reset();
     lap("solve", "teardown");
+  });
+}
+
+int b200pdlp_solve_device(const b200pdlp_lp* lp, const b200pdlp_params* params, const b200pdlp_warm* warm, b200pdlp_result* out) {
+  DeviceGuard dg;
+  const char* who = "b200pdlp_solve_device";
+  return guarded([&] {
+    if (!lp || !params || !out) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": null argument");
+    check_params(*params);
+    if (!lp_fields_ok(lp)) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": b200pdlp: malformed b200pdlp_lp");
+    if (lp->sense != 1.0 && lp->sense != -1.0) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": b200pdlp: sense must be +1 or -1");
+    const int device = select_device(params->device);
+    check_device_lp(*lp, device, -1, who);
+    if (warm) {
+      check_device_array(warm->col_value, device, -1, "warm col_value", who);
+      check_device_array(warm->row_value, device, -1, "warm row_value", who);
+      check_device_array(warm->row_dual, device, -1, "warm row_dual", who);
+    }
+    check_device_result(*out, device, -1, who);
+    const auto t0 = std::chrono::steady_clock::now();
+    b200pdlp_params prm = *params;
+    prm.device = device;
+    ProblemPtr p(new b200pdlp_problem());   // its stream serves the sizing and, in tree mode, the solve
+    open_problem(p.get(), device, 0, 1);
+    int nnz = 0;
+    const DeviceRoute route = device_lp_route(p->stream, *lp, false, prm.ordered_max, who, &nnz);
+    if (route == DeviceRoute::Ordered) {
+      solve_batch_device(1, lp, prm, warm, out);
+    } else if (route == DeviceRoute::Degenerate) {
+      solve_degenerate(p->stream, *lp, warm, out, [&](const b200pdlp_lp& hl, const b200pdlp_warm* hw, b200pdlp_result* r) {
+        ProblemPtr q(new b200pdlp_problem());
+        create_problem(hl, prm, 0, 1, q.get());
+        r->setup_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+        solve_on_device(q.get(), prm, hw, r);
+      });
+    } else {
+      p->device_io = true;
+      p->prep.inputs_on_device = true;
+      p->prep.device_nnz = nnz;
+      create_problem_device(*lp, prm, p.get());
+      out->setup_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+      solve_on_device(p.get(), prm, warm, out);
+    }
+    CUDA_OK(cudaGetLastError());
   });
 }
 

@@ -19,6 +19,7 @@
 #include <mutex>
 #include <stdexcept>
 #include <string>
+#include <functional>
 #include <thread>
 #include <vector>
 
@@ -274,6 +275,9 @@ struct b200pdlp_problem {
   DevicePrologue prep;
   double beta_cost_sq = 0.0, beta_rhs_sq = 0.0;   // |c|^2, |b|^2 of the scaled data (tree sums)
   DevBuf<double> io_col, io_row;   // staging of the hot start / the returned solution (original order)
+  // b200pdlp_solve_device / _hipdlp_device: the LP's arrays, the hot start and the result vectors are device memory; the
+  // prologue reads the LP in place, the solve reads the hot start and the postsolve writes the results there (no io_col / io_row)
+  bool device_io = false;
   DevBuf<SolveCtl> ctl;
   SolveCtl* hctl = nullptr;        // pinned
   int* htime = nullptr;            // pinned + mapped
@@ -493,6 +497,25 @@ void alloc_peer_words(b200pdlp_problem* p);
 void alloc_postsolve_staging(b200pdlp_problem* p);
 int std_form_cols(const b200pdlp_lp& lp, double inf);
 bool device_prep_fits(const b200pdlp_lp& lp, int ordered_max, double inf);
+
+// engine.cu: what the entry points on device arrays share (the batches of engine_batch.cu, the single solves)
+const char* prep_error_text(int err);
+void check_device_array(const void* ptr, int device, int i, const char* field, const char* who);
+void check_device_lp(const b200pdlp_lp& lp, int device, int i, const char* who);
+void check_device_result(const b200pdlp_result& out, int device, int i, const char* who);
+// the single solves on device arrays (b200pdlp_solve_device, b200pdlp_solve_hipdlp_device)
+enum class DeviceRoute { Ordered, Tree, Degenerate };
+DeviceRoute device_lp_route(cudaStream_t s, const b200pdlp_lp& lp, bool hipdlp, int ordered_max, const char* who, int* nnz);
+using HostSolve = std::function<void(const b200pdlp_lp&, const b200pdlp_warm*, b200pdlp_result*)>;
+void solve_degenerate(cudaStream_t s, const b200pdlp_lp& lp, const b200pdlp_warm* warm, b200pdlp_result* out,
+                      const HostSolve& solve);
+
+// engine_batch.cu: the device-array batches, which the single device-array solves take for ordered-mode LPs
+int select_device(int device);
+void solve_batch_device(int count, const b200pdlp_lp* lps, const b200pdlp_params& prm, const b200pdlp_warm* warms,
+                        b200pdlp_result* outs);
+void solve_hipdlp_batch_device(int count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params& prm, b200pdlp_result* outs,
+                               bool mixed);
 void adopt_matrix(DeviceMatrix& M, DevSellOwned& O);
 void apply_spmv_grid(b200pdlp_problem* p);
 void ensure_host_maps(b200pdlp_problem* p);

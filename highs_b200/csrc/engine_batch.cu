@@ -11,7 +11,7 @@ namespace b200 {
 // bits b200pdlp_solve returns for it alone.
 
 // every batch runs on `device` (< 0: the current device); returns its number
-static int select_device(int device) {
+int select_device(int device) {
   device_count_checked();
   if (device >= 0) CUDA_OK(cudaSetDevice(device));
   int current = 0;
@@ -420,29 +420,6 @@ static void check_batch_device_member(const b200pdlp_lp* lp, int ordered_max, in
   if (rc != B200PDLP_OK) throw Error(rc, std::string(who) + ": member " + std::to_string(i) + ": " + g_last_error);
 }
 
-// ptr (NULL: not given) must be device or managed memory of `device`
-static void check_device_array(const void* ptr, int device, int i, const char* field, const char* who) {
-  if (!ptr) return;
-  cudaPointerAttributes a{};
-  const cudaError_t e = cudaPointerGetAttributes(&a, ptr);
-  if (e != cudaSuccess) cudaGetLastError();
-  if (e != cudaSuccess || !((a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == device))
-    throw Error(B200PDLP_ERR_ARG, std::string(who) + ": member " + std::to_string(i) + ": " + field +
-                                      " is not device memory of device " + std::to_string(device));
-}
-
-// the arrays of member i's LP, in this order
-static void check_device_lp(const b200pdlp_lp& lp, int device, int i, const char* who) {
-  check_device_array(lp.a_start, device, i, "a_start", who);
-  check_device_array(lp.a_index, device, i, "a_index", who);
-  check_device_array(lp.a_value, device, i, "a_value", who);
-  check_device_array(lp.col_cost, device, i, "col_cost", who);
-  check_device_array(lp.col_lower, device, i, "col_lower", who);
-  check_device_array(lp.col_upper, device, i, "col_upper", who);
-  check_device_array(lp.row_lower, device, i, "row_lower", who);
-  check_device_array(lp.row_upper, device, i, "row_upper", who);
-}
-
 // every array pointer of the batch (warms: NULL for none) must be device memory of `device`: the lowest failing member, field
 static void check_device_arrays(int count, const b200pdlp_lp* lps, const b200pdlp_warm* warms, const b200pdlp_result* outs,
                                 int device, const char* who) {
@@ -453,10 +430,7 @@ static void check_device_arrays(int count, const b200pdlp_lp* lps, const b200pdl
       check_device_array(warms[i].row_value, device, i, "warm row_value", who);
       check_device_array(warms[i].row_dual, device, i, "warm row_dual", who);
     }
-    check_device_array(outs[i].col_value, device, i, "result col_value", who);
-    check_device_array(outs[i].col_dual, device, i, "result col_dual", who);
-    check_device_array(outs[i].row_value, device, i, "result row_value", who);
-    check_device_array(outs[i].row_dual, device, i, "result row_dual", who);
+    check_device_result(outs[i], device, i, who);
   }
 }
 
@@ -482,15 +456,6 @@ struct PrepMode {
   int scaling = 0;           // PDLP: b200pdlp_params::scaling; HiPDLP: scaling_mode
   int ruiz_iterations = 0;   // HiPDLP only
 };
-
-static const char* prep_error_text(int err) {
-  switch (err) {
-    case kPrepStart0: return "b200pdlp: a_start[0] must be 0 and a_start[num_col] >= 0";
-    case kPrepDecreasing: return "b200pdlp: a_start must be non-decreasing";
-    case kPrepIndex: return "b200pdlp: a_index entry outside [0, num_row)";
-    default: return "b200pdlp: malformed b200pdlp_lp";
-  }
-}
 
 // The members' descriptors and the sizing kernel (the array checks, the row classes and orders, the form's dimensions):
 // one read-back of `count` records into D.size, on stream s of the current device.  lps[i] / warms[i]: host structs whose
@@ -613,7 +578,7 @@ static void device_batch_prologue(cudaStream_t s, int count, const b200pdlp_lp* 
   lap("batch device", "prologue (device)");
 }
 
-static void solve_batch_device(int count, const b200pdlp_lp* lps, const b200pdlp_params& prm, const b200pdlp_warm* warms,
+void solve_batch_device(int count, const b200pdlp_lp* lps, const b200pdlp_params& prm, const b200pdlp_warm* warms,
                                b200pdlp_result* outs) {
   using clk = std::chrono::steady_clock;
   const auto t_begin = clk::now();
@@ -1362,7 +1327,7 @@ static void device_form(StdForm& f, const BatchPrep& P, const b200pdlp_lp& lp, c
 
 // `mixed`: a member past ordered_max is a tree member and the results take the blocks' trace rows; otherwise such a member
 // is an error
-static void solve_hipdlp_batch_device(int count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params& prm,
+void solve_hipdlp_batch_device(int count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params& prm,
                                       b200pdlp_result* outs, bool mixed) {
   using clk = std::chrono::steady_clock;
   const char* who = mixed ? "b200pdlp_solve_hipdlp_batch_mixed_device" : "b200pdlp_solve_hipdlp_batch_device";

@@ -41,13 +41,16 @@ static void create_problem_hipdlp_device(const b200pdlp_lp& lp, const b200pdlp_h
   P.ruiz_iterations = prm.ruiz_iterations;
   run_prologue(P, p->stream, lp, true);
   lap("setup", "device prologue (HiPDLP)");
-  if (lap.on) fprintf(stderr, "[b200pdlp setup] ordered |c|^2, |b|^2 (side stream, under the layouts) %8.3f ms\n", P.sc.norms_ms);
+  if (lap.on) {
+    fprintf(stderr, "[b200pdlp setup] ordered |c|^2, |b|^2 (side stream, under the layouts) %8.3f ms\n", P.sc.norms_ms);
+    fprintf(stderr, "[b200pdlp setup] LP arrays copied to the device: %zu bytes\n", P.h2d_bytes);
+  }
   take_prologue(lp, P, p);
   adopt_matrix(p->A, P.A);
   adopt_matrix(p->AT, P.AT);
   apply_spmv_grid(p);
   hipdlp_buffers(p);
-  alloc_postsolve_staging(p);
+  if (!p->device_io) alloc_postsolve_staging(p);
   CUDA_OK(cudaStreamSynchronize(p->stream));
   lap("setup", "vectors + scratch");
 }
@@ -452,7 +455,15 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
   // unscaleSolution + postprocess (pdhg.cc:1883-1897, :359-492): the iterate is copied out ONLY on convergence --
   // an iteration-limited run returns x = y = 0, like the reference
   // (several GPUs: rank 0 holds the whole iterate and slacks after the final check; the other ranks return no vectors)
-  if (p->dev_form && p->rank == 0) {
+  const bool have_out = out->col_value && out->col_dual && out->row_value && out->row_dual;
+  if (p->dev_form && p->device_io) {
+    // on the device, straight into the caller's device vectors
+    if (have_out)
+      launch_hip_postsolve(s, p->prep.arr, f.sense, converged ? 1 : 0, f.scaled ? 1 : 0, sol_x, sol_y, h.sp.p, h.sn.p,
+                           p->colscale.p, p->rowscale.p, out->col_value, out->col_dual, out->row_value, out->row_dual);
+    CUDA_OK(cudaGetLastError());
+    CUDA_OK(cudaStreamSynchronize(s));
+  } else if (p->dev_form && p->rank == 0) {
     // on the device (launch_hip_postsolve), one download of the four original-order vectors
     const int n0 = f.n_orig;
     double* cv = p->io_col.p;
@@ -462,7 +473,7 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
     launch_hip_postsolve(s, p->prep.arr, f.sense, converged ? 1 : 0, f.scaled ? 1 : 0, sol_x, sol_y, h.sp.p, h.sn.p, p->colscale.p,
                          p->rowscale.p, cv, cd, rv, rd);
     CUDA_OK(cudaGetLastError());
-    if (out->col_value && out->col_dual && out->row_value && out->row_dual) {
+    if (have_out) {
       auto dn = [&](double* dst, const double* src, int len) {
         if (len > 0) CUDA_OK(cudaMemcpyAsync(dst, src, (size_t)len * sizeof(double), cudaMemcpyDeviceToHost, s));
       };
@@ -573,6 +584,44 @@ int b200pdlp_solve_hipdlp(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params* p
     create_problem_hipdlp(*lp, *params, p.get());
     out->setup_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
     solve_hipdlp_on_device(p.get(), *lp, *params, out);
+    CUDA_OK(cudaGetLastError());
+  });
+}
+
+int b200pdlp_solve_hipdlp_device(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params* params, b200pdlp_result* out) {
+  DeviceGuard dg;
+  const char* who = "b200pdlp_solve_hipdlp_device";
+  return guarded([&] {
+    if (!lp || !params || !out) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": null argument");
+    if (!lp_fields_ok(lp)) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": b200pdlp: malformed b200pdlp_lp");
+    if (lp->sense != 1.0 && lp->sense != -1.0) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": b200pdlp: sense must be +1 or -1");
+    const int device = select_device(params->device);
+    check_device_lp(*lp, device, -1, who);
+    check_device_result(*out, device, -1, who);
+    const auto t0 = std::chrono::steady_clock::now();
+    b200pdlp_hipdlp_params prm = *params;
+    prm.device = device;
+    ProblemPtr p(new b200pdlp_problem());   // its stream serves the sizing and, in tree mode, the solve
+    open_problem(p.get(), device, 0, 1);
+    int nnz = 0;
+    const DeviceRoute route = device_lp_route(p->stream, *lp, true, prm.ordered_max, who, &nnz);
+    if (route == DeviceRoute::Ordered) {
+      solve_hipdlp_batch_device(1, lp, prm, out, /*mixed=*/true);
+    } else if (route == DeviceRoute::Degenerate) {
+      solve_degenerate(p->stream, *lp, nullptr, out, [&](const b200pdlp_lp& hl, const b200pdlp_warm*, b200pdlp_result* r) {
+        ProblemPtr q(new b200pdlp_problem());
+        create_problem_hipdlp(hl, prm, q.get());
+        r->setup_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+        solve_hipdlp_on_device(q.get(), hl, prm, r);
+      });
+    } else {
+      p->device_io = true;
+      p->prep.inputs_on_device = true;
+      p->prep.device_nnz = nnz;
+      create_problem_hipdlp_device(*lp, prm, p.get());
+      out->setup_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+      solve_hipdlp_on_device(p.get(), *lp, prm, out);
+    }
     CUDA_OK(cudaGetLastError());
   });
 }

@@ -110,6 +110,7 @@ ABI_SYMBOLS = [
     "b200pdlp_kkt_check_batch_device", "b200pdlp_hipdlp_problem_create", "b200pdlp_hipdlp_step", "b200pdlp_hipdlp_check",
     "b200pdlp_hipdlp_problem_power_method", "b200pdlp_solve_hipdlp_batch_mixed",
     "b200pdlp_solve_hipdlp_batch_mixed_device", "b200pdlp_debug_hipdlp_tree_prep_compare", "b200pdlp_check_device",
+    "b200pdlp_solve_device", "b200pdlp_solve_hipdlp_device",
 ]
 HIP_TRACE_COLS = 16   # B200PDLP_HIP_TRACE_COLS: the per-block trace of the HiPDLP solves
 
@@ -365,6 +366,48 @@ def solve_batch_device(dlps, warms=None, trace_cap: int = 0, **params) -> list:
     return [_result_dict(cres[i], arrays[i]) for i in range(count)]
 
 
+def _device_result(d: dict, dev, trace_cap: int, trace_cols: int):
+    """a CResult whose four vectors are new float64 CUDA tensors on `dev` for the LP of lp_to_device dict `d` (at least one
+    element each, so that an LP without rows or columns still gets four non-NULL vectors), with a host trace array of
+    trace_cap rows; and the arrays the result dict returns"""
+    import torch
+    n, m = d["num_col"], d["num_row"]
+    vecs = [torch.empty(max(k, 1), dtype=torch.float64, device=dev) for k in (n, n, m, m)]
+    res = CResult()
+    res.col_value, res.col_dual, res.row_value, res.row_dual = (_dev_ptr(v, torch.float64, _dp, "result") for v in vecs)
+    out = tuple(v[:k] for v, k in zip(vecs, (n, n, m, m)))
+    if trace_cap > 0:
+        tr = np.zeros((trace_cap, trace_cols))
+        res.trace, res.trace_cap = _p(tr, _dp), trace_cap
+        out = out + (tr,)
+    return res, out
+
+
+def solve_device(dlp: dict, warm=None, trace_cap: int = 0, **params) -> dict:
+    """b200pdlp_solve_device: solve() for an LP already in GPU memory (a dict of lp_to_device), at any size.  warm: None or
+    (col_value, row_value, row_dual) as float64 CUDA tensors.  Returns the dict solve() returns for host copies of the same
+    arrays, bit for bit, with the four vectors as float64 CUDA tensors (kkt_check_batch_device takes them as they are).  A
+    tree-mode LP's prologue reads the tensors in place; an ordered-mode LP is solved as a batch of one (solve_batch_device),
+    whose timings and kernel_launches it returns.  `device` defaults to the device of the LP's tensors; torch's current
+    stream is synchronised first, so that inputs it is still writing are complete."""
+    import torch
+    L = lib()
+    L.b200pdlp_solve_device.argtypes = [C.POINTER(CLp), C.POINTER(CParams), C.POINTER(CWarm), C.POINTER(CResult)]
+    params.setdefault("device", dlp["a_start"].device.index)
+    prm = make_params(**params)
+    dev = torch.device("cuda", prm.device if prm.device >= 0 else torch.cuda.current_device())
+    clp = make_clp_device(dlp)
+    res, arrays = _device_result(dlp, dev, trace_cap, 16)
+    cw = None
+    if warm is not None:   # (an empty vector gets one element: a NULL pointer would mean a cold start)
+        keep = [w if w.numel() else torch.zeros(1, dtype=torch.float64, device=dev) for w in warm]
+        cw = CWarm(*(_dev_ptr(w, torch.float64, _dp, "warm start") for w in keep))
+    torch.cuda.current_stream(dev).synchronize()
+    _check(L.b200pdlp_solve_device(C.byref(clp), C.byref(prm), C.byref(cw) if cw else None, C.byref(res)),
+           "b200pdlp_solve_device")
+    return _result_dict(res, arrays)
+
+
 def _prep_compare(name: str, items, lps, *ints) -> list:
     """the call of a batch prologue comparison `name` on host LPs, with the int arguments `ints`: one dict of mismatch counts
     per LP (`items`)"""
@@ -599,17 +642,40 @@ def _hipdlp_params(params) -> CHipdlpParams:
     return prm
 
 
-def solve_hipdlp(lp: HighsLp, trace_cap: int = 0, **params) -> dict:
+def solve_hipdlp(lp: HighsLp, trace_cap: int = 0, out_arrays=None, **params) -> dict:
     """b200pdlp_solve_hipdlp: the HiPDLP mode (reflected Halpern PDHG, solver=hipdlp) on one GPU; parameters are the
     HighsOptions of the same meaning (tolerance, iter_limit, scaling_mode, ruiz_iterations, step_size_strategy ...), and
     device_prep=-1 for the host prologue instead of the device-resident one.  trace_cap > 0: "trace" holds one row of
-    HIP_TRACE_COLS per block of 40 steps (include/b200pdlp.h, B200PDLP_HIP_TRACE_COLS)."""
+    HIP_TRACE_COLS per block of 40 steps (include/b200pdlp.h, B200PDLP_HIP_TRACE_COLS).
+    out_arrays = (col_value, col_dual, row_value, row_dual): caller-owned (e.g. page-locked) result storage, as in solve()."""
     L = lib()
     L.b200pdlp_solve_hipdlp.argtypes = [C.POINTER(CLp), C.POINTER(CHipdlpParams), C.POINTER(CResult)]
     clp, keep = make_clp(lp)
     prm = _hipdlp_params(params)
     res, arrays = _mk_result(lp, trace_cap)
+    if out_arrays is not None:
+        arrays = tuple(out_arrays) + arrays[4:]
+        res.col_value, res.col_dual, res.row_value, res.row_dual = (_p(a, _dp) for a in arrays[:4])
     _check(L.b200pdlp_solve_hipdlp(C.byref(clp), C.byref(prm), C.byref(res)), "b200pdlp_solve_hipdlp")
+    return _result_dict(res, arrays)
+
+
+def solve_hipdlp_device(dlp: dict, trace_cap: int = 0, **params) -> dict:
+    """b200pdlp_solve_hipdlp_device: solve_hipdlp() for an LP already in GPU memory (a dict of lp_to_device), at any size.
+    Returns the dict solve_hipdlp() returns for host copies of the same arrays, bit for bit, with the four vectors as
+    float64 CUDA tensors.  A tree-mode LP's prologue reads the tensors in place; an ordered-mode LP is solved as a batch of
+    one (solve_hipdlp_batch_mixed_device), whose timings and kernel_launches it returns.  `device` defaults to the device of
+    the LP's tensors; torch's current stream is synchronised first."""
+    import torch
+    L = lib()
+    L.b200pdlp_solve_hipdlp_device.argtypes = [C.POINTER(CLp), C.POINTER(CHipdlpParams), C.POINTER(CResult)]
+    params.setdefault("device", dlp["a_start"].device.index)
+    prm = _hipdlp_params(params)
+    dev = torch.device("cuda", prm.device if prm.device >= 0 else torch.cuda.current_device())
+    clp = make_clp_device(dlp)
+    res, arrays = _device_result(dlp, dev, trace_cap, HIP_TRACE_COLS)
+    torch.cuda.current_stream(dev).synchronize()
+    _check(L.b200pdlp_solve_hipdlp_device(C.byref(clp), C.byref(prm), C.byref(res)), "b200pdlp_solve_hipdlp_device")
     return _result_dict(res, arrays)
 
 

@@ -181,6 +181,32 @@ int b200pdlp_solve_batch_device(int32_t count, const b200pdlp_lp* lps, const b20
                                 const b200pdlp_warm* warms /* [count] or NULL; device vectors; a member whose pointers are NULL starts cold */,
                                 b200pdlp_result* outs /* [count]; vectors in device memory */);
 
+/* b200pdlp_solve for an LP that is already in GPU memory, at any size.  Pointers follow b200pdlp_solve_batch_device's rules:
+ * the LP's eight arrays, the three warm vectors and the four result vectors are device (or managed) memory of params->device
+ * (< 0: the current device); num_col, num_row, sense and offset are host scalars; `trace` stays a host pointer.  Returns
+ * exactly what b200pdlp_solve returns for host copies of the same arrays with the same params, cold or warm: term_code,
+ * term_iterate, iters, passes, restarts, the residual scalars, the form dimensions, the trace rows and the four vectors, bit
+ * for bit.  The call never writes an input, uses a stream of its own and returns once the outputs are complete on the device.
+ * The four result vectors may be NULL only together (then none is written).  One grid-wide sizing kernel validates the arrays and counts the slack rows (one read-back); then the route:
+ *  - tree mode (the standard form past ordered_max, and rows, columns and nonzeros): b200pdlp_solve's device prologue reads
+ *    the eight arrays in place (no copy of the LP: B200PDLP_TIMING=1 prints "LP arrays copied to the device: 0 bytes"), the
+ *    hot start goes straight to the initial point and the postsolve writes the caller's vectors.  device_scaling = -1 and
+ *    B200PDLP_DEVICE_PREP=0 are ignored: the result is b200pdlp_solve's with its default, device prologue;
+ *  - ordered mode: b200pdlp_solve_batch_device with this one LP; setup_seconds, solve_seconds, loop_device_ms,
+ *    iter_device_ms and kernel_launches are then the batch's (kernel_launches = its rounds);
+ *  - an LP without rows, columns or nonzeros past ordered_max (it has no matrix): its vectors are copied to the host, solved
+ *    as b200pdlp_solve solves them (host prologue), and the four result vectors copied back.
+ * Returns B200PDLP_ERR_ARG, with nothing written, in b200pdlp_solve_batch_device's order: before any device work for NULL
+ * arguments, a bad device_scaling, a malformed b200pdlp_lp or a sense other than +-1; then, naming the field, for a pointer
+ * that is not device memory of the device; then, with b200pdlp_solve's messages and in its order, for a malformed a_start or
+ * a_index (a_index is read only once a_start has passed).  No device: B200PDLP_ERR_CUDA.
+ * Known limitation: an LP without rows past ordered_max takes b200pdlp_solve's host path, which does not return on such an
+ * LP today (b200pdlp_solve_hipdlp_device solves it).
+ * STATUS: runs on hardware; tests/test_gpu_solve_device.py (byte equality with b200pdlp_solve on host copies),
+ * tools/solve_device_bench.py. */
+int b200pdlp_solve_device(const b200pdlp_lp* lp, const b200pdlp_params* params,
+                          const b200pdlp_warm* warm /* NULL or device vectors */, b200pdlp_result* out /* device vectors */);
+
 /* ---- persistent problem handle (bench + kernel-level parity tests) --------- */
 typedef struct b200pdlp_problem b200pdlp_problem;
 
@@ -426,6 +452,15 @@ int b200pdlp_solve_hipdlp_batch_device(int32_t count, const b200pdlp_lp* lps, co
  * b200pdlp_solve_hipdlp_batch_mixed on host copies and with b200pdlp_solve_hipdlp), tools/hipdlp_batch_mixed_device_bench.py. */
 int b200pdlp_solve_hipdlp_batch_mixed_device(int32_t count, const b200pdlp_lp* lps, const b200pdlp_hipdlp_params* params,
                                              b200pdlp_result* outs /* [count]; vectors in device memory */);
+/* b200pdlp_solve_hipdlp for an LP that is already in GPU memory, at any size: b200pdlp_solve_device's pointer rules, bits,
+ * routes and errors, with HiPDLP's classification (+-infinity row bounds, FREE rows with a slack column).  Tree mode reads
+ * the LP in place through the HiPDLP device prologue (device_prep = -1 and B200PDLP_DEVICE_PREP=0 are ignored, as above); ordered mode
+ * is b200pdlp_solve_hipdlp_batch_mixed_device with this one LP, whose trace rows are b200pdlp_solve_hipdlp's and whose
+ * setup_seconds, solve_seconds, loop_device_ms, iter_device_ms and kernel_launches are the batch's.
+ * STATUS: runs on hardware; tests/test_gpu_solve_device.py (byte equality with b200pdlp_solve_hipdlp on host copies),
+ * tools/solve_device_bench.py. */
+int b200pdlp_solve_hipdlp_device(const b200pdlp_lp* lp, const b200pdlp_hipdlp_params* params,
+                                 b200pdlp_result* out /* device vectors */);
 /* debug (tests): the tree-mode device prologue of b200pdlp_solve_hipdlp_batch_mixed_device on host LPs (uploaded first),
  * every member treated as a tree member, against formulate_hipdlp + scale_hipdlp(scaling_mode, ruiz_iterations) +
  * build_layout(ordered_max = -1), then the device postsolve of a fixed pseudo-random iterate against hip_host_postsolve.
