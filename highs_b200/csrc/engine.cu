@@ -319,7 +319,8 @@ void check_device_result(const b200pdlp_result& out, int device, int i, const ch
 // lp_size_kernel: check_lp(deep) and the slack rows under the mode's classification) and one read-back of its record: Ordered when the
 // standard form is within ordered_max (device_prep_fits' rule), else Tree when it has rows, columns and nonzeros, else
 // Degenerate.  A malformed LP is ERR_ARG with check_lp's message, in check_lp's order.  *nnz = a_start[num_col].
-DeviceRoute device_lp_route(cudaStream_t s, const b200pdlp_lp& lp, bool hipdlp, int ordered_max, const char* who, int* nnz) {
+enum class DeviceRoute { Ordered, Tree, Degenerate };
+static DeviceRoute device_lp_route(cudaStream_t s, const b200pdlp_lp& lp, bool hipdlp, int ordered_max, const char* who, int* nnz) {
   BatchPrep P{};
   P.n0 = lp.num_col; P.m = lp.num_row; P.sense = lp.sense;
   P.a_start = lp.a_start; P.a_index = lp.a_index; P.a_value = lp.a_value;
@@ -344,8 +345,8 @@ DeviceRoute device_lp_route(cudaStream_t s, const b200pdlp_lp& lp, bool hipdlp, 
 // A degenerate LP of a single device-array solve (no rows, no columns or no nonzeros: well-formed, it has no matrix) takes
 // the host prologue, as in the host-array solve: its vectors (and hot start) come down, solve() runs on host copies, and the
 // four result vectors go back up into the caller's device vectors (those given) on stream s.
-void solve_degenerate(cudaStream_t s, const b200pdlp_lp& lp, const b200pdlp_warm* warm, b200pdlp_result* out,
-                      const HostSolve& solve) {
+static void solve_degenerate(cudaStream_t s, const b200pdlp_lp& lp, const b200pdlp_warm* warm, b200pdlp_result* out,
+                             const std::function<void(const b200pdlp_lp&, const b200pdlp_warm*, b200pdlp_result*)>& solve) {
   const int n0 = lp.num_col, m = lp.num_row;
   std::vector<int> start((size_t)n0 + 1);
   std::vector<std::vector<double>> h(12);
@@ -373,6 +374,44 @@ void solve_degenerate(cudaStream_t s, const b200pdlp_lp& lp, const b200pdlp_warm
   CUDA_OK(cudaStreamSynchronize(s));
   r.col_value = out->col_value; r.col_dual = out->col_dual; r.row_value = out->row_value; r.row_dual = out->row_dual;
   *out = r;
+}
+
+void solve_lp_device(const b200pdlp_lp& lp, bool hipdlp, int& device, int ordered_max, const b200pdlp_warm* warm,
+                     b200pdlp_result* out, const char* who, const std::function<void()>& batch, const CreateProblem& create_host,
+                     const CreateProblem& create_device, const SolveProblem& solve) {
+  if (!lp_fields_ok(&lp)) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": b200pdlp: malformed b200pdlp_lp");
+  if (lp.sense != 1.0 && lp.sense != -1.0) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": b200pdlp: sense must be +1 or -1");
+  device = select_device(device);
+  check_device_lp(lp, device, -1, who);
+  if (warm) {
+    check_device_array(warm->col_value, device, -1, "warm col_value", who);
+    check_device_array(warm->row_value, device, -1, "warm row_value", who);
+    check_device_array(warm->row_dual, device, -1, "warm row_dual", who);
+  }
+  check_device_result(*out, device, -1, who);
+  const auto t0 = std::chrono::steady_clock::now();
+  ProblemPtr p(new b200pdlp_problem());   // its stream serves the sizing and, in tree mode, the solve
+  open_problem(p.get(), device, 0, 1);
+  int nnz = 0;
+  const DeviceRoute route = device_lp_route(p->stream, lp, hipdlp, ordered_max, who, &nnz);
+  auto setup_seconds = [&] { return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(); };
+  if (route == DeviceRoute::Ordered) {
+    batch();
+  } else if (route == DeviceRoute::Degenerate) {
+    solve_degenerate(p->stream, lp, warm, out, [&](const b200pdlp_lp& hl, const b200pdlp_warm* hw, b200pdlp_result* r) {
+      ProblemPtr q(new b200pdlp_problem());
+      create_host(hl, q.get());
+      r->setup_seconds = setup_seconds();
+      solve(q.get(), hl, hw, r);
+    });
+  } else {
+    p->device_io = true;
+    p->prep.inputs_on_device = true;
+    p->prep.device_nnz = nnz;
+    create_device(lp, p.get());
+    out->setup_seconds = setup_seconds();
+    solve(p.get(), lp, warm, out);
+  }
 }
 
 // Several GPUs (default; B200PDLP_MG_DEVICE_PREP=0 for the host path): every rank needs the whole scaled standard form to cut its shard out of
@@ -587,14 +626,7 @@ static void enqueue_pass_mg(b200pdlp_problem* p) {
 }
 
 static cudaGraphExec_t capture_passes(b200pdlp_problem* p, int passes) {
-  cudaGraph_t g = nullptr;
-  CUDA_OK(cudaStreamBeginCapture(p->stream, cudaStreamCaptureModeThreadLocal));
-  for (int i = 0; i < passes; i++) enqueue_pass(p);
-  CUDA_OK(cudaStreamEndCapture(p->stream, &g));
-  cudaGraphExec_t ge = nullptr;
-  CUDA_OK(cudaGraphInstantiate(&ge, g, 0));
-  CUDA_OK(cudaGraphDestroy(g));
-  return ge;
+  return capture_graph(p->stream, [&] { for (int i = 0; i < passes; i++) enqueue_pass(p); });
 }
 
 void fill_pow_tables(PdhgState* h) {
@@ -610,13 +642,20 @@ void fill_pow_tables(PdhgState* h) {
 static void push_state(b200pdlp_problem* p) {
   CUDA_OK(cudaMemcpyAsync(p->state.p, p->hstate, sizeof(PdhgState), cudaMemcpyHostToDevice, p->stream));
 }
+static const char kPeerLate[] = "P2P barrier timed out (a peer rank did not arrive)";
+// P2P: reads the barriers' fault word behind the work on the stream (and synchronises the stream).  A barrier that gave up
+// waiting for a peer leaves inconsistent data behind: stop with `msg` instead of going on with it.
+static void throw_if_peer_fault(b200pdlp_problem* p, const char* msg) {
+  if (!p->p2p) return;
+  int* hfault = reinterpret_cast<int*>(p->hflag + 2);
+  CUDA_OK(cudaMemcpyAsync(hfault, p->fault.p, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
+  CUDA_OK(cudaStreamSynchronize(p->stream));
+  if (*hfault) throw Error(B200PDLP_ERR_STATE, msg);
+}
 static void pull_state(b200pdlp_problem* p) {
   CUDA_OK(cudaMemcpyAsync(p->hstate, p->state.p, sizeof(PdhgState), cudaMemcpyDeviceToHost, p->stream));
-  int* hfault = reinterpret_cast<int*>(p->hflag + 2);
-  if (p->p2p) CUDA_OK(cudaMemcpyAsync(hfault, p->fault.p, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
-  CUDA_OK(cudaStreamSynchronize(p->stream));
-  // a barrier gave up waiting for a peer: stop here instead of iterating on inconsistent data
-  if (p->p2p && *hfault) throw Error(B200PDLP_ERR_STATE, "P2P barrier timed out (a peer rank did not arrive)");
+  if (p->p2p) throw_if_peer_fault(p, kPeerLate);
+  else CUDA_OK(cudaStreamSynchronize(p->stream));
 }
 static void pull_outs(b200pdlp_problem* p, int count) {
   CUDA_OK(cudaMemcpyAsync(p->houts, p->outs.p, count * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
@@ -943,6 +982,20 @@ void arm_step(PdhgState* h) {
   }
 }
 
+double time_limit_or_none(double time_limit) { return (time_limit >= 0 && std::isfinite(time_limit)) ? time_limit : -1.0; }
+
+double step_beta(double cost_sq, double rhs_sq) { return std::fmin(cost_sq, rhs_sq) > 1e-6 ? cost_sq / rhs_sq : 1.0; }
+void adaptive_step_sizes(PdhgState* h, double amax) {
+  h->tau = (1.0 / amax) / std::sqrt(h->beta);
+  h->sigma = h->tau * h->beta;
+}
+void fixed_step_sizes(PdhgState* h, double lambda) {
+  h->tau = 0.8 / std::sqrt(lambda);
+  h->sigma = h->tau;
+  h->tau /= std::sqrt(h->beta);
+  h->sigma *= std::sqrt(h->beta);
+}
+
 static double vec_norm2_sq(b200pdlp_problem* p, const double* v, int len, bool reduce_over_ranks) {
   double* o = p->outs.p + 44;
   launch_diff_norm2(p->stream, len, v, nullptr, p->rs(kSlotChk, len), o);
@@ -1229,14 +1282,7 @@ static int enqueue_check_device(b200pdlp_problem* p, bool light = false) {
 }
 
 static cudaGraphExec_t capture_check(b200pdlp_problem* p, bool light, int* launches) {
-  cudaGraph_t g = nullptr;
-  cudaGraphExec_t ge = nullptr;
-  CUDA_OK(cudaStreamBeginCapture(p->stream, cudaStreamCaptureModeThreadLocal));
-  *launches = enqueue_check_device(p, light);
-  CUDA_OK(cudaStreamEndCapture(p->stream, &g));
-  CUDA_OK(cudaGraphInstantiate(&ge, g, 0));
-  CUDA_OK(cudaGraphDestroy(g));
-  return ge;
+  return capture_graph(p->stream, [&] { *launches = enqueue_check_device(p, light); });
 }
 
 static void launch_check_graph(b200pdlp_problem* p, bool light = false) {
@@ -1252,7 +1298,7 @@ static void launch_check_graph(b200pdlp_problem* p, bool light = false) {
 // 32/16/8/4 passes and single passes.  Kernels beyond the check iteration are no-ops.
 static void enqueue_passes_device(b200pdlp_problem* p, int d) {
   if (d <= 0) return;
-  const int kp = p->kernels_per_pass;
+  const int kp = p->kernels_per_pass();
   if (p->no_graph) { for (; d > 0; d--) { enqueue_pass(p); p->launches += kp; } return; }
   if (d > p->graph_main_passes - 12 && !p->graph_main) p->graph_main = capture_passes(p, p->graph_main_passes);
   if (d > p->graph_main_passes - 12 && d <= p->graph_main_passes) {
@@ -1276,58 +1322,60 @@ static void enqueue_passes_device(b200pdlp_problem* p, int d) {
   for (; d > 0; d--) { enqueue_pass(p); p->launches += kp; }
 }
 
-static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, const b200pdlp_warm* warm, b200pdlp_result* out) {
-  NvtxRange nvtx("b200pdlp: solve");
-  nvtxRangePushA("b200pdlp: initial point + graphs");
-  using clk = std::chrono::steady_clock;
-  set_device(p);
-  const auto t_begin = clk::now();
+// ---- the phases of the single solve, in the order solve_on_device runs them
+// the check control block: pinned host copy, mapped time-limit word, device copy (filled by a copy on p->stream)
+static void ensure_ctl(b200pdlp_problem* p) {
+  if (p->hctl) return;
+  p->hctl = static_cast<SolveCtl*>(pinned_cache_alloc(sizeof(SolveCtl), false));
+  p->htime = static_cast<int*>(pinned_cache_alloc(64, true));
+  p->ctl.alloc(1, false);
+}
+static int* mapped_time_flag(b200pdlp_problem* p) {
+  int* d = nullptr;
+  CUDA_OK(cudaHostGetDevicePointer(&d, p->htime, 0));
+  return d;
+}
+// the control block zeroed, with the fields every check reads (the caller adds the time flag, the trace and the memo)
+static SolveCtl* reset_ctl(b200pdlp_problem* p, double tol_p, double tol_d, double tol_gap, int iter_limit, int interval,
+                           bool restart_on) {
+  ensure_ctl(p);
+  SolveCtl* c = p->hctl;
+  memset(c, 0, sizeof(SolveCtl));
+  c->tol_p = tol_p; c->tol_d = tol_d; c->tol_gap = tol_gap;
+  c->sense = p->form.sense; c->offset = p->form.offset;
+  c->iter_limit = iter_limit; c->interval = interval; c->restart_on = restart_on; c->world = p->world;
+  c->term = -1;
+  return c;
+}
+
+// Graphs: one check interval of passes, and a short one for top-ups after rejected steps.  A few spare passes per replay:
+// a rejected line-search step then still reaches the next check iteration inside the same replay (spare passes are no-ops
+// once state.iter == state.stop_iter) instead of costing a host round trip.  The device-driven loop captures its graphs
+// when it first needs them, unless `eager` (logical shards): everything that allocates or instantiates happens before ANY
+// rank launches a kernel that waits for its peers (see LocalGroup), so every graph is captured and uploaded here.
+static void prepare_graphs(b200pdlp_problem* p, const b200pdlp_params& prm, int interval, bool dev_checks, bool eager) {
+  cudaStream_t s = p->stream;
+  const int want = std::min(prm.graph_passes > 0 ? prm.graph_passes : interval + 4, kPowTab - 16);   // the step-rule tables cover one replay
+  if (p->graph_main && p->graph_main_passes != want) { cudaGraphExecDestroy(p->graph_main); p->graph_main = nullptr; }
+  p->graph_main_passes = want;
+  p->no_graph = getenv("B200PDLP_NO_GRAPH") != nullptr;
+  if (p->no_graph || (dev_checks && !eager)) return;
+  if (!p->graph_main) p->graph_main = capture_passes(p, want);
+  if (!p->graph_small) { p->graph_small_passes = 4; p->graph_small = capture_passes(p, 4); }
+  if (!eager) return;
+  for (cudaGraphExec_t g : {p->graph_main, p->graph_small}) CUDA_OK(cudaGraphUpload(g, s));
+  if (!dev_checks) return;
+  ensure_ctl(p);
+  for (int k = 2; k <= 5; k++) if (!p->graph_pow2[k]) { p->graph_pow2[k] = capture_passes(p, 1 << k); CUDA_OK(cudaGraphUpload(p->graph_pow2[k], s)); }
+  if (!p->graph_check) { p->graph_check = capture_check(p, false, &p->check_launches[0]); CUDA_OK(cudaGraphUpload(p->graph_check, s)); }
+  if (!p->graph_check_light) { p->graph_check_light = capture_check(p, true, &p->check_launches[1]); CUDA_OK(cudaGraphUpload(p->graph_check_light, s)); }
+}
+
+// initial point: PDHG_PreSolve (hot start, cupdlp_solver.c:1217-1279) + PDHG_Init_Variables (:531-591) before the steps
+static void start_point(b200pdlp_problem* p, const b200pdlp_warm* warm) {
   const StdForm& f = p->form;
   cudaStream_t s = p->stream;
-  const int n = p->n, m = p->m, ml = p->ml;
-  const int interval = prm.check_interval > 0 ? prm.check_interval : 40;
-  const double t_lim = (prm.time_limit >= 0 && std::isfinite(prm.time_limit)) ? prm.time_limit : -1.0;   // < 0: none
-  const long long launches0 = p->launches;
-  PdhgState* h = p->hstate;
-  memset(h, 0, sizeof(PdhgState));
-  h->adaptive = prm.adaptive_step != 0;
-  out->trace_len = 0;
-  Laps lap;
-  lap.rank = p->world > 1 ? p->rank : -1;
-  if (p->local_link && p->group) {
-    // logical shards: everything that allocates or instantiates happens before ANY rank launches a kernel that waits for
-    // its peers (see LocalGroup)
-    const int interval0 = prm.check_interval > 0 ? prm.check_interval : 40;
-    const int want0 = std::min(prm.graph_passes > 0 ? prm.graph_passes : interval0 + 4, kPowTab - 16);
-    p->kernels_per_pass = p->p2p ? 5 : 6;
-    if (p->graph_main && p->graph_main_passes != want0) { cudaGraphExecDestroy(p->graph_main); p->graph_main = nullptr; }
-    p->graph_main_passes = want0;
-    if (!getenv("B200PDLP_NO_GRAPH")) {
-      if (!p->graph_main) p->graph_main = capture_passes(p, want0);
-      if (!p->graph_small) { p->graph_small_passes = 4; p->graph_small = capture_passes(p, 4); }
-      CUDA_OK(cudaGraphUpload(p->graph_main, s));
-      CUDA_OK(cudaGraphUpload(p->graph_small, s));
-      if (use_device_checks(p, prm)) {
-        if (!p->hctl) {
-          p->hctl = static_cast<SolveCtl*>(pinned_cache_alloc(sizeof(SolveCtl), false));
-          p->htime = static_cast<int*>(pinned_cache_alloc(64, true));
-          p->ctl.alloc(1, false);
-        }
-        for (int k = 2; k <= 5; k++) if (!p->graph_pow2[k]) { p->graph_pow2[k] = capture_passes(p, 1 << k); CUDA_OK(cudaGraphUpload(p->graph_pow2[k], s)); }
-        if (!p->graph_check) { p->graph_check = capture_check(p, false, &p->check_launches[0]); CUDA_OK(cudaGraphUpload(p->graph_check, s)); }
-        if (!p->graph_check_light) { p->graph_check_light = capture_check(p, true, &p->check_launches[1]); CUDA_OK(cudaGraphUpload(p->graph_check_light, s)); }
-      }
-    }
-    CUDA_OK(cudaStreamSynchronize(s));
-    lap("solve", "graphs ready (logical shards)");
-    p->group->arrive_and_wait();
-  }
-
-  // ---- initial point: PDHG_PreSolve (hot start, cupdlp_solver.c:1217-1279) + PDHG_Init_Variables (:531-591)
-  const bool dev_form = p->dev_form;
-  std::vector<double> x0, y0;
-  if (!dev_form) host_start_point(f, warm, x0, y0);
-  const int nl = p->nl;   // column entries held by this rank (== n on one GPU)
+  const int m = p->m, ml = p->ml, nl = p->nl;   // nl: column entries held by this rank (== n on one GPU)
   for (int k = 0; k < 2; k++) {
     CUDA_OK(cudaMemsetAsync(p->x[k].p, 0, (size_t)nl * sizeof(double), s));
     CUDA_OK(cudaMemsetAsync(p->aty[k].p, 0, (size_t)nl * sizeof(double), s));
@@ -1343,7 +1391,7 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
     if (p->p2p) CUDA_OK(cudaMemsetAsync(p->fault.p, 0, sizeof(int), s));
     if (p->p2p) { launch_p2p_exchange(s, p->outs.p + 60, 0, p->peers, p->world, p->rank, p->epochs.p, p->fault.p); p->launches++; }
   }
-  if (dev_form) {
+  if (p->dev_form) {
     // maps and scales live in HBM: the hot start goes up in original order and is permuted / scaled / projected there
     const double *wc = nullptr, *wv = nullptr, *wd = nullptr;
     if (warm && warm->col_value && warm->row_value && warm->row_dual && p->device_io) {
@@ -1358,6 +1406,8 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
                       p->xsum.p, p->y[0].p);
     p->launches += 2;
   } else {
+    std::vector<double> x0, y0;
+    host_start_point(f, warm, x0, y0);
     std::vector<double> xp(std::max(nl, 1), 0.0), yp(std::max(ml, 1));
     for (int i = 0; i < p->nl_real; i++) xp[i] = x0[p->cperm[p->c0 + i]];
     for (int i = 0; i < ml; i++) yp[i] = y0[p->r0 + p->rperm[i]];
@@ -1365,31 +1415,30 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
     if (ml) CUDA_OK(cudaMemcpyAsync(p->y[0].p, yp.data(), (size_t)ml * sizeof(double), cudaMemcpyHostToDevice, s));
     CUDA_OK(cudaStreamSynchronize(s));
   }
+}
 
-  // ---- PDHG_Init_Step_Sizes (cupdlp_step.c:312-375)
-  {
-    double a = 0.0, b = 0.0;   // cupdlp_twoNormSquared = dot(x,x), sequential on the reference's CPU path
-    if (dev_form) { a = p->beta_cost_sq; b = p->beta_rhs_sq; }   // tree sums from the device prologue
-    else {
-      for (int j = 0; j < n; j++) a += f.cost[j] * f.cost[j];
-      for (int i = 0; i < m; i++) b += f.rhs[i] * f.rhs[i];
-    }
-    h->beta = std::fmin(a, b) > 1e-6 ? a / b : 1.0;
-    if (h->adaptive) {
-      h->tau = (1.0 / f.amax) / std::sqrt(h->beta);
-      h->sigma = h->tau * h->beta;
-    } else {
-      const double lambda = power_method(p);
-      h->tau = 0.8 / std::sqrt(lambda);
-      h->sigma = h->tau;
-      h->tau /= std::sqrt(h->beta);
-      h->sigma *= std::sqrt(h->beta);
-    }
+// PDHG_Init_Step_Sizes (cupdlp_step.c:312-375)
+static void init_step_sizes(b200pdlp_problem* p, PdhgState* h) {
+  const StdForm& f = p->form;
+  double a = 0.0, b = 0.0;   // cupdlp_twoNormSquared = dot(x,x), sequential on the reference's CPU path
+  if (p->dev_form) { a = p->beta_cost_sq; b = p->beta_rhs_sq; }   // tree sums from the device prologue
+  else {
+    for (int j = 0; j < f.n; j++) a += f.cost[j] * f.cost[j];
+    for (int i = 0; i < f.m; i++) b += f.rhs[i] * f.rhs[i];
   }
+  h->beta = step_beta(a, b);
+  if (h->adaptive) adaptive_step_sizes(h, f.amax);
+  else fixed_step_sizes(h, power_method(p));
+}
+
+// sums start at proj(0) like PDHG_Init_Variables :577-583; the average is recomputed at every check
+static void start_products_and_sums(b200pdlp_problem* p) {
+  const StdForm& f = p->form;
+  cudaStream_t s = p->stream;
+  const int nl = p->nl, ml = p->ml;
   full_ax(p, p->x[0].p, p->ax[0].p);
   full_aty(p, p->y[0].p, p->aty[0].p);
-  // sums start at proj(0) like PDHG_Init_Variables :577-583; the average is recomputed at every check
-  if (!dev_form) {
+  if (!p->dev_form) {
     std::vector<double> z(std::max(nl, 1), 0.0);
     bool nz = false;
     for (int i = 0; i < p->nl_real; i++) {
@@ -1404,197 +1453,171 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
   CUDA_OK(cudaMemsetAsync(p->ysum.p, 0, (size_t)std::max(ml, 1) * sizeof(double), s));
   CUDA_OK(cudaMemsetAsync(p->xlr.p, 0, (size_t)nl * sizeof(double), s));
   CUDA_OK(cudaMemsetAsync(p->ylr.p, 0, (size_t)std::max(ml, 1) * sizeof(double), s));
-  arm_step(h);
-  fill_pow_tables(h);
-  push_state(p);
-  CUDA_OK(cudaStreamSynchronize(s));
-  lap("solve", "initial point + state");
+}
 
-  // ---- graphs: one check interval of passes, and a short one for top-ups after rejected steps
-  // a few spare passes per replay: a rejected line-search step then still reaches the next check iteration inside
-  // the same replay (spare passes are no-ops once state.iter == state.stop_iter) instead of costing a host round trip
-  const int want_main = std::min(prm.graph_passes > 0 ? prm.graph_passes : interval + 4, kPowTab - 16);   // the step-rule tables cover one replay
-  const bool dev_checks = use_device_checks(p, prm);
-  if (p->graph_main && p->graph_main_passes != want_main) { cudaGraphExecDestroy(p->graph_main); p->graph_main = nullptr; }
-  p->graph_main_passes = want_main;
-  p->no_graph = getenv("B200PDLP_NO_GRAPH") != nullptr;
-  if (!dev_checks && !p->no_graph) {   // (the device-driven loop captures the graphs it needs when it first needs them)
-    if (!p->graph_main) p->graph_main = capture_passes(p, want_main);
-    if (!p->graph_small) { p->graph_small_passes = 4; p->graph_small = capture_passes(p, 4); }
-  }
-  p->kernels_per_pass = p->world == 1 ? 4 : (p->p2p ? 5 : 6);   // ours; NCCL kernels not counted
-  lap("solve", "graph capture");
-  nvtxRangePop();
-  nvtxRangePushA("b200pdlp: PDHG loop");
-
-  const double tol_p = prm.tol_primal * (1.0 + f.norm_rhs), tol_d = prm.tol_dual * (1.0 + f.norm_cost);
-  RestartMemo memo;
-  CheckResult chk;
+struct LoopLimits {   // the time limit counts from t_loop
+  int interval;
+  double tol_p, tol_d, t_lim;   // t_lim < 0: none
+  std::chrono::steady_clock::time_point t_loop;
+  double elapsed() const { return std::chrono::duration<double>(std::chrono::steady_clock::now() - t_loop).count(); }
+  bool over() const { return t_lim >= 0 && elapsed() > t_lim; }
+};
+struct LoopOutcome {
   int term = B200PDLP_TIMELIMIT_OR_ITERLIMIT, term_iterate = 0, restarts = 0;
   bool have_check = false;
+  CheckResult chk;
+  double iter_ms = 0.0;   // device time of the passes
+};
+
+// device-driven loop: the checks decide on the device (termination, restarts, next check iteration); the host
+// enqueues [check, passes to the next check] rounds ahead from the deterministic check schedule and reads the control
+// block once per batch.  A rejected line-search step makes a round fall short; the following rounds make up for it
+// (kernels are no-ops outside their turn) and the next read-back re-synchronises the prediction.
+static LoopOutcome device_loop(b200pdlp_problem* p, const b200pdlp_params& prm, const b200pdlp_warm* warm,
+                               const LoopLimits& lim, b200pdlp_result* out) {
+  cudaStream_t s = p->stream;
+  PdhgState* h = p->hstate;
+  const int nl = p->nl, ml = p->ml;
+  SolveCtl* c = reset_ctl(p, lim.tol_p, lim.tol_d, prm.tol_gap, prm.iter_limit, lim.interval, prm.restart != 0);
+  *p->htime = lim.over() ? 1 : 0;
+  c->time_flag = lim.t_lim >= 0 ? mapped_time_flag(p) : nullptr;   // (no limit: spare the device the read over PCIe)
+  // dense-check phase (iterations 0 .. kDenseChecks-1 are all check iterations): the passes carry A xSum and A'ySum, the
+  // checks are two vector sweeps.  B200PDLP_LIGHT_CHECK=0: every check multiplies the average iterate by A and A'.
+  const bool hot = warm && warm->col_value && warm->row_value && warm->row_dual;
+  bool h_light = p->axsum.p && p->atysum.p && (p->world == 1 || !hot);   // (several GPUs: A_g xSum of a hot start would need the gathered xSum)
+  if (const char* e = getenv("B200PDLP_LIGHT_CHECK")) if (atoi(e) == 0) h_light = false;
+  h->light_on = h_light ? 1 : 0;
+  if (h_light) {
+    // xSum starts at proj(0) (PDHG_Init_Variables): without a hot start that IS x, whose product is at hand
+    if (hot) { launch_spmv_plain(s, p->A.dev, p->xsum.p, p->axsum.p); p->launches++; }
+    else CUDA_OK(cudaMemcpyAsync(p->axsum.p, p->ax[0].p, (size_t)std::max(ml, 1) * sizeof(double), cudaMemcpyDeviceToDevice, s));
+    CUDA_OK(cudaMemsetAsync(p->atysum.p, 0, (size_t)std::max(nl, 1) * sizeof(double), s));
+  }
+  if (out->trace && out->trace_cap > 0) {
+    if (p->trace_dev.n < (size_t)out->trace_cap * B200PDLP_TRACE_COLS) p->trace_dev.alloc((size_t)out->trace_cap * B200PDLP_TRACE_COLS, false);
+    c->trace = p->trace_dev.p; c->trace_cap = out->trace_cap;
+  }
+  CUDA_OK(cudaMemcpyAsync(p->ctl.p, c, sizeof(SolveCtl), cudaMemcpyHostToDevice, s));
+  h->stop_iter = 0;   // the first check is due at once (iteration 0)
+  push_state(p);
+  LoopOutcome o;
+  std::vector<std::unique_ptr<CudaEvent>> evs;
+  int pred_iter = 0, carry = 0;   // carry: passes still owed before the next check (after a re-synchronisation)
+  while (true) {
+    size_t nev = 0;
+    NvtxRange nvtx_batch("b200pdlp: batch of [check, passes] rounds");
+    auto ev = [&]() -> cudaEvent_t {
+      if (nev == evs.size()) evs.emplace_back(new CudaEvent());
+      return *evs[nev++];
+    };
+    int rounds = 0, passes = 0;
+    if (carry > 0) {
+      CUDA_OK(cudaEventRecord(ev(), s));
+      enqueue_passes_device(p, carry);
+      CUDA_OK(cudaEventRecord(ev(), s));
+      passes += carry; pred_iter += carry; carry = 0;
+    }
+    while (rounds < 12 && passes < 48) {
+      // pred_iter never runs behind the device's iteration count, so pred_iter < kDenseChecks implies the device is
+      // inside the dense phase as well (the light kernels check it once more themselves)
+      launch_check_graph(p, h_light && pred_iter < kDenseChecks);
+      rounds++;
+      if (pred_iter >= prm.iter_limit - 1) break;
+      const int next = next_check_iter(pred_iter, lim.interval, prm.iter_limit);
+      CUDA_OK(cudaEventRecord(ev(), s));
+      enqueue_passes_device(p, next - pred_iter);
+      CUDA_OK(cudaEventRecord(ev(), s));
+      passes += next - pred_iter;
+      pred_iter = next;
+    }
+    CUDA_OK(cudaMemcpyAsync(c, p->ctl.p, sizeof(SolveCtl), cudaMemcpyDeviceToHost, s));
+    CUDA_OK(cudaMemcpyAsync(h, p->state.p, sizeof(PdhgState), cudaMemcpyDeviceToHost, s));
+    const size_t npairs = nev / 2;   // events so far come in (before, after) pairs around the passes
+    cudaEvent_t fin = ev();
+    CUDA_OK(cudaEventRecord(fin, s));
+    if (lim.t_lim >= 0) {
+      // poll, so that the time-limit word can be raised while the batch runs
+      while (cudaEventQuery(fin) == cudaErrorNotReady) {
+        if (lim.elapsed() > lim.t_lim) *p->htime = 1;
+        std::this_thread::yield();
+      }
+    }
+    CUDA_OK(cudaEventSynchronize(fin));
+    throw_if_peer_fault(p, kPeerLate);
+    for (size_t k = 0; k < npairs; k++) {
+      float ms = 0.f;
+      CUDA_OK(cudaEventElapsedTime(&ms, *evs[2 * k], *evs[2 * k + 1]));
+      o.iter_ms += ms;
+    }
+    if (c->term >= 0) break;
+    // not finished: continue from where the device really is
+    h_light = h_light && h->light_on != 0;
+    pred_iter = h->iter;
+    carry = std::max(0, h->stop_iter - h->iter);
+  }
+  o.term = c->term; o.term_iterate = c->term_iterate; o.restarts = c->restarts;
+  o.have_check = c->checks > 0;
+  for (int t = 0; t < 2; t++) {
+    const DevResiduals& d = c->res[t];
+    Residuals& R = o.chk.it[t];
+    R.pobj = d.pobj; R.dobj = d.dobj; R.pfeas = d.pfeas; R.dfeas = d.dfeas; R.gap = d.gap; R.relgap = d.relgap;
+    R.pinf_obj = d.pinf_obj; R.pinf_res = d.pinf_res; R.dinf_obj = d.dinf_obj; R.dinf_res = d.dinf_res;
+  }
+  if (c->trace) {
+    out->trace_len = std::min(c->trace_len, out->trace_cap);
+    if (out->trace_len > 0)
+      CUDA_OK(cudaMemcpyAsync(out->trace, p->trace_dev.p, (size_t)out->trace_len * B200PDLP_TRACE_COLS * sizeof(double),
+                              cudaMemcpyDeviceToHost, s));
+  }
+  return o;
+}
+
+// host-driven loop (cupdlp_solver.c:939-1106)
+static LoopOutcome host_loop(b200pdlp_problem* p, const b200pdlp_params& prm, const LoopLimits& lim, b200pdlp_result* out) {
+  cudaStream_t s = p->stream;
+  PdhgState* h = p->hstate;
+  LoopOutcome o;
+  RestartMemo memo;
   bool have_spec = false, spec_flag = false;   // a speculative check already produced the next check's scalars
   const bool speculate = can_speculate_check(p);
-  bool h_light = false;
-  CudaEvent ev0, ev1, evl0, evl1;
-  double iter_ms = 0.0;
-  CUDA_OK(cudaEventRecord(evl0, s));
-  const auto t_loop = clk::now();
-
-  if (dev_checks) {
-    // ---- device-driven loop: the checks decide on the device (termination, restarts, next check iteration); the host
-    // enqueues [check, passes to the next check] rounds ahead from the deterministic check schedule and reads the
-    // control block once per batch.  A rejected line-search step makes a round fall short; the following rounds make
-    // up for it (kernels are no-ops outside their turn) and the next read-back re-synchronises the prediction.
-    if (!p->hctl) {
-      p->hctl = static_cast<SolveCtl*>(pinned_cache_alloc(sizeof(SolveCtl), false));
-      p->htime = static_cast<int*>(pinned_cache_alloc(64, true));
-      p->ctl.alloc(1, false);   // (filled by the copy below; a cudaMemset on the legacy stream would not be ordered against p->stream)
-    }
-    SolveCtl* c = p->hctl;
-    memset(c, 0, sizeof(SolveCtl));
-    c->tol_p = tol_p; c->tol_d = tol_d; c->tol_gap = prm.tol_gap;
-    c->sense = f.sense; c->offset = f.offset;
-    c->iter_limit = prm.iter_limit; c->interval = interval; c->restart_on = prm.restart != 0; c->world = p->world;
-    *p->htime = (t_lim >= 0 && std::chrono::duration<double>(clk::now() - t_loop).count() > t_lim) ? 1 : 0;
-    {
-      int* dflag = nullptr;
-      CUDA_OK(cudaHostGetDevicePointer(&dflag, p->htime, 0));
-      c->time_flag = t_lim >= 0 ? dflag : nullptr;   // (no limit: spare the device the read over PCIe)
-    }
-    c->term = -1;
-    // dense-check phase (iterations 0 .. kDenseChecks-1 are all check iterations): the passes carry A xSum and A'ySum, the
-    // checks are two vector sweeps.  B200PDLP_LIGHT_CHECK=0: every check multiplies the average iterate by A and A'.
-    const bool hot = warm && warm->col_value && warm->row_value && warm->row_dual;
-    h_light = p->axsum.p && p->atysum.p && (p->world == 1 || !hot);   // (several GPUs: A_g xSum of a hot start would need the gathered xSum)
-    if (const char* e = getenv("B200PDLP_LIGHT_CHECK")) if (atoi(e) == 0) h_light = false;
-    h->light_on = h_light ? 1 : 0;
-    if (h_light) {
-      // xSum starts at proj(0) (PDHG_Init_Variables): without a hot start that IS x, whose product is at hand
-      if (hot) { launch_spmv_plain(s, p->A.dev, p->xsum.p, p->axsum.p); p->launches++; }
-      else CUDA_OK(cudaMemcpyAsync(p->axsum.p, p->ax[0].p, (size_t)std::max(ml, 1) * sizeof(double), cudaMemcpyDeviceToDevice, s));
-      CUDA_OK(cudaMemsetAsync(p->atysum.p, 0, (size_t)std::max(nl, 1) * sizeof(double), s));
-    }
-    if (out->trace && out->trace_cap > 0) {
-      if (p->trace_dev.n < (size_t)out->trace_cap * B200PDLP_TRACE_COLS) p->trace_dev.alloc((size_t)out->trace_cap * B200PDLP_TRACE_COLS, false);
-      c->trace = p->trace_dev.p; c->trace_cap = out->trace_cap;
-    }
-    CUDA_OK(cudaMemcpyAsync(p->ctl.p, c, sizeof(SolveCtl), cudaMemcpyHostToDevice, s));
-    h->stop_iter = 0;   // the first check is due at once (iteration 0)
-    push_state(p);
-    auto next_stop = [&](int it) { return next_check_iter(it, interval, prm.iter_limit); };
-    std::vector<std::unique_ptr<CudaEvent>> evs;
-    int pred_iter = 0, carry = 0;   // carry: passes still owed before the next check (after a re-synchronisation)
-    while (true) {
-      size_t nev = 0;
-      NvtxRange nvtx_batch("b200pdlp: batch of [check, passes] rounds");
-      auto ev = [&]() -> cudaEvent_t {
-        if (nev == evs.size()) evs.emplace_back(new CudaEvent());
-        return *evs[nev++];
-      };
-      int rounds = 0, passes = 0;
-      if (carry > 0) {
-        CUDA_OK(cudaEventRecord(ev(), s));
-        enqueue_passes_device(p, carry);
-        CUDA_OK(cudaEventRecord(ev(), s));
-        passes += carry; pred_iter += carry; carry = 0;
-      }
-      while (rounds < 12 && passes < 48) {
-        // pred_iter never runs behind the device's iteration count, so pred_iter < kDenseChecks implies the device is
-        // inside the dense phase as well (the light kernels check it once more themselves)
-        launch_check_graph(p, h_light && pred_iter < kDenseChecks);
-        rounds++;
-        if (pred_iter >= prm.iter_limit - 1) break;
-        const int next = next_stop(pred_iter);
-        CUDA_OK(cudaEventRecord(ev(), s));
-        enqueue_passes_device(p, next - pred_iter);
-        CUDA_OK(cudaEventRecord(ev(), s));
-        passes += next - pred_iter;
-        pred_iter = next;
-      }
-      CUDA_OK(cudaMemcpyAsync(c, p->ctl.p, sizeof(SolveCtl), cudaMemcpyDeviceToHost, s));
-      CUDA_OK(cudaMemcpyAsync(h, p->state.p, sizeof(PdhgState), cudaMemcpyDeviceToHost, s));
-      int* hfault = reinterpret_cast<int*>(p->hflag + 2);
-      if (p->p2p) CUDA_OK(cudaMemcpyAsync(hfault, p->fault.p, sizeof(int), cudaMemcpyDeviceToHost, s));
-      const size_t npairs = nev / 2;   // events so far come in (before, after) pairs around the passes
-      cudaEvent_t fin = ev();
-      CUDA_OK(cudaEventRecord(fin, s));
-      if (t_lim >= 0) {
-        // poll, so that the time-limit word can be raised while the batch runs
-        while (cudaEventQuery(fin) == cudaErrorNotReady) {
-          if (std::chrono::duration<double>(clk::now() - t_loop).count() > t_lim) *p->htime = 1;
-          std::this_thread::yield();
-        }
-      }
-      CUDA_OK(cudaEventSynchronize(fin));
-      if (p->p2p && *hfault) throw Error(B200PDLP_ERR_STATE, "P2P barrier timed out (a peer rank did not arrive)");
-      for (size_t k = 0; k < npairs; k++) {
-        float ms = 0.f;
-        CUDA_OK(cudaEventElapsedTime(&ms, *evs[2 * k], *evs[2 * k + 1]));
-        iter_ms += ms;
-      }
-      if (c->term >= 0) break;
-      // not finished: continue from where the device really is
-      h_light = h_light && h->light_on != 0;
-      pred_iter = h->iter;
-      carry = std::max(0, h->stop_iter - h->iter);
-    }
-    term = c->term; term_iterate = c->term_iterate; restarts = c->restarts;
-    have_check = c->checks > 0;
-    for (int t = 0; t < 2; t++) {
-      const DevResiduals& d = c->res[t];
-      Residuals& R = chk.it[t];
-      R.pobj = d.pobj; R.dobj = d.dobj; R.pfeas = d.pfeas; R.dfeas = d.dfeas; R.gap = d.gap; R.relgap = d.relgap;
-      R.pinf_obj = d.pinf_obj; R.pinf_res = d.pinf_res; R.dinf_obj = d.dinf_obj; R.dinf_res = d.dinf_res;
-    }
-    if (c->trace) {
-      out->trace_len = std::min(c->trace_len, out->trace_cap);
-      if (out->trace_len > 0)
-        CUDA_OK(cudaMemcpyAsync(out->trace, p->trace_dev.p, (size_t)out->trace_len * B200PDLP_TRACE_COLS * sizeof(double),
-                                cudaMemcpyDeviceToHost, s));
-    }
-  } else
-  // ---- main loop (cupdlp_solver.c:939-1106)
+  CudaEvent ev0, ev1;
   while (h->iter < prm.iter_limit) {
-    const double elapsed = std::chrono::duration<double>(clk::now() - t_loop).count();
-    const bool timed_out_local = t_lim >= 0 && elapsed > t_lim;
-    if (have_spec) { chk = parse_fused_check(p, spec_flag); have_spec = false; }
-    else chk = run_check(p, timed_out_local);
-    have_check = true;
-    const Residuals &L = chk.it[0], &A = chk.it[1];
+    const bool timed_out_local = lim.over();
+    if (have_spec) { o.chk = parse_fused_check(p, spec_flag); have_spec = false; }
+    else o.chk = run_check(p, timed_out_local);
+    o.have_check = true;
+    const Residuals &L = o.chk.it[0], &A = o.chk.it[1];
     if (prm.log_level >= 2)
       printf("[b200pdlp] it %8d  pobj %+.8e dobj %+.8e  pfeas %.2e dfeas %.2e | avg pobj %+.8e dobj %+.8e pfeas %.2e dfeas %.2e  tau %.3e sigma %.3e\n",
              h->iter, L.pobj, L.dobj, L.pfeas, L.dfeas, A.pobj, A.dobj, A.pfeas, A.dfeas, h->tau, h->sigma);
     int choice = 0;
-    const int t_code = check_decision(prm, tol_p, tol_d, h, chk, memo, &term_iterate, &choice);
-    if (t_code >= 0) { term = t_code; trace_row(out, h, chk, 0); break; }
-    bool dirty = false;
-    if (choice) { do_restart(p, choice, chk, memo); restarts++; arm_step(h); dirty = true; }
-    trace_row(out, h, chk, choice);
-    const int next = next_check_iter(h->iter, interval, prm.iter_limit);
+    const int t_code = check_decision(prm, lim.tol_p, lim.tol_d, h, o.chk, memo, &o.term_iterate, &choice);
+    if (t_code >= 0) { o.term = t_code; trace_row(out, h, o.chk, 0); break; }
+    if (choice) { do_restart(p, choice, o.chk, memo); o.restarts++; arm_step(h); }
+    trace_row(out, h, o.chk, choice);
+    const int next = next_check_iter(h->iter, lim.interval, prm.iter_limit);
     h->stop_iter = next;
     fill_pow_tables(h);
-    dirty = true;
-    if (dirty) push_state(p);
+    push_state(p);
     CUDA_OK(cudaEventRecord(ev0, s));
     bool have_ev1 = false;
     while (true) {
       const int need = next - h->iter;
       if (p->no_graph) {
-        for (int q = 0; q < std::min(need + 4, p->graph_main_passes); q++) { enqueue_pass(p); p->launches += p->kernels_per_pass; }
+        for (int q = 0; q < std::min(need + 4, p->graph_main_passes); q++) { enqueue_pass(p); p->launches += p->kernels_per_pass(); }
       } else if (need >= p->graph_main_passes / 2 || need > p->graph_small_passes) {
         CUDA_OK(cudaGraphLaunch(p->graph_main, s));
-        p->launches += (long long)p->graph_main_passes * p->kernels_per_pass;
+        p->launches += (long long)p->graph_main_passes * p->kernels_per_pass();
       } else if (need > 1) {
         CUDA_OK(cudaGraphLaunch(p->graph_small, s));
-        p->launches += (long long)p->graph_small_passes * p->kernels_per_pass;
+        p->launches += (long long)p->graph_small_passes * p->kernels_per_pass();
       } else {
         enqueue_pass(p);
-        p->launches += p->kernels_per_pass;
+        p->launches += p->kernels_per_pass();
       }
       if (speculate) {
         if (!have_ev1) { CUDA_OK(cudaEventRecord(ev1, s)); have_ev1 = true; }
-        const double el = std::chrono::duration<double>(clk::now() - t_loop).count();
-        spec_flag = t_lim >= 0 && el > t_lim;
+        spec_flag = lim.over();
         enqueue_check_dev(p, spec_flag);
       }
       pull_state(p);
@@ -1606,36 +1629,129 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
     CUDA_OK(cudaEventSynchronize(ev1));
     float ms = 0.f;
     CUDA_OK(cudaEventElapsedTime(&ms, ev0, ev1));
-    iter_ms += ms;
+    o.iter_ms += ms;
   }
-  CUDA_OK(cudaEventRecord(evl1, s));
-  CUDA_OK(cudaEventSynchronize(evl1));
-  float loop_ms = 0.f;
-  CUDA_OK(cudaEventElapsedTime(&loop_ms, evl0, evl1));
-  const double solve_seconds = std::chrono::duration<double>(clk::now() - t_loop).count();
-  out->loop_device_ms = loop_ms;
-  lap("solve", "iterations");
-  nvtxRangePop();
-  NvtxRange nvtx_post("b200pdlp: postsolve + download");
+  return o;
+}
 
-  if (p->world > 1 && getenv("B200PDLP_DEBUG_MG")) {
-    // diagnostics: per-rank barrier / exchange counts and checksums of what the postsolve is about to assemble
-    unsigned long long ep[16] = {0};
-    if (p->epochs.p) CUDA_OK(cudaMemcpy(ep, p->epochs.p, sizeof(ep), cudaMemcpyDeviceToHost));
-    auto csum = [&](const double* d, int len) {
-      std::vector<double> t(std::max(len, 1));
-      if (len > 0) CUDA_OK(cudaMemcpy(t.data(), d, (size_t)len * sizeof(double), cudaMemcpyDeviceToHost));
-      double a = 0.0; for (int i = 0; i < len; i++) a += t[i] * (1.0 + (i % 7)); return a;
-    };
-    fprintf(stderr, "[b200pdlp mg-debug] rank %d iter %d cur %d term %d term_iterate %d light_on %d | barrier0 %llu barrier1 %llu exchange %llu | "
-            "x[cur] %.17g xavg %.17g y[cur] %.17g yavg %.17g ax[cur] %.17g axavg %.17g aty0 %.17g atyavg %.17g\n",
-            p->rank, h->iter, h->cur, term, term_iterate, h->light_on, ep[0], ep[1], ep[10],
-            csum(p->x[h->cur].p, p->nl), csum(p->xavg.p, p->nl), csum(p->y[h->cur].p, ml), csum(p->yavg.p, ml),
-            csum(p->ax[h->cur].p, ml), csum(p->axavg.p, ml), csum(p->aty[0].p, p->nl), csum(p->atyavg.p, p->nl));
+// B200PDLP_DEBUG_MG: per-rank barrier / exchange counts and checksums of what the postsolve is about to assemble
+static void debug_mg_dump(b200pdlp_problem* p, const LoopOutcome& o) {
+  const PdhgState* h = p->hstate;
+  const int ml = p->ml;
+  unsigned long long ep[16] = {0};
+  if (p->epochs.p) CUDA_OK(cudaMemcpy(ep, p->epochs.p, sizeof(ep), cudaMemcpyDeviceToHost));
+  auto csum = [&](const double* d, int len) {
+    std::vector<double> t(std::max(len, 1));
+    if (len > 0) CUDA_OK(cudaMemcpy(t.data(), d, (size_t)len * sizeof(double), cudaMemcpyDeviceToHost));
+    double a = 0.0; for (int i = 0; i < len; i++) a += t[i] * (1.0 + (i % 7)); return a;
+  };
+  fprintf(stderr, "[b200pdlp mg-debug] rank %d iter %d cur %d term %d term_iterate %d light_on %d | barrier0 %llu barrier1 %llu exchange %llu | "
+          "x[cur] %.17g xavg %.17g y[cur] %.17g yavg %.17g ax[cur] %.17g axavg %.17g aty0 %.17g atyavg %.17g\n",
+          p->rank, h->iter, h->cur, o.term, o.term_iterate, h->light_on, ep[0], ep[1], ep[10],
+          csum(p->x[h->cur].p, p->nl), csum(p->xavg.p, p->nl), csum(p->y[h->cur].p, ml), csum(p->yavg.p, ml),
+          csum(p->ax[h->cur].p, ml), csum(p->axavg.p, ml), csum(p->aty[0].p, p->nl), csum(p->atyavg.p, p->nl));
+}
+
+// device order -> standard-form order, whole vectors on every rank.
+// Logical shards share ONE CUDA context: a context-synchronising driver call on one rank's host thread (a pageable copy
+// that needs staging memory, a lazy module load, an allocation) waits for every running kernel, including a peer's
+// barrier kernel that is spinning for THIS rank's next launch -- a deadlock that only the barrier's timeout breaks
+// (and the assembly would then run on with stale segments).  So with local links every host-blocking copy
+// of the assembly sits between two host-side rendezvous, when no barrier kernel is in flight.  Separate processes
+// (CUDA IPC) have separate contexts and do not need this.
+struct Assembly {
+  b200pdlp_problem* p;
+  std::vector<double> t = std::vector<double>(std::max<size_t>(std::max(p->n, std::max(p->ml, 1)), p->xfull.n));   // staging
+  const bool dbg = p->world > 1 && getenv("B200PDLP_DEBUG_MG") != nullptr, rendezvous = p->local_link && p->group;
+  int dbg_stage = 0;
+  void dbg_segments(const char* what) {
+    if (!dbg) return;
+    char line[1024]; int k = snprintf(line, sizeof line, "[b200pdlp mg-debug] rank %d stage %d %s segments:", p->rank, dbg_stage++, what);
+    for (int g = 0; g < p->world && k < 900; g++) {
+      double a = 0.0;
+      for (int i = 0; i < p->seg_len; i++) a += t[(size_t)g * p->seg_len + i] * (1.0 + (i % 7));
+      k += snprintf(line + k, sizeof line - k, " %.15g", a);
+    }
+    fprintf(stderr, "%s\n", line);
   }
-  // ---- PDHG_PostSolve (cupdlp_solver.c:1281-1435)
-  const int cur = h->cur;
-  const bool use_avg = (term == B200PDLP_OPTIMAL && term_iterate == 1);
+  // barrier of the assembly; with local links the ranks also meet on the host before AND after it (see above): nobody
+  // launches a kernel that spins for its peers while a peer's host may still sit in a blocking copy, and nobody starts a
+  // blocking copy while a peer's barrier kernel is still in flight
+  void xchg() {
+    cudaStream_t s = p->stream;
+    if (rendezvous) { CUDA_OK(cudaStreamSynchronize(s)); p->group->arrive_and_wait(); }
+    launch_p2p_exchange(s, p->outs.p + 60, 0, p->peers, p->world, p->rank, p->epochs.p, p->fault.p);
+    p->launches++;
+    if (rendezvous) { CUDA_OK(cudaStreamSynchronize(s)); p->group->arrive_and_wait(); }
+  }
+  // this rank's column shard d -> h, the whole column vector
+  void download_cols(const double* d, std::vector<double>& h) {
+    cudaStream_t s = p->stream;
+    const bool peers = p->world > 1 && p->p2p && !p->comm;
+    if (peers) {
+      // no NCCL communicator (logical shards of one process, or B200PDLP_NO_NCCL): all-gather through the peers' xfull,
+      // with a barrier before anyone reads and one before anyone overwrites
+      launch_push_shard(s, d, p->nl, p->peers, p->world, p->rank, p->seg_len);
+      p->launches++;
+      xchg();
+      CUDA_OK(cudaMemcpyAsync(t.data(), p->xfull.p, p->xfull.n * sizeof(double), cudaMemcpyDeviceToHost, s));
+      xchg();
+    } else if (p->world > 1) {   // all-gather the column shards
+      CUDA_OK(cudaMemcpyAsync(p->send.p, d, (size_t)p->nl * sizeof(double), cudaMemcpyDeviceToDevice, s));
+      gather_shards(p);
+      CUDA_OK(cudaMemcpyAsync(t.data(), p->xfull.p, p->xfull.n * sizeof(double), cudaMemcpyDeviceToHost, s));
+    } else {
+      CUDA_OK(cudaMemcpyAsync(t.data(), d, (size_t)p->n * sizeof(double), cudaMemcpyDeviceToHost, s));
+    }
+    CUDA_OK(cudaStreamSynchronize(s));
+    if (peers) dbg_segments("columns");
+    for (int j = 0; j < p->n; j++) h[p->cperm[j]] = t[seg_pos(p, j)];   // (several GPUs: a segmented vector)
+  }
+  // this rank's rows d -> h, the whole row vector
+  void download_rows(const double* d, std::vector<double>& h) {
+    cudaStream_t s = p->stream;
+    const int m = p->m, ml = p->ml;
+    if (ml) CUDA_OK(cudaMemcpyAsync(t.data(), d, (size_t)ml * sizeof(double), cudaMemcpyDeviceToHost, s));
+    CUDA_OK(cudaStreamSynchronize(s));
+    for (int i = 0; i < ml; i++) h[p->r0 + p->rperm[i]] = t[i];
+    if (p->world > 1 && p->p2p && !p->comm) {
+      // no NCCL communicator: every rank stores its rows (standard-form order) into slot `rank` of every peer's
+      // receive buffer, seg_len rows at a time; all ranks run the same number of rounds
+      int max_ml = 0;
+      for (int g = 0; g < p->world; g++) max_ml = std::max(max_ml, p->row_bounds[g + 1] - p->row_bounds[g]);
+      if (ml) CUDA_OK(cudaMemcpyAsync(p->redbuf.p, h.data() + p->r0, (size_t)ml * sizeof(double), cudaMemcpyHostToDevice, s));
+      const int rounds = (max_ml + p->seg_len - 1) / p->seg_len;
+      for (int c = 0; c < rounds; c++) {
+        const int off = c * p->seg_len;
+        launch_push_rows(s, p->redbuf.p + off, std::max(0, std::min(ml - off, p->seg_len)), p->peers, p->world, p->rank, p->seg_len);
+        p->launches++;
+        xchg();
+        CUDA_OK(cudaMemcpyAsync(t.data(), p->recv.p, (size_t)p->world * p->seg_len * sizeof(double), cudaMemcpyDeviceToHost, s));
+        xchg();
+        CUDA_OK(cudaStreamSynchronize(s));
+        dbg_segments("rows");
+        for (int g = 0; g < p->world; g++) {
+          const int mg = p->row_bounds[g + 1] - p->row_bounds[g];
+          const int cnt = std::max(0, std::min(mg - off, p->seg_len));
+          for (int i = 0; i < cnt; i++) h[p->row_bounds[g] + off + i] = t[(size_t)g * p->seg_len + i];
+        }
+      }
+    } else if (p->world > 1) {   // other ranks' rows: zero-padded sum
+      CUDA_OK(cudaMemcpyAsync(p->redbuf.p, h.data(), (size_t)m * sizeof(double), cudaMemcpyHostToDevice, s));
+      allreduce_inplace(p, p->redbuf.p, m);
+      CUDA_OK(cudaMemcpyAsync(h.data(), p->redbuf.p, (size_t)m * sizeof(double), cudaMemcpyDeviceToHost, s));
+      CUDA_OK(cudaStreamSynchronize(s));
+    }
+  }
+};
+
+// PDHG_PostSolve (cupdlp_solver.c:1281-1435), on the device (device_prep.cu post_*_kernel) or on the host
+static void write_solution(b200pdlp_problem* p, const LoopOutcome& o, b200pdlp_result* out, Laps& lap) {
+  const StdForm& f = p->form;
+  cudaStream_t s = p->stream;
+  const PdhgState* h = p->hstate;
+  const int cur = h->cur, nl = p->nl, m = p->m;
+  const bool use_avg = (o.term == B200PDLP_OPTIMAL && o.term_iterate == 1);
   const double* dx = use_avg ? p->xavg.p : p->x[cur].p;
   const double* dy = use_avg ? p->yavg.p : p->y[cur].p;
   const double* dax = use_avg ? p->axavg.p : p->ax[cur].p;
@@ -1643,138 +1759,97 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
     if (p->p2p) launch_reduce_part_p2p(s, nl, p->aty[0].p, p->peers, p->world, p->rank, p->seg_len, 1);
     else CUDA_OK(cudaMemcpyAsync(p->aty[0].p, p->red.p, (size_t)nl * sizeof(double), cudaMemcpyDeviceToDevice, s));
   }
-  if (p->p2p) {
-    int fault = 0;
-    CUDA_OK(cudaMemcpyAsync(&fault, p->fault.p, sizeof(int), cudaMemcpyDeviceToHost, s));
-    CUDA_OK(cudaStreamSynchronize(s));
-    if (fault) throw Error(B200PDLP_ERR_STATE, "P2P barrier timed out (a peer rank did not arrive)");
-  }
+  throw_if_peer_fault(p, kPeerLate);
   const double* daty = use_avg ? p->atyavg.p : p->aty[p->world == 1 ? cur : 0].p;
-  if (dev_form) {
-    // PDHG_PostSolve on the device (device_prep.cu post_*_kernel): un-permute, un-scale, sign conventions, slacks of
-    // BOUND rows; four original-order vectors come back
-    if (out->col_value && out->col_dual && out->row_value && out->row_dual && p->device_io) {
-      launch_postsolve(s, p->prep.arr, f.sense, have_check ? 1 : 0, dx, daty, dy, dax, p->cost.p, p->lower.p, p->upper.p,
-                       p->colscale.p, p->rowscale.p, out->col_value, out->col_dual, out->row_value, out->row_dual);
-      p->launches += 2;
-    } else if (out->col_value && out->col_dual && out->row_value && out->row_dual) {
+  if (p->dev_form) {
+    // un-permute, un-scale, sign conventions, slacks of BOUND rows; four original-order vectors come back
+    if (out->col_value && out->col_dual && out->row_value && out->row_dual) {
       const int n0 = f.n_orig;
-      launch_postsolve(s, p->prep.arr, f.sense, have_check ? 1 : 0, dx, daty, dy, dax, p->cost.p, p->lower.p, p->upper.p,
-                       p->colscale.p, p->rowscale.p, p->io_col.p, p->io_col.p + n0, p->io_row.p, p->io_row.p + m);
+      const bool direct = p->device_io;
+      launch_postsolve(s, p->prep.arr, f.sense, o.have_check ? 1 : 0, dx, daty, dy, dax, p->cost.p, p->lower.p, p->upper.p,
+                       p->colscale.p, p->rowscale.p, direct ? out->col_value : p->io_col.p, direct ? out->col_dual : p->io_col.p + n0,
+                       direct ? out->row_value : p->io_row.p, direct ? out->row_dual : p->io_row.p + m);
       p->launches += 2;
-      CUDA_OK(cudaMemcpyAsync(out->col_value, p->io_col.p, (size_t)n0 * sizeof(double), cudaMemcpyDeviceToHost, s));
-      CUDA_OK(cudaMemcpyAsync(out->col_dual, p->io_col.p + n0, (size_t)n0 * sizeof(double), cudaMemcpyDeviceToHost, s));
-      CUDA_OK(cudaMemcpyAsync(out->row_value, p->io_row.p, (size_t)m * sizeof(double), cudaMemcpyDeviceToHost, s));
-      CUDA_OK(cudaMemcpyAsync(out->row_dual, p->io_row.p + m, (size_t)m * sizeof(double), cudaMemcpyDeviceToHost, s));
+      if (!direct) {
+        CUDA_OK(cudaMemcpyAsync(out->col_value, p->io_col.p, (size_t)n0 * sizeof(double), cudaMemcpyDeviceToHost, s));
+        CUDA_OK(cudaMemcpyAsync(out->col_dual, p->io_col.p + n0, (size_t)n0 * sizeof(double), cudaMemcpyDeviceToHost, s));
+        CUDA_OK(cudaMemcpyAsync(out->row_value, p->io_row.p, (size_t)m * sizeof(double), cudaMemcpyDeviceToHost, s));
+        CUDA_OK(cudaMemcpyAsync(out->row_dual, p->io_row.p + m, (size_t)m * sizeof(double), cudaMemcpyDeviceToHost, s));
+      }
     }
     CUDA_OK(cudaStreamSynchronize(s));
     lap("solve", "postsolve (device) + download");
-  } else {
-  std::vector<double> hx(n), hy(m, 0.0), hax(m, 0.0), haty(n);
-  {
-    // device order -> standard-form order
-    std::vector<double> t(std::max<size_t>(std::max(n, std::max(ml, 1)), p->xfull.n));
-    const bool dbg = p->world > 1 && getenv("B200PDLP_DEBUG_MG") != nullptr;
-    // Logical shards share ONE CUDA context: a context-synchronising driver call on one rank's host thread (a pageable copy
-    // that needs staging memory, a lazy module load, an allocation) waits for every running kernel, including a peer's
-    // barrier kernel that is spinning for THIS rank's next launch -- a deadlock that only the barrier's timeout breaks
-    // (and the assembly would then run on with stale segments).  So with local links every host-blocking copy
-    // of the assembly sits between two host-side rendezvous, when no barrier kernel is in flight.  Separate processes
-    // (CUDA IPC) have separate contexts and do not need this.
-    const bool rendezvous = p->local_link && p->group;
-    int dbg_stage = 0;
-    auto dbg_segments = [&](const char* what) {
-      if (!dbg) return;
-      char line[1024]; int k = snprintf(line, sizeof line, "[b200pdlp mg-debug] rank %d stage %d %s segments:", p->rank, dbg_stage++, what);
-      for (int g = 0; g < p->world && k < 900; g++) {
-        double a = 0.0;
-        for (int i = 0; i < p->seg_len; i++) a += t[(size_t)g * p->seg_len + i] * (1.0 + (i % 7));
-        k += snprintf(line + k, sizeof line - k, " %.15g", a);
-      }
-      fprintf(stderr, "%s\n", line);
-    };
-    // barrier of the assembly; with local links the ranks also meet on the host before AND after it (see above): nobody
-    // launches a kernel that spins for its peers while a peer's host may still sit in a blocking copy, and nobody starts a
-    // blocking copy while a peer's barrier kernel is still in flight
-    auto xchg = [&]() {
-      if (rendezvous) { CUDA_OK(cudaStreamSynchronize(s)); p->group->arrive_and_wait(); }
-      launch_p2p_exchange(s, p->outs.p + 60, 0, p->peers, p->world, p->rank, p->epochs.p, p->fault.p);
-      p->launches++;
-      if (rendezvous) { CUDA_OK(cudaStreamSynchronize(s)); p->group->arrive_and_wait(); }
-    };
-    auto down_col = [&](const double* d, std::vector<double>& h) {
-      if (p->world == 1) {
-        CUDA_OK(cudaMemcpyAsync(t.data(), d, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, s));
-        CUDA_OK(cudaStreamSynchronize(s));
-        for (int j = 0; j < n; j++) h[p->cperm[j]] = t[j];
-      } else if (p->p2p && !p->comm) {
-        // no NCCL communicator (logical shards of one process, or B200PDLP_NO_NCCL): all-gather through the peers' xfull,
-        // with a barrier before anyone reads and one before anyone overwrites
-        launch_push_shard(s, d, nl, p->peers, p->world, p->rank, p->seg_len);
-        p->launches++;
-        xchg();
-        CUDA_OK(cudaMemcpyAsync(t.data(), p->xfull.p, p->xfull.n * sizeof(double), cudaMemcpyDeviceToHost, s));
-        xchg();
-        CUDA_OK(cudaStreamSynchronize(s));
-        dbg_segments("columns");
-        for (int j = 0; j < n; j++) h[p->cperm[j]] = t[seg_pos(p, j)];
-      } else {   // all-gather the column shards, then unpack the segmented vector
-        CUDA_OK(cudaMemcpyAsync(p->send.p, d, (size_t)nl * sizeof(double), cudaMemcpyDeviceToDevice, s));
-        gather_shards(p);
-        CUDA_OK(cudaMemcpyAsync(t.data(), p->xfull.p, p->xfull.n * sizeof(double), cudaMemcpyDeviceToHost, s));
-        CUDA_OK(cudaStreamSynchronize(s));
-        for (int j = 0; j < n; j++) h[p->cperm[j]] = t[seg_pos(p, j)];
-      }
-    };
-    auto down_row = [&](const double* d, std::vector<double>& h) {
-      if (ml) CUDA_OK(cudaMemcpyAsync(t.data(), d, (size_t)ml * sizeof(double), cudaMemcpyDeviceToHost, s));
-      CUDA_OK(cudaStreamSynchronize(s));
-      for (int i = 0; i < ml; i++) h[p->r0 + p->rperm[i]] = t[i];
-      if (p->world > 1 && p->p2p && !p->comm) {
-        // no NCCL communicator: every rank stores its rows (standard-form order) into slot `rank` of every peer's
-        // receive buffer, seg_len rows at a time; all ranks run the same number of rounds
-        int max_ml = 0;
-        for (int g = 0; g < p->world; g++) max_ml = std::max(max_ml, p->row_bounds[g + 1] - p->row_bounds[g]);
-        if (ml) CUDA_OK(cudaMemcpyAsync(p->redbuf.p, h.data() + p->r0, (size_t)ml * sizeof(double), cudaMemcpyHostToDevice, s));
-        const int rounds = (max_ml + p->seg_len - 1) / p->seg_len;
-        for (int c = 0; c < rounds; c++) {
-          const int off = c * p->seg_len;
-          launch_push_rows(s, p->redbuf.p + off, std::max(0, std::min(ml - off, p->seg_len)), p->peers, p->world, p->rank, p->seg_len);
-          p->launches++;
-          xchg();
-          CUDA_OK(cudaMemcpyAsync(t.data(), p->recv.p, (size_t)p->world * p->seg_len * sizeof(double), cudaMemcpyDeviceToHost, s));
-          xchg();
-          CUDA_OK(cudaStreamSynchronize(s));
-          dbg_segments("rows");
-          for (int g = 0; g < p->world; g++) {
-            const int mg = p->row_bounds[g + 1] - p->row_bounds[g];
-            const int cnt = std::max(0, std::min(mg - off, p->seg_len));
-            for (int i = 0; i < cnt; i++) h[p->row_bounds[g] + off + i] = t[(size_t)g * p->seg_len + i];
-          }
-        }
-      } else if (p->world > 1) {   // other ranks' rows: zero-padded sum
-        CUDA_OK(cudaMemcpyAsync(p->redbuf.p, h.data(), (size_t)m * sizeof(double), cudaMemcpyHostToDevice, s));
-        allreduce_inplace(p, p->redbuf.p, m);
-        CUDA_OK(cudaMemcpyAsync(h.data(), p->redbuf.p, (size_t)m * sizeof(double), cudaMemcpyDeviceToHost, s));
-        CUDA_OK(cudaStreamSynchronize(s));
-      }
-    };
-    down_col(dx, hx); down_col(daty, haty); down_row(dy, hy); down_row(dax, hax);
-    if (p->p2p) {   // a barrier of the assembly that timed out leaves stale segments behind: an error, not a result
-      int fault = 0;
-      CUDA_OK(cudaMemcpyAsync(&fault, p->fault.p, sizeof(int), cudaMemcpyDeviceToHost, s));
-      CUDA_OK(cudaStreamSynchronize(s));
-      if (fault) throw Error(B200PDLP_ERR_STATE, "P2P barrier timed out while the solution was being assembled (a peer rank did not arrive)");
-    }
+    return;
   }
+  std::vector<double> hx(p->n), hy(m, 0.0), hax(m, 0.0), haty(p->n);
+  {
+    Assembly a{p};
+    a.download_cols(dx, hx); a.download_cols(daty, haty); a.download_rows(dy, hy); a.download_rows(dax, hax);
+  }
+  // a barrier of the assembly that timed out leaves stale segments behind: an error, not a result
+  throw_if_peer_fault(p, "P2P barrier timed out while the solution was being assembled (a peer rank did not arrive)");
   lap("solve", "solution download");
-  host_postsolve(f, have_check, hx, hy, hax, haty, out);
-  }   // host postsolve
-  fill_result(out, f, h, term, term_iterate, restarts, chk);
+  host_postsolve(f, o.have_check, hx, hy, hax, haty, out);
+}
+
+static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, const b200pdlp_warm* warm, b200pdlp_result* out) {
+  NvtxRange nvtx("b200pdlp: solve");
+  nvtxRangePushA("b200pdlp: initial point + graphs");
+  using clk = std::chrono::steady_clock;
+  set_device(p);
+  const auto t_begin = clk::now();
+  const StdForm& f = p->form;
+  const int interval = prm.check_interval > 0 ? prm.check_interval : 40;
+  const bool dev_checks = use_device_checks(p, prm);
+  const bool logical_shards = p->local_link && p->group;
+  const long long launches0 = p->launches;
+  PdhgState* h = p->hstate;
+  memset(h, 0, sizeof(PdhgState));
+  h->adaptive = prm.adaptive_step != 0;
+  out->trace_len = 0;
+  Laps lap;
+  lap.rank = p->world > 1 ? p->rank : -1;
+  if (logical_shards) {
+    prepare_graphs(p, prm, interval, dev_checks, /*eager=*/true);
+    CUDA_OK(cudaStreamSynchronize(p->stream));
+    lap("solve", "graphs ready (logical shards)");
+    p->group->arrive_and_wait();
+  }
+  start_point(p, warm);
+  init_step_sizes(p, h);
+  start_products_and_sums(p);
+  arm_step(h);
+  fill_pow_tables(h);
+  push_state(p);
+  CUDA_OK(cudaStreamSynchronize(p->stream));
+  lap("solve", "initial point + state");
+  if (!logical_shards) prepare_graphs(p, prm, interval, dev_checks, /*eager=*/false);
+  lap("solve", "graph capture");
+  nvtxRangePop();
+
+  nvtxRangePushA("b200pdlp: PDHG loop");
+  CudaEvent evl0, evl1;
+  CUDA_OK(cudaEventRecord(evl0, p->stream));
+  const LoopLimits lim{interval, prm.tol_primal * (1.0 + f.norm_rhs), prm.tol_dual * (1.0 + f.norm_cost),
+                       time_limit_or_none(prm.time_limit), clk::now()};
+  const LoopOutcome o = dev_checks ? device_loop(p, prm, warm, lim, out) : host_loop(p, prm, lim, out);
+  CUDA_OK(cudaEventRecord(evl1, p->stream));
+  CUDA_OK(cudaEventSynchronize(evl1));
+  float loop_ms = 0.f;
+  CUDA_OK(cudaEventElapsedTime(&loop_ms, evl0, evl1));
+  const double solve_seconds = lim.elapsed();
+  out->loop_device_ms = loop_ms;
+  lap("solve", "iterations");
+  nvtxRangePop();
+
+  NvtxRange nvtx_post("b200pdlp: postsolve + download");
+  if (p->world > 1 && getenv("B200PDLP_DEBUG_MG")) debug_mg_dump(p, o);
+  write_solution(p, o, out, lap);
+  fill_result(out, f, h, o.term, o.term_iterate, o.restarts, o.chk);
   out->kernel_launches = (int)std::min<long long>(p->launches - launches0, 2147483647LL);
   out->solve_seconds = solve_seconds;
-  out->iter_device_ms = iter_ms;
-  out->setup_seconds += std::chrono::duration<double>(t_loop - t_begin).count();
+  out->iter_device_ms = o.iter_ms;
+  out->setup_seconds += std::chrono::duration<double>(lim.t_loop - t_begin).count();
   lap("solve", "postsolve (host)");
 }
 
@@ -2165,26 +2240,14 @@ int b200pdlp_check_device(b200pdlp_problem* p, const b200pdlp_check_in* in, doub
     h->pow_base = -1;
     h->stop_iter = in->iter; h->cur = 0; h->light_on = light ? 1 : 0; h->done = 0;
     push_state(p);
-    if (!p->hctl) {
-      p->hctl = static_cast<SolveCtl*>(pinned_cache_alloc(sizeof(SolveCtl), false));
-      p->htime = static_cast<int*>(pinned_cache_alloc(64, true));
-      p->ctl.alloc(1, false);
-    }
     if (p->trace_dev.n < (size_t)B200PDLP_TRACE_COLS) p->trace_dev.alloc(B200PDLP_TRACE_COLS, false);
     CUDA_OK(cudaMemsetAsync(p->trace_dev.p, 0, B200PDLP_TRACE_COLS * sizeof(double), s));
-    SolveCtl* c = p->hctl;
-    memset(c, 0, sizeof(SolveCtl));
-    c->tol_p = in->tol_p; c->tol_d = in->tol_d; c->tol_gap = in->tol_gap;
-    c->sense = p->form.sense; c->offset = p->form.offset;
-    c->iter_limit = in->iter_limit; c->interval = in->interval; c->restart_on = in->restart_on != 0; c->world = 1;
+    SolveCtl* c = reset_ctl(p, in->tol_p, in->tol_d, in->tol_gap, in->iter_limit, in->interval, in->restart_on != 0);
     *p->htime = in->time_flag;
-    int* dflag = nullptr;
-    CUDA_OK(cudaHostGetDevicePointer(&dflag, p->htime, 0));
-    c->time_flag = dflag;
+    c->time_flag = mapped_time_flag(p);
     c->pf_lr = in->pf_lr; c->df_lr = in->df_lr; c->gap_lr = in->gap_lr;
     c->pf_lc = in->pf_lc; c->df_lc = in->df_lc; c->gap_lc = in->gap_lc;
     c->last_restart_iter = in->last_restart_iter;
-    c->term = -1;
     c->trace = p->trace_dev.p; c->trace_cap = 1;
     CUDA_OK(cudaMemcpyAsync(p->ctl.p, c, sizeof(SolveCtl), cudaMemcpyHostToDevice, s));
     p->launches += enqueue_check_device(p, light);
@@ -2257,7 +2320,6 @@ int b200pdlp_bench_pass(b200pdlp_problem* p, int32_t reps, float ms[4]) {
     set_device(p);
     cudaStream_t s = p->stream;
     PdhgState* st = p->state.p;
-    p->kernels_per_pass = p->world == 1 ? 4 : (p->p2p ? 5 : 6);
     pull_state(p);
     p->hstate->stop_iter = 2147483647;
     fill_pow_tables(p->hstate);
@@ -2299,7 +2361,7 @@ int b200pdlp_bench_pass(b200pdlp_problem* p, int32_t reps, float ms[4]) {
                              p->epochs.p, p->fault.p);
           CUDA_OK(cudaEventRecord(ev[4], s));
           CUDA_OK(cudaEventSynchronize(ev[4]));
-          p->launches += p->kernels_per_pass;
+          p->launches += p->kernels_per_pass();
           for (int k = 0; k < 4; k++) { float t = 0.f; CUDA_OK(cudaEventElapsedTime(&t, ev[k], ev[k + 1])); acc[k] += t; }
           continue;
         }
@@ -2320,7 +2382,7 @@ int b200pdlp_bench_pass(b200pdlp_problem* p, int32_t reps, float ms[4]) {
       }
       CUDA_OK(cudaEventRecord(ev[4], s));
       CUDA_OK(cudaEventSynchronize(ev[4]));
-      p->launches += p->kernels_per_pass;
+      p->launches += p->kernels_per_pass();
       for (int k = 0; k < 4; k++) {
         float t = 0.f;
         CUDA_OK(cudaEventElapsedTime(&t, ev[k], ev[k + 1]));
@@ -2370,40 +2432,11 @@ int b200pdlp_solve_device(const b200pdlp_lp* lp, const b200pdlp_params* params, 
   return guarded([&] {
     if (!lp || !params || !out) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": null argument");
     check_params(*params);
-    if (!lp_fields_ok(lp)) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": b200pdlp: malformed b200pdlp_lp");
-    if (lp->sense != 1.0 && lp->sense != -1.0) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": b200pdlp: sense must be +1 or -1");
-    const int device = select_device(params->device);
-    check_device_lp(*lp, device, -1, who);
-    if (warm) {
-      check_device_array(warm->col_value, device, -1, "warm col_value", who);
-      check_device_array(warm->row_value, device, -1, "warm row_value", who);
-      check_device_array(warm->row_dual, device, -1, "warm row_dual", who);
-    }
-    check_device_result(*out, device, -1, who);
-    const auto t0 = std::chrono::steady_clock::now();
     b200pdlp_params prm = *params;
-    prm.device = device;
-    ProblemPtr p(new b200pdlp_problem());   // its stream serves the sizing and, in tree mode, the solve
-    open_problem(p.get(), device, 0, 1);
-    int nnz = 0;
-    const DeviceRoute route = device_lp_route(p->stream, *lp, false, prm.ordered_max, who, &nnz);
-    if (route == DeviceRoute::Ordered) {
-      solve_batch_device(1, lp, prm, warm, out);
-    } else if (route == DeviceRoute::Degenerate) {
-      solve_degenerate(p->stream, *lp, warm, out, [&](const b200pdlp_lp& hl, const b200pdlp_warm* hw, b200pdlp_result* r) {
-        ProblemPtr q(new b200pdlp_problem());
-        create_problem(hl, prm, 0, 1, q.get());
-        r->setup_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-        solve_on_device(q.get(), prm, hw, r);
-      });
-    } else {
-      p->device_io = true;
-      p->prep.inputs_on_device = true;
-      p->prep.device_nnz = nnz;
-      create_problem_device(*lp, prm, p.get());
-      out->setup_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-      solve_on_device(p.get(), prm, warm, out);
-    }
+    solve_lp_device(*lp, false, prm.device, prm.ordered_max, warm, out, who, [&] { solve_batch_device(1, lp, prm, warm, out); },
+                    [&](const b200pdlp_lp& l, b200pdlp_problem* q) { create_problem(l, prm, 0, 1, q); },
+                    [&](const b200pdlp_lp& l, b200pdlp_problem* q) { create_problem_device(l, prm, q); },
+                    [&](b200pdlp_problem* q, const b200pdlp_lp&, const b200pdlp_warm* w, b200pdlp_result* r) { solve_on_device(q, prm, w, r); });
     CUDA_OK(cudaGetLastError());
   });
 }

@@ -288,7 +288,7 @@ struct b200pdlp_problem {
   cudaGraphExec_t graph_check_light = nullptr;   // the dense-check phase's check: two sweeps instead of two SpMV (see kDenseChecks)
   DevBuf<double> axsum, atysum;                   // A xSum (ml), A'ySum (n): carried by the passes while iter < kDenseChecks
   long long launches = 0;
-  int kernels_per_pass = 4;
+  int kernels_per_pass() const { return world == 1 ? 4 : (p2p ? 5 : 6); }   // of a PDHG pass: ours, NCCL's not counted
 
   ~b200pdlp_problem() {
     if (stream) cudaStreamSynchronize(stream);   // the buffers go back to the block cache: nothing may still use them
@@ -400,6 +400,19 @@ void run_per_rank(int count, const char* label, F&& fn, const int* ids = nullptr
     if (codes[i] != B200PDLP_OK) throw Error(codes[i], std::string(label) + " " + std::to_string(ids ? ids[i] : i) + ": " + msgs[i]);
 }
 
+// the work enqueue() puts on stream s, captured (thread-local mode) and instantiated
+template <class F>
+cudaGraphExec_t capture_graph(cudaStream_t s, F&& enqueue) {
+  cudaGraph_t g = nullptr;
+  cudaGraphExec_t ge = nullptr;
+  CUDA_OK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+  enqueue();
+  CUDA_OK(cudaStreamEndCapture(s, &g));
+  CUDA_OK(cudaGraphInstantiate(&ge, g, 0));
+  CUDA_OK(cudaGraphDestroy(g));
+  return ge;
+}
+
 // owning handle of a problem: deleted with its own device selected
 struct ProblemDeleter {
   void operator()(b200pdlp_problem* p) const { cudaSetDevice(p->device); delete p; }
@@ -503,12 +516,14 @@ const char* prep_error_text(int err);
 void check_device_array(const void* ptr, int device, int i, const char* field, const char* who);
 void check_device_lp(const b200pdlp_lp& lp, int device, int i, const char* who);
 void check_device_result(const b200pdlp_result& out, int device, int i, const char* who);
-// the single solves on device arrays (b200pdlp_solve_device, b200pdlp_solve_hipdlp_device)
-enum class DeviceRoute { Ordered, Tree, Degenerate };
-DeviceRoute device_lp_route(cudaStream_t s, const b200pdlp_lp& lp, bool hipdlp, int ordered_max, const char* who, int* nnz);
-using HostSolve = std::function<void(const b200pdlp_lp&, const b200pdlp_warm*, b200pdlp_result*)>;
-void solve_degenerate(cudaStream_t s, const b200pdlp_lp& lp, const b200pdlp_warm* warm, b200pdlp_result* out,
-                      const HostSolve& solve);
+// b200pdlp_solve_device and b200pdlp_solve_hipdlp_device after their null and parameter checks: the LP's checks, then the
+// route: `batch` (ordered mode), create_host on host copies (an LP without a matrix) or create_device (tree mode), then
+// `solve`.  `device` is the requested device on entry and the selected one on return.
+using CreateProblem = std::function<void(const b200pdlp_lp&, b200pdlp_problem*)>;
+using SolveProblem = std::function<void(b200pdlp_problem*, const b200pdlp_lp&, const b200pdlp_warm*, b200pdlp_result*)>;
+void solve_lp_device(const b200pdlp_lp& lp, bool hipdlp, int& device, int ordered_max, const b200pdlp_warm* warm,
+                     b200pdlp_result* out, const char* who, const std::function<void()>& batch, const CreateProblem& create_host,
+                     const CreateProblem& create_device, const SolveProblem& solve);
 
 // engine_batch.cu: the device-array batches, which the single device-array solves take for ordered-mode LPs
 int select_device(int device);
@@ -521,6 +536,13 @@ void apply_spmv_grid(b200pdlp_problem* p);
 void ensure_host_maps(b200pdlp_problem* p);
 
 // engine.cu: the PDLP solve's host control, which the batch rounds share
+// a time limit in seconds, or -1 for none (negative or not finite)
+double time_limit_or_none(double time_limit);
+// PDHG_Init_Step_Sizes (cupdlp_step.c:312-375): beta from |c|^2 and |b|^2 of the scaled form; then tau and sigma, adaptive
+// from max |a_ij|, or fixed from the power method's estimate lambda of |A|^2
+double step_beta(double cost_sq, double rhs_sq);
+void adaptive_step_sizes(PdhgState* h, double amax);
+void fixed_step_sizes(PdhgState* h, double lambda);
 void fill_pow_tables(PdhgState* h);
 void arm_step(PdhgState* h);
 void assemble_check_a(const StdForm& f, const double* o, CheckResult& cr, double dscale[2], double pscale[2]);
@@ -558,5 +580,7 @@ double dev_mismatches(const T* dev, const T* host, size_t count) {
 void hip_host_postsolve(const b200pdlp_lp& lp, const StdForm& f, const int* cperm, const int* rperm, const double* x,
                         const double* y, const double* sp, const double* sn, b200pdlp_result* out);
 void hip_trace_row(b200pdlp_result* out, const HipController& ctl, const double* sums, bool restart, bool converged);
+// the fields of one HiPDLP solve's result besides the vectors, the timings and kernel_launches
+void hip_fill_result(b200pdlp_result* out, const StdForm& f, const HipController& ctl, bool converged, bool timed_out);
 
 }  // namespace b200

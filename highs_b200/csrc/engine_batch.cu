@@ -215,12 +215,8 @@ static BatchLoop batch_rounds(cudaStream_t s, int count, const b200pdlp_params& 
     PdhgState* h = hst + i;
     memset(h, 0, sizeof(PdhgState));
     h->adaptive = prm.adaptive_step != 0;
-    const double a = r.cost_sq, b = r.rhs_sq;
-    h->beta = std::fmin(a, b) > 1e-6 ? a / b : 1.0;
-    if (h->adaptive) {
-      h->tau = (1.0 / r.f.amax) / std::sqrt(h->beta);
-      h->sigma = h->tau * h->beta;
-    }
+    h->beta = step_beta(r.cost_sq, r.rhs_sq);
+    if (h->adaptive) adaptive_step_sizes(h, r.f.amax);
     arm_step(h);
     fill_pow_tables(h);
     h->stop_iter = 0;   // the first check is due at once (iteration 0)
@@ -234,7 +230,7 @@ static BatchLoop batch_rounds(cudaStream_t s, int count, const b200pdlp_params& 
   dst.alloc(count, false); dctl.alloc(count, false);
 
   const int interval = prm.check_interval > 0 ? prm.check_interval : 40;
-  const double t_lim = (prm.time_limit >= 0 && std::isfinite(prm.time_limit)) ? prm.time_limit : -1.0;   // < 0: none
+  const double t_lim = time_limit_or_none(prm.time_limit);
   CudaEvent evl0, evl1, ev0, ev1;
   BatchLoop L;
   int active = count;
@@ -270,11 +266,7 @@ static BatchLoop batch_rounds(cudaStream_t s, int count, const b200pdlp_params& 
         continue;
       }
       if (first && c.fixed_step) {
-        const double lambda = c.outs[kBatchLambda];
-        h->tau = 0.8 / std::sqrt(lambda);
-        h->sigma = h->tau;
-        h->tau /= std::sqrt(h->beta);
-        h->sigma *= std::sqrt(h->beta);
+        fixed_step_sizes(h, c.outs[kBatchLambda]);
         arm_step(h);
       }
       CheckResult& chk = b.chk;
@@ -860,7 +852,7 @@ static BatchLoop hip_batch_rounds(cudaStream_t s, int count, const b200pdlp_hipd
     memset(&c, 0, sizeof(HipBatchCtl));
     c.active = 1; c.first = 1;
   }
-  const double t_lim = (prm.time_limit >= 0 && std::isfinite(prm.time_limit)) ? prm.time_limit : -1.0;   // < 0: none
+  const double t_lim = time_limit_or_none(prm.time_limit);
   CudaEvent evl0, evl1, ev0, ev1;
   BatchLoop L;
   int active = count;
@@ -905,8 +897,7 @@ static BatchLoop hip_batch_rounds(cudaStream_t s, int count, const b200pdlp_hipd
       } else {
         if (c.fpe) ctl.restart_reference(c.outs + kHipBatchFpe);
         restart = ctl.after_block(c.outs);
-        const bool block_converged =
-            ctl.pfeas < ctl.tol * (1.0 + f.norm_rhs) && ctl.dfeas < ctl.tol * (1.0 + f.norm_cost) && ctl.relgap < ctl.tol;
+        const bool block_converged = ctl.block_converged();
         if (b.trace) hip_trace_row(b.trace, ctl, c.outs, restart, block_converged);
         if (block_converged) {
           b.converged = true; b.sol = 1; done = true;
@@ -931,20 +922,12 @@ static BatchLoop hip_batch_rounds(cudaStream_t s, int count, const b200pdlp_hipd
 
 // the fields of a HiPDLP batch result besides the vectors; the timings and kernel_launches are the batch's
 static void hip_batch_result(b200pdlp_result* out, const HipBatchRun& b, const BatchLoop& L, double setup_seconds) {
-  const StdForm& f = b.f;
-  const HipController& ctl = b.ctl;
-  out->value_valid = 1; out->dual_valid = 1;
-  out->term_code = b.converged ? B200PDLP_OPTIMAL : B200PDLP_TIMELIMIT_OR_ITERLIMIT;
-  out->term_iterate = b.timed_out ? 2 : 0;
-  out->iters = ctl.iters; out->passes = ctl.iters; out->restarts = ctl.restarts;
+  hip_fill_result(out, b.f, b.ctl, b.converged, b.timed_out);
   out->kernel_launches = (int)std::min<long long>(L.rounds, 2147483647LL);
-  out->primal_obj = ctl.pobj; out->dual_obj = ctl.dobj; out->primal_feas = ctl.pfeas; out->dual_feas = ctl.dfeas;
-  out->gap = ctl.pobj - ctl.dobj; out->rel_gap = ctl.relgap;
   out->setup_seconds = setup_seconds;
   out->solve_seconds = L.solve_seconds;
   out->loop_device_ms = L.loop_ms;
   out->iter_device_ms = L.iter_ms;
-  out->form_cols = f.n; out->form_rows = f.m; out->form_nnz = f.nnz; out->form_neq = f.neq;
 }
 
 // b200pdlp_solve_hipdlp_batch_mixed: the same rounds for members of any size up to kTreeMemberMax.  The tree-mode members

@@ -342,6 +342,16 @@ void hip_trace_row(b200pdlp_result* out, const HipController& ctl, const double*
   out->trace_len++;
 }
 
+void hip_fill_result(b200pdlp_result* out, const StdForm& f, const HipController& ctl, bool converged, bool timed_out) {
+  out->value_valid = 1; out->dual_valid = 1;
+  out->term_code = converged ? B200PDLP_OPTIMAL : B200PDLP_TIMELIMIT_OR_ITERLIMIT;
+  out->term_iterate = timed_out ? 2 : 0;   // 2: the time limit, not the iteration limit, ended the run
+  out->iters = ctl.iters; out->passes = ctl.iters; out->restarts = ctl.restarts;
+  out->primal_obj = ctl.pobj; out->dual_obj = ctl.dobj; out->primal_feas = ctl.pfeas; out->dual_feas = ctl.dfeas;
+  out->gap = ctl.pobj - ctl.dobj; out->rel_gap = ctl.relgap;
+  out->form_cols = f.n; out->form_rows = f.m; out->form_nnz = f.nnz; out->form_neq = f.neq;
+}
+
 static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, const b200pdlp_hipdlp_params& prm, b200pdlp_result* out) {
   NvtxRange nvtx("b200pdlp: solve (HiPDLP mode)");
   using clk = std::chrono::steady_clock;
@@ -358,13 +368,10 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
   CudaEvent evl0, evl1;
   if (!h.graph) {   // steps 2 .. 40 of a block: 38 minor steps and the closing major step (:629-632)
     const long long l0 = p->launches;
-    cudaGraph_t g = nullptr;
-    CUDA_OK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-    for (int i = 2; i <= 39; i++) hip_step(p, i, 0);
-    hip_step(p, 40, 1);
-    CUDA_OK(cudaStreamEndCapture(s, &g));
-    CUDA_OK(cudaGraphInstantiate(&h.graph, g, 0));
-    CUDA_OK(cudaGraphDestroy(g));
+    h.graph = capture_graph(s, [&] {
+      for (int i = 2; i <= 39; i++) hip_step(p, i, 0);
+      hip_step(p, 40, 1);
+    });
     h.graph_launches = p->launches - l0;   // counted when replayed
     p->launches = l0;
   }
@@ -398,8 +405,7 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
     h.hstate->primal_step = ctl.primal_step; h.hstate->dual_step = ctl.dual_step; h.hstate->halpern_iteration = ctl.halpern_iteration;
     CUDA_OK(cudaMemcpyAsync(h.state.p, h.hstate, sizeof(HipState), cudaMemcpyHostToDevice, s));
   };
-  const double t_lim = (prm.time_limit >= 0 && std::isfinite(prm.time_limit)) ? prm.time_limit : -1.0;   // < 0: none
-  int term = B200PDLP_TIMELIMIT_OR_ITERLIMIT;
+  const double t_lim = time_limit_or_none(prm.time_limit);
   bool converged = false, timed_out = false;
   const auto t_loop = clk::now();
   CUDA_OK(cudaEventRecord(evl0, s));
@@ -425,8 +431,7 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
       if (prm.log_level >= 2)
         printf("[b200pdlp hipdlp] it %8d  pobj %+.8e dobj %+.8e  pfeas %.2e dfeas %.2e  fpe %.3e  weight %.3e\n", ctl.iters,
                ctl.pobj, ctl.dobj, ctl.pfeas, ctl.dfeas, ctl.fpe, ctl.primal_weight);
-      const bool block_converged =
-          ctl.pfeas < ctl.tol * (1.0 + f.norm_rhs) && ctl.dfeas < ctl.tol * (1.0 + f.norm_cost) && ctl.relgap < ctl.tol;
+      const bool block_converged = ctl.block_converged();
       hip_trace_row(out, ctl, p->houts, restart, block_converged);
       if (block_converged) { converged = true; sol_x = h.xn.p; sol_y = h.yn.p; break; }
       if (restart) {   // anchors and iterates <- the PDHG iterate of the last major step (:664-688)
@@ -440,9 +445,6 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
       }
     }
   }
-  const int iters = ctl.iters, restarts = ctl.restarts;
-  const double pfeas = ctl.pfeas, dfeas = ctl.dfeas, pobj = ctl.pobj, dobj = ctl.dobj, relgap = ctl.relgap;
-  if (converged) term = B200PDLP_OPTIMAL;
   CUDA_OK(cudaEventRecord(evl1, s));
   CUDA_OK(cudaEventSynchronize(evl1));
   // the postsolve's pageable copies wait for every kernel of the context: no barrier kernel may still be in flight
@@ -496,16 +498,10 @@ static void solve_hipdlp_on_device(b200pdlp_problem* p, const b200pdlp_lp& lp, c
   if (getenv("B200PDLP_TIMING"))
     fprintf(stderr, "[b200pdlp solve] postsolve (%s) %8.3f ms\n", p->dev_form ? "device" : "host",
             std::chrono::duration<double, std::milli>(clk::now() - t_loop).count() - 1e3 * solve_seconds);
-  out->value_valid = 1; out->dual_valid = 1;
-  out->term_code = term;
-  out->term_iterate = timed_out ? 2 : 0;   // 2: the time limit, not the iteration limit, ended the run
-  out->iters = iters; out->passes = iters; out->restarts = restarts;
+  hip_fill_result(out, f, ctl, converged, timed_out);
   out->kernel_launches = (int)std::min<long long>(p->launches - launches0, 2147483647LL);
-  out->primal_obj = pobj; out->dual_obj = dobj; out->primal_feas = pfeas; out->dual_feas = dfeas;
-  out->gap = pobj - dobj; out->rel_gap = relgap;
   out->solve_seconds = solve_seconds;
   out->setup_seconds += std::chrono::duration<double>(t_loop - t_begin).count();
-  out->form_cols = n; out->form_rows = m; out->form_nnz = f.nnz; out->form_neq = f.neq;
 }
 
 // b200pdlp_solve_hipdlp_multi's device prologue: one host thread per distinct device in `dev` runs the block-mode prologue
@@ -557,7 +553,7 @@ int b200pdlp_hipdlp_controller_replay(double norm_cost, double norm_rhs, double 
     const bool restart = ctl.after_block(sums + 9 * (size_t)b);
     double* o = out + 8 * (size_t)b;
     o[0] = restart ? 1.0 : 0.0; o[1] = ctl.primal_weight; o[2] = ctl.primal_step; o[3] = ctl.dual_step; o[4] = ctl.fpe;
-    o[5] = (ctl.pfeas < ctl.tol * (1.0 + norm_rhs) && ctl.dfeas < ctl.tol * (1.0 + norm_cost) && ctl.relgap < ctl.tol) ? 1.0 : 0.0;
+    o[5] = ctl.block_converged() ? 1.0 : 0.0;
     o[6] = ctl.iters; o[7] = ctl.halpern_iteration;
   }
   return B200PDLP_OK;
@@ -593,35 +589,11 @@ int b200pdlp_solve_hipdlp_device(const b200pdlp_lp* lp, const b200pdlp_hipdlp_pa
   const char* who = "b200pdlp_solve_hipdlp_device";
   return guarded([&] {
     if (!lp || !params || !out) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": null argument");
-    if (!lp_fields_ok(lp)) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": b200pdlp: malformed b200pdlp_lp");
-    if (lp->sense != 1.0 && lp->sense != -1.0) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": b200pdlp: sense must be +1 or -1");
-    const int device = select_device(params->device);
-    check_device_lp(*lp, device, -1, who);
-    check_device_result(*out, device, -1, who);
-    const auto t0 = std::chrono::steady_clock::now();
     b200pdlp_hipdlp_params prm = *params;
-    prm.device = device;
-    ProblemPtr p(new b200pdlp_problem());   // its stream serves the sizing and, in tree mode, the solve
-    open_problem(p.get(), device, 0, 1);
-    int nnz = 0;
-    const DeviceRoute route = device_lp_route(p->stream, *lp, true, prm.ordered_max, who, &nnz);
-    if (route == DeviceRoute::Ordered) {
-      solve_hipdlp_batch_device(1, lp, prm, out, /*mixed=*/true);
-    } else if (route == DeviceRoute::Degenerate) {
-      solve_degenerate(p->stream, *lp, nullptr, out, [&](const b200pdlp_lp& hl, const b200pdlp_warm*, b200pdlp_result* r) {
-        ProblemPtr q(new b200pdlp_problem());
-        create_problem_hipdlp(hl, prm, q.get());
-        r->setup_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-        solve_hipdlp_on_device(q.get(), hl, prm, r);
-      });
-    } else {
-      p->device_io = true;
-      p->prep.inputs_on_device = true;
-      p->prep.device_nnz = nnz;
-      create_problem_hipdlp_device(*lp, prm, p.get());
-      out->setup_seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-      solve_hipdlp_on_device(p.get(), *lp, prm, out);
-    }
+    solve_lp_device(*lp, true, prm.device, prm.ordered_max, nullptr, out, who, [&] { solve_hipdlp_batch_device(1, lp, prm, out, /*mixed=*/true); },
+                    [&](const b200pdlp_lp& l, b200pdlp_problem* q) { create_problem_hipdlp(l, prm, q); },
+                    [&](const b200pdlp_lp& l, b200pdlp_problem* q) { create_problem_hipdlp_device(l, prm, q); },
+                    [&](b200pdlp_problem* q, const b200pdlp_lp& l, const b200pdlp_warm*, b200pdlp_result* r) { solve_hipdlp_on_device(q, l, prm, r); });
     CUDA_OK(cudaGetLastError());
   });
 }

@@ -112,6 +112,8 @@ struct HipController {
   void init(double norm_cost_, double norm_rhs_, double op_norm_sq, double tol_, int strategy_);   // initializeStepSizes, :1944-1977
   double fixed_point_error(const double* s) const;                                                 // :733-739
   bool converged(const double* s);                                                                 // checkConvergence, :1474-1527
+  // the convergence test on the measures of the last check (converged() sets them, and so does after_block())
+  bool block_converged() const { return pfeas < tol * (1.0 + norm_rhs) && dfeas < tol * (1.0 + norm_cost) && relgap < tol; }
   void restart_reference(const double* s) { fpe = fixed_point_error(s); fpe0 = fpe; pending_restart_fpe = false; }   // :600-608
   // after steps 2..40 of a block (s = the block-end check); returns true if the loop restarts now (anchors <- iterate),
   // with the primal weight and the step sizes already updated

@@ -265,7 +265,7 @@ bool HipController::converged(const double* s) {
   dobj = s[6];
   const double gap = pobj - dobj;
   relgap = std::fabs(gap) / (1.0 + std::fabs(pobj) + std::fabs(dobj));
-  return pfeas < tol * (1.0 + norm_rhs) && dfeas < tol * (1.0 + norm_cost) && relgap < tol;
+  return block_converged();
 }
 
 bool HipController::after_block(const double* s) {
