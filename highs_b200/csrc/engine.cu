@@ -2287,6 +2287,57 @@ int b200pdlp_check_device(b200pdlp_problem* p, const b200pdlp_check_in* in, doub
   });
 }
 
+// one record per long row of M: {standard-form row, first slot, segments}; perm maps M's device rows to standard-form order
+static int long_row_records(const DeviceMatrix& M, const std::vector<int>& perm, int32_t* out) {
+  std::vector<int4> lr(M.long_rows.n);
+  if (!lr.empty()) CUDA_OK(cudaMemcpy(lr.data(), M.long_rows.p, lr.size() * sizeof(int4), cudaMemcpyDeviceToHost));
+  for (size_t k = 0; k < lr.size(); k++) {
+    out[3 * k] = perm[lr[k].x];
+    out[3 * k + 1] = M.dev.nblocks_body + lr[k].y;
+    out[3 * k + 2] = lr[k].z;
+  }
+  return (int)lr.size();
+}
+
+int b200pdlp_pass_partials(b200pdlp_problem* p, const double* x, const double* y, const double* ax, const double* aty,
+                           double tau, double sigma, double* x_new, double* y_new, double* ax_new, double* aty_new,
+                           double* slots, int32_t cap, int32_t* long_rows, int32_t long_cap, b200pdlp_pass_out* out) {
+  DeviceGuard dg;
+  return guarded([&] {
+    const char* who = "b200pdlp_pass_partials";
+    if (!p || !x || !y || !ax || !aty || !x_new || !y_new || !ax_new || !aty_new || !slots || !long_rows || !out)
+      throw Error(B200PDLP_ERR_ARG, std::string(who) + ": null argument");
+    require_mode(p, false, who);
+    if (p->world != 1) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": kernel-level entry points are single-GPU");
+    if (p->ordered) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": an ordered-mode problem (its sums add terms, not slots)");
+    const int n = p->n;
+    const int nb[3] = {primal_step_grid(n), p->A.grid(), p->AT.grid()};
+    const int nlong = (int)(p->A.long_rows.n + p->AT.long_rows.n);
+    if (cap < std::max(nb[0], std::max(nb[1], nb[2])) || long_cap < nlong)
+      throw Error(B200PDLP_ERR_ARG, std::string(who) + ": cap must be >= " + std::to_string(std::max(nb[0], std::max(nb[1], nb[2]))) +
+                                        " and long_cap >= " + std::to_string(nlong));
+    set_device(p);
+    ensure_host_maps(p);
+    upload_perm(p, p->x[0].p, x, p->cperm); upload_perm(p, p->aty[0].p, aty, p->cperm);
+    upload_perm(p, p->y[0].p, y, p->rperm); upload_perm(p, p->ax[0].p, ax, p->rperm);
+    kernel_api_state(p, tau, sigma);
+    enqueue_pass(p);
+    p->launches += p->kernels_per_pass();
+    CUDA_OK(cudaGetLastError());
+    const int slot_ids[3] = {kSlotK1, kSlotK2, kSlotK3};
+    for (int k = 0; k < 3; k++)
+      CUDA_OK(cudaMemcpyAsync(slots + (size_t)k * cap, p->rs(slot_ids[k], 0).partials, (size_t)nb[k] * sizeof(double),
+                              cudaMemcpyDeviceToHost, p->stream));
+    pull_state(p);
+    out->dx2 = p->hstate->dx2; out->dy2 = p->hstate->dy2; out->inter = p->hstate->inter;
+    for (int k = 0; k < 3; k++) out->slots[k] = nb[k];
+    out->long_a = long_row_records(p->A, p->rperm, long_rows);
+    out->long_at = long_row_records(p->AT, p->cperm, long_rows + 3 * (size_t)out->long_a);
+    download_perm(p, x_new, p->x[1].p, p->cperm); download_perm(p, aty_new, p->aty[1].p, p->cperm);
+    download_perm(p, y_new, p->y[1].p, p->rperm); download_perm(p, ax_new, p->ax[1].p, p->rperm);
+  });
+}
+
 int b200pdlp_bench_spmv(b200pdlp_problem* p, int32_t which, int32_t reps, float* ms_total) {
   DeviceGuard dg;
   return guarded([&] {

@@ -105,7 +105,7 @@ __device__ __forceinline__ void slice_end(const Epi& e, int slice, bool live) {
 // L1TEX pipe only sees the coalesced streams and the (irreducible) one-line-per-lane gathers.
 // Rows longer than the long-row threshold live outside the body as segments of kNnzBlk nonzeros
 // (one CTA each, tree-summed); the last segment of a row to finish combines the partial sums in
-// segment order and runs the epilogue.
+// segment order and runs the epilogue, whose terms go to the partial-sum slot of the row's first segment.
 // `due` != nullptr: speculative check-iteration launch -- run only if the check iteration has been reached
 __device__ __forceinline__ bool check_not_due(const PdhgState* due) { return due && (due->done || due->iter < due->stop_iter); }
 
@@ -423,7 +423,9 @@ __global__ void __launch_bounds__(kThreads) spmv_sell_kernel(DevSell A, Epi epi_
       slice_end(epi, slice, live);
     }
   } else {
-    // one segment of a long row
+    // one segment of a long row.  Its slot of the partial sums is +0.0, stored before the ticket (the fence after the
+    // long_partial store orders it); the finisher stores the row's terms, 0.0 + term, into the slot of the row's FIRST segment.
+    // So where a term lands does not depend on which segment finishes last, and K4's sums are the same run to run.
     __shared__ double sm[kThreads / 32];
     const int4 sg = A.segs[blockIdx.x - A.nblocks_body];
     double s = 0.0;
@@ -432,6 +434,10 @@ __global__ void __launch_bounds__(kThreads) spmv_sell_kernel(DevSell A, Epi epi_
     if (threadIdx.x == 0) {
       const int4 lr = A.long_rows[sg.w];
       const int seg = (int)(blockIdx.x - A.nblocks_body) - lr.y;
+      if constexpr (Epi::NACC > 0) {
+#pragma unroll
+        for (int a = 0; a < Epi::NACC; a++) rs.partials[(size_t)a * gridDim.x + blockIdx.x] = 0.0;
+      }
       A.long_partial[lr.w + seg] = s;
       __threadfence();
       const unsigned t = atomicAdd(&A.long_counter[sg.w], 1u);
@@ -442,18 +448,25 @@ __global__ void __launch_bounds__(kThreads) spmv_sell_kernel(DevSell A, Epi epi_
         for (int q = 0; q < lr.z; q++) tot += p[q];
         A.long_counter[sg.w] = 0u;
         epi.prefetch(lr.x);
+        const size_t first = (size_t)A.nblocks_body + lr.y;
         if constexpr (kSmemAcc) {
           epi.row(lr.x, tot, StridedOut{&sacc[0][threadIdx.x]});
+#pragma unroll
+          for (int a = 0; a < Epi::NACC; a++) rs.partials[(size_t)a * gridDim.x + first] = 0.0 + sacc[a][threadIdx.x];
         } else {
           double t[Epi::NACC > 0 ? Epi::NACC : 1];
           epi.row(lr.x, tot, t);
           if constexpr (Epi::NACC > 0) {
 #pragma unroll
-            for (int a = 0; a < Epi::NACC; a++) add_term(acc[a], t[a], rs, a, lr.x);
+            for (int a = 0; a < Epi::NACC; a++) {
+              rs.partials[(size_t)a * gridDim.x + first] = 0.0 + t[a];
+              if (rs.terms) rs.terms[(size_t)a * rs.len + lr.x] = t[a];   // ordered mode: K4 adds these, in row order
+            }
           }
         }
       }
     }
+    return;   // (no block tree: the slot is written above)
   }
   if constexpr (kSmemAcc) {
     // same tree as block_partials: lanes, then the block's warps in order
@@ -532,7 +545,8 @@ __global__ void __launch_bounds__(kTileThreads, 1) spmv_sell_tile_kernel(DevSell
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int tile = blockIdx.x;
   if (tile >= A.nblocks_body) {
-    // one segment of a long row (same scheme as spmv_sell_kernel, on this kernel's 1024 threads): gathers from global memory
+    // one segment of a long row (same scheme as spmv_sell_kernel, on this kernel's 1024 threads, the same slots: +0.0 in
+    // every segment's, the finisher's 0.0 + term in the first segment's): gathers from global memory
     const int4 sg = A.segs[tile - A.nblocks_body];
     double s = 0.0;
     for (int e = sg.y + threadIdx.x; e < sg.z; e += kTileThreads) s += A.lval[e] * xin[A.lcol[e]];
@@ -544,6 +558,10 @@ __global__ void __launch_bounds__(kTileThreads, 1) spmv_sell_tile_kernel(DevSell
       for (int q = 0; q < kTileThreads / 32; q++) tot_seg += smp[0][q];
       const int4 lr = A.long_rows[sg.w];
       const int seg = (tile - A.nblocks_body) - lr.y;
+      if constexpr (Epi::NACC > 0) {
+#pragma unroll
+        for (int a = 0; a < Epi::NACC; a++) rs.partials[(size_t)a * gridDim.x + blockIdx.x] = 0.0;
+      }
       A.long_partial[lr.w + seg] = tot_seg;
       __threadfence();
       const unsigned t = atomicAdd(&A.long_counter[sg.w], 1u);
@@ -558,11 +576,8 @@ __global__ void __launch_bounds__(kTileThreads, 1) spmv_sell_tile_kernel(DevSell
         epi.row(lr.x, tot, t2);
         if constexpr (Epi::NACC > 0) {
 #pragma unroll
-          for (int a = 0; a < Epi::NACC; a++) rs.partials[(size_t)a * gridDim.x + blockIdx.x] = t2[a];
+          for (int a = 0; a < Epi::NACC; a++) rs.partials[(size_t)a * gridDim.x + A.nblocks_body + lr.y] = 0.0 + t2[a];
         }
-      } else if constexpr (Epi::NACC > 0) {
-#pragma unroll
-        for (int a = 0; a < Epi::NACC; a++) rs.partials[(size_t)a * gridDim.x + blockIdx.x] = 0.0;
       }
     }
     return;
@@ -759,7 +774,8 @@ __global__ void __launch_bounds__(kZThreads, 1) spmv_sell_zskip_kernel(DevSell A
     }
     group_partials<Epi::NACC>(acc, rs, c, nslots, smp);
   }
-  // long-row segments: as one kThreads CTA of spmv_sell_kernel does them (block_sum's tree, the ticket, the finisher's term)
+  // long-row segments: as one kThreads CTA of spmv_sell_kernel does them (block_sum's tree, the ticket, the slots: +0.0 in
+  // every segment's, the finisher's 0.0 + term in the first segment's, nb + lr.y)
   const int t = threadIdx.x % kThreads;
   for (int q = gid; q < A.nsegs; q += ngroups) {
     const int4 sg = A.segs[q];
@@ -768,12 +784,13 @@ __global__ void __launch_bounds__(kZThreads, 1) spmv_sell_zskip_kernel(DevSell A
     sv = warp_sum(sv);
     if (lane == 0) sseg[grp][w] = sv;
     asm volatile("bar.sync %0, %1;" ::"r"(1 + grp), "r"(kThreads) : "memory");
-    double acc[Epi::NACC] = {};
     if (w == 0) {
       double r = lane < kThreads / 32 ? sseg[grp][lane] : 0.0;
       r = warp_sum(r);
       if (lane == 0) {
         const int4 lr = A.long_rows[sg.w];
+#pragma unroll
+        for (int a = 0; a < Epi::NACC; a++) rs.partials[(size_t)a * nslots + nb + q] = 0.0;
         A.long_partial[lr.w + q - lr.y] = r;
         __threadfence();
         const unsigned tk = atomicAdd(&A.long_counter[sg.w], 1u);
@@ -787,11 +804,11 @@ __global__ void __launch_bounds__(kZThreads, 1) spmv_sell_zskip_kernel(DevSell A
           double tt[Epi::NACC];
           epi.row(lr.x, tot, tt);
 #pragma unroll
-          for (int a = 0; a < Epi::NACC; a++) acc[a] += tt[a];
+          for (int a = 0; a < Epi::NACC; a++) rs.partials[(size_t)a * nslots + nb + lr.y] = 0.0 + tt[a];
         }
       }
     }
-    group_partials<Epi::NACC>(acc, rs, nb + q, nslots, smp);   // (its first barrier also ends the group's use of sseg)
+    asm volatile("bar.sync %0, %1;" ::"r"(1 + grp), "r"(kThreads) : "memory");   // warp 0 is done with sseg[grp]
   }
 }
 

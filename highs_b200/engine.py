@@ -70,6 +70,12 @@ class CCheckOut(C.Structure):
                 ("pow_red", C.c_double * 128), ("pow_grow", C.c_double * 128), ("trace", C.c_double * 16)]
 
 
+class CPassOut(C.Structure):
+    """b200pdlp_pass_out: K4's sums and the sizes of what b200pdlp_pass_partials returned"""
+    _fields_ = [("dx2", C.c_double), ("dy2", C.c_double), ("inter", C.c_double), ("slots", C.c_int32 * 3),
+                ("long_a", C.c_int32), ("long_at", C.c_int32)]
+
+
 CHECK_VECTORS = ("x", "y", "ax", "aty", "xsum", "ysum", "xlr", "ylr", "axsum", "atysum", "xavg", "yavg", "axavg", "atyavg")
 RESIDUAL_NAMES = ("pobj", "dobj", "pfeas", "dfeas", "gap", "relgap", "pinf_obj", "pinf_res", "dinf_obj", "dinf_res")
 
@@ -110,7 +116,7 @@ ABI_SYMBOLS = [
     "b200pdlp_kkt_check_batch_device", "b200pdlp_hipdlp_problem_create", "b200pdlp_hipdlp_step", "b200pdlp_hipdlp_check",
     "b200pdlp_hipdlp_problem_power_method", "b200pdlp_solve_hipdlp_batch_mixed",
     "b200pdlp_solve_hipdlp_batch_mixed_device", "b200pdlp_debug_hipdlp_tree_prep_compare", "b200pdlp_check_device",
-    "b200pdlp_solve_device", "b200pdlp_solve_hipdlp_device",
+    "b200pdlp_solve_device", "b200pdlp_solve_hipdlp_device", "b200pdlp_pass_partials",
 ]
 HIP_TRACE_COLS = 16   # B200PDLP_HIP_TRACE_COLS: the per-block trace of the HiPDLP solves
 
@@ -187,6 +193,8 @@ def lib():
         L.b200pdlp_dual_step.argtypes = [C.c_void_p, _dp, _dp, _dp, C.c_double, _dp, _dp, _dp]
         L.b200pdlp_residuals.argtypes = [C.c_void_p, _dp, _dp, _dp]
         L.b200pdlp_check_device.argtypes = [C.c_void_p, C.POINTER(CCheckIn)] + [_dp] * 14 + [C.POINTER(CCheckOut)]
+        L.b200pdlp_pass_partials.argtypes = ([C.c_void_p] + [_dp] * 4 + [C.c_double] * 2 + [_dp] * 5 +
+                                             [C.c_int32, _ip, C.c_int32, C.POINTER(CPassOut)])
         _lib = L
     return _lib
 
@@ -962,6 +970,30 @@ class Problem:
             r[k] = np.ctypeslib.as_array(a).copy() if hasattr(t, "_length_") else a
         r["res"] = [dict(zip(RESIDUAL_NAMES, r["res"][t].tolist())) for t in range(2)]
         r.update(v)
+        return r
+
+    def pass_partials(self, x, y, ax, aty, tau, sigma) -> dict:
+        """One PDHG pass of a tree-mode solve and its partial sums (b200pdlp_pass_partials).  Vectors in standard-form order.
+        Returns x_new, y_new, ax_new, aty_new; k1, k2, k3, the slot arrays of the three pass kernels; long_a and long_at, one
+        row (standard-form row, first slot, segments) per long row of A and of A'; dx2, dy2 and inter as K4 left them."""
+        n, m = self.n, self.m
+        x, aty = (np.array(v, dtype=np.float64, copy=True).reshape(n) for v in (x, aty))
+        y, ax = (np.array(v, dtype=np.float64, copy=True).reshape(m) for v in (y, ax))
+        r = dict(x_new=np.zeros(n), y_new=np.zeros(m), ax_new=np.zeros(m), aty_new=np.zeros(n))
+        # bounds of the slot counts: K1's grid is capped at 16 x 148 CTAs; K2 and K3 have at most one CTA per 256 rows and
+        # one per started 2048 entries of a long row (longer than 512 entries)
+        nlong = self.nnz // 513 + 1
+        cap = max(16 * 148, (max(n, m) + 255) // 256 + self.nnz // 2048 + nlong)
+        slots = np.zeros((3, cap))
+        lr = np.zeros((2 * nlong, 3), dtype=np.int32)
+        out = CPassOut()
+        _check(lib().b200pdlp_pass_partials(self._h, _p(x, _dp), _p(y, _dp), _p(ax, _dp), _p(aty, _dp), float(tau), float(sigma),
+                                            *(_p(r[k], _dp) for k in ("x_new", "y_new", "ax_new", "aty_new")), _p(slots, _dp),
+                                            cap, _p(lr, _ip), lr.shape[0], C.byref(out)), "b200pdlp_pass_partials")
+        for k in range(3):
+            r[f"k{k + 1}"] = slots[k, : out.slots[k]].copy()
+        r["long_a"], r["long_at"] = lr[: out.long_a].copy(), lr[out.long_a: out.long_a + out.long_at].copy()
+        r.update(dx2=out.dx2, dy2=out.dy2, inter=out.inter)
         return r
 
     def bench_spmv(self, which: int, reps: int) -> float:

@@ -286,6 +286,27 @@ int b200pdlp_check_device(b200pdlp_problem* p, const b200pdlp_check_in* in, doub
                           double* xsum, double* ysum, double* xlr, double* ylr, double* axsum, double* atysum, double* xavg,
                           double* yavg, double* axavg, double* atyavg, b200pdlp_check_out* out);
 
+/* One PDHG pass of a tree-mode solve and the partial sums it leaves (parity tests; one GPU): K1 (primal step, |dx|^2), K2
+ * (A x' + dual step, |dy|^2) and K3 (A'y' + interaction) by the launchers of the solve's pass graph under the problem's SpMV
+ * shapes (zero-skip, tiled, persistent), then step_rule_kernel (K4).  Inputs are host arrays in standard-form order: x, aty
+ * (n), y, ax (m) and the step sizes tau, sigma; written: x_new, aty_new (n), y_new, ax_new (m).
+ * slots[3][cap]: the partial-sum slots of K1, K2 and K3 as the launches left them (out->slots[k] entries each).
+ * long_rows[long_cap][3]: one record {standard-form row, first slot, segments} per long row of A (out->long_a records), then
+ * per long row of A' = long column of A (out->long_at).  A long row's segments have the slots first .. first + segments - 1;
+ * its epilogue term goes to the first one, and every other one holds +0.0.
+ * out->dx2, dy2, inter: K4's sums, read from the state block.
+ * Rejected with B200PDLP_ERR_ARG before anything is written: NULL arguments, a problem in ordered mode, on several GPUs or
+ * of b200pdlp_hipdlp_problem_create, cap below the longest slot array and long_cap below the number of long rows.
+ * No device: B200PDLP_ERR_CUDA. */
+typedef struct {
+  double dx2, dy2, inter;
+  int32_t slots[3];         /* K1, K2, K3 */
+  int32_t long_a, long_at;  /* long rows of A, of A' */
+} b200pdlp_pass_out;
+int b200pdlp_pass_partials(b200pdlp_problem* p, const double* x, const double* y, const double* ax, const double* aty,
+                           double tau, double sigma, double* x_new, double* y_new, double* ax_new, double* aty_new,
+                           double* slots, int32_t cap, int32_t* long_rows, int32_t long_cap, b200pdlp_pass_out* out);
+
 /* device-pointer variants on the problem's stream (bench roofline loop):
  * time `reps` back-to-back launches with CUDA events; returns ms in *ms_total */
 int b200pdlp_bench_spmv(b200pdlp_problem* p, int32_t which /*0 Ax, 1 ATy*/, int32_t reps, float* ms_total);

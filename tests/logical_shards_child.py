@@ -17,6 +17,16 @@ from highs_b200 import engine  # noqa: E402
 from highs_b200.lp import read_b2lp, synthetic_lp  # noqa: E402
 
 
+def long_rows_lp():
+    """two row blocks of 9000 rows, each with one row of 3 segments (6000 and 4500 entries): DualEpilogueMg and
+    CheckRowEpilogue write the long rows' terms"""
+    import scipy.sparse as sp
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from test_gpu_zero_skip import planted_lp
+    a = [synthetic_lp(7000, 9000, 5, seed=s, dense_col_nnz=k).a_matrix_.to_scipy() for s, k in ((5, 6000), (6, 4500))]
+    return planted_lp(sp.vstack([a[0].T, a[1].T]), 19, "long_rows")
+
+
 def main():
     world, case = int(sys.argv[1]), sys.argv[2]
     tol = 1e-5
@@ -24,6 +34,8 @@ def main():
         lp = synthetic_lp(6000, 5000, 6, seed=11)
     elif case == "dense":
         lp = synthetic_lp(9000, 7000, 5, seed=5, dense_col_nnz=4000)     # long rows of A' on every rank
+    elif case == "long_rows":
+        lp = long_rows_lp()
     else:
         lp = read_b2lp(os.path.join(ROOT, "tests", "golden", case + ".b2lp"))
         tol = 1e-7
@@ -33,18 +45,28 @@ def main():
     from oracle import binding as ob
     ref = ob.solve(lp, **prm)
     one = engine.solve(lp, ordered_max=-1, **prm)
+    rerun_fails = []
     if len(sys.argv) > 3 and sys.argv[3] == "c_entry":
         # the same thing through the one-call C entry point the HiGHS shim uses for B200PDLP_GPUS > 1, all ranks on device 0
         r = engine.solve_multi(lp, world, devices=[0] * world, **prm)
         res = [r, r]
     else:
         res = engine.solve_logical_shards(lp, world, **prm)
+    if case == "long_rows":
+        # a second solve returns the same bits on every rank: the long rows' terms have fixed slots
+        again = engine.solve_logical_shards(lp, world, **prm)
+        for g, (r, q) in enumerate(zip(res, again)):
+            for k in ("col_value", "col_dual", "row_value", "row_dual"):
+                if not np.array_equal(r[k], q[k]):
+                    rerun_fails.append(f"rank {g} {k}: the second solve differs")
+            if (r["iters"], r["term_code"]) != (q["iters"], q["term_code"]):
+                rerun_fails.append(f"rank {g}: iters/term {q['iters']}/{q['term_code']} in the second solve vs {r['iters']}/{r['term_code']}")
     o_ref = lp.objectiveValue(ref["col_value"])
     out = dict(world=world, case=case, ref_iters=ref["iters"], ref_term=ref["term_code"], ref_obj=o_ref,
                one_gpu_iters=one["iters"], one_gpu_obj=lp.objectiveValue(one["col_value"]),
                iters=[r["iters"] for r in res], term=[r["term_code"] for r in res],
                obj=[lp.objectiveValue(r["col_value"]) for r in res])
-    fails = []
+    fails = list(rerun_fails)
     for g, r in enumerate(res[1:], start=1):   # every rank takes the same decisions and returns the same (complete) solution
         for k in ("col_value", "col_dual", "row_value", "row_dual"):
             if not np.array_equal(r[k], res[0][k]):

@@ -167,17 +167,11 @@ def case_hot_starts():
     pdlp_vs_host("rows_long own iterate", lp, warm=(own["col_value"], own["row_value"], own["row_dual"]), iter_limit=400)
 
 
-# b200pdlp_solve does not reproduce its own bits on cols_long (its 4500-entry columns, one stored in descending row order): two
-# host-array solves on an H100 differed from iteration 10 on.  So that LP is compared in the HiPDLP mode only.
-PDLP_IRREPRODUCIBLE = ("cols_long",)
-
-
 def case_synthetic():
     named = midsize_set() + [("mixed1", mixed_lp(1)), ("classes_differ", classes_differ_lp())]
     for nm, lp in named:
         for ordered_max in (0, -1):
-            if nm not in PDLP_IRREPRODUCIBLE:
-                pdlp_vs_host(nm, lp, ordered_max=ordered_max, iter_limit=1000, tol_primal=1e-5, tol_dual=1e-5)
+            pdlp_vs_host(nm, lp, ordered_max=ordered_max, iter_limit=1000, tol_primal=1e-5, tol_dual=1e-5)
             hip_vs_host(nm, lp, ordered_max=ordered_max, iter_limit=1000, tolerance=1e-5)
 
 

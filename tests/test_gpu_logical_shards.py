@@ -25,7 +25,7 @@ pytestmark = pytest.mark.gpu
 
 @pytest.mark.parametrize("devcheck", [0, 1], ids=["hostcheck", "devcheck"])
 @pytest.mark.parametrize("world,case,mode", [(2, "synthetic", "threads"), (3, "adlittle", "threads"), (4, "dense", "threads"),
-                                             (2, "synthetic", "c_entry")])
+                                             (2, "synthetic", "c_entry"), (2, "long_rows", "threads")])
 def test_logical_shards(world, case, mode, devcheck):
     env = dict(os.environ, B200PDLP_MG_DEVICE_CHECK=str(devcheck))
     try:
