@@ -2203,6 +2203,53 @@ static void finish_order_sums(const std::vector<double>& prst, int nbs, double d
   }
 }
 
+// the state and control blocks of a solve at its check iteration, from the scalars of a b200pdlp_check_in (pushed to the
+// device on the problem's stream; the trace row cleared)
+static SolveCtl* check_api_state(b200pdlp_problem* p, const b200pdlp_check_in* in, bool light) {
+  cudaStream_t s = p->stream;
+  const double nan = std::numeric_limits<double>::quiet_NaN();
+  PdhgState* h = p->hstate;
+  memset(h, 0, sizeof(PdhgState));
+  h->iter = in->iter; h->step_iter = in->step_iter; h->adaptive = in->adaptive; h->pending = in->pending;
+  h->beta = in->beta; h->tau = in->tau; h->sigma = in->sigma; h->sum_step = in->sum_step; h->w_pending = in->w_pending;
+  h->eta = h->tau_try = h->sigma_try = nan;
+  for (int t = 0; t < kPowTab; t++) h->pow_red[t] = h->pow_grow[t] = nan;
+  h->pow_base = -1;
+  h->stop_iter = in->iter; h->cur = 0; h->light_on = light ? 1 : 0; h->done = 0;
+  push_state(p);
+  if (p->trace_dev.n < (size_t)B200PDLP_TRACE_COLS) p->trace_dev.alloc(B200PDLP_TRACE_COLS, false);
+  CUDA_OK(cudaMemsetAsync(p->trace_dev.p, 0, B200PDLP_TRACE_COLS * sizeof(double), s));
+  SolveCtl* c = reset_ctl(p, in->tol_p, in->tol_d, in->tol_gap, in->iter_limit, in->interval, in->restart_on != 0);
+  *p->htime = in->time_flag;
+  c->time_flag = mapped_time_flag(p);
+  c->pf_lr = in->pf_lr; c->df_lr = in->df_lr; c->gap_lr = in->gap_lr;
+  c->pf_lc = in->pf_lc; c->df_lc = in->df_lc; c->gap_lc = in->gap_lc;
+  c->last_restart_iter = in->last_restart_iter;
+  c->trace = p->trace_dev.p; c->trace_cap = 1;
+  CUDA_OK(cudaMemcpyAsync(p->ctl.p, c, sizeof(SolveCtl), cudaMemcpyHostToDevice, s));
+  return c;
+}
+// a b200pdlp_check_out from the control and state blocks after the check (out->trace already downloaded; restart_sq is the
+// caller's)
+static void check_api_out(const SolveCtl* c, const PdhgState* h, b200pdlp_check_out* out) {
+  for (int a = 0; a < 28; a++) out->sums[a] = c->sums[a];
+  for (int t = 0; t < 2; t++) {
+    const DevResiduals& R = c->res[t];
+    const double v[10] = {R.pobj, R.dobj, R.pfeas, R.dfeas, R.gap, R.relgap, R.pinf_obj, R.pinf_res, R.dinf_obj, R.dinf_res};
+    for (int k = 0; k < 10; k++) out->res[t][k] = v[k];
+  }
+  out->term = c->term; out->term_iterate = c->term_iterate;
+  out->restart_choice = c->trace_len > 0 ? (int)out->trace[12] : 0;
+  out->restarts = c->restarts; out->checks = c->checks; out->trace_len = c->trace_len; out->done = h->done;
+  out->stop_iter = h->stop_iter; out->pending = h->pending; out->pow_base = h->pow_base;
+  out->pf_lr = c->pf_lr; out->df_lr = c->df_lr; out->gap_lr = c->gap_lr;
+  out->pf_lc = c->pf_lc; out->df_lc = c->df_lc; out->gap_lc = c->gap_lc;
+  out->last_restart_iter = c->last_restart_iter; out->reserved = 0;
+  out->beta = h->beta; out->tau = h->tau; out->sigma = h->sigma; out->eta = h->eta;
+  out->tau_try = h->tau_try; out->sigma_try = h->sigma_try; out->sum_step = h->sum_step;
+  for (int t = 0; t < kPowTab; t++) { out->pow_red[t] = h->pow_red[t]; out->pow_grow[t] = h->pow_grow[t]; }
+}
+
 int b200pdlp_check_device(b200pdlp_problem* p, const b200pdlp_check_in* in, double* x, double* y, double* ax, double* aty,
                           double* xsum, double* ysum, double* xlr, double* ylr, double* axsum, double* atysum, double* xavg,
                           double* yavg, double* axavg, double* atyavg, b200pdlp_check_out* out) {
@@ -2229,27 +2276,8 @@ int b200pdlp_check_device(b200pdlp_problem* p, const b200pdlp_check_in* in, doub
     upload_perm(p, p->y[0].p, y, p->rperm); upload_perm(p, p->ax[0].p, ax, p->rperm);
     upload_perm(p, p->ysum.p, ysum, p->rperm); upload_perm(p, p->ylr.p, ylr, p->rperm);
     if (light) { upload_perm(p, p->atysum.p, atysum, p->cperm); upload_perm(p, p->axsum.p, axsum, p->rperm); }
-    // the state and control blocks of a solve at its check iteration
-    const double nan = std::numeric_limits<double>::quiet_NaN();
+    SolveCtl* c = check_api_state(p, in, light);
     PdhgState* h = p->hstate;
-    memset(h, 0, sizeof(PdhgState));
-    h->iter = in->iter; h->step_iter = in->step_iter; h->adaptive = in->adaptive; h->pending = in->pending;
-    h->beta = in->beta; h->tau = in->tau; h->sigma = in->sigma; h->sum_step = in->sum_step; h->w_pending = in->w_pending;
-    h->eta = h->tau_try = h->sigma_try = nan;
-    for (int t = 0; t < kPowTab; t++) h->pow_red[t] = h->pow_grow[t] = nan;
-    h->pow_base = -1;
-    h->stop_iter = in->iter; h->cur = 0; h->light_on = light ? 1 : 0; h->done = 0;
-    push_state(p);
-    if (p->trace_dev.n < (size_t)B200PDLP_TRACE_COLS) p->trace_dev.alloc(B200PDLP_TRACE_COLS, false);
-    CUDA_OK(cudaMemsetAsync(p->trace_dev.p, 0, B200PDLP_TRACE_COLS * sizeof(double), s));
-    SolveCtl* c = reset_ctl(p, in->tol_p, in->tol_d, in->tol_gap, in->iter_limit, in->interval, in->restart_on != 0);
-    *p->htime = in->time_flag;
-    c->time_flag = mapped_time_flag(p);
-    c->pf_lr = in->pf_lr; c->df_lr = in->df_lr; c->gap_lr = in->gap_lr;
-    c->pf_lc = in->pf_lc; c->df_lc = in->df_lc; c->gap_lc = in->gap_lc;
-    c->last_restart_iter = in->last_restart_iter;
-    c->trace = p->trace_dev.p; c->trace_cap = 1;
-    CUDA_OK(cudaMemcpyAsync(p->ctl.p, c, sizeof(SolveCtl), cudaMemcpyHostToDevice, s));
     p->launches += enqueue_check_device(p, light);
     CUDA_OK(cudaGetLastError());
     CUDA_OK(cudaMemcpyAsync(c, p->ctl.p, sizeof(SolveCtl), cudaMemcpyDeviceToHost, s));
@@ -2259,24 +2287,9 @@ int b200pdlp_check_device(b200pdlp_problem* p, const b200pdlp_check_in* in, doub
     std::vector<double> prst((size_t)2 * nbs);
     CUDA_OK(cudaMemcpyAsync(prst.data(), p->rs(kSlotK1, n).partials, prst.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
     CUDA_OK(cudaStreamSynchronize(s));
-    for (int a = 0; a < 28; a++) out->sums[a] = c->sums[a];
-    for (int t = 0; t < 2; t++) {
-      const DevResiduals& R = c->res[t];
-      const double v[10] = {R.pobj, R.dobj, R.pfeas, R.dfeas, R.gap, R.relgap, R.pinf_obj, R.pinf_res, R.dinf_obj, R.dinf_res};
-      for (int k = 0; k < 10; k++) out->res[t][k] = v[k];
-    }
-    out->term = c->term; out->term_iterate = c->term_iterate;
-    out->restart_choice = c->trace_len > 0 ? (int)out->trace[12] : 0;
-    out->restarts = c->restarts; out->checks = c->checks; out->trace_len = c->trace_len; out->done = h->done;
-    out->stop_iter = h->stop_iter; out->pending = h->pending; out->pow_base = h->pow_base;
-    out->pf_lr = c->pf_lr; out->df_lr = c->df_lr; out->gap_lr = c->gap_lr;
-    out->pf_lc = c->pf_lc; out->df_lc = c->df_lc; out->gap_lc = c->gap_lc;
-    out->last_restart_iter = c->last_restart_iter; out->reserved = 0;
-    out->beta = h->beta; out->tau = h->tau; out->sigma = h->sigma; out->eta = h->eta;
-    out->tau_try = h->tau_try; out->sigma_try = h->sigma_try; out->sum_step = h->sum_step;
+    check_api_out(c, h, out);
     out->restart_sq[0] = out->restart_sq[1] = 0.0;
     if (out->restart_choice) finish_order_sums(prst, nbs, out->restart_sq);
-    for (int t = 0; t < kPowTab; t++) { out->pow_red[t] = h->pow_red[t]; out->pow_grow[t] = h->pow_grow[t]; }
     download_perm(p, x, p->x[0].p, p->cperm); download_perm(p, aty, p->aty[0].p, p->cperm);
     download_perm(p, xsum, p->xsum.p, p->cperm); download_perm(p, xlr, p->xlr.p, p->cperm);
     download_perm(p, xavg, p->xavg.p, p->cperm); download_perm(p, atyavg, p->atyavg.p, p->cperm);
@@ -2287,12 +2300,12 @@ int b200pdlp_check_device(b200pdlp_problem* p, const b200pdlp_check_in* in, doub
   });
 }
 
-// one record per long row of M: {standard-form row, first slot, segments}; perm maps M's device rows to standard-form order
-static int long_row_records(const DeviceMatrix& M, const std::vector<int>& perm, int32_t* out) {
+// one record per long row of M: {standard-form row, first slot, segments}; row_of maps M's device rows to standard-form order
+static int long_row_records(const DeviceMatrix& M, const std::function<int(int)>& row_of, int32_t* out) {
   std::vector<int4> lr(M.long_rows.n);
   if (!lr.empty()) CUDA_OK(cudaMemcpy(lr.data(), M.long_rows.p, lr.size() * sizeof(int4), cudaMemcpyDeviceToHost));
   for (size_t k = 0; k < lr.size(); k++) {
-    out[3 * k] = perm[lr[k].x];
+    out[3 * k] = row_of(lr[k].x);
     out[3 * k + 1] = M.dev.nblocks_body + lr[k].y;
     out[3 * k + 2] = lr[k].z;
   }
@@ -2331,10 +2344,220 @@ int b200pdlp_pass_partials(b200pdlp_problem* p, const double* x, const double* y
     pull_state(p);
     out->dx2 = p->hstate->dx2; out->dy2 = p->hstate->dy2; out->inter = p->hstate->inter;
     for (int k = 0; k < 3; k++) out->slots[k] = nb[k];
-    out->long_a = long_row_records(p->A, p->rperm, long_rows);
-    out->long_at = long_row_records(p->AT, p->cperm, long_rows + 3 * (size_t)out->long_a);
+    out->long_a = long_row_records(p->A, [&](int r) { return p->rperm[r]; }, long_rows);
+    out->long_at = long_row_records(p->AT, [&](int r) { return p->cperm[r]; }, long_rows + 3 * (size_t)out->long_a);
     download_perm(p, x_new, p->x[1].p, p->cperm); download_perm(p, aty_new, p->aty[1].p, p->cperm);
     download_perm(p, y_new, p->y[1].p, p->rperm); download_perm(p, ax_new, p->ax[1].p, p->rperm);
+  });
+}
+
+// ---- kernel-level entry points on linked logical shards (ranks of this process, b200pdlp_p2p_link_local).  Vectors in
+// standard-form order: each rank takes its column shard (device columns c0 .. c0 + nl_real, padded to nl with zeros) and
+// its row block (standard-form rows r0 + rperm[i]).
+
+// probs[g] must be rank g of a `world` of tree-mode pdlp problems, all linked to each other: a rank whose peers are not
+// its barrier's partners would wait out the barrier's timeout, so anything else is rejected here, before any launch
+static void check_linked_world(b200pdlp_problem* const* probs, int world, const char* who) {
+  if (world < 2 || world > kMaxPeers) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": world must be 2 .. 16");
+  for (int g = 0; g < world; g++)
+    if (!probs[g]) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": null argument");
+  for (int g = 0; g < world; g++) require_mode(probs[g], false, who);
+  for (int g = 0; g < world; g++) {
+    const b200pdlp_problem* p = probs[g];
+    if (p->world != world || p->rank != g)
+      throw Error(B200PDLP_ERR_ARG, std::string(who) + ": problem " + std::to_string(g) + " is not rank " + std::to_string(g) +
+                                        " of a world of " + std::to_string(world));
+    if (p->ordered) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": an ordered-mode problem (its passes add terms, not slots)");
+    bool linked = p->p2p && p->local_link && p->group && p->group == probs[0]->group;
+    for (int h = 0; linked && h < world; h++)
+      linked = p->peers.part[h] == probs[h]->part.p && p->peers.xfull[h] == probs[h]->xfull.p &&
+               p->peers.flags[h] == probs[h]->flags.p && p->peers.recv[h] == probs[h]->recv.p;
+    if (!linked)
+      throw Error(B200PDLP_ERR_ARG, std::string(who) + ": rank " + std::to_string(g) +
+                                        " is not linked to the others (b200pdlp_p2p_link_local)");
+  }
+}
+// column shard: d[i] = v[cperm[c0 + i]] for the real columns, 0 on the padding (as the solve's column vectors are padded)
+static void upload_shard(b200pdlp_problem* p, double* d, const double* v) {
+  std::vector<double> t((size_t)p->nl, 0.0);
+  for (int i = 0; i < p->nl_real; i++) t[i] = v[p->cperm[p->c0 + i]];
+  CUDA_OK(cudaMemcpyAsync(d, t.data(), t.size() * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+  CUDA_OK(cudaStreamSynchronize(p->stream));
+}
+static void download_shard(b200pdlp_problem* p, double* v, const double* d) {
+  std::vector<double> t((size_t)p->nl);
+  CUDA_OK(cudaMemcpyAsync(t.data(), d, t.size() * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+  CUDA_OK(cudaStreamSynchronize(p->stream));
+  for (int i = 0; i < p->nl_real; i++) v[p->cperm[p->c0 + i]] = t[i];
+}
+// a segmented full-length vector (`part`, `xfull`): column j at seg_pos, tails and padding 0
+static void upload_segmented(b200pdlp_problem* p, double* d, const double* v) {
+  std::vector<double> t((size_t)p->world * p->seg_len, 0.0);
+  for (int j = 0; j < p->n; j++) t[seg_pos(p, j)] = v[p->cperm[j]];
+  CUDA_OK(cudaMemcpyAsync(d, t.data(), t.size() * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+  CUDA_OK(cudaStreamSynchronize(p->stream));
+}
+static void download_segmented(b200pdlp_problem* p, double* v, const double* d) {
+  std::vector<double> t((size_t)p->world * p->seg_len);
+  CUDA_OK(cudaMemcpyAsync(t.data(), d, t.size() * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+  CUDA_OK(cudaStreamSynchronize(p->stream));
+  for (int j = 0; j < p->n; j++) v[p->cperm[j]] = t[seg_pos(p, j)];
+}
+
+int b200pdlp_pass_partials_mg(b200pdlp_problem** probs, int32_t world, const b200pdlp_pass_in* in, const double* x,
+                              const double* y, const double* ax, const double* aty, const double* part_in, double* xsum,
+                              double* ysum, double* axsum, double* atysum, double* x_new, double* y_new, double* ax_new,
+                              double* aty_used, double* aty_new, double* part, double* slots, int32_t cap, int32_t* long_rows,
+                              int32_t long_cap, b200pdlp_pass_mg_out* out) {
+  DeviceGuard dg;
+  return guarded([&] {
+    const char* who = "b200pdlp_pass_partials_mg";
+    if (!probs || !in || !x || !y || !ax || !aty || !xsum || !ysum || !axsum || !atysum || !x_new || !y_new || !ax_new ||
+        !aty_used || !aty_new || !part || !slots || !long_rows || !out)
+      throw Error(B200PDLP_ERR_ARG, std::string(who) + ": null argument");
+    check_linked_world(probs, world, who);
+    if (in->iter < 0 || in->step_iter < 0) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": iter and step_iter must be >= 0");
+    int need = 0, need_long = 0;
+    for (int g = 0; g < world; g++) {
+      const b200pdlp_problem* p = probs[g];
+      need = std::max(need, std::max(primal_shard_p2p_grid(p->nl), p->A.grid()));
+      need_long = std::max(need_long, (int)(p->A.long_rows.n + p->AT.long_rows.n));
+    }
+    if (cap < need || long_cap < need_long)
+      throw Error(B200PDLP_ERR_ARG, std::string(who) + ": cap must be >= " + std::to_string(need) + " and long_cap >= " +
+                                        std::to_string(need_long));
+    const size_t n = (size_t)probs[0]->n;
+    LocalGroup& group = *probs[0]->group;
+    run_per_rank(world, "rank", [&](int g) {
+      b200pdlp_problem* p = probs[g];
+      set_device(p);
+      cudaStream_t s = p->stream;
+      // (1) every copy, before any rank launches a kernel that waits for its peers (see LocalGroup)
+      upload_shard(p, p->x[0].p, x); upload_shard(p, p->aty[0].p, aty);
+      upload_shard(p, p->xsum.p, xsum); upload_shard(p, p->atysum.p, atysum);
+      upload_perm(p, p->y[0].p, y + p->r0, p->rperm); upload_perm(p, p->ax[0].p, ax + p->r0, p->rperm);
+      upload_perm(p, p->ysum.p, ysum + p->r0, p->rperm); upload_perm(p, p->axsum.p, axsum + p->r0, p->rperm);
+      if (part_in) upload_segmented(p, p->part.p, part_in + (size_t)g * n);
+      std::vector<int> outpos(p->AT.long_rows.n ? n : 0);   // A_g' rows -> positions in the segmented vector
+      if (!outpos.empty()) CUDA_OK(cudaMemcpy(outpos.data(), p->at_outpos.p, n * sizeof(int), cudaMemcpyDeviceToHost));
+      PdhgState* h = p->hstate;
+      memset(h, 0, sizeof(PdhgState));
+      h->adaptive = 1; h->beta = in->beta; h->eta = in->eta;
+      h->tau = h->tau_try = in->tau; h->sigma = h->sigma_try = in->sigma;
+      h->step_iter = in->step_iter; h->iter = in->iter; h->pending = in->pending; h->w_pending = in->w_pending;
+      h->sum_step = in->sum_step; h->light_on = in->light_on; h->accepted_last = part_in ? 1 : 0;
+      h->stop_iter = std::numeric_limits<int>::max();
+      fill_pow_tables(h);
+      push_state(p);
+      CUDA_OK(cudaMemsetAsync(p->fault.p, 0, sizeof(int), s));
+      CUDA_OK(cudaStreamSynchronize(s));
+      group.arrive_and_wait();
+      // (2) the pass, then the reduce of the partial A_g'y' behind a barrier (as full_aty forms it)
+      enqueue_pass_mg(p);
+      launch_p2p_exchange(s, p->outs.p + 60, 0, p->peers, p->world, p->rank, p->epochs.p, p->fault.p);
+      launch_reduce_part_p2p(s, p->nl, p->atyavg.p, p->peers, p->world, p->rank, p->seg_len, 1);
+      p->launches += p->kernels_per_pass() + 2;
+      CUDA_OK(cudaGetLastError());
+      CUDA_OK(cudaStreamSynchronize(s));
+      group.arrive_and_wait();
+      // (3) downloads, when no barrier kernel is in flight
+      throw_if_peer_fault(p, kPeerLate);
+      unsigned long long ep = 0;
+      CUDA_OK(cudaMemcpy(&ep, p->epochs.p, sizeof(ep), cudaMemcpyDeviceToHost));
+      CUDA_OK(cudaMemcpy(h, p->state.p, sizeof(PdhgState), cudaMemcpyDeviceToHost));
+      b200pdlp_pass_mg_out& o = out[g];
+      o.dx2 = h->dx2; o.dy2 = h->dy2; o.inter = h->inter;
+      o.tau = h->tau; o.sigma = h->sigma; o.tau_try = h->tau_try; o.sigma_try = h->sigma_try; o.eta = h->eta;
+      o.sum_step = h->sum_step; o.w_pending = h->w_pending;
+      o.step_iter = h->step_iter; o.iter = h->iter; o.accepted_last = h->accepted_last; o.pending = h->pending;
+      o.parity = (int)(ep & 1);   // barrier 1 reads the slot of the epoch barrier 0 of this pass reached
+      const int nb1 = primal_shard_p2p_grid(p->nl), nb2 = p->A.grid();
+      o.slots[0] = nb1; o.slots[1] = nb2;
+      double* sl = slots + (size_t)g * 3 * cap;
+      CUDA_OK(cudaMemcpy(sl, p->rs(kSlotK1, 0).partials, (size_t)nb1 * sizeof(double), cudaMemcpyDeviceToHost));
+      CUDA_OK(cudaMemcpy(sl + cap, p->rs(kSlotK2, 0).partials, (size_t)nb2 * sizeof(double), cudaMemcpyDeviceToHost));
+      CUDA_OK(cudaMemcpy(sl + 2 * (size_t)cap, p->rs(kSlotK2, 0).partials + nb2, (size_t)nb2 * sizeof(double),
+                         cudaMemcpyDeviceToHost));
+      int32_t* lr = long_rows + (size_t)g * 3 * long_cap;
+      o.long_a = long_row_records(p->A, [&](int r) { return p->r0 + p->rperm[r]; }, lr);
+      o.long_at = long_row_records(p->AT, [&](int r) {
+        const int pos = outpos[r];
+        return p->cperm[(pos / p->seg_len) * p->shard_len + pos % p->seg_len];
+      }, lr + 3 * (size_t)o.long_a);
+      o.c0 = p->c0; o.nl_real = p->nl_real; o.shard_len = p->shard_len; o.seg_len = p->seg_len; o.r0 = p->r0; o.ml = p->ml;
+      o.reserved = 0;
+      // column shards and row blocks are disjoint: the ranks write different entries of the caller's arrays
+      download_shard(p, x_new, p->x[1].p); download_shard(p, aty_used, p->aty[0].p); download_shard(p, aty_new, p->atyavg.p);
+      download_shard(p, xsum, p->xsum.p); download_shard(p, atysum, p->atysum.p);
+      download_perm(p, y_new + p->r0, p->y[1].p, p->rperm); download_perm(p, ax_new + p->r0, p->ax[1].p, p->rperm);
+      download_perm(p, ysum + p->r0, p->ysum.p, p->rperm); download_perm(p, axsum + p->r0, p->axsum.p, p->rperm);
+      download_segmented(p, part + (size_t)g * n, p->part.p);
+    });
+  });
+}
+
+int b200pdlp_check_device_mg(b200pdlp_problem** probs, int32_t world, const b200pdlp_check_in* in, double* x, double* y,
+                             double* ax, double* aty, double* xsum, double* ysum, double* xlr, double* ylr, double* axsum,
+                             double* atysum, double* xavg, double* yavg, double* axavg, double* atyavg, b200pdlp_check_out* out) {
+  DeviceGuard dg;
+  return guarded([&] {
+    const char* who = "b200pdlp_check_device_mg";
+    if (!probs || !in || !x || !y || !ax || !aty || !xsum || !ysum || !xlr || !ylr || !xavg || !yavg || !axavg || !atyavg ||
+        !out || (in->light && (!axsum || !atysum)))
+      throw Error(B200PDLP_ERR_ARG, std::string(who) + ": null argument");
+    check_linked_world(probs, world, who);
+    if (in->interval < 1 || in->iter < 0 || in->step_iter < 0)
+      throw Error(B200PDLP_ERR_ARG, std::string(who) + ": interval must be >= 1, iter and step_iter >= 0");
+    if (in->light && in->iter >= kDenseChecks)
+      throw Error(B200PDLP_ERR_ARG, std::string(who) + ": the light check needs iter < 10");
+    const bool light = in->light != 0;
+    LocalGroup& group = *probs[0]->group;
+    run_per_rank(world, "rank", [&](int g) {
+      b200pdlp_problem* p = probs[g];
+      set_device(p);
+      cudaStream_t s = p->stream;
+      // (1) every copy, allocation and graph instantiation before any rank launches a kernel that waits for its peers: the
+      // check runs as the graph the solve replays
+      upload_shard(p, p->x[0].p, x); upload_shard(p, p->aty[0].p, aty);
+      upload_shard(p, p->xsum.p, xsum); upload_shard(p, p->xlr.p, xlr);
+      upload_perm(p, p->y[0].p, y + p->r0, p->rperm); upload_perm(p, p->ax[0].p, ax + p->r0, p->rperm);
+      upload_perm(p, p->ysum.p, ysum + p->r0, p->rperm); upload_perm(p, p->ylr.p, ylr + p->r0, p->rperm);
+      if (light) { upload_shard(p, p->atysum.p, atysum); upload_perm(p, p->axsum.p, axsum + p->r0, p->rperm); }
+      SolveCtl* c = check_api_state(p, in, light);   // (accepted_last = 0: aty stays the caller's)
+      PdhgState* h = p->hstate;
+      cudaGraphExec_t& ge = light ? p->graph_check_light : p->graph_check;
+      if (!ge) {
+        ge = capture_check(p, light, &p->check_launches[light ? 1 : 0]);
+        CUDA_OK(cudaGraphUpload(ge, s));
+      }
+      CUDA_OK(cudaMemsetAsync(p->fault.p, 0, sizeof(int), s));
+      CUDA_OK(cudaStreamSynchronize(s));
+      group.arrive_and_wait();
+      // (2) the check
+      CUDA_OK(cudaGraphLaunch(ge, s));
+      p->launches += p->check_launches[light ? 1 : 0];
+      CUDA_OK(cudaStreamSynchronize(s));
+      group.arrive_and_wait();
+      // (3) downloads, when no barrier kernel is in flight
+      throw_if_peer_fault(p, kPeerLate);
+      b200pdlp_check_out& o = out[g];
+      CUDA_OK(cudaMemcpy(c, p->ctl.p, sizeof(SolveCtl), cudaMemcpyDeviceToHost));
+      CUDA_OK(cudaMemcpy(h, p->state.p, sizeof(PdhgState), cudaMemcpyDeviceToHost));
+      CUDA_OK(cudaMemcpy(o.trace, p->trace_dev.p, B200PDLP_TRACE_COLS * sizeof(double), cudaMemcpyDeviceToHost));
+      double rsq[2];   // on a restart: the all-reduced |x - xlr|^2, |y - ylr|^2 the finish kernel read
+      CUDA_OK(cudaMemcpy(rsq, p->outs.p + 40, sizeof(rsq), cudaMemcpyDeviceToHost));
+      check_api_out(c, h, &o);
+      o.restart_sq[0] = o.restart_choice ? rsq[0] : 0.0;
+      o.restart_sq[1] = o.restart_choice ? rsq[1] : 0.0;
+      // column shards and row blocks are disjoint: the ranks write different entries of the caller's arrays
+      download_shard(p, x, p->x[0].p); download_shard(p, aty, p->aty[0].p);
+      download_shard(p, xsum, p->xsum.p); download_shard(p, xlr, p->xlr.p);
+      download_shard(p, xavg, p->xavg.p); download_shard(p, atyavg, p->atyavg.p);
+      download_perm(p, y + p->r0, p->y[0].p, p->rperm); download_perm(p, ax + p->r0, p->ax[0].p, p->rperm);
+      download_perm(p, ysum + p->r0, p->ysum.p, p->rperm); download_perm(p, ylr + p->r0, p->ylr.p, p->rperm);
+      download_perm(p, yavg + p->r0, p->yavg.p, p->rperm); download_perm(p, axavg + p->r0, p->axavg.p, p->rperm);
+      if (light) { download_shard(p, atysum, p->atysum.p); download_perm(p, axsum + p->r0, p->axsum.p, p->rperm); }
+    });
   });
 }
 

@@ -6,6 +6,7 @@ entry point raises `EngineError`.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import os
 
@@ -80,6 +81,23 @@ CHECK_VECTORS = ("x", "y", "ax", "aty", "xsum", "ysum", "xlr", "ylr", "axsum", "
 RESIDUAL_NAMES = ("pobj", "dobj", "pfeas", "dfeas", "gap", "relgap", "pinf_obj", "pinf_res", "dinf_obj", "dinf_res")
 
 
+class CPassIn(C.Structure):
+    """b200pdlp_pass_in: the PdhgState scalars of one fused multi-GPU pass (b200pdlp_pass_partials_mg)"""
+    _fields_ = [("tau", C.c_double), ("sigma", C.c_double), ("beta", C.c_double), ("eta", C.c_double),
+                ("w_pending", C.c_double), ("sum_step", C.c_double), ("step_iter", C.c_int32), ("iter", C.c_int32),
+                ("pending", C.c_int32), ("light_on", C.c_int32)]
+
+
+class CPassMgOut(C.Structure):
+    """b200pdlp_pass_mg_out: one rank's state after the pass, and the sizes of what it returned"""
+    _fields_ = [("dx2", C.c_double), ("dy2", C.c_double), ("inter", C.c_double), ("tau", C.c_double), ("sigma", C.c_double),
+                ("tau_try", C.c_double), ("sigma_try", C.c_double), ("eta", C.c_double), ("sum_step", C.c_double),
+                ("w_pending", C.c_double), ("step_iter", C.c_int32), ("iter", C.c_int32), ("accepted_last", C.c_int32),
+                ("pending", C.c_int32), ("parity", C.c_int32), ("slots", C.c_int32 * 2), ("long_a", C.c_int32),
+                ("long_at", C.c_int32), ("c0", C.c_int32), ("nl_real", C.c_int32), ("shard_len", C.c_int32),
+                ("seg_len", C.c_int32), ("r0", C.c_int32), ("ml", C.c_int32), ("reserved", C.c_int32)]
+
+
 class CWarm(C.Structure):
     _fields_ = [("col_value", _dp), ("row_value", _dp), ("row_dual", _dp)]
 
@@ -116,7 +134,8 @@ ABI_SYMBOLS = [
     "b200pdlp_kkt_check_batch_device", "b200pdlp_hipdlp_problem_create", "b200pdlp_hipdlp_step", "b200pdlp_hipdlp_check",
     "b200pdlp_hipdlp_problem_power_method", "b200pdlp_solve_hipdlp_batch_mixed",
     "b200pdlp_solve_hipdlp_batch_mixed_device", "b200pdlp_debug_hipdlp_tree_prep_compare", "b200pdlp_check_device",
-    "b200pdlp_solve_device", "b200pdlp_solve_hipdlp_device", "b200pdlp_pass_partials",
+    "b200pdlp_solve_device", "b200pdlp_solve_hipdlp_device", "b200pdlp_pass_partials", "b200pdlp_pass_partials_mg",
+    "b200pdlp_check_device_mg",
 ]
 HIP_TRACE_COLS = 16   # B200PDLP_HIP_TRACE_COLS: the per-block trace of the HiPDLP solves
 
@@ -195,6 +214,10 @@ def lib():
         L.b200pdlp_check_device.argtypes = [C.c_void_p, C.POINTER(CCheckIn)] + [_dp] * 14 + [C.POINTER(CCheckOut)]
         L.b200pdlp_pass_partials.argtypes = ([C.c_void_p] + [_dp] * 4 + [C.c_double] * 2 + [_dp] * 5 +
                                              [C.c_int32, _ip, C.c_int32, C.POINTER(CPassOut)])
+        L.b200pdlp_check_device_mg.argtypes = ([C.POINTER(C.c_void_p), C.c_int32, C.POINTER(CCheckIn)] + [_dp] * 14 +
+                                               [C.POINTER(CCheckOut)])
+        L.b200pdlp_pass_partials_mg.argtypes = ([C.POINTER(C.c_void_p), C.c_int32, C.POINTER(CPassIn)] + [_dp] * 15 +
+                                                [_dp, C.c_int32, _ip, C.c_int32, C.POINTER(CPassMgOut)])
         _lib = L
     return _lib
 
@@ -867,6 +890,30 @@ def solve_multi(lp: HighsLp, ngpus: int, devices=None, warm=None, **params) -> d
     return _result_dict(res, arrays)
 
 
+def _check_args(n, m, x, y, ax, aty, xsum, ysum, xlr, ylr, axsum, atysum, scalars):
+    """a b200pdlp_check_in from the scalars, copies of the vectors (standard-form order) and their pointers"""
+    cin = CCheckIn()
+    for k, v in scalars.items():
+        if not hasattr(cin, k):
+            raise TypeError(f"unknown check_device field {k}")
+        setattr(cin, k, v)
+    vec = lambda v, ln: np.array(v, dtype=np.float64, copy=True).reshape(ln)
+    v = dict(x=vec(x, n), y=vec(y, m), ax=vec(ax, m), aty=vec(aty, n), xsum=vec(xsum, n), ysum=vec(ysum, m),
+             xlr=vec(xlr, n), ylr=vec(ylr, m), xavg=np.zeros(n), yavg=np.zeros(m), axavg=np.zeros(m), atyavg=np.zeros(n))
+    if cin.light:
+        v["axsum"], v["atysum"] = vec(axsum, m), vec(atysum, n)
+    return cin, v, [_p(v[k], _dp) if k in v else None for k in CHECK_VECTORS]
+
+
+def _check_out_dict(out) -> dict:
+    r = {}
+    for k, t in CCheckOut._fields_:
+        a = getattr(out, k)
+        r[k] = np.ctypeslib.as_array(a).copy() if hasattr(t, "_length_") else a
+    r["res"] = [dict(zip(RESIDUAL_NAMES, r["res"][t].tolist())) for t in range(2)]
+    return r
+
+
 class Problem:
     """Persistent device-resident problem (b200pdlp_problem_*)."""
 
@@ -949,26 +996,10 @@ class Problem:
         fields of b200pdlp_check_in (iter, tau, ..., light, time_flag).  Returns the fields of b200pdlp_check_out as numbers
         and arrays ("res" as two dicts keyed by RESIDUAL_NAMES) and every vector of CHECK_VECTORS after the check (axsum /
         atysum only for light = 1)."""
-        n, m = self.n, self.m
-        cin = CCheckIn()
-        for k, v in scalars.items():
-            if not hasattr(cin, k):
-                raise TypeError(f"unknown check_device field {k}")
-            setattr(cin, k, v)
-        light = bool(cin.light)
-        vec = lambda v, ln: np.array(v, dtype=np.float64, copy=True).reshape(ln)
-        v = dict(x=vec(x, n), y=vec(y, m), ax=vec(ax, m), aty=vec(aty, n), xsum=vec(xsum, n), ysum=vec(ysum, m),
-                 xlr=vec(xlr, n), ylr=vec(ylr, m), xavg=np.zeros(n), yavg=np.zeros(m), axavg=np.zeros(m), atyavg=np.zeros(n))
-        if light:
-            v["axsum"], v["atysum"] = vec(axsum, m), vec(atysum, n)
+        cin, v, ptrs = _check_args(self.n, self.m, x, y, ax, aty, xsum, ysum, xlr, ylr, axsum, atysum, scalars)
         out = CCheckOut()
-        ptrs = [_p(v[k], _dp) if k in v else None for k in CHECK_VECTORS]
         _check(lib().b200pdlp_check_device(self._h, C.byref(cin), *ptrs, C.byref(out)), "b200pdlp_check_device")
-        r = {}
-        for k, t in CCheckOut._fields_:
-            a = getattr(out, k)
-            r[k] = np.ctypeslib.as_array(a).copy() if hasattr(t, "_length_") else a
-        r["res"] = [dict(zip(RESIDUAL_NAMES, r["res"][t].tolist())) for t in range(2)]
+        r = _check_out_dict(out)
         r.update(v)
         return r
 
@@ -1226,10 +1257,7 @@ def solve_logical_shards(lp: HighsLp, world: int, device: int = -1, **params) ->
     device): one problem per rank, buffers wired to each other with b200pdlp_p2p_link_local, one host thread per rank
     (ctypes releases the GIL during the solve).  Returns the per-rank result dicts (identical by construction)."""
     import threading
-    probs = [Problem(lp, rank=g, world=world, device=device, **params) for g in range(world)]
-    try:
-        arr = (C.c_void_p * world)(*[q._h for q in probs])
-        _check(lib().b200pdlp_p2p_link_local(arr, world), "b200pdlp_p2p_link_local")
+    with linked_shards(lp, world, device=device, **params) as probs:
         out, err = [None] * world, [None] * world
 
         def run(g):
@@ -1247,6 +1275,19 @@ def solve_logical_shards(lp: HighsLp, world: int, device: int = -1, **params) ->
             if e is not None:
                 raise e
         return out
+
+
+@contextlib.contextmanager
+def linked_shards(lp: HighsLp, world: int, device: int = -1, **params):
+    """`world` problems of `lp` (rank g at index g) in this process, linked with b200pdlp_p2p_link_local: the logical shards
+    of solve_logical_shards and of the multi-GPU kernel-level entry points.  Released and closed on exit."""
+    probs = []
+    try:
+        for g in range(world):
+            probs.append(Problem(lp, rank=g, world=world, device=device, **params))
+        arr = (C.c_void_p * world)(*[q._h for q in probs])
+        _check(lib().b200pdlp_p2p_link_local(arr, world), "b200pdlp_p2p_link_local")
+        yield probs
     finally:
         for q in probs:
             try:
@@ -1255,6 +1296,68 @@ def solve_logical_shards(lp: HighsLp, world: int, device: int = -1, **params) ->
                 pass
         for q in probs:
             q.close()
+
+
+def _handles(probs):
+    return (C.c_void_p * len(probs))(*[q._h for q in probs])
+
+
+def check_device_mg(probs, x, y, ax, aty, xsum, ysum, xlr, ylr, axsum=None, atysum=None, **scalars) -> dict:
+    """One device check on linked ranks (b200pdlp_check_device_mg; probs from linked_shards): Problem.check_device's
+    arguments and vectors, and "ranks", the fields of every rank's b200pdlp_check_out as Problem.check_device returns them
+    (the top level holds rank 0's)."""
+    world = len(probs)
+    cin, v, ptrs = _check_args(probs[0].n, probs[0].m, x, y, ax, aty, xsum, ysum, xlr, ylr, axsum, atysum, scalars)
+    out = (CCheckOut * world)()
+    _check(lib().b200pdlp_check_device_mg(_handles(probs), world, C.byref(cin), *ptrs, out), "b200pdlp_check_device_mg")
+    ranks = [_check_out_dict(out[g]) for g in range(world)]
+    r = dict(ranks[0])
+    r.update(v)
+    r["ranks"] = ranks
+    r["raw"] = [bytes(out[g]) for g in range(world)]
+    return r
+
+
+def pass_partials_mg(probs, x, y, ax, aty, part_in=None, xsum=None, ysum=None, axsum=None, atysum=None, **scalars) -> dict:
+    """One fused multi-GPU PDHG pass on linked ranks (b200pdlp_pass_partials_mg; probs from linked_shards).  Vectors in
+    standard-form order; part_in [world][n]: the ranks' partial A_g'y, which the primal kernel then adds up; the sums default
+    to zeros.  Scalars: the fields of b200pdlp_pass_in.  Returns x_new, y_new, ax_new, aty_used, aty_new, part (world x n)
+    and the four sums after the pass, and "ranks": per rank the fields of b200pdlp_pass_mg_out, its slot arrays k1, k2_dy2,
+    k2_inter and its long-row records long_a, long_at ({standard-form row, first slot, segments})."""
+    world, n, m, nnz = len(probs), probs[0].n, probs[0].m, probs[0].nnz
+    cin = CPassIn()
+    for k, v in scalars.items():
+        if not hasattr(cin, k):
+            raise TypeError(f"unknown pass_partials_mg field {k}")
+        setattr(cin, k, v)
+    vec = lambda v, ln: np.zeros(ln) if v is None else np.array(v, dtype=np.float64, copy=True).reshape(ln)
+    v = dict(x=vec(x, n), y=vec(y, m), ax=vec(ax, m), aty=vec(aty, n), xsum=vec(xsum, n), ysum=vec(ysum, m),
+             axsum=vec(axsum, m), atysum=vec(atysum, n), x_new=np.zeros(n), y_new=np.zeros(m), ax_new=np.zeros(m),
+             aty_used=np.zeros(n), aty_new=np.zeros(n), part=np.zeros((world, n)))
+    pin = None if part_in is None else np.array(part_in, dtype=np.float64, copy=True).reshape(world, n)
+    # slot bounds as in Problem.pass_partials: the primal kernel's grid is capped at 16 x 148 CTAs; A_g has at most one CTA
+    # per 256 rows and one per started 2048 entries of a long row
+    nlong = nnz // 513 + 1
+    cap = max(16 * 148, (max(n, m) + 255) // 256 + nnz // 2048 + nlong)
+    slots = np.zeros((world, 3, cap))
+    lr = np.zeros((world, 2 * nlong, 3), dtype=np.int32)
+    out = (CPassMgOut * world)()
+    order = ("x", "y", "ax", "aty")
+    io = ("xsum", "ysum", "axsum", "atysum", "x_new", "y_new", "ax_new", "aty_used", "aty_new", "part")
+    _check(lib().b200pdlp_pass_partials_mg(_handles(probs), world, C.byref(cin), *(_p(v[k], _dp) for k in order),
+                                           None if pin is None else _p(pin, _dp), *(_p(v[k], _dp) for k in io),
+                                           _p(slots, _dp), cap, _p(lr, _ip), lr.shape[1], out), "b200pdlp_pass_partials_mg")
+    ranks = []
+    for g in range(world):
+        o = out[g]
+        r = {k: (list(getattr(o, k)) if k == "slots" else getattr(o, k)) for k, _ in CPassMgOut._fields_}
+        nb1, nb2 = o.slots[0], o.slots[1]
+        r.update(k1=slots[g, 0, :nb1].copy(), k2_dy2=slots[g, 1, :nb2].copy(), k2_inter=slots[g, 2, :nb2].copy(),
+                 long_a=lr[g, :o.long_a].copy(), long_at=lr[g, o.long_a:o.long_a + o.long_at].copy())
+        ranks.append(r)
+    res = {k: v[k] for k in io}
+    res["ranks"] = ranks
+    return res
 
 
 def device_count() -> int:

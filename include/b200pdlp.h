@@ -307,6 +307,56 @@ int b200pdlp_pass_partials(b200pdlp_problem* p, const double* x, const double* y
                            double tau, double sigma, double* x_new, double* y_new, double* ax_new, double* aty_new,
                            double* slots, int32_t cap, int32_t* long_rows, int32_t long_cap, b200pdlp_pass_out* out);
 
+/* One fused PDHG pass of a multi-GPU solve on linked ranks (parity tests): probs[g] is rank g of a world of `world`
+ * tree-mode problems linked by b200pdlp_p2p_link_local.  Every rank runs, on its own host thread, the five launches of the
+ * solve's pass (primal_shard_p2p_kernel, barrier 0, A_g x' + dual step, partial A_g'y', barrier 1 with the step rule), then
+ * a barrier and the reduce of the peers' partial A_g'y' into its shard.  Uploads come before a host rendezvous and downloads
+ * after a second one, so no blocking driver call meets a barrier kernel that waits for a peer.
+ * The scalars in `in` become every rank's PdhgState (tau = tau_try, sigma = sigma_try, the step rule's power tables filled
+ * from step_iter as the solve fills them).  Vectors are host arrays in standard-form order; each rank takes its column
+ * shard and its row block from them, and the results are assembled.  Inputs: x, aty (n), y, ax (m); part_in [world][n]
+ * (optional): rank g's partial A_g'y, seeded into its `part` buffer, so that the primal kernel adds the ranks' partials
+ * (accepted_last = 1) instead of reading aty.  In and out: xsum, atysum (n), ysum, axsum (m).  Written: x_new,
+ * aty_used (the A'y the primal kernel used), aty_new (the reduced A'y') (n), y_new, ax_new (m), part [world][n] (each rank's
+ * partial A_g'y').
+ * slots[world][3][cap]: rank g's block partials of the primal kernel (|dx|^2) and of A_g x' (|dy|^2, then the interaction),
+ * out[g].slots[0] and out[g].slots[1] entries.  long_rows[world][long_cap][3]: rank g's records {standard-form row, first
+ * slot, segments} per long row of A_g (out[g].long_a), then per long row of A_g' (out[g].long_at; the row is a column).
+ * Rejected with B200PDLP_ERR_ARG before anything is written and before any launch: NULL arguments, world outside 2..16, a
+ * problem that is not rank g of this world at probs[g], is not linked to the others, is in ordered mode or is a HiPDLP
+ * problem, iter or step_iter < 0, and cap or long_cap below what a rank needs. */
+typedef struct {
+  double tau, sigma, beta, eta, w_pending, sum_step;
+  int32_t step_iter, iter, pending, light_on;
+} b200pdlp_pass_in;
+typedef struct {
+  double dx2, dy2, inter;   /* the sums of every rank's scalars the step rule read */
+  double tau, sigma, tau_try, sigma_try, eta, sum_step, w_pending;   /* after the step rule */
+  int32_t step_iter, iter, accepted_last, pending;
+  int32_t parity;           /* epochs[0] & 1 after the pass: by barrier 1's rule, the tail slot it reads |dx|^2 from */
+  int32_t slots[2];         /* block partials of the primal kernel, of A_g x' (per accumulator) */
+  int32_t long_a, long_at;  /* long rows of A_g, of A_g' */
+  int32_t c0, nl_real, shard_len, seg_len, r0, ml;   /* the rank's column shard and row block */
+  int32_t reserved;
+} b200pdlp_pass_mg_out;
+int b200pdlp_pass_partials_mg(b200pdlp_problem** probs, int32_t world, const b200pdlp_pass_in* in, const double* x,
+                              const double* y, const double* ax, const double* aty, const double* part_in, double* xsum,
+                              double* ysum, double* axsum, double* atysum, double* x_new, double* y_new, double* ax_new,
+                              double* aty_used, double* aty_new, double* part, double* slots, int32_t cap, int32_t* long_rows,
+                              int32_t long_cap, b200pdlp_pass_mg_out* out);
+
+/* b200pdlp_check_device on linked ranks (parity tests): probs[g] is rank g of a world of `world` tree-mode problems linked
+ * by b200pdlp_p2p_link_local.  Every rank runs, on its own host thread, the check graph the multi-GPU solve replays
+ * (engine.cu enqueue_check_device_mg: full or, for light = 1, the dense-check phase's variant), captured and uploaded before
+ * a host rendezvous; downloads come after a second one.  `in` and the vectors are those of b200pdlp_check_device, full
+ * length in standard-form order; each rank takes its column shard and row block from them, and the results are assembled.
+ * out[world]: one b200pdlp_check_out per rank (restart_sq: the all-reduced sums the finish kernel read).
+ * Rejected with B200PDLP_ERR_ARG before anything is written and before any launch: NULL arguments, and everything
+ * b200pdlp_pass_partials_mg and b200pdlp_check_device reject on their own problems and scalars. */
+int b200pdlp_check_device_mg(b200pdlp_problem** probs, int32_t world, const b200pdlp_check_in* in, double* x, double* y,
+                             double* ax, double* aty, double* xsum, double* ysum, double* xlr, double* ylr, double* axsum,
+                             double* atysum, double* xavg, double* yavg, double* axavg, double* atyavg, b200pdlp_check_out* out);
+
 /* device-pointer variants on the problem's stream (bench roofline loop):
  * time `reps` back-to-back launches with CUDA events; returns ms in *ms_total */
 int b200pdlp_bench_spmv(b200pdlp_problem* p, int32_t which /*0 Ax, 1 ATy*/, int32_t reps, float* ms_total);
