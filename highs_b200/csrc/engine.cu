@@ -104,6 +104,16 @@ void apply_spmv_grid(b200pdlp_problem* p) {
     zskip(p->A, p->n);
     zskip(p->AT, p->m);
   }
+  // L2 cache policies of K1 and the zero-skip K2 / K3 (L2Hints in pdhg_kernels.cu) where one copy of the matrix does not fit
+  // in L2: there nothing the pass streams survives to the next pass anyway, and evict-first keeps x' and y' resident for the
+  // gathers.  Where it fits (S2: 12 MB), the whole pass stays in L2 from one iteration to the next and evict-first would
+  // throw that away.  Measured on one H100 (DESIGN.md section 6).
+  if (!p->form.hipdlp) {
+    int l2 = 0;
+    cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, p->device);
+    const int hints = 12 * (long long)p->form.nnz >= l2 ? 1 : 0;
+    p->A.dev.l2_hints = p->AT.dev.l2_hints = hints;
+  }
   if (getenv("B200PDLP_TIMING")) {
     fprintf(stderr, "[b200pdlp setup] SpMV shapes: A %s (%d CTAs, tiles staged %d/%d)  A' %s (%d CTAs, tiles staged %d/%d)\n",
             p->A.dev.tiled ? "tiled" : (p->A.dev.pipelined ? "persistent" : "one slice per warp"), p->A.dev.nblocks_body,
@@ -588,7 +598,7 @@ static void enqueue_pass(b200pdlp_problem* p) {
   PdhgState* st = p->state.p;
   const ReduceScratch r1 = p->rs(kSlotK1, p->n), r2 = p->rs(kSlotK2, p->ml), r3 = p->rs(kSlotK3, p->n);
   launch_primal_step(s, p->n, st, p->x[0].p, p->x[1].p, p->aty[0].p, p->aty[1].p, p->cost.p, p->lower.p,
-                     p->upper.p, p->xsum.p, r1, p->A.dev.nzmap);
+                     p->upper.p, p->xsum.p, r1, p->A.dev.nzmap, p->A.dev.l2_hints);
   launch_spmv_dual(s, p->A.dev, st, p->x[0].p, p->x[1].p, p->y[0].p, p->y[1].p, p->ax[0].p, p->ax[1].p,
                    p->rhs.p, p->ysum.p, p->neq_local, 0, r2, p->axsum.p, p->AT.dev.nzmap);
   launch_spmv_primal(s, p->AT.dev, st, p->y[0].p, p->y[1].p, p->x[0].p, p->x[1].p, p->aty[0].p, p->aty[1].p, r3, p->atysum.p);
@@ -2114,7 +2124,7 @@ int b200pdlp_primal_step(b200pdlp_problem* p, const double* x, const double* aty
     kernel_api_state(p, tau, tau);
     const ReduceScratch r1 = p->rs(kSlotK1, n);
     launch_primal_step(p->stream, n, p->state.p, p->x[0].p, p->x[1].p, p->aty[0].p, p->aty[1].p, p->cost.p, p->lower.p,
-                       p->upper.p, p->xsum.p, r1, p->A.dev.nzmap);
+                       p->upper.p, p->xsum.p, r1, p->A.dev.nzmap, p->A.dev.l2_hints);
     p->launches++;
     download_perm(p, x_new, p->x[1].p, p->cperm);
     if (dx2) *dx2 = sum_partials(p, r1, primal_step_grid(n));
@@ -2607,7 +2617,7 @@ int b200pdlp_bench_pass(b200pdlp_problem* p, int32_t reps, float ms[4]) {
         const ReduceScratch r1 = p->rs(kSlotK1, p->n), r2 = p->rs(kSlotK2, p->ml), r3 = p->rs(kSlotK3, p->n);
         CUDA_OK(cudaEventRecord(ev[0], s));
         launch_primal_step(s, p->n, st, p->x[0].p, p->x[1].p, p->aty[0].p, p->aty[1].p, p->cost.p, p->lower.p,
-                           p->upper.p, p->xsum.p, r1, p->A.dev.nzmap);
+                           p->upper.p, p->xsum.p, r1, p->A.dev.nzmap, p->A.dev.l2_hints);
         CUDA_OK(cudaEventRecord(ev[1], s));
         launch_spmv_dual(s, p->A.dev, st, p->x[0].p, p->x[1].p, p->y[0].p, p->y[1].p, p->ax[0].p, p->ax[1].p,
                          p->rhs.p, p->ysum.p, p->neq_local, 0, r2, nullptr, p->AT.dev.nzmap);

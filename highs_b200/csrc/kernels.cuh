@@ -143,6 +143,7 @@ struct DevSell {
   int zskip_grid;
   int nz_bytes;                           // staged bytes: the bitmap rounded up to 16 bytes
   unsigned* nzmap;
+  int l2_hints;                           // 1: K1 and the zero-skip K2 / K3 load and store with L2 cache policies (L2Hints)
 };
 constexpr int kTileSlices = 256;          // slices per tile (8192 rows)
 constexpr int kTileThreads = 1024;

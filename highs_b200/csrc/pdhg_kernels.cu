@@ -1,14 +1,100 @@
 // highs_b200/csrc/pdhg_kernels.cu -- kernel definitions + launchers (see kernels.cuh).
+#include <utility>
+
 #include "pdhg_arith.cuh"
 #include "pdhg_kernels.hpp"
 
 namespace b200 {
+
+// ============================================================ L2 cache policies of the pass kernels
+// A one-GPU pass streams 50-100 MB of data it touches once (K1: c, l, u, aty, xSum; K2 / K3: the matrix and the epilogue
+// vectors) between the store of x' (y') and its random gathers, which read one 32-byte sector per entry and are as many
+// bytes as the matrix stream.  x' and y' (8 MB each at S3) fit in L2; under the default policy the streams evict them.  So
+// K1, K2 and K3 on the zero-skip shape load what they read once evict-first and store x', y' and their bitmaps, and gather
+// them, evict-last.  Per instruction only (createpolicy + .L2::cache_hint): no L2 set-aside, no access-policy window.
+// The descriptors are compile-time constants (SASS: a UMOV, no load per access).  Loads marked .nc read data that no thread
+// of the kernel writes.
+struct L2Hints {
+  unsigned long long first, last;
+  __device__ __forceinline__ static L2Hints make() {
+    L2Hints h;
+    asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(h.first));
+    asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(h.last));
+    return h;
+  }
+};
+// read once: evict-first
+__device__ __forceinline__ int ld_stream(const int* p, unsigned long long pol) {
+  int v;
+  asm("ld.global.nc.L2::cache_hint.b32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
+  return v;
+}
+__device__ __forceinline__ int4 ld_stream(const int4* p, unsigned long long pol) {
+  int4 v;
+  asm("ld.global.nc.L2::cache_hint.v4.b32 {%0, %1, %2, %3}, [%4], %5;" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p), "l"(pol));
+  return v;
+}
+__device__ __forceinline__ double ld_stream(const double* p, unsigned long long pol) {
+  double v;
+  asm("ld.global.nc.L2::cache_hint.f64 %0, [%1], %2;" : "=d"(v) : "l"(p), "l"(pol));
+  return v;
+}
+__device__ __forceinline__ double2 ld_stream(const double2* p, unsigned long long pol) {
+  double2 v;
+  asm("ld.global.nc.L2::cache_hint.v2.f64 {%0, %1}, [%2], %3;" : "=d"(v.x), "=d"(v.y) : "l"(p), "l"(pol));
+  return v;
+}
+// read once by the thread that then writes it (xSum, ySum, A xSum, A'ySum): evict-first, through the coherent path
+__device__ __forceinline__ double ld_stream_rw(const double* p, unsigned long long pol) {
+  double v;
+  asm("ld.global.L2::cache_hint.f64 %0, [%1], %2;" : "=d"(v) : "l"(p), "l"(pol));
+  return v;
+}
+__device__ __forceinline__ double2 ld_stream_rw(const double2* p, unsigned long long pol) {
+  double2 v;
+  asm("ld.global.L2::cache_hint.v2.f64 {%0, %1}, [%2], %3;" : "=d"(v.x), "=d"(v.y) : "l"(p), "l"(pol));
+  return v;
+}
+// the gathers of x' / y': evict-last
+__device__ __forceinline__ double ld_keep(const double* p, unsigned long long pol) {
+  double v;
+  asm("ld.global.nc.L2::cache_hint.f64 %0, [%1], %2;" : "=d"(v) : "l"(p), "l"(pol));
+  return v;
+}
+// x' / y' and their bitmaps, handed to the next kernel's gathers: evict-last
+__device__ __forceinline__ void st_keep(double* p, double v, unsigned long long pol) {
+  asm volatile("st.global.L2::cache_hint.f64 [%0], %1, %2;" ::"l"(p), "d"(v), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void st_keep(double2* p, double2 v, unsigned long long pol) {
+  asm volatile("st.global.L2::cache_hint.v2.f64 [%0], {%1, %2}, %3;" ::"l"(p), "d"(v.x), "d"(v.y), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void st_keep(unsigned* p, unsigned v, unsigned long long pol) {
+  asm volatile("st.global.L2::cache_hint.b32 [%0], %1, %2;" ::"l"(p), "r"(v), "l"(pol) : "memory");
+}
+// the loads and stores that take a policy: PlainMem leaves them to the compiler (every other kernel, and K1 / K2 / K3 where
+// one copy of the matrix fits in L2: DevSell::l2_hints), HintedMem applies the policies above
+struct PlainMem {
+  __device__ __forceinline__ static PlainMem make() { return {}; }
+  template <class T> __device__ __forceinline__ T gather(const T* p) const { return *p; }
+  template <class T> __device__ __forceinline__ T stream(const T* p) const { return *p; }
+  template <class T> __device__ __forceinline__ T stream_rw(const T* p) const { return *p; }
+  template <class T> __device__ __forceinline__ void keep(T* p, T v) const { *p = v; }
+};
+struct HintedMem {
+  L2Hints h;
+  __device__ __forceinline__ static HintedMem make() { return {L2Hints::make()}; }
+  template <class T> __device__ __forceinline__ T gather(const T* p) const { return ld_keep(p, h.last); }
+  template <class T> __device__ __forceinline__ T stream(const T* p) const { return ld_stream(p, h.first); }
+  template <class T> __device__ __forceinline__ T stream_rw(const T* p) const { return ld_stream_rw(p, h.first); }
+  template <class T> __device__ __forceinline__ void keep(T* p, T v) const { st_keep(p, v, h.last); }
+};
 
 // =============================================================== K1: primal step
 // PDHG_primalGradientStep (CPU operation order, cupdlp_step.c:28-38):
 //   x' = x; x' += (-tau) c; x' += tau aty; x' = min(x', u); x' = max(x', l)
 // fused with |x - x'|^2 (cupdlp_linalg.c:790) and the deferred average update
 // xSum += w x (PDHG_Update_Average, cupdlp_step.c:436) of the previous accepted step.
+template <class M>
 __global__ void __launch_bounds__(kThreads)
 primal_step_kernel(int n, PdhgState* __restrict__ st, double* __restrict__ x0, double* __restrict__ x1,
                    const double* __restrict__ aty0, const double* __restrict__ aty1,
@@ -31,17 +117,18 @@ primal_step_kernel(int n, PdhgState* __restrict__ st, double* __restrict__ x0, d
   const int npair = n >> 1, nq = (n + 1) >> 1;
   const int lane = threadIdx.x & 31;
   const int stride = gridDim.x * kThreads;
+  const M mem = M::make();
   for (int i0 = blockIdx.x * kThreads + (threadIdx.x & ~31); i0 < nq; i0 += stride) {
     const int i = i0 + lane;
     unsigned nz = 3u;   // two bits: entries 2i, 2i + 1 (1 = may be nonzero; past the end nothing reads them)
     if (i < npair) {
       const double2 xc = reinterpret_cast<const double2*>(x)[i];
-      const double2 ci = reinterpret_cast<const double2*>(c)[i];
-      const double2 ai = reinterpret_cast<const double2*>(aty)[i];
-      const double2 u = reinterpret_cast<const double2*>(up)[i];
-      const double2 l = reinterpret_cast<const double2*>(lo)[i];
+      const double2 ci = mem.stream(reinterpret_cast<const double2*>(c) + i);
+      const double2 ai = mem.stream(reinterpret_cast<const double2*>(aty) + i);
+      const double2 u = mem.stream(reinterpret_cast<const double2*>(up) + i);
+      const double2 l = mem.stream(reinterpret_cast<const double2*>(lo) + i);
       if (pend) {
-        double2 sm = reinterpret_cast<double2*>(xsum)[i];
+        double2 sm = mem.stream_rw(reinterpret_cast<const double2*>(xsum) + i);
         sm.x = sm.x + w * xc.x;
         sm.y = sm.y + w * xc.y;
         reinterpret_cast<double2*>(xsum)[i] = sm;
@@ -49,7 +136,7 @@ primal_step_kernel(int n, PdhgState* __restrict__ st, double* __restrict__ x0, d
       double2 o;
       const double t0 = one(xc.x, ci.x, ai.x, u.x, l.x, o.x);
       const double t1 = one(xc.y, ci.y, ai.y, u.y, l.y, o.y);
-      reinterpret_cast<double2*>(xn)[i] = o;
+      mem.keep(reinterpret_cast<double2*>(xn) + i, o);
       add_term(acc[0], t0, rs, 0, 2 * i);
       add_term(acc[0], t1, rs, 0, 2 * i + 1);
       nz = (o.x != 0.0 ? 1u : 0u) | (o.y != 0.0 ? 2u : 0u);
@@ -65,8 +152,8 @@ primal_step_kernel(int n, PdhgState* __restrict__ st, double* __restrict__ x0, d
       const unsigned w_lo = __reduce_or_sync(0xffffffffu, lane < 16 ? sh : 0u);
       const unsigned w_hi = __reduce_or_sync(0xffffffffu, lane < 16 ? 0u : sh);
       const int wd = i0 >> 4;   // entries 2 i0 .. 2 i0 + 63
-      if (lane == 0) xnz[wd] = w_lo;
-      if (lane == 16 && 32 * (wd + 1) < n) xnz[wd + 1] = w_hi;
+      if (lane == 0) mem.keep(xnz + wd, w_lo);
+      if (lane == 16 && 32 * (wd + 1) < n) mem.keep(xnz + wd + 1, w_hi);
     }
   }
   if ((n & 1) && blockIdx.x == 0 && threadIdx.x == 0) {
@@ -91,10 +178,12 @@ struct StridedOut {
 };
 // an epilogue that has slice_end(slice, live) gets it after every slice of the body, with the whole warp converged
 template <class E, class = void> struct HasSliceEnd { static constexpr bool value = false; };
-template <class E> struct HasSliceEnd<E, decltype(void(&E::slice_end))> { static constexpr bool value = true; };
-template <class Epi>
-__device__ __forceinline__ void slice_end(const Epi& e, int slice, bool live) {
-  if constexpr (HasSliceEnd<Epi>::value) e.slice_end(slice, live);
+template <class E> struct HasSliceEnd<E, decltype(void(std::declval<const E&>().slice_end(0, true)))> {
+  static constexpr bool value = true;
+};
+template <class Epi, class M = PlainMem>
+__device__ __forceinline__ void slice_end(const Epi& e, int slice, bool live, const M& mem = M{}) {
+  if constexpr (HasSliceEnd<Epi>::value) e.slice_end(slice, live, mem);
 }
 // ===================================================================== SpMV
 // Sliced-ELL body: one warp per slice of 32 rows, one lane per row.  A warp reads the slice's
@@ -152,19 +241,21 @@ struct DualEpilogueT {
   __device__ const double* input() const { return x0; }
   // the row's epilogue operands are requested BEFORE the gather loop so that they arrive under it
   double p_y, p_b, p_ax, p_ys, p_axs;
-  __device__ void prefetch(int r) {
-    p_y = y[r]; p_b = b[r]; p_ax = ax[r];
-    p_ys = pend ? ysum[r] : 0.0;
-    p_axs = accum ? axsum[r] : 0.0;
+  template <class M = PlainMem>
+  __device__ void prefetch(int r, const M& mem = M{}) {
+    p_y = mem.stream(y + r); p_b = mem.stream(b + r); p_ax = mem.stream(ax + r);
+    p_ys = pend ? mem.stream_rw(ysum + r) : 0.0;
+    p_axs = accum ? mem.stream_rw(axsum + r) : 0.0;
   }
   bool nz;
-  __device__ void row(int r, double s, double* t) {
+  template <class M = PlainMem>
+  __device__ void row(int r, double s, double* t, const M& mem = M{}) {
     axn[r] = s;
     const double yc = p_y;
     if (pend) ysum[r] = p_ys + w * yc;
     if (accum) axsum[r] = p_axs + w * p_ax;   // A xSum += w A x  (x = the iterate accepted by the previous pass)
     const double v = dual_update(yc, p_b, s, p_ax, sigma, r >= neq);
-    yn[r] = v;
+    mem.keep(yn + r, v);
     nz = v != 0.0;
     const double d = yc - v;
     t[0] = d * d;
@@ -172,10 +263,11 @@ struct DualEpilogueT {
   }
   // after a slice's rows (the whole warp, lane = row of the slice): the slice's word of the bitmap.  Lanes without a live
   // row write 1 -- among them the long rows, whose y' the segment finisher writes later in this launch.
-  __device__ void slice_end(int slice, bool live) const {
+  template <class M = PlainMem>
+  __device__ void slice_end(int slice, bool live, const M& mem = M{}) const {
     if (!ynz) return;
     const unsigned bits = __ballot_sync(0xffffffffu, !live || nz);
-    if ((threadIdx.x & 31) == 0) ynz[slice] = bits;
+    if ((threadIdx.x & 31) == 0) mem.keep(ynz + slice, bits);
   }
 };
 using DualEpilogue = DualEpilogueT<1>;
@@ -206,8 +298,13 @@ struct PrimalEpilogue {
   }
   __device__ const double* input() const { return y0; }
   double p_x, p_xn, p_aty, p_as;
-  __device__ void prefetch(int r) { p_x = x[r]; p_xn = xn[r]; p_aty = aty[r]; p_as = accum ? atysum[r] : 0.0; }
-  __device__ void row(int r, double s, double* t) const {
+  template <class M = PlainMem>
+  __device__ void prefetch(int r, const M& mem = M{}) {
+    p_x = mem.stream(x + r); p_xn = mem.stream(xn + r); p_aty = mem.stream(aty + r);
+    p_as = accum ? mem.stream_rw(atysum + r) : 0.0;
+  }
+  template <class M = PlainMem>   // (A'y' is not gathered by the next kernel: its stores take no policy)
+  __device__ void row(int r, double s, double* t, const M& = M{}) const {
     atyn[r] = s;
     if (accum) atysum[r] = p_as + w * p_aty;   // A'ySum += w A'y
     const double dx = p_x - p_xn;
@@ -506,7 +603,8 @@ __device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)_
 
 // `bytes` (a multiple of 16, from a 16-byte aligned address) into shared memory by the TMA unit: bulk copies of <= 32 KB
 // completed on one mbarrier, which every thread of the CTA waits for (SASS: UBLKCP / SYNCS).  Contains a __syncthreads.
-__device__ __forceinline__ void bulk_stage(void* dst, const void* src, unsigned bytes, unsigned long long* mbar) {
+// bulk_stage = bulk_stage_issue + bulk_stage_wait; work between the two overlaps the copy.
+__device__ __forceinline__ void bulk_stage_issue(void* dst, const void* src, unsigned bytes, unsigned long long* mbar) {
   const unsigned bar = smem_u32(mbar);
   if (threadIdx.x == 0) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(1) : "memory");
@@ -524,6 +622,9 @@ __device__ __forceinline__ void bulk_stage(void* dst, const void* src, unsigned 
                    : "memory");
     }
   }
+}
+__device__ __forceinline__ void bulk_stage_wait(unsigned long long* mbar) {
+  const unsigned bar = smem_u32(mbar);
   unsigned done = 0;
   do {
     asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
@@ -531,6 +632,10 @@ __device__ __forceinline__ void bulk_stage(void* dst, const void* src, unsigned 
                  : "r"(bar), "r"(0)
                  : "memory");
   } while (!done);
+}
+__device__ __forceinline__ void bulk_stage(void* dst, const void* src, unsigned bytes, unsigned long long* mbar) {
+  bulk_stage_issue(dst, src, bytes, mbar);
+  bulk_stage_wait(mbar);
 }
 
 template <class Epi>
@@ -684,12 +789,13 @@ static void launch_tile(cudaStream_t s, const DevSell& A, const Epi& e, const Re
 // -0.0; a row sum starts at +0.0 and +0 + -0 = +0, so it never is.  Skipping those terms therefore leaves every row sum
 // bit-identical, and it saves their gathers, which bound these kernels on random columns (one 32-byte sector per
 // gathered double).  The producers of x' / y' write the nonzero bitmap (DevSell::nzmap); every CTA stages it in shared
-// memory with one bulk copy and tests a bit before it gathers.
+// memory with one bulk copy and tests a bit before it gathers.  The matrix stream and the epilogue operands are loaded
+// evict-first, the gathers and y' (K2's output, K3's gather input) evict-last (L2Hints).
 // The block partial sums are those of the shape described by nblocks_body / pipelined: a CTA is kZGroups groups of
 // kThreads, and group q of the grid does the work of that shape's CTAs q, q + Q, q + 2Q, ... (Q = groups in the grid) --
 // warp w of the group walks the slices 8c + w, 8c + w + W, ... (W = 8 nblocks_body) of CTA c, in the same order, and the
 // group writes CTA c's partials with the same tree.  Then the long-row segments, one per group, likewise.
-template <class Epi>
+template <class Epi, class M>
 __global__ void __launch_bounds__(kZThreads, 1) spmv_sell_zskip_kernel(DevSell A, Epi epi_arg, ReduceScratch rs) {
   extern __shared__ __align__(16) unsigned nzs[];
   __shared__ __align__(8) unsigned long long mbar;
@@ -698,7 +804,8 @@ __global__ void __launch_bounds__(kZThreads, 1) spmv_sell_zskip_kernel(DevSell A
   Epi epi = epi_arg;
   if (!epi.begin()) return;
   const double* __restrict__ xin = epi.input();
-  bulk_stage(nzs, A.nzmap, (unsigned)A.nz_bytes, &mbar);
+  bulk_stage_issue(nzs, A.nzmap, (unsigned)A.nz_bytes, &mbar);
+  const M mem = M::make();
   auto bit = [&](int c) { return (nzs[c >> 5] >> (c & 31)) & 1u; };
   const int lane = threadIdx.x & 31, grp = threadIdx.x / kThreads, w = (threadIdx.x % kThreads) >> 5;
   const int ngroups = gridDim.x * kZGroups, gid = grp * gridDim.x + blockIdx.x;
@@ -709,10 +816,11 @@ __global__ void __launch_bounds__(kZThreads, 1) spmv_sell_zskip_kernel(DevSell A
   int4 d = make_int4(0, 0, -1, 0);
   int cpre[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   if (gid < nb && s < ns) {
-    d = A.slices[s];
+    d = mem.stream(A.slices + s);
 #pragma unroll
-    for (int u = 0; u < 8; u++) if (u < d.y) cpre[u] = A.col[d.x + lane + 32 * u];
+    for (int u = 0; u < 8; u++) if (u < d.y) cpre[u] = mem.stream(A.col + d.x + lane + 32 * u);
   }
+  bulk_stage_wait(&mbar);   // (the first descriptor and column ids arrive under the copy of the bitmap)
   for (int c = gid; c < nb; c += ngroups) {   // group-uniform
     double acc[Epi::NACC] = {};
     bool more = s < ns;
@@ -723,13 +831,13 @@ __global__ void __launch_bounds__(kZThreads, 1) spmv_sell_zskip_kernel(DevSell A
       int4 dn = make_int4(0, 0, -1, 0);
       int cnx[8] = {0, 0, 0, 0, 0, 0, 0, 0};
       if (sn < ns) {
-        dn = A.slices[sn];
+        dn = mem.stream(A.slices + sn);
 #pragma unroll
-        for (int u = 0; u < 8; u++) if (u < dn.y) cnx[u] = A.col[dn.x + lane + 32 * u];
+        for (int u = 0; u < 8; u++) if (u < dn.y) cnx[u] = mem.stream(A.col + dn.x + lane + 32 * u);
       }
       const int row = s * 32 + lane;
       const bool live = !((unsigned)d.z >> lane & 1u);
-      if (live) epi.prefetch(row);
+      if (live) epi.prefetch(row, mem);
       const int* __restrict__ cp = A.col + d.x + lane;
       const double* __restrict__ vp = A.val + d.x + lane;
       double sum = 0.0;
@@ -737,9 +845,9 @@ __global__ void __launch_bounds__(kZThreads, 1) spmv_sell_zskip_kernel(DevSell A
       {
         double v[8], g[8];
 #pragma unroll
-        for (int u = 0; u < 8; u++) g[u] = (u < d.y && bit(cpre[u])) ? xin[cpre[u]] : 0.0;
+        for (int u = 0; u < 8; u++) g[u] = (u < d.y && bit(cpre[u])) ? mem.gather(xin + cpre[u]) : 0.0;
 #pragma unroll
-        for (int u = 0; u < 8; u++) v[u] = u < d.y ? vp[32 * u] : 0.0;
+        for (int u = 0; u < 8; u++) v[u] = u < d.y ? mem.stream(vp + 32 * u) : 0.0;
 #pragma unroll
         for (int u = 0; u < 8; u++) if (u < d.y) sum += v[u] * g[u];
         k = d.y < 8 ? d.y : 8;
@@ -748,25 +856,25 @@ __global__ void __launch_bounds__(kZThreads, 1) spmv_sell_zskip_kernel(DevSell A
         int cc[8];
         double v[8], g[8];
 #pragma unroll
-        for (int u = 0; u < 8; u++) cc[u] = cp[32 * (k + u)];
+        for (int u = 0; u < 8; u++) cc[u] = mem.stream(cp + 32 * (k + u));
 #pragma unroll
-        for (int u = 0; u < 8; u++) g[u] = bit(cc[u]) ? xin[cc[u]] : 0.0;
+        for (int u = 0; u < 8; u++) g[u] = bit(cc[u]) ? mem.gather(xin + cc[u]) : 0.0;
 #pragma unroll
-        for (int u = 0; u < 8; u++) v[u] = vp[32 * (k + u)];
+        for (int u = 0; u < 8; u++) v[u] = mem.stream(vp + 32 * (k + u));
 #pragma unroll
         for (int u = 0; u < 8; u++) sum += v[u] * g[u];
       }
       for (; k < d.y; k++) {
-        const int cc = cp[32 * k];
-        sum += vp[32 * k] * (bit(cc) ? xin[cc] : 0.0);
+        const int cc = mem.stream(cp + 32 * k);
+        sum += mem.stream(vp + 32 * k) * (bit(cc) ? mem.gather(xin + cc) : 0.0);
       }
       if (live) {
         double t[Epi::NACC];
-        epi.row(row, sum, t);
+        epi.row(row, sum, t, mem);
 #pragma unroll
         for (int a = 0; a < Epi::NACC; a++) acc[a] += t[a];
       }
-      slice_end(epi, s, live);
+      slice_end(epi, s, live, mem);
       d = dn;
 #pragma unroll
       for (int u = 0; u < 8; u++) cpre[u] = cnx[u];
@@ -780,7 +888,7 @@ __global__ void __launch_bounds__(kZThreads, 1) spmv_sell_zskip_kernel(DevSell A
   for (int q = gid; q < A.nsegs; q += ngroups) {
     const int4 sg = A.segs[q];
     double sv = 0.0;
-    for (int e = sg.y + t; e < sg.z; e += kThreads) sv += A.lval[e] * xin[A.lcol[e]];
+    for (int e = sg.y + t; e < sg.z; e += kThreads) sv += mem.stream(A.lval + e) * mem.gather(xin + mem.stream(A.lcol + e));
     sv = warp_sum(sv);
     if (lane == 0) sseg[grp][w] = sv;
     asm volatile("bar.sync %0, %1;" ::"r"(1 + grp), "r"(kThreads) : "memory");
@@ -800,9 +908,9 @@ __global__ void __launch_bounds__(kZThreads, 1) spmv_sell_zskip_kernel(DevSell A
           double tot = 0.0;
           for (int i = 0; i < lr.z; i++) tot += pp[i];
           A.long_counter[sg.w] = 0u;
-          epi.prefetch(lr.x);
+          epi.prefetch(lr.x, mem);
           double tt[Epi::NACC];
-          epi.row(lr.x, tot, tt);
+          epi.row(lr.x, tot, tt, mem);
 #pragma unroll
           for (int a = 0; a < Epi::NACC; a++) rs.partials[(size_t)a * nslots + nb + lr.y] = 0.0 + tt[a];
         }
@@ -812,7 +920,7 @@ __global__ void __launch_bounds__(kZThreads, 1) spmv_sell_zskip_kernel(DevSell A
   }
 }
 
-template <class Epi>
+template <class Epi, class M>
 static void launch_zskip(cudaStream_t s, const DevSell& A, const Epi& e, const ReduceScratch& rs) {
   static bool attr_set[64] = {false};   // per instantiation AND per device (see launch_tile)
   int dev = 0;
@@ -821,11 +929,16 @@ static void launch_zskip(cudaStream_t s, const DevSell& A, const Epi& e, const R
     int cap = 0;
     cudaDeviceGetAttribute(&cap, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
     cudaFuncAttributes fa;
-    cudaFuncGetAttributes(&fa, spmv_sell_zskip_kernel<Epi>);
-    cudaFuncSetAttribute(spmv_sell_zskip_kernel<Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap - (int)fa.sharedSizeBytes);
+    cudaFuncGetAttributes(&fa, spmv_sell_zskip_kernel<Epi, M>);
+    cudaFuncSetAttribute(spmv_sell_zskip_kernel<Epi, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap - (int)fa.sharedSizeBytes);
     if (dev >= 0 && dev < 64) attr_set[dev] = true;
   }
-  spmv_sell_zskip_kernel<Epi><<<A.zskip_grid, kZThreads, A.nz_bytes, s>>>(A, e, rs);
+  spmv_sell_zskip_kernel<Epi, M><<<A.zskip_grid, kZThreads, A.nz_bytes, s>>>(A, e, rs);
+}
+template <class Epi>
+static void launch_zskip(cudaStream_t s, const DevSell& A, const Epi& e, const ReduceScratch& rs) {
+  if (A.l2_hints) launch_zskip<Epi, HintedMem>(s, A, e, rs);
+  else launch_zskip<Epi, PlainMem>(s, A, e, rs);
 }
 
 // ============================================================ multi-GPU kernels
@@ -2015,8 +2128,9 @@ static inline int ew_grid(int len) {
 
 void launch_primal_step(cudaStream_t s, int n, PdhgState* st, double* x0, double* x1, const double* aty0,
                         const double* aty1, const double* c, const double* lo, const double* up, double* xsum,
-                        ReduceScratch rs, unsigned* xnz) {
-  primal_step_kernel<<<ew_grid((n + 1) / 2), kThreads, 0, s>>>(n, st, x0, x1, aty0, aty1, c, lo, up, xsum, rs, xnz);
+                        ReduceScratch rs, unsigned* xnz, int l2_hints) {
+  if (l2_hints) primal_step_kernel<HintedMem><<<ew_grid((n + 1) / 2), kThreads, 0, s>>>(n, st, x0, x1, aty0, aty1, c, lo, up, xsum, rs, xnz);
+  else primal_step_kernel<PlainMem><<<ew_grid((n + 1) / 2), kThreads, 0, s>>>(n, st, x0, x1, aty0, aty1, c, lo, up, xsum, rs, xnz);
 }
 
 // the nonzero bitmap (DevSell::nzmap) of a vector that no pass kernel produced (kernel-level entry points)
@@ -2044,8 +2158,10 @@ int zskip_ctas_per_sm(int nz_bytes) {
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&k, kern, kZThreads, (size_t)nz_bytes) != cudaSuccess) k = 0;
     best = k < best ? k : best;
   };
-  one(spmv_sell_zskip_kernel<DualEpilogue>);
-  one(spmv_sell_zskip_kernel<PrimalEpilogue>);
+  one(spmv_sell_zskip_kernel<DualEpilogue, PlainMem>);
+  one(spmv_sell_zskip_kernel<PrimalEpilogue, PlainMem>);
+  one(spmv_sell_zskip_kernel<DualEpilogue, HintedMem>);
+  one(spmv_sell_zskip_kernel<PrimalEpilogue, HintedMem>);
   cudaGetLastError();
   return best;
 }
@@ -2182,7 +2298,7 @@ int primal_step_grid(int n) { return ew_grid((n + 1) / 2); }
 // loaded up front.
 void preload_multi_gpu_kernels() {
   const void* fns[] = {
-      (const void*)primal_step_kernel, (const void*)primal_shard_kernel, (const void*)primal_shard_p2p_kernel,
+      (const void*)primal_step_kernel<PlainMem>, (const void*)primal_step_kernel<HintedMem>, (const void*)primal_shard_kernel, (const void*)primal_shard_p2p_kernel,
       (const void*)push_shard_kernel, (const void*)push_rows_kernel,
       (const void*)p2p_exchange_kernel, (const void*)reduce_part_p2p_kernel, (const void*)p2p_barrier_kernel,
       (const void*)stash_scalars_kernel<1>, (const void*)stash_scalars_kernel<2>, (const void*)step_rule_mg_kernel,

@@ -9,7 +9,7 @@ struct RowIter { const double* y; const double* ax; };    // one dual-side itera
 
 void launch_primal_step(cudaStream_t s, int n, PdhgState* st, double* x0, double* x1, const double* aty0,
                         const double* aty1, const double* c, const double* lo, const double* up, double* xsum,
-                        ReduceScratch rs, unsigned* xnz = nullptr);
+                        ReduceScratch rs, unsigned* xnz = nullptr, int l2_hints = 0);
 // xnz / ynz: where K1 / K2 write the nonzero bitmap of x' / y' (DevSell::nzmap of A / A'), nullptr: nowhere
 void launch_nz_bitmap(cudaStream_t s, int len, const double* v, unsigned* out);
 int zskip_ctas_per_sm(int nz_bytes);
