@@ -2,13 +2,15 @@
 // plumbing and the C ABI (include/b200pdlp.h) of everything but the HiPDLP mode (engine_hipdlp.cu) and the batches
 // (engine_batch.cu).
 //
-// The host owns what cuPDLP-C's PDHG_Solve owns (/root/reference/highs/pdlp/cupdlp/
-// cupdlp_solver.c:899-1106): the outer loop, the check schedule (first 10
-// iterations, then every 40), termination, infeasibility detection and the
-// restart decisions (cupdlp_restart.c:3-99, cupdlp_proj.c:88-148).  Everything that
-// touches an n- or m-vector runs in pdhg_kernels.cu.  Between two checks the host
-// does not synchronise: it points state.stop_iter at the next check iteration and
-// replays a CUDA graph of PDHG passes; the adaptive step rule runs on the device.
+// The outer loop of cuPDLP-C's PDHG_Solve (/root/reference/highs/pdlp/cupdlp/cupdlp_solver.c:899-1106) runs in one of
+// two ways, by mode.  Tree mode (one GPU, or several over peer memory) runs device_loop: the check iterations decide on
+// the device (termination, infeasibility, restarts, the next check iteration) and the host enqueues batches of [check,
+// passes] rounds as CUDA graphs and reads the control block once per batch.  Ordered mode (bit for bit the reference's,
+// with glibc log / exp / pow) and tree mode over NCCL run host_loop: the host owns the check schedule (first 10
+// iterations, then every 40), termination, infeasibility detection and the restart decisions (cupdlp_restart.c:3-99,
+// cupdlp_proj.c:88-148); between two checks it points state.stop_iter at the next check iteration and replays a graph
+// of PDHG passes.  Everything that touches an n- or m-vector runs in pdhg_kernels.cu; the adaptive step rule runs on
+// the device in both loops.
 #include "engine.hpp"
 
 namespace b200 {
@@ -248,8 +250,8 @@ void alloc_scratch(b200pdlp_problem* p, bool zero) {
 // the PDHG solve's pinned mirrors, zeroed
 static void alloc_host_mirrors(b200pdlp_problem* p) {
   p->hstate = static_cast<PdhgState*>(pinned_cache_alloc(sizeof(PdhgState), false));
-  p->hflag = static_cast<double*>(pinned_cache_alloc(4 * sizeof(double), false));   // [0] time-limit flag, [2] read-back of the barrier fault word
-  memset(p->hflag, 0, 4 * sizeof(double));
+  p->hfault = static_cast<int*>(pinned_cache_alloc(sizeof(int), false));
+  *p->hfault = 0;
   memset(p->hstate, 0, sizeof(PdhgState));
 }
 
@@ -657,10 +659,9 @@ static const char kPeerLate[] = "P2P barrier timed out (a peer rank did not arri
 // waiting for a peer leaves inconsistent data behind: stop with `msg` instead of going on with it.
 static void throw_if_peer_fault(b200pdlp_problem* p, const char* msg) {
   if (!p->p2p) return;
-  int* hfault = reinterpret_cast<int*>(p->hflag + 2);
-  CUDA_OK(cudaMemcpyAsync(hfault, p->fault.p, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
+  CUDA_OK(cudaMemcpyAsync(p->hfault, p->fault.p, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
   CUDA_OK(cudaStreamSynchronize(p->stream));
-  if (*hfault) throw Error(B200PDLP_ERR_STATE, msg);
+  if (*p->hfault) throw Error(B200PDLP_ERR_STATE, msg);
 }
 static void pull_state(b200pdlp_problem* p) {
   CUDA_OK(cudaMemcpyAsync(p->hstate, p->state.p, sizeof(PdhgState), cudaMemcpyDeviceToHost, p->stream));
@@ -737,53 +738,6 @@ static CheckResult parse_fused_check(b200pdlp_problem* p, bool timed_out_local) 
   return cr;
 }
 
-// SPECULATIVE check: the same sequence as run_check's tree-mode branch, but enqueued right behind the PDHG passes
-// BEFORE the host has read the state -- every kernel takes buffer parity, pending weight and step sum from the device
-// state block and does nothing unless state.iter has reached state.stop_iter.  The host launch overhead of the ~10
-// kernels hides behind the running pass graph, one synchronisation per check interval remains, and on several GPUs
-// the barriers inside the check no longer wait for every rank's host thread.
-static bool can_speculate_check(const b200pdlp_problem* p) { return !p->ordered && (p->world == 1 || p->p2p); }
-
-static void enqueue_check_dev(b200pdlp_problem* p, bool timed_out_local) {
-  cudaStream_t s = p->stream;
-  PdhgState* st = p->state.p;
-  const int n = p->nl, ml = p->ml;
-  if (p->world > 1) {
-    launch_reduce_part_p2p(s, n, p->aty[0].p, p->peers, p->world, p->rank, p->seg_len, 1, st, 1);   // if accepted_last
-    p->launches++;
-  }
-  launch_average_dev(s, n, p->x[0].p, p->x[1].p, p->xsum.p, p->xavg.p, st);
-  launch_average_dev(s, ml, p->y[0].p, p->y[1].p, p->ysum.p, p->yavg.p, st);
-  launch_check_clear(s, st);
-  p->launches += 3;
-  if (p->world == 1) {
-    launch_spmv_plain(s, p->A.dev, p->xavg.p, p->axavg.p, st);
-    launch_spmv_plain(s, p->AT.dev, p->yavg.p, p->atyavg.p, st);
-    p->launches += 2;
-  } else {
-    launch_push_shard(s, p->xavg.p, p->nl, p->peers, p->world, p->rank, p->seg_len, st);
-    launch_spmv_partial_aty(s, p->AT.dev, nullptr, p->yavg.p, p->yavg.p, p->recv.p, p->at_outpos.p, st);
-    launch_p2p_exchange(s, p->outs.p + 60, 0, p->peers, p->world, p->rank, p->epochs.p, p->fault.p, st);
-    launch_spmv_plain(s, p->A.dev, p->xfull.p, p->axavg.p, st);
-    launch_reduce_part_p2p(s, n, p->atyavg.p, p->peers, p->world, p->rank, p->seg_len, 2, st, 0);
-    p->launches += 5;
-  }
-  double* o = p->outs.p;
-  const bool one_aty = p->world > 1;   // multi-GPU keeps a single current A^T y shard
-  ColIter c0{p->x[0].p, p->aty[0].p}, calt{p->x[1].p, one_aty ? p->aty[0].p : p->aty[1].p}, c1{p->xavg.p, p->atyavg.p};
-  RowIter r0{p->y[0].p, p->ax[0].p}, ralt{p->y[1].p, p->ax[1].p}, r1{p->yavg.p, p->axavg.p};
-  launch_col_check_fused(s, n, c0, c1, p->cost.p, p->lower.p, p->upper.p, p->colscale.p, p->rs(kSlotChk, n), o, st, calt);
-  launch_row_check_fused(s, ml, r0, r1, p->rhs.p, p->rowscale.p, p->neq_local, p->rs(kSlotChk, ml), o + 20, st, ralt);
-  p->launches += 2;
-  if (p->world > 1) {
-    p->hflag[0] = timed_out_local ? 1.0 : 0.0;
-    CUDA_OK(cudaMemcpyAsync(o + 28, p->hflag, sizeof(double), cudaMemcpyHostToDevice, s));
-    launch_p2p_exchange(s, o, 29, p->peers, p->world, p->rank, p->epochs.p, p->fault.p, st);
-    p->launches++;
-  }
-  CUDA_OK(cudaMemcpyAsync(p->houts, o, 29 * sizeof(double), cudaMemcpyDeviceToHost, s));
-}
-
 // Ordered-mode check, host arithmetic on the sums of sweeps A (o[0..20]: 7 column sums, then 3 row sums, per iterate):
 // residuals of both iterates and the ray scales sweeps B need
 void assemble_check_a(const StdForm& f, const double* o, CheckResult& cr, double dscale[2], double pscale[2]) {
@@ -829,15 +783,9 @@ static CheckResult run_check(b200pdlp_problem* p, bool timed_out_local) {
   const int n = p->nl, ml = p->ml, cur = h->cur;   // n = column entries held by this rank
   const int acur = p->world == 1 ? cur : 0;        // multi-GPU keeps one current A^T y shard
   const double scale = h->sum_step > 0.0 ? 1.0 / h->sum_step : 1.0;
-  const bool fused = p->world > 1 && p->p2p;
   if (p->world > 1 && h->accepted_last) {
-    // the last accepted pass left its A^T y' un-reduced (P2P) / in the reduce-scatter buffer (NCCL): make it current
-    if (p->p2p) {
-      launch_reduce_part_p2p(s, n, p->aty[0].p, p->peers, p->world, p->rank, p->seg_len, 1);
-      p->launches++;
-    } else {
-      CUDA_OK(cudaMemcpyAsync(p->aty[0].p, p->red.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, s));
-    }
+    // the last accepted pass left its A^T y' in the reduce-scatter buffer: make it current
+    CUDA_OK(cudaMemcpyAsync(p->aty[0].p, p->red.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, s));
     h->accepted_last = 0;
     push_state(p);
   }
@@ -845,19 +793,8 @@ static CheckResult run_check(b200pdlp_problem* p, bool timed_out_local) {
   launch_average(s, ml, p->y[cur].p, p->ysum.p, p->yavg.p, h->pending, h->w_pending, scale);
   p->launches += 2;
   if (h->pending) { h->pending = 0; push_state(p); }
-  if (fused) {
-    // one barrier for both exchanges: x-bar shards are stored into every peer's xfull, the partial A_g^T y-bar is
-    // parked in my `recv` buffer (so `part`, which a slower peer may still be reducing from, stays intact)
-    launch_push_shard(s, p->xavg.p, p->nl, p->peers, p->world, p->rank, p->seg_len);
-    launch_spmv_partial_aty(s, p->AT.dev, nullptr, p->yavg.p, p->yavg.p, p->recv.p, p->at_outpos.p);
-    launch_p2p_exchange(s, p->outs.p + 60, 0, p->peers, p->world, p->rank, p->epochs.p, p->fault.p);
-    launch_spmv_plain(s, p->A.dev, p->xfull.p, p->axavg.p);
-    launch_reduce_part_p2p(s, n, p->atyavg.p, p->peers, p->world, p->rank, p->seg_len, 2);
-    p->launches += 5;
-  } else {
-    full_ax(p, p->xavg.p, p->axavg.p);
-    full_aty(p, p->yavg.p, p->atyavg.p);
-  }
+  full_ax(p, p->xavg.p, p->axavg.p);
+  full_aty(p, p->yavg.p, p->atyavg.p);
   ColIter c0{p->x[cur].p, p->aty[acur].p}, c1{p->xavg.p, p->atyavg.p};
   RowIter r0{p->y[cur].p, p->ax[cur].p}, r1{p->yavg.p, p->axavg.p};
   double* o = p->outs.p;
@@ -1174,20 +1111,6 @@ static void drop_graphs(b200pdlp_problem* p) {
   if (p->graph_check_light) { cudaGraphExecDestroy(p->graph_check_light); p->graph_check_light = nullptr; }
 }
 
-static bool use_device_checks(const b200pdlp_problem* p, const b200pdlp_params& prm) {
-  if (p->ordered || prm.log_level >= 2 || prm.iter_limit <= 0) return false;
-  if (p->world != 1) {
-    // several GPUs: only on the fused peer-memory path (the checks' collectives are our own barrier / exchange kernels)
-    if (!p->p2p) return false;
-    // default since it passed on hardware against the oracle (2 GPUs: tests/test_gpu_multi.py; 2 / 3 / 4 logical shards:
-    // tests/test_gpu_logical_shards.py; both run both settings).  B200PDLP_MG_DEVICE_CHECK=0: round 1's host-driven checks.
-    const char* e = getenv("B200PDLP_MG_DEVICE_CHECK");
-    if (e && atoi(e) == 0) return false;
-  }
-  if (const char* e = getenv("B200PDLP_HOST_CHECK")) if (atoi(e) != 0) return false;   // the round-1 host-driven checks
-  return true;
-}
-
 // several GPUs (fused peer-memory path): the same check with the vectors sharded -- xbar shards go to every peer's xfull,
 // the partial A_g'ybar are parked in `recv` and reduced by their owners after a barrier, the 28 sums (+ the time-limit
 // word) are all-reduced by the exchange kernel (identical on every rank, added in rank order), so every rank takes the
@@ -1296,7 +1219,6 @@ static cudaGraphExec_t capture_check(b200pdlp_problem* p, bool light, int* launc
 }
 
 static void launch_check_graph(b200pdlp_problem* p, bool light = false) {
-  if (p->no_graph) { p->launches += enqueue_check_device(p, light); return; }
   cudaGraphExec_t& ge = light ? p->graph_check_light : p->graph_check;
   int& nl = p->check_launches[light ? 1 : 0];
   if (!ge) ge = capture_check(p, light, &nl);
@@ -1309,7 +1231,6 @@ static void launch_check_graph(b200pdlp_problem* p, bool light = false) {
 static void enqueue_passes_device(b200pdlp_problem* p, int d) {
   if (d <= 0) return;
   const int kp = p->kernels_per_pass();
-  if (p->no_graph) { for (; d > 0; d--) { enqueue_pass(p); p->launches += kp; } return; }
   if (d > p->graph_main_passes - 12 && !p->graph_main) p->graph_main = capture_passes(p, p->graph_main_passes);
   if (d > p->graph_main_passes - 12 && d <= p->graph_main_passes) {
     CUDA_OK(cudaGraphLaunch(p->graph_main, p->stream));
@@ -1333,12 +1254,20 @@ static void enqueue_passes_device(b200pdlp_problem* p, int d) {
 }
 
 // ---- the phases of the single solve, in the order solve_on_device runs them
-// the check control block: pinned host copy, mapped time-limit word, device copy (filled by a copy on p->stream)
+// The device-driven loop enqueues at most kBatchRounds check launches per batch, and a check writes at most one trace row
+// (check_decide_kernel / finish_scalars), so a window of kTraceWindow rows, rewound at the start of every batch, holds
+// every row of a batch; a full window would mean rows were dropped.
+constexpr int kBatchRounds = 12, kTraceWindow = 16;
+static_assert(kBatchRounds < kTraceWindow, "a batch's trace rows must fit the window with room to spare");
+// the check control block: pinned host copy, mapped time-limit word, device copy (filled by a copy on p->stream), and the
+// trace window with its pinned host copy
 static void ensure_ctl(b200pdlp_problem* p) {
   if (p->hctl) return;
   p->hctl = static_cast<SolveCtl*>(pinned_cache_alloc(sizeof(SolveCtl), false));
   p->htime = static_cast<int*>(pinned_cache_alloc(64, true));
+  p->htrace = static_cast<double*>(pinned_cache_alloc(kTraceWindow * B200PDLP_TRACE_COLS * sizeof(double), false));
   p->ctl.alloc(1, false);
+  p->trace_dev.alloc(kTraceWindow * B200PDLP_TRACE_COLS, false);
 }
 static int* mapped_time_flag(b200pdlp_problem* p) {
   int* d = nullptr;
@@ -1358,23 +1287,25 @@ static SolveCtl* reset_ctl(b200pdlp_problem* p, double tol_p, double tol_d, doub
   return c;
 }
 
-// Graphs: one check interval of passes, and a short one for top-ups after rejected steps.  A few spare passes per replay:
-// a rejected line-search step then still reaches the next check iteration inside the same replay (spare passes are no-ops
-// once state.iter == state.stop_iter) instead of costing a host round trip.  The device-driven loop captures its graphs
-// when it first needs them, unless `eager` (logical shards): everything that allocates or instantiates happens before ANY
-// rank launches a kernel that waits for its peers (see LocalGroup), so every graph is captured and uploaded here.
+// Graphs: one check interval of passes (both loops), and for the host-driven loop a short one for top-ups after rejected
+// steps.  A few spare passes per replay: a rejected line-search step then still reaches the next check iteration inside the
+// same replay (spare passes are no-ops once state.iter == state.stop_iter) instead of costing a host round trip.  The
+// device-driven loop captures its graphs when it first needs them, unless `eager` (logical shards, which always run the
+// device-driven loop): everything that allocates or instantiates happens before ANY rank launches a kernel that waits for
+// its peers (see LocalGroup), so every graph is captured and uploaded here.
 static void prepare_graphs(b200pdlp_problem* p, const b200pdlp_params& prm, int interval, bool dev_checks, bool eager) {
   cudaStream_t s = p->stream;
   const int want = std::min(prm.graph_passes > 0 ? prm.graph_passes : interval + 4, kPowTab - 16);   // the step-rule tables cover one replay
   if (p->graph_main && p->graph_main_passes != want) { cudaGraphExecDestroy(p->graph_main); p->graph_main = nullptr; }
   p->graph_main_passes = want;
-  p->no_graph = getenv("B200PDLP_NO_GRAPH") != nullptr;
-  if (p->no_graph || (dev_checks && !eager)) return;
-  if (!p->graph_main) p->graph_main = capture_passes(p, want);
-  if (!p->graph_small) { p->graph_small_passes = 4; p->graph_small = capture_passes(p, 4); }
+  if (!dev_checks) {
+    if (!p->graph_main) p->graph_main = capture_passes(p, want);
+    if (!p->graph_small) { p->graph_small_passes = 4; p->graph_small = capture_passes(p, 4); }
+    return;
+  }
   if (!eager) return;
-  for (cudaGraphExec_t g : {p->graph_main, p->graph_small}) CUDA_OK(cudaGraphUpload(g, s));
-  if (!dev_checks) return;
+  if (!p->graph_main) p->graph_main = capture_passes(p, want);
+  CUDA_OK(cudaGraphUpload(p->graph_main, s));
   ensure_ctl(p);
   for (int k = 2; k <= 5; k++) if (!p->graph_pow2[k]) { p->graph_pow2[k] = capture_passes(p, 1 << k); CUDA_OK(cudaGraphUpload(p->graph_pow2[k], s)); }
   if (!p->graph_check) { p->graph_check = capture_check(p, false, &p->check_launches[0]); CUDA_OK(cudaGraphUpload(p->graph_check, s)); }
@@ -1479,6 +1410,12 @@ struct LoopOutcome {
   double iter_ms = 0.0;   // device time of the passes
 };
 
+// log_level >= 2: one line per check from the first 11 columns of a trace row (iteration, both iterates' residuals, tau, sigma)
+static void log_check(const double* t) {
+  printf("[b200pdlp] it %8d  pobj %+.8e dobj %+.8e  pfeas %.2e dfeas %.2e | avg pobj %+.8e dobj %+.8e pfeas %.2e dfeas %.2e  tau %.3e sigma %.3e\n",
+         (int)t[0], t[1], t[2], t[3], t[4], t[5], t[6], t[7], t[8], t[9], t[10]);
+}
+
 // device-driven loop: the checks decide on the device (termination, restarts, next check iteration); the host
 // enqueues [check, passes to the next check] rounds ahead from the deterministic check schedule and reads the control
 // block once per batch.  A rejected line-search step makes a round fall short; the following rounds make up for it
@@ -1503,10 +1440,9 @@ static LoopOutcome device_loop(b200pdlp_problem* p, const b200pdlp_params& prm, 
     else CUDA_OK(cudaMemcpyAsync(p->axsum.p, p->ax[0].p, (size_t)std::max(ml, 1) * sizeof(double), cudaMemcpyDeviceToDevice, s));
     CUDA_OK(cudaMemsetAsync(p->atysum.p, 0, (size_t)std::max(nl, 1) * sizeof(double), s));
   }
-  if (out->trace && out->trace_cap > 0) {
-    if (p->trace_dev.n < (size_t)out->trace_cap * B200PDLP_TRACE_COLS) p->trace_dev.alloc((size_t)out->trace_cap * B200PDLP_TRACE_COLS, false);
-    c->trace = p->trace_dev.p; c->trace_cap = out->trace_cap;
-  }
+  // trace rows (for the caller's trace or the log) come back through the window after every batch
+  const bool rows = (out->trace && out->trace_cap > 0) || prm.log_level >= 2;
+  if (rows) { c->trace = p->trace_dev.p; c->trace_cap = kTraceWindow; }
   CUDA_OK(cudaMemcpyAsync(p->ctl.p, c, sizeof(SolveCtl), cudaMemcpyHostToDevice, s));
   h->stop_iter = 0;   // the first check is due at once (iteration 0)
   push_state(p);
@@ -1520,6 +1456,10 @@ static LoopOutcome device_loop(b200pdlp_problem* p, const b200pdlp_params& prm, 
       if (nev == evs.size()) evs.emplace_back(new CudaEvent());
       return *evs[nev++];
     };
+    if (rows) {
+      c->trace_len = 0;
+      CUDA_OK(cudaMemcpyAsync(&p->ctl.p->trace_len, &c->trace_len, sizeof(int), cudaMemcpyHostToDevice, s));
+    }
     int rounds = 0, passes = 0;
     if (carry > 0) {
       CUDA_OK(cudaEventRecord(ev(), s));
@@ -1527,7 +1467,7 @@ static LoopOutcome device_loop(b200pdlp_problem* p, const b200pdlp_params& prm, 
       CUDA_OK(cudaEventRecord(ev(), s));
       passes += carry; pred_iter += carry; carry = 0;
     }
-    while (rounds < 12 && passes < 48) {
+    while (rounds < kBatchRounds && passes < 48) {
       // pred_iter never runs behind the device's iteration count, so pred_iter < kDenseChecks implies the device is
       // inside the dense phase as well (the light kernels check it once more themselves)
       launch_check_graph(p, h_light && pred_iter < kDenseChecks);
@@ -1542,6 +1482,9 @@ static LoopOutcome device_loop(b200pdlp_problem* p, const b200pdlp_params& prm, 
     }
     CUDA_OK(cudaMemcpyAsync(c, p->ctl.p, sizeof(SolveCtl), cudaMemcpyDeviceToHost, s));
     CUDA_OK(cudaMemcpyAsync(h, p->state.p, sizeof(PdhgState), cudaMemcpyDeviceToHost, s));
+    if (rows)
+      CUDA_OK(cudaMemcpyAsync(p->htrace, p->trace_dev.p, kTraceWindow * B200PDLP_TRACE_COLS * sizeof(double),
+                              cudaMemcpyDeviceToHost, s));
     const size_t npairs = nev / 2;   // events so far come in (before, after) pairs around the passes
     cudaEvent_t fin = ev();
     CUDA_OK(cudaEventRecord(fin, s));
@@ -1559,6 +1502,15 @@ static LoopOutcome device_loop(b200pdlp_problem* p, const b200pdlp_params& prm, 
       CUDA_OK(cudaEventElapsedTime(&ms, *evs[2 * k], *evs[2 * k + 1]));
       o.iter_ms += ms;
     }
+    if (rows) {
+      if (c->trace_len >= kTraceWindow) throw Error(B200PDLP_ERR_STATE, "a batch of checks filled the trace window");
+      for (int r = 0; r < c->trace_len; r++) {
+        const double* t = p->htrace + (size_t)r * B200PDLP_TRACE_COLS;
+        if (prm.log_level >= 2) log_check(t);
+        if (out->trace && out->trace_len < out->trace_cap)
+          memcpy(out->trace + (size_t)out->trace_len++ * B200PDLP_TRACE_COLS, t, B200PDLP_TRACE_COLS * sizeof(double));
+      }
+    }
     if (c->term >= 0) break;
     // not finished: continue from where the device really is
     h_light = h_light && h->light_on != 0;
@@ -1573,33 +1525,25 @@ static LoopOutcome device_loop(b200pdlp_problem* p, const b200pdlp_params& prm, 
     R.pobj = d.pobj; R.dobj = d.dobj; R.pfeas = d.pfeas; R.dfeas = d.dfeas; R.gap = d.gap; R.relgap = d.relgap;
     R.pinf_obj = d.pinf_obj; R.pinf_res = d.pinf_res; R.dinf_obj = d.dinf_obj; R.dinf_res = d.dinf_res;
   }
-  if (c->trace) {
-    out->trace_len = std::min(c->trace_len, out->trace_cap);
-    if (out->trace_len > 0)
-      CUDA_OK(cudaMemcpyAsync(out->trace, p->trace_dev.p, (size_t)out->trace_len * B200PDLP_TRACE_COLS * sizeof(double),
-                              cudaMemcpyDeviceToHost, s));
-  }
   return o;
 }
 
-// host-driven loop (cupdlp_solver.c:939-1106)
+// host-driven loop (cupdlp_solver.c:939-1106): ordered mode (glibc log / exp / pow and ordered sums, bit for bit the
+// reference's) and tree mode over NCCL (several GPUs without peer access)
 static LoopOutcome host_loop(b200pdlp_problem* p, const b200pdlp_params& prm, const LoopLimits& lim, b200pdlp_result* out) {
   cudaStream_t s = p->stream;
   PdhgState* h = p->hstate;
   LoopOutcome o;
   RestartMemo memo;
-  bool have_spec = false, spec_flag = false;   // a speculative check already produced the next check's scalars
-  const bool speculate = can_speculate_check(p);
   CudaEvent ev0, ev1;
   while (h->iter < prm.iter_limit) {
-    const bool timed_out_local = lim.over();
-    if (have_spec) { o.chk = parse_fused_check(p, spec_flag); have_spec = false; }
-    else o.chk = run_check(p, timed_out_local);
+    o.chk = run_check(p, lim.over());
     o.have_check = true;
-    const Residuals &L = o.chk.it[0], &A = o.chk.it[1];
-    if (prm.log_level >= 2)
-      printf("[b200pdlp] it %8d  pobj %+.8e dobj %+.8e  pfeas %.2e dfeas %.2e | avg pobj %+.8e dobj %+.8e pfeas %.2e dfeas %.2e  tau %.3e sigma %.3e\n",
-             h->iter, L.pobj, L.dobj, L.pfeas, L.dfeas, A.pobj, A.dobj, A.pfeas, A.dfeas, h->tau, h->sigma);
+    if (prm.log_level >= 2) {
+      const Residuals &L = o.chk.it[0], &A = o.chk.it[1];
+      const double t[11] = {(double)h->iter, L.pobj, L.dobj, L.pfeas, L.dfeas, A.pobj, A.dobj, A.pfeas, A.dfeas, h->tau, h->sigma};
+      log_check(t);
+    }
     int choice = 0;
     const int t_code = check_decision(prm, lim.tol_p, lim.tol_d, h, o.chk, memo, &o.term_iterate, &choice);
     if (t_code >= 0) { o.term = t_code; trace_row(out, h, o.chk, 0); break; }
@@ -1610,12 +1554,9 @@ static LoopOutcome host_loop(b200pdlp_problem* p, const b200pdlp_params& prm, co
     fill_pow_tables(h);
     push_state(p);
     CUDA_OK(cudaEventRecord(ev0, s));
-    bool have_ev1 = false;
     while (true) {
       const int need = next - h->iter;
-      if (p->no_graph) {
-        for (int q = 0; q < std::min(need + 4, p->graph_main_passes); q++) { enqueue_pass(p); p->launches += p->kernels_per_pass(); }
-      } else if (need >= p->graph_main_passes / 2 || need > p->graph_small_passes) {
+      if (need >= p->graph_main_passes / 2 || need > p->graph_small_passes) {
         CUDA_OK(cudaGraphLaunch(p->graph_main, s));
         p->launches += (long long)p->graph_main_passes * p->kernels_per_pass();
       } else if (need > 1) {
@@ -1625,17 +1566,11 @@ static LoopOutcome host_loop(b200pdlp_problem* p, const b200pdlp_params& prm, co
         enqueue_pass(p);
         p->launches += p->kernels_per_pass();
       }
-      if (speculate) {
-        if (!have_ev1) { CUDA_OK(cudaEventRecord(ev1, s)); have_ev1 = true; }
-        spec_flag = lim.over();
-        enqueue_check_dev(p, spec_flag);
-      }
       pull_state(p);
-      if (h->iter >= next) { have_spec = speculate; break; }
-      have_ev1 = false;
+      if (h->iter >= next) break;
       if (h->step_iter - h->pow_base > kPowTab - p->graph_main_passes - 8) { fill_pow_tables(h); push_state(p); }
     }
-    if (!have_ev1) CUDA_OK(cudaEventRecord(ev1, s));
+    CUDA_OK(cudaEventRecord(ev1, s));
     CUDA_OK(cudaEventSynchronize(ev1));
     float ms = 0.f;
     CUDA_OK(cudaEventElapsedTime(&ms, ev0, ev1));
@@ -1810,7 +1745,9 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
   const auto t_begin = clk::now();
   const StdForm& f = p->form;
   const int interval = prm.check_interval > 0 ? prm.check_interval : 40;
-  const bool dev_checks = use_device_checks(p, prm);
+  // tree mode decides its checks on the device (on several GPUs only over peer memory: the checks' collectives are our own
+  // barrier / exchange kernels); ordered mode and NCCL run the host-driven loop
+  const bool dev_checks = !p->ordered && (p->world == 1 || p->p2p);
   const bool logical_shards = p->local_link && p->group;
   const long long launches0 = p->launches;
   PdhgState* h = p->hstate;
@@ -1842,7 +1779,10 @@ static void solve_on_device(b200pdlp_problem* p, const b200pdlp_params& prm, con
   CUDA_OK(cudaEventRecord(evl0, p->stream));
   const LoopLimits lim{interval, prm.tol_primal * (1.0 + f.norm_rhs), prm.tol_dual * (1.0 + f.norm_cost),
                        time_limit_or_none(prm.time_limit), clk::now()};
-  const LoopOutcome o = dev_checks ? device_loop(p, prm, warm, lim, out) : host_loop(p, prm, lim, out);
+  // iter_limit <= 0: no check at all (the device loop's check of iteration 0 would give the postsolve a check)
+  const LoopOutcome o = prm.iter_limit <= 0 ? LoopOutcome{}
+                        : dev_checks        ? device_loop(p, prm, warm, lim, out)
+                                            : host_loop(p, prm, lim, out);
   CUDA_OK(cudaEventRecord(evl1, p->stream));
   CUDA_OK(cudaEventSynchronize(evl1));
   float loop_ms = 0.f;
@@ -2227,9 +2167,8 @@ static SolveCtl* check_api_state(b200pdlp_problem* p, const b200pdlp_check_in* i
   h->pow_base = -1;
   h->stop_iter = in->iter; h->cur = 0; h->light_on = light ? 1 : 0; h->done = 0;
   push_state(p);
-  if (p->trace_dev.n < (size_t)B200PDLP_TRACE_COLS) p->trace_dev.alloc(B200PDLP_TRACE_COLS, false);
-  CUDA_OK(cudaMemsetAsync(p->trace_dev.p, 0, B200PDLP_TRACE_COLS * sizeof(double), s));
   SolveCtl* c = reset_ctl(p, in->tol_p, in->tol_d, in->tol_gap, in->iter_limit, in->interval, in->restart_on != 0);
+  CUDA_OK(cudaMemsetAsync(p->trace_dev.p, 0, B200PDLP_TRACE_COLS * sizeof(double), s));
   *p->htime = in->time_flag;
   c->time_flag = mapped_time_flag(p);
   c->pf_lr = in->pf_lr; c->df_lr = in->df_lr; c->gap_lr = in->gap_lr;

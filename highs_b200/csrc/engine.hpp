@@ -241,7 +241,6 @@ struct b200pdlp_problem {
   int hip_r0 = 0, hip_r1 = 0, hip_c0 = 0, hip_c1 = 0;
   bool local_link = false;         // peers are problems of this process (logical shards, b200pdlp_p2p_link_local)
   std::shared_ptr<b200::LocalGroup> group;   // their host-side rendezvous
-  bool no_graph = false;           // B200PDLP_NO_GRAPH: every pass and check as direct launches (debugging aid)
   bool p2p = false;
   PeerPtrs peers{};
   std::vector<void*> ipc_opened;
@@ -263,7 +262,7 @@ struct b200pdlp_problem {
   DevBuf<PdhgState> state;
   PdhgState* hstate = nullptr;     // pinned mirror
   double* houts = nullptr;         // pinned
-  double* hflag = nullptr;         // pinned: time-limit flag of the speculative check
+  int* hfault = nullptr;           // pinned: read-back of the barrier fault word
   ncclComm_t comm = nullptr;
   cudaGraphExec_t graph_main = nullptr, graph_small = nullptr;
   int graph_main_passes = 0, graph_small_passes = 0;
@@ -281,7 +280,8 @@ struct b200pdlp_problem {
   DevBuf<SolveCtl> ctl;
   SolveCtl* hctl = nullptr;        // pinned
   int* htime = nullptr;            // pinned + mapped
-  DevBuf<double> trace_dev;
+  DevBuf<double> trace_dev;        // trace window of the device-driven loop (a row of the check entry points)
+  double* htrace = nullptr;        // pinned copy of the window
   cudaGraphExec_t graph_pow2[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // 1 << k passes
   cudaGraphExec_t graph_check = nullptr;
   int check_launches[2] = {0, 0};                 // kernels in graph_check / graph_check_light
@@ -300,11 +300,12 @@ struct b200pdlp_problem {
     if (graph_check_light) cudaGraphExecDestroy(graph_check_light);
     if (hctl) pinned_cache_free(hctl);
     if (htime) pinned_cache_free(htime);
+    if (htrace) pinned_cache_free(htrace);
     for (void* q : ipc_opened) cudaIpcCloseMemHandle(q);
     if (comm) NcclApi::get().CommDestroy(comm);
     if (hstate) pinned_cache_free(hstate);
     if (houts) pinned_cache_free(houts);
-    if (hflag) pinned_cache_free(hflag);
+    if (hfault) pinned_cache_free(hfault);
     if (ev_fork) cudaEventDestroy(ev_fork);
     if (ev_join) cudaEventDestroy(ev_join);
     if (side_stream) cudaStreamDestroy(side_stream);

@@ -195,7 +195,7 @@ __device__ __forceinline__ void slice_end(const Epi& e, int slice, bool live, co
 // Rows longer than the long-row threshold live outside the body as segments of kNnzBlk nonzeros
 // (one CTA each, tree-summed); the last segment of a row to finish combines the partial sums in
 // segment order and runs the epilogue, whose terms go to the partial-sum slot of the row's first segment.
-// `due` != nullptr: speculative check-iteration launch -- run only if the check iteration has been reached
+// `due` != nullptr: a launch of the device-side check -- run only if the check iteration has been reached
 __device__ __forceinline__ bool check_not_due(const PdhgState* due) { return due && (due->done || due->iter < due->stop_iter); }
 
 struct PlainEpilogue {
@@ -1317,9 +1317,8 @@ average_kernel(int len, const double* __restrict__ v, double* __restrict__ sum, 
   }
 }
 
-// Device-parametrised variants for the SPECULATIVE check: enqueued right behind the pass graph, before the host
-// knows the state; they read buffer parity / pending weight / step sum from the state block and do nothing unless
-// the check iteration has been reached.
+// Device-parametrised variant (the device-side check on several GPUs): reads buffer parity / pending weight / step sum
+// from the state block and does nothing unless the check iteration has been reached.
 __global__ void __launch_bounds__(kThreads)
 average_dev_kernel(int len, const double* __restrict__ v0, const double* __restrict__ v1, double* __restrict__ sum,
                    double* __restrict__ avg, const PdhgState* __restrict__ st) {
@@ -1334,12 +1333,6 @@ average_dev_kernel(int len, const double* __restrict__ v0, const double* __restr
     if (pending) { s = s + w * v[i]; sum[i] = s; }
     avg[i] = s * scale;
   }
-}
-// after both averages (and the multi-GPU A^T y materialisation) consumed them
-__global__ void check_clear_kernel(PdhgState* st) {
-  if (check_not_due(st)) return;
-  st->pending = 0;
-  st->accepted_last = 0;
 }
 
 // column-side pass A for up to two iterates (current, average):
@@ -1384,7 +1377,8 @@ __global__ void __launch_bounds__(kThreads)
 col_check_fused_kernel(int n, ColIter it0, ColIter it1, const double* __restrict__ c, const double* __restrict__ lo,
                        const double* __restrict__ up, const double* __restrict__ cs, ReduceScratch rs,
                        double* __restrict__ out, const PdhgState* __restrict__ st, ColIter alt0) {
-  // st != nullptr (speculative launch): skip unless due; the current iterate is it0 if cur == 0, alt0 otherwise
+  // st != nullptr (the device-side check on several GPUs): skip unless due; the current iterate is it0 if cur == 0, alt0
+  // otherwise
   if (st) {
     if (check_not_due(st)) return;
     if (st->cur) it0 = alt0;
@@ -1422,11 +1416,7 @@ col_check_fused_kernel(int n, ColIter it0, ColIter it1, const double* __restrict
 // out per iterate (4): 0 y.b, 1 |primal residual|^2, 2 |y|^2, 3 |[ax]_eq, min([ax]_ineq,0) rowScale|^2
 __global__ void __launch_bounds__(kThreads)
 row_check_fused_kernel(int m, RowIter it0, RowIter it1, const double* __restrict__ b, const double* __restrict__ rsca,
-                       int neq, ReduceScratch rs, double* __restrict__ out, const PdhgState* __restrict__ st, RowIter alt0) {
-  if (st) {
-    if (check_not_due(st)) return;
-    if (st->cur) it0 = alt0;
-  }
+                       int neq, ReduceScratch rs, double* __restrict__ out) {
   double acc[8];
 #pragma unroll
   for (int a = 0; a < 8; a++) acc[a] = 0.0;
@@ -1564,7 +1554,7 @@ __global__ void __launch_bounds__(kThreads) fill_kernel(int len, double* __restr
 //   C5 restart_sweep_kernel        only if C4 chose a restart: copies, clears the sums, |x - x_lr|^2, |y - y_lr|^2
 //   C6 check_finish_kernel         restart scalars (beta, tau, sigma), trace row, next check iteration, power tables
 // Every kernel is a no-op unless the check iteration has been reached and the solve is still running, so the host can
-// enqueue checks speculatively between graphs of passes.
+// enqueue checks ahead, between graphs of passes.
 __device__ __forceinline__ bool check_live(const PdhgState* st, const SolveCtl* ctl) {
   return ctl->term < 0 && !st->done && st->iter >= st->stop_iter;
 }
@@ -2303,7 +2293,7 @@ void preload_multi_gpu_kernels() {
       (const void*)p2p_exchange_kernel, (const void*)reduce_part_p2p_kernel, (const void*)p2p_barrier_kernel,
       (const void*)stash_scalars_kernel<1>, (const void*)stash_scalars_kernel<2>, (const void*)step_rule_mg_kernel,
       (const void*)step_rule_kernel, (const void*)average_kernel, (const void*)average_dev_kernel,
-      (const void*)check_clear_kernel, (const void*)col_check_a_kernel, (const void*)col_check_b_kernel,
+      (const void*)col_check_a_kernel, (const void*)col_check_b_kernel,
       (const void*)row_check_a_kernel, (const void*)row_check_b_kernel, (const void*)col_check_fused_kernel,
       (const void*)row_check_fused_kernel, (const void*)diff_norm2_kernel, (const void*)scale_kernel,
       (const void*)fill_kernel, (const void*)check_avg_x_kernel, (const void*)check_decide_kernel,
@@ -2407,15 +2397,14 @@ void launch_col_check_fused(cudaStream_t s, int n, ColIter a, ColIter b, const d
   col_check_fused_kernel<<<ew_grid(n), kThreads, 0, s>>>(n, a, b, c, lo, up, cs, rs, out, st, alt);
 }
 void launch_row_check_fused(cudaStream_t s, int m, RowIter a, RowIter b, const double* rhs, const double* rsca, int neq,
-                            ReduceScratch rs, double* out, const PdhgState* st, RowIter alt) {
-  row_check_fused_kernel<<<ew_grid(m), kThreads, 0, s>>>(m, a, b, rhs, rsca, neq, rs, out, st, alt);
+                            ReduceScratch rs, double* out) {
+  row_check_fused_kernel<<<ew_grid(m), kThreads, 0, s>>>(m, a, b, rhs, rsca, neq, rs, out);
 }
 void launch_average_dev(cudaStream_t s, int len, const double* v0, const double* v1, double* sum, double* avg,
                         const PdhgState* st) {
   if (len == 0) return;
   average_dev_kernel<<<ew_grid(len), kThreads, 0, s>>>(len, v0, v1, sum, avg, st);
 }
-void launch_check_clear(cudaStream_t s, PdhgState* st) { check_clear_kernel<<<1, 1, 0, s>>>(st); }
 void launch_row_check_a(cudaStream_t s, int m, int nit, RowIter a, RowIter b, const double* rhs,
                         const double* rsca, int neq, int row_offset, ReduceScratch rs, double* out) {
   row_check_a_kernel<<<ew_grid(m), kThreads, 0, s>>>(m, nit, a, b, rhs, rsca, neq, row_offset, rs, out);

@@ -61,11 +61,9 @@ void launch_col_check_fused(cudaStream_t s, int n, ColIter a, ColIter b, const d
                             const double* up, const double* cs, ReduceScratch rs, double* out,
                             const PdhgState* st = nullptr, ColIter alt = ColIter{nullptr, nullptr});
 void launch_row_check_fused(cudaStream_t s, int m, RowIter a, RowIter b, const double* rhs, const double* rsca, int neq,
-                            ReduceScratch rs, double* out, const PdhgState* st = nullptr,
-                            RowIter alt = RowIter{nullptr, nullptr});
+                            ReduceScratch rs, double* out);
 void launch_average_dev(cudaStream_t s, int len, const double* v0, const double* v1, double* sum, double* avg,
                         const PdhgState* st);
-void launch_check_clear(cudaStream_t s, PdhgState* st);
 void launch_row_check_a(cudaStream_t s, int m, int nit, RowIter a, RowIter b, const double* rhs,
                         const double* rsca, int neq, int row_offset, ReduceScratch rs, double* out);
 void launch_col_check_b(cudaStream_t s, int n, int nit, ColIter a, ColIter b, const double inv_d[2],

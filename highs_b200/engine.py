@@ -1252,17 +1252,18 @@ def host_layout_eval(lp: HighsLp, world: int = 1, ordered_max: int = 0, x=None, 
         L.b200pdlp_form_destroy(h)
 
 
-def solve_logical_shards(lp: HighsLp, world: int, device: int = -1, **params) -> list:
+def solve_logical_shards(lp: HighsLp, world: int, device: int = -1, trace_cap: int = 0, **params) -> list:
     """SURVEY.md 8(e): the multi-GPU code path with `world` logical shards inside this process (normally all on one
     device): one problem per rank, buffers wired to each other with b200pdlp_p2p_link_local, one host thread per rank
-    (ctypes releases the GIL during the solve).  Returns the per-rank result dicts (identical by construction)."""
+    (ctypes releases the GIL during the solve).  Returns the per-rank result dicts (identical by construction), each with
+    its own trace when trace_cap > 0."""
     import threading
     with linked_shards(lp, world, device=device, **params) as probs:
         out, err = [None] * world, [None] * world
 
         def run(g):
             try:
-                out[g] = probs[g].solve(device=device, **params)
+                out[g] = probs[g].solve(device=device, trace_cap=trace_cap, **params)
             except Exception as e:   # noqa: BLE001 -- reported to the caller below
                 err[g] = e
 

@@ -1,5 +1,5 @@
 """Child process of tests/test_gpu_logical_shards.py: the multi-GPU code path (row blocks + column shards, the fused
-peer-memory kernels, flag barriers, device-side step rule, speculative check, NCCL-free solution assembly) with G
+peer-memory kernels, flag barriers, device-side step rule and checks, NCCL-free solution assembly) with G
 LOGICAL shards on ONE device -- SURVEY.md 8(e): "the same code path must run with G logical shards on 1 device".
 Run in its own process so that a stuck barrier can be killed by PID without taking the test session along.
 usage: python tests/logical_shards_child.py <world> <case>      prints one JSON line and exits 0 on success"""

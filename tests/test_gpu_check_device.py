@@ -702,8 +702,8 @@ def _child_rejections():
 
 
 def _child_e2e(env_name):
-    """the ordered goldens that end INFEASIBLE_OR_UNBOUNDED, solved in tree mode (device checks unless the environment says
-    otherwise): the golden's model status.  The `unbounded` golden's status (10, Unbounded) is HiGHS's own verdict, which no
+    """the ordered goldens that end INFEASIBLE_OR_UNBOUNDED, solved in tree mode (device checks, light or split as the
+    environment says): the golden's model status.  The `unbounded` golden's status (10, Unbounded) is HiGHS's own verdict, which no
     PDLP term code maps to; there the status must be the one the oracle's PDLP verdict maps to (9)."""
     from conftest import golden_lp, load_golden, options_to_params, term_to_model_status
     from highs_b200 import engine
@@ -767,7 +767,7 @@ _HITS = set()
 
 def _run_child(case, env=None, timeout=900):
     from test_gpu_spmv_shapes import _ENV
-    e = {k: v for k, v in os.environ.items() if k not in _ENV + ("B200PDLP_TIMING", "B200PDLP_HOST_CHECK", "B200PDLP_LIGHT_CHECK")}
+    e = {k: v for k, v in os.environ.items() if k not in _ENV + ("B200PDLP_TIMING", "B200PDLP_LIGHT_CHECK")}
     e.update(env or {})
     try:
         r = subprocess.run([sys.executable, os.path.abspath(__file__), "child", case], capture_output=True, text=True,
@@ -815,8 +815,8 @@ def test_every_branch_was_hit():
     assert BRANCHES <= _HITS, sorted(BRANCHES - _HITS)
 
 
-@pytest.mark.parametrize("env_name,env", [("device_checks", {}), ("host_checks", {"B200PDLP_HOST_CHECK": "1"}),
-                                          ("split_only", {"B200PDLP_LIGHT_CHECK": "0"})])
+@pytest.mark.parametrize("env_name,env", [("device_checks", {}), ("split_only", {"B200PDLP_LIGHT_CHECK": "0"})],
+                         ids=["device_checks-env0", "split_only-env2"])   # (the ids these two cases have always had)
 def test_tree_mode_verdicts_of_the_goldens(env_name, env):
     _assert_all_ok(_run_child(f"e2e:{env_name}", env=env), 4)
 

@@ -1,5 +1,5 @@
 """GPU side of tools/s2_order_sensitivity.py: S2 solved to `tol` by the engine under settings that only regroup floating-point
-sums (grid shapes of the SpMV kernels, host- vs device-side checks, light vs SpMV checks) -- the spread of the iteration count.
+sums (grid shapes of the SpMV kernels, light vs SpMV checks) -- the spread of the iteration count.
     python tools/s2_gpu_spread.py <tol> [<tol> ...]      (one JSON line per run)"""
 import json
 import os
@@ -16,7 +16,6 @@ SETTINGS = [
     ("at_grid_2", {"B200PDLP_SPMV_AT_CTAS_PER_SM": "2"}),
     ("a_grid_3", {"B200PDLP_SPMV_A_CTAS_PER_SM": "3"}),
     ("spmv_checks", {"B200PDLP_LIGHT_CHECK": "0"}),
-    ("host_checks", {"B200PDLP_HOST_CHECK": "1"}),
     ("host_prologue", {"B200PDLP_DEVICE_PREP": "0"}),
 ]
 for tol in [float(a) for a in sys.argv[1:]]:
