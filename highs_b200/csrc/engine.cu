@@ -110,10 +110,12 @@ void apply_spmv_grid(b200pdlp_problem* p) {
   // in L2: there nothing the pass streams survives to the next pass anyway, and evict-first keeps x' and y' resident for the
   // gathers.  Where it fits (S2: 12 MB), the whole pass stays in L2 from one iteration to the next and evict-first would
   // throw that away.  Measured on one H100 (DESIGN.md section 6).
+  // B200PDLP_L2_HINTS=0 / 1 overrides the size rule (to test and compare both variants on any matrix); it changes no result.
   if (!p->form.hipdlp) {
     int l2 = 0;
     cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, p->device);
-    const int hints = 12 * (long long)p->form.nnz >= l2 ? 1 : 0;
+    const int forced = val("B200PDLP_L2_HINTS", -1);
+    const int hints = forced >= 0 ? (forced != 0 ? 1 : 0) : (12 * (long long)p->form.nnz >= l2 ? 1 : 0);
     p->A.dev.l2_hints = p->AT.dev.l2_hints = hints;
   }
   if (getenv("B200PDLP_TIMING")) {
@@ -124,6 +126,7 @@ void apply_spmv_grid(b200pdlp_problem* p) {
             p->AT.tiles_staged, p->AT.ntiles);
     fprintf(stderr, "[b200pdlp setup] zero-skip pass SpMVs: A %d CTAs  A' %d CTAs (0: off)\n", p->A.dev.zskip_grid,
             p->AT.dev.zskip_grid);
+    fprintf(stderr, "[b200pdlp setup] L2 policies: %s\n", p->A.dev.l2_hints ? "on" : "off");
   }
 }
 
@@ -2261,6 +2264,97 @@ static int long_row_records(const DeviceMatrix& M, const std::function<int(int)>
   return (int)lr.size();
 }
 
+// the PdhgState of a kernel-level pass from the caller's scalars (tau = tau_try, sigma = sigma_try), with the step rule's
+// power tables filled from step_iter as the solve fills them
+static void seed_pass_state(PdhgState* h, const b200pdlp_pass_state_in& in) {
+  memset(h, 0, sizeof(PdhgState));
+  h->adaptive = in.adaptive; h->beta = in.beta; h->eta = in.eta;
+  h->tau = h->tau_try = in.tau; h->sigma = h->sigma_try = in.sigma;
+  h->step_iter = in.step_iter; h->iter = in.iter; h->pending = in.pending; h->w_pending = in.w_pending;
+  h->sum_step = in.sum_step; h->light_on = in.light_on; h->cur = in.cur; h->stop_iter = in.stop_iter;
+  fill_pow_tables(h);
+}
+
+// a nonzero bitmap (DevSell::nzmap, bit i & 31 of word i >> 5 for device index i) as one byte per entry in standard-form order
+static void download_bitmap(b200pdlp_problem* p, uint8_t* v, const DevBuf<unsigned>& d, const std::vector<int>& perm) {
+  std::vector<unsigned> w(d.n);
+  if (!w.empty()) CUDA_OK(cudaMemcpyAsync(w.data(), d.p, w.size() * sizeof(unsigned), cudaMemcpyDeviceToHost, p->stream));
+  CUDA_OK(cudaStreamSynchronize(p->stream));
+  for (size_t i = 0; i < perm.size(); i++) v[perm[i]] = (uint8_t)(w[i >> 5] >> (i & 31) & 1u);
+}
+
+// b200pdlp_pass_state, and b200pdlp_pass_partials through it; `who` names the caller in the errors
+static void run_pass_state(b200pdlp_problem* p, const char* who, const b200pdlp_pass_state_in* in, double* x, double* aty,
+                           double* y, double* ax, double* xsum, double* atysum, double* ysum, double* axsum, double* slots,
+                           int32_t cap, int32_t* long_rows, int32_t long_cap, uint8_t* x_nz, uint8_t* y_nz,
+                           b200pdlp_pass_state_out* out) {
+  if (!p || !in || !x || !aty || !y || !ax || !xsum || !atysum || !ysum || !axsum || !slots || !long_rows || !x_nz || !y_nz ||
+      !out)
+    throw Error(B200PDLP_ERR_ARG, std::string(who) + ": null argument");
+  if ((in->cur != 0 && in->cur != 1) || in->iter < 0 || in->step_iter < 0)
+    throw Error(B200PDLP_ERR_ARG, std::string(who) + ": cur must be 0 or 1, iter and step_iter >= 0");
+  require_mode(p, false, who);
+  if (p->world != 1) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": kernel-level entry points are single-GPU");
+  if (p->ordered) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": an ordered-mode problem (its sums add terms, not slots)");
+  const int n = p->n, m = p->m;
+  const int nb[3] = {primal_step_grid(n), p->A.grid(), p->AT.grid()};
+  const int nlong = (int)(p->A.long_rows.n + p->AT.long_rows.n);
+  if (cap < std::max(nb[0], std::max(nb[1], nb[2])) || long_cap < nlong)
+    throw Error(B200PDLP_ERR_ARG, std::string(who) + ": cap must be >= " + std::to_string(std::max(nb[0], std::max(nb[1], nb[2]))) +
+                                      " and long_cap >= " + std::to_string(nlong));
+  set_device(p);
+  ensure_host_maps(p);
+  cudaStream_t s = p->stream;
+  for (int h = 0; h < 2; h++) {
+    upload_perm(p, p->x[h].p, x + (size_t)h * n, p->cperm); upload_perm(p, p->aty[h].p, aty + (size_t)h * n, p->cperm);
+    upload_perm(p, p->y[h].p, y + (size_t)h * m, p->rperm); upload_perm(p, p->ax[h].p, ax + (size_t)h * m, p->rperm);
+  }
+  upload_perm(p, p->xsum.p, xsum, p->cperm); upload_perm(p, p->atysum.p, atysum, p->cperm);
+  upload_perm(p, p->ysum.p, ysum, p->rperm); upload_perm(p, p->axsum.p, axsum, p->rperm);
+  // zero words are the unsafe value: a word the pass fails to write reads as "exactly zero" for every entry
+  for (const DevBuf<unsigned>* nz : {&p->A.nz, &p->AT.nz})
+    if (nz->p) CUDA_OK(cudaMemsetAsync(nz->p, 0, nz->n * sizeof(unsigned), s));
+  seed_pass_state(p->hstate, *in);
+  push_state(p);
+  enqueue_pass(p);
+  p->launches += p->kernels_per_pass();
+  CUDA_OK(cudaGetLastError());
+  const int slot_ids[3] = {kSlotK1, kSlotK2, kSlotK3};
+  for (int k = 0; k < 3; k++)
+    CUDA_OK(cudaMemcpyAsync(slots + (size_t)k * cap, p->rs(slot_ids[k], 0).partials, (size_t)nb[k] * sizeof(double),
+                            cudaMemcpyDeviceToHost, s));
+  pull_state(p);
+  const PdhgState* h = p->hstate;
+  out->dx2 = h->dx2; out->dy2 = h->dy2; out->inter = h->inter;
+  out->tau = h->tau; out->sigma = h->sigma; out->tau_try = h->tau_try; out->sigma_try = h->sigma_try; out->eta = h->eta;
+  out->sum_step = h->sum_step; out->w_pending = h->w_pending; out->mov = h->mov; out->lim = h->lim;
+  out->iter = h->iter; out->step_iter = h->step_iter; out->cur = h->cur; out->pending = h->pending;
+  out->passes = h->passes; out->rejects = h->rejects;
+  for (int k = 0; k < 3; k++) out->slots[k] = nb[k];
+  out->long_a = long_row_records(p->A, [&](int r) { return p->rperm[r]; }, long_rows);
+  out->long_at = long_row_records(p->AT, [&](int r) { return p->cperm[r]; }, long_rows + 3 * (size_t)out->long_a);
+  out->x_nz = p->A.dev.nzmap ? 1 : 0; out->y_nz = p->AT.dev.nzmap ? 1 : 0;
+  out->l2_hints = p->A.dev.l2_hints;
+  for (int k = 0; k < 2; k++) {
+    download_perm(p, x + (size_t)k * n, p->x[k].p, p->cperm); download_perm(p, aty + (size_t)k * n, p->aty[k].p, p->cperm);
+    download_perm(p, y + (size_t)k * m, p->y[k].p, p->rperm); download_perm(p, ax + (size_t)k * m, p->ax[k].p, p->rperm);
+  }
+  download_perm(p, xsum, p->xsum.p, p->cperm); download_perm(p, atysum, p->atysum.p, p->cperm);
+  download_perm(p, ysum, p->ysum.p, p->rperm); download_perm(p, axsum, p->axsum.p, p->rperm);
+  if (out->x_nz) download_bitmap(p, x_nz, p->A.nz, p->cperm);
+  if (out->y_nz) download_bitmap(p, y_nz, p->AT.nz, p->rperm);
+}
+
+int b200pdlp_pass_state(b200pdlp_problem* p, const b200pdlp_pass_state_in* in, double* x, double* aty, double* y,
+                        double* ax, double* xsum, double* atysum, double* ysum, double* axsum, double* slots, int32_t cap,
+                        int32_t* long_rows, int32_t long_cap, uint8_t* x_nz, uint8_t* y_nz, b200pdlp_pass_state_out* out) {
+  DeviceGuard dg;
+  return guarded([&] {
+    run_pass_state(p, "b200pdlp_pass_state", in, x, aty, y, ax, xsum, atysum, ysum, axsum, slots, cap, long_rows, long_cap,
+                   x_nz, y_nz, out);
+  });
+}
+
 int b200pdlp_pass_partials(b200pdlp_problem* p, const double* x, const double* y, const double* ax, const double* aty,
                            double tau, double sigma, double* x_new, double* y_new, double* ax_new, double* aty_new,
                            double* slots, int32_t cap, int32_t* long_rows, int32_t long_cap, b200pdlp_pass_out* out) {
@@ -2270,33 +2364,24 @@ int b200pdlp_pass_partials(b200pdlp_problem* p, const double* x, const double* y
     if (!p || !x || !y || !ax || !aty || !x_new || !y_new || !ax_new || !aty_new || !slots || !long_rows || !out)
       throw Error(B200PDLP_ERR_ARG, std::string(who) + ": null argument");
     require_mode(p, false, who);
-    if (p->world != 1) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": kernel-level entry points are single-GPU");
-    if (p->ordered) throw Error(B200PDLP_ERR_ARG, std::string(who) + ": an ordered-mode problem (its sums add terms, not slots)");
-    const int n = p->n;
-    const int nb[3] = {primal_step_grid(n), p->A.grid(), p->AT.grid()};
-    const int nlong = (int)(p->A.long_rows.n + p->AT.long_rows.n);
-    if (cap < std::max(nb[0], std::max(nb[1], nb[2])) || long_cap < nlong)
-      throw Error(B200PDLP_ERR_ARG, std::string(who) + ": cap must be >= " + std::to_string(std::max(nb[0], std::max(nb[1], nb[2]))) +
-                                        " and long_cap >= " + std::to_string(nlong));
-    set_device(p);
-    ensure_host_maps(p);
-    upload_perm(p, p->x[0].p, x, p->cperm); upload_perm(p, p->aty[0].p, aty, p->cperm);
-    upload_perm(p, p->y[0].p, y, p->rperm); upload_perm(p, p->ax[0].p, ax, p->rperm);
-    kernel_api_state(p, tau, sigma);
-    enqueue_pass(p);
-    p->launches += p->kernels_per_pass();
-    CUDA_OK(cudaGetLastError());
-    const int slot_ids[3] = {kSlotK1, kSlotK2, kSlotK3};
-    for (int k = 0; k < 3; k++)
-      CUDA_OK(cudaMemcpyAsync(slots + (size_t)k * cap, p->rs(slot_ids[k], 0).partials, (size_t)nb[k] * sizeof(double),
-                              cudaMemcpyDeviceToHost, p->stream));
-    pull_state(p);
-    out->dx2 = p->hstate->dx2; out->dy2 = p->hstate->dy2; out->inter = p->hstate->inter;
-    for (int k = 0; k < 3; k++) out->slots[k] = nb[k];
-    out->long_a = long_row_records(p->A, [&](int r) { return p->rperm[r]; }, long_rows);
-    out->long_at = long_row_records(p->AT, [&](int r) { return p->cperm[r]; }, long_rows + 3 * (size_t)out->long_a);
-    download_perm(p, x_new, p->x[1].p, p->cperm); download_perm(p, aty_new, p->aty[1].p, p->cperm);
-    download_perm(p, y_new, p->y[1].p, p->rperm); download_perm(p, ax_new, p->ax[1].p, p->rperm);
+    // half 1 of every buffer is what the pass writes: seeded with the inputs, and the sums (not pending) stay zero
+    const size_t n = (size_t)p->n, m = (size_t)p->m;
+    std::vector<double> xs(2 * n), atys(2 * n), ys(2 * m), axs(2 * m), nsum(2 * n, 0.0), msum(2 * m, 0.0);
+    for (size_t h = 0; h < 2; h++) {
+      std::copy(x, x + n, xs.begin() + h * n); std::copy(aty, aty + n, atys.begin() + h * n);
+      std::copy(y, y + m, ys.begin() + h * m); std::copy(ax, ax + m, axs.begin() + h * m);
+    }
+    std::vector<uint8_t> x_nz(std::max<size_t>(n, 1)), y_nz(std::max<size_t>(m, 1));
+    b200pdlp_pass_state_in in{};
+    in.tau = tau; in.sigma = sigma; in.beta = 1.0; in.adaptive = 1; in.stop_iter = std::numeric_limits<int>::max();
+    b200pdlp_pass_state_out o{};
+    run_pass_state(p, who, &in, xs.data(), atys.data(), ys.data(), axs.data(), nsum.data(), nsum.data() + n, msum.data(),
+                   msum.data() + m, slots, cap, long_rows, long_cap, x_nz.data(), y_nz.data(), &o);
+    std::copy(xs.begin() + n, xs.end(), x_new); std::copy(atys.begin() + n, atys.end(), aty_new);
+    std::copy(ys.begin() + m, ys.end(), y_new); std::copy(axs.begin() + m, axs.end(), ax_new);
+    out->dx2 = o.dx2; out->dy2 = o.dy2; out->inter = o.inter;
+    for (int k = 0; k < 3; k++) out->slots[k] = o.slots[k];
+    out->long_a = o.long_a; out->long_at = o.long_at;
   });
 }
 
@@ -2390,13 +2475,12 @@ int b200pdlp_pass_partials_mg(b200pdlp_problem** probs, int32_t world, const b20
       std::vector<int> outpos(p->AT.long_rows.n ? n : 0);   // A_g' rows -> positions in the segmented vector
       if (!outpos.empty()) CUDA_OK(cudaMemcpy(outpos.data(), p->at_outpos.p, n * sizeof(int), cudaMemcpyDeviceToHost));
       PdhgState* h = p->hstate;
-      memset(h, 0, sizeof(PdhgState));
-      h->adaptive = 1; h->beta = in->beta; h->eta = in->eta;
-      h->tau = h->tau_try = in->tau; h->sigma = h->sigma_try = in->sigma;
-      h->step_iter = in->step_iter; h->iter = in->iter; h->pending = in->pending; h->w_pending = in->w_pending;
-      h->sum_step = in->sum_step; h->light_on = in->light_on; h->accepted_last = part_in ? 1 : 0;
-      h->stop_iter = std::numeric_limits<int>::max();
-      fill_pow_tables(h);
+      b200pdlp_pass_state_in si{};
+      si.tau = in->tau; si.sigma = in->sigma; si.beta = in->beta; si.eta = in->eta; si.w_pending = in->w_pending;
+      si.sum_step = in->sum_step; si.iter = in->iter; si.step_iter = in->step_iter; si.pending = in->pending;
+      si.light_on = in->light_on; si.adaptive = 1; si.cur = 0; si.stop_iter = std::numeric_limits<int>::max();
+      seed_pass_state(h, si);
+      h->accepted_last = part_in ? 1 : 0;
       push_state(p);
       CUDA_OK(cudaMemsetAsync(p->fault.p, 0, sizeof(int), s));
       CUDA_OK(cudaStreamSynchronize(s));

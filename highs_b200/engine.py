@@ -19,6 +19,7 @@ LIB_PATH = os.path.join(HERE, "libb200pdlp.so")
 
 _dp = C.POINTER(C.c_double)
 _ip = C.POINTER(C.c_int32)
+_u8p = C.POINTER(C.c_uint8)
 
 TERM_NAMES = {0: "OPTIMAL", 1: "INFEASIBLE", 2: "UNBOUNDED", 3: "INFEASIBLE_OR_UNBOUNDED",
               4: "TIMELIMIT_OR_ITERLIMIT", 5: "FEASIBLE"}
@@ -75,6 +76,24 @@ class CPassOut(C.Structure):
     """b200pdlp_pass_out: K4's sums and the sizes of what b200pdlp_pass_partials returned"""
     _fields_ = [("dx2", C.c_double), ("dy2", C.c_double), ("inter", C.c_double), ("slots", C.c_int32 * 3),
                 ("long_a", C.c_int32), ("long_at", C.c_int32)]
+
+
+class CPassStateIn(C.Structure):
+    """b200pdlp_pass_state_in: the PdhgState a one-GPU pass starts from (b200pdlp_pass_state)"""
+    _fields_ = [("tau", C.c_double), ("sigma", C.c_double), ("beta", C.c_double), ("eta", C.c_double),
+                ("w_pending", C.c_double), ("sum_step", C.c_double), ("iter", C.c_int32), ("step_iter", C.c_int32),
+                ("pending", C.c_int32), ("light_on", C.c_int32), ("adaptive", C.c_int32), ("cur", C.c_int32),
+                ("stop_iter", C.c_int32), ("reserved", C.c_int32)]
+
+
+class CPassStateOut(C.Structure):
+    """b200pdlp_pass_state_out: K4's sums, the state after the step rule and the sizes of what b200pdlp_pass_state returned"""
+    _fields_ = [("dx2", C.c_double), ("dy2", C.c_double), ("inter", C.c_double), ("tau", C.c_double), ("sigma", C.c_double),
+                ("tau_try", C.c_double), ("sigma_try", C.c_double), ("eta", C.c_double), ("sum_step", C.c_double),
+                ("w_pending", C.c_double), ("mov", C.c_double), ("lim", C.c_double), ("iter", C.c_int32),
+                ("step_iter", C.c_int32), ("cur", C.c_int32), ("pending", C.c_int32), ("passes", C.c_int32),
+                ("rejects", C.c_int32), ("slots", C.c_int32 * 3), ("long_a", C.c_int32), ("long_at", C.c_int32),
+                ("x_nz", C.c_int32), ("y_nz", C.c_int32), ("l2_hints", C.c_int32)]
 
 
 CHECK_VECTORS = ("x", "y", "ax", "aty", "xsum", "ysum", "xlr", "ylr", "axsum", "atysum", "xavg", "yavg", "axavg", "atyavg")
@@ -135,7 +154,7 @@ ABI_SYMBOLS = [
     "b200pdlp_hipdlp_problem_power_method", "b200pdlp_solve_hipdlp_batch_mixed",
     "b200pdlp_solve_hipdlp_batch_mixed_device", "b200pdlp_debug_hipdlp_tree_prep_compare", "b200pdlp_check_device",
     "b200pdlp_solve_device", "b200pdlp_solve_hipdlp_device", "b200pdlp_pass_partials", "b200pdlp_pass_partials_mg",
-    "b200pdlp_check_device_mg",
+    "b200pdlp_check_device_mg", "b200pdlp_pass_state",
 ]
 HIP_TRACE_COLS = 16   # B200PDLP_HIP_TRACE_COLS: the per-block trace of the HiPDLP solves
 
@@ -214,6 +233,8 @@ def lib():
         L.b200pdlp_check_device.argtypes = [C.c_void_p, C.POINTER(CCheckIn)] + [_dp] * 14 + [C.POINTER(CCheckOut)]
         L.b200pdlp_pass_partials.argtypes = ([C.c_void_p] + [_dp] * 4 + [C.c_double] * 2 + [_dp] * 5 +
                                              [C.c_int32, _ip, C.c_int32, C.POINTER(CPassOut)])
+        L.b200pdlp_pass_state.argtypes = ([C.c_void_p, C.POINTER(CPassStateIn)] + [_dp] * 9 +
+                                          [C.c_int32, _ip, C.c_int32, _u8p, _u8p, C.POINTER(CPassStateOut)])
         L.b200pdlp_check_device_mg.argtypes = ([C.POINTER(C.c_void_p), C.c_int32, C.POINTER(CCheckIn)] + [_dp] * 14 +
                                                [C.POINTER(CCheckOut)])
         L.b200pdlp_pass_partials_mg.argtypes = ([C.POINTER(C.c_void_p), C.c_int32, C.POINTER(CPassIn)] + [_dp] * 15 +
@@ -1025,6 +1046,41 @@ class Problem:
             r[f"k{k + 1}"] = slots[k, : out.slots[k]].copy()
         r["long_a"], r["long_at"] = lr[: out.long_a].copy(), lr[out.long_a: out.long_a + out.long_at].copy()
         r.update(dx2=out.dx2, dy2=out.dy2, inter=out.inter)
+        return r
+
+    def pass_state(self, x, aty, y, ax, xsum, atysum, ysum, axsum, **scalars) -> dict:
+        """One PDHG pass of a tree-mode solve from the state the caller chooses (b200pdlp_pass_state).  Vectors in
+        standard-form order: x, aty (2 x n) and y, ax (2 x m) are both halves of the double buffers; the sums are n- or
+        m-vectors.  Scalars: the fields of b200pdlp_pass_state_in; beta, adaptive and stop_iter default to 1, 1 and
+        INT_MAX, the others to 0.  Returns every vector after the pass (same names and shapes); k1, k2, k3 and long_a, long_at as Problem.pass_partials returns them; x_nz, y_nz, the nonzero bitmaps of x'
+        and y' (uint8, one entry per column / row), or None where the zero-skip shape is off; and every field of
+        b200pdlp_pass_state_out but the sizes (x_nz / y_nz become the bitmaps)."""
+        n, m = self.n, self.m
+        # what b200pdlp_pass_partials runs with: a due, adaptive pass with beta 1 (zero there would be no pass / NaN steps)
+        cin = CPassStateIn(beta=1.0, adaptive=1, stop_iter=2**31 - 1)
+        for k, v in scalars.items():
+            if not hasattr(cin, k) or k == "reserved":
+                raise TypeError(f"unknown pass_state field {k}")
+            setattr(cin, k, v)
+        vec = lambda v, shape: np.array(v, dtype=np.float64, copy=True).reshape(shape)
+        r = dict(x=vec(x, (2, n)), aty=vec(aty, (2, n)), y=vec(y, (2, m)), ax=vec(ax, (2, m)), xsum=vec(xsum, n),
+                 atysum=vec(atysum, n), ysum=vec(ysum, m), axsum=vec(axsum, m))
+        nlong = self.nnz // 513 + 1   # slot bounds as in pass_partials
+        cap = max(16 * 148, (max(n, m) + 255) // 256 + self.nnz // 2048 + nlong)
+        slots = np.zeros((3, cap))
+        lr = np.zeros((2 * nlong, 3), dtype=np.int32)
+        x_nz, y_nz = np.zeros(max(n, 1), dtype=np.uint8), np.zeros(max(m, 1), dtype=np.uint8)
+        out = CPassStateOut()
+        order = ("x", "aty", "y", "ax", "xsum", "atysum", "ysum", "axsum")
+        _check(lib().b200pdlp_pass_state(self._h, C.byref(cin), *(_p(r[k], _dp) for k in order), _p(slots, _dp), cap,
+                                         _p(lr, _ip), lr.shape[0], _p(x_nz, _u8p), _p(y_nz, _u8p), C.byref(out)),
+               "b200pdlp_pass_state")
+        for k in range(3):
+            r[f"k{k + 1}"] = slots[k, : out.slots[k]].copy()
+        r["long_a"], r["long_at"] = lr[: out.long_a].copy(), lr[out.long_a: out.long_a + out.long_at].copy()
+        r.update({k: getattr(out, k) for k, _ in CPassStateOut._fields_ if k not in ("slots", "long_a", "long_at", "x_nz", "y_nz")})
+        r["x_nz"] = x_nz[:n] if out.x_nz else None
+        r["y_nz"] = y_nz[:m] if out.y_nz else None
         return r
 
     def bench_spmv(self, which: int, reps: int) -> float:

@@ -307,6 +307,40 @@ int b200pdlp_pass_partials(b200pdlp_problem* p, const double* x, const double* y
                            double tau, double sigma, double* x_new, double* y_new, double* ax_new, double* aty_new,
                            double* slots, int32_t cap, int32_t* long_rows, int32_t long_cap, b200pdlp_pass_out* out);
 
+/* One PDHG pass of a tree-mode solve from a state the caller chooses, and everything it writes (parity tests; one GPU):
+ * the launches of b200pdlp_pass_partials (which is this call with tau = tau_try, sigma = sigma_try, beta 1, eta 0, iter 0,
+ * step_iter 0, pending 0, light_on 0, adaptive 1, cur 0 and no stop).  The scalars in `in` become the PdhgState (tau =
+ * tau_try, sigma = sigma_try, the step rule's power tables filled from step_iter as the solve fills them); a pass with
+ * iter >= stop_iter is not due and writes nothing.
+ * In and out, host arrays in standard-form order: both halves of the double buffers, half h at offset h n (or h m):
+ * x[2][n], aty[2][n], y[2][m], ax[2][m]; the sums xsum, atysum (n), ysum, axsum (m).
+ * slots, long_rows: as b200pdlp_pass_partials (out->slots, out->long_a, out->long_at).
+ * x_nz[n], y_nz[m]: the nonzero bitmaps of x' and y' that K1 and K2 write for the zero-skip SpMVs, one byte (0 or 1) per
+ * entry; both bitmaps are zeroed before the pass.  A bitmap exists only where the zero-skip shape is on for its matrix
+ * (out->x_nz for A, out->y_nz for A'); where it does not, its array is left untouched.
+ * out: K4's sums, every PdhgState field the step rule writes, the sizes of the slot arrays and whether the L2 cache
+ * policies were on (B200PDLP_L2_HINTS).
+ * Rejected with B200PDLP_ERR_ARG before anything is written: NULL arguments, cur outside {0, 1}, iter or step_iter < 0, a
+ * problem in ordered mode, on several GPUs or of b200pdlp_hipdlp_problem_create, cap below the longest slot array and
+ * long_cap below the number of long rows.  No device: B200PDLP_ERR_CUDA. */
+typedef struct {
+  double tau, sigma, beta, eta, w_pending, sum_step;
+  int32_t iter, step_iter, pending, light_on, adaptive, cur, stop_iter;
+  int32_t reserved;
+} b200pdlp_pass_state_in;
+typedef struct {
+  double dx2, dy2, inter;   /* K4's sums */
+  double tau, sigma, tau_try, sigma_try, eta, sum_step, w_pending, mov, lim;   /* after the step rule */
+  int32_t iter, step_iter, cur, pending, passes, rejects;
+  int32_t slots[3];         /* K1, K2, K3 */
+  int32_t long_a, long_at;  /* long rows of A, of A' */
+  int32_t x_nz, y_nz;       /* 1: the bitmap of x' (of y') exists */
+  int32_t l2_hints;         /* 1: K1 and the zero-skip K2 / K3 ran with L2 cache policies */
+} b200pdlp_pass_state_out;
+int b200pdlp_pass_state(b200pdlp_problem* p, const b200pdlp_pass_state_in* in, double* x, double* aty, double* y,
+                        double* ax, double* xsum, double* atysum, double* ysum, double* axsum, double* slots, int32_t cap,
+                        int32_t* long_rows, int32_t long_cap, uint8_t* x_nz, uint8_t* y_nz, b200pdlp_pass_state_out* out);
+
 /* One fused PDHG pass of a multi-GPU solve on linked ranks (parity tests): probs[g] is rank g of a world of `world`
  * tree-mode problems linked by b200pdlp_p2p_link_local.  Every rank runs, on its own host thread, the five launches of the
  * solve's pass (primal_shard_p2p_kernel, barrier 0, A_g x' + dual step, partial A_g'y', barrier 1 with the step rule), then

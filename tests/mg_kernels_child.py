@@ -8,7 +8,6 @@ import os
 import sys
 import traceback
 
-os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")   # one hardware queue per logical rank's stream
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -108,24 +107,37 @@ def dual_replay(y, b, ax_new, ax, sigma, neq):
     return np.where(ineq & ~(v > 0.0), 0.0, v)
 
 
+# the fields of b200pdlp_pass_mg_out that step_rule_replay predicts
+MG_STATE = ("step_iter", "iter", "tau", "sigma", "sum_step", "w_pending", "pending", "eta", "tau_try", "sigma_try",
+            "accepted_last")
+
+
 def step_rule_replay(s, dx2, dy2, inter):
-    """step_rule (pdhg_arith.cuh) with the power tables fill_pow_tables leaves (glibc pow through math.pow)"""
+    """step_rule (pdhg_arith.cuh) with the power tables fill_pow_tables leaves (glibc pow through math.pow), from the state
+    the kernel-level entry points seed: s's scalars, tau_try = tau, sigma_try = sigma, lim 0, passes and rejects 0 (cur,
+    adaptive: 0 and 1 unless s has them).  The fixed step (adaptive 0) keeps tau, sigma, eta and the trial steps."""
     rb = math.sqrt(s["beta"])
     mov = dx2 * 0.5 * rb + dy2 / (2.0 * rb)
+    r = dict(step_iter=s["step_iter"], iter=s["iter"], tau=s["tau"], sigma=s["sigma"], sum_step=s.get("sum_step", 0.0),
+             w_pending=s.get("w_pending", 0.0), pending=s.get("pending", 0), eta=s["eta"], tau_try=s["tau"],
+             sigma_try=s["sigma"], cur=s.get("cur", 0), passes=1, rejects=0, mov=mov, lim=0.0)
+    if not s.get("adaptive", 1):
+        w = math.sqrt(r["tau"] * r["sigma"])
+        r.update(sum_step=r["sum_step"] + w, w_pending=w, pending=1, cur=r["cur"] ^ 1, iter=s["iter"] + 1)
+        return r
     k = s["step_iter"] + 1
     eta = s["eta"]
     lim = mov / abs(inter) if inter != 0.0 else math.inf
     accept = eta <= lim
     pr, pg = math.pow(k + 1.0, -0.3), math.pow(k + 1.0, -0.6)
     eta_new = min((1.0 - pr) * lim, (1.0 + pg) * eta)
-    r = dict(step_iter=k, iter=s["iter"], tau=s["tau"], sigma=s["sigma"], sum_step=s.get("sum_step", 0.0),
-             w_pending=s.get("w_pending", 0.0), pending=s.get("pending", 0))
+    r.update(step_iter=k, lim=lim)
     if accept:
         r["tau"], r["sigma"] = eta_new / rb, eta_new * rb
         w = math.sqrt(r["tau"] * r["sigma"])
-        r.update(sum_step=r["sum_step"] + w, w_pending=w, pending=1, iter=s["iter"] + 1, eta=w)
+        r.update(sum_step=r["sum_step"] + w, w_pending=w, pending=1, iter=s["iter"] + 1, eta=w, cur=r["cur"] ^ 1)
     else:
-        r.update(eta=eta_new, pending=0)
+        r.update(eta=eta_new, pending=0, rejects=1)
     r.update(tau_try=r["eta"] / rb, sigma_try=r["eta"] * rb, accepted_last=int(accept))
     return r
 
@@ -301,8 +313,8 @@ def check_pass(ck, f, lp, world, inp, s, r, one=None, tag=""):
         gamma_ok(inter, it, "inter", extra=world + 2048)
         want = step_rule_replay(s, dx2, dy2, inter)
         for g, q in enumerate(ranks):
-            for k, v in want.items():
-                assert _bits(float(q[k])) == _bits(float(v)), (g, k, q[k], v)
+            for k in MG_STATE:
+                assert _bits(float(q[k])) == _bits(float(want[k])), (g, k, q[k], want[k])
     ck(tag + "scalars", scalars)
 
     # 6. the dense-phase sums
@@ -550,6 +562,7 @@ def run_check(world):
 
 
 def main():
+    os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")   # one hardware queue per logical rank's stream
     case = sys.argv[1]
     if case == "rejections":
         out = rejections()

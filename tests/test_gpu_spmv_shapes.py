@@ -237,16 +237,25 @@ def extended_rows(beg, idx, val, x):
     return ref.astype(ld), np.abs(ref).astype(ld) * U
 
 
-def assert_within_bound(got, beg, idx, val, x, what):
-    """|got - ref| <= gamma_k sum |a_ij x_j| for every row, k = its length (plus the reference's own error)"""
+def row_bounds(beg, idx, val, x):
+    """(ref, bound): each row's extended-precision sum, and gamma_k sum |a_ij x_j| (k = its length) plus the reference's
+    own error"""
     ld = np.longdouble
     ref, err = extended_rows(beg, idx, val, x)
-    mag = np.zeros(len(got), ld)
     ln = np.diff(beg)
+    mag = np.zeros(len(ln), ld)
     nz = np.flatnonzero(ln > 0)
     mag[nz] = np.add.reduceat(np.abs(val.astype(ld) * x[idx].astype(ld)), beg[:-1][nz])
     k = ln.astype(ld)
-    bound = k * ld(U) / (1 - k * ld(U)) * mag * (1 + ld(2.0 ** -40)) + err
+    return ref, k * ld(U) / (1 - k * ld(U)) * mag * (1 + ld(2.0 ** -40)) + err
+
+
+def assert_within_bound(got, beg, idx, val, x, what, bounds=None):
+    """|got - ref| <= gamma_k sum |a_ij x_j| for every row, k = its length (plus the reference's own error); bounds: the
+    rows' (ref, bound) from row_bounds, when the caller has them"""
+    ld = np.longdouble
+    ref, bound = row_bounds(beg, idx, val, x) if bounds is None else bounds
+    ln = np.diff(beg)
     dev = np.abs(got.astype(ld) - ref)
     bad = np.flatnonzero(dev > bound)
     assert bad.size == 0, (what, f"{bad.size} rows outside the bound, e.g. row {bad[0]} (length {ln[bad[0]]}): "
